@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the B200 hot path (BASELINE.json: DLRM & TwoTower fwd samples/s).
+"""bench.py — headline benchmark of the H100 hot path (BASELINE.json: DLRM & TwoTower fwd samples/s).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
                     [--workload all|dlrm|dlrm-sharded|twotower|dcn|dlrm-train] [--batch B]
+                    [--dump-outputs DIR]
 
 Headline workload = BASELINE.json configs[1]: mm.DLRMModel, Criteo shape (26 cat, 13 dense, emb 64,
 bundled cardinalities = 45.6 M rows / 11.7 GB of tables), batch 65 536, README MLP dims.
@@ -10,10 +11,10 @@ A step = one forward pass over one batch of synthetic input.  N>1 (torchrun): on
 GPU on disjoint batches, no data-path collective (the forward is replica-local; DESIGN.md (e)),
 weak scaling.
 
-Prints ONE JSON line (contract in the task statement): value = device-resident samples/s,
+Prints ONE JSON line: value = device-resident samples/s,
 e2e = the same metric through the public host-buffer call (pinned H2D of a PACKED batch — ids at 1/2/3
-bytes — + forward + D2H inside the timed region), roofline = dominant kernel vs measured HBM peak (both
-the algorithmic-bytes fraction and the DRAM-traffic fraction), cpu_baseline = CPU restatement of the
+bytes — + forward + D2H inside the timed region), roofline = dominant kernel vs the HBM peak (the
+algorithmic-bytes fraction), cpu_baseline = CPU restatement of the
 reference op sequence on this box's host cores (rank 0, N=1 only).
 The default `--workload all` adds to the same line:
   "secondary": {"twotower": {...}, "dcn": {...}} — configs[2] (10 M-item catalog, in-batch negatives,
@@ -26,6 +27,9 @@ The default `--workload all` adds to the same line:
       protocol timed beside it.
 `--impl reference` times the CPU restatement alone on the SAME 65 536-sample step (TensorFlow is not
 installable: no network).  `--workload dlrm|twotower|dcn|dlrm-sharded` print a line for that workload only.
+`--dump-outputs DIR` writes the predictions of the last timed headline step to DIR/dlrm_predictions.npy
+(float32, (batch, 1)); inputs and weights are seeded, so two builds run with the same arguments can be
+compared output for output.
 """
 from __future__ import annotations
 
@@ -42,7 +46,10 @@ import numpy as np
 ROOT = Path(__file__).resolve().parent
 sys.path.insert(0, str(ROOT))
 
-HBM_FALLBACK_GBS = 6650.0  # B200_PROFILING.md fallback when MEASURED_PEAKS.json is absent
+# NVIDIA H100 SXM data sheet (700 W card): used when MEASURED_PEAKS.json is absent; never reached in practice
+HBM_FALLBACK_GBS = 3350.0
+BF16_DENSE_FALLBACK_TFLOPS = 989.0
+FALLBACK_SOURCE = "data sheet (H100 SXM, 700 W)"
 
 
 def measured_peaks():
@@ -50,7 +57,7 @@ def measured_peaks():
     if p.exists():
         d = json.loads(p.read_text())
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return HBM_FALLBACK_GBS, "fallback (B200_PROFILING.md)"
+    return HBM_FALLBACK_GBS, FALLBACK_SOURCE
 
 
 # ---------------------------------------------------------------------------------------------
@@ -58,8 +65,8 @@ def measured_peaks():
 # ---------------------------------------------------------------------------------------------
 class ClockSampler:
     """Polls NVML (SM clock + clock-event reasons) every ~2 ms in a thread for the duration of the
-    timed region; the same fields `nvidia-smi --query-gpu=clocks.sm,clocks_event_reasons.*` prints
-    (B200_PROFILING.md), without its ~100 ms start-up that would miss a short region."""
+    timed region; the same fields `nvidia-smi --query-gpu=clocks.sm,clocks_event_reasons.*` prints,
+    without its ~100 ms start-up that would miss a short region."""
 
     REASONS = {0x8: "hw_slowdown", 0x40: "hw_thermal_slowdown", 0x20: "sw_thermal_slowdown", 0x4: "sw_power_cap"}
 
@@ -135,31 +142,12 @@ def host_batches(datasets, schema, B, n, seed0=1234):
     return out
 
 
-def ncu_traffic_bytes(summary: Path):
-    """DRAM bytes (read + write) per launch of the dominant kernel, from the committed summary of an
-    `ncu --set full` capture (profiles/); None if the file is missing."""
-    try:
-        rd = wr = None
-        for ln in summary.read_text().splitlines():
-            parts = ln.split()
-            if len(parts) >= 3 and parts[0] == "dram__bytes_read.sum":
-                rd = float(parts[1]) * {"Mbyte": 1e6, "Gbyte": 1e9, "Kbyte": 1e3, "byte": 1}[parts[2]]
-            if len(parts) >= 3 and parts[0] == "dram__bytes_write.sum":
-                wr = float(parts[1]) * {"Mbyte": 1e6, "Gbyte": 1e9, "Kbyte": 1e3, "byte": 1}[parts[2]]
-        return None if rd is None or wr is None else rd + wr
-    except Exception:
-        return None
-
-
 def dlrm_bytes_per_sample(T=26, D=64, id_bytes_total=104, P=64):
     """SURVEY §8(d): rows read + ids + bottom vector + output row = 8 676 B with int32 ids."""
     F = T + 1
     fused = T * D * 4 + id_bytes_total + D * 4 + (P + F * (F - 1) // 2) * 4
     gather = 2 * T * D * 4 + id_bytes_total  # standalone gather: 13 416 B
     return fused, gather
-
-
-NCU_FUSED_SUMMARY = "profiles/r02_ncu_fused_operand.txt"  # `ncu --set full` summary of THIS round's dominant kernel
 
 
 def cpu_baseline_dlrm(model, feats_host, sample_rows, threads):
@@ -351,6 +339,12 @@ def dlrm_record(ctx):
     assert torch.equal(model(devs[1]), pf.output(0)), "pipelined replay diverges from model.__call__"
 
     elapsed_ms, clocks = timed_replay(ctx, pf, packed_dev, args.steps, args.warmup)
+    if args.dump_outputs and ctx.rank == 0:
+        # what the last timed step returned to its caller: the (B, 1) predictions of batch (steps - 1) % n_bufs
+        last = pf.output((args.warmup + args.steps - 1) % depth).float().cpu().numpy()
+        out_dir = Path(args.dump_outputs)
+        out_dir.mkdir(parents=True, exist_ok=True)
+        np.save(out_dir / "dlrm_predictions.npy", last)
     launches = cf.launches_per_replay * args.steps
     serial_ms = timed_serial(cf, packed_dev, args.steps)
 
@@ -379,7 +373,7 @@ def dlrm_record(ctx):
 
     kern_ms = event_times(dominant, args.steps, args.warmup)
 
-    e2e_steps = max(5, args.steps)
+    e2e_steps = args.steps
     e2e_ms, res = timed_e2e(ctx, pf, hbs, e2e_steps, depth)
     ref_host = cf(hbs[(e2e_steps - 1) % n_bufs]).clone()
     assert torch.equal(res, ref_host), "pipelined e2e result differs from the serial graph call"
@@ -391,7 +385,6 @@ def dlrm_record(ctx):
     peak, peak_src = measured_peaks()
     fused_b, _ = dlrm_bytes_per_sample(id_bytes_total=id_bytes_total)
     achieved = fused_b * B / (kern_ms * 1e-3) / 1e9
-    traffic = ncu_traffic_bytes(ROOT / NCU_FUSED_SUMMARY) if B == 65536 else None
     line = {
         "metric": "DLRM fwd samples/sec (Criteo shape, batch 65536/GPU)",
         "value": world * B * args.steps / (elapsed_ms * 1e-3),
@@ -429,11 +422,7 @@ def dlrm_record(ctx):
                      "timing": "CUDA events around each of K back-to-back launches on the same rotating inputs (graph nodes cannot be bracketed)",
                      "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                      "peak_source": peak_src, "algorithmic_bytes_per_launch": fused_b * B,
-                     "kernel_ms": kern_ms,
-                     "traffic": traffic,
-                     "dram_frac": None if traffic is None else traffic / (kern_ms * 1e-3) / 1e9 / peak,
-                     "traffic_source": f"{NCU_FUSED_SUMMARY} (ncu --set full of this round's kernel, one launch, B=65536; the 19 "
-                                       "small tables are L2-resident, so DRAM traffic < algorithmic bytes)"},
+                     "kernel_ms": kern_ms},
     }
     return line, model, hosts
 
@@ -448,6 +437,8 @@ def main():
     ap.add_argument("--batch", type=int, default=None)
     ap.add_argument("--cpu-sample", type=int, default=None, help="samples per CPU pass (default: the full batch)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the predictions of the last timed headline step to DIR/dlrm_predictions.npy")
     ap.add_argument("--pipeline-depth", type=int, default=3,
                     help="graph instances / streams of model.pipeline (3: one more pinned H2D in flight than 2)")
     args = ap.parse_args()
@@ -472,7 +463,7 @@ def main():
         return reference_arm(args, mm, datasets, cores)
 
     if not torch.cuda.is_available():
-        print(json.dumps({"error": "no CUDA device: the B200 hot path has no CPU fallback"}))
+        print(json.dumps({"error": "no CUDA device: the H100 hot path has no CPU fallback"}))
         return 1
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
@@ -629,7 +620,7 @@ def sharded_record(ctx):
                    "runtime": f"CUDA graph replay, {args.pipeline_depth} graph instances (no collective, no barrier in the graph)"},
         "placements": {},
     }
-    link_ref = 770.0  # GB/s per direction per GPU: measured peer copy (B200_PROFILING.md); nominal 900
+    link_ref = 450.0  # GB/s per direction per GPU: NVLink 4 nominal (H100 SXM data sheet: 900 GB/s bidirectional)
     for label, below in (("sharded_from_65536_rows", 65536), ("sharded_from_1000_rows", 1000), ("all_tables_sharded", 0)):
         model = make(below)
         se = model.body.sharded
@@ -860,7 +851,6 @@ def train_record(ctx):
             rec["roofline"] = {"bound": "hbm", "kernel": "interact_bwd_ps_kernel (mm_dlrm_interact_backward, operand-format rows)",
                                "unit": "GB/s", "achieved": ach, "peak": peak, "peak_source": peak_src, "frac": ach / peak, "kernel_ms": k_ms,
                                "algorithmic_bytes_per_launch": per_sample * B,
-                               "traffic": 749990144.0, "dram_frac": 749990144.0 / (k_ms * 1e-3) / 1e9 / peak, "traffic_source": "profiles/r02_ncu_train_kernels.txt (ncu --set full, dram read + write of one launch)",
                                "share_of_step": k_ms / (ms_max / steps)}
     except Exception as e:  # evidence, never fatal
         rec["roofline"] = {"error": f"{type(e).__name__}: {e}"}
@@ -992,7 +982,7 @@ def secondary_record(ctx, kind):
     if roof["bound"] == "hbm":
         achieved, peak, src = algo / (kern_ms * 1e-3) / 1e9, hbm, hbm_src
     else:
-        achieved, peak, src = algo / (kern_ms * 1e-3) / 1e12, tf_peak or 1590.0, "measured (MEASURED_PEAKS.json)" if tf_peak else "fallback (B200_PROFILING.md)"
+        achieved, peak, src = algo / (kern_ms * 1e-3) / 1e12, tf_peak or BF16_DENSE_FALLBACK_TFLOPS, "measured (MEASURED_PEAKS.json)" if tf_peak else FALLBACK_SOURCE
     roof.update({"achieved": achieved, "peak": peak, "frac": achieved / peak, "peak_source": src, "kernel_ms": kern_ms,
                  "algorithmic_per_launch": algo, "traffic": None})
     rec = {

@@ -1,5 +1,5 @@
 /*
- * mm_b200.h — C-ABI of the B200-native (sm_100a) hot path of NVIDIA-Merlin/models:
+ * mm_b200.h — C-ABI of the H100-native (sm_90a) hot path of NVIDIA-Merlin/models:
  *             embedding lookup -> MLP tower -> interaction / scoring.
  *
  * The reference (/root/reference, merlin/models/tf) has no FFI layer: every byte on this
@@ -222,10 +222,10 @@ int mm_dense_fp32(const float* x, int64_t B, int K, int64_t x_stride, const floa
                   float* out, int64_t out_stride, void* stream);
 
 /* ---------------------------------------------------------------------------------------
- * K4/K7  Tensor-core dense layer (tcgen05.mma kind::f16, TMA-fed, TMEM accumulators).
+ * K4/K7  Tensor-core dense layer (wgmma bf16, TMA-fed, fp32 register accumulators).
  * fp32 operands are carried as split-bf16 pairs (hi, lo): x ~ hi + lo with
- * hi = bf16(x), lo = bf16(x - hi).  passes = 3 computes hi*hi + hi*lo + lo*hi in one fp32
- * TMEM accumulator (|err| ~ 2^-16 relative: fp32-grade, holds the 1e-3 logit tolerance);
+ * hi = bf16(x), lo = bf16(x - hi).  passes = 3 computes hi*hi + hi*lo + lo*hi in one
+ * fp32 accumulator (|err| ~ 2^-16 relative: fp32-grade, holds the 1e-3 logit tolerance);
  * passes = 1 is plain bf16.
  *   a_split : (M, 2*Kp) bf16, row = [hi(0..Kp) | lo(0..Kp)], Kp = K padded to 64
  *   w_split : (Np, 2*Kp) bf16, K-major transpose of the Keras kernel, same split, Np = N
@@ -256,9 +256,9 @@ int mm_dense_tc_head(const void* a_split, int64_t M, int K, int Kp, const void* 
  * `_Dense.call` :275-280; optionally followed by BinaryOutput's Dense(1), outputs/classification.py:114):
  *   h_1 = act_1(x W_1 + b_1); h_l = act_l(h_{l-1} W_l + b_l), l = 2..n_layers (n_layers <= 4);
  *   out (M, widths[n-1]) fp32 rows (or null) and/or head_out[m] = head_act(h_n[m,:] . head_w + head_b).
- * Layer 1 is the TMA-fed tcgen05 GEMM of mm_dense_tc (any K); layers 2..n run on chip: the
- * activations go TMEM -> registers (bias, activation, bf16 split) -> TMEM and are the A operand of the
- * next tcgen05.mma, the weights of layers 2..n stay resident in shared memory.  Every width must be
+ * Layer 1 is the TMA-fed wgmma GEMM of mm_dense_tc (any K); layers 2..n run on chip: the
+ * activations stay in registers (bias, activation, bf16 split) and are the register A operand of the
+ * next wgmma, the weights of layers 2..n stay resident in shared memory.  Every width must be
  * <= 128 (README towers: 13->128->64 and 415->128->64->32->1); fp32 parity by 3-pass split-bf16.
  * a_split: mm_split_rows layout (M, 2*Kp(K)); w_split[l]: mm_split_weights layout of layer l;
  * bias[l]: (widths[l],) device or null; acts[l]: MM_ACT_*; the head needs widths[n-1] <= 32.
@@ -297,7 +297,7 @@ int mm_tower2_small(const mm_concat_piece* pieces_host, int n_pieces, int64_t B,
  * NULL) and a caller-provided workspace — for callers outside this package's Python host; nothing is
  * allocated, no pre-split weights are needed (the bf16 splits live in the workspace).
  *   mm_mlp_forward: MLPBlock, h_l = act_l(h_{l-1} W_l + b_l), 1..8 layers (blocks/mlp.py:97-139,
- *     :275-280); the whole-tower kernel when mm_mlp_tc_supported, else one tcgen05 launch per layer.
+ *     :275-280); the whole-tower kernel when mm_mlp_tc_supported, else one wgmma launch per layer.
  *   mm_cross_forward: CrossBlock, x_{l+1} = x0 * (x_l W_l + b_l) + x_l, W_l (d, d)
  *     (blocks/cross.py:29-109, :188-202); depth > 1 needs x_stride == d.
  * workspace: 256-B aligned device memory of at least mm_*_workspace_bytes(...) (-1 on bad arguments). */
@@ -331,7 +331,7 @@ int mm_inbatch_scores(const float* q, const float* pos, const float* neg, int64_
                       float temperature, float* out, int64_t out_stride, void* stream);
 /* Tensor-core version of the same logits, in two calls:
  *   mm_positive_scores   : column 0   (row-wise dot, logQ, temperature)
- *   mm_inbatch_scores_tc : columns 1..N — tcgen05 GEMM Q.N^T on split-bf16 operands
+ *   mm_inbatch_scores_tc : columns 1..N — wgmma GEMM Q.N^T on split-bf16 operands
  *                          (q_split (B, 2*Kp) and neg_split (N, 2*Kp), both from mm_split_rows,
  *                          Kp = mm_tc_padded_k(D)) with mask / logQ / temperature in the epilogue. */
 int mm_positive_scores(const float* q, const float* pos, int64_t B, int D, const float* pos_prob,
@@ -345,7 +345,7 @@ int mm_inbatch_scores_tc(const void* q_split, const void* neg_split, int64_t B, 
  * K10  Query x catalog scoring without materialising (B, N_I):
  *   logits[b,i] = q[b].E[i] (+ bias[i])   (outputs/classification.py:347-357 EmbeddingTablePrediction;
  *   blocks/retrieval/base.py:431-438; outputs/topk.py:221-223 BruteForce; core/index.py:236-237)
- * One tcgen05 GEMM pass over the catalog whose epilogue folds every logits tile into per-row
+ * One wgmma GEMM pass over the catalog whose epilogue folds every logits tile into per-row
  *   out_stats (B,3) = [max, log-sum-exp, logit[target]]   — the inputs of
  *                     CategoricalCrossEntropy(from_logits=True) (losses/listwise.py:38-50); nullable
  *   topk_scores/topk_ids (B,k): tf.math.top_k order (descending, ties -> lower id), k <= 32; k = 0: off
@@ -366,7 +366,7 @@ int mm_catalog_score(const void* q_split, int64_t B, int D, const void* e_split,
  *   out_stats (B,3) = [row max, log-sum-exp over {pos} U {negatives}, pos]   ->  loss[b] = out_stats[b,1] - out_stats[b,2]
  * pos_logit (B,): column 0 as mm_positive_scores writes it (logQ and temperature already applied);
  * negatives: (pos_ids[b] == neg_ids[n] && downscore ? false_neg_score : q[b].neg[n] - log(neg_prob[n] + 1e-16)) / temperature.
- * One tcgen05 pass of the catalog-scoring kernel (its epilogue with the id mask) + the merge kernel; 1.07 GB of
+ * One wgmma pass of the catalog-scoring kernel (its epilogue with the id mask) + the merge kernel; 1.07 GB of
  * logits at B = N = 16 384 never exist.  workspace: mm_catalog_workspace_bytes(B, N, 0). */
 int mm_inbatch_softmax_ce(const void* q_split, const void* neg_split, int64_t B, int64_t N, int D, const void* pos_ids,
                           const void* neg_ids, int id_dtype, int downscore, float false_neg_score, const float* pos_logit,

@@ -1,4 +1,4 @@
-"""models_b200 — B200-native (sm_100a) implementation of the Merlin Models hot path:
+"""models_b200 — H100-native (sm_90a) implementation of the Merlin Models hot path:
 embedding lookup -> MLP tower -> interaction / scoring, behind the reference's constructors.
 
     import models_b200 as mm

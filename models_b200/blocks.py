@@ -19,7 +19,7 @@ from .inputs import (ContinuousFeatures, EmbeddingOptions, Embeddings, Embedding
                      infer_embedding_dim)
 from .schema import Schema, Tags
 
-# dense-layer engine: "fp32" = exact CUDA-core kernel (mm_dense_fp32); "tc" = tcgen05 split-bf16
+# dense-layer engine: "fp32" = exact CUDA-core kernel (mm_dense_fp32); "tc" = wgmma split-bf16
 _DENSE_ENGINE = ["auto"]
 
 
@@ -77,7 +77,7 @@ def run_dense_chain(x: Optional[torch.Tensor], layers: "List[_Dense]", a_split: 
     epilogue when it applies, by one mm_split_rows pass over the fp32 result otherwise.
 
     tensor-core engine ("auto"/"tc"): x is split once into bf16 (hi, lo); every layer is one
-    tcgen05 launch whose epilogue (bias + activation) directly emits the NEXT layer's split-bf16
+    wgmma launch whose epilogue (bias + activation) directly emits the NEXT layer's split-bf16
     operand, so intermediate activations never exist in fp32 in HBM; the last layer writes fp32.
     "fp32" engine: exact CUDA-core kernels (parity anchor)."""
     if a_split is not None:  # producer (interaction kernel) already emitted the split-bf16 operand
@@ -108,7 +108,7 @@ def run_dense_chain(x: Optional[torch.Tensor], layers: "List[_Dense]", a_split: 
         raise ValueError(f"{layers[0].name}: input width {K} != kernel rows {layers[0].input_dim}")
     widths = [l.units for l in layers]
     if _MLP_FUSION[0] and ops.mlp_tc_supported(K, widths, head=fuse_head):
-        # whole tower in one launch: layers 2..n run on chip, activations stay in tensor memory
+        # whole tower in one launch: layers 2..n run on chip, activations stay in registers
         _LAST_PATH[0] = "mlp_tc"
         kw = {}
         if fuse_head:
@@ -696,7 +696,7 @@ class CrossBlockSeq(SequentialBlock):
         return x
 
     def _call_tc(self, x0: torch.Tensor, layers) -> torch.Tensor:
-        """x_{l+1} = x0 * (x_l W_l + b_l) + x_l with every layer one tcgen05 launch: the epilogue reads
+        """x_{l+1} = x0 * (x_l W_l + b_l) + x_l with every layer one wgmma launch: the epilogue reads
         x0 and x_l (fp32) and writes x_{l+1} both as fp32 (next residual) and split-bf16 (next operand)."""
         B, d = x0.shape
         for l in layers:

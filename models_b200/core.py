@@ -1,4 +1,4 @@
-"""Block plumbing for the B200 hot path: lazy device weights, Keras-style initialisers, the
+"""Block plumbing for the H100 hot path: lazy device weights, Keras-style initialisers, the
 reference's dict-of-features conventions (sorted-name aggregation, `__values`/`__offsets` ragged
 pairs) and a Prediction record.
 
@@ -74,7 +74,7 @@ def set_buffer_namespace(ns: int) -> int:
 def default_device() -> torch.device:
     if not torch.cuda.is_available():
         raise RuntimeError(
-            "models_b200 needs a CUDA device: the hot path is hand-written sm_100a kernels and has no "
+            "models_b200 needs a CUDA device: the hot path is hand-written sm_90a kernels and has no "
             "CPU fallback (the CPU restatement lives in oracle/ and is test infrastructure only)"
         )
     return torch.device("cuda", torch.cuda.current_device())

@@ -1,9 +1,9 @@
-"""Build libmm_b200.so (the C-ABI in include/mm_b200.h) for sm_100a with nvcc, in-tree.
+"""Build libmm_b200.so (the C-ABI in include/mm_b200.h) for sm_90a with nvcc, in-tree.
 
     python -m models_b200.csrc.build [--force] [--verbose]
 
-The library is written to models_b200/_lib/libmm_b200.so so that it travels with the
-repository snapshot to the GPU box (it is git-ignored, not gpurun-ignored).
+The library is written to models_b200/_lib/libmm_b200.so (git-ignored), so the package is importable from
+the repository tree without an install step.
 """
 from __future__ import annotations
 
@@ -20,7 +20,7 @@ LIB_DIR = PKG / "_lib"
 LIB = LIB_DIR / "libmm_b200.so"
 OBJ_DIR = CSRC / "build"
 
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC,-O3", "--expt-relaxed-constexpr"]
 
 

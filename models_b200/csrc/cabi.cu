@@ -37,7 +37,7 @@ int sm_count() {
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0)
       cached = n;
     else
-      cached = 148;  // B200
+      cached = 132;  // H100 SXM
   }
   return cached;
 }

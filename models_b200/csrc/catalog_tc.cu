@@ -1,4 +1,4 @@
-// Query x catalog scoring without materialising the (B, N_I) logits: tcgen05 GEMM whose epilogue
+// Query x catalog scoring without materialising the (B, N_I) logits: wgmma GEMM whose epilogue
 // streams every 128x128 logits tile straight into per-row running statistics —
 //   * soft-max cross-entropy inputs: row max, log-sum-exp, logit of the target item
 //     (CategoricalCrossEntropy(from_logits=True), merlin/models/tf/losses/listwise.py:38-50), and/or
@@ -8,11 +8,13 @@
 //
 // Work item = (128-query block, split of the item range).  The query tile (A, split-bf16) is
 // loaded once per work item and stays in shared memory; item tiles (B operand, 128 items x Kp,
-// split-bf16, precomputed once per catalog with mm_split_rows) stream through a TMA pipeline; the
-// fp32 accumulator is double-buffered in TMEM so the reduction of tile j overlaps the MMAs of tile
-// j+1.  Every epilogue thread owns one query row and keeps (max, sum-exp, target logit, top-k list)
-// for the columns it sees; partial results go to a small workspace and a second kernel merges the
-// 2*S partials per row.  3-pass split-bf16 = fp32-grade logits.
+// split-bf16, precomputed once per catalog with mm_split_rows) stream through a TMA pipeline that
+// refills while the consumers reduce.  CTA = two consumer warpgroups (64 query rows each) + one TMA
+// producer warp.  The reduction works on the wgmma accumulator fragment in registers: a thread holds
+// two query rows and, of every tile, the 32 columns 8 j + 2 (lane % 4) + {0, 1}; it keeps (max,
+// sum-exp, target logit, top-k list) per row for the columns it sees, so the four lanes of a quad are
+// the kParts partial results of a row.  Partials go to a small workspace and a second kernel merges
+// the kParts*S partials per row.  3-pass split-bf16 = fp32-grade logits.
 #include <cstring>
 
 #include "tc_common.cuh"
@@ -22,11 +24,11 @@ namespace cat {
 
 using namespace mm::tc;
 
-constexpr int BM = 128, BN = 128, BLOCK_K = 64, UMMA_K = 16;
-constexpr int kEpiWarps = 16;                   // 4 per TMEM lane quadrant: one 32-column chunk of every tile each
-constexpr int kParts = kEpiWarps / 4;            // partial results per (row, item-range split)
-constexpr int kThreads = 64 + 32 * kEpiWarps;
-constexpr int MAX_K = 32;  // top-k list length held per thread
+constexpr int BM = 128, BN = 128, BLOCK_K = 64, MMA_K = 16;
+constexpr int kConsumerWarps = 8;                // two warpgroups
+constexpr int kParts = 4;                        // partial results per (row, item-range split): the lanes of a quad
+constexpr int kThreads = 32 * (kConsumerWarps + 1);  // + warp 8: TMA producer
+constexpr int MAX_K = 32;  // top-k list length held per thread and row
 constexpr uint32_t TILE_BYTES = 128 * BLOCK_K * 2;  // one 128-row x 64-col bf16 tile = 16 KB
 
 struct Params {
@@ -67,7 +69,7 @@ static __device__ __noinline__ float topk_insert(float* tv, long long* ti, int k
 }
 
 // LSE / TOPK / MASK select the epilogue at compile time: the log-sum-exp-only variants keep no top-k list (64 local
-// words per thread otherwise) and the unmasked ones no id compares.
+// words per thread and row otherwise) and the unmasked ones no id compares.
 template <bool LSE, bool TOPK, bool MASK>
 __global__ void __launch_bounds__(kThreads, 1)
 catalog_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const Params p) {
@@ -79,48 +81,31 @@ catalog_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   uint8_t* smem_b = smem + A_BYTES;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem_b + (size_t)p.stages * STAGE_BYTES);
   uint64_t* full_bar = bars;                        // [stages]
-  uint64_t* empty_bar = bars + p.stages;            // [stages]
-  uint64_t* tmem_full = bars + 2 * p.stages;        // [2]
-  uint64_t* tmem_empty = bars + 2 * p.stages + 2;   // [2]
-  uint64_t* a_full = bars + 2 * p.stages + 4;       // [1]
-  uint64_t* a_empty = bars + 2 * p.stages + 5;      // [1]
-  uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(bars + 2 * p.stages + 6);
-  float* bias_s = reinterpret_cast<float*>(bars + 2 * p.stages + 8);  // [2][128]
+  uint64_t* empty_bar = bars + p.stages;            // [stages] one arrive per consumer warp
+  uint64_t* a_full = bars + 2 * p.stages;           // [1]
+  uint64_t* a_empty = bars + 2 * p.stages + 1;      // [1] one arrive per consumer warp
+  float* bias_s = reinterpret_cast<float*>(bars + 2 * p.stages + 2);  // [2][128]
   int* ids_lo = reinterpret_cast<int*>(bias_s + 2 * BN);                // [2][128] low words of the column ids (MASK)
   int* ids_hi = ids_lo + 2 * BN;                                        // [2][128] high words
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long long m_blocks = (p.M + BM - 1) / BM;
   const long long items = m_blocks * p.S;
-  const uint32_t tmem_cols = 256;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kConsumerWarps && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(smem_u32(full_bar + s), 1);
-      mbar_init(smem_u32(empty_bar + s), 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(smem_u32(tmem_full + a), 1);
-      mbar_init(smem_u32(tmem_empty + a), kEpiWarps);
+      mbar_init(smem_u32(empty_bar + s), kConsumerWarps);
     }
     mbar_init(smem_u32(a_full), 1);
-    mbar_init(smem_u32(a_empty), 1);
+    mbar_init(smem_u32(a_empty), kConsumerWarps);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_base_slot)),
-                 "r"(tmem_cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_base_slot;
 
-  if (warp == 0) {
+  if (warp == kConsumerWarps) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       int stage = 0;
@@ -153,99 +138,59 @@ catalog_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc(BM, BN);
-      int stage = 0, acc = 0;
-      uint32_t phase = 0, acc_phase = 0, a_phase = 0;
-      for (long long item = blockIdx.x; item < items; item += gridDim.x) {
-        const int split = (int)(item % p.S);
-        const int t0 = split * p.tiles_per_split, t1 = min(p.n_tiles, t0 + p.tiles_per_split);
-        mbar_wait(smem_u32(a_full), a_phase);
-        a_phase ^= 1;
-        tcgen05_fence_after();
-        const uint32_t a_base = smem_u32(smem_a);
-        for (int t = t0; t < t1; ++t) {
-          mbar_wait(smem_u32(tmem_empty + acc), acc_phase ^ 1);
-          mbar_wait(smem_u32(full_bar + stage), phase);
-          tcgen05_fence_after();
-          const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN);
-          const uint32_t b_base = smem_u32(smem_b + (size_t)stage * STAGE_BYTES);
-          uint32_t accumulate = 0;
-          for (int kb = 0; kb < p.KB; ++kb) {
-            const uint32_t a_hi = a_base + kb * TILE_BYTES, a_lo = a_base + (p.KB + kb) * TILE_BYTES;
-            const uint32_t b_hi = b_base + kb * TILE_BYTES, b_lo = b_base + (p.KB + kb) * TILE_BYTES;
-#pragma unroll
-            for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-              umma_bf16(d_tmem, make_desc_sw128(a_hi + k * 32), make_desc_sw128(b_lo + k * 32), idesc, accumulate);
-              accumulate = 1;
-            }
-#pragma unroll
-            for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-              umma_bf16(d_tmem, make_desc_sw128(a_lo + k * 32), make_desc_sw128(b_hi + k * 32), idesc, 1);
-#pragma unroll
-            for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-              umma_bf16(d_tmem, make_desc_sw128(a_hi + k * 32), make_desc_sw128(b_hi + k * 32), idesc, 1);
-          }
-          tcgen05_commit(smem_u32(empty_bar + stage));
-          tcgen05_commit(smem_u32(tmem_full + acc));
-          if (++stage == p.stages) {
-            stage = 0;
-            phase ^= 1;
-          }
-          if (++acc == 2) {
-            acc = 0;
-            acc_phase ^= 1;
-          }
-        }
-        tcgen05_commit(smem_u32(a_empty));  // all MMAs reading this query tile have retired
-      }
-    }
   } else {
-    // ===================== epilogue: streaming reduction =====================
-    // 16 warps: warp w reads TMEM lanes 32*(w&3).. (its query rows) and owns column chunk `part` of every tile,
-    // so a thread sees 32 logits per tile.  Per logit: one FMNMX for the chunk maximum, then FFMA + MUFU.EX2 +
-    // FADD into one of four independent partial sums (round 1: 8 warps, exp2f with range handling, a bounds
-    // select and a shared-memory bias add per logit, one serial sum: ~5 900 cycles per tile against ~1 080 of MMA).
-    const int q = warp & 3;
-    const int part = (warp - 2) >> 2;
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    // ===================== consumers: MMA + streaming reduction =====================
+    // Per logit: one FMNMX for the chunk maximum, then FFMA + MUFU.EX2 + FADD into one of four independent
+    // partial sums.
+    const int wg = warp >> 2;
+    const int part = lane & 3;
+    const int frow = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // tile row of fragment row 0 (row 1 is 8 further)
+    int stage = 0, buf = 0;
+    uint32_t phase = 0, a_phase = 0;
     const float LOG2E = 1.4426950408889634f;
     const bool has_bias = p.bias != nullptr;
     for (long long item = blockIdx.x; item < items; item += gridDim.x) {
       const long long m0 = (item / p.S) * BM;
       const int split = (int)(item % p.S);
       const int t0 = split * p.tiles_per_split, t1 = min(p.n_tiles, t0 + p.tiles_per_split);
-      const long long row = m0 + q * 32 + lane;
-      long long target = -1;
-      if (LSE && p.targets && row < p.M)
-        target = p.id_is64 ? reinterpret_cast<const long long*>(p.targets)[row]
-                           : (long long)reinterpret_cast<const int*>(p.targets)[row];
+      long long row[2], target[2] = {-1, -1}, my_id[2] = {0, 0};
       const bool do_mask = MASK && p.row_ids != nullptr;
-      long long my_id = 0;
-      if (do_mask && row < p.M)
-        my_id = p.id_is64 ? reinterpret_cast<const long long*>(p.row_ids)[row] : (long long)reinterpret_cast<const int*>(p.row_ids)[row];
-      float run_m = -INFINITY, run_s = 0.0f, tlogit = __int_as_float(0x7fc00000);  // NaN = "not seen"
-      float tv[TOPK ? MAX_K : 1];
-      long long ti[TOPK ? MAX_K : 1];
-      float thr = -INFINITY;  // k-th best value of this thread's list (register copy of tv[topk-1])
-      if (TOPK) {
+      float run_m[2], run_s[2], tlogit[2], thr[2];
+      float tv[2][TOPK ? MAX_K : 1];
+      long long ti[2][TOPK ? MAX_K : 1];
 #pragma unroll
-        for (int r = 0; r < MAX_K; ++r) {
-          tv[r] = -INFINITY;
-          ti[r] = -1;
+      for (int h = 0; h < 2; ++h) {
+        row[h] = m0 + frow + 8 * h;
+        if (LSE && p.targets && row[h] < p.M)
+          target[h] = p.id_is64 ? reinterpret_cast<const long long*>(p.targets)[row[h]]
+                                : (long long)reinterpret_cast<const int*>(p.targets)[row[h]];
+        if (do_mask && row[h] < p.M)
+          my_id[h] = p.id_is64 ? reinterpret_cast<const long long*>(p.row_ids)[row[h]]
+                               : (long long)reinterpret_cast<const int*>(p.row_ids)[row[h]];
+        run_m[h] = -INFINITY;
+        run_s[h] = 0.0f;
+        tlogit[h] = __int_as_float(0x7fc00000);  // NaN = "not seen"
+        thr[h] = -INFINITY;  // k-th best value of this row's list (register copy of tv[h][topk-1])
+        if (TOPK) {
+#pragma unroll
+          for (int r = 0; r < MAX_K; ++r) {
+            tv[h][r] = -INFINITY;
+            ti[h][r] = -1;
+          }
         }
       }
+      mbar_wait(smem_u32(a_full), a_phase);
+      a_phase ^= 1;
+      const uint32_t a_base = smem_u32(smem_a) + (uint32_t)wg * (TILE_BYTES / 2);
       for (int t = t0; t < t1; ++t) {
         const long long n0 = (long long)t * BN;
-        float* bs = bias_s + acc * BN;
-        int* cl = ids_lo + acc * BN;
-        int* chh = ids_hi + acc * BN;
+        float* bs = bias_s + buf * BN;
+        int* cl = ids_lo + buf * BN;
+        int* chh = ids_hi + buf * BN;
+        buf ^= 1;
         if (has_bias || do_mask) {  // per-tile column data -> shared memory (the buffer of tile t-2 is free: its readers passed bar 1 of t-1)
-          asm volatile("bar.sync 1, %0;" ::"n"(32 * kEpiWarps) : "memory");
-          for (int i = threadIdx.x - 64; i < BN; i += 32 * kEpiWarps) {
+          named_bar(1, 32 * kConsumerWarps);
+          for (int i = threadIdx.x; i < BN; i += 32 * kConsumerWarps) {
             const bool in = n0 + i < p.I;
             if (has_bias) {
               float bv = in ? p.bias[n0 + i] : 0.0f;
@@ -260,107 +205,120 @@ catalog_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
               chh[i] = (int)(cid >> 32);
             }
           }
-          asm volatile("bar.sync 1, %0;" ::"n"(32 * kEpiWarps) : "memory");
+          named_bar(1, 32 * kConsumerWarps);
         }
-        mbar_wait(smem_u32(tmem_full + acc), acc_phase);
-        tcgen05_fence_after();
-        const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BN);
-        const int c0 = part << 5;
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(t_row + c0, r);
-        tmem_ld_wait();
-        tcgen05_fence_before();
+        // ---- 64 x 128 logits of this warpgroup ----
+        float acc[64];
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
+        mbar_wait(smem_u32(full_bar + stage), phase);
+        const uint32_t b_base = smem_u32(smem_b + (size_t)stage * STAGE_BYTES);
+        wgmma_fence_acc(acc);
+        wgmma_fence();
+        for (int kb = 0; kb < p.KB; ++kb) {
+          const uint32_t a_hi = a_base + kb * TILE_BYTES, a_lo = a_base + (p.KB + kb) * TILE_BYTES;
+          const uint32_t b_hi = b_base + kb * TILE_BYTES, b_lo = b_base + (p.KB + kb) * TILE_BYTES;
+#pragma unroll
+          for (int k = 0; k < BLOCK_K / MMA_K; ++k) wgmma_ss(BN, acc, make_desc_sw128(a_hi + k * 32), make_desc_sw128(b_lo + k * 32));
+#pragma unroll
+          for (int k = 0; k < BLOCK_K / MMA_K; ++k) wgmma_ss(BN, acc, make_desc_sw128(a_lo + k * 32), make_desc_sw128(b_hi + k * 32));
+#pragma unroll
+          for (int k = 0; k < BLOCK_K / MMA_K; ++k) wgmma_ss(BN, acc, make_desc_sw128(a_hi + k * 32), make_desc_sw128(b_hi + k * 32));
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+        wgmma_fence_acc(acc);
         __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(tmem_empty + acc));  // this warp's slice of the accumulator is in registers
-        float v[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-        if (has_bias) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] += bs[c0 + j];
+        if (lane == 0) mbar_arrive(smem_u32(empty_bar + stage));
+        if (++stage == p.stages) {
+          stage = 0;
+          phase ^= 1;
         }
-        if (MASK) {
-          if (do_mask) {  // compare the low words (one LDS.128 per 4 columns); the high word only on a low-word match
-            const int my_lo = (int)my_id, my_hi = (int)(my_id >> 32);
 #pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              const int4 c4 = *reinterpret_cast<const int4*>(cl + c0 + j);
-              if (c4.x == my_lo && chh[c0 + j] == my_hi) v[j] = p.false_neg_score;
-              if (c4.y == my_lo && chh[c0 + j + 1] == my_hi) v[j + 1] = p.false_neg_score;
-              if (c4.z == my_lo && chh[c0 + j + 2] == my_hi) v[j + 2] = p.false_neg_score;
-              if (c4.w == my_lo && chh[c0 + j + 3] == my_hi) v[j + 3] = p.false_neg_score;
+        for (int h = 0; h < 2; ++h) {
+          // fragment row h: v[j] is column 8 (j / 2) + 2 part + (j % 2) of the tile (ascending in j)
+          float v[32];
+#pragma unroll
+          for (int j = 0; j < 32; ++j) v[j] = acc[4 * (j >> 1) + 2 * h + (j & 1)];
+          if (has_bias) {
+#pragma unroll
+            for (int j = 0; j < 32; ++j) v[j] += bs[8 * (j >> 1) + 2 * part + (j & 1)];
+          }
+          if (MASK) {
+            if (do_mask) {  // compare the low words; the high word only on a low-word match
+              const int my_lo = (int)my_id[h], my_hi = (int)(my_id[h] >> 32);
+#pragma unroll
+              for (int j = 0; j < 32; j += 2) {
+                const int c = 8 * (j >> 1) + 2 * part;
+                const int2 c2 = *reinterpret_cast<const int2*>(cl + c);
+                if (c2.x == my_lo && chh[c] == my_hi) v[j] = p.false_neg_score;
+                if (c2.y == my_lo && chh[c + 1] == my_hi) v[j + 1] = p.false_neg_score;
+              }
+            }
+            if (p.inv_temp != 1.0f) {
+#pragma unroll
+              for (int j = 0; j < 32; ++j) v[j] *= p.inv_temp;
             }
           }
-          if (p.inv_temp != 1.0f) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] *= p.inv_temp;
-          }
-        }
-        if (n0 + c0 + 32 > p.I) {  // ragged last tile only
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (n0 + c0 + j >= p.I) v[j] = -INFINITY;
-        }
-        float cmax = v[0];
-#pragma unroll
-        for (int j = 1; j < 32; ++j) cmax = fmaxf(cmax, v[j]);
-        if (LSE && cmax > -INFINITY) {
-          const float m_new = fmaxf(run_m, cmax);
-          const float mb = m_new * LOG2E;
-          float s0 = run_s * ex2_approx(fmaf(run_m, LOG2E, -mb)), s1 = 0.0f, s2 = 0.0f, s3 = 0.0f;  // run_m = -inf -> 0
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            s0 += ex2_approx(fmaf(v[j], LOG2E, -mb));
-            s1 += ex2_approx(fmaf(v[j + 1], LOG2E, -mb));
-            s2 += ex2_approx(fmaf(v[j + 2], LOG2E, -mb));
-            s3 += ex2_approx(fmaf(v[j + 3], LOG2E, -mb));
-          }
-          run_m = m_new;
-          run_s = (s0 + s1) + (s2 + s3);
-          const long long dt = target - (n0 + c0);
-          if (dt >= 0 && dt < 32) {  // once per row: predicated moves (a dynamic v[dt] would put v[] in local memory)
-            const int di = (int)dt;
+          if (n0 + BN > p.I) {  // ragged last tile only
 #pragma unroll
             for (int j = 0; j < 32; ++j)
-              asm("{\n\t.reg .pred p;\n\tsetp.eq.s32 p, %1, %2;\n\t@p mov.f32 %0, %3;\n\t}" : "+f"(tlogit) : "r"(di), "r"(j), "f"(v[j]));
+              if (n0 + 8 * (j >> 1) + 2 * part + (j & 1) >= p.I) v[j] = -INFINITY;
+          }
+          float cmax = v[0];
+#pragma unroll
+          for (int j = 1; j < 32; ++j) cmax = fmaxf(cmax, v[j]);
+          if (LSE && cmax > -INFINITY) {
+            const float m_new = fmaxf(run_m[h], cmax);
+            const float mb = m_new * LOG2E;
+            float s0 = run_s[h] * ex2_approx(fmaf(run_m[h], LOG2E, -mb)), s1 = 0.0f, s2 = 0.0f, s3 = 0.0f;  // run_m = -inf -> 0
+#pragma unroll
+            for (int j = 0; j < 32; j += 4) {
+              s0 += ex2_approx(fmaf(v[j], LOG2E, -mb));
+              s1 += ex2_approx(fmaf(v[j + 1], LOG2E, -mb));
+              s2 += ex2_approx(fmaf(v[j + 2], LOG2E, -mb));
+              s3 += ex2_approx(fmaf(v[j + 3], LOG2E, -mb));
+            }
+            run_m[h] = m_new;
+            run_s[h] = (s0 + s1) + (s2 + s3);
+            const long long dt = target[h] - n0 - 2 * part;
+            if (dt >= 0 && dt < BN) {  // predicated selects (a dynamic v[dt] would put v[] in local memory)
+              const int di = (int)dt;
+#pragma unroll
+              for (int j = 0; j < 32; ++j)
+                if (di == 8 * (j >> 1) + (j & 1)) tlogit[h] = v[j];
+            }
+          }
+          if (TOPK && cmax > thr[h]) {
+            // ascending item order inside a thread; strict '>' keeps the lower id on ties.  The values stay in
+            // registers (fully unrolled compares against the list's k-th value); only the rare insertion touches
+            // the list, which lives in local memory.
+#pragma unroll
+            for (int j = 0; j < 32; ++j)
+              if (v[j] > thr[h]) thr[h] = topk_insert(tv[h], ti[h], p.topk, v[j], n0 + 8 * (j >> 1) + 2 * part + (j & 1));
           }
         }
-        if (TOPK && cmax > thr) {
-          // ascending item order inside a thread; strict '>' keeps the lower id on ties.  The chunk stays in
-          // registers (fully unrolled compares against the list's k-th value); only the rare insertion touches the
-          // list, which lives in local memory.  (A dynamically indexed v[j] here spilled the whole chunk to local
-          // memory on every tile: 373 ms instead of 85 ms for 16 384 x 10 M.)
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (v[j] > thr) thr = topk_insert(tv, ti, p.topk, v[j], n0 + c0 + j);
-        }
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1;
-        }
       }
-      if (row < p.M) {
-        const long long pidx = row * ((long long)kParts * p.S) + split * kParts + part;
-        if (LSE) {
-          p.ws_lse[pidx * 3 + 0] = run_m;
-          p.ws_lse[pidx * 3 + 1] = run_s;
-          p.ws_lse[pidx * 3 + 2] = tlogit;
-        }
-        if (TOPK) {
-          for (int r = 0; r < p.topk; ++r) {
-            p.ws_vals[pidx * p.topk + r] = tv[r];
-            p.ws_ids[pidx * p.topk + r] = ti[r];
+      __syncwarp();
+      if (lane == 0) mbar_arrive(smem_u32(a_empty));  // every MMA of this warp that read the query tile has completed
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (row[h] < p.M) {
+          const long long pidx = row[h] * ((long long)kParts * p.S) + split * kParts + part;
+          if (LSE) {
+            p.ws_lse[pidx * 3 + 0] = run_m[h];
+            p.ws_lse[pidx * 3 + 1] = run_s[h];
+            p.ws_lse[pidx * 3 + 2] = tlogit[h];
+          }
+          if (TOPK) {
+            for (int r = 0; r < p.topk; ++r) {
+              p.ws_vals[pidx * p.topk + r] = tv[h][r];
+              p.ws_ids[pidx * p.topk + r] = ti[h][r];
+            }
           }
         }
       }
     }
-  }
-
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(tmem_cols) : "memory");
   }
 }
 
@@ -524,11 +482,12 @@ static int launch(const char* who, const void* q_split, int64_t B, int D, const 
   p.ws_ids = (long long*)(ws + ((B * P * 3 * (int64_t)sizeof(float) + 15) / 16) * 16);
   p.ws_vals = (float*)((uint8_t*)p.ws_ids + B * P * (int64_t)k * sizeof(long long));
   const size_t a_bytes = 2ull * p.KB * TILE_BYTES, stage_bytes = 2ull * p.KB * TILE_BYTES;
-  int stages = (int)((220 * 1024 - 4096 - a_bytes) / stage_bytes);
+  const size_t fixed = 1024 + a_bytes + 16 * sizeof(uint64_t) + 2 * BN * sizeof(float) + 2 * BN * sizeof(long long);
+  int stages = (int)((227 * 1024 - fixed) / stage_bytes);
   if (stages > 4) stages = 4;
   MM_REQUIRE(stages >= 2, MM_ERR_UNSUPPORTED, "%s: tiles do not fit two pipeline stages", who);
   p.stages = stages;
-  const size_t smem = 1024 + a_bytes + stages * stage_bytes + (2 * stages + 8) * sizeof(uint64_t) + 2 * BN * sizeof(float) +
+  const size_t smem = 1024 + a_bytes + stages * stage_bytes + (2 * stages + 2) * sizeof(uint64_t) + 2 * BN * sizeof(float) +
                       2 * BN * sizeof(long long);
   CUtensorMap tmA, tmB;
   int rc = make_map(&tmA, q_split, (uint64_t)B, (uint64_t)2 * Kp, BM);

@@ -1,12 +1,12 @@
-// Tensor-core dense layer for sm_100a: tcgen05.mma (kind::f16, bf16 operands, fp32 TMEM
-// accumulators) fed by TMA, warp-specialised persistent CTAs.
+// Tensor-core dense layer for sm_90a: wgmma (bf16 operands, fp32 register accumulators) fed by
+// TMA through an mbarrier ring, warp-specialised persistent CTAs.
 //
 //   out = act(x @ W + bias)            (Keras Dense, merlin/models/tf/blocks/mlp.py:275-280)
 //   out = x0 * (x @ W + bias) + x      (DCN-v2 cross, blocks/cross.py:196-198)
 //
 // fp32 parity on bf16 tensor cores: every fp32 operand is carried as a split-bf16 pair
 // x = hi + lo (hi = bf16(x), lo = bf16(x - hi)); passes = 3 accumulates hi*lo + lo*hi + hi*hi
-// into ONE fp32 TMEM accumulator (relative error ~2^-16: fp32-grade, well inside the 1e-3 logit
+// into ONE fp32 accumulator (relative error ~2^-16: fp32-grade, well inside the 1e-3 logit
 // tolerance of the north star); passes = 1 is plain bf16.
 //
 // Layout in HBM:  a_split (M, 2*Kp) bf16 = [hi(0..Kp) | lo(0..Kp)]      K-major rows
@@ -14,10 +14,12 @@
 // Kp = K rounded up to 64 (one 128-byte swizzle row per k-block), Np = N rounded up to 16
 // (<= 128) or to 128 (> 128).  Padding is zero, so it contributes nothing.
 //
-// CTA = 6 warps: warp 0 TMA producer, warp 1 MMA issuer (+TMEM owner), warps 2-5 epilogue
-// (TMEM -> registers -> bias/activation/cross -> global).  A pipeline stage holds the four
-// 64-wide k-block tiles {A_hi, A_lo, B_hi, B_lo}; the accumulator is double-buffered in TMEM so
-// the epilogue of tile i overlaps the MMAs of tile i+1.
+// CTA = 9 warps: warps 0-7 are two consumer warpgroups (wgmma over 64 rows of the 128-row tile
+// each, then the epilogue of those rows), warp 8 is the TMA producer.  A pipeline stage holds the
+// four 64-wide k-block tiles {A_hi, A_lo, B_hi, B_lo}; the producer refills the ring while the
+// consumers run the epilogue.  The epilogue goes through a shared-memory image of the fp32
+// accumulator (thread = one row, 32 columns per step), whose 32x32 chunks double as the per-warp
+// transpose tiles of the coalesced stores.
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -29,12 +31,13 @@ namespace tc {
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;   // bf16 elements = 128 bytes = one SWIZZLE_128B row
-constexpr int UMMA_K = 16;
-constexpr int kEpiWarps = 8;              // two per TMEM lane quarter, interleaved over 32-column chunks
-constexpr int kThreads = 64 + 32 * kEpiWarps;  // warp 0 TMA, warp 1 MMA, warps 2.. epilogue
+constexpr int MMA_K = 16;
+constexpr int kEpiWarps = 8;              // two consumer warpgroups
+constexpr int kThreads = 32 * (kEpiWarps + 1);  // + warp 8: TMA producer
 constexpr uint32_t A_TILE_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KB
-constexpr uint32_t EPI_STAGE_BYTES = 32 * 80 * 2;         // per epilogue warp: max(32x36 fp32, 2 x 32x80 B)
-static_assert(EPI_STAGE_BYTES >= 32 * 36 * 4, "transpose tile too small");
+
+// row pitch (floats) of the accumulator image: whole 32-column chunks + 4 floats (bank spread)
+__host__ __device__ constexpr int image_pitch(int BN) { return ((BN + 31) / 32) * 32 + 4; }
 
 struct Params {
   long long M;
@@ -73,25 +76,23 @@ struct Params {
 __global__ void __launch_bounds__(kThreads, 1)
 dense_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const Params p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve: [stages][A_hi | A_lo | B_hi | B_lo] (1024-B aligned tiles), then barriers
+  // carve: [resident A] [stages][A_hi | A_lo | B_hi | B_lo] (1024-B aligned tiles), accumulator image, barriers
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // pointer arithmetic keeps the shared state space (LDS/STS, not generic LD/ST)
   const uint32_t B_TILE_BYTES = (uint32_t)p.BN * BLOCK_K * 2;
   const int KB_ = p.Kp / BLOCK_K;
   const uint32_t A_RES_BYTES = p.resident_a ? (uint32_t)KB_ * 2 * A_TILE_BYTES : 0u;  // [kb][A_hi | A_lo]
   const uint32_t STAGE_BYTES = p.resident_a ? 2 * B_TILE_BYTES : 2 * A_TILE_BYTES + 2 * B_TILE_BYTES;
+  const int IP = image_pitch(p.BN);
   uint8_t* a_res = smem;
   smem += A_RES_BYTES;  // the ring starts after the resident A region
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * STAGE_BYTES);
+  float* img = reinterpret_cast<float*>(smem + (size_t)p.stages * STAGE_BYTES);  // [BLOCK_M][IP] fp32 accumulator
+  uint64_t* bars = reinterpret_cast<uint64_t*>(img + (size_t)BLOCK_M * IP);
   uint64_t* full_bar = bars;                       // [stages]
-  uint64_t* empty_bar = bars + p.stages;           // [stages]
-  uint64_t* tmem_full = bars + 2 * p.stages;       // [2]
-  uint64_t* tmem_empty = bars + 2 * p.stages + 2;  // [2]
-  uint64_t* a_full = bars + 2 * p.stages + 4;      // resident A landed (TMA tx)
-  uint64_t* a_empty = bars + 2 * p.stages + 5;     // MMAs of the m-row retired (tcgen05.commit)
-  uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(bars + 2 * p.stages + 6);
-  long long* ids_s = reinterpret_cast<long long*>(bars + 2 * p.stages + 8);                // [256] negative ids of the tile (scorer)
+  uint64_t* empty_bar = bars + p.stages;           // [stages] one arrive per consumer warp
+  uint64_t* a_full = bars + 2 * p.stages;          // resident A landed (TMA tx)
+  uint64_t* a_empty = bars + 2 * p.stages + 1;     // MMAs of the m-row retired (one arrive per consumer warp)
+  long long* ids_s = reinterpret_cast<long long*>(bars + 2 * p.stages + 2);               // [256] negative ids of the tile (scorer)
   float* bias_s = reinterpret_cast<float*>(ids_s + 256);                                   // [256] bias of the tile, zero padded
-  uint8_t* stage_tiles = reinterpret_cast<uint8_t*>(bias_s + 256);                         // kEpiWarps x EPI_STAGE_BYTES
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long long m_tiles = (p.M + BLOCK_M - 1) / BLOCK_M;
@@ -101,36 +102,21 @@ dense_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   const long long tile_first = p.resident_a ? (long long)blockIdx.x * p.tiles_per_cta : (long long)blockIdx.x;
   const long long tile_step = p.resident_a ? 1 : (long long)gridDim.x;
   const long long tile_end = p.resident_a ? (tile_first + p.tiles_per_cta < tiles ? tile_first + p.tiles_per_cta : tiles) : tiles;
-  uint32_t tmem_cols = 32;
-  while (tmem_cols < 2u * p.BN) tmem_cols <<= 1;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kEpiWarps && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(smem_u32(full_bar + s), 1);
-      mbar_init(smem_u32(empty_bar + s), 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(smem_u32(tmem_full + a), 1);
-      mbar_init(smem_u32(tmem_empty + a), kEpiWarps);  // one arrive per epilogue warp
+      mbar_init(smem_u32(empty_bar + s), kEpiWarps);
     }
     mbar_init(smem_u32(a_full), 1);
-    mbar_init(smem_u32(a_empty), 1);
+    mbar_init(smem_u32(a_empty), kEpiWarps);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {  // TMEM allocation (whole warp, .sync.aligned)
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_base_slot)),
-                 "r"(tmem_cols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_base_slot;
 
-  if (warp == 0) {
+  if (warp == kEpiWarps) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       int stage = 0;
@@ -176,74 +162,19 @@ dense_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc(BLOCK_M, p.BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      long long cur_mrow = -1;
-      uint32_t a_seen = 0;
-      for (long long tile = tile_first; tile < tile_end; tile += tile_step) {
-        if (p.resident_a && tile / p.n_tiles_n != cur_mrow) {
-          mbar_wait(smem_u32(a_full), a_seen & 1);
-          ++a_seen;
-          cur_mrow = tile / p.n_tiles_n;
-        }
-        mbar_wait(smem_u32(tmem_empty + acc), acc_phase ^ 1);
-        tcgen05_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * p.BN);
-        uint32_t accumulate = 0;
-        for (int kb = 0; kb < KB; ++kb) {
-          mbar_wait(smem_u32(full_bar + stage), phase);
-          tcgen05_fence_after();
-          const uint32_t st = smem_u32(smem + (size_t)stage * STAGE_BYTES);
-          const uint32_t a_hi = p.resident_a ? smem_u32(a_res + (size_t)kb * 2 * A_TILE_BYTES) : st, a_lo = a_hi + A_TILE_BYTES;
-          const uint32_t b_hi = p.resident_a ? st : st + 2 * A_TILE_BYTES, b_lo = b_hi + B_TILE_BYTES;
-          if (p.passes == 3) {
-            // small cross terms first, the dominant hi*hi product last
-#pragma unroll
-            for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-              umma_bf16(d_tmem, make_desc_sw128(a_hi + k * 32), make_desc_sw128(b_lo + k * 32), idesc, accumulate);
-              accumulate = 1;
-            }
-#pragma unroll
-            for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-              umma_bf16(d_tmem, make_desc_sw128(a_lo + k * 32), make_desc_sw128(b_hi + k * 32), idesc, 1);
-          }
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-            umma_bf16(d_tmem, make_desc_sw128(a_hi + k * 32), make_desc_sw128(b_hi + k * 32), idesc, accumulate);
-            accumulate = 1;
-          }
-          tcgen05_commit(smem_u32(empty_bar + stage));  // frees the smem stage when the MMAs retire
-          if (++stage == p.stages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        tcgen05_commit(smem_u32(tmem_full + acc));  // accumulator complete -> epilogue
-        if (p.resident_a && (tile + 1 >= tile_end || (tile + 1) / p.n_tiles_n != cur_mrow))
-          tcgen05_commit(smem_u32(a_empty));  // last tile of this m-row: the resident A may be replaced once these MMAs retire
-        if (++acc == 2) {
-          acc = 0;
-          acc_phase ^= 1;
-        }
-      }
-    }
   } else {
-    // ===================== epilogue warps (2..9) =====================
-    // TMEM -> registers (thread = one accumulator row, 32 columns per step) -> bias/act/cross ->
-    // per-warp shared-memory transpose tile -> coalesced 16-byte global stores (a warp store
-    // covers whole 64/128-byte row segments instead of 32 scattered 16-byte pieces).
-    const int q = warp & 3;            // TMEM lane quarter this warp may access
-    const int half = (warp - 2) >> 2;  // which interleaved set of 32-column chunks
-    uint8_t* stg = stage_tiles + (size_t)(warp - 2) * EPI_STAGE_BYTES;
-    float* stg_f = reinterpret_cast<float*>(stg);
-    int acc = 0;
-    uint32_t acc_phase = 0;
+    // ===================== consumer warpgroups (warps 0..7): MMA, then epilogue =====================
+    // warpgroup wg computes accumulator rows 64 wg ..; its warps then finish the 32-row quarters 2 wg, 2 wg + 1
+    // from the image: thread = one accumulator row, 32 columns per step, two warps per quarter interleaved over
+    // 32-column chunks.  Epilogue: image -> registers -> bias/act/cross -> per-warp shared-memory transpose
+    // tile (the chunk's own image region) -> coalesced 16-byte global stores.
+    const int wg = warp >> 2;
+    const int q = 2 * wg + (warp & 1);  // 32-row quarter of the tile this warp finishes
+    const int half = (warp >> 1) & 1;   // which interleaved set of 32-column chunks
+    int stage = 0;
+    uint32_t phase = 0;
+    long long cur_mrow = -1;
+    uint32_t a_seen = 0;
     const bool vec_f32 = p.out_f32 && ((p.out_stride & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.out_f32) & 15) == 0);
     const bool vec_x = p.x0 && ((p.x_stride & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.x0) & 15) == 0) &&
                        ((reinterpret_cast<uintptr_t>(p.xres) & 15) == 0);
@@ -251,7 +182,7 @@ dense_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     long long col_id = 0;
     uint32_t tile_wide = 0u;  // 1 when a negative id of the current tile needs 64 bits (OR-reduced by the staging barrier)
     auto load_columns = [&](int n0_, float& b, float& h, long long& id) {  // thread i < BN owns column n0_ + i (BN <= 256 threads)
-      const int i = (int)threadIdx.x - 64;
+      const int i = (int)threadIdx.x;
       b = 0.0f;
       h = 0.0f;
       id = -0x7fffffffffffffffll;
@@ -271,9 +202,9 @@ dense_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       // The global loads for tile t+1 are issued while tile t is processed (registers), so only shared-memory
       // stores sit between the two barriers — not a global-memory round trip per tile.
       if (tile == tile_first) load_columns(n0, col_b, col_h, col_id);
-      asm volatile("bar.sync 1, %0;" ::"n"(32 * kEpiWarps) : "memory");  // previous tile's readers are done
+      named_bar(1, 32 * kEpiWarps);  // previous tile's readers are done
       {
-        const int i = (int)threadIdx.x - 64;
+        const int i = (int)threadIdx.x;
         const bool col_hi_flag = p.score_mode && p.neg_ids && i < p.BN && col_id != -0x7fffffffffffffffll &&
                                  ((unsigned long long)col_id >> 32) != 0ull;
         if (i < p.BN) {
@@ -299,41 +230,90 @@ dense_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       if (p.score_mode && p.pos_ids && row0 + lane < p.M)
         my_pid = p.id_is64 ? reinterpret_cast<const long long*>(p.pos_ids)[row0 + lane]
                            : (long long)reinterpret_cast<const int*>(p.pos_ids)[row0 + lane];
-      mbar_wait(smem_u32(tmem_full + acc), acc_phase);
-      tcgen05_fence_after();
-      const uint32_t t_row = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * p.BN);
-      const int n_chunks = (p.BN + 31) >> 5;
-      if (half >= n_chunks) {  // nothing to read for this warp (BN <= 32): release the accumulator right away
-        tcgen05_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(tmem_empty + acc));
+
+      // ---- main loop: this warpgroup's 64 x BN accumulator over all k-blocks ----
+      if (p.resident_a && tile / p.n_tiles_n != cur_mrow) {
+        mbar_wait(smem_u32(a_full), a_seen & 1);
+        ++a_seen;
+        cur_mrow = tile / p.n_tiles_n;
       }
+      float acc[64];
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
+      for (int kb = 0; kb < KB; ++kb) {
+        mbar_wait(smem_u32(full_bar + stage), phase);
+        const uint32_t st = smem_u32(smem + (size_t)stage * STAGE_BYTES);
+        const uint32_t a_hi = (p.resident_a ? smem_u32(a_res + (size_t)kb * 2 * A_TILE_BYTES) : st) + (uint32_t)wg * (A_TILE_BYTES / 2),
+                       a_lo = a_hi + A_TILE_BYTES;
+        const uint32_t b_hi = p.resident_a ? st : st + 2 * A_TILE_BYTES, b_lo = b_hi + B_TILE_BYTES;
+        wgmma_fence_acc(acc);
+        wgmma_fence();
+        if (p.passes == 3) {
+          // small cross terms first, the dominant hi*hi product last
+#pragma unroll
+          for (int k = 0; k < BLOCK_K / MMA_K; ++k) wgmma_ss(p.BN, acc, make_desc_sw128(a_hi + k * 32), make_desc_sw128(b_lo + k * 32));
+#pragma unroll
+          for (int k = 0; k < BLOCK_K / MMA_K; ++k) wgmma_ss(p.BN, acc, make_desc_sw128(a_lo + k * 32), make_desc_sw128(b_hi + k * 32));
+        }
+#pragma unroll
+        for (int k = 0; k < BLOCK_K / MMA_K; ++k) wgmma_ss(p.BN, acc, make_desc_sw128(a_hi + k * 32), make_desc_sw128(b_hi + k * 32));
+        wgmma_commit();
+        wgmma_wait_all();
+        wgmma_fence_acc(acc);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(smem_u32(empty_bar + stage));  // this warp is done with the stage
+        if (++stage == p.stages) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
+      if (p.resident_a && (tile + 1 >= tile_end || (tile + 1) / p.n_tiles_n != cur_mrow)) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(smem_u32(a_empty));  // last tile of this m-row: the resident A may be replaced
+      }
+      // ---- accumulator fragment -> image rows 64 wg .. (the warpgroup's previous epilogue is done with them) ----
+      named_bar(2 + wg, 128);
+      {
+        const int r = 64 * wg + 16 * (warp & 3) + (lane >> 2), c = 2 * (lane & 3);
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          if (8 * j < p.BN) {
+            *reinterpret_cast<float2*>(img + (size_t)r * IP + 8 * j + c) = make_float2(acc[4 * j], acc[4 * j + 1]);
+            *reinterpret_cast<float2*>(img + (size_t)(r + 8) * IP + 8 * j + c) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+          }
+        }
+      }
+      named_bar(2 + wg, 128);
+
+      const int n_chunks = (p.BN + 31) >> 5;
       for (int ch = half; ch < n_chunks; ch += 2) {
         const int c0 = ch << 5;
-        uint32_t r[32];
         const int ncols = min(32, p.BN - c0);  // BN is a multiple of 16
-        if (ncols == 32) tmem_ld_32x32b_x32(t_row + c0, r);
-        else tmem_ld_32x32b_x16(t_row + c0, r);
-        tmem_ld_wait();
-        if (ch + 2 >= n_chunks) {  // this warp's last TMEM read of the accumulator: hand it back
-          tcgen05_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(smem_u32(tmem_empty + acc));
-        }
+        // this warp's 32 x 32 chunk of the image: read row `lane`, then reuse the chunk as its transpose tile
+        float* stg_f = img + (size_t)(q * 32) * IP + c0;
         float v[32];
-        if (p.bias != nullptr) {  // warp-uniform; bias_s is zero padded, read 4 columns per shared-memory load
-          const float4* b4 = reinterpret_cast<const float4*>(bias_s + c0);
+        {
+          const float4* a4 = reinterpret_cast<const float4*>(stg_f + (size_t)lane * IP);
+          if (p.bias != nullptr) {  // warp-uniform; bias_s is zero padded, read 4 columns per shared-memory load
+            const float4* b4 = reinterpret_cast<const float4*>(bias_s + c0);
 #pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 b = b4[j >> 2];
-            v[j] = __uint_as_float(r[j]) + b.x;
-            v[j + 1] = __uint_as_float(r[j + 1]) + b.y;
-            v[j + 2] = __uint_as_float(r[j + 2]) + b.z;
-            v[j + 3] = __uint_as_float(r[j + 3]) + b.w;
+            for (int j = 0; j < 32; j += 4) {
+              const float4 a = a4[j >> 2], b = b4[j >> 2];
+              v[j] = a.x + b.x;
+              v[j + 1] = a.y + b.y;
+              v[j + 2] = a.z + b.z;
+              v[j + 3] = a.w + b.w;
+            }
+          } else {
+#pragma unroll
+            for (int j = 0; j < 32; j += 4) {
+              const float4 a = a4[j >> 2];
+              v[j] = a.x;
+              v[j + 1] = a.y;
+              v[j + 2] = a.z;
+              v[j + 3] = a.w;
+            }
           }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
         }
         if (p.x0) {
           // cross epilogue: x0 * (xW + b) + x ; x0 / x tiles come in through the transpose tile (coalesced)
@@ -357,12 +337,12 @@ dense_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                   if (n + 3 < p.N) t.w = g[3];
                 }
               }
-              *reinterpret_cast<float4*>(stg_f + rr * 36 + cv) = t;
+              *reinterpret_cast<float4*>(stg_f + rr * IP + cv) = t;
             }
             __syncwarp();
 #pragma unroll
             for (int j = 0; j < 32; j += 4) {
-              const float4 t = *reinterpret_cast<const float4*>(stg_f + lane * 36 + j);
+              const float4 t = *reinterpret_cast<const float4*>(stg_f + lane * IP + j);
               if (which == 0) {
                 v[j] = __fmul_rn(t.x, v[j]); v[j + 1] = __fmul_rn(t.y, v[j + 1]);
                 v[j + 2] = __fmul_rn(t.z, v[j + 2]); v[j + 3] = __fmul_rn(t.w, v[j + 3]);
@@ -426,16 +406,16 @@ dense_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
           __syncwarp();
 #pragma unroll
           for (int j = 0; j < 32; j += 4)
-            *reinterpret_cast<float4*>(stg_f + lane * 36 + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
+            *reinterpret_cast<float4*>(stg_f + lane * IP + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
           __syncwarp();
           if (vec_f32 && row0 + 32 <= p.M && n0 + c0 + 32 <= p.N) {
             // interior chunk (the common case): no per-element predicates
             const int rsub = lane >> 3, cv = (lane & 7) * 4;
             float* g = p.out_f32 + (row0 + rsub) * p.out_stride + (n0 + c0 + cv);
-            const float* src = stg_f + rsub * 36 + cv;
+            const float* src = stg_f + rsub * IP + cv;
 #pragma unroll
             for (int it = 0; it < 8; ++it)
-              *reinterpret_cast<float4*>(g + (long long)it * 4 * p.out_stride) = *reinterpret_cast<const float4*>(src + it * 4 * 36);
+              *reinterpret_cast<float4*>(g + (long long)it * 4 * p.out_stride) = *reinterpret_cast<const float4*>(src + it * 4 * IP);
           } else if (vec_f32) {
 #pragma unroll
             for (int it = 0; it < 8; ++it) {
@@ -443,7 +423,7 @@ dense_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
               const long long grow = row0 + rr;
               const int n = n0 + c0 + cv;
               if (grow < p.M && cv < ncols && n < p.N) {
-                const float4 t = *reinterpret_cast<const float4*>(stg_f + rr * 36 + cv);
+                const float4 t = *reinterpret_cast<const float4*>(stg_f + rr * IP + cv);
                 float* g = p.out_f32 + grow * p.out_stride + n;
                 if (n + 3 < p.N) *reinterpret_cast<float4*>(g) = t;
                 else {
@@ -459,22 +439,23 @@ dense_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
             const int n = n0 + c0 + lane;
             if (lane < ncols && n < p.N) {
               const int rmax = (int)min((long long)32, p.M - row0);
-              for (int rr = 0; rr < rmax; ++rr) p.out_f32[(row0 + rr) * p.out_stride + n] = stg_f[rr * 36 + lane];
+              for (int rr = 0; rr < rmax; ++rr) p.out_f32[(row0 + rr) * p.out_stride + n] = stg_f[rr * IP + lane];
             }
           }
         }
         if (p.out_split && n0 + c0 < p.out_Kp) {
-          // [hi | lo] bf16 rows of the next layer's A operand; tile rows are 80 B apart (bank spread)
+          // [hi | lo] bf16 rows of the next layer's A operand: hi in the first 64 B of each tile row, lo in the next
           __syncwarp();
-          uint8_t* th = stg;             // hi: 32 rows x 64 B (+16 pad)
-          uint8_t* tl = stg + 32 * 80;   // lo
+          uint8_t* th = reinterpret_cast<uint8_t*>(stg_f);
+          uint8_t* tl = th + 64;
+          const int pitch = IP * 4;
 #pragma unroll
           for (int j = 0; j < 32; j += 8) {
             __align__(16) __nv_bfloat16 h[8], l[8];
 #pragma unroll
             for (int e = 0; e < 8; ++e) split_bf16(v[j + e], h[e], l[e]);
-            *reinterpret_cast<uint4*>(th + lane * 80 + j * 2) = *reinterpret_cast<const uint4*>(h);
-            *reinterpret_cast<uint4*>(tl + lane * 80 + j * 2) = *reinterpret_cast<const uint4*>(l);
+            *reinterpret_cast<uint4*>(th + lane * pitch + j * 2) = *reinterpret_cast<const uint4*>(h);
+            *reinterpret_cast<uint4*>(tl + lane * pitch + j * 2) = *reinterpret_cast<const uint4*>(l);
           }
           __syncwarp();
 #pragma unroll
@@ -483,24 +464,13 @@ dense_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
             const long long grow = row0 + rr;
             if (grow < p.M && cv < ncols && n0 + c0 + cv < p.out_Kp) {
               __nv_bfloat16* oh = p.out_split + grow * (2ll * p.out_Kp) + n0 + c0 + cv;
-              *reinterpret_cast<uint4*>(oh) = *reinterpret_cast<const uint4*>(th + rr * 80 + cv * 2);
-              *reinterpret_cast<uint4*>(oh + p.out_Kp) = *reinterpret_cast<const uint4*>(tl + rr * 80 + cv * 2);
+              *reinterpret_cast<uint4*>(oh) = *reinterpret_cast<const uint4*>(th + rr * pitch + cv * 2);
+              *reinterpret_cast<uint4*>(oh + p.out_Kp) = *reinterpret_cast<const uint4*>(tl + rr * pitch + cv * 2);
             }
           }
         }
       }
-      if (++acc == 2) {
-        acc = 0;
-        acc_phase ^= 1;
-      }
     }
-  }
-
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(tmem_cols) : "memory");
   }
 }
 
@@ -631,13 +601,15 @@ static int dense_tc_launch(const void* a_split, int64_t M, int K, int Kp, const 
   p.resident_a = (score_mode && passes == 3 && Kp <= 2 * BLOCK_K && p.n_tiles_n >= 8) ? 1 : 0;
   const size_t a_res_bytes = p.resident_a ? (size_t)(Kp / BLOCK_K) * 2 * A_TILE_BYTES : 0;
   const size_t stage_bytes = (p.resident_a ? 0 : 2 * (size_t)A_TILE_BYTES) + 2 * (size_t)p.BN * BLOCK_K * 2;
-  const size_t epi_bytes = 256 * sizeof(long long) + 256 * sizeof(float) + (size_t)kEpiWarps * EPI_STAGE_BYTES;
-  int stages = (int)((224 * 1024 - 2048 - epi_bytes - a_res_bytes) / stage_bytes);
+  const size_t epi_bytes = 256 * sizeof(long long) + 256 * sizeof(float);
+  const size_t image_bytes = (size_t)BLOCK_M * image_pitch(p.BN) * sizeof(float);
+  const size_t fixed = 1024 + a_res_bytes + image_bytes + 16 * sizeof(uint64_t) + epi_bytes;
+  int stages = (int)((227 * 1024 - fixed) / stage_bytes);
   if (stages > 6) stages = 6;
   if (!p.resident_a && stages > Kp / BLOCK_K * 2) stages = Kp / BLOCK_K * 2 > 2 ? Kp / BLOCK_K * 2 : 2;
   MM_REQUIRE(stages >= 2, MM_ERR_UNSUPPORTED, "mm_dense_tc: tile does not fit two pipeline stages");
   p.stages = stages;
-  const size_t smem = 1024 + a_res_bytes + stages * stage_bytes + (2 * stages + 8) * sizeof(uint64_t) + epi_bytes;
+  const size_t smem = 1024 + a_res_bytes + stages * stage_bytes + image_bytes + (2 * stages + 2) * sizeof(uint64_t) + epi_bytes;
 
   CUtensorMap tmA, tmB;
   int rc = make_map(&tmA, a_split, (uint64_t)M, (uint64_t)2 * Kp, BLOCK_M);

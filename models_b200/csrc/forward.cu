@@ -5,7 +5,7 @@
 //   mm_mlp_forward   : MLPBlock (merlin/models/tf/blocks/mlp.py:97-139, Dense :275-280)
 //   mm_cross_forward : CrossBlock stack x_{l+1} = x0 * (x_l W_l + b_l) + x_l (blocks/cross.py:29-109, :188-202)
 //
-// Both split the fp32 operands to bf16 (hi, lo) pairs inside the workspace and run the tcgen05 kernels with the
+// Both split the fp32 operands to bf16 (hi, lo) pairs inside the workspace and run the wgmma kernels with the
 // 3-pass fp32-grade accumulation; the MLP uses the whole-tower kernel (mm_mlp_tc) when the widths allow it and
 // one mm_dense_tc launch per layer otherwise.
 #include <cuda_bf16.h>

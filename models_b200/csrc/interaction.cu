@@ -12,12 +12,6 @@ namespace mm {
 
 bool use_imma_v1();
 
-namespace itc {  // interaction_tc.cu: tcgen05 path, four samples per 128x128 tile (F <= 32, D == 64)
-template <int MODE, typename IdxT>
-int launch(const float* x, int64_t x_stride, const GatherParams& gp, const float* prefix, int64_t prefix_stride,
-           int P, int bottom_slot, int64_t B, int F, int D, float* out_f32, int64_t out_stride, void* out_split,
-           int out_Kp, int32_t* oob, cudaStream_t st, const char* who);
-}
 namespace imma2 {  // interaction_v2.cu: second-generation warp-per-sample kernel (packed ids, sharded tables)
 template <int MODE>
 int launch(const float* x, int64_t x_stride, const LookupParams& lk, const float* prefix, int64_t prefix_stride, int P,
@@ -333,9 +327,6 @@ int mm_dot_interaction(const float* x, int64_t B, int F, int D, int64_t x_stride
     if (rc2 != MM_ERR_UNSUPPORTED) return rc2;
   }
   if (!self_interaction) {
-    const int rc0 = mm::itc::launch<0, int32_t>(x, x_stride, p, prefix, prefix_stride, P, -1, B, F, D, out, out_stride,
-                                                out_split, out_Kp, nullptr, (cudaStream_t)stream, "mm_dot_interaction");
-    if (rc0 != MM_ERR_UNSUPPORTED) return rc0;
     const int rc = mm::imma::launch<0, int32_t>(x, x_stride, p, prefix, prefix_stride, P, -1, B, F, D, out, out_stride,
                                                 out_split, out_Kp, nullptr, (cudaStream_t)stream, "mm_dot_interaction");
     if (rc != MM_ERR_UNSUPPORTED) return rc;
@@ -401,12 +392,6 @@ int mm_dlrm_gather_interact(const mm_gather_table* tables_host, int n_tables, in
   }
   {
     const int bs = bottom ? bottom_slot : -1;
-    const int rc0 = idx_dtype == MM_I32
-                        ? mm::itc::launch<1, int32_t>(nullptr, 0, p, bottom, bottom_stride, P, bs, B, F, D, out, out_stride,
-                                                      out_split, out_Kp, oob_count, st, "mm_dlrm_gather_interact")
-                        : mm::itc::launch<1, int64_t>(nullptr, 0, p, bottom, bottom_stride, P, bs, B, F, D, out, out_stride,
-                                                      out_split, out_Kp, oob_count, st, "mm_dlrm_gather_interact");
-    if (rc0 != MM_ERR_UNSUPPORTED) return rc0;
     const int rc = idx_dtype == MM_I32
                        ? mm::imma::launch<1, int32_t>(nullptr, 0, p, bottom, bottom_stride, P, bs, B, F, D, out, out_stride,
                                                       out_split, out_Kp, oob_count, st, "mm_dlrm_gather_interact")

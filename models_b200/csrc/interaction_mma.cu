@@ -1,18 +1,17 @@
 // DLRM pairwise interaction on tensor cores, one warp per sample — FIRST-GENERATION kernel, kept for A/B measurements
 // (MM_IMMA_V1=1) and as the fallback of the legacy entry points; the product path is interaction_v2.cu.
 //
-// The per-sample Gram matrix X X^T (X = F x D, F <= 32) is far too small for tcgen05 (M >= 64 per
+// The per-sample Gram matrix X X^T (X = F x D, F <= 32) is far too small for wgmma (M >= 64 per
 // instruction would waste > 4x on block-diagonal padding), so it runs on the warp-level
 // mma.sync.m16n8k16 bf16 path with the same 3-pass split as the dense layers (hi*lo + lo*hi + hi*hi,
-// fp32 accumulate).  It is NOT HBM-bound: ncu shows 1 155 warp instructions per sample at 62 % issue
-// utilisation and DRAM at 35 % of peak (profiles/r01_notes.md §h) — the v2 kernel cuts the instruction count in half.
+// fp32 accumulate).  It is NOT HBM-bound but instruction-issue bound — the v2 kernel cuts the instruction count in half.
 //
 // Data movement: rows go from the embedding tables — or the stacked (B,F,D) tensor — straight
 // into a padded shared-memory tile with 16-byte cp.async (LDGSTS: no register staging, zero-fill
 // for out-of-range ids), one commit group per sample; each warp keeps NBUF-1 samples in flight
 // while it computes one.  (A first version issued one cp.async.bulk per row: UBLKCP takes uniform
 // registers, so the compiler serialised the 27 per-lane copies through an ELECT/R2UR loop that
-// cost ~20 % of the issue slots — see profiles/r01_notes.md.)
+// cost a large share of the issue slots.)
 // Because B = X^T, the B fragments of n-tile nt ARE registers of the A fragment of m-tile nt/2, so X
 // is read from shared memory once per k-step.  The output row [prefix | upper triangle] is assembled
 // in shared memory and written coalesced, either as fp32 or directly as the split-bf16 operand

@@ -1,7 +1,6 @@
 // DLRM lookup + pairwise interaction, one warp per sample (second generation of interaction_mma.cu).
 //
-// What changed against the first kernel (profiles/r01_notes.md §h: 1 155 warp instructions per sample,
-// 436 of them in the row-copy loop, issue-bound at 12 warps per SM):
+// What changed against the first kernel (issue-bound, a large share of its instructions in the row-copy loop):
 //   * copy loop: 8 lanes move one 128-byte half row per LDGSTS, 4 rows per instruction.  Staged row r is
 //     owned by lane r (tables arrive sorted by slot, so row == slot), a row's source pointer travels
 //     with two shuffles, and because row = 4*i + lane/8 the XOR swizzle of a lane's destination does
@@ -107,9 +106,9 @@ struct RawIdx {
 
 // Negative result kept as a note (the code is gone): issuing the Gram matrix as m16n8k8 MMAs.  With k16 every bf16x2
 // register must sit both in an A quad {X[g],X[g+8]} x {k-lo,k-hi} and in a B pair {k-lo,k-hi} of one row — two
-// incompatible adjacencies that cost ~180 register moves per sample (ncu, r2a).  k8 operands are an A pair and a single
-// B register: no moves, but twice as many MMAs, and HMMA.1688 occupies the legacy tensor pipe as long as HMMA.16816
-// (8 cycles per SMSP): 0.128 ms instead of 0.103 ms (profiles/r02_notes.md §a).
+// incompatible adjacencies that cost many register moves per sample.  k8 operands are an A pair and a single
+// B register: no moves, but twice as many MMAs, and HMMA.1688 occupies the legacy tensor pipe as long as HMMA.16816,
+// so it was slower.
 //
 // PS ("pre-split", D = 64): the staged rows are split-bf16 rows [hi(0..D) | lo(0..D)] — the operand format of every
 // tensor-core layer of this library (mm_split_rows) — read from a second copy of the tables in HBM; the bottom vector
@@ -122,9 +121,8 @@ struct RawIdx {
 // the A quads still had to be assembled with moves and nothing overlapped the load -> HMMA latency: 0.116 ms vs 0.104.)
 // NBUF sample buffers per warp: NBUF-1 samples in flight behind the one being computed.  The product uses 2 with
 // 16 warps, for local tables and for rows that come over NVLink alike.  NBUF = 3 / 4 (10 / 7 warps, ids through a
-// shared-memory ring) exist for experiments (MM_IMMA_NBUF): measured on 2 x B200 they are never faster — what looked
-// like remote latency was hot rows of tiny sharded tables serialising on single cache lines of the owner
-// (profiles/r02_notes.md §b); with those tables replicated, 16 warps x 1 sample in flight reach 420-580 GB/s.
+// shared-memory ring) exist for experiments (MM_IMMA_NBUF): remote latency is dominated by hot rows of tiny
+// sharded tables serialising on single cache lines of the owner, which replicating those tables removes.
 template <int MODE, int KD /* embedding dim: 16, 32, 64, 128 */, int NWARPS /* launch bound */, bool PS, int NBUF>
 __global__ void __launch_bounds__(32 * NWARPS, 1)
 interact_v2_kernel(const __grid_constant__ LookupParams lk, const Params p) {

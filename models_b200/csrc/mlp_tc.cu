@@ -1,8 +1,8 @@
-// Whole-tower MLP for sm_100a: the first Dense layer is a TMA-fed tcgen05 GEMM (as dense_tc.cu); every
-// following layer whose width is <= 128 runs ON CHIP — its activations never leave tensor memory:
+// Whole-tower MLP for sm_90a: the first Dense layer is a TMA-fed wgmma GEMM (as dense_tc.cu); every
+// following layer whose width is <= 128 runs ON CHIP — its activations never leave the registers:
 //
-//   D1 (TMEM, fp32)  --epilogue warps: bias + act, split-bf16-->  A2 (TMEM, packed bf16 hi | lo)
-//   A2 x W2 (weights resident in shared memory, SWIZZLE_128B K-major)  --tcgen05.mma, A from TMEM-->  D2
+//   D1 (registers, fp32)  --bias + act, split-bf16-->  A2 (registers: the wgmma A fragment, packed bf16 hi | lo)
+//   A2 x W2 (weights resident in shared memory, SWIZZLE_128B K-major)  --wgmma, A from registers-->  D2
 //   D2 --bias + act, split--> A3 --x W3--> D3 ... --> last layer: fp32 rows to HBM and/or the fused
 //   Dense(N -> 1) output head (BinaryOutput: sigmoid(x.w + b)).
 //
@@ -10,25 +10,18 @@
 // SequentialBlock of Keras Dense layers, `_Dense.call` :275-280) + BinaryOutput's Dense(1)
 // (outputs/classification.py:114) for the README towers (bottom 13 -> 128 -> 64, top 415 -> 128 -> 64 -> 32 -> 1):
 // one launch instead of one per layer, and the (B, 128) / (B, 64) intermediate activations (33 + 17 MB of
-// split-bf16 rows written and re-read per step at B = 65 536) stay in TMEM.
+// split-bf16 rows written and re-read per step at B = 65 536) never reach HBM.
 //
 // fp32 parity: all operands are split-bf16 pairs (x = hi + lo), every layer accumulates
-// hi*lo + lo*hi + hi*hi into one fp32 TMEM accumulator (same arithmetic as mm_dense_tc, passes = 3).
+// hi*lo + lo*hi + hi*hi into one fp32 accumulator (same arithmetic as mm_dense_tc, passes = 3).
 //
-// CTA = 12 warps, persistent over 128-row tiles: warp 0 TMA producer (layer-1 operands; the chain
-// weights once), warp 1 layer-1 MMA issuer, warps 2-3 chain MMA issuers, warps 4-11 epilogue.
-// The chain of one tile is a serial ping-pong (epilogue -> MMA -> epilogue ...), so two tiles are kept in
-// flight whenever tensor memory allows it:
-//   dual mode (every chain width <= 64): D1 0..127 (single buffer), two chain sets s = 0, 1 with operand
-//     A_s at 128 + 192 s (hi pairs +0, lo pairs +64) and accumulator D_s at A_s + 128; epilogue group s
-//     (4 warps, one per TMEM lane quarter) and chain issuer s own the tiles with local index = s mod 2;
-//   single mode (a chain width > 64): D1[0] 0..127, D1[1] 128..255, A 256..383, D 384..511, all eight
-//     epilogue warps on every tile (two per lane quarter, interleaved over 32-column chunks).
+// CTA = 9 warps, persistent over 128-row tiles: warps 0-7 are two consumer warpgroups (64 rows of the
+// tile each: layer-1 MMAs, every epilogue and every chain MMA of those rows), warp 8 is the TMA producer
+// (layer-1 operands; the chain weights once).  The accumulator fragment of a layer maps register for
+// register onto the A fragment of the next layer's MMA (columns 16 s .. 16 s + 15 of D are k-step s of A).
 #include <cuda.h>
 #include <cuda_bf16.h>
 
-#include <cstdio>
-#include <cstdlib>
 #include <cstring>
 
 #include "mm_common.cuh"
@@ -41,25 +34,23 @@ using namespace mm::tc;
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 64;
-constexpr int UMMA_K = 16;
-constexpr int kEpiWarps = 8;
-constexpr int kThreads = 32 * (4 + kEpiWarps);
+constexpr int MMA_K = 16;
+constexpr int kConsumerWarps = 8;
+constexpr int kThreads = 32 * (kConsumerWarps + 1);
 constexpr int kMaxChain = 3;
 constexpr uint32_t A_TILE_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KB
-constexpr uint32_t EPI_STAGE_BYTES = 32 * 36 * 4;         // per epilogue warp: 32 x 32 fp32 transpose tile (+4 pad)
-constexpr uint32_t COL_A_LO = 64;  // lo pairs sit 64 columns after the hi pairs inside a chain operand region
 
 struct ChainLayer {
   int N, Np;        // true / padded (multiple of 16) width of this layer
   int Kp;           // K padded to 64 (row pitch of the split weights = 2 * Kp elements)
-  int ksteps;       // UMMA k-steps actually issued = padded width of the previous layer / 16
+  int ksteps;       // MMA k-steps actually issued = padded width of the previous layer / 16
   int act;
   uint32_t w_off;   // byte offset of this layer's resident weight tiles inside the weight arena
 };
 
 struct Params {
   long long M;
-  int K1p, N1, N1p, act1, stages, n_chain, dual;
+  int K1p, N1, N1p, act1, stages, n_chain;
   ChainLayer c[kMaxChain];
   const float* bias[kMaxChain + 1];  // layer 1, chain layers
   uint32_t w_bytes;                  // total resident weight bytes
@@ -70,29 +61,7 @@ struct Params {
   float head_b;
   int head_act;
   float* head_out;
-  long long* trace;  // MM_MLP_TRACE=1: CTA 0 logs (tag, clock64) pairs here (debug only)
 };
-
-__device__ __forceinline__ void umma_bf16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n .reg .pred p;\n setp.ne.b32 p, %4, 0;\n tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x32b_x8(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(r[0]),
-               "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
 __device__ __forceinline__ void split_pair(float x, float y, uint32_t& hi, uint32_t& lo) {
   __nv_bfloat162 h = __floats2bfloat162_rn(x, y);  // .x (low half) = x: K element 2c in the low 16 bits
@@ -100,16 +69,6 @@ __device__ __forceinline__ void split_pair(float x, float y, uint32_t& hi, uint3
   const float xh = __uint_as_float(hi << 16), yh = __uint_as_float(hi & 0xffff0000u);
   __nv_bfloat162 l = __floats2bfloat162_rn(x - xh, y - yh);
   lo = *reinterpret_cast<uint32_t*>(&l);
-}
-
-__device__ __forceinline__ void trace_event(const Params& p, int tag) {
-  if (p.trace != nullptr && blockIdx.x == 0 && (threadIdx.x & 31) == 0) {
-    const unsigned long long i = atomicAdd(reinterpret_cast<unsigned long long*>(p.trace), 1ull);
-    if (i < 2000) {
-      p.trace[1 + 2 * i] = tag;
-      p.trace[2 + 2 * i] = clock64();
-    }
-  }
 }
 
 __global__ void __launch_bounds__(kThreads, 1)
@@ -125,42 +84,24 @@ mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
   uint8_t* wres = smem + (size_t)p.stages * STAGE_BYTES;  // resident chain weights (1024-B aligned tiles)
   uint64_t* bars = reinterpret_cast<uint64_t*>(wres + p.w_bytes);
   uint64_t* full_bar = bars;                        // [stages]
-  uint64_t* empty_bar = bars + p.stages;            // [stages]
-  uint64_t* d1_full = bars + 2 * p.stages;          // [2] tcgen05.commit of layer 1
-  uint64_t* d1_empty = bars + 2 * p.stages + 2;     // [2] count kEpiWarps
-  uint64_t* a_full = bars + 2 * p.stages + 4;       // [2] chain operand of set s written (count = warps of a group)
-  uint64_t* d_full = bars + 2 * p.stages + 6;       // [2] chain accumulator of set s complete (tcgen05.commit)
-  uint64_t* w_full = bars + 2 * p.stages + 8;       // resident weights landed
-  uint32_t* tmem_base_slot = reinterpret_cast<uint32_t*>(bars + 2 * p.stages + 9);
-  float* bias_s = reinterpret_cast<float*>(bars + 2 * p.stages + 10);  // [kMaxChain + 1][128], zero padded
-  float* head_s = bias_s + (kMaxChain + 1) * 128;                     // [32], zero padded
-  uint8_t* stage_tiles = reinterpret_cast<uint8_t*>(head_s + 32);     // kEpiWarps x EPI_STAGE_BYTES
+  uint64_t* empty_bar = bars + p.stages;            // [stages] one arrive per consumer warp
+  uint64_t* w_full = bars + 2 * p.stages;           // resident weights landed
+  float* bias_s = reinterpret_cast<float*>(bars + 2 * p.stages + 2);  // [kMaxChain + 1][128], zero padded
+  float* head_s = bias_s + (kMaxChain + 1) * 128;                     // [128], zero padded
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long long tiles = (p.M + BLOCK_M - 1) / BLOCK_M;
   const int KB = p.K1p / BLOCK_K;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kConsumerWarps && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmW1) : "memory");
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(smem_u32(full_bar + s), 1);
-      mbar_init(smem_u32(empty_bar + s), 1);
-    }
-    const uint32_t group_warps = p.dual ? kEpiWarps / 2 : kEpiWarps;
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(smem_u32(d1_full + a), 1);
-      mbar_init(smem_u32(d1_empty + a), group_warps);
-      mbar_init(smem_u32(a_full + a), group_warps);
-      mbar_init(smem_u32(d_full + a), 1);
+      mbar_init(smem_u32(empty_bar + s), kConsumerWarps);
     }
     mbar_init(smem_u32(w_full), 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_base_slot)), "r"(512u)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
   // biases / head weights are the same for every tile (each layer is a single n-tile): stage them once
   for (int i = threadIdx.x; i < (kMaxChain + 1) * 128; i += kThreads) {
@@ -168,16 +109,13 @@ mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
     const int N = l == 0 ? p.N1 : (l <= p.n_chain ? p.c[l - 1].N : 0);
     bias_s[i] = (p.bias[l] != nullptr && n < N) ? p.bias[l][n] : 0.0f;
   }
-  if (threadIdx.x < 32) {
+  if (threadIdx.x < 128) {
     const int Nl = p.n_chain ? p.c[p.n_chain - 1].N : p.N1;
     head_s[threadIdx.x] = (p.head_w != nullptr && (int)threadIdx.x < Nl) ? p.head_w[threadIdx.x] : 0.0f;
   }
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_base_slot;
 
-  if (warp == 0) {
+  if (warp == kConsumerWarps) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       if (p.n_chain > 0) {  // chain weights: loaded once, resident for the whole kernel
@@ -212,241 +150,160 @@ mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== layer-1 MMA issuer =====================
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc(BLOCK_M, p.N1p);
-      int stage = 0;
-      uint32_t phase = 0;
-      long long it = 0;  // local tile index; barrier pair index = it & 1, use count = it >> 1
-      for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++it) {
-        const int acc = (int)(it & 1);
-        if (p.dual) {  // one D1 buffer: wait until the previous tile's first epilogue has drained it
-          if (it > 0) mbar_wait(smem_u32(d1_empty + ((it - 1) & 1)), (uint32_t)(((it - 1) >> 1) & 1));
-        } else {       // two D1 buffers: wait for the drain of tile it - 2
-          mbar_wait(smem_u32(d1_empty + acc), (uint32_t)(((it >> 1) & 1) ^ 1));
-        }
-        tcgen05_fence_after();
-        trace_event(p, 100);
-        const uint32_t d_tmem = tmem_base + (p.dual ? 0u : (uint32_t)(acc * 128));
-        uint32_t accumulate = 0;
-        for (int kb = 0; kb < KB; ++kb) {
-          // hi slot: the dominant hi*hi product starts as soon as it lands
-          const int s_hi = stage;
-          mbar_wait(smem_u32(full_bar + s_hi), phase);
-          tcgen05_fence_after();
-          const uint32_t a_hi = smem_u32(smem + (size_t)s_hi * STAGE_BYTES), b_hi = a_hi + A_TILE_BYTES;
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; ++k) {
-            umma_bf16(d_tmem, make_desc_sw128(a_hi + k * 32), make_desc_sw128(b_hi + k * 32), idesc, accumulate);
-            accumulate = 1;
-          }
-          if (++stage == p.stages) {
-            stage = 0;
-            phase ^= 1;
-          }
-          // lo slot: the two cross terms
-          const int s_lo = stage;
-          mbar_wait(smem_u32(full_bar + s_lo), phase);
-          tcgen05_fence_after();
-          const uint32_t a_lo = smem_u32(smem + (size_t)s_lo * STAGE_BYTES), b_lo = a_lo + A_TILE_BYTES;
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-            umma_bf16(d_tmem, make_desc_sw128(a_hi + k * 32), make_desc_sw128(b_lo + k * 32), idesc, 1);
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-            umma_bf16(d_tmem, make_desc_sw128(a_lo + k * 32), make_desc_sw128(b_hi + k * 32), idesc, 1);
-          tcgen05_commit(smem_u32(empty_bar + s_hi));  // both slots are free once these MMAs retire
-          tcgen05_commit(smem_u32(empty_bar + s_lo));
-          if (++stage == p.stages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        tcgen05_commit(smem_u32(d1_full + acc));
-        trace_event(p, 200);
-      }
-    }
-  } else if (warp == 2 || warp == 3) {
-    // ===================== chain MMA issuer (A operand in TMEM, weights resident in smem) =====================
-    const int set = warp - 2;  // dual mode: issuer of chain set `set`; single mode: warp 2 serves every tile
-    if (lane == 0 && p.n_chain > 0 && (p.dual || set == 0)) {
-      mbar_wait(smem_u32(w_full), 0);
-      uint32_t a_phase = 0;
-      const uint32_t col_a = p.dual ? 128u + 192u * (uint32_t)set : 256u;
-      const uint32_t a_hi = tmem_base + col_a, a_lo = a_hi + COL_A_LO, d_tmem = a_hi + 128;
-      long long it = 0;
-      for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++it) {
-        if (p.dual && (it & 1) != set) continue;
-        for (int c = 0; c < p.n_chain; ++c) {
-          const ChainLayer& L = p.c[c];
-          mbar_wait(smem_u32(a_full + set), a_phase);
-          a_phase ^= 1;
-          tcgen05_fence_after();
-          trace_event(p, 300 + c);
-          const uint32_t idesc = make_idesc(BLOCK_M, L.Np);
-          const uint32_t tile_b = (uint32_t)L.Np * BLOCK_K * 2;
-          const uint32_t w_hi = smem_u32(wres + L.w_off), w_lo = w_hi + (uint32_t)(L.Kp / BLOCK_K) * tile_b;
-          uint32_t accumulate = 0;
-          // a k-step covers 16 K elements = 8 packed TMEM columns of A and 32 bytes of a weight row
-          for (int ks = 0; ks < L.ksteps; ++ks) {
-            umma_bf16_ts(d_tmem, a_hi + ks * 8, make_desc_sw128(w_lo + (ks >> 2) * tile_b + (ks & 3) * 32), idesc, accumulate);
-            accumulate = 1;
-          }
-          for (int ks = 0; ks < L.ksteps; ++ks)
-            umma_bf16_ts(d_tmem, a_lo + ks * 8, make_desc_sw128(w_hi + (ks >> 2) * tile_b + (ks & 3) * 32), idesc, 1);
-          for (int ks = 0; ks < L.ksteps; ++ks)
-            umma_bf16_ts(d_tmem, a_hi + ks * 8, make_desc_sw128(w_hi + (ks >> 2) * tile_b + (ks & 3) * 32), idesc, 1);
-          tcgen05_commit(smem_u32(d_full + set));
-        }
-      }
-    }
   } else {
-    // ===================== epilogue warps (3..10) =====================
-    const int e = warp - 4;
-    const int q = warp & 3;    // TMEM lane quarter this warp may access
-    const int group = e >> 2;  // dual: owns the tiles with local index = group mod 2; single: chunk interleave
-    const int half = p.dual ? 0 : group, chunk_step = p.dual ? 1 : 2;
-    const int set = p.dual ? group : 0;
-    const uint32_t col_a = p.dual ? 128u + 192u * (uint32_t)set : 256u;
-    float* stg_f = reinterpret_cast<float*>(stage_tiles + (size_t)e * EPI_STAGE_BYTES);
-    const bool vec_f32 = p.out_operand ||  // (the host checks that a fp32 output beside an operand output is vector-aligned)
-                         (p.out_f32 && ((p.out_stride & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.out_f32) & 15) == 0));
-    const uint32_t lane_base = tmem_base + ((uint32_t)(q * 32) << 16);
-    uint32_t d_phase = 0;
-    long long it = 0;
+    // ===================== consumer warpgroups: 64 rows each, every layer =====================
+    const int wg = warp >> 2;
+    const int c2 = 2 * (lane & 3);  // fragment column offset inside an 8-column block
+    const int frow = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // tile row of fragment row 0 (row 1 is 8 further)
+    const uint32_t a_off = (uint32_t)wg * (A_TILE_BYTES / 2);
+    int stage = 0;
+    uint32_t phase = 0;
+    bool weights_ready = p.n_chain == 0;
+    for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+      float acc[64];
+#pragma unroll
+      for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
+      for (int kb = 0; kb < KB; ++kb) {
+        // hi slot: the dominant hi*hi product starts as soon as it lands
+        const int s_hi = stage;
+        mbar_wait(smem_u32(full_bar + s_hi), phase);
+        const uint32_t a_hi = smem_u32(smem + (size_t)s_hi * STAGE_BYTES), b_hi = a_hi + A_TILE_BYTES;
+        wgmma_fence_acc(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BLOCK_K / MMA_K; ++k)
+          wgmma_ss(p.N1p, acc, make_desc_sw128(a_hi + a_off + k * 32), make_desc_sw128(b_hi + k * 32));
+        wgmma_commit();
+        if (++stage == p.stages) {
+          stage = 0;
+          phase ^= 1;
+        }
+        // lo slot: the two cross terms
+        const int s_lo = stage;
+        mbar_wait(smem_u32(full_bar + s_lo), phase);
+        const uint32_t a_lo = smem_u32(smem + (size_t)s_lo * STAGE_BYTES), b_lo = a_lo + A_TILE_BYTES;
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BLOCK_K / MMA_K; ++k)
+          wgmma_ss(p.N1p, acc, make_desc_sw128(a_hi + a_off + k * 32), make_desc_sw128(b_lo + k * 32));
+#pragma unroll
+        for (int k = 0; k < BLOCK_K / MMA_K; ++k)
+          wgmma_ss(p.N1p, acc, make_desc_sw128(a_lo + a_off + k * 32), make_desc_sw128(b_hi + k * 32));
+        wgmma_commit();
+        wgmma_wait_all();
+        wgmma_fence_acc(acc);
+        __syncwarp();
+        if (lane == 0) {  // both slots are free once this warp's MMAs have completed
+          mbar_arrive(smem_u32(empty_bar + s_hi));
+          mbar_arrive(smem_u32(empty_bar + s_lo));
+        }
+        if (++stage == p.stages) {
+          stage = 0;
+          phase ^= 1;
+        }
+      }
 
-    for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x, ++it) {
-      if (p.dual && (it & 1) != group) continue;
-      const int acc = (int)(it & 1);
-      const uint32_t acc_phase = (uint32_t)((it >> 1) & 1);
-      const long long row0 = tile * BLOCK_M + q * 32;
       for (int layer = 0; layer <= p.n_chain; ++layer) {
         const bool last = layer == p.n_chain;
         const int N = layer == 0 ? p.N1 : p.c[layer - 1].N;
         const int Np = layer == 0 ? p.N1p : p.c[layer - 1].Np;
         const int act = layer == 0 ? p.act1 : p.c[layer - 1].act;
         const float* bs = bias_s + layer * 128;
-        uint32_t src;
-        if (layer == 0) {
-          mbar_wait(smem_u32(d1_full + acc), acc_phase);
-          src = lane_base + (p.dual ? 0u : (uint32_t)(acc * 128));
-        } else {
-          mbar_wait(smem_u32(d_full + set), d_phase);
-          d_phase ^= 1;
-          src = lane_base + col_a + 128;
+        // bias + activation on the fragment; padding columns (>= N) become exact zeros
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          if (8 * j < Np) {
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              const int col = 8 * j + c2 + (e & 1);
+              float v = acc[4 * j + e] + bs[col];
+              if (act == MM_ACT_RELU) v = fmaxf(v, 0.0f);
+              else if (act != MM_ACT_LINEAR && col < N) v = apply_act_slow(v, act);
+              acc[4 * j + e] = col < N ? v : 0.0f;
+            }
+          }
         }
-        tcgen05_fence_after();
-        if ((e & 3) == 0) trace_event(p, (e ? 450 : 400) + layer);
-        const int n_chunks = (Np + 31) >> 5;
-        for (int ch = half; ch < n_chunks; ch += chunk_step) {
-          const int c0 = ch << 5;
-          const int ncols = min(32, Np - c0);  // Np is a multiple of 16
-          uint32_t r[32];
-          if (ncols == 32) tmem_ld_32x32b_x32(src + c0, r);
-          else tmem_ld_32x32b_x16(src + c0, r);
-          tmem_ld_wait();
-          float v[32];
+        if (!last) {
+          // next layer's A fragment: k-step s = columns 16 s .. 16 s + 15 = n8 blocks 2 s, 2 s + 1
+          uint32_t ahi[32], alo[32];
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]) + bs[c0 + j];
-          if (act == MM_ACT_RELU) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.0f);
-          } else if (act != MM_ACT_LINEAR) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (c0 + j < N) v[j] = apply_act_slow(v[j], act);
+          for (int i = 0; i < 32; ++i) split_pair(acc[2 * i], acc[2 * i + 1], ahi[i], alo[i]);
+          const ChainLayer& L = p.c[layer];
+          if (!weights_ready) {
+            mbar_wait(smem_u32(w_full), 0);
+            weights_ready = true;
           }
-          if (c0 + 32 > N) {  // padding columns are exact zeros (x16 loads leave r[16..31] undefined)
+          const uint32_t tile_b = (uint32_t)L.Np * BLOCK_K * 2;
+          const uint32_t w_hi = smem_u32(wres + L.w_off), w_lo = w_hi + (uint32_t)(L.Kp / BLOCK_K) * tile_b;
 #pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (c0 + j >= N) v[j] = 0.0f;
+          for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
+          wgmma_fence_acc(acc);
+          wgmma_fence();
+          // a k-step covers 16 K elements = 32 bytes of a weight row
+#pragma unroll
+          for (int ks = 0; ks < 8; ++ks) {
+            if (ks < L.ksteps) {
+              const uint32_t f[4] = {ahi[4 * ks], ahi[4 * ks + 1], ahi[4 * ks + 2], ahi[4 * ks + 3]};
+              wgmma_rs(L.Np, acc, f, make_desc_sw128(w_lo + (ks >> 2) * tile_b + (ks & 3) * 32));
+            }
           }
-          if (!last) {
-            // next layer's A operand: packed bf16 pairs, hi at col_a + c0/2, lo 64 columns further
-            uint32_t h[16], l[16];
 #pragma unroll
-            for (int j = 0; j < 16; ++j) split_pair(v[2 * j], v[2 * j + 1], h[j], l[j]);
-            const uint32_t dst = lane_base + col_a + (uint32_t)(c0 >> 1);
-            if (ncols == 32) {
-              tmem_st_32x32b_x16(dst, h);
-              tmem_st_32x32b_x16(dst + COL_A_LO, l);
-            } else {
-              tmem_st_32x32b_x8(dst, h);
-              tmem_st_32x32b_x8(dst + COL_A_LO, l);
+          for (int ks = 0; ks < 8; ++ks) {
+            if (ks < L.ksteps) {
+              const uint32_t f[4] = {alo[4 * ks], alo[4 * ks + 1], alo[4 * ks + 2], alo[4 * ks + 3]};
+              wgmma_rs(L.Np, acc, f, make_desc_sw128(w_hi + (ks >> 2) * tile_b + (ks & 3) * 32));
             }
-          } else {
-            if (p.head_w) {  // fused Dense(N -> 1): Np <= 32, this chunk is the whole row
-              float hsum = p.head_b;
+          }
 #pragma unroll
-              for (int j = 0; j < 32; ++j) hsum = fmaf(v[j], head_s[j], hsum);
-              if (row0 + lane < p.M) p.head_out[row0 + lane] = apply_act(hsum, p.head_act);
+          for (int ks = 0; ks < 8; ++ks) {
+            if (ks < L.ksteps) {
+              const uint32_t f[4] = {ahi[4 * ks], ahi[4 * ks + 1], ahi[4 * ks + 2], ahi[4 * ks + 3]};
+              wgmma_rs(L.Np, acc, f, make_desc_sw128(w_hi + (ks >> 2) * tile_b + (ks & 3) * 32));
             }
-            if (p.out_f32 || p.out_operand) {
-              __syncwarp();
+          }
+          wgmma_commit();
+          wgmma_wait_all();
+          wgmma_fence_acc(acc);
+        } else {
 #pragma unroll
-              for (int j = 0; j < 32; j += 4)
-                *reinterpret_cast<float4*>(stg_f + lane * 36 + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-              __syncwarp();
-              if (vec_f32) {
+          for (int h = 0; h < 2; ++h) {
+            const long long row = tile * BLOCK_M + frow + 8 * h;
+            if (p.head_w) {  // fused Dense(N -> 1): Np <= 32; the four lanes of a quad hold a row's columns
+              float hsum = 0.0f;
 #pragma unroll
-                for (int it = 0; it < 8; ++it) {
-                  const int rr = it * 4 + (lane >> 3), cv = (lane & 7) * 4;
-                  const long long grow = row0 + rr;
-                  const int n = c0 + cv;
-                  if (grow < p.M && cv < ncols && n < N) {
-                    const float4 t = *reinterpret_cast<const float4*>(stg_f + rr * 36 + cv);
-                    if (p.out_operand) {  // N % 4 == 0: the chunk is whole
-                      uint32_t h0, l0, h1, l1;
-                      split_pair(t.x, t.y, h0, l0);
-                      split_pair(t.z, t.w, h1, l1);
-                      uint8_t* rowp = p.out_operand + grow * ((long long)N * 4);
-                      *reinterpret_cast<uint2*>(rowp + n * 2) = make_uint2(h0, h1);
-                      *reinterpret_cast<uint2*>(rowp + N * 2 + n * 2) = make_uint2(l0, l1);
-                    }
-                    if (p.out_f32) {
-                      float* g = p.out_f32 + grow * p.out_stride + n;
-                      if (n + 3 < N) *reinterpret_cast<float4*>(g) = t;
-                      else {
-                        g[0] = t.x;
-                        if (n + 1 < N) g[1] = t.y;
-                        if (n + 2 < N) g[2] = t.z;
-                      }
-                    }
+              for (int j = 0; j < 4; ++j) {
+                hsum = fmaf(acc[4 * j + 2 * h], head_s[8 * j + c2], hsum);
+                hsum = fmaf(acc[4 * j + 2 * h + 1], head_s[8 * j + c2 + 1], hsum);
+              }
+              hsum += __shfl_xor_sync(0xffffffffu, hsum, 1);
+              hsum += __shfl_xor_sync(0xffffffffu, hsum, 2);
+              if ((lane & 3) == 0 && row < p.M) p.head_out[row] = apply_act(hsum + p.head_b, p.head_act);
+            }
+            if (row < p.M && (p.out_f32 || p.out_operand)) {
+#pragma unroll
+              for (int j = 0; j < 16; ++j) {
+                const int n = 8 * j + c2;
+                if (8 * j < Np && n < N) {
+                  const float x = acc[4 * j + 2 * h], y = acc[4 * j + 2 * h + 1];
+                  if (p.out_operand) {  // N % 4 == 0: the pair (n, n + 1) is whole
+                    uint32_t hi, lo;
+                    split_pair(x, y, hi, lo);
+                    uint8_t* rowp = p.out_operand + row * ((long long)N * 4);
+                    *reinterpret_cast<uint32_t*>(rowp + n * 2) = hi;
+                    *reinterpret_cast<uint32_t*>(rowp + N * 2 + n * 2) = lo;
                   }
-                }
-              } else {
-                const int n = c0 + lane;
-                if (lane < ncols && n < N) {
-                  const int rmax = (int)min((long long)32, p.M - row0);
-                  for (int rr = 0; rr < rmax; ++rr) p.out_f32[(row0 + rr) * p.out_stride + n] = stg_f[rr * 36 + lane];
+                  if (p.out_f32) {
+                    float* g = p.out_f32 + row * p.out_stride + n;
+                    g[0] = x;
+                    if (n + 1 < N) g[1] = y;
+                  }
                 }
               }
             }
           }
         }
-        // all of this warp's TMEM reads of the layer's accumulator are done
-        tcgen05_fence_before();
-        if ((e & 3) == 0) trace_event(p, (e ? 550 : 500) + layer);
-        if (layer == 0) {
-          __syncwarp();
-          if (lane == 0) mbar_arrive(smem_u32(d1_empty + acc));
-        }
-        if (!last) {
-          tmem_st_wait();
-          tcgen05_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(smem_u32(a_full + set));
-        }
       }
     }
-  }
-
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
   }
 }
 
@@ -454,7 +311,7 @@ mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
 }  // namespace mm
 
 // Fills the shape-dependent part of Params and the shared-memory size; false when the tower does not fit.
-static bool plan_tower(int K, int n_layers, const int* widths, bool fp32_rows, mm::mlp::Params& p, size_t& smem) {
+static bool plan_tower(int K, int n_layers, const int* widths, mm::mlp::Params& p, size_t& smem) {
   using namespace mm::mlp;
   memset(&p, 0, sizeof(p));
   p.K1p = mm_tc_padded_k(K);
@@ -468,32 +325,24 @@ static bool plan_tower(int K, int n_layers, const int* widths, bool fp32_rows, m
     L.N = widths[c + 1];
     L.Np = mm_tc_padded_n(L.N);
     L.Kp = mm_tc_padded_k(prev_n);
-    L.ksteps = prev_np / UMMA_K;
+    L.ksteps = prev_np / MMA_K;
     L.w_off = w_off;
     w_off += (uint32_t)(2 * (L.Kp / BLOCK_K)) * (uint32_t)L.Np * BLOCK_K * 2;
     prev_np = L.Np;
     prev_n = L.N;
   }
   p.w_bytes = w_off;
-  // Two chain sets (two tiles in flight) cost the second layer-1 accumulator: measured SLOWER on the README
-  // towers (top 41 -> 46.5 us, bottom 29.6 -> 30.4 us: the next tile's layer 1 then waits for the first
-  // epilogue of the previous one), so the mode is opt-in (MM_MLP_DUAL=1) and kept for narrow/deep towers.
-  p.dual = p.n_chain > 0 && getenv("MM_MLP_DUAL") && getenv("MM_MLP_DUAL")[0] == '1';
-  for (int c = 0; c < p.n_chain; ++c)
-    if (p.c[c].Np > 64) p.dual = 0;  // two chain sets only fit when every chain accumulator is <= 64 columns
-  // ring slot = one half ({A_hi, W_hi} or {A_lo, W_lo}) of a k-block; the fp32 transpose tiles of the
-  // epilogue are only carved when fp32 rows are written (the head-only top tower gets a deeper ring)
+  // ring slot = one half ({A_hi, W_hi} or {A_lo, W_lo}) of a k-block
   const size_t stage_bytes = (size_t)A_TILE_BYTES + (size_t)p.N1p * BLOCK_K * 2;
-  const size_t epi = fp32_rows ? (size_t)kEpiWarps * EPI_STAGE_BYTES : 0;
-  const size_t fixed = 1024 + (size_t)p.w_bytes + 40 * sizeof(uint64_t) + ((kMaxChain + 1) * 128 + 32) * sizeof(float) + epi;
+  const size_t fixed = 1024 + (size_t)p.w_bytes + 40 * sizeof(uint64_t) + ((kMaxChain + 1) * 128 + 128) * sizeof(float);
   if (fixed + 4 * stage_bytes > 227 * 1024) return false;
   int stages = (int)((227 * 1024 - fixed) / stage_bytes);
   if (stages > 12) stages = 12;
   const int kb1 = p.K1p / BLOCK_K;
   if (stages > 4 * kb1) stages = 4 * kb1 > 4 ? 4 * kb1 : 4;
   p.stages = stages;
-  smem = 1024 + stages * stage_bytes + p.w_bytes + (2 * stages + 10) * sizeof(uint64_t) +
-         ((kMaxChain + 1) * 128 + 32) * sizeof(float) + epi;
+  smem = 1024 + stages * stage_bytes + p.w_bytes + (2 * stages + 2) * sizeof(uint64_t) +
+         ((kMaxChain + 1) * 128 + 128) * sizeof(float);
   return true;
 }
 
@@ -506,7 +355,7 @@ int mm_mlp_tc_supported(int K, int n_layers, const int* widths, int with_head) {
   if (with_head && widths[n_layers - 1] > 32) return 0;
   mm::mlp::Params p;
   size_t smem = 0;
-  return plan_tower(K, n_layers, widths, true, p, smem) ? 1 : 0;
+  return plan_tower(K, n_layers, widths, p, smem) ? 1 : 0;
 }
 
 }  // extern "C"
@@ -539,7 +388,7 @@ static int mlp_tc_impl(const void* a_split, int64_t M, int K, int n_layers, cons
 
   Params p;
   size_t smem = 0;
-  MM_REQUIRE(plan_tower(K, n_layers, widths, out != nullptr || out_operand != nullptr, p, smem), MM_ERR_UNSUPPORTED,
+  MM_REQUIRE(plan_tower(K, n_layers, widths, p, smem), MM_ERR_UNSUPPORTED,
              "mm_mlp_tc: the tower does not fit in shared memory with two pipeline stages (mm_mlp_tc_supported)");
   p.M = M;
   p.act1 = acts[0];
@@ -579,26 +428,7 @@ static int mlp_tc_impl(const void* a_split, int64_t M, int K, int n_layers, cons
   const long long tiles = (M + BLOCK_M - 1) / BLOCK_M;
   const int sms = mm::sm_count();
   const unsigned grid = (unsigned)(tiles < sms ? tiles : sms);
-  static long long* trace_buf = nullptr;
-  const char* tr = getenv("MM_MLP_TRACE");
-  p.trace = nullptr;
-  if (tr && tr[0] == '1') {  // debug: timeline of CTA 0 on stderr (synchronises; never set in production)
-    if (!trace_buf) cudaMalloc(&trace_buf, 4001 * sizeof(long long));
-    cudaMemsetAsync(trace_buf, 0, 4001 * sizeof(long long), (cudaStream_t)stream);
-    p.trace = trace_buf;
-  }
   mlp_tc_kernel<<<grid, kThreads, smem, (cudaStream_t)stream>>>(tmA, tmW1, tmC[0], tmC[1], tmC[2], p);
-  if (p.trace) {
-    static long long host[4001];
-    cudaStreamSynchronize((cudaStream_t)stream);
-    cudaMemcpy(host, trace_buf, sizeof(host), cudaMemcpyDeviceToHost);
-    const long long n = host[0] < 2000 ? host[0] : 2000;
-    long long t0 = n ? host[2] : 0;
-    for (long long i = 0; i < n; ++i) t0 = host[2 + 2 * i] < t0 ? host[2 + 2 * i] : t0;
-    fprintf(stderr, "mm_mlp_tc trace (K1p=%d n_chain=%d stages=%d): tag:cycles", p.K1p, p.n_chain, p.stages);
-    for (long long i = 0; i < n; ++i) fprintf(stderr, " %lld:%lld", host[1 + 2 * i], host[2 + 2 * i] - t0);
-    fprintf(stderr, "\n");
-  }
   return mm::check_launch("mm_mlp_tc");
 }
 

@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a kernels behind include/mm_b200.h.
+// Shared helpers for the sm_90a kernels behind include/mm_b200.h.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

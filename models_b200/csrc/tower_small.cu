@@ -1,7 +1,7 @@
 // Narrow-input two-layer tower in one launch:  h = act2(act1(concat(columns) W1 + b1) W2 + b2)
 //
 // The DLRM bottom tower (13 continuous columns -> 128 -> 64) is 1.3 GFLOP and 20 MB of traffic per 65 536-sample
-// batch — far too small for the TMA/tcgen05 tower kernel, whose per-tile latency chain (plus the separate
+// batch — far too small for the TMA/wgmma tower kernel, whose per-tile latency chain (plus the separate
 // concat+split launch in front of it) cost 34 us of a 147 us step.  Here one warp owns 16 samples:
 //   * the <= 16 input columns are read straight from their column arrays (ContinuousFeatures + ConcatFeatures:
 //     sorted-name order, cast to fp32; merlin/models/tf/inputs/continuous.py:117-138, core/aggregation.py:54-66)

@@ -14,7 +14,7 @@ TensorFlow is not a dependency here, so the on-disk form is:
                                   references into variables/) — the analogue of SavedModel's custom objects
 
 `Model.load_weights` also accepts a plain {name: array} mapping, which is how a Keras checkpoint exported
-with `{v.name: v.numpy() for v in keras_model.variables}` (plus a name map) is served by the B200 path.
+with `{v.name: v.numpy() for v in keras_model.variables}` (plus a name map) is served by the H100 path.
 """
 from __future__ import annotations
 

@@ -8,7 +8,7 @@ dict keyed by schema column names, scalar features `(B,)`, list features as the 
 tag; `shuffle`, `drop_last`, `global_size` / `global_rank` sharding (one loader per GPU process, as Horovod
 does), `peek()`, `len()`, `output_schema`.
 
-B200 hand-off: every batch is packed on the host into ONE pinned allocation (HostBatch) and moved with ONE
+H100 hand-off: every batch is packed on the host into ONE pinned allocation (HostBatch) and moved with ONE
 cudaMemcpyAsync on a copy stream; a background thread packs batch i+1 while batch i is consumed, and an event
 orders the consumer's stream after the copy — so parquet decode, host packing and H2D all overlap the forward.
 Categorical ids are narrowed to int32 when the schema's domain allows (halves the index traffic of the gather).

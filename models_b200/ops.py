@@ -311,7 +311,7 @@ def inbatch_scores(q, pos, neg, out, pos_ids=None, neg_ids=None, downscore=True,
                    false_neg_score: float = -655.04, pos_prob=None, neg_prob=None,
                    temperature: float = 1.0, tensor_cores: bool = True) -> torch.Tensor:
     """out (B, 1+N) = [q.pos | masked(q @ neg^T)] / T  (include/mm_b200.h: mm_inbatch_scores[_tc]).
-    tensor_cores=True: tcgen05 split-bf16 GEMM (fp32-grade); False: exact fp32 CUDA-core kernel."""
+    tensor_cores=True: wgmma split-bf16 GEMM (fp32-grade); False: exact fp32 CUDA-core kernel."""
     for n_, t_ in (("q", q), ("pos", pos), ("neg", neg)):
         _dev(t_, n_, torch.float32)
         if not t_.is_contiguous():
@@ -519,7 +519,7 @@ def l2_normalize(x: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.T
 
 
 # ---------------------------------------------------------------------------------------------
-# tensor-core dense path (tcgen05 split-bf16)
+# tensor-core dense path (wgmma split-bf16)
 # ---------------------------------------------------------------------------------------------
 def tc_padded_k(K: int) -> int:
     return int(_lib().mm_tc_padded_k(int(K)))
@@ -682,7 +682,7 @@ def mlp_tc(a_split: torch.Tensor, K: int, w_splits: Sequence[torch.Tensor], widt
            head_w: Optional[torch.Tensor] = None, head_b: float = 0.0, head_act: Optional[str] = None,
            head_out: Optional[torch.Tensor] = None, out_operand: Optional[torch.Tensor] = None):
     """Whole MLP tower in one launch (mm_mlp_tc): layer 1 from the split-bf16 rows `a_split`, layers 2..n on
-    chip (activations stay in tensor memory).  out: (M, widths[-1]) fp32 and/or head_out: (M, 1); out_operand:
+    chip (activations stay in registers).  out: (M, widths[-1]) fp32 and/or head_out: (M, 1); out_operand:
     (M, 2*widths[-1]) bf16 split rows [hi | lo] for the interaction kernel (mm_mlp_tc_operand_out)."""
     n = len(widths)
     if not (len(w_splits) == len(biases) == len(acts) == n):

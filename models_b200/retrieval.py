@@ -499,7 +499,7 @@ class CategoricalOutput(Block):
                                     CategoricalCrossEntropy(from_logits=True) needs
                                     (losses/listwise.py:38-50): loss = lse - logit[target]
     top_k(x, k)                  -> (scores, ids) in tf.math.top_k order (outputs/topk.py:221-223)
-    The last two stream the catalog through one tcgen05 GEMM without ever writing (B, N_I)."""
+    The last two stream the catalog through one wgmma GEMM without ever writing (B, N_I)."""
 
     def __init__(self, to_call, logits_temperature: float = 1.0, use_bias: bool = True, name: Optional[str] = None, **kwargs):
         from .inputs import EmbeddingTable

@@ -4,9 +4,8 @@ Partitioning: row r of every sharded table lives on rank `r % world` at local ro
 (balanced under skew).  Tables with fewer than `replicate_below_rows` rows (default 65 536 = 16 MB at
 D = 64) are kept whole on every rank (SURVEY §8(e): "replicate tables with <= 64 k rows and shard only
 the big ones"): a table of a handful of rows has nothing to shard, and sharding it anyway makes every
-sample of every GPU read the same few cache lines of one owner over NVLink — measured on 2 x B200, the
-8 tables under 1 000 rows of the Criteo-TB shape double the step time when sharded
-(profiles/r02_notes.md §b).  `replicate_below_rows=0` shards everything.  Dense / MLP / interaction
+sample of every GPU read the same few cache lines of one owner over NVLink (the 8 tables under 1 000 rows
+of the Criteo-TB shape are such tables).  `replicate_below_rows=0` shards everything.  Dense / MLP / interaction
 weights are replicated; the batch is sharded data-parallel.
 
 Forward (one process per GPU): all shards live in ONE symmetric-memory arena per rank

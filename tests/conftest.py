@@ -10,13 +10,13 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 @pytest.fixture(scope="session", autouse=True)
 def _built_library():
-    """Build libmm_b200.so when nvcc is present (CPU container); on the GPU box the prebuilt
-    in-tree .so travels with the snapshot and is used as is."""
+    """Build libmm_b200.so when it is missing (nvcc needs no GPU); a library that build() already
+    compiled in-tree is used as is."""
     from models_b200 import _cabi
 
     if not _cabi.LIB_PATH.exists():

@@ -1,6 +1,6 @@
-"""Tensor-core dense path (tcgen05 + TMA, split-bf16) against the fp32 oracle.
+"""Tensor-core dense path (wgmma + TMA, split-bf16) against the fp32 oracle.
 
-passes=3 (hi*hi + hi*lo + lo*hi in one fp32 TMEM accumulator) must be fp32-grade: asserted at
+passes=3 (hi*hi + hi*lo + lo*hi in one fp32 accumulator) must be fp32-grade: asserted at
 5e-5 of the output scale, 20x inside the north-star 1e-3.  passes=1 is plain bf16 (~1e-2)."""
 import numpy as np
 import pytest

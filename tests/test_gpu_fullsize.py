@@ -1,4 +1,4 @@
-"""BASELINE.json's FULL sizes on the B200, checked through size-independent properties and sampled
+"""BASELINE.json's FULL sizes on the H100, checked through size-independent properties and sampled
 oracle comparisons (the oracle cannot run 65 536 x 45.6 M-row lookups in seconds, but the tables are
 hash-initialised, so any row can be regenerated on the host bit-exactly).
 

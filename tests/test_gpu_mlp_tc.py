@@ -1,5 +1,5 @@
-"""Whole-tower MLP kernel (mm_mlp_tc: layer 1 TMA-fed tcgen05, layers 2..n on chip with the A operand
-in tensor memory) against the fp64 NumPy chain of oracle.dense — the reference's MLPBlock
+"""Whole-tower MLP kernel (mm_mlp_tc: layer 1 TMA-fed wgmma, layers 2..n on chip with the A operand
+in registers) against the fp64 NumPy chain of oracle.dense — the reference's MLPBlock
 (merlin/models/tf/blocks/mlp.py:97-139) + BinaryOutput Dense(1) (outputs/classification.py:114).
 Tolerance: 5e-5 of the output scale per layer (3-pass split-bf16), 20x inside the north-star 1e-3."""
 import numpy as np
@@ -37,7 +37,7 @@ def _oracle_chain(x, Ws, bs, acts):
     (65536 // 16, 415, [128, 64, 32]),      # README top tower
     (1000, 13, [128, 64]),                  # README bottom tower
     (777, 415, [128, 64]),
-    (129, 69, [32, 128, 64, 128]),          # wide chain: A and D regions of TMEM full, 96 KB of resident weights
+    (129, 69, [32, 128, 64, 128]),          # wide chain: 96 KB of resident weights
     (5, 200, [100, 50, 20]),                # widths that are not multiples of 16 / 32
     (300, 64, [16, 16]),
     (4096, 129, [96, 48, 112, 8]),
@@ -86,7 +86,7 @@ def test_mlp_tc_equals_layer_by_layer_tc(device):
     """Same arithmetic as the per-layer mm_dense_tc chain (3-pass split-bf16, fp32 accumulate): the
     fused tower must agree with it to the last few ulps, on many tiles (persistent CTAs wrap around)."""
     rng = np.random.default_rng(13)
-    M, K, widths = 148 * 128 * 2 + 77, 415, [128, 64, 32]
+    M, K, widths = 132 * 128 * 2 + 77, 415, [128, 64, 32]
     x = rng.standard_normal((M, K)).astype(np.float32)
     Ws, bs = _tower(rng, K, widths)
     a = ops.split_rows(dev(x, device))
@@ -189,30 +189,11 @@ def test_mlp_block_on_feature_dict_uses_concat_split(device):
     assert H.rel_err(got.cpu().numpy(), ref) < 1e-4
 
 
-def test_mlp_tc_dual_chain_sets_match_single(device, monkeypatch):
-    """MM_MLP_DUAL=1: two tiles in flight (two chain sets in tensor memory, two epilogue groups) — same
-    arithmetic, so the result must be bit-identical to the default single-set schedule."""
-    rng = np.random.default_rng(17)
-    M, K, widths = 148 * 128 * 3 + 5, 415, [128, 64, 32]
-    x = rng.standard_normal((M, K)).astype(np.float32)
-    Ws, bs = _tower(rng, K, widths)
-    a = ops.split_rows(dev(x, device))
-    w = [ops.split_weights(dev(W, device)) for W in Ws]
-    b = [dev(v, device) for v in bs]
-    single = torch.empty((M, 32), dtype=torch.float32, device=device)
-    ops.mlp_tc(a, K, w, widths, b, ["relu"] * 3, out=single)
-    monkeypatch.setenv("MM_MLP_DUAL", "1")
-    dual = torch.empty((M, 32), dtype=torch.float32, device=device)
-    ops.mlp_tc(a, K, w, widths, b, ["relu"] * 3, out=dual)
-    torch.cuda.synchronize()
-    assert torch.equal(single, dual)
-
-
 @pytest.mark.parametrize("K,widths", [(415, [128, 64, 32]), (13, [512, 256, 64]), (69, [256, 128]), (200, [100, 50, 20, 7, 3]),
                                       (64, [16])])
 def test_mm_mlp_forward_whole_op_matches_oracle(device, K, widths):
     """mm_mlp_forward: fp32 Keras-layout kernels in, one C call, workspace-backed (fused tower when the widths
-    allow it, per-layer tcgen05 otherwise) == oracle.dense chain."""
+    allow it, per-layer wgmma otherwise) == oracle.dense chain."""
     rng = np.random.default_rng(18)
     M = 1537
     x = rng.standard_normal((M, K)).astype(np.float32)
@@ -250,7 +231,7 @@ def test_mm_cross_forward_whole_op_matches_oracle(device, d, depth):
 @pytest.mark.parametrize("B", [1, 17, 4099])
 def test_tower2_small_matches_oracle_and_tower_kernel(device, dims, K, acts, B):
     """mm_tower2_small: <= 16 scalar columns (mixed dtypes, (B,) and (B,1) and one (B,2) piece) -> two dense layers, fp32 rows and
-    split-bf16 rows; against the oracle MLP over the sorted-name concat, and against the TMA/tcgen05 tower path."""
+    split-bf16 rows; against the oracle MLP over the sorted-name concat, and against the TMA/wgmma tower path."""
     import models_b200 as mm
     from models_b200 import blocks
     from oracle import oracle

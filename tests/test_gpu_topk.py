@@ -1,4 +1,4 @@
-"""Top-k retrieval / evaluation on the B200 (SURVEY §8f-2) against the oracle restatement of
+"""Top-k retrieval / evaluation on the H100 (SURVEY §8f-2) against the oracle restatement of
 TopKIndexBlock (core/index.py:232-284), BruteForce (outputs/topk.py:180-243), RetrievalModel.evaluate
 (models/base.py:2266-2351) and metrics/topk.py.  Scores: 3-pass split-bf16 (atol 2e-4 at |q.v| ~ 10);
 identifiers: exact whenever the gap between neighbouring scores exceeds the score tolerance."""

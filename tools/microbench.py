@@ -4,7 +4,7 @@
     python tools/microbench.py [--only gather,interact,fused,dense,scores] [--iters 20]
 
 Prints one JSON line per kernel with achieved algorithmic GB/s (or TFLOP/s) and the fraction of
-the measured peak (MEASURED_PEAKS.json).  Used to produce profiles/*.md; never under a profiler.
+the measured peak (MEASURED_PEAKS.json).  Never under a profiler.
 """
 import argparse
 import json
@@ -149,7 +149,7 @@ def main():
         o = torch.empty((Bq, Bq + 4), device=dev)[:, 3:]  # negatives 16-B aligned (as retrieval._score allocates)
         for tc in (False, True):
             m, mn = timeit(lambda i: ops.inbatch_scores(q, it, it, o, pos_ids=ids, neg_ids=ids, tensor_cores=tc), max(5, args.iters // 2))
-            report(f"mm_inbatch_scores 16384x16384 D=64 ({'tcgen05 split-bf16 incl. operand split' if tc else 'fp32 SIMT'})", m, mn,
+            report(f"mm_inbatch_scores 16384x16384 D=64 ({'wgmma split-bf16 incl. operand split' if tc else 'fp32 SIMT'})", m, mn,
                    bytes_=Bq * (Bq + 1) * 4, flops=2.0 * Bq * Bq * Dq)
 
     if "fusedce" in only:
@@ -186,7 +186,7 @@ def main():
                    bytes_=B * (2 * ops.tc_padded_k(K) * 2 + 2 * ops.tc_padded_k(N) * 2), logical_flops=2.0 * B * K * N)
 
     if "mlp" in only:
-        # README towers: whole-tower kernel (mm_mlp_tc) vs the per-layer tcgen05 chain (mm_dense_tc)
+        # README towers: whole-tower kernel (mm_mlp_tc) vs the per-layer wgmma chain (mm_dense_tc)
         for K, widths, head in ((415, [128, 64, 32], True), (13, [128, 64], False)):
             x = torch.randn((B, K), device=dev)
             Ws = [torch.randn((k, n), device=dev) / (k ** 0.5) for k, n in zip([K] + widths[:-1], widths)]

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Summarise an .ncu-rep (raw page) into the handful of metrics the profiles/ notes quote.
+"""Summarise an .ncu-rep (raw page) into a handful of DRAM / issue metrics.
 
-    python tools/ncu_summary.py gpurun_out/prof.ncu-rep [pattern ...]
+    python tools/ncu_summary.py prof.ncu-rep [pattern ...]
 """
 import csv
 import subprocess

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """ONE process, TWO GPUs: the fused lookup+interaction kernel on GPU 0 with half of every Criteo-TB table on GPU 1
 (peer access), timed (a) with GPU 1 idle, (b) with GPU 1 running the mirrored kernel.  Separates requester-side
-from serving-side effects of the NVLink row reads (profiles/r02_notes.md).  Can run under ncu (single process).
+from serving-side effects of the NVLink row reads.  Can run under ncu (single process).
 
     python tools/probe/fused_peer.py [--batch 65536] [--tables all|big]
 """

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """NVLink peer access patterns (torchrun, 2+ ranks): GB/s of pulling / pushing 256-byte rows from / to the next
-rank's HBM, by access pattern.  Diagnostic for the row-sharded lookup (profiles/r02_notes.md); not a product path.
+rank's HBM, by access pattern.  Diagnostic for the row-sharded lookup; not a product path.
 
     python -m torch.distributed.run --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29540 tools/probe/peer_probe.py
 """
@@ -22,7 +22,7 @@ def build():
     so = HERE / "_peer_probe.so"
     src = HERE / "peer_probe.cu"
     if not so.exists() or so.stat().st_mtime < src.stat().st_mtime:
-        subprocess.run(["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC",
+        subprocess.run(["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC",
                         "-shared", "-o", str(so), str(src), "-lcudart"], check=True)
     lib = C.CDLL(str(so))
     lib.probe_run.restype = C.c_int
@@ -60,7 +60,7 @@ def main():
         rc = lib.probe_run(mode, src, dst, idx.data_ptr(), n, depth, rpg, blocks, threads, sink.data_ptr(), st)
         assert rc == 0, rc
 
-    def bench(label, mode, target, depth=1, rpg=24, blocks=148, threads=512, both=True):
+    def bench(label, mode, target, depth=1, rpg=24, blocks=132, threads=512, both=True):
         src = ptrs[rank] if target == "local" else peer
         dst = (ptrs[rank] if target == "local" else peer) + half_off
         if mode == 5:
@@ -93,13 +93,13 @@ def main():
         def mixed(label, mode, depth, rpg, threads):
             dist.barrier(device_ids=[local])
             for _ in range(2):
-                rc = lib.probe_run(mode, ptrs[rank], peer, idx.data_ptr(), n, depth, rpg, 148, threads, sink.data_ptr(), st); assert rc == 0
+                rc = lib.probe_run(mode, ptrs[rank], peer, idx.data_ptr(), n, depth, rpg, 132, threads, sink.data_ptr(), st); assert rc == 0
             torch.cuda.synchronize()
             dist.barrier(device_ids=[local])
             t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             t0.record()
             for _ in range(4):
-                lib.probe_run(mode, ptrs[rank], peer, idx.data_ptr(), n, depth, rpg, 148, threads, sink.data_ptr(), st)
+                lib.probe_run(mode, ptrs[rank], peer, idx.data_ptr(), n, depth, rpg, 132, threads, sink.data_ptr(), st)
             t1.record()
             torch.cuda.synchronize()
             t = torch.tensor([t0.elapsed_time(t1) / 4], device=dev, dtype=torch.float64)
@@ -116,23 +116,23 @@ def main():
         return
     if os.environ.get("PROBE_SHORT"):
         for target in ("local", "peer"):
-            bench("random rows, ld.global.v4 x8 in flight/lane (16 lanes/row)", 4, target, blocks=148 * 4, threads=512)
-            bench("random rows, LDGSTS 8 lanes/row", 1, target, 1, 24, 148, 512)
-            bench("random rows, LDGSTS 8 lanes/row", 1, target, 2, 24, 148, 512)
-            bench("random rows, cp.async.bulk 256 B", 2, target, 2, 24, 148, 512)
+            bench("random rows, ld.global.v4 x8 in flight/lane (16 lanes/row)", 4, target, blocks=132 * 4, threads=512)
+            bench("random rows, LDGSTS 8 lanes/row", 1, target, 1, 24, 132, 512)
+            bench("random rows, LDGSTS 8 lanes/row", 1, target, 2, 24, 132, 512)
+            bench("random rows, cp.async.bulk 256 B", 2, target, 2, 24, 132, 512)
         dist.destroy_process_group()
         return
     for target in ("local", "peer"):
         for both in ((True, False) if target == "peer" else (True,)):
-            bench("sequential 16-B loads", 0, target, blocks=148 * 8, threads=512, both=both)
-            bench("sequential 16-B stores", 3, target, blocks=148 * 8, threads=512, both=both)
-            bench("random rows, ld.global.v4 x8 in flight/lane (16 lanes/row)", 4, target, blocks=148 * 4, threads=512, both=both)
-            bench("random rows PUSH (local read -> peer store)", 5, target, blocks=148 * 4, threads=512, both=both)
+            bench("sequential 16-B loads", 0, target, blocks=132 * 8, threads=512, both=both)
+            bench("sequential 16-B stores", 3, target, blocks=132 * 8, threads=512, both=both)
+            bench("random rows, ld.global.v4 x8 in flight/lane (16 lanes/row)", 4, target, blocks=132 * 4, threads=512, both=both)
+            bench("random rows PUSH (local read -> peer store)", 5, target, blocks=132 * 4, threads=512, both=both)
             for depth, rpg, threads in ((1, 24, 512), (2, 24, 512), (4, 24, 256), (8, 12, 256)):
-                bench("random rows, LDGSTS 8 lanes/row", 1, target, depth, rpg, 148, threads, both)
-            bench("random rows, LDGSTS 16 lanes/row", 6, target, 2, 24, 148, 512, both)
+                bench("random rows, LDGSTS 8 lanes/row", 1, target, depth, rpg, 132, threads, both)
+            bench("random rows, LDGSTS 16 lanes/row", 6, target, 2, 24, 132, 512, both)
             for depth, rpg, threads in ((1, 24, 512), (2, 24, 512), (4, 24, 256), (8, 12, 256)):
-                bench("random rows, cp.async.bulk 256 B", 2, target, depth, rpg, 148, threads, both)
+                bench("random rows, cp.async.bulk 256 B", 2, target, depth, rpg, 132, threads, both)
     dist.destroy_process_group()
 
 

@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""Per-kernel SASS opcode histogram of libmm_b200.so (cuobjdump -sass): which kernels are Blackwell-native
-(UTC*MMA = tcgen05.mma, UTMALDG/UTMASTG/UBLKCP = TMA, LDTM/STTM = tcgen05.ld/st) and which use the legacy tensor path
-(HMMA = mma.sync) or cp.async (LDGSTS).  Writes the table profiles/ quotes.
+"""Per-kernel SASS opcode histogram of libmm_b200.so (cuobjdump -sass): which kernels use the Hopper
+tensor path (HGMMA = wgmma, UTMALDG/UTMASTG/UBLKCP = TMA) and which the warp-level one (HMMA = mma.sync) or
+cp.async (LDGSTS).
 
-    python tools/sass_histogram.py > profiles/r02_sass_opcodes.txt
+    python tools/sass_histogram.py
 """
 import re
 import subprocess
@@ -13,7 +13,7 @@ from pathlib import Path
 
 ROOT = Path(__file__).resolve().parent.parent
 LIB = ROOT / "models_b200" / "_lib" / "libmm_b200.so"
-KEY = ["UTCHMMA", "UTCQMMA", "UTMALDG", "UTMASTG", "UBLKCP", "LDTM", "STTM", "HMMA", "LDSM", "LDGSTS", "LDG", "STG", "LDS", "STS", "SHFL",
+KEY = ["HGMMA", "UTMALDG", "UTMASTG", "UBLKCP", "HMMA", "LDSM", "LDGSTS", "LDG", "STG", "LDS", "STS", "SHFL",
        "MUFU", "BAR", "SYNCS", "ATOM", "RED"]
 
 
@@ -31,7 +31,7 @@ def main():
         if m and cur:
             kernels[cur][m.group(1)] += 1
     demangle = subprocess.run(["c++filt"], input="\n".join(kernels), capture_output=True, text=True).stdout.splitlines()
-    print(f"# SASS opcode counts per kernel of {LIB.name} (static instruction counts; cuobjdump -sass, sm_100a)")
+    print(f"# SASS opcode counts per kernel of {LIB.name} (static instruction counts; cuobjdump -sass, sm_90a)")
     print("# columns:", " ".join(KEY), "| total")
     for raw, name in sorted(zip(kernels, demangle), key=lambda kv: kv[1]):
         c = kernels[raw]
