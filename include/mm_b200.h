@@ -157,8 +157,8 @@ int mm_cross_combine(const float* x0, const float* proj, const float* x, int64_t
  * Output: either fp32 `out` (B, >= P+pairs) or `out_split`, the split-bf16 operand (B, 2*out_Kp)
  * = [hi | lo] of the next tensor-core dense layer (out_Kp = mm_tc_padded_k(P+pairs), padding
  * columns written as zeros) — exactly one of the two must be non-null.
- * Tensor-core path (mma.sync bf16, 3-pass split, one warp per sample, cp.async.bulk row staging)
- * when F <= 32, D % 16 == 0, P in {0, D}, no self interaction; CUDA-core path otherwise.
+ * Tensor-core path (mma.sync bf16, 3-pass split, one warp per sample, 16-byte cp.async row staging)
+ * when F <= 32, D in {16, 32, 64, 128}, P in {0, D}, no self interaction; CUDA-core path otherwise.
  * ------------------------------------------------------------------------------------- */
 int mm_dot_interaction(const float* x, int64_t B, int F, int D, int64_t x_stride,
                        const float* prefix, int P, int64_t prefix_stride, int self_interaction,

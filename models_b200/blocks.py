@@ -5,8 +5,6 @@ execution is a handful of fused kernel launches (models_b200.ops), not a Keras l
 """
 from __future__ import annotations
 
-import os
-
 from typing import Dict, List, Optional, Sequence, Union
 
 import torch
@@ -37,13 +35,7 @@ def _use_tc() -> bool:
     return _DENSE_ENGINE[0] in ("auto", "tc")
 
 
-_MLP_FUSION = [os.environ.get("MM_MLP_FUSION", "1") != "0"]
 _LAST_PATH = ["none"]
-
-
-def set_mlp_fusion(on: bool) -> None:
-    """Whole-tower kernel (mm_mlp_tc) for towers whose widths are all <= 128; off = one launch per layer."""
-    _MLP_FUSION[0] = bool(on)
 
 
 def last_dense_path() -> str:
@@ -107,7 +99,7 @@ def run_dense_chain(x: Optional[torch.Tensor], layers: "List[_Dense]", a_split: 
     if K != layers[0].input_dim:
         raise ValueError(f"{layers[0].name}: input width {K} != kernel rows {layers[0].input_dim}")
     widths = [l.units for l in layers]
-    if _MLP_FUSION[0] and ops.mlp_tc_supported(K, widths, head=fuse_head):
+    if ops.mlp_tc_supported(K, widths, head=fuse_head):
         # whole tower in one launch: layers 2..n run on chip, activations stay in registers
         _LAST_PATH[0] = "mlp_tc"
         kw = {}

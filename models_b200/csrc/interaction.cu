@@ -10,19 +10,11 @@
 
 namespace mm {
 
-bool use_imma_v1();
-
-namespace imma2 {  // interaction_v2.cu: second-generation warp-per-sample kernel (packed ids, sharded tables)
+namespace imma2 {  // interaction_v2.cu: warp-per-sample mma.sync kernel (F <= 32, D in {16,32,64,128})
 template <int MODE>
 int launch(const float* x, int64_t x_stride, const LookupParams& lk, const float* prefix, int64_t prefix_stride, int P,
            int bottom_slot, int64_t B, int F, int D, float* out_f32, int64_t out_stride, void* out_split, int out_Kp,
            int32_t* oob, cudaStream_t st, const char* who, bool presplit);
-}
-namespace imma {  // interaction_mma.cu: warp-level mma.sync path (F <= 32, D in {16,32,64,128})
-template <int MODE, typename IdxT>
-int launch(const float* x, int64_t x_stride, const GatherParams& gp, const float* prefix, int64_t prefix_stride,
-           int P, int bottom_slot, int64_t B, int F, int D, float* out_f32, int64_t out_stride, void* out_split,
-           int out_Kp, int32_t* oob, cudaStream_t st, const char* who);
 }
 
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src) {
@@ -222,15 +214,6 @@ static int launch_interact(const float* x, int64_t x_stride, const GatherParams&
   return check_launch(who);
 }
 
-bool use_imma_v1() {  // MM_IMMA_V1=1: first-generation kernel (interaction_mma.cu), kept for A/B measurements
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("MM_IMMA_V1");
-    v = (e && e[0] == '1') ? 1 : 0;
-  }
-  return v == 1;
-}
-
 }  // namespace mm
 
 extern "C" {
@@ -318,18 +301,13 @@ int mm_dot_interaction(const float* x, int64_t B, int F, int D, int64_t x_stride
   if (B == 0) return MM_OK;
   mm::GatherParams p;
   memset(&p, 0, sizeof(p));
-  if (!self_interaction && !mm::use_imma_v1()) {
+  if (!self_interaction) {
     mm::LookupParams lk;
     memset(&lk, 0, sizeof(lk));
     lk.world = 1;
     const int rc2 = mm::imma2::launch<0>(x, x_stride, lk, prefix, prefix_stride, P, -1, B, F, D, out, out_stride, out_split,
                                          out_Kp, nullptr, (cudaStream_t)stream, "mm_dot_interaction", false);
     if (rc2 != MM_ERR_UNSUPPORTED) return rc2;
-  }
-  if (!self_interaction) {
-    const int rc = mm::imma::launch<0, int32_t>(x, x_stride, p, prefix, prefix_stride, P, -1, B, F, D, out, out_stride,
-                                                out_split, out_Kp, nullptr, (cudaStream_t)stream, "mm_dot_interaction");
-    if (rc != MM_ERR_UNSUPPORTED) return rc;
   }
   MM_REQUIRE(out != nullptr, MM_ERR_UNSUPPORTED,
              "mm_dot_interaction: split-bf16 output needs the tensor-core path (F<=32, D%%16==0, P in {0,D})");
@@ -375,7 +353,7 @@ int mm_dlrm_gather_interact(const mm_gather_table* tables_host, int n_tables, in
   p.n_tables = n_tables;
   for (int t = 0; t < n_tables; ++t) p.t[t] = tables_host[t];
   cudaStream_t st = (cudaStream_t)stream;
-  if (!mm::use_imma_v1() && F <= mm::MM_LOOKUP_MAX_ROWS) {
+  if (F <= mm::MM_LOOKUP_MAX_ROWS) {
     mm::LookupParams lk;
     memset(&lk, 0, sizeof(lk));
     lk.world = 1;
@@ -389,15 +367,6 @@ int mm_dlrm_gather_interact(const mm_gather_table* tables_host, int n_tables, in
     const int rc2 = mm::imma2::launch<1>(nullptr, 0, lk, bottom, bottom_stride, P, bottom ? bottom_slot : -1, B, F, D, out,
                                          out_stride, out_split, out_Kp, oob_count, st, "mm_dlrm_gather_interact", false);
     if (rc2 != MM_ERR_UNSUPPORTED) return rc2;
-  }
-  {
-    const int bs = bottom ? bottom_slot : -1;
-    const int rc = idx_dtype == MM_I32
-                       ? mm::imma::launch<1, int32_t>(nullptr, 0, p, bottom, bottom_stride, P, bs, B, F, D, out, out_stride,
-                                                      out_split, out_Kp, oob_count, st, "mm_dlrm_gather_interact")
-                       : mm::imma::launch<1, int64_t>(nullptr, 0, p, bottom, bottom_stride, P, bs, B, F, D, out, out_stride,
-                                                      out_split, out_Kp, oob_count, st, "mm_dlrm_gather_interact");
-    if (rc != MM_ERR_UNSUPPORTED) return rc;
   }
   MM_REQUIRE(out != nullptr, MM_ERR_UNSUPPORTED,
              "mm_dlrm_gather_interact: split-bf16 output needs the tensor-core path (F<=32, D%%16==0)");

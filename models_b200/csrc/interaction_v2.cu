@@ -1,12 +1,14 @@
-// DLRM lookup + pairwise interaction, one warp per sample (second generation of interaction_mma.cu).
+// DLRM lookup + pairwise interaction on mma.sync, one warp per sample: the tensor-core path of
+// mm_dlrm_lookup_interact, mm_dlrm_gather_interact and mm_dot_interaction (F <= 32, D in {16, 32, 64, 128}, P in {0, D}).
 //
-// What changed against the first kernel (issue-bound, a large share of its instructions in the row-copy loop):
+// The kernel is bound on the SM side (instruction issue and the mma.sync pipe), not by DRAM, so every phase is built
+// to issue few instructions per sample:
 //   * copy loop: 8 lanes move one 128-byte half row per LDGSTS, 4 rows per instruction.  Staged row r is
 //     owned by lane r (tables arrive sorted by slot, so row == slot), a row's source pointer travels
 //     with two shuffles, and because row = 4*i + lane/8 the XOR swizzle of a lane's destination does
 //     not depend on i: every destination is `lane constant + immediate`.  7 iterations x (2 SHFL +
-//     2 IADD + 2 LDGSTS) per sample instead of 14 x 23 instructions.  Bad ids read a zero row in global
-//     memory (no zero-fill operand, no predicates).
+//     2 IADD + 2 LDGSTS) per sample.  Bad ids read a zero row in global memory (no zero-fill operand,
+//     no predicates).
 //   * fragment loads: the k index of a 16-wide k-step is permuted (lane t takes floats 4t..4t+3 and
 //     calls them k = 2t, 2t+1, 2t+8, 2t+9).  A and B fragments are the same registers (B = X^T), so the
 //     permutation cancels in the dot products and one LDS.128 replaces two LDS.64.
@@ -25,15 +27,20 @@
 // DotProductInteraction (blocks/interaction.py:86-116) + shortcut concat (blocks/dlrm.py:126-130).
 #include <cuda_bf16.h>
 
-#include <cstdlib>
 #include <cstring>
 
 #include "mm_common.cuh"
+#include "warp_mma.cuh"
 
 namespace mm {
 namespace imma2 {
 
 __device__ __align__(16) float g_zero_row[128];  // zero-initialised: source of rows for out-of-range ids
+
+// Sample buffers per warp: one sample in flight behind the one being computed, for local tables and for rows that come
+// over NVLink alike.  Deeper pipelines do not pay for rows read over NVLink: remote latency is dominated by hot rows of
+// tiny sharded tables serialising on single cache lines of the owner, which replicating those tables removes.
+constexpr int NBUF = 2;
 
 struct Params {
   const float* x;  // MODE 0: stacked input
@@ -54,39 +61,8 @@ struct Params {
   unsigned buf_bytes;   // one sample buffer (>= rows*D*4 and >= the staged output row)
   unsigned stage_cols;  // floats of the staged output row (out_Kp, or OW rounded up to 4)
   unsigned peer_off;    // byte offset of the peer pointer table in shared memory
-  unsigned ids_off;     // byte offset of the per-warp id rings (NBUF > 2)
 };
 
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-// predicated form: no branch / reconvergence bookkeeping around the copy
-__device__ __forceinline__ void cp_async16_if(bool pred, uint32_t dst, const void* src) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %2, 0;\n\t@p cp.async.cg.shared.global [%0], [%1], 16;\n\t}" ::"r"(dst),
-      "l"(src), "r"((uint32_t)pred)
-      : "memory");
-}
-template <int N>
-__device__ __forceinline__ void cp_async_wait() {
-  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
-}
-__device__ __forceinline__ void mma_bf16_16816(float (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3,
-                                               uint32_t b0, uint32_t b1) {
-  asm("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-}
-// (x, y) -> packed bf16x2 hi (x in the low half) and the bf16x2 of the residuals
-__device__ __forceinline__ void split_pair(float x, float y, uint32_t& hi, uint32_t& lo) {
-  __nv_bfloat162 h = __floats2bfloat162_rn(x, y);
-  hi = *reinterpret_cast<uint32_t*>(&h);
-  const float xh = __uint_as_float(hi << 16), yh = __uint_as_float(hi & 0xffff0000u);
-  __nv_bfloat162 l = __floats2bfloat162_rn(x - xh, y - yh);
-  lo = *reinterpret_cast<uint32_t*>(&l);
-}
 __device__ __forceinline__ float4 lds128(uint32_t addr) {
   float4 v;
   asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
@@ -94,10 +70,6 @@ __device__ __forceinline__ float4 lds128(uint32_t addr) {
 }
 __device__ __forceinline__ void sts32(uint32_t addr, float v) {
   asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(v) : "memory");
-}
-
-__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
 }
 
 struct RawIdx {
@@ -119,11 +91,7 @@ struct RawIdx {
 // + ~180 operand moves + 72 HMMA.  Same values as the in-kernel split => bit-identical output.
 // (A first attempt kept the lane-private LDS.128 scheme with hi and lo interleaved per chunk: fewer instructions, but
 // the A quads still had to be assembled with moves and nothing overlapped the load -> HMMA latency: 0.116 ms vs 0.104.)
-// NBUF sample buffers per warp: NBUF-1 samples in flight behind the one being computed.  The product uses 2 with
-// 16 warps, for local tables and for rows that come over NVLink alike.  NBUF = 3 / 4 (10 / 7 warps, ids through a
-// shared-memory ring) exist for experiments (MM_IMMA_NBUF): remote latency is dominated by hot rows of tiny
-// sharded tables serialising on single cache lines of the owner, which replicating those tables removes.
-template <int MODE, int KD /* embedding dim: 16, 32, 64, 128 */, int NWARPS /* launch bound */, bool PS, int NBUF>
+template <int MODE, int KD /* embedding dim: 16, 32, 64, 128 */, int NWARPS /* launch bound */, bool PS>
 __global__ void __launch_bounds__(32 * NWARPS, 1)
 interact_v2_kernel(const __grid_constant__ LookupParams lk, const Params p) {
   extern __shared__ __align__(256) uint8_t smem_raw[];
@@ -183,40 +151,6 @@ interact_v2_kernel(const __grid_constant__ LookupParams lk, const Params p) {
     }
     id_ptr += id_step;
     k_load += nw;
-    return r;
-  };
-
-  // ---- NBUF > 2 (rows over NVLink): ids travel through a per-warp shared-memory ring instead of registers.
-  // A register prefetch one sample ahead is useless here: the id load queues in the memory pipeline behind
-  // the row copies issued just before it and returns only after THEIR 10-20 us NVLink round trip, so every
-  // sample would wait for the previous one (ncu, r2h: 49 % of the stall samples sat on the id decode).  Instead
-  // the ids of sample j are copied (cp.async, 4-byte words) A = 2*NBUF-1 iterations before their rows are issued;
-  // they ride in the same commit groups as the rows, so `wait_group` orders everything and no extra wait exists.
-  constexpr bool IDS = NBUF > 2;
-  constexpr int A = 2 * NBUF - 1, SLOTS = NBUF + 1;
-  const uint32_t ring = smem_u32(smem_raw) + p.ids_off + (uint32_t)warp * (SLOTS * 256) + (uint32_t)lane * 8u;
-  uint32_t slot_w = 0, slot_r = 0;  // byte offsets of the ring slots written / read next
-  const uint8_t* idr_ptr = id_ptr;  // address of the id whose rows are issued next (bit offset inside its word)
-  auto submit_ids = [&]() {
-    if (MODE == 1 && is_table && k_load < n_cta) {
-      const uintptr_t a = reinterpret_cast<uintptr_t>(id_ptr);
-      const uint32_t* wp = reinterpret_cast<const uint32_t*>(a & ~(uintptr_t)3);
-      asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(ring + slot_w), "l"(wp) : "memory");
-      if (my_64 || (int)(a & 3) + my_w > 4)
-        asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(ring + slot_w + 4u), "l"(wp + 1) : "memory");
-    }
-    id_ptr += id_step;
-    k_load += nw;
-    slot_w += 256u;
-    if (slot_w == SLOTS * 256u) slot_w = 0;
-  };
-  auto read_ids = [&]() -> RawIdx {
-    RawIdx r;
-    asm volatile("ld.shared.v2.u32 {%0,%1}, [%2];" : "=r"(r.a), "=r"(r.b) : "r"(ring + slot_r));
-    r.sh = 8u * (uint32_t)(reinterpret_cast<uintptr_t>(idr_ptr) & 3);
-    idr_ptr += id_step;
-    slot_r += 256u;
-    if (slot_r == SLOTS * 256u) slot_r = 0;
     return r;
   };
 
@@ -346,34 +280,22 @@ interact_v2_kernel(const __grid_constant__ LookupParams lk, const Params p) {
   float* of32 = p.out_f32 ? p.out_f32 + s0 * p.out_stride : nullptr;
   const bool f32_vec = ((p.out_stride & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.out_f32) & 15) == 0);
 
-  // ---- software pipeline: NBUF-1 samples in flight behind the one being computed.
-  // registers (NBUF == 2): ids one iteration ahead of their rows; ring (NBUF > 2): iteration `it` submits the ids
-  // of sample it+A, issues the rows of sample it+NBUF-1, computes sample it — the first A iterations only fill.
-  RawIdx raw_pref{0u, 0u, 0u};
-  if (!IDS) {
-    raw_pref = load_raw();
+  // ---- software pipeline: NBUF-1 samples in flight behind the one being computed; ids one iteration ahead of their rows
+  RawIdx raw_pref = load_raw();
 #pragma unroll
-    for (int i = 0; i < NBUF - 1; ++i) {
-      const RawIdx cur = raw_pref;
-      raw_pref = load_raw();
-      issue(cur);
-    }
+  for (int i = 0; i < NBUF - 1; ++i) {
+    const RawIdx cur = raw_pref;
+    raw_pref = load_raw();
+    issue(cur);
   }
   int k_cmp = warp;
   uint32_t buf_cmp = 0;
-  for (int it = IDS ? -A : 0; it < n_iter; ++it) {
-    if (IDS) {
-      submit_ids();
-      if (it + NBUF - 1 >= 0) issue(read_ids());
-      else cp_async_commit();
-    } else {
-      const RawIdx cur = raw_pref;
-      raw_pref = load_raw();
-      issue(cur);  // refills the buffer consumed (and used as output stage) in the previous iteration
-    }
+  for (int it = 0; it < n_iter; ++it) {
+    const RawIdx cur = raw_pref;
+    raw_pref = load_raw();
+    issue(cur);  // refills the buffer consumed (and used as output stage) in the previous iteration
     cp_async_wait<NBUF - 1>();
     __syncwarp();
-    if (IDS && it < 0) continue;
     const uint32_t xs = wbase + buf_cmp;
     buf_cmp += p.buf_bytes;
     if (buf_cmp == NBUF * p.buf_bytes) buf_cmp = 0;
@@ -384,11 +306,12 @@ interact_v2_kernel(const __grid_constant__ LookupParams lk, const Params p) {
 #pragma unroll
         for (int c = 0; c < 4; ++c) acc[ti][c] = 0.0f;
 
-      if (PS) {
-        const uint32_t a0b = xs + la[0], a1b = xs + la[1], b0b = xs + lb[0], b1b = xs + lb[1];
+      const uint32_t a0b = xs + la[0], a1b = xs + la[1], b0b = xs + lb[0], b1b = xs + lb[1];
 #pragma unroll
-        for (int ks = 0; ks < KS; ++ks) {
-          uint32_t ah[2][4], al[2][4], bh[4][2], bl[4][2];
+      for (int ks = 0; ks < KS; ++ks) {
+        // A quads of m-tiles 0, 1 and B pairs of n-tiles 0..3 (n-tile nt = rows 8nt + g), hi and lo
+        uint32_t ah[2][4], al[2][4], bh[4][2], bl[4][2];
+        if (PS) {
           const uint32_t kx = 32u * ks;
           ldsm_x4(a0b ^ kx, ah[0][0], ah[0][1], ah[0][2], ah[0][3]);
           ldsm_x4((a0b ^ kx) + 128u, al[0][0], al[0][1], al[0][2], al[0][3]);
@@ -398,50 +321,36 @@ interact_v2_kernel(const __grid_constant__ LookupParams lk, const Params p) {
           ldsm_x4((b0b ^ kx) + 128u, bl[0][0], bl[0][1], bl[1][0], bl[1][1]);
           ldsm_x4(b1b ^ kx, bh[2][0], bh[2][1], bh[3][0], bh[3][1]);
           ldsm_x4((b1b ^ kx) + 128u, bl[2][0], bl[2][1], bl[3][0], bl[3][1]);
+        } else {
 #pragma unroll
-          for (int ti = 0; ti < 6; ++ti) {
-            const int mt = ti < 4 ? 0 : 1, nt = ti < 4 ? ti : ti - 2;
-            mma_bf16_16816(acc[ti], ah[mt][0], ah[mt][1], ah[mt][2], ah[mt][3], bl[nt][0], bl[nt][1]);
+          for (int q = 0; q < 4; ++q) {
+            const float4 v = lds128(xs + ((ks & 1) ? po[q] : pe[q]) + 64u * ks);
+            split_pair(v.x, v.y, bh[q][0], bl[q][0]);
+            split_pair(v.z, v.w, bh[q][1], bl[q][1]);
           }
+          // the A quad of m-tile mt is made of the B pairs of rows q = 2mt, 2mt+1
 #pragma unroll
-          for (int ti = 0; ti < 6; ++ti) {
-            const int mt = ti < 4 ? 0 : 1, nt = ti < 4 ? ti : ti - 2;
-            mma_bf16_16816(acc[ti], al[mt][0], al[mt][1], al[mt][2], al[mt][3], bh[nt][0], bh[nt][1]);
-          }
-#pragma unroll
-          for (int ti = 0; ti < 6; ++ti) {
-            const int mt = ti < 4 ? 0 : 1, nt = ti < 4 ? ti : ti - 2;
-            mma_bf16_16816(acc[ti], ah[mt][0], ah[mt][1], ah[mt][2], ah[mt][3], bh[nt][0], bh[nt][1]);
+          for (int mt = 0; mt < 2; ++mt) {
+            ah[mt][0] = bh[2 * mt][0], ah[mt][1] = bh[2 * mt + 1][0], ah[mt][2] = bh[2 * mt][1], ah[mt][3] = bh[2 * mt + 1][1];
+            al[mt][0] = bl[2 * mt][0], al[mt][1] = bl[2 * mt + 1][0], al[mt][2] = bl[2 * mt][1], al[mt][3] = bl[2 * mt + 1][1];
           }
         }
-      } else {
-#pragma unroll
-      for (int ks = 0; ks < KS; ++ks) {
-        uint32_t h[4][2], l[4][2];
-#pragma unroll
-        for (int q = 0; q < 4; ++q) {
-          const float4 v = lds128(xs + ((ks & 1) ? po[q] : pe[q]) + 64u * ks);
-          split_pair(v.x, v.y, h[q][0], l[q][0]);
-          split_pair(v.z, v.w, h[q][1], l[q][1]);
-        }
-        // tile (mt, nt): A = rows q = 2mt, 2mt+1; B (n-tile nt = rows 8nt + g) = the registers of q = nt.
-        // Pass-major order: six independent accumulators between dependent MMAs.
+        // tile ti = (mt, nt).  Pass-major order: six independent accumulators between dependent MMAs.
 #pragma unroll
         for (int ti = 0; ti < 6; ++ti) {
           const int mt = ti < 4 ? 0 : 1, nt = ti < 4 ? ti : ti - 2;
-          mma_bf16_16816(acc[ti], h[2 * mt][0], h[2 * mt + 1][0], h[2 * mt][1], h[2 * mt + 1][1], l[nt][0], l[nt][1]);
+          mma16816(acc[ti], ah[mt], bl[nt][0], bl[nt][1]);
         }
 #pragma unroll
         for (int ti = 0; ti < 6; ++ti) {
           const int mt = ti < 4 ? 0 : 1, nt = ti < 4 ? ti : ti - 2;
-          mma_bf16_16816(acc[ti], l[2 * mt][0], l[2 * mt + 1][0], l[2 * mt][1], l[2 * mt + 1][1], h[nt][0], h[nt][1]);
+          mma16816(acc[ti], al[mt], bh[nt][0], bh[nt][1]);
         }
 #pragma unroll
         for (int ti = 0; ti < 6; ++ti) {
           const int mt = ti < 4 ? 0 : 1, nt = ti < 4 ? ti : ti - 2;
-          mma_bf16_16816(acc[ti], h[2 * mt][0], h[2 * mt + 1][0], h[2 * mt][1], h[2 * mt + 1][1], h[nt][0], h[nt][1]);
+          mma16816(acc[ti], ah[mt], bh[nt][0], bh[nt][1]);
         }
-      }
       }
 
       // ---- the prefix row leaves the buffer before the buffer becomes the output stage
@@ -492,17 +401,9 @@ interact_v2_kernel(const __grid_constant__ LookupParams lk, const Params p) {
         if (f32_vec) {
           const int n4 = OW >> 2;
           for (int e = lane; e < n4; e += 32) reinterpret_cast<float4*>(of32)[e] = lds128(xs + (uint32_t)e * 16u);
-          for (int e = (n4 << 2) + lane; e < OW; e += 32) {
-            float v;
-            asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(xs + (uint32_t)e * 4u));
-            of32[e] = v;
-          }
+          for (int e = (n4 << 2) + lane; e < OW; e += 32) of32[e] = lds32(xs + (uint32_t)e * 4u);
         } else {
-          for (int e = lane; e < OW; e += 32) {
-            float v;
-            asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(xs + (uint32_t)e * 4u));
-            of32[e] = v;
-          }
+          for (int e = lane; e < OW; e += 32) of32[e] = lds32(xs + (uint32_t)e * 4u);
         }
       }
     }
@@ -513,24 +414,22 @@ interact_v2_kernel(const __grid_constant__ LookupParams lk, const Params p) {
   }
 }
 
-static int env_int(const char* name, int dflt) {
-  const char* e = getenv(name);
-  return e ? atoi(e) : dflt;
-}
-
-template <int MODE, int KD, int NWARPS, bool PS, int NBUF>
+// Two launch bounds per shape: 16 warps when they fit, else the 12-warp variant (more registers per thread), which
+// takes any smaller count (D = 128, F = 32: 32 KB per warp, 7 warps).
+template <int MODE, int KD, bool PS>
 static int launch_kd(const LookupParams& lk, const Params& p, size_t smem, unsigned grid, cudaStream_t st, const char* who) {
-  auto kern = interact_v2_kernel<MODE, KD, NWARPS, PS, NBUF>;
-  static bool attr_set[64] = {};  // per device: function attributes belong to the device's copy of the kernel
+  const int wide = p.n_warps > 12;
+  auto kern = wide ? interact_v2_kernel<MODE, KD, 16, PS> : interact_v2_kernel<MODE, KD, 12, PS>;
+  static bool attr_set[2][64] = {};  // per device: function attributes belong to the device's copy of the kernel
   int dev = 0;
   cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64 || !attr_set[dev]) {
+  if (dev < 0 || dev >= 64 || !attr_set[wide][dev]) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) {
       set_error("%s: cudaFuncSetAttribute failed: %s", who, cudaGetErrorString(e));
       return (int)e;
     }
-    if (dev >= 0 && dev < 64) attr_set[dev] = true;
+    if (dev >= 0 && dev < 64) attr_set[wide][dev] = true;
   }
   kern<<<grid, 32 * p.n_warps, smem, st>>>(lk, p);
   return check_launch(who);
@@ -571,49 +470,25 @@ int launch(const float* x, int64_t x_stride, const LookupParams& lk, const float
   p.stage_cols = out_split ? (unsigned)out_Kp : (unsigned)((OW + 3) & ~3);
   const unsigned in_bytes = (unsigned)(rows * D * 4), stage_bytes = p.stage_cols * 4u;
   p.buf_bytes = ((in_bytes > stage_bytes ? in_bytes : stage_bytes) + 255u) & ~255u;  // 256-B aligned (ldmatrix address XOR)
-  bool remote = false;
-  if (MODE == 1 && lk.world > 1)
-    for (int r = 0; r < rows; ++r) remote = remote || lk.sharded[r];
-  static int nbuf_env = -2;
-  if (nbuf_env == -2) nbuf_env = env_int("MM_IMMA_NBUF", 0);
-  const int nbuf = (nbuf_env >= 2 && nbuf_env <= 4) ? nbuf_env : 2;
-  (void)remote;
-  const unsigned ring_bytes = nbuf > 2 ? (unsigned)(nbuf + 1) * 256u : 0u;  // per-warp id ring
-  const unsigned per_warp = (unsigned)nbuf * p.buf_bytes + ring_bytes;
+  const unsigned per_warp = NBUF * p.buf_bytes;
   const unsigned peer_bytes = (MODE == 1 && lk.world > 1) ? (unsigned)(rows * lk.world * 8) : 0u;
   const unsigned budget = 227u * 1024u - peer_bytes;
-  static int warps_env = -2;
-  if (warps_env == -2) warps_env = env_int("MM_IMMA_WARPS", 0);
-  const int want_warps = warps_env > 0 ? warps_env : (nbuf == 4 ? 8 : nbuf == 3 ? 10 : 16);
   int warps = (int)(budget / per_warp);
-  if (warps > want_warps) warps = want_warps;
   if (warps > 16) warps = 16;
-  if (nbuf > 2 && warps > 12) warps = 12;
   if (warps < 2) return MM_ERR_UNSUPPORTED;
   p.n_warps = warps;
-  p.ids_off = (unsigned)warps * nbuf * p.buf_bytes;
   p.peer_off = (unsigned)warps * per_warp;
   const size_t smem = (size_t)p.peer_off + peer_bytes;
   const long long sms = sm_count();
   long long want = (B + warps - 1) / warps;
   const unsigned grid = (unsigned)(want < sms ? want : sms);
-  // instantiated variants: 16 (or 12) warps x 2 buffers; operand-format rows (presplit) only with 2 buffers;
-  // 3 / 4 buffers (id ring) for experiments
-#define MM_V2_LAUNCH(KD)                                                                                                \
-  (nbuf == 4 ? launch_kd<MODE, KD, 12, false, 4>(lk, p, smem, grid, st, who)                                            \
-   : nbuf == 3 ? launch_kd<MODE, KD, 12, false, 3>(lk, p, smem, grid, st, who)                                          \
-   : (presplit && MODE == 1 && KD == 64)                                                                                \
-       ? (warps > 12 ? launch_kd<1, 64, 16, true, 2>(lk, p, smem, grid, st, who) : launch_kd<1, 64, 12, true, 2>(lk, p, smem, grid, st, who)) \
-       : (warps > 12 ? launch_kd<MODE, KD, 16, false, 2>(lk, p, smem, grid, st, who)                                    \
-                     : launch_kd<MODE, KD, 12, false, 2>(lk, p, smem, grid, st, who)))
-  if (presplit && nbuf != 2) return MM_ERR_UNSUPPORTED;
+  if (presplit) return launch_kd<1, 64, true>(lk, p, smem, grid, st, who);  // MODE 1, D = 64 (checked above)
   switch (D) {
-    case 16: return MM_V2_LAUNCH(16);
-    case 32: return MM_V2_LAUNCH(32);
-    case 64: return MM_V2_LAUNCH(64);
-    default: return MM_V2_LAUNCH(128);
+    case 16: return launch_kd<MODE, 16, false>(lk, p, smem, grid, st, who);
+    case 32: return launch_kd<MODE, 32, false>(lk, p, smem, grid, st, who);
+    case 64: return launch_kd<MODE, 64, false>(lk, p, smem, grid, st, who);
+    default: return launch_kd<MODE, 128, false>(lk, p, smem, grid, st, who);
   }
-#undef MM_V2_LAUNCH
 }
 
 template int launch<0>(const float*, int64_t, const LookupParams&, const float*, int64_t, int, int, int64_t, int, int,

@@ -6,6 +6,7 @@
 #include <cstring>
 
 #include "mm_common.cuh"
+#include "warp_mma.cuh"
 
 namespace mm {
 
@@ -92,11 +93,7 @@ concat_split_kernel(const __grid_constant__ ConcatParams cp, long long B, __nv_b
     if (b >= B) continue;
     __align__(16) __nv_bfloat16 h[8], l[8];
 #pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float v = tile[r * ld + g * 8 + j];
-      h[j] = __float2bfloat16_rn(v);
-      l[j] = __float2bfloat16_rn(v - __bfloat162float(h[j]));
-    }
+    for (int j = 0; j < 8; ++j) split_bf16(tile[r * ld + g * 8 + j], h[j], l[j]);
     __nv_bfloat16* o = out + b * (2ll * Kp) + g * 8;
     *reinterpret_cast<uint4*>(o) = *reinterpret_cast<const uint4*>(h);
     *reinterpret_cast<uint4*>(o + Kp) = *reinterpret_cast<const uint4*>(l);

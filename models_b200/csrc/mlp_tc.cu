@@ -63,14 +63,6 @@ struct Params {
   float* head_out;
 };
 
-__device__ __forceinline__ void split_pair(float x, float y, uint32_t& hi, uint32_t& lo) {
-  __nv_bfloat162 h = __floats2bfloat162_rn(x, y);  // .x (low half) = x: K element 2c in the low 16 bits
-  hi = *reinterpret_cast<uint32_t*>(&h);
-  const float xh = __uint_as_float(hi << 16), yh = __uint_as_float(hi & 0xffff0000u);
-  __nv_bfloat162 l = __floats2bfloat162_rn(x - xh, y - yh);
-  lo = *reinterpret_cast<uint32_t*>(&l);
-}
-
 __global__ void __launch_bounds__(kThreads, 1)
 mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW1,
               const __grid_constant__ CUtensorMap tmC0, const __grid_constant__ CUtensorMap tmC1,

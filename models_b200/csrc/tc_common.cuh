@@ -4,6 +4,7 @@
 #include <cuda_bf16.h>
 
 #include "mm_common.cuh"
+#include "warp_mma.cuh"
 
 namespace mm {
 namespace tc {
@@ -11,8 +12,6 @@ namespace tc {
 // ---------------------------------------------------------------------------------------------
 // PTX wrappers
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
 }
@@ -208,12 +207,6 @@ __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr) {
   d |= (uint64_t)1 << 62;             // SWIZZLE_128B
   return d;
 }
-
-__device__ __forceinline__ void split_bf16(float v, __nv_bfloat16& hi, __nv_bfloat16& lo) {
-  hi = __float2bfloat16_rn(v);
-  lo = __float2bfloat16_rn(v - __bfloat162float(hi));
-}
-
 
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,

@@ -18,6 +18,7 @@
 #include <cstring>
 
 #include "mm_common.cuh"
+#include "warp_mma.cuh"
 
 namespace mm {
 namespace tsm {
@@ -53,21 +54,6 @@ __device__ __forceinline__ float load_col(const void* src, long long i, int dtyp
     case MM_F64: return (float)reinterpret_cast<const double*>(src)[i];
     default: return __ldg(reinterpret_cast<const float*>(src) + i);
   }
-}
-__device__ __forceinline__ void split_pair(float x, float y, uint32_t& hi, uint32_t& lo) {
-  __nv_bfloat162 h = __floats2bfloat162_rn(x, y);
-  hi = *reinterpret_cast<uint32_t*>(&h);
-  const float xh = __uint_as_float(hi << 16), yh = __uint_as_float(hi & 0xffff0000u);
-  __nv_bfloat162 l = __floats2bfloat162_rn(x - xh, y - yh);
-  lo = *reinterpret_cast<uint32_t*>(&l);
-}
-__device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
 }
 
 constexpr int W1_STRIDE = 80;  // bytes per n-row of W1 in shared memory: [hi k0..15 | lo k0..15] = 64 B + 16 B pad

@@ -21,46 +21,12 @@
 #include <cstring>
 
 #include "mm_common.cuh"
+#include "warp_mma.cuh"
 
 namespace mm {
 namespace trs {
 
 __device__ __align__(16) float g_zero_row[128];
-
-__device__ __forceinline__ void split_pair(float x, float y, uint32_t& hi, uint32_t& lo) {
-  __nv_bfloat162 h = __floats2bfloat162_rn(x, y);
-  hi = *reinterpret_cast<uint32_t*>(&h);
-  const float xh = __uint_as_float(hi << 16), yh = __uint_as_float(hi & 0xffff0000u);
-  __nv_bfloat162 l = __floats2bfloat162_rn(x - xh, y - yh);
-  lo = *reinterpret_cast<uint32_t*>(&l);
-}
-__device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void cp_async16_if(bool pred, uint32_t dst, const void* src) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %2, 0;\n\t@p cp.async.cg.shared.global [%0], [%1], 16;\n\t}" ::"r"(dst),
-      "l"(src), "r"((uint32_t)pred)
-      : "memory");
-}
-__device__ __forceinline__ void cp_async4_if(bool pred, uint32_t dst, const void* src) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %2, 0;\n\t@p cp.async.ca.shared.global [%0], [%1], 4;\n\t}" ::"r"(dst),
-      "l"(src), "r"((uint32_t)pred)
-      : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() {
-  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
-}
-__device__ __forceinline__ float lds32(uint32_t addr) {
-  float v;
-  asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(addr));
-  return v;
-}
 
 __device__ __forceinline__ long long load_id(const void* base, int w, long long s) {
   switch (w) {
@@ -306,15 +272,6 @@ static int launch_ibwd(const LookupParams& lk, IbwdParams p, cudaStream_t st) {
 //     fragments assembled in registers through a packed offset table, 12 warps at 168 registers: 241 us against 217 us —
 //     it is the dependent instruction chains of the compute phase, not the copy latency, that occupancy has to hide.)
 // ---------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];" : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr));
-}
-__device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
-               : "r"(addr));
-}
-
 constexpr int PS_WARPS = 16;
 constexpr unsigned PS_G_STRIDE = 80;  // bytes per row of a G matrix (64 + 16: conflict-free ldmatrix)
 constexpr unsigned PS_G_BYTES = 2 * 32 * PS_G_STRIDE;
@@ -430,8 +387,8 @@ interact_bwd_ps_kernel(const __grid_constant__ LookupParams lk, const __grid_con
       const float v = lds32(st + (uint32_t)(p.P + e) * 4u);
       const uint32_t ij = pair_ij[e];
       const uint32_t i = ij >> 8, j = ij & 255u;
-      const __nv_bfloat16 h = __float2bfloat16_rn(v);
-      const __nv_bfloat16 l = __float2bfloat16_rn(v - __bfloat162float(h));
+      __nv_bfloat16 h, l;
+      split_bf16(v, h, l);
       const uint32_t a1 = gs + i * PS_G_STRIDE + j * 2, a2 = gs + j * PS_G_STRIDE + i * 2;
       const unsigned short hb = __bfloat16_as_ushort(h), lb = __bfloat16_as_ushort(l);
       asm volatile("st.shared.u16 [%0], %1;" ::"r"(a1), "h"(hb) : "memory");
