@@ -188,7 +188,14 @@ int mm_dlrm_gather_interact(const mm_gather_table* tables_host, int n_tables, in
  *     lookup, all-to-all of vectors) is part of the same kernel as the interaction.  No collective,
  *     no barrier: tables are read-only in the forward pass.
  * `rows` is always the GLOBAL row count; ids outside [0, rows) give a zero row and bump *oob_count.
- * F = n_tables + (bottom ? 1 : 0) <= 32, D in {16, 32, 64, 128}, world <= 8. */
+ * F = n_tables + (bottom ? 1 : 0) <= 32, D in {16, 32, 64, 128}, world <= 8.
+ * Id columns (indices, idx_bytes, rows) of mm_lookup_table and mm_sparse_table are checked alike by every entry point
+ * that takes them (mm_dlrm_lookup_interact, mm_dlrm_interact_backward, mm_deepfm_head, mm_sparse_rows_apply), before
+ * any launch: null indices, rows <= 0, idx_bytes outside {1, 2, 3, 4, 8} or a 1-, 2- or 3-byte width that cannot
+ * address every row (rows > 2^(8 idx_bytes)) return MM_ERR_ARG; 4- and 8-byte id arrays not aligned to their width
+ * return MM_ERR_ALIGN.  mm_dlrm_interact_backward, mm_deepfm_head and mm_sparse_rows_apply return these codes where
+ * they used to launch with such a column; weights that are not 16-byte aligned now return MM_ERR_ALIGN from both
+ * mm_dlrm_lookup_interact (formerly MM_ERR_ARG) and mm_dlrm_interact_backward. */
 typedef struct {
   const float* weights;
   const void* indices; /* (B,) ids of this feature, idx_bytes each */

@@ -517,14 +517,12 @@ class FM(Block):
     def head(self, inputs: TabularData, addend: Optional[torch.Tensor] = None, out_layer: Optional["_Dense"] = None) -> torch.Tensor:
         """(B, 1) = [out_layer](wide + pairwise [+ addend]) in one kernel (ops.deepfm_head)."""
         from .core import get_feature
-        from .inputs import _as_index
 
         dev = next(iter(inputs.values())).device
         self.build(dev)
         B = batch_size_of(inputs)
         emb = self.embeddings
-        raw = [get_feature(inputs, f) for f in self.cat_names]
-        idx = [i if i.dtype in (torch.uint8, torch.uint16) else _as_index(i).reshape(-1) for i in raw]
+        idx = [ops.fused_ids(get_feature(inputs, f)) for f in self.cat_names]
         tabs = [emb.feature_to_table[f].table for f in self.cat_names]
         cont = []
         for n in self.cont_names:
@@ -814,7 +812,7 @@ class DLRM(Block):
         emb = self.embeddings
         feats = emb.feature_names
         from .core import get_feature
-        from .inputs import _as_index, _raise_on_oob
+        from .inputs import _raise_on_oob
 
         if self.sharded is not None:
             oob = emb.counter(dev)
@@ -837,12 +835,12 @@ class DLRM(Block):
             raw = [get_feature(inputs, f) for f in feats]
             if self.can_emit_split():
                 # ids travel at their own width (packed uint8 / uint16 / 24-bit host batches, int32, int64)
-                idx = [i if i.dtype in (torch.uint8, torch.uint16) else _as_index(i).reshape(-1) for i in raw]
+                idx = [ops.fused_ids(i) for i in raw]
                 tabs = [emb.feature_to_table[f].operand_mirror() if operand_rows else emb.feature_to_table[f].table for f in feats]
                 ops.dlrm_lookup_interact(tabs, idx, [slots[f] for f in feats], [t.shape[0] for t in tabs], D, bottom,
                                          slots.get("bottom_block", -1), out, oob, operand_rows=operand_rows)
             else:
-                idx = [_as_index(i).reshape(-1) for i in raw]
+                idx = [ops.as_index(i).reshape(-1) for i in raw]
                 if len({i.dtype for i in idx}) > 1:
                     idx = [i.to(torch.int64) for i in idx]
                 ops.dlrm_gather_interact([emb.feature_to_table[f].table for f in feats], idx, [slots[f] for f in feats], D,

@@ -1,5 +1,6 @@
 // Library-wide state of the C-ABI (include/mm_b200.h): error text, launch counter, version,
-// and the deterministic table initialiser.
+// the checks of id columns and lookup-table descriptors shared by the entry points, and the
+// deterministic table initialiser.
 #include <atomic>
 #include <cstdarg>
 #include <cstring>
@@ -40,6 +41,44 @@ int sm_count() {
       cached = 132;  // H100 SXM
   }
   return cached;
+}
+
+int check_id_column(const char* who, int t, const void* indices, int w, long long rows) {
+  MM_REQUIRE(indices && rows > 0, MM_ERR_ARG, "%s: table %d: null ids or rows <= 0", who, t);
+  MM_REQUIRE(w == 1 || w == 2 || w == 3 || w == 4 || w == 8, MM_ERR_ARG, "%s: table %d: idx_bytes must be 1, 2, 3, 4 or 8", who, t);
+  MM_REQUIRE(w >= 4 || rows <= (1ll << (8 * w)), MM_ERR_ARG, "%s: table %d: %lld rows do not fit %d-byte ids", who, t, rows, w);
+  MM_REQUIRE((w != 4 && w != 8) || ((uintptr_t)indices % w) == 0, MM_ERR_ALIGN, "%s: table %d: misaligned ids", who, t);
+  return MM_OK;
+}
+
+int fill_lookup_params(const char* who, const mm_lookup_table* tables, int n_tables, int F, int bottom_slot, int rank,
+                       bool sharded_ok, LookupParams& lk) {
+  unsigned seen = bottom_slot >= 0 ? (1u << bottom_slot) : 0u;
+  for (int t = 0; t < n_tables; ++t) {
+    const mm_lookup_table& tb = tables[t];
+    const int r = tb.slot;
+    MM_REQUIRE(tb.weights && r >= 0 && r < F, MM_ERR_ARG, "%s: table %d: null weights or slot %d outside [0, %d)", who, t, r, F);
+    MM_REQUIRE(!(seen & (1u << r)), MM_ERR_ARG, "%s: slot %d used twice", who, r);
+    seen |= 1u << r;
+    MM_REQUIRE(((uintptr_t)tb.weights % 16) == 0, MM_ERR_ALIGN, "%s: table %d: weights must be 16-byte aligned", who, t);
+    if (const int rc = check_id_column(who, t, tb.indices, tb.idx_bytes, tb.rows)) return rc;
+    lk.weights[r] = tb.weights;
+    lk.indices[r] = tb.indices;
+    lk.rows[r] = tb.rows;
+    lk.idx_bytes[r] = (unsigned char)tb.idx_bytes;
+    if (tb.peer_weights_host) {
+      MM_REQUIRE(sharded_ok, MM_ERR_UNSUPPORTED, "%s: row-sharded tables are not supported", who);
+      MM_REQUIRE(lk.world > 1, MM_ERR_ARG, "%s: table %d is sharded but world == 1", who, t);
+      lk.sharded[r] = 1;
+      for (int k = 0; k < lk.world; ++k) {
+        MM_REQUIRE(tb.peer_weights_host[k] && ((uintptr_t)tb.peer_weights_host[k] % 16) == 0, MM_ERR_ARG,
+                   "%s: table %d: null / misaligned shard pointer of rank %d", who, t, k);
+        lk.peers[r * lk.world + k] = tb.peer_weights_host[k];
+      }
+      MM_REQUIRE(tb.peer_weights_host[rank] == tb.weights, MM_ERR_ARG, "%s: table %d: peer_weights_host[rank] != weights", who, t);
+    }
+  }
+  return MM_OK;
 }
 
 // splitmix64 finaliser over (seed, element index): identical integer arithmetic in

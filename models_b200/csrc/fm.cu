@@ -47,27 +47,6 @@ struct Params {
   int D;
 };
 
-__device__ __forceinline__ long long load_id(const void* base, int w, long long s) {
-  switch (w) {
-    case 1: return (long long)reinterpret_cast<const uint8_t*>(base)[s];
-    case 2: return (long long)reinterpret_cast<const uint16_t*>(base)[s];
-    case 3: {
-      const uint8_t* b = reinterpret_cast<const uint8_t*>(base) + 3 * s;
-      return (long long)b[0] | ((long long)b[1] << 8) | ((long long)b[2] << 16);
-    }
-    case 8: return reinterpret_cast<const long long*>(base)[s];
-    default: return (long long)reinterpret_cast<const int32_t*>(base)[s];
-  }
-}
-__device__ __forceinline__ float load_cont(const void* src, long long i, int dtype) {
-  switch (dtype) {
-    case MM_I32: return (float)reinterpret_cast<const int32_t*>(src)[i];
-    case MM_I64: return (float)reinterpret_cast<const long long*>(src)[i];
-    case MM_F64: return (float)reinterpret_cast<const double*>(src)[i];
-    default: return reinterpret_cast<const float*>(src)[i];
-  }
-}
-
 __global__ void __launch_bounds__(256) deepfm_head_kernel(const __grid_constant__ Params p) {
   const int lane = threadIdx.x & 31;
   const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -93,7 +72,7 @@ __global__ void __launch_bounds__(256) deepfm_head_kernel(const __grid_constant_
     }
     sq = warp_sum(sq);
     if (lane == 0) {
-      for (int c = 0; c < p.C; ++c) wide = fmaf(__ldg(p.wide + p.coff[c]), load_cont(p.csrc[c], b * p.cstride[c], p.cdtype[c]), wide);
+      for (int c = 0; c < p.C; ++c) wide = fmaf(__ldg(p.wide + p.coff[c]), load_as_f32(p.csrc[c], b * p.cstride[c], p.cdtype[c]), wide);
       float z = 0.5f * (pair - sq) + wide + (p.wide_bias ? p.wide_bias[0] : 0.0f);
       if (p.addend) z += p.addend[b * p.addend_stride];
       if (p.out_w) z = apply_act(fmaf(z, p.out_w[0], p.out_b ? p.out_b[0] : 0.0f), p.out_act);
@@ -149,9 +128,8 @@ int mm_deepfm_head(const mm_lookup_table* tables_host, const int64_t* wide_offse
   memset(&p, 0, sizeof(p));
   for (int i = 0; i < n_tables; ++i) {
     const mm_lookup_table& t = tables_host[i];
-    MM_REQUIRE(t.weights && t.indices && t.rows > 0 && wide_offsets_host[i] >= 0, MM_ERR_ARG, "mm_deepfm_head: table %d: null pointer / no rows", i);
-    MM_REQUIRE(t.idx_bytes == 1 || t.idx_bytes == 2 || t.idx_bytes == 3 || t.idx_bytes == 4 || t.idx_bytes == 8, MM_ERR_ARG,
-               "mm_deepfm_head: table %d: idx_bytes %d", i, t.idx_bytes);
+    MM_REQUIRE(t.weights && wide_offsets_host[i] >= 0, MM_ERR_ARG, "mm_deepfm_head: table %d: null weights or negative wide offset", i);
+    if (const int rc = mm::check_id_column("mm_deepfm_head", i, t.indices, t.idx_bytes, t.rows)) return rc;
     MM_REQUIRE(!t.peer_weights_host, MM_ERR_UNSUPPORTED, "mm_deepfm_head: row-sharded tables are not supported");
     p.w[i] = t.weights;
     p.ids[i] = t.indices;

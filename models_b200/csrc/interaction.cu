@@ -242,34 +242,7 @@ int mm_dlrm_lookup_interact(const mm_lookup_table* tables_host, int n_tables, in
   lk.log2_world = -1;
   for (int b = 0; b < 4; ++b)
     if ((1 << b) == world) lk.log2_world = b;
-  unsigned seen = bottom ? (1u << bottom_slot) : 0u;
-  for (int t = 0; t < n_tables; ++t) {
-    const mm_lookup_table& tb = tables_host[t];
-    const int r = tb.slot;
-    MM_REQUIRE(tb.weights && tb.indices && tb.rows > 0 && r >= 0 && r < F && ((uintptr_t)tb.weights % 16) == 0, MM_ERR_ARG,
-               "%s: table %d: null pointer, rows <= 0, bad slot or misaligned weights", who, t);
-    MM_REQUIRE(!(seen & (1u << r)), MM_ERR_ARG, "%s: slot %d used twice", who, r);
-    seen |= 1u << r;
-    const int w = tb.idx_bytes;
-    MM_REQUIRE(w == 1 || w == 2 || w == 3 || w == 4 || w == 8, MM_ERR_ARG, "%s: table %d: idx_bytes must be 1, 2, 3, 4 or 8", who, t);
-    MM_REQUIRE(w >= 4 || tb.rows <= (1ll << (8 * w)), MM_ERR_ARG, "%s: table %d: %lld rows do not fit %d-byte ids", who, t,
-               (long long)tb.rows, w);
-    MM_REQUIRE((w != 4 && w != 8) || ((uintptr_t)tb.indices % w) == 0, MM_ERR_ALIGN, "%s: table %d: misaligned ids", who, t);
-    lk.weights[r] = tb.weights;
-    lk.indices[r] = tb.indices;
-    lk.rows[r] = tb.rows;
-    lk.idx_bytes[r] = (unsigned char)w;
-    if (tb.peer_weights_host) {
-      MM_REQUIRE(world > 1, MM_ERR_ARG, "%s: table %d is sharded but world == 1", who, t);
-      lk.sharded[r] = 1;
-      for (int k = 0; k < world; ++k) {
-        MM_REQUIRE(tb.peer_weights_host[k] && ((uintptr_t)tb.peer_weights_host[k] % 16) == 0, MM_ERR_ARG,
-                   "%s: table %d: null / misaligned shard pointer of rank %d", who, t, k);
-        lk.peers[r * world + k] = tb.peer_weights_host[k];
-      }
-      MM_REQUIRE(tb.peer_weights_host[rank] == tb.weights, MM_ERR_ARG, "%s: table %d: peer_weights_host[rank] != weights", who, t);
-    }
-  }
+  if (const int rc = mm::fill_lookup_params(who, tables_host, n_tables, F, bottom ? bottom_slot : -1, rank, true, lk)) return rc;
   const int P = bottom ? D : 0;
   MM_REQUIRE(!out || out_stride >= P + F * (F - 1) / 2, MM_ERR_ARG, "%s: out_stride too small", who);
   MM_REQUIRE(!out_split || (out_Kp % 64 == 0 && out_Kp >= P + F * (F - 1) / 2 && ((uintptr_t)out_split % 16) == 0), MM_ERR_ARG,

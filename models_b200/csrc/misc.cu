@@ -17,15 +17,6 @@ struct ConcatParams {
   int total_width;
 };
 
-__device__ __forceinline__ float load_as_f32(const void* src, long long i, int dtype) {
-  switch (dtype) {
-    case MM_I32: return (float)reinterpret_cast<const int32_t*>(src)[i];
-    case MM_I64: return (float)reinterpret_cast<const long long*>(src)[i];
-    case MM_F64: return (float)reinterpret_cast<const double*>(src)[i];
-    default: return reinterpret_cast<const float*>(src)[i];
-  }
-}
-
 // One thread per (row, piece-column); consecutive threads walk the pieces of one row, so the
 // writes of a row are contiguous and the reads of width-1 pieces are coalesced across rows in
 // the transposed launch below.

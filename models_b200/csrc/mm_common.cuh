@@ -90,9 +90,45 @@ struct LookupParams {
   int world, log2_world;  // log2_world = -1: world is not a power of two
 };
 
+// Host checks of C-ABI input (cabi.cu).  Each returns MM_OK, or sets the error text (prefixed by `who`) and returns its code.
+// One packed id column of table t: non-null, idx_bytes in {1, 2, 3, 4, 8}, rows > 0 and all addressable by a narrow
+// width, 4- and 8-byte ids aligned to their width.
+int check_id_column(const char* who, int t, const void* indices, int idx_bytes, long long rows);
+// An mm_lookup_table array -> `lk` by staged row (= slot), on top of the caller's zeroed lk.world / lk.log2_world:
+// slots in [0, F) and used once (with `bottom_slot`, -1: none), 16-byte aligned weights, check_id_column, and shard
+// pointers for row-sharded tables (lk.world > 1 and sharded_ok; otherwise such a table is refused).
+int fill_lookup_params(const char* who, const mm_lookup_table* tables, int n_tables, int F, int bottom_slot, int rank,
+                       bool sharded_ok, LookupParams& lk);
+
 template <typename T>
 __device__ __forceinline__ long long load_index(const void* p, long long i) {
   return (long long)reinterpret_cast<const T*>(p)[i];
+}
+
+// Id s of a packed id column (mm_lookup_table.idx_bytes): 1, 2, 3 (unsigned, little-endian), 4 or 8 (signed) bytes.
+__device__ __forceinline__ long long load_id(const void* base, int w, long long s) {
+  switch (w) {
+    case 1: return (long long)reinterpret_cast<const uint8_t*>(base)[s];
+    case 2: return (long long)reinterpret_cast<const uint16_t*>(base)[s];
+    case 3: {
+      const uint8_t* b = reinterpret_cast<const uint8_t*>(base) + 3 * s;
+      return (long long)b[0] | ((long long)b[1] << 8) | ((long long)b[2] << 16);
+    }
+    case 8: return reinterpret_cast<const long long*>(base)[s];
+    default: return (long long)reinterpret_cast<const int32_t*>(base)[s];
+  }
+}
+
+// Element i of an input column (mm_concat_piece.dtype, BCE targets) as fp32.  NC_F32: fp32 columns are read through the
+// read-only data cache (__ldg).
+template <bool NC_F32 = false>
+__device__ __forceinline__ float load_as_f32(const void* src, long long i, int dtype) {
+  switch (dtype) {
+    case MM_I32: return (float)reinterpret_cast<const int32_t*>(src)[i];
+    case MM_I64: return (float)reinterpret_cast<const long long*>(src)[i];
+    case MM_F64: return (float)reinterpret_cast<const double*>(src)[i];
+    default: return NC_F32 ? __ldg(reinterpret_cast<const float*>(src) + i) : reinterpret_cast<const float*>(src)[i];
+  }
 }
 
 }  // namespace mm

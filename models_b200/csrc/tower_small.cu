@@ -47,15 +47,6 @@ struct Params {
   __nv_bfloat16* out_split;  // (B, 2*N2) [hi | lo]
 };
 
-__device__ __forceinline__ float load_col(const void* src, long long i, int dtype) {
-  switch (dtype) {
-    case MM_I32: return (float)reinterpret_cast<const int32_t*>(src)[i];
-    case MM_I64: return (float)reinterpret_cast<const long long*>(src)[i];
-    case MM_F64: return (float)reinterpret_cast<const double*>(src)[i];
-    default: return __ldg(reinterpret_cast<const float*>(src) + i);
-  }
-}
-
 constexpr int W1_STRIDE = 80;  // bytes per n-row of W1 in shared memory: [hi k0..15 | lo k0..15] = 64 B + 16 B pad
 
 // N1T / N2T: number of 8-column n-tiles of layer 1 / layer 2 (N1 = 8*N1T is also the K of layer 2, a multiple of 16)
@@ -115,14 +106,6 @@ tower_small_kernel(const __grid_constant__ Cols cols, const Params p) {
                  : nullptr;
     cdts |= (uint32_t)dt << (8 * j);
   }
-  auto load_at = [&](const uint8_t* ptr, int dt) -> float {
-    switch (dt) {
-      case MM_I32: return (float)*reinterpret_cast<const int32_t*>(ptr);
-      case MM_I64: return (float)*reinterpret_cast<const long long*>(ptr);
-      case MM_F64: return (float)*reinterpret_cast<const double*>(ptr);
-      default: return __ldg(reinterpret_cast<const float*>(ptr));
-    }
-  };
   for (long long tile = tile0; tile < tiles; tile += tstep) {
     const long long r0 = tile * 16 + g, r1 = r0 + 8;
     const bool v0 = r0 < p.B, v1 = r1 < p.B;
@@ -131,8 +114,8 @@ tower_small_kernel(const __grid_constant__ Cols cols, const Params p) {
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const int dt = (int)((cdts >> (8 * j)) & 0xff);
-      x[0][j] = (cptr[j] && v0) ? load_at(cptr[j], dt) : 0.0f;
-      x[1][j] = (cptr[j] && v1) ? load_at(cptr[j] + 8 * (long long)cstep[j], dt) : 0.0f;
+      x[0][j] = (cptr[j] && v0) ? load_as_f32<true>(cptr[j], 0, dt) : 0.0f;
+      x[1][j] = (cptr[j] && v1) ? load_as_f32<true>(cptr[j] + 8 * (long long)cstep[j], 0, dt) : 0.0f;
       if (cptr[j]) cptr[j] += tstep * 16 * (long long)cstep[j];
     }
     uint32_t ah[4], al[4];

@@ -48,15 +48,6 @@ struct HeadParams {
   float* db;  // scalar accumulated
 };
 
-__device__ __forceinline__ float load_target(const void* y, long long i, int dt) {
-  switch (dt) {
-    case MM_I32: return (float)reinterpret_cast<const int32_t*>(y)[i];
-    case MM_I64: return (float)reinterpret_cast<const long long*>(y)[i];
-    case MM_F64: return (float)reinterpret_cast<const double*>(y)[i];
-    default: return reinterpret_cast<const float*>(y)[i];
-  }
-}
-
 constexpr int HEAD_KMAX = 256;  // 8 columns per lane
 
 __global__ void __launch_bounds__(256) head_kernel(const HeadParams p) {
@@ -83,7 +74,7 @@ __global__ void __launch_bounds__(256) head_kernel(const HeadParams p) {
       dot = fmaf(x[c], w[c], dot);
     }
     const float z = warp_sum(dot) + b;
-    const float y = load_target(p.y, m, p.y_dtype);
+    const float y = load_as_f32(p.y, m, p.y_dtype);
     const float sw = p.sample_w ? p.sample_w[m] : 1.0f;
     const float e = expf(-fabsf(z));
     const float l = fmaxf(z, 0.0f) - z * y + log1pf(e);
@@ -153,7 +144,7 @@ __global__ void __launch_bounds__(256) head_kernel_v4(const HeadParams p) {
     const float z = dot + b;
     float dz = 0.0f;
     if (live) {
-      const float y = load_target(p.y, m, p.y_dtype);
+      const float y = load_as_f32(p.y, m, p.y_dtype);
       const float sw = p.sample_w ? p.sample_w[m] : 1.0f;
       const float e = expf(-fabsf(z));
       const float sig = z >= 0.0f ? 1.0f / (1.0f + e) : e / (1.0f + e);

@@ -28,19 +28,6 @@ namespace trs {
 
 __device__ __align__(16) float g_zero_row[128];
 
-__device__ __forceinline__ long long load_id(const void* base, int w, long long s) {
-  switch (w) {
-    case 1: return (long long)reinterpret_cast<const uint8_t*>(base)[s];
-    case 2: return (long long)reinterpret_cast<const uint16_t*>(base)[s];
-    case 3: {
-      const uint8_t* b = reinterpret_cast<const uint8_t*>(base) + 3 * s;
-      return (long long)b[0] | ((long long)b[1] << 8) | ((long long)b[2] << 16);
-    }
-    case 8: return reinterpret_cast<const long long*>(base)[s];
-    default: return (long long)reinterpret_cast<const int32_t*>(base)[s];
-  }
-}
-
 struct IbwdParams {
   long long B;
   int F, P, bottom_slot;
@@ -853,24 +840,12 @@ int mm_dlrm_interact_backward(const mm_lookup_table* tables_host, int n_tables, 
   lk.world = 1;
   IbwdParams p;
   memset(&p, 0, sizeof(p));
-  bool used[MM_LOOKUP_MAX_ROWS] = {};
-  if (bottom) used[bottom_slot] = true;
+  if (const int rc = fill_lookup_params("mm_dlrm_interact_backward", tables_host, n_tables, F, bottom ? bottom_slot : -1, 0, false, lk))
+    return rc;
   for (int i = 0; i < n_tables; ++i) {
-    const mm_lookup_table& tb = tables_host[i];
-    MM_REQUIRE(tb.weights && tb.indices && tb.rows > 0, MM_ERR_ARG, "mm_dlrm_interact_backward: table %d: null pointer or no rows", i);
-    MM_REQUIRE(tb.slot >= 0 && tb.slot < F && !used[tb.slot], MM_ERR_ARG, "mm_dlrm_interact_backward: table %d: bad or repeated slot %d", i, tb.slot);
-    MM_REQUIRE(tb.idx_bytes == 1 || tb.idx_bytes == 2 || tb.idx_bytes == 3 || tb.idx_bytes == 4 || tb.idx_bytes == 8, MM_ERR_ARG,
-               "mm_dlrm_interact_backward: table %d: idx_bytes %d", i, tb.idx_bytes);
-    MM_REQUIRE(!tb.peer_weights_host, MM_ERR_UNSUPPORTED, "mm_dlrm_interact_backward: row-sharded tables are not supported");
-    MM_REQUIRE(((uintptr_t)tb.weights & 15) == 0, MM_ERR_ALIGN, "mm_dlrm_interact_backward: table %d: weights must be 16-byte aligned", i);
-    used[tb.slot] = true;
-    lk.weights[tb.slot] = tb.weights;
-    lk.indices[tb.slot] = tb.indices;
-    lk.rows[tb.slot] = tb.rows;
-    lk.idx_bytes[tb.slot] = (unsigned char)tb.idx_bytes;
     float* gr = grad_rows_host[i];
     MM_REQUIRE(!gr || ((uintptr_t)gr & 7) == 0, MM_ERR_ALIGN, "mm_dlrm_interact_backward: grad_rows[%d] must be 8-byte aligned", i);
-    p.grad[tb.slot] = gr;
+    p.grad[tables_host[i].slot] = gr;
   }
   p.B = B;
   p.F = F;
@@ -919,6 +894,7 @@ int mm_sparse_rows_apply(const mm_sparse_table* tables_host, int n_tables, int64
     MM_REQUIRE(opt != MM_OPT_ADAM || s.state2, MM_ERR_ARG, "mm_sparse_rows_apply: table %d: second optimizer state missing", i);
     MM_REQUIRE((((uintptr_t)s.weights | (uintptr_t)s.grad_rows | (uintptr_t)s.state1 | (uintptr_t)s.state2 | (uintptr_t)s.dense_grad) & 15) == 0,
                MM_ERR_ALIGN, "mm_sparse_rows_apply: table %d: 16-byte alignment", i);
+    if (const int rc = check_id_column("mm_sparse_rows_apply", i, s.indices, s.idx_bytes, s.rows)) return rc;
     SparseTable t;
     t.w = s.weights;
     t.rows = s.rows;

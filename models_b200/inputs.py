@@ -171,12 +171,12 @@ class EmbeddingTable(Block):
         kind = self.lookup_kind(feat)
         if kind == "bag":  # ragged + combiner -> safe_embedding_lookup_sparse (:432-441)
             values, offsets = feat
-            ops.gather_bag(self.table, _as_index(values).reshape(-1), _as_index(offsets), self.sequence_combiner or "mean",
+            ops.gather_bag(self.table, ops.as_index(values).reshape(-1), ops.as_index(offsets), self.sequence_combiner or "mean",
                            out, out_col, oob)
         elif kind == "onehot":
-            ops.gather_multi([self.table], [_as_index(feat).reshape(-1)], [out_col], out, oob)
+            ops.gather_multi([self.table], [ops.as_index(feat).reshape(-1)], [out_col], out, oob)
         else:  # dense (B, L): gather then combiner over axis 1, padding not masked (:457-461)
-            ids = _as_index(feat).reshape(feat.shape[0], -1).contiguous()
+            ids = ops.as_index(feat).reshape(feat.shape[0], -1).contiguous()
             comb = self.sequence_combiner or "mean"
             if comb == "sqrtn":
                 raise ValueError("sequence_combiner 'sqrtn' is only defined for ragged inputs")
@@ -200,14 +200,6 @@ class EmbeddingTable(Block):
         self.lookup_into(feat, out, 0, oob)
         _raise_on_oob(oob, self.table_name)
         return out
-
-
-def _as_index(t: torch.Tensor) -> torch.Tensor:
-    if t.dtype in (torch.int32, torch.int64):
-        return t
-    if t.dtype in (torch.uint8, torch.uint16):  # packed host-batch ids (graph.HostBatch id_bytes)
-        return ops.widen_index(t)
-    return t.to(torch.int32)  # reference casts non-int ids to int32 (inputs/embedding.py:1127-1129)
 
 
 def _raise_on_oob(oob: torch.Tensor, what: str) -> None:
@@ -279,7 +271,7 @@ class EmbeddingsBlock(Block):
             feat = get_feature(inputs, fname)
             if table.lookup_kind(feat) == "onehot":
                 one_w.append(table.table)
-                one_i.append(_as_index(feat).reshape(-1))
+                one_i.append(ops.as_index(feat).reshape(-1))
                 one_c.append(out_cols[fname])
             else:
                 table.lookup_into(feat, out, out_cols[fname], oob)

@@ -230,6 +230,39 @@ def widen_index(t: torch.Tensor) -> torch.Tensor:
     return t.reshape(-1).to(torch.int32)
 
 
+def as_index(t: torch.Tensor) -> torch.Tensor:
+    """Ids as int32 / int64, the two index dtypes of the gather kernels: the forms of index_bytes_of are widened
+    (widen_index), any other dtype is cast to int32 as the reference does (inputs/embedding.py:1127-1129)."""
+    try:
+        return widen_index(t)
+    except TypeError:
+        return t.to(torch.int32)
+
+
+def fused_ids(t: torch.Tensor) -> torch.Tensor:
+    """Ids as the fused lookup kernels take them (dlrm_lookup_interact, dlrm_interact_backward, deepfm_head,
+    sparse_rows_apply): packed host-batch ids (uint8, uint16, uint8 (B, 3)) at their own width, others as (B,) as_index."""
+    return t if t.dtype in (torch.uint8, torch.uint16) else as_index(t).reshape(-1)
+
+
+def _lookup_tables(weights, indices, B: int, wdt: torch.dtype, wcols: int, slots=None, rows=None):
+    """mm_lookup_table array: table t is weights[t], a contiguous (rows, wcols) wdt matrix, read at the B ids indices[t]
+    (any width of index_bytes_of), staged at slots[t] (default t), with rows[t] rows (default weights[t].shape[0])."""
+    arr = (_cabi.LookupTable * len(weights))()
+    for t in range(len(weights)):
+        w = _dev(weights[t], f"weights[{t}]", wdt)
+        ix = _dev(indices[t], f"indices[{t}]")
+        if w.dim() != 2 or w.shape[1] != wcols or not w.is_contiguous():
+            raise ValueError(f"weights[{t}] must be a contiguous (rows, {wcols}) {wdt} matrix")
+        wb = index_bytes_of(ix)
+        if ix.numel() != B * (3 if wb == 3 else 1) or not ix.is_contiguous():
+            raise ValueError(f"indices[{t}] must be contiguous with {B} ids, got {tuple(ix.shape)}")
+        arr[t].weights, arr[t].indices, arr[t].idx_bytes = w.data_ptr(), ix.data_ptr(), wb
+        arr[t].rows = w.shape[0] if rows is None else int(rows[t])
+        arr[t].slot = t if slots is None else int(slots[t])
+    return arr
+
+
 def dlrm_lookup_interact(weights, indices, slots, rows, D: int, bottom: Optional[torch.Tensor], bottom_slot: int,
                          out: torch.Tensor, oob: Optional[torch.Tensor] = None, peers=None, rank: int = 0,
                          world: int = 1, operand_rows: bool = False) -> torch.Tensor:
@@ -244,24 +277,12 @@ def dlrm_lookup_interact(weights, indices, slots, rows, D: int, bottom: Optional
     n = len(weights)
     if not (len(indices) == n and len(slots) == n and len(rows) == n):
         raise ValueError("weights / indices / slots / rows length mismatch")
-    arr = (_cabi.LookupTable * n)()
     keep = []
     wdt, wcols = (torch.bfloat16, 2 * D) if operand_rows else (torch.float32, D)
     if operand_rows and bottom is not None and (bottom.dtype != torch.bfloat16 or bottom.shape[1] != 2 * D):
         raise ValueError(f"operand_rows: bottom must be bf16 split rows (B, {2 * D})")
+    arr = _lookup_tables(weights, indices, B, wdt, wcols, slots, rows)
     for t in range(n):
-        w = _dev(weights[t], f"weights[{t}]", wdt)
-        ix = _dev(indices[t], f"indices[{t}]")
-        if w.dim() != 2 or w.shape[1] != wcols or not w.is_contiguous():
-            raise ValueError(f"weights[{t}] must be a contiguous (rows, {wcols}) {wdt} matrix")
-        wb = index_bytes_of(ix)
-        if ix.numel() != B * (3 if wb == 3 else 1) or not ix.is_contiguous():
-            raise ValueError(f"indices[{t}] must be contiguous with {B} ids, got {tuple(ix.shape)}")
-        arr[t].weights = w.data_ptr()
-        arr[t].indices = ix.data_ptr()
-        arr[t].rows = int(rows[t])
-        arr[t].slot = int(slots[t])
-        arr[t].idx_bytes = wb
         pt = None if peers is None else peers[t]
         if pt is not None:
             if len(pt) != world:
@@ -307,6 +328,18 @@ def rowwise_dot(q: torch.Tensor, items: torch.Tensor, out: torch.Tensor) -> torc
     return out
 
 
+def _item_ids(pos_ids, neg_ids, downscore: bool):
+    """(pos_ids, neg_ids, id dtype code) for the false-negative mask of the in-batch kernels: with downscore, both as
+    contiguous (B,) / (N,) vectors of the negative ids' dtype (utils/tf_utils.py:136 casts the positive ids to it)."""
+    if not downscore:
+        return pos_ids, neg_ids, MM_I64
+    if pos_ids is None or neg_ids is None:
+        raise ValueError("downscore_false_negatives requires positive and negative item ids")
+    neg_ids = neg_ids.reshape(-1).contiguous()
+    pos_ids = pos_ids.reshape(-1).to(neg_ids.dtype).contiguous()
+    return pos_ids, neg_ids, _idx_dtype(neg_ids, "neg_ids")
+
+
 def inbatch_scores(q, pos, neg, out, pos_ids=None, neg_ids=None, downscore=True,
                    false_neg_score: float = -655.04, pos_prob=None, neg_prob=None,
                    temperature: float = 1.0, tensor_cores: bool = True) -> torch.Tensor:
@@ -321,14 +354,7 @@ def inbatch_scores(q, pos, neg, out, pos_ids=None, neg_ids=None, downscore=True,
         raise ValueError("out must be (B, 1+N) with unit inner stride")
     B, D = q.shape
     N = neg.shape[0]
-    id_dt = MM_I64
-    if downscore:
-        if pos_ids is None or neg_ids is None:
-            raise ValueError("downscore_false_negatives requires positive and negative item ids")
-        neg_ids = neg_ids.reshape(-1).contiguous()
-        # reference: positive ids are cast to the negative ids' dtype (utils/tf_utils.py:136)
-        pos_ids = pos_ids.reshape(-1).to(neg_ids.dtype).contiguous()
-        id_dt = _idx_dtype(neg_ids, "neg_ids")
+    pos_ids, neg_ids, id_dt = _item_ids(pos_ids, neg_ids, downscore)
     if tensor_cores and N > 0 and B > 0:
         _cabi.check(_lib().mm_positive_scores(q.data_ptr(), pos.data_ptr(), B, D, _ptr(pos_prob), float(temperature),
                                               out.data_ptr(), out.stride(0), _stream()), "mm_positive_scores")
@@ -362,13 +388,7 @@ def inbatch_softmax_ce(q, pos, neg, pos_ids=None, neg_ids=None, downscore=True, 
     N = neg.shape[0]
     if N == 0 or B == 0:
         raise ValueError("in-batch softmax needs at least one query and one negative")
-    id_dt = MM_I64
-    if downscore:
-        if pos_ids is None or neg_ids is None:
-            raise ValueError("downscore_false_negatives requires positive and negative item ids")
-        neg_ids = neg_ids.reshape(-1).contiguous()
-        pos_ids = pos_ids.reshape(-1).to(neg_ids.dtype).contiguous()  # utils/tf_utils.py:136
-        id_dt = _idx_dtype(neg_ids, "neg_ids")
+    pos_ids, neg_ids, id_dt = _item_ids(pos_ids, neg_ids, downscore)
     dev = q.device
     pos_logit = torch.empty((B, 1), dtype=torch.float32, device=dev)
     _cabi.check(_lib().mm_positive_scores(q.data_ptr(), pos.data_ptr(), B, D, _ptr(pos_prob), float(temperature),
@@ -391,6 +411,31 @@ _CONCAT_DTYPES = {torch.int32: _cabi.MM_I32, torch.int64: _cabi.MM_I64, torch.fl
                   torch.float64: _cabi.MM_F64}
 
 
+def _concat_pieces(pieces: Sequence[torch.Tensor], B: int, name: str = "pieces", out_cols: Optional[Sequence[int]] = None,
+                   max_width: Optional[int] = None):
+    """(mm_concat_piece array, pieces in it, row width) of the (B,) / (B, w) input columns `pieces`, read as fp32 into
+    columns out_cols[i] (default: one after the other).  max_width: wider pieces are split into pieces of that width."""
+    flat, col = [], 0
+    for i, t in enumerate(pieces):
+        _dev(t, f"{name}[{i}]")
+        if t.dtype not in _CONCAT_DTYPES:
+            raise TypeError(f"{name}[{i}]: unsupported dtype {t.dtype}")
+        if t.dim() == 1:
+            t = t.unsqueeze(1)
+        if t.dim() != 2 or t.shape[0] != B or (t.shape[1] > 1 and t.stride(1) != 1):
+            raise ValueError(f"{name}[{i}] must be (B,) or (B,w) with unit inner stride, got {tuple(t.shape)}")
+        w = int(t.shape[1])
+        oc = col if out_cols is None else int(out_cols[i])
+        for c0 in range(0, w, max_width) if max_width else [0]:
+            flat.append((t.data_ptr() + c0 * t.element_size(), t.stride(0), min(max_width, w - c0) if max_width else w,
+                         _CONCAT_DTYPES[t.dtype], oc + c0))
+        col = oc + w
+    arr = (_cabi.ConcatPiece * max(len(flat), 1))()
+    for i, (ptr, sstride, w, dt, oc) in enumerate(flat):
+        arr[i].src, arr[i].src_stride, arr[i].width, arr[i].dtype, arr[i].out_col = ptr, sstride, w, dt, oc
+    return arr, len(flat), col
+
+
 def concat_columns(pieces: Sequence[torch.Tensor], out: torch.Tensor, out_cols: Optional[Sequence[int]] = None,
                    max_width: int = 256) -> torch.Tensor:
     """out[:, out_cols[i] : out_cols[i]+w_i] = float32(pieces[i])  — (B,) pieces count as (B,1).
@@ -399,36 +444,20 @@ def concat_columns(pieces: Sequence[torch.Tensor], out: torch.Tensor, out_cols: 
     _dev(out, "out", torch.float32)
     B = out.shape[0]
     stride = _row_stride(out, "out")
-    flat = []
-    col = 0
-    for i, t in enumerate(pieces):
-        _dev(t, f"pieces[{i}]")
-        if t.dtype not in _CONCAT_DTYPES:
-            raise TypeError(f"pieces[{i}]: unsupported dtype {t.dtype}")
-        if t.dim() == 1:
-            t = t.unsqueeze(1)
-        if t.dim() != 2 or t.shape[0] != B or (t.shape[1] > 1 and t.stride(1) != 1):
-            raise ValueError(f"pieces[{i}] must be (B,) or (B,w) with unit inner stride, got {tuple(t.shape)}")
-        w = t.shape[1]
-        oc = col if out_cols is None else int(out_cols[i])
-        for c0 in range(0, w, max_width):  # split very wide pieces so a launch tile fits in smem
-            flat.append((t.data_ptr() + c0 * t.element_size(), t.stride(0), min(max_width, w - c0),
-                         _CONCAT_DTYPES[t.dtype], oc + c0))
-        col = oc + w
+    # very wide pieces are split so that a launch tile fits in shared memory
+    arr, n, _ = _concat_pieces(pieces, B, out_cols=out_cols, max_width=max_width)
     groups, cur, cur_w = [], [], 0
-    for f in flat:
-        if cur and (cur_w + f[2] > max_width or len(cur) == 64):
+    for f in arr[:n]:
+        if cur and (cur_w + f.width > max_width or len(cur) == 64):
             groups.append(cur)
             cur, cur_w = [], 0
         cur.append(f)
-        cur_w += f[2]
+        cur_w += f.width
     if cur:
         groups.append(cur)
     for g in groups:
-        arr = (_cabi.ConcatPiece * len(g))()
-        for i, (ptr, sstride, w, dt, oc) in enumerate(g):
-            arr[i].src, arr[i].src_stride, arr[i].width, arr[i].dtype, arr[i].out_col = ptr, sstride, w, dt, oc
-        _cabi.check(_lib().mm_concat_columns(arr, len(g), B, out.data_ptr(), stride, _stream()), "mm_concat_columns")
+        ga = (_cabi.ConcatPiece * len(g))(*g)
+        _cabi.check(_lib().mm_concat_columns(ga, len(g), B, out.data_ptr(), stride, _stream()), "mm_concat_columns")
     return out
 
 
@@ -441,28 +470,15 @@ def concat_split_supported(pieces: Sequence[torch.Tensor]) -> bool:
 def concat_split(pieces: Sequence[torch.Tensor], out: Optional[torch.Tensor] = None):
     """ConcatFeatures + bf16 split in one launch (mm_concat_split): returns (a_split (B, 2*Kp) bf16, K).
     Pieces in the reference's sorted-name order; (B,) pieces count as (B,1)."""
-    flat, col = [], 0
     B = pieces[0].shape[0]
-    for i, t in enumerate(pieces):
-        _dev(t, f"pieces[{i}]")
-        if t.dtype not in _CONCAT_DTYPES:
-            raise TypeError(f"pieces[{i}]: unsupported dtype {t.dtype}")
-        if t.dim() == 1:
-            t = t.unsqueeze(1)
-        if t.dim() != 2 or t.shape[0] != B or (t.shape[1] > 1 and t.stride(1) != 1):
-            raise ValueError(f"pieces[{i}] must be (B,) or (B,w) with unit inner stride, got {tuple(t.shape)}")
-        flat.append((t.data_ptr(), t.stride(0), int(t.shape[1]), _CONCAT_DTYPES[t.dtype], col))
-        col += int(t.shape[1])
-    K, Kp = col, tc_padded_k(col)
+    arr, n, K = _concat_pieces(pieces, B)
+    Kp = tc_padded_k(K)
     if out is None:
         out = torch.empty((B, 2 * Kp), dtype=torch.bfloat16, device=pieces[0].device)
     _dev(out, "out", torch.bfloat16)
     if tuple(out.shape) != (B, 2 * Kp) or not out.is_contiguous():
         raise ValueError(f"out must be a contiguous ({B}, {2 * Kp}) bf16 matrix")
-    arr = (_cabi.ConcatPiece * len(flat))()
-    for i, (ptr, sstride, w, dt, oc) in enumerate(flat):
-        arr[i].src, arr[i].src_stride, arr[i].width, arr[i].dtype, arr[i].out_col = ptr, sstride, w, dt, oc
-    _cabi.check(_lib().mm_concat_split(arr, len(flat), B, out.data_ptr(), Kp, _stream()), "mm_concat_split")
+    _cabi.check(_lib().mm_concat_split(arr, n, B, out.data_ptr(), Kp, _stream()), "mm_concat_split")
     return out, K
 
 
@@ -478,16 +494,8 @@ def tower2_small(pieces: Sequence[torch.Tensor], w1_split: torch.Tensor, N1: int
                  bias2, act2, out: Optional[torch.Tensor] = None, out_split: Optional[torch.Tensor] = None):
     """act2(act1(concat(pieces) W1 + b1) W2 + b2) in one launch (mm_tower2_small).  out: (B, N2) fp32 and / or
     out_split: (B, 2*N2) bf16 [hi | lo]."""
-    flat, col = [], 0
     B = pieces[0].shape[0]
-    for i, t in enumerate(pieces):
-        _dev(t, f"pieces[{i}]")
-        if t.dim() == 1:
-            t = t.unsqueeze(1)
-        if t.dim() != 2 or t.shape[0] != B or (t.shape[1] > 1 and t.stride(1) != 1):
-            raise ValueError(f"pieces[{i}] must be (B,) or (B,w) with unit inner stride, got {tuple(t.shape)}")
-        flat.append((t.data_ptr(), t.stride(0), int(t.shape[1]), _CONCAT_DTYPES[t.dtype], col))
-        col += int(t.shape[1])
+    arr, n, col = _concat_pieces(pieces, B)
     _dev(w1_split, "w1_split", torch.bfloat16), _dev(w2_split, "w2_split", torch.bfloat16)
     if tuple(w1_split.shape) != (tc_padded_n(N1), 2 * tc_padded_k(col)) or tuple(w2_split.shape) != (tc_padded_n(N2), 2 * tc_padded_k(N1)):
         raise ValueError("w1_split / w2_split must be the mm_split_weights layouts of the (K, N1) and (N1, N2) kernels")
@@ -499,11 +507,8 @@ def tower2_small(pieces: Sequence[torch.Tensor], w1_split: torch.Tensor, N1: int
         _dev(out_split, "out_split", torch.bfloat16)
         if tuple(out_split.shape) != (B, 2 * N2) or not out_split.is_contiguous():
             raise ValueError(f"out_split must be a contiguous ({B}, {2 * N2}) bf16 matrix")
-    arr = (_cabi.ConcatPiece * len(flat))()
-    for i, (ptr, sstride, w, dt, oc) in enumerate(flat):
-        arr[i].src, arr[i].src_stride, arr[i].width, arr[i].dtype, arr[i].out_col = ptr, sstride, w, dt, oc
     _cabi.check(
-        _lib().mm_tower2_small(arr, len(flat), B, w1_split.data_ptr(), N1, _ptr(bias1), ACTIVATIONS[act1], w2_split.data_ptr(), N2,
+        _lib().mm_tower2_small(arr, n, B, w1_split.data_ptr(), N1, _ptr(bias1), ACTIVATIONS[act1], w2_split.data_ptr(), N2,
                                _ptr(bias2), ACTIVATIONS[act2], _ptr(out), out.stride(0) if out is not None else 0, _ptr(out_split),
                                _stream()), "mm_tower2_small")
     return out if out is not None else out_split
@@ -847,19 +852,11 @@ def dlrm_interact_backward(weights, indices, slots, rows, D: int, bottom: Option
     n = len(weights)
     if not (len(indices) == n and len(slots) == n and len(rows) == n and len(grad_rows) == n):
         raise ValueError("weights / indices / slots / rows / grad_rows length mismatch")
-    arr = (_cabi.LookupTable * n)()
     gp = (C.c_void_p * n)()
     gstride = None
     wdt, wcols = (torch.bfloat16, 2 * D) if operand_rows else (torch.float32, D)
+    arr = _lookup_tables(weights, indices, B, wdt, wcols, slots, rows)
     for t in range(n):
-        w = _dev(weights[t], f"weights[{t}]", wdt)
-        ix = _dev(indices[t], f"indices[{t}]")
-        if w.dim() != 2 or w.shape[1] != wcols or not w.is_contiguous():
-            raise ValueError(f"weights[{t}] must be a contiguous (rows, {wcols}) {wdt} matrix")
-        wb = index_bytes_of(ix)
-        if ix.numel() != B * (3 if wb == 3 else 1) or not ix.is_contiguous():
-            raise ValueError(f"indices[{t}] must be contiguous with {B} ids")
-        arr[t].weights, arr[t].indices, arr[t].rows, arr[t].slot, arr[t].idx_bytes = w.data_ptr(), ix.data_ptr(), int(rows[t]), int(slots[t]), wb
         g = grad_rows[t]
         if g is not None:
             _dev(g, f"grad_rows[{t}]", torch.float32)
@@ -964,27 +961,15 @@ def deepfm_head(weights, indices, wide_offsets, cont, cont_offsets, wide_kernel:
     if not (len(indices) == n and len(wide_offsets) == n):
         raise ValueError("weights / indices / wide_offsets length mismatch")
     D = weights[0].shape[1]
-    arr = (_cabi.LookupTable * n)()
-    for t in range(n):
-        w = _dev(weights[t], f"weights[{t}]", torch.float32)
-        ix = _dev(indices[t], f"indices[{t}]")
-        if w.dim() != 2 or w.shape[1] != D or not w.is_contiguous():
-            raise ValueError(f"weights[{t}] must be a contiguous (rows, {D}) float32 matrix")
-        wb = index_bytes_of(ix)
-        if ix.numel() != B * (3 if wb == 3 else 1) or not ix.is_contiguous():
-            raise ValueError(f"indices[{t}] must be contiguous with {B} ids")
-        arr[t].weights, arr[t].indices, arr[t].rows, arr[t].slot, arr[t].idx_bytes = w.data_ptr(), ix.data_ptr(), w.shape[0], t, wb
+    arr = _lookup_tables(weights, indices, B, torch.float32, D)
     woff = (C.c_int64 * n)(*[int(o) for o in wide_offsets])
     m = len(cont)
     if len(cont_offsets) != m:
         raise ValueError("cont / cont_offsets length mismatch")
-    carr = (_cabi.ConcatPiece * max(m, 1))()
     for c, t in enumerate(cont):
-        _dev(t, f"cont[{c}]")
-        if t.dtype not in _CONCAT_DTYPES or t.numel() != B:
-            raise ValueError(f"cont[{c}] must hold {B} int32 / int64 / float32 / float64 values")
-        v = t.reshape(-1)
-        carr[c].src, carr[c].src_stride, carr[c].width, carr[c].dtype, carr[c].out_col = v.data_ptr(), v.stride(0), 1, _CONCAT_DTYPES[t.dtype], c
+        if _dev(t, f"cont[{c}]").numel() != B:
+            raise ValueError(f"cont[{c}] must hold {B} values")
+    carr, _, _ = _concat_pieces([t.reshape(-1) for t in cont], B, "cont")
     coff = (C.c_int64 * max(m, 1))(*[int(o) for o in cont_offsets])
     if addend is not None and (_dev(addend, "addend", torch.float32).numel() != B):
         raise ValueError(f"addend must hold {B} values")

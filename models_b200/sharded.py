@@ -37,7 +37,7 @@ import torch.distributed as dist
 
 from . import _cabi, ops
 from .core import create_variable
-from .inputs import EmbeddingsBlock, _as_index
+from .inputs import EmbeddingsBlock
 
 
 # ---- ownership maths (pure, also used by the tests) -------------------------------------------------
@@ -217,8 +217,7 @@ class ShardedEmbeddings:
         from .core import get_feature
 
         names = [self.embeddings.feature_to_table[f].table_name for f in self.feature_names]
-        idx = [get_feature(local_inputs, f) for f in self.feature_names]
-        idx = [i if i.dtype in (torch.uint8, torch.uint16) else _as_index(i).reshape(-1) for i in idx]
+        idx = [ops.fused_ids(get_feature(local_inputs, f)) for f in self.feature_names]
         if operand_rows and not self.mirrors:
             raise RuntimeError("operand-format rows requested but build_mirrors() has not run")
         tabs = self.mirrors if operand_rows else self.shards
@@ -232,8 +231,8 @@ class ShardedEmbeddings:
     # ---- step 1: replicate the indices ----------------------------------------------------------------
     def gather_indices(self, local_inputs: Dict[str, torch.Tensor]) -> torch.Tensor:
         """(T, B_local) local -> (T, world*B_local) global, rank-major sample order."""
-        idx = torch.stack([_as_index(local_inputs[f]).reshape(-1) for f in self.feature_names], dim=0).contiguous()
-        if len({_as_index(local_inputs[f]).dtype for f in self.feature_names}) > 1:
+        idx = torch.stack([ops.as_index(local_inputs[f]).reshape(-1) for f in self.feature_names], dim=0).contiguous()
+        if len({ops.as_index(local_inputs[f]).dtype for f in self.feature_names}) > 1:
             idx = idx.to(torch.int64)
         T, Bl = idx.shape
         out = torch.empty((self.world, T, Bl), dtype=idx.dtype, device=idx.device)
@@ -297,14 +296,14 @@ def lookup_stack_nccl(se: "ShardedEmbeddings", local_inputs: Dict[str, torch.Ten
     names = [(f, se.embeddings.feature_to_table[f].table_name) for f in se.feature_names]
     sharded = [(f, n) for f, n in names if se.is_sharded(n)]
     dev = next(iter(local_inputs.values())).device
-    Bl = _as_index(local_inputs[se.feature_names[0]]).reshape(-1).shape[0]
+    Bl = ops.as_index(local_inputs[se.feature_names[0]]).reshape(-1).shape[0]
     stack = torch.zeros((Bl, n_slots * D), dtype=torch.float32, device=dev)
     for f, n in names:
         if not se.is_sharded(n):
-            stack.view(Bl, n_slots, D)[:, slots[f]] = se.shards[n][_as_index(local_inputs[f]).reshape(-1).long()]
+            stack.view(Bl, n_slots, D)[:, slots[f]] = se.shards[n][ops.as_index(local_inputs[f]).reshape(-1).long()]
     if not sharded:
         return stack
-    ids = torch.stack([_as_index(local_inputs[f]).reshape(-1).long() for f, _ in sharded], dim=1).contiguous()  # (Bl, Ts)
+    ids = torch.stack([ops.as_index(local_inputs[f]).reshape(-1).long() for f, _ in sharded], dim=1).contiguous()  # (Bl, Ts)
     Ts = ids.shape[1]
     gids = torch.empty((W, Bl, Ts), dtype=torch.int64, device=dev)
     dist.all_gather_into_tensor(gids.view(-1), ids.view(-1), group=se.group)

@@ -287,13 +287,7 @@ class DLRMTrainer:
 
     # ---- one step on device tensors ------------------------------------------------------------------------------
     def _indices(self, inputs) -> List[torch.Tensor]:
-        from .inputs import _as_index
-
-        out = []
-        for f in self.feats:
-            i = get_feature(inputs, f)
-            out.append(i if i.dtype in (torch.uint8, torch.uint16) else _as_index(i).reshape(-1))
-        return out
+        return [ops.fused_ids(get_feature(inputs, f)) for f in self.feats]
 
     def forward_backward(self, inputs: Dict[str, torch.Tensor], targets: torch.Tensor, sample_weight=None) -> None:
         """Forward (activations saved), loss and backward: fills the gradient arena and the IndexedSlices.  Batches smaller

@@ -26,6 +26,8 @@ def test_library_exports_every_declared_symbol():
 def test_struct_layouts_match_header():
     assert ctypes.sizeof(_cabi.GatherTable) == 32
     assert ctypes.sizeof(_cabi.ConcatPiece) == 32
+    assert ctypes.sizeof(_cabi.LookupTable) == 40
+    assert ctypes.sizeof(_cabi.SparseTable) == 80
 
 
 def test_argument_errors_are_reported_without_a_gpu():
