@@ -164,16 +164,10 @@ int mm_dot_interaction(const float* x, int64_t B, int F, int D, int64_t x_stride
                        const float* prefix, int P, int64_t prefix_stride, int self_interaction,
                        float* out, int64_t out_stride, void* out_split, int out_Kp, void* stream);
 
-/* Fused K1+K5+K6+K3 for DLRM: gather T rows per sample straight into shared memory, append
- * the bottom-MLP vector at slot `bottom_slot`, write [bottom | interactions]; the (B,F,D)
- * stack never touches HBM.  tables[t].out_col is interpreted as slot(t)*D.  All dims == D. */
-int mm_dlrm_gather_interact(const mm_gather_table* tables_host, int n_tables, int idx_dtype,
-                            int64_t B, int D, const float* bottom, int64_t bottom_stride,
-                            int bottom_slot, float* out, int64_t out_stride, void* out_split,
-                            int out_Kp, int32_t* oob_count, void* stream);
-
-/* Second-generation fused lookup + interaction (same result as mm_dlrm_gather_interact), with a richer
- * table descriptor:
+/* Fused K1+K5+K6+K3 for DLRM: look up one row per table and sample straight into shared memory,
+ * place the bottom-MLP vector at slot `bottom_slot`, write [bottom | interactions] as mm_dot_interaction
+ * does (fp32 `out` or split-bf16 `out_split`); the (B,F,D) stack never touches HBM.  All rows are D wide.
+ * Table descriptor:
  *   - per-table id width: idx_bytes = 1, 2, 3 (unsigned little-endian — what a loader ships when the
  *     table has <= 2^8 / 2^16 / 2^24 rows), 4 (int32) or 8 (int64).  Narrow arrays need no alignment;
  *     the kernel reads the aligned 32-bit words that contain an id, so the array must be readable up
@@ -195,7 +189,10 @@ int mm_dlrm_gather_interact(const mm_gather_table* tables_host, int n_tables, in
  * address every row (rows > 2^(8 idx_bytes)) return MM_ERR_ARG; 4- and 8-byte id arrays not aligned to their width
  * return MM_ERR_ALIGN.  mm_dlrm_interact_backward, mm_deepfm_head and mm_sparse_rows_apply return these codes where
  * they used to launch with such a column; weights that are not 16-byte aligned now return MM_ERR_ALIGN from both
- * mm_dlrm_lookup_interact (formerly MM_ERR_ARG) and mm_dlrm_interact_backward. */
+ * mm_dlrm_lookup_interact (formerly MM_ERR_ARG) and mm_dlrm_interact_backward.
+ * The earlier fused entry point over mm_gather_table descriptors (int32 / int64 ids only) is removed.  Its callers pass the
+ * same tables here as mm_lookup_table with idx_bytes 4 or 8; for shapes outside this kernel they gather the (B,F,D) stack
+ * with mm_gather_multi and call mm_dot_interaction. */
 typedef struct {
   const float* weights;
   const void* indices; /* (B,) ids of this feature, idx_bytes each */

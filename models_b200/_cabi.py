@@ -100,7 +100,6 @@ SIGNATURES = {
     "mm_scale_shift": (_i, [_vp, _i64, _i, _i64, _vp, _vp, _vp, _i64, _vp]),
     "mm_cross_combine": (_i, [_vp, _vp, _vp, _i64, _i, _i64, _i64, _i64, _vp, _i64, _vp]),
     "mm_dot_interaction": (_i, [_vp, _i64, _i, _i, _i64, _vp, _i, _i64, _i, _vp, _i64, _vp, _i, _vp]),
-    "mm_dlrm_gather_interact": (_i, [_tables, _i, _i, _i64, _i, _vp, _i64, _i, _vp, _i64, _vp, _i, _vp, _vp]),
     "mm_dlrm_lookup_interact": (_i, [C.POINTER(LookupTable), _i, _i64, _i, _i, _i, _vp, _i64, _i, _vp, _i64, _vp, _i, _vp, _i, _vp]),
     "mm_dense_fp32": (_i, [_vp, _i64, _i, _i64, _vp, _vp, _i, _i, _vp, _i64, _vp, _i64, _vp]),
     "mm_tc_padded_k": (_i, [_i]),

@@ -724,8 +724,9 @@ class DLRM(Block):
               -> stack in sorted(name) order, "bottom_block" last for C*/I* style names
               -> pairwise dots (B, F(F-1)/2) -> [bottom | interactions] -> top MLP
     `fused=True` runs gather + stack + interaction + concat as ONE kernel (the (B,F,D) stack never
-    reaches HBM); `fused=False` keeps the reference's staging ((B,F,D) materialised once) for
-    block-level parity tests.
+    reaches HBM) when every feature is one-hot and the shape fits that kernel (can_emit_split);
+    `fused=False` keeps the reference's staging ((B,F,D) materialised once) for block-level parity
+    tests, and every other shape is staged the same way.
     """
 
     def __init__(self, embeddings: EmbeddingsBlock, continuous: Optional[ContinuousFeatures], bottom_block: Optional[MLP],
@@ -812,44 +813,33 @@ class DLRM(Block):
         emb = self.embeddings
         feats = emb.feature_names
         from .core import get_feature
-        from .inputs import _raise_on_oob
 
-        if self.sharded is not None:
+        all_onehot = self.sharded is None and all(emb.feature_to_table[f].lookup_kind(get_feature(inputs, f)) == "onehot"
+                                                  for f in feats)
+        if self.can_emit_split() and with_prefix == (bottom is not None) and (self.sharded is not None or (self.fused and all_onehot)):
             oob = emb.counter(dev)
-            if with_prefix == (bottom is not None) and self.can_emit_split():
+            if self.sharded is not None:
                 # row-sharded tables, product path: the lookup is part of the interaction kernel — rows owned
                 # by other ranks are read over NVLink straight into shared memory (no exchange, no barrier)
                 self.sharded.lookup_interact(inputs, slots, bottom, out, oob, operand_rows=operand_rows)
-                emb.finish_check(oob)
-                return out
-            # staged protocol (index all-gather + owner-computes NVLink push + barrier) rebuilds the (B,F,D)
-            # stack of the local samples; the interaction then reads it like the staged path
-            stack = self.sharded.lookup_stack(inputs, slots, F, oob)
-            emb.finish_check(oob)
-            if bottom is not None:
-                ops.concat_columns([bottom], stack, [slots["bottom_block"] * D])
-            return ops.dot_interaction(stack.view(B, F, D), out, prefix=bottom if with_prefix else None)
-        all_onehot = all(emb.feature_to_table[f].lookup_kind(get_feature(inputs, f)) == "onehot" for f in feats)
-        if self.fused and all_onehot and with_prefix == (bottom is not None):
-            oob = emb.counter(dev)
-            raw = [get_feature(inputs, f) for f in feats]
-            if self.can_emit_split():
+            else:
                 # ids travel at their own width (packed uint8 / uint16 / 24-bit host batches, int32, int64)
-                idx = [ops.fused_ids(i) for i in raw]
+                idx = [ops.fused_ids(get_feature(inputs, f)) for f in feats]
                 tabs = [emb.feature_to_table[f].operand_mirror() if operand_rows else emb.feature_to_table[f].table for f in feats]
                 ops.dlrm_lookup_interact(tabs, idx, [slots[f] for f in feats], [t.shape[0] for t in tabs], D, bottom,
                                          slots.get("bottom_block", -1), out, oob, operand_rows=operand_rows)
-            else:
-                idx = [ops.as_index(i).reshape(-1) for i in raw]
-                if len({i.dtype for i in idx}) > 1:
-                    idx = [i.to(torch.int64) for i in idx]
-                ops.dlrm_gather_interact([emb.feature_to_table[f].table for f in feats], idx, [slots[f] for f in feats], D,
-                                         bottom, slots.get("bottom_block", -1), out, oob)
             emb.finish_check(oob)
             return out
-        # staged path: one fused gather into the (B,F,D) stack, then the interaction kernel
-        stack = torch.empty((B, F * D), dtype=torch.float32, device=dev)
-        emb.lookup_all_into(inputs, stack, {f: slots[f] * D for f in feats})
+        # staged path: the (B,F,D) stack in HBM, then the interaction kernel
+        if self.sharded is not None:
+            # staged protocol (index all-gather + owner-computes NVLink push + barrier) rebuilds the stack of the
+            # local samples
+            oob = emb.counter(dev)
+            stack = self.sharded.lookup_stack(inputs, slots, F, oob)
+            emb.finish_check(oob)
+        else:
+            stack = torch.empty((B, F * D), dtype=torch.float32, device=dev)
+            emb.lookup_all_into(inputs, stack, {f: slots[f] * D for f in feats})  # one fused gather
         if bottom is not None:
             ops.concat_columns([bottom], stack, [slots["bottom_block"] * D])
         return ops.dot_interaction(stack.view(B, F, D), out, prefix=bottom if with_prefix else None)

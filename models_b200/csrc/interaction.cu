@@ -1,9 +1,12 @@
-// Pairwise dot-product interaction (DLRM), standalone and fused with the embedding gather.
+// Pairwise dot-product interaction (DLRM): the entry points mm_dot_interaction (from a (B,F,D) stack)
+// and mm_dlrm_lookup_interact (fused with the embedding lookup).  Both run the tensor-core kernel of
+// interaction_v2.cu; mm_dot_interaction falls back to interact_kernel below, exact fp32 on CUDA
+// cores, for the shapes that kernel does not take (F > 32, self interaction, other D or P).
 // Replaces tf.matmul(x, x^T) + band_part + boolean_mask (merlin/models/tf/blocks/interaction.py:
 // 86-116), StackFeatures (core/aggregation.py:101-108) and the [bottom | interactions] concat
-// (blocks/dlrm.py:126-130).  HBM-bound by design: every input row is read once (cp.async into
-// shared memory, no register staging), the (B,F,F) Gram matrix never exists, the output row is
-// assembled in shared memory and written with coalesced 128-bit stores.
+// (blocks/dlrm.py:126-130).  interact_kernel is HBM-bound by design: every input row is read once
+// (cp.async into shared memory, no register staging), the (B,F,F) Gram matrix never exists, the
+// output row is assembled in shared memory and written with coalesced 128-bit stores.
 #include <cstring>
 
 #include "mm_common.cuh"
@@ -30,15 +33,13 @@ __device__ __forceinline__ int pair_index(int i, int j, int F, int self) {
   return self ? i * F - (i * (i - 1)) / 2 + (j - i) : i * (2 * F - i - 1) / 2 + (j - i - 1);
 }
 
-// Shared-memory plan (floats): xs[G][F][DS] | os[G][OWP] | (fused) idx as long long [G][T]
+// Shared-memory plan (floats): xs[G][F][DS] | os[G][OWP]
 // Compute: 3x3 register blocks over the upper triangle of the FxF Gram matrix; a task is
 // (sample g, block pair bp); tasks are flattened over the CTA so all lanes stay busy.
-template <int MODE /*0 = x from HBM stack, 1 = gather rows from tables*/, typename IdxT>
 __global__ void __launch_bounds__(128)
-interact_kernel(const float* __restrict__ x, long long x_stride, const __grid_constant__ GatherParams p,
-                const float* __restrict__ prefix, long long prefix_stride, int P, int bottom_slot,
-                long long B, int F, int D, int G, int self_inter, float* __restrict__ out,
-                long long out_stride, int* __restrict__ oob_count) {
+interact_kernel(const float* __restrict__ x, long long x_stride, const float* __restrict__ prefix,
+                long long prefix_stride, int P, long long B, int F, int D, int G, int self_inter,
+                float* __restrict__ out, long long out_stride) {
   extern __shared__ __align__(16) float smem[];
   const int DS = D + 4;
   const int npairs = self_inter ? F * (F + 1) / 2 : F * (F - 1) / 2;
@@ -46,7 +47,6 @@ interact_kernel(const float* __restrict__ x, long long x_stride, const __grid_co
   const int OWP = (OW + 3) & ~3;
   float* xs = smem;
   float* os = xs + (size_t)G * F * DS;
-  long long* idx_s = reinterpret_cast<long long*>(os + (size_t)G * OWP);
   const int nb = (F + 2) / 3;
   const int nbp = nb * (nb + 1) / 2;
   const int V = D >> 2;
@@ -55,40 +55,10 @@ interact_kernel(const float* __restrict__ x, long long x_stride, const __grid_co
   for (long long b0 = (long long)blockIdx.x * G; b0 < B; b0 += (long long)gridDim.x * G) {
     const int gcount = (int)((B - b0) < G ? (B - b0) : G);
     // ---- load phase -------------------------------------------------------------------
-    if (MODE == 0) {
-      const int total = gcount * F * V;
-      for (int e = tid; e < total; e += nth) {
-        const int v = e % V, f = (e / V) % F, g = e / (V * F);
-        cp_async16(xs + ((size_t)g * F + f) * DS + v * 4, x + (b0 + g) * x_stride + (size_t)f * D + v * 4);
-      }
-    } else {
-      const int T = p.n_tables;
-      for (int e = tid; e < gcount * T; e += nth) {
-        const int g = e % gcount, t = e / gcount;  // consecutive threads -> consecutive samples
-        long long id = (long long)reinterpret_cast<const IdxT*>(p.t[t].indices)[b0 + g];
-        if (id < 0 || id >= p.t[t].rows) {
-          id = -1;
-          if (oob_count) atomicAdd(oob_count, 1);
-        }
-        idx_s[g * T + t] = id;
-      }
-      __syncthreads();
-      const int total = gcount * T * V;
-      for (int e = tid; e < total; e += nth) {
-        const int v = e % V, t = (e / V) % T, g = e / (V * T);
-        const long long id = idx_s[g * T + t];
-        const int slot = p.t[t].out_col / D;
-        float* dst = xs + ((size_t)g * F + slot) * DS + v * 4;
-        if (id >= 0) cp_async16(dst, p.t[t].weights + id * D + v * 4);
-        else *reinterpret_cast<float4*>(dst) = make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-      if (bottom_slot >= 0) {
-        for (int e = tid; e < gcount * V; e += nth) {
-          const int v = e % V, g = e / V;
-          cp_async16(xs + ((size_t)g * F + bottom_slot) * DS + v * 4,
-                     prefix + (b0 + g) * prefix_stride + v * 4);
-        }
-      }
+    const int total = gcount * F * V;
+    for (int e = tid; e < total; e += nth) {
+      const int v = e % V, f = (e / V) % F, g = e / (V * F);
+      cp_async16(xs + ((size_t)g * F + f) * DS + v * 4, x + (b0 + g) * x_stride + (size_t)f * D + v * 4);
     }
     // prefix (shortcut branch) goes to the head of the output row
     if (P > 0) {
@@ -177,29 +147,25 @@ interact_kernel(const float* __restrict__ x, long long x_stride, const __grid_co
   }
 }
 
-static size_t interact_smem(int G, int F, int D, int OW, int T) {
+static size_t interact_smem(int G, int F, int D, int OW) {
   const int OWP = (OW + 3) & ~3;
-  return ((size_t)G * F * (D + 4) + (size_t)G * OWP) * sizeof(float) + (size_t)G * T * sizeof(long long);
+  return ((size_t)G * F * (D + 4) + (size_t)G * OWP) * sizeof(float);
 }
 
-template <int MODE, typename IdxT>
-static int launch_interact(const float* x, int64_t x_stride, const GatherParams& p,
-                           const float* prefix, int64_t prefix_stride, int P, int bottom_slot,
-                           int64_t B, int F, int D, int self_inter, float* out, int64_t out_stride,
-                           int32_t* oob, cudaStream_t st, const char* who) {
+static int launch_interact(const float* x, int64_t x_stride, const float* prefix, int64_t prefix_stride, int P,
+                           int64_t B, int F, int D, int self_inter, float* out, int64_t out_stride, cudaStream_t st,
+                           const char* who) {
   const int npairs = self_inter ? F * (F + 1) / 2 : F * (F - 1) / 2;
   const int OW = P + npairs;
-  const int T = MODE ? p.n_tables : 0;
   // samples per CTA: fill ~56 KB so that 3-4 CTAs are resident per SM (load/compute overlap)
   int G = 1;
-  while (G < 16 && interact_smem(G + 1, F, D, OW, T) <= 56 * 1024) ++G;
-  const size_t smem = interact_smem(G, F, D, OW, T);
+  while (G < 16 && interact_smem(G + 1, F, D, OW) <= 56 * 1024) ++G;
+  const size_t smem = interact_smem(G, F, D, OW);
   MM_REQUIRE(smem <= 200 * 1024, MM_ERR_UNSUPPORTED,
              "%s: F=%d D=%d needs %zu B of shared memory per sample (> 200 KB)", who, F, D, smem);
-  auto kern = interact_kernel<MODE, IdxT>;
-  static size_t smem_set = 0;  // per template instantiation
+  static size_t smem_set = 0;
   if (smem > smem_set) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(interact_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     if (e != cudaSuccess) {
       set_error("%s: cudaFuncSetAttribute(200 KB smem) failed: %s", who, cudaGetErrorString(e));
       return (int)e;
@@ -209,8 +175,8 @@ static int launch_interact(const float* x, int64_t x_stride, const GatherParams&
   long long tiles = (B + G - 1) / G;
   const long long cap = (long long)sm_count() * 4 * 8;
   const unsigned blocks = (unsigned)(tiles < cap ? tiles : cap);
-  kern<<<blocks, 128, smem, st>>>(x, x_stride, p, prefix, prefix_stride, P, bottom_slot, B, F, D, G,
-                                  self_inter, out, out_stride, oob);
+  interact_kernel<<<blocks, 128, smem, st>>>(x, x_stride, prefix, prefix_stride, P, B, F, D, G, self_inter, out,
+                                             out_stride);
   return check_launch(who);
 }
 
@@ -272,8 +238,6 @@ int mm_dot_interaction(const float* x, int64_t B, int F, int D, int64_t x_stride
   MM_REQUIRE(!out_split || (out_Kp % 64 == 0 && out_Kp >= P + npairs && ((uintptr_t)out_split % 16) == 0), MM_ERR_ARG,
              "mm_dot_interaction: out_Kp must be a multiple of 64 >= %d and out_split 16-B aligned", P + npairs);
   if (B == 0) return MM_OK;
-  mm::GatherParams p;
-  memset(&p, 0, sizeof(p));
   if (!self_interaction) {
     mm::LookupParams lk;
     memset(&lk, 0, sizeof(lk));
@@ -284,72 +248,8 @@ int mm_dot_interaction(const float* x, int64_t B, int F, int D, int64_t x_stride
   }
   MM_REQUIRE(out != nullptr, MM_ERR_UNSUPPORTED,
              "mm_dot_interaction: split-bf16 output needs the tensor-core path (F<=32, D%%16==0, P in {0,D})");
-  return mm::launch_interact<0, int32_t>(x, x_stride, p, prefix, prefix_stride, P, -1, B, F, D,
-                                         self_interaction ? 1 : 0, out, out_stride, nullptr,
-                                         (cudaStream_t)stream, "mm_dot_interaction");
-}
-
-int mm_dlrm_gather_interact(const mm_gather_table* tables_host, int n_tables, int idx_dtype,
-                            int64_t B, int D, const float* bottom, int64_t bottom_stride,
-                            int bottom_slot, float* out, int64_t out_stride, void* out_split,
-                            int out_Kp, int32_t* oob_count, void* stream) {
-  MM_REQUIRE(tables_host && n_tables > 0 && n_tables <= MM_MAX_TABLES && (out || out_split) && B >= 0, MM_ERR_ARG,
-             "mm_dlrm_gather_interact: bad table list / null out / B<0");
-  MM_REQUIRE(!(out && out_split), MM_ERR_ARG, "mm_dlrm_gather_interact: give either out or out_split");
-  MM_REQUIRE(D >= 4 && D % 4 == 0, MM_ERR_ALIGN, "mm_dlrm_gather_interact: D must be a multiple of 4");
-  MM_REQUIRE(idx_dtype == MM_I32 || idx_dtype == MM_I64, MM_ERR_ARG,
-             "mm_dlrm_gather_interact: bad idx_dtype");
-  const int F = n_tables + (bottom ? 1 : 0);
-  MM_REQUIRE(F <= 64, MM_ERR_UNSUPPORTED, "mm_dlrm_gather_interact: at most 64 feature slots");
-  MM_REQUIRE(!bottom || (bottom_slot >= 0 && bottom_slot < F && bottom_stride >= D &&
-                         bottom_stride % 4 == 0 && ((uintptr_t)bottom % 16) == 0),
-             MM_ERR_ARG, "mm_dlrm_gather_interact: bad bottom slot / stride / alignment");
-  unsigned long long seen = 0;
-  if (bottom) seen |= 1ull << bottom_slot;
-  for (int t = 0; t < n_tables; ++t) {
-    const mm_gather_table& tb = tables_host[t];
-    MM_REQUIRE(tb.weights && tb.indices && tb.rows > 0 && tb.dim == D && tb.out_col % D == 0 &&
-                   tb.out_col / D < F && ((uintptr_t)tb.weights % 16) == 0,
-               MM_ERR_ARG, "mm_dlrm_gather_interact: table %d: dim != D, bad slot or misaligned", t);
-    MM_REQUIRE(!(seen & (1ull << (tb.out_col / D))), MM_ERR_ARG,
-               "mm_dlrm_gather_interact: slot %d used twice", tb.out_col / D);
-    seen |= 1ull << (tb.out_col / D);
-  }
-  const int P = bottom ? D : 0;
-  MM_REQUIRE(!out || out_stride >= P + F * (F - 1) / 2, MM_ERR_ARG,
-             "mm_dlrm_gather_interact: out_stride too small");
-  MM_REQUIRE(!out_split || (out_Kp % 64 == 0 && out_Kp >= P + F * (F - 1) / 2 && ((uintptr_t)out_split % 16) == 0),
-             MM_ERR_ARG, "mm_dlrm_gather_interact: out_Kp must be a multiple of 64 >= the row width, out_split 16-B aligned");
-  if (B == 0) return MM_OK;
-  mm::GatherParams p;
-  memset(&p, 0, sizeof(p));
-  p.n_tables = n_tables;
-  for (int t = 0; t < n_tables; ++t) p.t[t] = tables_host[t];
-  cudaStream_t st = (cudaStream_t)stream;
-  if (F <= mm::MM_LOOKUP_MAX_ROWS) {
-    mm::LookupParams lk;
-    memset(&lk, 0, sizeof(lk));
-    lk.world = 1;
-    for (int t = 0; t < n_tables; ++t) {
-      const int r = tables_host[t].out_col / D;
-      lk.weights[r] = tables_host[t].weights;
-      lk.indices[r] = tables_host[t].indices;
-      lk.rows[r] = tables_host[t].rows;
-      lk.idx_bytes[r] = idx_dtype == MM_I32 ? 4 : 8;
-    }
-    const int rc2 = mm::imma2::launch<1>(nullptr, 0, lk, bottom, bottom_stride, P, bottom ? bottom_slot : -1, B, F, D, out,
-                                         out_stride, out_split, out_Kp, oob_count, st, "mm_dlrm_gather_interact", false);
-    if (rc2 != MM_ERR_UNSUPPORTED) return rc2;
-  }
-  MM_REQUIRE(out != nullptr, MM_ERR_UNSUPPORTED,
-             "mm_dlrm_gather_interact: split-bf16 output needs the tensor-core path (F<=32, D%%16==0)");
-  return idx_dtype == MM_I32
-             ? mm::launch_interact<1, int32_t>(nullptr, 0, p, bottom, bottom_stride, P,
-                                               bottom ? bottom_slot : -1, B, F, D, 0, out,
-                                               out_stride, oob_count, st, "mm_dlrm_gather_interact")
-             : mm::launch_interact<1, int64_t>(nullptr, 0, p, bottom, bottom_stride, P,
-                                               bottom ? bottom_slot : -1, B, F, D, 0, out,
-                                               out_stride, oob_count, st, "mm_dlrm_gather_interact");
+  return mm::launch_interact(x, x_stride, prefix, prefix_stride, P, B, F, D, self_interaction ? 1 : 0, out, out_stride,
+                             (cudaStream_t)stream, "mm_dot_interaction");
 }
 
 }  // extern "C"

@@ -1,5 +1,5 @@
 // DLRM lookup + pairwise interaction on mma.sync, one warp per sample: the tensor-core path of
-// mm_dlrm_lookup_interact, mm_dlrm_gather_interact and mm_dot_interaction (F <= 32, D in {16, 32, 64, 128}, P in {0, D}).
+// mm_dlrm_lookup_interact and mm_dot_interaction (F <= 32, D in {16, 32, 64, 128}, P in {0, D}).
 //
 // The kernel is bound on the SM side (instruction issue and the mma.sync pipe), not by DRAM, so every phase is built
 // to issue few instructions per sample:

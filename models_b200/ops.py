@@ -168,20 +168,6 @@ def dot_interaction(x: torch.Tensor, out: torch.Tensor, prefix: Optional[torch.T
     return out
 
 
-def dlrm_gather_interact(weights, indices, slots, D: int, bottom: Optional[torch.Tensor], bottom_slot: int,
-                         out: torch.Tensor, oob: Optional[torch.Tensor] = None) -> torch.Tensor:
-    _dev(out, "out")
-    B = out.shape[0]
-    arr, n, dt = _table_array(weights, indices, [s * D for s in slots], B)
-    o32, ostride, osplit, okp = _split_out_args(out)
-    _cabi.check(
-        _lib().mm_dlrm_gather_interact(arr, n, dt, B, D, _ptr(bottom),
-                                       0 if bottom is None else _row_stride(_dev(bottom, "bottom", torch.float32), "bottom"),
-                                       bottom_slot, o32, ostride, osplit, okp, _ptr(oob), _stream()),
-        "mm_dlrm_gather_interact")
-    return out
-
-
 def scale_shift(x: torch.Tensor, scale: torch.Tensor, shift: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """out = x * scale + shift per column (BatchNormalization at inference; mm_scale_shift)."""
     _dev(x, "x", torch.float32), _dev(scale, "scale", torch.float32), _dev(shift, "shift", torch.float32)

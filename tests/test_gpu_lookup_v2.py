@@ -141,6 +141,49 @@ def test_lookup_interact_out_of_range_narrow_ids(device):
     np.testing.assert_allclose(out.cpu().numpy(), ref, rtol=2e-4, atol=4e-4)
 
 
+@pytest.mark.parametrize("idx_dtype", [np.int32, np.int64])
+def test_lookup_interact_wide_ids_match_oracle(device, idx_dtype):
+    """4- and 8-byte ids, permuted slots and a bottom vector: the prefix is a pure copy and the interactions
+    match the oracle."""
+    rng = np.random.default_rng(9)
+    B, T, D = 515, 26, 64
+    rows = [int(r) for r in rng.integers(3, 5000, T)]
+    tables = [rng.standard_normal((r, D)).astype(np.float32) for r in rows]
+    idx = [rng.integers(0, r, B).astype(idx_dtype) for r in rows]
+    bottom = rng.standard_normal((B, D)).astype(np.float32)
+    slots = rng.permutation(T + 1).tolist()
+    bslot, tslots = slots[-1], slots[:-1]
+    F = T + 1
+    out = torch.empty((B, D + F * (F - 1) // 2), dtype=torch.float32, device=device)
+    ops.dlrm_lookup_interact([dev(t, device) for t in tables], [dev(i, device) for i in idx], tslots, rows, D,
+                             dev(bottom, device), bslot, out)
+    got = out.cpu().numpy()
+    assert np.array_equal(got[:, :D], bottom)
+    ref = reference(tables, idx, rows, tslots, bottom, bslot, F, D)
+    np.testing.assert_allclose(got[:, D:], ref[:, D:], rtol=1e-4, atol=2e-4)
+
+
+def test_lookup_interact_split_output_and_out_of_range_wide_ids(device):
+    """4-byte ids below 0 and at or above `rows` read zero rows and are counted; split-bf16 output."""
+    rng = np.random.default_rng(21)
+    B, T, D = 3000, 26, 64
+    rows = [int(r) for r in rng.integers(3, 5000, T)]
+    tables = [rng.standard_normal((r, D)).astype(np.float32) for r in rows]
+    idx = [rng.integers(0, r, B).astype(np.int32) for r in rows]
+    idx[3][7] = rows[3] + 5
+    idx[9][11] = -2
+    bottom = rng.standard_normal((B, D)).astype(np.float32)
+    F = T + 1
+    W = D + F * (F - 1) // 2
+    out = torch.empty((B, 2 * ops.tc_padded_k(W)), dtype=torch.bfloat16, device=device)
+    oob = torch.zeros(1, dtype=torch.int32, device=device)
+    ops.dlrm_lookup_interact([dev(t, device) for t in tables], [dev(i, device) for i in idx], list(range(T)), rows, D,
+                             dev(bottom, device), T, out, oob)
+    assert int(oob.item()) == 2
+    ref = reference(tables, idx, rows, list(range(T)), bottom, T, F, D)
+    np.testing.assert_allclose(unsplit(out, W), ref, rtol=2e-4, atol=2e-4)
+
+
 def test_lookup_interact_rejects_bad_descriptors(device):
     t = torch.zeros((300, 64), device=device)
     out = torch.empty((4, 1), dtype=torch.float32, device=device)

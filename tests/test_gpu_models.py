@@ -86,6 +86,29 @@ def test_dlrm_out_of_range_index_raises(device):
         model(H.device_batch(feats, device))
 
 
+@pytest.mark.parametrize("n_cat,D", [(26, 8), (33, 16)])
+def test_dlrm_model_outside_the_fused_kernel(device, n_cat, D):
+    """Shapes the fused lookup + interaction kernel does not take (D = 8; F = 34 > 32 feature slots): fused=True
+    gives the same predictions as fused=False, bit for bit, matches the oracle, and still reports bad ids."""
+    mm.set_seed(41)
+    schema = mm.Schema(list(small_criteo(3000)) + [datasets._cat(f"C{i}", 3000) for i in range(27, n_cat + 1)])
+    model = mm.DLRMModel(schema, embedding_dim=D, bottom_block=mm.MLPBlock([32, D]), top_block=mm.MLPBlock([64, 16]))
+    assert not model.body.can_emit_split()
+    feats, _ = datasets.split_targets(schema, datasets.generate_batch(schema, 500, seed=8, index_law="uniform"))
+    batch = H.device_batch(feats, device)
+    fused = model(batch).cpu().numpy()
+    model.body.fused = False
+    staged = model(batch).cpu().numpy()
+    model.body.fused = True
+    assert np.array_equal(fused, staged)
+    assert H.rel_err(fused, H.oracle_dlrm(model, feats)) < 2e-4
+    bad = dict(feats)
+    bad["C3"] = feats["C3"].copy()
+    bad["C3"][4] = 10_000
+    with pytest.raises(IndexError, match="out of range"):
+        model(H.device_batch(bad, device))
+
+
 @pytest.mark.parametrize("stacked", [True, False])
 def test_dcn_model_matches_oracle(device, stacked):
     mm.set_seed(11)

@@ -168,29 +168,6 @@ def test_dot_interaction_with_prefix_is_bottom_first(device):
     np.testing.assert_allclose(got[:, D:], oracle.dot_interaction(x), rtol=RTOL, atol=2e-4)
 
 
-@pytest.mark.parametrize("idx_dtype", [np.int32, np.int64])
-def test_dlrm_gather_interact_equals_staged(device, idx_dtype):
-    rng = np.random.default_rng(9)
-    B, T, D = 515, 26, 64
-    rows = rng.integers(3, 5000, T)
-    tables = [rng.standard_normal((int(r), D)).astype(np.float32) for r in rows]
-    idx = [rng.integers(0, int(r), B).astype(idx_dtype) for r in rows]
-    bottom = rng.standard_normal((B, D)).astype(np.float32)
-    slots = rng.permutation(T + 1).tolist()
-    bslot, tslots = slots[-1], slots[:-1]
-    F = T + 1
-    out = torch.empty((B, D + F * (F - 1) // 2), dtype=torch.float32, device=device)
-    ops.dlrm_gather_interact([dev(t, device) for t in tables], [dev(i, device) for i in idx], tslots, D,
-                             dev(bottom, device), bslot, out)
-    stack = np.zeros((B, F, D), dtype=np.float32)
-    for t in range(T):
-        stack[:, tslots[t]] = tables[t][idx[t]]
-    stack[:, bslot] = bottom
-    got = out.cpu().numpy()
-    assert np.array_equal(got[:, :D], bottom)
-    np.testing.assert_allclose(got[:, D:], oracle.dot_interaction(stack), rtol=RTOL, atol=2e-4)
-
-
 @pytest.mark.parametrize("act", ["relu", "linear", "sigmoid", "tanh", "selu", "elu", "gelu"])
 def test_dense_fp32_activations(device, act):
     rng = np.random.default_rng(10)
@@ -309,33 +286,6 @@ def test_dot_interaction_split_output(device, B):
     o32 = torch.empty((B, W), dtype=torch.float32, device=device)
     ops.dot_interaction(dev(x, device), o32, prefix=dev(bottom, device))
     assert torch.equal(ops.split_rows(o32), out)
-
-
-def test_dlrm_gather_interact_split_and_oob(device):
-    rng = np.random.default_rng(21)
-    B, T, D = 3000, 26, 64
-    rows = rng.integers(3, 5000, T)
-    tables = [rng.standard_normal((int(r), D)).astype(np.float32) for r in rows]
-    idx = [rng.integers(0, int(r), B).astype(np.int32) for r in rows]
-    idx[3][7] = int(rows[3]) + 5   # out of range -> zero row + counted
-    idx[9][11] = -2
-    bottom = rng.standard_normal((B, D)).astype(np.float32)
-    F = T + 1
-    slots = list(range(T))
-    W = D + F * (F - 1) // 2
-    out = torch.empty((B, 2 * ops.tc_padded_k(W)), dtype=torch.bfloat16, device=device)
-    oob = torch.zeros(1, dtype=torch.int32, device=device)
-    ops.dlrm_gather_interact([dev(t, device) for t in tables], [dev(i, device) for i in idx], slots, D,
-                             dev(bottom, device), T, out, oob)
-    assert int(oob.item()) == 2
-    stack = np.zeros((B, F, D), dtype=np.float32)
-    for t in range(T):
-        ok = (idx[t] >= 0) & (idx[t] < rows[t])
-        stack[ok, t] = tables[t][idx[t][ok]]
-    stack[:, T] = bottom
-    rec, _ = _unsplit(out, W)
-    ref = np.concatenate([bottom, oracle.dot_interaction(stack)], axis=1)
-    np.testing.assert_allclose(rec, ref, rtol=2e-4, atol=2e-4)
 
 
 @pytest.mark.parametrize("F,D", [(2, 16), (32, 32), (17, 48), (9, 256)])

@@ -96,9 +96,11 @@ def main():
             report("mm_dot_interaction (F=27, D=64, +prefix)", m, mn, bytes_=B * (F * D * 4 + (D + 351) * 4),
                    flops=B * 351 * 64 * 2)
         if "fused" in only:
-            m, mn = timeit(lambda i: ops.dlrm_gather_interact(tables, idx[i % nb], [slots[n] for n in names], D, bottom,
+            rows = [t.shape[0] for t in tables]
+            m, mn = timeit(lambda i: ops.dlrm_lookup_interact(tables, idx[i % nb], [slots[n] for n in names], rows, D, bottom,
                                                               slots["bottom_block"], out[i % 2]), args.iters)
-            report("mm_dlrm_gather_interact", m, mn, bytes_=B * (T * D * 4 + T * 4 + D * 4 + (D + 351) * 4), law=args.law)
+            report("mm_dlrm_lookup_interact (int32 ids, fp32 out)", m, mn, bytes_=B * (T * D * 4 + T * 4 + D * 4 + (D + 351) * 4),
+                   law=args.law)
 
     if "fused2" in only:
         # the real step's launch: split-bf16 output row (B, 2*448); ids as int32 and packed (1/2/3-byte)
@@ -129,8 +131,6 @@ def main():
         report(f"mm_dlrm_lookup_interact (operand-format rows, packed ids {idb} B/sample, split out)", m, mn,
                bytes_=B * (T * D * 4 + idb + D * 4 + (D + 351) * 4), law=args.law)
         del mirrors
-        m, mn = timeit(lambda i: ops.dlrm_gather_interact(tables, idx[i % nb], sl, D, bottom, slots["bottom_block"], osplit[i % 2]), args.iters)
-        report("mm_dlrm_gather_interact (legacy entry, split out)", m, mn, bytes_=B * (T * D * 4 + T * 4 + D * 4 + (D + 351) * 4), law=args.law)
 
     if "dense" in only:
         for (K, N) in [(13, 128), (128, 64), (415, 128), (128, 64), (64, 32), (32, 1), (1037, 1037), (1024, 1024)]:

@@ -51,7 +51,8 @@ elif what in ("gather", "fused", "fused_operand", "interact"):
         if what == "gather":
             ops.gather_multi(tables, idx, [slots[n] * D for n in names], stack)
         elif what == "fused":
-            ops.dlrm_gather_interact(tables, idx, [slots[n] for n in names], D, bottom, slots["bottom_block"], out)
+            ops.dlrm_lookup_interact(tables, idx, [slots[n] for n in names], [t.shape[0] for t in tables], D, bottom,
+                                     slots["bottom_block"], out)
         elif what == "fused_operand":
             if i == 0:
                 mirrors, bottom_op = [ops.split_rows(t) for t in tables], ops.split_rows(bottom)
