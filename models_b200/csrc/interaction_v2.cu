@@ -1,8 +1,8 @@
 // DLRM lookup + pairwise interaction on mma.sync, one warp per sample: the tensor-core path of
 // mm_dlrm_lookup_interact and mm_dot_interaction (F <= 32, D in {16, 32, 64, 128}, P in {0, D}).
 //
-// The kernel is bound on the SM side (instruction issue and the mma.sync pipe), not by DRAM, so every phase is built
-// to issue few instructions per sample:
+// The kernel is bound on the SM side, not by DRAM: serving the large tables' rows from L2 saves 1-3 % on H100 (DESIGN.md
+// §4 has the measurements, phase by phase), so every phase is built to issue few instructions per sample:
 //   * copy loop: 8 lanes move one 128-byte half row per LDGSTS, 4 rows per instruction.  Staged row r is
 //     owned by lane r (tables arrive sorted by slot, so row == slot), a row's source pointer travels
 //     with two shuffles, and because row = 4*i + lane/8 the XOR swizzle of a lane's destination does
@@ -86,9 +86,9 @@ struct RawIdx {
 // tensor-core layer of this library (mm_split_rows) — read from a second copy of the tables in HBM; the bottom vector
 // arrives in the same format from the tower kernel.  The rows land in shared memory with the 128-byte XOR swizzle
 // (16-byte chunk c of row r at chunk c ^ (r & 7)) and the MMA fragments are loaded by ldmatrix.x4: per 16-wide k-step
-// four loads give the A quads (hi and lo, two m-tiles) and four the B pairs (hi and lo, four n-tiles), each already in the
-// register shape HMMA wants.  Per sample: 32 LDSM + 16 LOP3 + 72 HMMA instead of 16 LDS.128 + 192 split instructions
-// + ~180 operand moves + 72 HMMA.  Same values as the in-kernel split => bit-identical output.
+// four loads give the A quads (hi and lo, two m-tiles), already in the register shape HMMA wants, and the B pairs of the
+// four n-tiles are the same registers (B = X^T).  Per sample: 16 LDSM + 72 HMMA instead of 16 LDS.128 + 192 split
+// instructions + ~180 operand moves + 72 HMMA.  Same values as the in-kernel split => bit-identical output.
 // (A first attempt kept the lane-private LDS.128 scheme with hi and lo interleaved per chunk: fewer instructions, but
 // the A quads still had to be assembled with moves and nothing overlapped the load -> HMMA latency: 0.116 ms vs 0.104.)
 template <int MODE, int KD /* embedding dim: 16, 32, 64, 128 */, int NWARPS /* launch bound */, bool PS>
@@ -247,17 +247,15 @@ interact_v2_kernel(const __grid_constant__ LookupParams lk, const Params p) {
   }
   // ---- PS: ldmatrix row addresses.  Lane l supplies row (l & 7) of matrix (l >> 3).
   //   A quad of m-tile mt (rows 16mt..): matrices (rows +0..7, k-lo) (rows +8..15, k-lo) (rows +0..7, k-hi) (rows +8..15, k-hi)
-  //   B pairs of n-tiles 2u, 2u+1 (rows 16u..): matrices (rows +0..7, k-lo) (rows +0..7, k-hi) (rows +8..15, k-lo) (rows +8..15, k-hi)
   // k-lo / k-hi = chunks 2ks / 2ks+1 of the hi half (+128 bytes: lo half).  With 256-byte aligned buffers the byte offset
   // is row*256 | ((chunk ^ (row & 7)) << 4), and (2ks + b) ^ x = (2ks) ^ (b ^ x): one XOR with 32*ks per k-step.
-  uint32_t la[2], lb[2];
+  uint32_t la[2];
   {
     const int mi = lane >> 3, j = lane & 7;
 #pragma unroll
     for (int u = 0; u < 2; ++u) {
-      const int ra = min(16 * u + (mi & 1) * 8 + j, F - 1), rbq = min(16 * u + (mi >> 1) * 8 + j, F - 1);
+      const int ra = min(16 * u + (mi & 1) * 8 + j, F - 1);
       la[u] = (uint32_t)ra * 256u | (uint32_t)((((mi >> 1) ^ ra) & 7) << 4);
-      lb[u] = (uint32_t)rbq * 256u | (uint32_t)((((mi & 1) ^ rbq) & 7) << 4);
     }
   }
 
@@ -306,7 +304,7 @@ interact_v2_kernel(const __grid_constant__ LookupParams lk, const Params p) {
 #pragma unroll
         for (int c = 0; c < 4; ++c) acc[ti][c] = 0.0f;
 
-      const uint32_t a0b = xs + la[0], a1b = xs + la[1], b0b = xs + lb[0], b1b = xs + lb[1];
+      const uint32_t a0b = xs + la[0], a1b = xs + la[1];
 #pragma unroll
       for (int ks = 0; ks < KS; ++ks) {
         // A quads of m-tiles 0, 1 and B pairs of n-tiles 0..3 (n-tile nt = rows 8nt + g), hi and lo
@@ -317,10 +315,12 @@ interact_v2_kernel(const __grid_constant__ LookupParams lk, const Params p) {
           ldsm_x4((a0b ^ kx) + 128u, al[0][0], al[0][1], al[0][2], al[0][3]);
           ldsm_x4(a1b ^ kx, ah[1][0], ah[1][1], ah[1][2], ah[1][3]);
           ldsm_x4((a1b ^ kx) + 128u, al[1][0], al[1][1], al[1][2], al[1][3]);
-          ldsm_x4(b0b ^ kx, bh[0][0], bh[0][1], bh[1][0], bh[1][1]);
-          ldsm_x4((b0b ^ kx) + 128u, bl[0][0], bl[0][1], bl[1][0], bl[1][1]);
-          ldsm_x4(b1b ^ kx, bh[2][0], bh[2][1], bh[3][0], bh[3][1]);
-          ldsm_x4((b1b ^ kx) + 128u, bl[2][0], bl[2][1], bl[3][0], bl[3][1]);
+          // B = X^T: the B pairs of n-tiles 2mt, 2mt+1 are registers of the A quad of m-tile mt (same rows, same clamp)
+#pragma unroll
+          for (int mt = 0; mt < 2; ++mt) {
+            bh[2 * mt][0] = ah[mt][0], bh[2 * mt][1] = ah[mt][2], bh[2 * mt + 1][0] = ah[mt][1], bh[2 * mt + 1][1] = ah[mt][3];
+            bl[2 * mt][0] = al[mt][0], bl[2 * mt][1] = al[mt][2], bl[2 * mt + 1][0] = al[mt][1], bl[2 * mt + 1][1] = al[mt][3];
+          }
         } else {
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
