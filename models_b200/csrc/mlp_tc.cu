@@ -42,8 +42,7 @@ constexpr uint32_t A_TILE_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KB
 
 struct ChainLayer {
   int N, Np;        // true / padded (multiple of 16) width of this layer
-  int Kp;           // K padded to 64 (row pitch of the split weights = 2 * Kp elements)
-  int ksteps;       // MMA k-steps actually issued = padded width of the previous layer / 16
+  int Kp;           // K padded to 64 (row pitch of the split weights = 2 * Kp elements): 64 or 128
   int act;
   uint32_t w_off;   // byte offset of this layer's resident weight tiles inside the weight arena
 };
@@ -63,6 +62,52 @@ struct Params {
   float* head_out;
 };
 
+// One chain layer's MMAs for a compile-time width NP and KS = Kp / 16 k-steps: three straight-line batches of HGMMAs under one
+// fence.  A runtime test between them (such as the previous layer's k-step count) would make ptxas serialise every wgmma of
+// the kernel.  The k-steps past the previous layer's padded width multiply zero A fragments (accumulator columns no MMA
+// wrote) by zero-padded weight rows: they add exact zeros.
+template <int NP, int KS>
+__device__ __forceinline__ void chain_mma(float (&acc)[64], const uint32_t (&ahi)[32], const uint32_t (&alo)[32], uint32_t w_hi,
+                                          uint32_t w_lo, uint32_t tile_b) {
+  wgmma_fence();
+  // a k-step covers 16 K elements = 32 bytes of a weight row
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) {
+    const uint32_t f[4] = {ahi[4 * ks], ahi[4 * ks + 1], ahi[4 * ks + 2], ahi[4 * ks + 3]};
+    wgmma_rs(NP, acc, f, make_desc_sw128(w_lo + (ks >> 2) * tile_b + (ks & 3) * 32));
+  }
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) {
+    const uint32_t f[4] = {alo[4 * ks], alo[4 * ks + 1], alo[4 * ks + 2], alo[4 * ks + 3]};
+    wgmma_rs(NP, acc, f, make_desc_sw128(w_hi + (ks >> 2) * tile_b + (ks & 3) * 32));
+  }
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) {
+    const uint32_t f[4] = {ahi[4 * ks], ahi[4 * ks + 1], ahi[4 * ks + 2], ahi[4 * ks + 3]};
+    wgmma_rs(NP, acc, f, make_desc_sw128(w_hi + (ks >> 2) * tile_b + (ks & 3) * 32));
+  }
+  wgmma_commit();
+  wgmma_wait_all();
+}
+// the same for the layer's padded width `np` (16 .. 128), chosen once per layer
+template <int KS>
+__device__ __forceinline__ void chain_mma(int np, float (&acc)[64], const uint32_t (&ahi)[32], const uint32_t (&alo)[32],
+                                          uint32_t w_hi, uint32_t w_lo, uint32_t tile_b) {
+  switch (np) {
+    case 16: chain_mma<16, KS>(acc, ahi, alo, w_hi, w_lo, tile_b); break;
+    case 32: chain_mma<32, KS>(acc, ahi, alo, w_hi, w_lo, tile_b); break;
+    case 48: chain_mma<48, KS>(acc, ahi, alo, w_hi, w_lo, tile_b); break;
+    case 64: chain_mma<64, KS>(acc, ahi, alo, w_hi, w_lo, tile_b); break;
+    case 80: chain_mma<80, KS>(acc, ahi, alo, w_hi, w_lo, tile_b); break;
+    case 96: chain_mma<96, KS>(acc, ahi, alo, w_hi, w_lo, tile_b); break;
+    case 112: chain_mma<112, KS>(acc, ahi, alo, w_hi, w_lo, tile_b); break;
+    default: chain_mma<128, KS>(acc, ahi, alo, w_hi, w_lo, tile_b); break;
+  }
+}
+
+// N1P = padded layer-1 width (16 .. 128), a compile-time constant: each layer-1 HGMMA is one fixed instruction, not a
+// switch on the width, and ptxas need not fence every one of them on its own
+template <int N1P>
 __global__ void __launch_bounds__(kThreads, 1)
 mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW1,
               const __grid_constant__ CUtensorMap tmC0, const __grid_constant__ CUtensorMap tmC1,
@@ -71,8 +116,8 @@ mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // keeps the shared state space
   // layer-1 ring: each slot holds ONE half of a k-block, {A_hi, W1_hi} or {A_lo, W1_lo} (32 KB at N1 = 128):
   // finer slots keep more bytes in flight than whole {hi, lo} stages in the same shared memory
-  const uint32_t B_TILE_BYTES = (uint32_t)p.N1p * BLOCK_K * 2;
-  const uint32_t STAGE_BYTES = A_TILE_BYTES + B_TILE_BYTES;
+  constexpr uint32_t B_TILE_BYTES = (uint32_t)N1P * BLOCK_K * 2;
+  constexpr uint32_t STAGE_BYTES = A_TILE_BYTES + B_TILE_BYTES;
   uint8_t* wres = smem + (size_t)p.stages * STAGE_BYTES;  // resident chain weights (1024-B aligned tiles)
   uint64_t* bars = reinterpret_cast<uint64_t*>(wres + p.w_bytes);
   uint64_t* full_bar = bars;                        // [stages]
@@ -164,7 +209,7 @@ mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < BLOCK_K / MMA_K; ++k)
-          wgmma_ss(p.N1p, acc, make_desc_sw128(a_hi + a_off + k * 32), make_desc_sw128(b_hi + k * 32));
+          wgmma_ss(N1P, acc, make_desc_sw128(a_hi + a_off + k * 32), make_desc_sw128(b_hi + k * 32));
         wgmma_commit();
         if (++stage == p.stages) {
           stage = 0;
@@ -177,10 +222,10 @@ mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < BLOCK_K / MMA_K; ++k)
-          wgmma_ss(p.N1p, acc, make_desc_sw128(a_hi + a_off + k * 32), make_desc_sw128(b_lo + k * 32));
+          wgmma_ss(N1P, acc, make_desc_sw128(a_hi + a_off + k * 32), make_desc_sw128(b_lo + k * 32));
 #pragma unroll
         for (int k = 0; k < BLOCK_K / MMA_K; ++k)
-          wgmma_ss(p.N1p, acc, make_desc_sw128(a_lo + a_off + k * 32), make_desc_sw128(b_hi + k * 32));
+          wgmma_ss(N1P, acc, make_desc_sw128(a_lo + a_off + k * 32), make_desc_sw128(b_hi + k * 32));
         wgmma_commit();
         wgmma_wait_all();
         wgmma_fence_acc(acc);
@@ -198,7 +243,7 @@ mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
       for (int layer = 0; layer <= p.n_chain; ++layer) {
         const bool last = layer == p.n_chain;
         const int N = layer == 0 ? p.N1 : p.c[layer - 1].N;
-        const int Np = layer == 0 ? p.N1p : p.c[layer - 1].Np;
+        const int Np = layer == 0 ? N1P : p.c[layer - 1].Np;
         const int act = layer == 0 ? p.act1 : p.c[layer - 1].act;
         const float* bs = bias_s + layer * 128;
         // bias + activation on the fragment; padding columns (>= N) become exact zeros
@@ -230,31 +275,8 @@ mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
 #pragma unroll
           for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
           wgmma_fence_acc(acc);
-          wgmma_fence();
-          // a k-step covers 16 K elements = 32 bytes of a weight row
-#pragma unroll
-          for (int ks = 0; ks < 8; ++ks) {
-            if (ks < L.ksteps) {
-              const uint32_t f[4] = {ahi[4 * ks], ahi[4 * ks + 1], ahi[4 * ks + 2], ahi[4 * ks + 3]};
-              wgmma_rs(L.Np, acc, f, make_desc_sw128(w_lo + (ks >> 2) * tile_b + (ks & 3) * 32));
-            }
-          }
-#pragma unroll
-          for (int ks = 0; ks < 8; ++ks) {
-            if (ks < L.ksteps) {
-              const uint32_t f[4] = {alo[4 * ks], alo[4 * ks + 1], alo[4 * ks + 2], alo[4 * ks + 3]};
-              wgmma_rs(L.Np, acc, f, make_desc_sw128(w_hi + (ks >> 2) * tile_b + (ks & 3) * 32));
-            }
-          }
-#pragma unroll
-          for (int ks = 0; ks < 8; ++ks) {
-            if (ks < L.ksteps) {
-              const uint32_t f[4] = {ahi[4 * ks], ahi[4 * ks + 1], ahi[4 * ks + 2], ahi[4 * ks + 3]};
-              wgmma_rs(L.Np, acc, f, make_desc_sw128(w_hi + (ks >> 2) * tile_b + (ks & 3) * 32));
-            }
-          }
-          wgmma_commit();
-          wgmma_wait_all();
+          if (L.Kp == BLOCK_K) chain_mma<BLOCK_K / MMA_K>(L.Np, acc, ahi, alo, w_hi, w_lo, tile_b);
+          else chain_mma<2 * BLOCK_K / MMA_K>(L.Np, acc, ahi, alo, w_hi, w_lo, tile_b);
           wgmma_fence_acc(acc);
         } else {
 #pragma unroll
@@ -311,16 +333,14 @@ static bool plan_tower(int K, int n_layers, const int* widths, mm::mlp::Params& 
   p.N1p = mm_tc_padded_n(widths[0]);
   p.n_chain = n_layers - 1;
   uint32_t w_off = 0;
-  int prev_np = p.N1p, prev_n = p.N1;
+  int prev_n = p.N1;
   for (int c = 0; c < p.n_chain; ++c) {
     ChainLayer& L = p.c[c];
     L.N = widths[c + 1];
     L.Np = mm_tc_padded_n(L.N);
     L.Kp = mm_tc_padded_k(prev_n);
-    L.ksteps = prev_np / MMA_K;
     L.w_off = w_off;
     w_off += (uint32_t)(2 * (L.Kp / BLOCK_K)) * (uint32_t)L.Np * BLOCK_K * 2;
-    prev_np = L.Np;
     prev_n = L.N;
   }
   p.w_bytes = w_off;
@@ -351,6 +371,25 @@ int mm_mlp_tc_supported(int K, int n_layers, const int* widths, int with_head) {
 }
 
 }  // extern "C"
+
+typedef void (*MlpKernel)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
+                          const mm::mlp::Params);
+
+// one instantiation per padded layer-1 width mm_tc_padded_n can return
+static MlpKernel kernel_for(int n1p) {
+  using namespace mm::mlp;
+  switch (n1p) {
+    case 16: return mlp_tc_kernel<16>;
+    case 32: return mlp_tc_kernel<32>;
+    case 48: return mlp_tc_kernel<48>;
+    case 64: return mlp_tc_kernel<64>;
+    case 80: return mlp_tc_kernel<80>;
+    case 96: return mlp_tc_kernel<96>;
+    case 112: return mlp_tc_kernel<112>;
+    case 128: return mlp_tc_kernel<128>;
+  }
+  return nullptr;
+}
 
 static int mlp_tc_impl(const void* a_split, int64_t M, int K, int n_layers, const void* const* w_split, const int* widths,
                        const float* const* bias, const int* acts, float* out, int64_t out_stride, const float* head_w,
@@ -408,19 +447,21 @@ static int mlp_tc_impl(const void* a_split, int64_t M, int K, int n_layers, cons
     }
   }
 
-  static size_t smem_set = 0;
-  if (smem > smem_set) {
-    cudaError_t e = cudaFuncSetAttribute(mlp_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+  MlpKernel kern = kernel_for(p.N1p);
+  MM_REQUIRE(kern != nullptr, MM_ERR_UNSUPPORTED, "mm_mlp_tc: no kernel for a padded layer-1 width of %d", p.N1p);
+  static bool smem_set[8] = {};
+  if (!smem_set[p.N1p / 16 - 1]) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) {
       mm::set_error("mm_mlp_tc: cudaFuncSetAttribute(227 KB smem) failed: %s", cudaGetErrorString(e));
       return (int)e;
     }
-    smem_set = 227 * 1024;
+    smem_set[p.N1p / 16 - 1] = true;
   }
   const long long tiles = (M + BLOCK_M - 1) / BLOCK_M;
   const int sms = mm::sm_count();
   const unsigned grid = (unsigned)(tiles < sms ? tiles : sms);
-  mlp_tc_kernel<<<grid, kThreads, smem, (cudaStream_t)stream>>>(tmA, tmW1, tmC[0], tmC[1], tmC[2], p);
+  kern<<<grid, kThreads, smem, (cudaStream_t)stream>>>(tmA, tmW1, tmC[0], tmC[1], tmC[2], p);
   return mm::check_launch("mm_mlp_tc");
 }
 
