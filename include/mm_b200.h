@@ -428,6 +428,21 @@ int mm_init_uniform_hash_rows(float* w, int64_t local_rows, int D, uint64_t seed
  *                             grad_rows is clobbered (duplicates are folded into the first occurrence's slice);
  *                             `mirror`: operand-format copy of the table (mm_dlrm_lookup_interact MM_ROWS_OPERAND)
  *                             kept in step with the weights, nullable.
+ *   mm_bag_grad_rows          backward of one pooled multi-hot feature (mm_gather_bag / mm_gather_seq): the pooled-row
+ *                             gradient g (B, D) -> out (nnz, D), row i = scale(i) * g[bag(i)] — the IndexedSlices values
+ *                             TF's gradient of safe_embedding_lookup_sparse / the (B, L) lookup + reduce produces; they go
+ *                             to mm_sparse_rows_apply with the bag's ids as indices and B = nnz.
+ *                               ragged (offsets non-null, (B+1,) int32 / int64; ids (nnz,)): mean 1/cnt, sum 1,
+ *                               sqrtn 1/sqrt(cnt), cnt = ids of the bag in [0, rows) (what mm_gather_bag divides by);
+ *                               fixed length (offsets null, ids (B, L), nnz = B*L): mean 1/L (padding not masked), sum 1.
+ *                             Ids outside [0, rows) get a zero row.  All nnz rows are written on every call: each bag's
+ *                             range is clamped to [0, nnz] and positions no bag covers get zeros, so malformed offsets
+ *                             never read or write outside ids / out.  D in {16, 32, 64, 128}; g (stride a multiple of 4)
+ *                             and out 16-byte aligned.  out_ids (nullable, nnz ids of the ids' dtype) receives the id of
+ *                             every row that carries a gradient and -1 for the others (positions no bag covers, ids
+ *                             outside [0, rows)): passed as the indices of mm_sparse_rows_apply, only rows some bag
+ *                             really holds are updated (with Adam, a zero-gradient row would still move).  The max
+ *                             combiner (and sqrtn on fixed-length bags) returns MM_ERR_UNSUPPORTED.
  *   mm_dense_apply            the same update rules over a flat fp32 arena; g is scaled by grad_scale and CLEARED.
  *   mm_opt_tick               step counter += 1 and the Adam bias-corrected rate (once per step, before the applies)
  * Update rules (hyper: device float[MM_HYPER_COUNT], so a captured CUDA graph follows a learning-rate schedule):
@@ -483,6 +498,9 @@ int mm_dlrm_interact_backward(const mm_lookup_table* tables_host, int n_tables, 
                               int64_t d_bottom_stride, int mask_bottom, int row_format, void* stream);
 int mm_sparse_rows_apply(const mm_sparse_table* tables_host, int n_tables, int64_t B, int D, int opt,
                          const float* hyper, void* stream);
+/* Added with multi-hot training (DLRM features given as ragged bags or (B, L) id matrices); no existing entry point changed. */
+int mm_bag_grad_rows(const float* g, int64_t B, int D, int64_t g_stride, const void* ids, int idx_dtype, const void* offsets,
+                     int off_dtype, int L, int64_t nnz, int64_t rows, int combiner, float* out, void* out_ids, void* stream);
 int mm_dense_apply(int opt, float* w, float* grad, float* state1, float* state2, int64_t n, const float* hyper,
                    float grad_scale, void* stream);
 int mm_opt_tick(float* hyper, void* stream);

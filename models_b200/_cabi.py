@@ -142,6 +142,7 @@ SIGNATURES = {
     "mm_dlrm_interact_backward": (_i, [C.POINTER(LookupTable), _i, _i64, _i, _vp, _i64, _i, _i, _vp, _i64,
                                        C.POINTER(C.c_void_p), _i64, _vp, _i64, _i, _i, _vp]),
     "mm_sparse_rows_apply": (_i, [C.POINTER(SparseTable), _i, _i64, _i, _i, _vp, _vp]),
+    "mm_bag_grad_rows": (_i, [_vp, _i64, _i, _i64, _vp, _i, _vp, _i, _i, _i64, _i64, _i, _vp, _vp, _vp]),
     "mm_dense_apply": (_i, [_i, _vp, _vp, _vp, _vp, _i64, _vp, _f, _vp]),
     "mm_opt_tick": (_i, [_vp, _vp]),
     "mm_fill_i32": (_i, [_vp, _i64, C.c_int32, _vp]),

@@ -14,6 +14,8 @@
 //       (rows x 4 B, HBM is plentiful) elects the smallest sample index of every id as its representative
 //       (atomicMin), the other duplicates add their slice into the representative's slice (vector reds), and
 //       the representatives apply the update and reset the map.
+//   mm_bag_grad_rows            backward of a pooled multi-hot feature: the pooled-row gradient expanded to one scaled
+//       row per id, the IndexedSlices that mm_sparse_rows_apply consumes.
 //   mm_dense_apply              SGD / Adagrad / Adam over a flat parameter arena (+ clears the gradients).
 #include <cuda_bf16.h>
 
@@ -796,6 +798,97 @@ __global__ void dense_apply_kernel(int opt, float* __restrict__ w, float* __rest
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Bag backward: the IndexedSlices values of a pooled (multi-hot) feature, out[i] = scale(bag(i)) * g[bag(i)].
+// One warp per task; tasks 0..B-1 are the bags.  Ragged form: a bag is [off[b], off[b+1]) clamped to [0, nnz] (empty when
+// decreasing), task B zero-fills [0, off[0]) and task B+1 [off[B], nnz).  Every position lies in one of these ranges
+// (the first b with off[b+1] > i brackets i), so all nnz rows are written whatever the offsets hold.  Per bag: g[b] is
+// read once (one float4 per lane), the ids are read 32 at a time (coalesced) for the count, then D/4 lanes per row
+// write 32/(D/4) rows per vector store, zero where the id is outside [0, rows).  out_ids (nullable) receives the id of
+// every row that carries a gradient and -1 for the others (uncovered positions, ids outside [0, rows)): the indices of
+// the sparse update, which skips -1.
+// ---------------------------------------------------------------------------------------------------------------
+template <typename IT, typename OT, int D>
+__global__ void __launch_bounds__(256)
+bag_grad_rows_kernel(const float* __restrict__ g, long long g_stride, const IT* __restrict__ ids, const OT* __restrict__ offsets,
+                     int L, long long B, long long nnz, long long rows, int combiner, float* __restrict__ out,
+                     IT* __restrict__ out_ids) {
+  constexpr int LR = D / 4;   // lanes per row
+  constexpr int R = 32 / LR;  // rows per store instruction
+  const int lane = threadIdx.x & 31, c = lane % LR, rl = lane / LR;
+  const long long n_tasks = offsets ? B + 2 : B;
+  const long long warp0 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const long long n_warps = ((long long)gridDim.x * blockDim.x) >> 5;
+  auto clampn = [nnz](long long v) { return v < 0 ? 0 : (v > nnz ? nnz : v); };
+  for (long long task = warp0; task < n_tasks; task += n_warps) {
+    long long beg, end;
+    const bool zero = task >= B;
+    if (!offsets) {
+      beg = task * L;
+      end = beg + L;
+    } else if (task < B) {
+      beg = clampn((long long)offsets[task]);
+      end = clampn((long long)offsets[task + 1]);
+    } else if (task == B) {
+      beg = 0;
+      end = clampn((long long)offsets[0]);
+    } else {
+      beg = clampn((long long)offsets[B]);
+      end = nnz;
+    }
+    if (beg >= end) continue;
+    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (!zero) {
+      v = *reinterpret_cast<const float4*>(g + task * g_stride + 4 * c);
+      if (combiner != MM_COMBINER_SUM) {
+        float den = (float)L;  // fixed length: mean over all L positions, padding not masked
+        if (offsets) {
+          int cnt = 0;  // the ids gather_bag_kernel sums: those in [0, rows)
+          for (long long i = beg; i < end; i += 32) {
+            const long long id = i + lane < end ? (long long)ids[i + lane] : -1;
+            cnt += __popc(__ballot_sync(0xffffffffu, id >= 0 && id < rows));
+          }
+          den = combiner == MM_COMBINER_SQRTN ? sqrtf((float)cnt) : (float)cnt;
+        }
+        if (den > 0.0f) {
+          v.x = __fdiv_rn(v.x, den);
+          v.y = __fdiv_rn(v.y, den);
+          v.z = __fdiv_rn(v.z, den);
+          v.w = __fdiv_rn(v.w, den);
+        }
+      }
+    }
+    for (long long i = beg; i < end; i += 32) {
+      const int lim = (int)(end - i < 32 ? end - i : 32);  // positions of this chunk
+      const long long id = (!zero && lane < lim) ? (long long)ids[i + lane] : -1;
+      const bool mine = id >= 0 && id < rows;
+      const unsigned ok = __ballot_sync(0xffffffffu, mine);
+      if (out_ids && lane < lim) out_ids[i + lane] = mine ? (IT)id : (IT)-1;
+      float* dst = out + (i + rl) * D + 4 * c;
+#pragma unroll
+      for (int r = 0; r < 32; r += R) {
+        const int k = r + rl;
+        const bool on = (ok >> k) & 1u;
+        if (k < lim) *reinterpret_cast<float4*>(dst + r * D) = make_float4(on ? v.x : 0.f, on ? v.y : 0.f, on ? v.z : 0.f, on ? v.w : 0.f);
+      }
+    }
+  }
+}
+
+template <typename IT, typename OT>
+static void launch_bag_grad(unsigned blocks, cudaStream_t st, const float* g, long long g_stride, const void* ids, const void* offsets,
+                            int L, long long B, long long nnz, long long rows, int combiner, int D, float* out, void* out_ids) {
+  const IT* i = reinterpret_cast<const IT*>(ids);
+  IT* oi = reinterpret_cast<IT*>(out_ids);
+  const OT* o = reinterpret_cast<const OT*>(offsets);
+  switch (D) {
+    case 16: bag_grad_rows_kernel<IT, OT, 16><<<blocks, 256, 0, st>>>(g, g_stride, i, o, L, B, nnz, rows, combiner, out, oi); break;
+    case 32: bag_grad_rows_kernel<IT, OT, 32><<<blocks, 256, 0, st>>>(g, g_stride, i, o, L, B, nnz, rows, combiner, out, oi); break;
+    case 64: bag_grad_rows_kernel<IT, OT, 64><<<blocks, 256, 0, st>>>(g, g_stride, i, o, L, B, nnz, rows, combiner, out, oi); break;
+    default: bag_grad_rows_kernel<IT, OT, 128><<<blocks, 256, 0, st>>>(g, g_stride, i, o, L, B, nnz, rows, combiner, out, oi); break;
+  }
+}
+
 __global__ void opt_tick_kernel(float* hyper) {
   const float t = hyper[MM_HYPER_STEP] + 1.0f;
   hyper[MM_HYPER_STEP] = t;
@@ -972,6 +1065,42 @@ int mm_opt_tick(float* hyper, void* stream) {
   MM_REQUIRE(hyper, MM_ERR_ARG, "mm_opt_tick: null pointer");
   mm::trs::opt_tick_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(hyper);
   return mm::check_launch("mm_opt_tick");
+}
+
+int mm_bag_grad_rows(const float* g, int64_t B, int D, int64_t g_stride, const void* ids, int idx_dtype, const void* offsets,
+                     int off_dtype, int L, int64_t nnz, int64_t rows, int combiner, float* out, void* out_ids, void* stream) {
+  MM_REQUIRE(B >= 0 && nnz >= 0 && rows > 0 && (g || B == 0) && ((ids && out) || nnz == 0), MM_ERR_ARG,
+             "mm_bag_grad_rows: null pointer or negative size");
+  MM_REQUIRE(D == 16 || D == 32 || D == 64 || D == 128, MM_ERR_UNSUPPORTED, "mm_bag_grad_rows: D=%d not in {16,32,64,128}", D);
+  MM_REQUIRE(idx_dtype == MM_I32 || idx_dtype == MM_I64, MM_ERR_ARG, "mm_bag_grad_rows: ids must be int32 or int64");
+  if (offsets) {
+    MM_REQUIRE(off_dtype == MM_I32 || off_dtype == MM_I64, MM_ERR_ARG, "mm_bag_grad_rows: offsets must be int32 or int64");
+    MM_REQUIRE(combiner == MM_COMBINER_MEAN || combiner == MM_COMBINER_SUM || combiner == MM_COMBINER_SQRTN, MM_ERR_UNSUPPORTED,
+               "mm_bag_grad_rows: ragged bags take the mean, sum or sqrtn combiner, got %d", combiner);
+  } else {
+    MM_REQUIRE(L > 0 && nnz == B * (int64_t)L, MM_ERR_ARG, "mm_bag_grad_rows: fixed-length bags need L > 0 and nnz = B * L");
+    MM_REQUIRE(combiner == MM_COMBINER_MEAN || combiner == MM_COMBINER_SUM, MM_ERR_UNSUPPORTED,
+               "mm_bag_grad_rows: fixed-length bags take the mean or sum combiner, got %d", combiner);
+  }
+  MM_REQUIRE(g_stride >= D && (g_stride & 3) == 0, MM_ERR_ARG, "mm_bag_grad_rows: g_stride must be a multiple of 4 and >= D");
+  MM_REQUIRE((((uintptr_t)g | (uintptr_t)out) & 15) == 0, MM_ERR_ALIGN, "mm_bag_grad_rows: g and out must be 16-byte aligned");
+  MM_REQUIRE(((uintptr_t)ids & (idx_dtype == MM_I64 ? 7 : 3)) == 0 &&
+                 (!offsets || ((uintptr_t)offsets & (off_dtype == MM_I64 ? 7 : 3)) == 0) &&
+                 ((uintptr_t)out_ids & (idx_dtype == MM_I64 ? 7 : 3)) == 0,
+             MM_ERR_ALIGN, "mm_bag_grad_rows: ids / offsets / out_ids not aligned to their width");
+  if (nnz == 0) return MM_OK;
+  const long long tasks = offsets ? B + 2 : B;
+  long long blocks = (tasks + 7) / 8;
+  const long long cap = 64LL * mm::sm_count();
+  if (blocks > cap) blocks = cap;
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool i64 = idx_dtype == MM_I64, o64 = offsets && off_dtype == MM_I64;
+  using mm::trs::launch_bag_grad;
+  if (i64 && o64) launch_bag_grad<long long, long long>((unsigned)blocks, st, g, g_stride, ids, offsets, L, B, nnz, rows, combiner, D, out, out_ids);
+  else if (i64) launch_bag_grad<long long, int>((unsigned)blocks, st, g, g_stride, ids, offsets, L, B, nnz, rows, combiner, D, out, out_ids);
+  else if (o64) launch_bag_grad<int, long long>((unsigned)blocks, st, g, g_stride, ids, offsets, L, B, nnz, rows, combiner, D, out, out_ids);
+  else launch_bag_grad<int, int>((unsigned)blocks, st, g, g_stride, ids, offsets, L, B, nnz, rows, combiner, D, out, out_ids);
+  return mm::check_launch("mm_bag_grad_rows");
 }
 
 int mm_fill_i32(int32_t* p, int64_t n, int32_t value, void* stream) {

@@ -904,6 +904,40 @@ def sparse_rows_apply(opt: str, tables, B: int, D: int, hyper: torch.Tensor) -> 
     _cabi.check(_lib().mm_sparse_rows_apply(arr, n, B, D, _cabi.OPTIMIZERS[opt], hyper.data_ptr(), _stream()), "mm_sparse_rows_apply")
 
 
+def bag_grad_rows(g: torch.Tensor, ids: torch.Tensor, offsets: Optional[torch.Tensor], rows: int, combiner: str,
+                  out: torch.Tensor, out_ids: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Backward of gather_bag (offsets given: ids (nnz,), offsets (B+1,)) or gather_seq (offsets None: ids (B, L)) for
+    the pooled-row gradient g (B, D): out (nnz, D) row i = scale(i) * g[bag(i)], zero for ids outside [0, rows)
+    (mm_bag_grad_rows).  Every row of `out` is written.  out_ids (nnz,), the ids' dtype: the id of every row that carries
+    a gradient, -1 for positions no bag covers and ids outside [0, rows) — the indices for sparse_rows_apply."""
+    _dev(g, "g", torch.float32), _dev(ids, "ids"), _dev(out, "out", torch.float32)
+    if combiner not in COMBINERS:
+        raise ValueError(f"unknown combiner {combiner!r}")
+    if g.dim() != 2:
+        raise ValueError(f"g must be (B, D), got {tuple(g.shape)}")
+    B, D = g.shape
+    if not ids.is_contiguous():
+        raise ValueError("ids must be contiguous")
+    nnz = ids.numel()
+    if tuple(out.shape) != (nnz, D) or not out.is_contiguous():
+        raise ValueError(f"out must be contiguous ({nnz}, {D}), got {tuple(out.shape)}")
+    if offsets is None:
+        if ids.dim() != 2 or ids.shape[0] != B:
+            raise ValueError(f"fixed-length bags need ids (B={B}, L), got {tuple(ids.shape)}")
+        L, off_ptr, off_dt = ids.shape[1], None, MM_I32
+    else:
+        _dev(offsets, "offsets")
+        if offsets.numel() != B + 1 or not offsets.is_contiguous():
+            raise ValueError(f"offsets must be contiguous with B+1={B + 1} elements, got {tuple(offsets.shape)}")
+        L, off_ptr, off_dt = 0, offsets.data_ptr(), _idx_dtype(offsets, "offsets")
+    if out_ids is not None and (_dev(out_ids, "out_ids", ids.dtype).numel() != nnz or not out_ids.is_contiguous()):
+        raise ValueError(f"out_ids must be contiguous with {nnz} elements of the ids' dtype")
+    _cabi.check(_lib().mm_bag_grad_rows(g.data_ptr(), B, D, _row_stride(g, "g"), ids.data_ptr(), _idx_dtype(ids, "ids"), off_ptr, off_dt,
+                                        L, nnz, int(rows), COMBINERS[combiner], out.data_ptr(), _ptr(out_ids), _stream()),
+                "mm_bag_grad_rows")
+    return out
+
+
 def dense_apply(opt: str, w: torch.Tensor, grad: torch.Tensor, state1: Optional[torch.Tensor], state2: Optional[torch.Tensor],
                 hyper: torch.Tensor, grad_scale: float = 1.0) -> None:
     """Optimizer step over a flat fp32 arena; grad is scaled by grad_scale and cleared (mm_dense_apply)."""

@@ -15,6 +15,12 @@ What a step launches (DLRM, bottom [.., D], top [...], BinaryOutput):
               parameter arena, mm_sparse_rows_apply (duplicate ids summed, one update per touched row), mm_split_weights
               refresh of the tensor-core operand copies (in place)
 
+Multi-hot features (ragged `name__values` + `name__offsets`, or (B, L) id matrices; combiners mean / sum / sqrtn) are pooled
+by mm_gather_bag / mm_gather_seq into a (B, D) buffer that the lookup + interaction kernels read as one more table of B rows
+at ids 0..B-1, so those kernels serve them unchanged; the backward's slice of that "table" is the pooled-row gradient, which
+mm_bag_grad_rows expands to one scaled row per id for one mm_sparse_rows_apply call per multi-hot table.  Ragged features are
+trained eagerly (their number of ids changes per batch); fixed-length ones can be captured like one-hot features.
+
 All Dense variables of the model are re-homed into ONE flat fp32 arena (gradients and optimizer slots mirror its layout), so
 the dense update is one launch and data-parallel training needs one all-reduce.  Every buffer is static: a step can be
 captured into a CUDA graph (`DLRMTrainer.capture()` / `replay()`), the learning rate lives in device memory.
@@ -28,7 +34,7 @@ import torch
 
 from . import _cabi, ops
 from .blocks import DLRM, MLP, _Dense
-from .core import default_device, get_feature
+from .core import batch_size_of, default_device, get_feature
 
 INT32_MAX = 2**31 - 1
 DENSE_PATH_MAX_ROWS = 131072  # tables up to this size accumulate duplicate ids in a dense (rows, D) gradient
@@ -280,14 +286,83 @@ class DLRMTrainer:
         self.logits = torch.zeros(B, **f32)
         self.loss = torch.zeros(1, **f32)
         self.oob = emb.counter(self.device)
+        # multi-hot features (ragged bags, (B, L) id matrices), by table position: pooled rows, their operand copy, the
+        # expanded row gradients; created on the first batch that carries the feature as a bag (see _indices)
+        self._bag_bufs: Dict[int, dict] = {}
+        self._iota: Optional[torch.Tensor] = None
+        self._bags: Dict[int, dict] = {}
         self.steps = 0
         self._graph = None
         self._static: Optional[Dict[str, torch.Tensor]] = None
         self._static_y: Optional[torch.Tensor] = None
 
     # ---- one step on device tensors ------------------------------------------------------------------------------
-    def _indices(self, inputs) -> List[torch.Tensor]:
-        return [ops.fused_ids(get_feature(inputs, f)) for f in self.feats]
+    def _indices(self, inputs, b: Optional[int] = None) -> List[torch.Tensor]:
+        """Ids the lookup + interaction kernels read per table.  A multi-hot feature is pooled first (gather_bag /
+        gather_seq, the forward's combiner) into a (B, D) buffer that those kernels then read as one more table of b rows
+        at ids 0..b-1; its backward returns the pooled-row gradient, which _bag_grads expands to one row per id."""
+        idx: List[torch.Tensor] = []
+        self._bags = {}
+        for t, f in enumerate(self.feats):
+            x = get_feature(inputs, f)
+            kind = self.tables[t].lookup_kind(x)
+            if kind == "onehot":
+                idx.append(ops.fused_ids(x))
+                continue
+            if b is None:  # the pooled rows and the ids that read them must agree on the batch size
+                b = batch_size_of(inputs)
+            self._bags[t] = self._pool(t, f, x, kind, b)
+            idx.append(self._iota[:b])
+        return idx
+
+    def _pool(self, t: int, f: str, x, kind: str, b: int) -> dict:
+        tb, D = self.tables[t], self.D
+        comb = tb.sequence_combiner or "mean"
+        if comb == "max":
+            raise NotImplementedError(f"feature {f!r}: training with the 'max' sequence combiner is not implemented")
+        if self.group is not None:  # gather_slices exchanges (T, B, D) slices: one row per sample and table
+            raise NotImplementedError(f"feature {f!r}: training multi-hot features with a process group is not implemented")
+        buf = self._bag_bufs.get(t)
+        if buf is None:
+            if self._iota is None:
+                self._iota = torch.arange(self.B, dtype=torch.int32, device=self.device)
+            buf = self._bag_bufs[t] = dict(
+                pooled=torch.zeros((self.B, D), dtype=torch.float32, device=self.device),
+                split=torch.zeros((self.B, 2 * ops.tc_padded_k(D)), dtype=torch.bfloat16, device=self.device) if self.operand_rows else None,
+                rows=None, ids=None)
+        pooled = buf["pooled"][:b]
+        if kind == "bag":
+            values, offsets = x
+            ids, offs = ops.as_index(values).reshape(-1), ops.as_index(offsets)
+            ops.gather_bag(tb.table, ids, offs, comb, pooled, 0, self.oob)
+        else:
+            if comb == "sqrtn":
+                raise ValueError(f"feature {f!r}: sequence_combiner 'sqrtn' is only defined for ragged inputs")
+            ids, offs = ops.as_index(x).reshape(x.shape[0], -1).contiguous(), None
+            ops.gather_seq(tb.table, ids, comb, pooled, 0, self.oob)
+        nnz = ids.numel()
+        if buf["rows"] is None or buf["rows"].shape[0] < nnz:  # ragged: grows to the largest batch; fixed length: b * L
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError(f"feature {f!r}: the expanded gradient buffer cannot grow during graph capture")
+            buf["rows"] = torch.empty((nnz, D), dtype=torch.float32, device=self.device)
+        if kind == "bag" and (buf["ids"] is None or buf["ids"].shape[0] < nnz or buf["ids"].dtype != ids.dtype):
+            # the update's indices: a ragged batch's offsets need not cover every value (offsets[0] > 0, offsets[B] < nnz);
+            # the expansion marks such positions -1 so that no row the batch does not hold is updated
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError(f"feature {f!r}: the expanded id buffer cannot grow during graph capture")
+            buf["ids"] = torch.empty(max(nnz, 1), dtype=ids.dtype, device=self.device)
+        split = None
+        if self.operand_rows:
+            split = buf["split"][:b]
+            ops.split_rows(pooled, out=split)
+        return dict(ids=ids, offsets=offs, comb=comb, pooled=pooled, split=split, rows=buf["rows"][:nnz],
+                    apply_ids=buf["ids"][:nnz] if kind == "bag" else ids.reshape(-1))
+
+    def _bag_grads(self) -> None:
+        """Pooled-row gradient (the feature's slice of the interaction backward) -> one scaled row per id."""
+        for t, bg in self._bags.items():
+            ops.bag_grad_rows(self._slices[t], bg["ids"], bg["offsets"], self.tables[t].table.shape[0], bg["comb"], bg["rows"],
+                              out_ids=bg["apply_ids"] if bg["offsets"] is not None else None)
 
     def forward_backward(self, inputs: Dict[str, torch.Tensor], targets: torch.Tensor, sample_weight=None) -> None:
         """Forward (activations saved), loss and backward: fills the gradient arena and the IndexedSlices.  Batches smaller
@@ -316,8 +391,9 @@ class DLRMTrainer:
             ops.dense_tc(op, K, self._wsplit[i], l.units, l.bias, l.activation, out_f32=h[i], out_split=nxt)
             op, K = nxt, l.units
         # -- lookup + interaction (fp32 rows)
-        idx = self._indices(inputs)
-        tabs = [t.table for t in self.tables]
+        idx = self._indices(inputs, b)
+        tabs = [self._bags[t]["pooled"] if t in self._bags else tb.table for t, tb in enumerate(self.tables)]
+        mirrors = [self._bags[t]["split"] if t in self._bags else tb._mirror for t, tb in enumerate(self.tables)]
         rows = [t.shape[0] for t in tabs]
         tslots = [self.slots[f] for f in self.feats]
         bslot = self.slots["bottom_block"]
@@ -325,7 +401,7 @@ class DLRMTrainer:
         if self.operand_rows:
             # operand-format rows in, split-bf16 operand of the top tower out: no fp32 copy of [bottom | interactions] exists
             A_view = None
-            ops.dlrm_lookup_interact([t._mirror for t in self.tables], idx, tslots, rows, D, v(self.h_split[-1]), bslot,
+            ops.dlrm_lookup_interact(mirrors, idx, tslots, rows, D, v(self.h_split[-1]), bslot,
                                      v(self.A_split), self.oob, operand_rows=True)
         else:
             A_view = self.A[:b, :self.OW]
@@ -356,11 +432,12 @@ class DLRMTrainer:
         # -- interaction + lookup backward
         self._slices = [self.slices[t][:b] for t in range(len(tabs))]
         if self.operand_rows:
-            ops.dlrm_interact_backward([t._mirror for t in self.tables], idx, tslots, rows, D, v(self.h_split[-1]), bslot, dA_view,
+            ops.dlrm_interact_backward(mirrors, idx, tslots, rows, D, v(self.h_split[-1]), bslot, dA_view,
                                        self._slices, dh[-1], mask_bottom=self.bottom[-1].activation == "relu", operand_rows=True)
         else:
             ops.dlrm_interact_backward(tabs, idx, tslots, rows, D, h[-1], bslot, dA_view, self._slices, dh[-1],
                                        mask_bottom=self.bottom[-1].activation == "relu")
+        self._bag_grads()
         # -- bottom tower backward
         for i in range(nb - 1, -1, -1):
             l = self.bottom[i]
@@ -407,9 +484,16 @@ class DLRMTrainer:
         tabs = []
         for t, tb in enumerate(self.tables):
             mirror = tb._mirror if (tb._mirror is not None and tb._mirror.shape[0] == tb.table.shape[0]) else None
-            tabs.append(dict(weights=tb.table, indices=idx[t], grad_rows=slices[t], rep_map=self.rep[t], state1=self.tstate1[t],
-                             state2=self.tstate2[t], mirror=mirror, dense_grad=self.tdense[t]))
-        ops.sparse_rows_apply(self.opt.kind, tabs, Bt, self.D, self.hyper)
+            tab = dict(weights=tb.table, indices=idx[t], grad_rows=slices[t], rep_map=self.rep[t], state1=self.tstate1[t],
+                       state2=self.tstate2[t], mirror=mirror, dense_grad=self.tdense[t])
+            bag = self._bags.get(t)
+            if bag is None:
+                tabs.append(tab)
+            elif bag["rows"].shape[0] > 0:  # a multi-hot table: its own call over the nnz expanded rows
+                tab.update(indices=bag["apply_ids"], grad_rows=bag["rows"])
+                ops.sparse_rows_apply(self.opt.kind, [tab], bag["rows"].shape[0], self.D, self.hyper)
+        if tabs:
+            ops.sparse_rows_apply(self.opt.kind, tabs, Bt, self.D, self.hyper)
         for l, ws in zip(self.bottom + self.top, self._wsplit):
             ops.split_weights(l.kernel, out=ws)
 
@@ -434,6 +518,10 @@ class DLRMTrainer:
         buffers (e.g. views of one packed device buffer that a single H2D copy refreshes before replay())."""
         if self.world > 1:
             raise NotImplementedError("graph capture of the data-parallel step is not implemented")
+        for f in self.feats:
+            if isinstance(get_feature(inputs, f), tuple):
+                raise NotImplementedError(f"graph capture with the ragged feature {f!r} is not implemented: its number of ids "
+                                          "changes from batch to batch (train it eagerly, or feed it as a fixed-length (B, L) matrix)")
         self._static = {k: (v.clone() if clone else v) for k, v in inputs.items()}
         self._static_y = targets.clone() if clone else targets
         self.model.defer_index_check(True)
