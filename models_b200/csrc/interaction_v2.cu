@@ -7,8 +7,8 @@
 //     owned by lane r (tables arrive sorted by slot, so row == slot), a row's source pointer travels
 //     with two shuffles, and because row = 4*i + lane/8 the XOR swizzle of a lane's destination does
 //     not depend on i: every destination is `lane constant + immediate`.  7 iterations x (2 SHFL +
-//     2 IADD + 2 LDGSTS) per sample.  Bad ids read a zero row in global memory (no zero-fill operand,
-//     no predicates).
+//     2 IADD + 2 LDGSTS) per sample at F = 27; the operand-format path runs all 8 without a branch.  Bad ids
+//     read a zero row in global memory (no zero-fill operand, no predicates).
 //   * fragment loads: the k index of a 16-wide k-step is permuted (lane t takes floats 4t..4t+3 and
 //     calls them k = 2t, 2t+1, 2t+8, 2t+9).  A and B fragments are the same registers (B = X^T), so the
 //     permutation cancels in the dot products and one LDS.128 replaces two LDS.64.
@@ -202,7 +202,9 @@ interact_v2_kernel(const __grid_constant__ LookupParams lk, const Params p) {
       const uint32_t src_lo = (uint32_t)(uintptr_t)my_src, src_hi = (uint32_t)((uintptr_t)my_src >> 32);
 #pragma unroll
       for (int i = 0; i < IMAX; ++i) {
-        if (i * R < p.rows) {  // kernel parameter: uniform branch
+        // PS: all 8 iterations, the copies of rows past p.rows predicated off (no branch and divergence check per pair of
+        // shuffles).  Otherwise a kernel parameter: uniform branch.
+        if (PS || i * R < p.rows) {
           const int row = i * R + rl;
           const uint32_t lo = __shfl_sync(0xffffffffu, src_lo, row);
           const uint32_t hi = __shfl_sync(0xffffffffu, src_hi, row);
