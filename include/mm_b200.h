@@ -269,12 +269,23 @@ int mm_dense_tc_head(const void* a_split, int64_t M, int K, int Kp, const void* 
  * Returns MM_ERR_UNSUPPORTED when the tower does not fit (caller then chains mm_dense_tc);
  * mm_mlp_tc_supported(K, n_layers, widths, with_head) answers that question (1 / 0) without launching:
  * 2..4 layers, widths <= 128, head only after <= 32 units, resident weights + two pipeline stages
- * within 227 KB of shared memory. */
+ * within 227 KB of shared memory (with_head = 2: the multi-head epilogue of mm_mlp_tc_heads). */
 int mm_mlp_tc_supported(int K, int n_layers, const int* widths, int with_head);
 int mm_mlp_tc(const void* a_split, int64_t M, int K, int n_layers, const void* const* w_split,
               const int* widths, const float* const* bias, const int* acts, float* out,
               int64_t out_stride, const float* head_w, float head_b, int head_act, float* head_out,
               void* stream);
+
+/* mm_mlp_tc with n_heads <= 8 fused output heads instead of one (OutputBlock's BinaryOutput / RegressionOutput heads,
+ * outputs/block.py:32-131, outputs/regression.py:35-58, on the same tower output):
+ *   heads_out[h * M + m] = heads_act[h](h_n[m,:] . heads_w[:, h] + heads_b[h])
+ * heads_w (widths[n-1], n_heads) Keras layout, heads_b (n_heads,) device or null (read on the device, so a captured graph
+ * follows training), heads_act: host array of MM_ACT_*; heads_out (n_heads, M): each head's (M, 1) is a contiguous slice.
+ * widths[n-1] <= 32; mm_mlp_tc_supported(K, n_layers, widths, 2) says whether the tower fits with this epilogue.  Only the
+ * heads are written (no fp32 rows). */
+int mm_mlp_tc_heads(const void* a_split, int64_t M, int K, int n_layers, const void* const* w_split, const int* widths,
+                    const float* const* bias, const int* acts, int n_heads, const float* heads_w, const float* heads_b,
+                    const int* heads_act, float* heads_out, void* stream);
 
 /* mm_mlp_tc whose last layer also (or only: out may be NULL) leaves its rows as split-bf16 rows
  * out_operand (M, 2 * widths[n-1]) bf16 = [hi | lo] per row (widths[n-1] % 4 == 0; the mm_split_rows layout when the
@@ -410,6 +421,7 @@ int mm_init_uniform_hash_rows(float* w, int64_t local_rows, int D, uint64_t seed
  *                               z = x.w + b;  *loss_sum += sum_i sw_i (max(z,0) - z y + log(1 + e^-|z|)) / M;
  *                               dz = sw_i (sigmoid(z) - y) / M;  dx = dz w (zeroed where x <= 0 when mask_relu);
  *                               dw += x^T dz;  *db += sum dz.      loss_sum / dw / db are ACCUMULATED (zero them first).
+ *   mm_heads_fwd_bwd          the same for H <= 8 BinaryOutput / RegressionOutput heads with loss weights (see below).
  *   mm_dense_wgrad            dW (K, N) += X^T dZ,  db (N) += column sums of dZ   (db nullable; accumulated)
  *   mm_dense_dgrad            dX (M, K) = dZ (M, N) W^T, W the Keras kernel (K, N), N <= 128; `mask` (M, K) nullable:
  *                             dX is zeroed where mask <= 0 (mask = the layer's input = the previous layer's relu
@@ -481,6 +493,28 @@ typedef struct {
 int mm_bce_head_fwd_bwd(const float* x, int64_t M, int K, int64_t x_stride, const float* w, const float* bias,
                         const void* targets, int target_dtype, const float* sample_weight, float* logits,
                         float* loss_sum, float* dx, int64_t dx_stride, int mask_relu, float* dw, float* db, void* stream);
+/* Loss kinds of mm_heads_fwd_bwd: BinaryOutput (sigmoid + binary cross-entropy on the logits) and RegressionOutput
+ * (linear + squared error). */
+#define MM_LOSS_BCE 0
+#define MM_LOSS_MSE 1
+/* H <= 8 output heads Dense(K -> 1) on the same x (M, K), K <= 256 (OutputBlock, outputs/block.py:32-131; BinaryOutput
+ * outputs/classification.py:114, RegressionOutput outputs/regression.py:35-58; Keras compile(loss_weights) sums the
+ * weighted per-output losses), forward AND backward in one pass over x:
+ *   z_h = x . W[:, h] + b_h                 W (K, H) Keras layout, b (H,) device or null
+ *   l_h,i = BCE: max(z,0) - z y + log(1 + e^-|z|)  |  MSE: (z - y)^2          (loss_kind[h] = MM_LOSS_BCE / MM_LOSS_MSE)
+ *   loss_h = sum_i sw_i l_h,i / M;  loss (1 + H) += [sum_h lambda_h loss_h, loss_0 .. loss_{H-1}]   (lambda = loss_weight)
+ *   dz_h = lambda_h sw_i (sigmoid(z_h) - y) / M  |  lambda_h sw_i 2 (z_h - y) / M
+ *   dx = sum_h dz_h W[:, h]^T (written once; zeroed where x <= 0 when mask_relu);  dW[:, h] += x^T dz_h;  db_h += sum dz_h
+ *   logits (H, M) nullable: z_h.  loss / dW / db are ACCUMULATED (zero them first).
+ * loss_kind, loss_weight, targets, target_dtypes, sample_weights are HOST arrays of H entries; targets[h] is (M,) of
+ * target_dtypes[h] (MM_I32 .. MM_F64); sample_weights (nullable array, entries nullable) holds (M,) fp32 per head — the
+ * same pointer for every head when the weights are shared.  targets == NULL: forward only — logits (H, M) receives the
+ * activated predictions (sigmoid(z) / z) and nothing else is read or written.  mm_bce_head_fwd_bwd is H = 1 with one
+ * BCE head and loss_weight 1 (its loss_sum is the total alone). */
+int mm_heads_fwd_bwd(const float* x, int64_t M, int K, int64_t x_stride, int H, const float* w, const float* bias,
+                     const int* loss_kind, const float* loss_weight, const void* const* targets, const int* target_dtypes,
+                     const float* const* sample_weights, float* logits, float* loss, float* dx, int64_t dx_stride,
+                     int mask_relu, float* dw, float* db, void* stream);
 int mm_dense_wgrad(const float* x, int64_t M, int K, int64_t x_stride, const float* dz, int N, int64_t dz_stride,
                    float* dw, float* db, void* stream);
 /* mm_dense_wgrad with X given as split-bf16 rows (M, 2*Kp) = [hi | lo] (mm_split_rows layout, Kp = mm_tc_padded_k(K)): the

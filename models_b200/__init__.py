@@ -19,7 +19,8 @@ from .blocks import BatchNormalization, FMBlock, FMPairwiseInteraction  # noqa: 
 from .retrieval import (CategoricalOutput, ContrastiveOutput, Encoder, InBatchSampler, InBatchSamplerV2,  # noqa: F401
                         ItemRetrievalScorer, ItemRetrievalTask, L2Norm, PopularityBasedSamplerV2, TwoTowerBlock,
                         log_uniform_sampling_probs)
-from .models import (BinaryClassificationTask, BinaryOutput, DCNModel, DeepFMModel, DLRMModel, Model,  # noqa: F401
+from .models import (BinaryClassificationTask, BinaryOutput, DCNModel, DeepFMModel, DLRMModel, Model, OutputBlock,  # noqa: F401
+                     ParallelOutputs, RegressionOutput,
                      RetrievalModel, RetrievalModelV2, TwoTowerModel, TwoTowerModelV2)
 from .topk import (AvgPrecisionAt, BruteForce, MRRAt, NDCGAt, PrecisionAt, RecallAt, TopKEncoder,  # noqa: F401
                    TopKIndexBlock, TopKPrediction, encode_candidates, unique_rows_by_features)

@@ -66,6 +66,7 @@ class SparseTable(C.Structure):
 
 
 OPTIMIZERS = {"sgd": 0, "adagrad": 1, "adam": 2}
+LOSS_KINDS = {"binary_crossentropy": 0, "mse": 1}  # MM_LOSS_BCE / MM_LOSS_MSE
 HYPER_LR, HYPER_BETA1, HYPER_BETA2, HYPER_EPS, HYPER_STEP, HYPER_LR_T, HYPER_COUNT = 0, 1, 2, 3, 4, 5, 8
 
 
@@ -117,6 +118,8 @@ SIGNATURES = {
     "mm_mlp_tc_supported": (_i, [_i, _i, C.POINTER(C.c_int), _i]),
     "mm_mlp_tc": (_i, [_vp, _i64, _i, _i, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_void_p), C.POINTER(C.c_int),
                        _vp, _i64, _vp, _f, _i, _vp, _vp]),
+    "mm_mlp_tc_heads": (_i, [_vp, _i64, _i, _i, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_void_p), C.POINTER(C.c_int),
+                             _i, _vp, _vp, C.POINTER(C.c_int), _vp, _vp]),
     "mm_mlp_tc_operand_out": (_i, [_vp, _i64, _i, _i, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_void_p),
                                    C.POINTER(C.c_int), _vp, _i64, _vp, _vp]),
     "mm_tower2_small_supported": (_i, [_i, _i, _i]),
@@ -135,6 +138,8 @@ SIGNATURES = {
     "mm_deepfm_head": (_i, [C.POINTER(LookupTable), C.POINTER(C.c_int64), _i, _i64, _i, C.POINTER(ConcatPiece), C.POINTER(C.c_int64), _i,
                             _vp, _vp, _vp, _i64, _vp, _vp, _i, _vp, _vp, _vp]),
     "mm_bce_head_fwd_bwd": (_i, [_vp, _i64, _i, _i64, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i64, _i, _vp, _vp, _vp]),
+    "mm_heads_fwd_bwd": (_i, [_vp, _i64, _i, _i64, _i, _vp, _vp, C.POINTER(C.c_int), C.POINTER(C.c_float), C.POINTER(C.c_void_p),
+                              C.POINTER(C.c_int), C.POINTER(C.c_void_p), _vp, _vp, _vp, _i64, _i, _vp, _vp, _vp]),
     "mm_dense_wgrad": (_i, [_vp, _i64, _i, _i64, _vp, _i, _i64, _vp, _vp, _vp]),
     "mm_dense_wgrad_split": (_i, [_vp, _i64, _i, _i, _vp, _i, _i64, _vp, _vp, _vp]),
     "mm_dense_dgrad": (_i, [_vp, _i64, _i, _i64, _vp, _i, _vp, _i64, _vp, _i64, _vp]),

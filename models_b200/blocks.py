@@ -63,7 +63,7 @@ def table_mirror() -> bool:
 
 
 def run_dense_chain(x: Optional[torch.Tensor], layers: "List[_Dense]", a_split: Optional[torch.Tensor] = None,
-                    K: Optional[int] = None, operand_out: bool = False) -> torch.Tensor:
+                    K: Optional[int] = None, operand_out: bool = False, heads=None) -> torch.Tensor:
     """A chain of Dense layers on one input matrix.  operand_out=True: the result rows come back as bf16 split rows
     (B, 2*Kp) = [hi | lo] (the interaction kernel's operand format) — directly from the whole-tower kernel's last
     epilogue when it applies, by one mm_split_rows pass over the fp32 result otherwise.
@@ -71,7 +71,30 @@ def run_dense_chain(x: Optional[torch.Tensor], layers: "List[_Dense]", a_split: 
     tensor-core engine ("auto"/"tc"): x is split once into bf16 (hi, lo); every layer is one
     wgmma launch whose epilogue (bias + activation) directly emits the NEXT layer's split-bf16
     operand, so intermediate activations never exist in fp32 in HBM; the last layer writes fp32.
-    "fp32" engine: exact CUDA-core kernels (parity anchor)."""
+    "fp32" engine: exact CUDA-core kernels (parity anchor).
+
+    heads (models.ParallelOutputs): the chain is followed by H output heads; the result is their (H, B) activated
+    predictions — from the whole-tower kernel's multi-head epilogue (mm_mlp_tc_heads) when it applies, else by
+    mm_heads_fwd_bwd (forward only) over the last layer's fp32 rows."""
+    if heads is not None:
+        hl = heads.to_call
+        dev = (x if x is not None else a_split).device
+        B = (x if x is not None else a_split).shape[0]
+        width = K if a_split is not None else x.shape[1]
+        for l in layers:
+            l.build(width, dev)
+            width = l.units
+        out = torch.empty((len(heads.outputs), B), dtype=torch.float32, device=dev)
+        if _use_tc() and width <= 32 and ops.mlp_tc_supported(K if a_split is not None else x.shape[1], [l.units for l in layers], heads=True):
+            _LAST_PATH[0] = "mlp_tc"
+            a = a_split if a_split is not None else ops.split_rows(x)
+            return ops.mlp_tc_heads(a, K if a_split is not None else x.shape[1], [l.split_kernel() for l in layers],
+                                    [l.units for l in layers], [l.bias for l in layers], [l.activation for l in layers],
+                                    hl.kernel, hl.bias, heads.activations, out)
+        if a_split is not None and not _use_tc():
+            raise ValueError("the fp32 dense engine needs an fp32 input")
+        h = run_dense_chain(x, layers, a_split=a_split, K=K)
+        return ops.heads_fwd_bwd(h.contiguous(), hl.kernel, hl.bias, heads.losses, None, out)
     if a_split is not None:  # producer (interaction kernel) already emitted the split-bf16 operand
         device, B, a = a_split.device, a_split.shape[0], a_split
     else:

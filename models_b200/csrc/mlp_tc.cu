@@ -38,6 +38,7 @@ constexpr int MMA_K = 16;
 constexpr int kConsumerWarps = 8;
 constexpr int kThreads = 32 * (kConsumerWarps + 1);
 constexpr int kMaxChain = 3;
+constexpr int kMaxHeads = 8;
 constexpr uint32_t A_TILE_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KB
 
 struct ChainLayer {
@@ -60,6 +61,12 @@ struct Params {
   float head_b;
   int head_act;
   float* head_out;
+  // mm_mlp_tc_heads: n_heads <= 8 Dense(N_last -> 1) heads, weights (N_last, n_heads) Keras layout, biases (n_heads,) device
+  int n_heads;
+  const float* heads_w;
+  const float* heads_b;
+  int heads_act[kMaxHeads];
+  float* heads_out;  // (n_heads, M)
 };
 
 // One chain layer's MMAs for a compile-time width NP and KS = Kp / 16 k-steps: three straight-line batches of HGMMAs under one
@@ -106,8 +113,10 @@ __device__ __forceinline__ void chain_mma(int np, float (&acc)[64], const uint32
 }
 
 // N1P = padded layer-1 width (16 .. 128), a compile-time constant: each layer-1 HGMMA is one fixed instruction, not a
-// switch on the width, and ptxas need not fence every one of them on its own
-template <int N1P>
+// switch on the width, and ptxas need not fence every one of them on its own.  HEADS: the multi-head epilogue of
+// mm_mlp_tc_heads (head_s[kMaxHeads][128], biases from device memory); the single-head kernel of mm_mlp_tc is its own
+// instantiation so that its code does not change.
+template <int N1P, bool HEADS>
 __global__ void __launch_bounds__(kThreads, 1)
 mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW1,
               const __grid_constant__ CUtensorMap tmC0, const __grid_constant__ CUtensorMap tmC1,
@@ -124,7 +133,7 @@ mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
   uint64_t* empty_bar = bars + p.stages;            // [stages] one arrive per consumer warp
   uint64_t* w_full = bars + 2 * p.stages;           // resident weights landed
   float* bias_s = reinterpret_cast<float*>(bars + 2 * p.stages + 2);  // [kMaxChain + 1][128], zero padded
-  float* head_s = bias_s + (kMaxChain + 1) * 128;                     // [128], zero padded
+  float* head_s = bias_s + (kMaxChain + 1) * 128;                     // [128] ([kMaxHeads][128] + [kMaxHeads] biases: HEADS), zero padded
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long long tiles = (p.M + BLOCK_M - 1) / BLOCK_M;
@@ -146,7 +155,15 @@ mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
     const int N = l == 0 ? p.N1 : (l <= p.n_chain ? p.c[l - 1].N : 0);
     bias_s[i] = (p.bias[l] != nullptr && n < N) ? p.bias[l][n] : 0.0f;
   }
-  if (threadIdx.x < 128) {
+  if (HEADS) {
+    const int Nl = p.n_chain ? p.c[p.n_chain - 1].N : p.N1;
+    for (int i = threadIdx.x; i < kMaxHeads * 128; i += kThreads) {
+      const int hh = i >> 7, n = i & 127;
+      head_s[i] = (hh < p.n_heads && n < Nl) ? p.heads_w[n * p.n_heads + hh] : 0.0f;
+    }
+    if (threadIdx.x < kMaxHeads)
+      head_s[kMaxHeads * 128 + threadIdx.x] = ((int)threadIdx.x < p.n_heads && p.heads_b) ? p.heads_b[threadIdx.x] : 0.0f;
+  } else if (threadIdx.x < 128) {
     const int Nl = p.n_chain ? p.c[p.n_chain - 1].N : p.N1;
     head_s[threadIdx.x] = (p.head_w != nullptr && (int)threadIdx.x < Nl) ? p.head_w[threadIdx.x] : 0.0f;
   }
@@ -282,7 +299,24 @@ mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             const long long row = tile * BLOCK_M + frow + 8 * h;
-            if (p.head_w) {  // fused Dense(N -> 1): Np <= 32; the four lanes of a quad hold a row's columns
+            if (HEADS) {  // H fused Dense(N -> 1) heads: Np <= 32; the four lanes of a quad hold a row's columns
+#pragma unroll
+              for (int hh = 0; hh < kMaxHeads; ++hh) {
+                if (hh < p.n_heads) {
+                  const float* hw = head_s + hh * 128;
+                  float hsum = 0.0f;
+#pragma unroll
+                  for (int j = 0; j < 4; ++j) {
+                    hsum = fmaf(acc[4 * j + 2 * h], hw[8 * j + c2], hsum);
+                    hsum = fmaf(acc[4 * j + 2 * h + 1], hw[8 * j + c2 + 1], hsum);
+                  }
+                  hsum += __shfl_xor_sync(0xffffffffu, hsum, 1);
+                  hsum += __shfl_xor_sync(0xffffffffu, hsum, 2);
+                  if ((lane & 3) == 0 && row < p.M)
+                    p.heads_out[hh * p.M + row] = apply_act(hsum + head_s[kMaxHeads * 128 + hh], p.heads_act[hh]);
+                }
+              }
+            } else if (p.head_w) {  // fused Dense(N -> 1): Np <= 32; the four lanes of a quad hold a row's columns
               float hsum = 0.0f;
 #pragma unroll
               for (int j = 0; j < 4; ++j) {
@@ -325,7 +359,7 @@ mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
 }  // namespace mm
 
 // Fills the shape-dependent part of Params and the shared-memory size; false when the tower does not fit.
-static bool plan_tower(int K, int n_layers, const int* widths, mm::mlp::Params& p, size_t& smem) {
+static bool plan_tower(int K, int n_layers, const int* widths, mm::mlp::Params& p, size_t& smem, bool heads = false) {
   using namespace mm::mlp;
   memset(&p, 0, sizeof(p));
   p.K1p = mm_tc_padded_k(K);
@@ -346,7 +380,8 @@ static bool plan_tower(int K, int n_layers, const int* widths, mm::mlp::Params& 
   p.w_bytes = w_off;
   // ring slot = one half ({A_hi, W_hi} or {A_lo, W_lo}) of a k-block
   const size_t stage_bytes = (size_t)A_TILE_BYTES + (size_t)p.N1p * BLOCK_K * 2;
-  const size_t fixed = 1024 + (size_t)p.w_bytes + 40 * sizeof(uint64_t) + ((kMaxChain + 1) * 128 + 128) * sizeof(float);
+  const size_t head_floats = heads ? kMaxHeads * 128 + kMaxHeads : 128;
+  const size_t fixed = 1024 + (size_t)p.w_bytes + 40 * sizeof(uint64_t) + ((kMaxChain + 1) * 128 + head_floats) * sizeof(float);
   if (fixed + 4 * stage_bytes > 227 * 1024) return false;
   int stages = (int)((227 * 1024 - fixed) / stage_bytes);
   if (stages > 12) stages = 12;
@@ -354,7 +389,7 @@ static bool plan_tower(int K, int n_layers, const int* widths, mm::mlp::Params& 
   if (stages > 4 * kb1) stages = 4 * kb1 > 4 ? 4 * kb1 : 4;
   p.stages = stages;
   smem = 1024 + stages * stage_bytes + p.w_bytes + (2 * stages + 2) * sizeof(uint64_t) +
-         ((kMaxChain + 1) * 128 + 128) * sizeof(float);
+         ((kMaxChain + 1) * 128 + head_floats) * sizeof(float);
   return true;
 }
 
@@ -367,7 +402,7 @@ int mm_mlp_tc_supported(int K, int n_layers, const int* widths, int with_head) {
   if (with_head && widths[n_layers - 1] > 32) return 0;
   mm::mlp::Params p;
   size_t smem = 0;
-  return plan_tower(K, n_layers, widths, p, smem) ? 1 : 0;
+  return plan_tower(K, n_layers, widths, p, smem, with_head > 1) ? 1 : 0;
 }
 
 }  // extern "C"
@@ -376,24 +411,26 @@ typedef void (*MlpKernel)(const CUtensorMap, const CUtensorMap, const CUtensorMa
                           const mm::mlp::Params);
 
 // one instantiation per padded layer-1 width mm_tc_padded_n can return
+template <bool HEADS>
 static MlpKernel kernel_for(int n1p) {
   using namespace mm::mlp;
   switch (n1p) {
-    case 16: return mlp_tc_kernel<16>;
-    case 32: return mlp_tc_kernel<32>;
-    case 48: return mlp_tc_kernel<48>;
-    case 64: return mlp_tc_kernel<64>;
-    case 80: return mlp_tc_kernel<80>;
-    case 96: return mlp_tc_kernel<96>;
-    case 112: return mlp_tc_kernel<112>;
-    case 128: return mlp_tc_kernel<128>;
+    case 16: return mlp_tc_kernel<16, HEADS>;
+    case 32: return mlp_tc_kernel<32, HEADS>;
+    case 48: return mlp_tc_kernel<48, HEADS>;
+    case 64: return mlp_tc_kernel<64, HEADS>;
+    case 80: return mlp_tc_kernel<80, HEADS>;
+    case 96: return mlp_tc_kernel<96, HEADS>;
+    case 112: return mlp_tc_kernel<112, HEADS>;
+    case 128: return mlp_tc_kernel<128, HEADS>;
   }
   return nullptr;
 }
 
 static int mlp_tc_impl(const void* a_split, int64_t M, int K, int n_layers, const void* const* w_split, const int* widths,
                        const float* const* bias, const int* acts, float* out, int64_t out_stride, const float* head_w,
-                       float head_b, int head_act, float* head_out, void* out_operand, void* stream) {
+                       float head_b, int head_act, float* head_out, void* out_operand, void* stream,
+                       int n_heads = 0, const float* heads_b = nullptr, const int* heads_act = nullptr) {
   using namespace mm::mlp;
   MM_REQUIRE(a_split && w_split && widths && bias && acts && M >= 0 && K > 0, MM_ERR_ARG, "mm_mlp_tc: null pointer or bad M/K");
   MM_REQUIRE(n_layers >= 1 && n_layers <= kMaxChain + 1, MM_ERR_UNSUPPORTED, "mm_mlp_tc: 1..%d layers (got %d)", kMaxChain + 1,
@@ -413,13 +450,17 @@ static int mlp_tc_impl(const void* a_split, int64_t M, int K, int n_layers, cons
   }
   const int n_last = widths[n_layers - 1];
   MM_REQUIRE(!head_w || n_last <= 32, MM_ERR_UNSUPPORTED, "mm_mlp_tc: the fused Dense(N->1) head needs a last width <= 32");
-  MM_REQUIRE(!head_w || (head_act >= MM_ACT_LINEAR && head_act <= MM_ACT_GELU), MM_ERR_ARG, "mm_mlp_tc: unknown head activation");
+  MM_REQUIRE(!head_w || n_heads || (head_act >= MM_ACT_LINEAR && head_act <= MM_ACT_GELU), MM_ERR_ARG,
+             "mm_mlp_tc: unknown head activation");
+  for (int hh = 0; hh < n_heads; ++hh)
+    MM_REQUIRE(heads_act[hh] >= MM_ACT_LINEAR && heads_act[hh] <= MM_ACT_GELU, MM_ERR_ARG, "mm_mlp_tc_heads: unknown activation of head %d",
+               hh);
   MM_REQUIRE(!out || out_stride >= n_last, MM_ERR_ARG, "mm_mlp_tc: out_stride < last width");
   if (M == 0) return MM_OK;
 
   Params p;
   size_t smem = 0;
-  MM_REQUIRE(plan_tower(K, n_layers, widths, p, smem), MM_ERR_UNSUPPORTED,
+  MM_REQUIRE(plan_tower(K, n_layers, widths, p, smem, n_heads > 0), MM_ERR_UNSUPPORTED,
              "mm_mlp_tc: the tower does not fit in shared memory with two pipeline stages (mm_mlp_tc_supported)");
   p.M = M;
   p.act1 = acts[0];
@@ -432,6 +473,15 @@ static int mlp_tc_impl(const void* a_split, int64_t M, int K, int n_layers, cons
   p.head_b = head_b;
   p.head_act = head_act;
   p.head_out = head_out;
+  if (n_heads > 0) {  // the multi-head epilogue reads heads_*; head_w / head_out only say "a head is fused"
+    p.head_w = nullptr;
+    p.head_out = nullptr;
+    p.n_heads = n_heads;
+    p.heads_w = head_w;
+    p.heads_b = heads_b;
+    for (int hh = 0; hh < n_heads; ++hh) p.heads_act[hh] = heads_act[hh];
+    p.heads_out = head_out;
+  }
 
   CUtensorMap tmA, tmW1, tmC[kMaxChain];
   int rc = mm::tc::make_map(&tmA, a_split, (uint64_t)M, (uint64_t)2 * p.K1p, BLOCK_M);
@@ -447,16 +497,16 @@ static int mlp_tc_impl(const void* a_split, int64_t M, int K, int n_layers, cons
     }
   }
 
-  MlpKernel kern = kernel_for(p.N1p);
+  MlpKernel kern = n_heads > 0 ? kernel_for<true>(p.N1p) : kernel_for<false>(p.N1p);
   MM_REQUIRE(kern != nullptr, MM_ERR_UNSUPPORTED, "mm_mlp_tc: no kernel for a padded layer-1 width of %d", p.N1p);
-  static bool smem_set[8] = {};
-  if (!smem_set[p.N1p / 16 - 1]) {
+  static bool smem_set[2][8] = {};
+  if (!smem_set[n_heads > 0][p.N1p / 16 - 1]) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) {
       mm::set_error("mm_mlp_tc: cudaFuncSetAttribute(227 KB smem) failed: %s", cudaGetErrorString(e));
       return (int)e;
     }
-    smem_set[p.N1p / 16 - 1] = true;
+    smem_set[n_heads > 0][p.N1p / 16 - 1] = true;
   }
   const long long tiles = (M + BLOCK_M - 1) / BLOCK_M;
   const int sms = mm::sm_count();
@@ -472,6 +522,16 @@ int mm_mlp_tc(const void* a_split, int64_t M, int K, int n_layers, const void* c
               float head_b, int head_act, float* head_out, void* stream) {
   return mlp_tc_impl(a_split, M, K, n_layers, w_split, widths, bias, acts, out, out_stride, head_w, head_b, head_act, head_out,
                      nullptr, stream);
+}
+
+int mm_mlp_tc_heads(const void* a_split, int64_t M, int K, int n_layers, const void* const* w_split, const int* widths,
+                    const float* const* bias, const int* acts, int n_heads, const float* heads_w, const float* heads_b,
+                    const int* heads_act, float* heads_out, void* stream) {
+  MM_REQUIRE(n_heads >= 1 && n_heads <= mm::mlp::kMaxHeads, MM_ERR_UNSUPPORTED, "mm_mlp_tc_heads: %d heads is not in 1..%d", n_heads,
+             mm::mlp::kMaxHeads);
+  MM_REQUIRE(heads_w && heads_out && heads_act, MM_ERR_ARG, "mm_mlp_tc_heads: null heads_w / heads_act / heads_out");
+  return mlp_tc_impl(a_split, M, K, n_layers, w_split, widths, bias, acts, nullptr, 0, heads_w, 0.0f, 0, heads_out, nullptr, stream,
+                     n_heads, heads_b, heads_act);
 }
 
 int mm_mlp_tc_operand_out(const void* a_split, int64_t M, int K, int n_layers, const void* const* w_split, const int* widths,

@@ -24,185 +24,322 @@ namespace mm {
 namespace trn {
 
 // ---------------------------------------------------------------------------------------------------------------
-// Head: Dense(K -> 1) + sigmoid + binary cross-entropy, forward and backward in one pass over x.
-// Keras evaluates BCE on the logits cached by the sigmoid activation (`_keras_logits`):
-//   l_i = max(z,0) - z*y + log(1 + exp(-|z|)),   loss = sum_i w_i l_i / sum... (mean over the batch: / M)
+// Heads: H <= 8 outputs Dense(K -> 1) on the same body vector, forward and backward in one pass over x.
+//   BCE (BinaryOutput): Keras evaluates BCE on the logits cached by the sigmoid activation (`_keras_logits`):
+//     l_i = max(z,0) - z*y + log(1 + exp(-|z|)),   dl/dz = sigmoid(z) - y
+//   MSE (RegressionOutput, linear):  l_i = (z - y)^2,   dl/dz = 2 (z - y)
+// loss_h = sum_i sw_i l_h,i / M (Keras "sum_over_batch_size"), total = sum_h lambda_h loss_h, dz_h = lambda_h sw_i l'_h / M.
+// H and TRAIN are template parameters; the loss kind of a head is a uniform runtime branch.  H = 1 with one BCE head and
+// lambda = 1 is mm_bce_head_fwd_bwd: the same products and sums in the same order (the products by lambda = 1 are exact).
 // ---------------------------------------------------------------------------------------------------------------
+constexpr int HEAD_MAX = 8;
+
 struct HeadParams {
   const float* x;
   long long ldx;
   long long M;
   int K;
-  const float* w;
-  const float* bias;  // device scalar or null
-  const void* y;
-  int y_dtype;
-  const float* sample_w;  // (M,) or null
+  const float* w;     // (K, H) Keras layout
+  const float* bias;  // (H,) device or null
+  const void* y[HEAD_MAX];
+  int y_dtype[HEAD_MAX];
+  int kind[HEAD_MAX];    // MM_LOSS_BCE / MM_LOSS_MSE
+  float lw[HEAD_MAX];    // loss weights lambda_h
+  const float* sample_w[HEAD_MAX];  // (M,) or null
   float inv_m;            // 1 / M  (Keras "sum_over_batch_size")
-  float* logits;          // (M,) or null
-  float* loss;            // device scalar, accumulated
+  float* logits;          // (H, M) or null; forward only: the activated predictions
+  float* loss;            // total, accumulated (device scalar) or null
+  float* loss_heads;      // (H,) unweighted per-head losses, accumulated, or null
   float* dx;
   long long lddx;
   int mask_relu;
-  float* dw;  // (K,) accumulated
-  float* db;  // scalar accumulated
+  float* dw;  // (K, H) accumulated
+  float* db;  // (H,) accumulated
 };
 
 constexpr int HEAD_KMAX = 256;  // 8 columns per lane
 
-__global__ void __launch_bounds__(256) head_kernel(const HeadParams p) {
+// loss term and d loss / dz (before lambda, sw and 1/M) of one head
+__device__ __forceinline__ void head_loss(int kind, float z, float y, float& l, float& g) {
+  if (kind == MM_LOSS_MSE) {
+    const float d = z - y;
+    l = d * d;
+    g = 2.0f * d;
+  } else {
+    const float e = expf(-fabsf(z));
+    l = fmaxf(z, 0.0f) - z * y + log1pf(e);
+    const float sig = z >= 0.0f ? 1.0f / (1.0f + e) : e / (1.0f + e);
+    g = sig - y;
+  }
+}
+
+__device__ __forceinline__ float head_pred(int kind, float z) {
+  if (kind == MM_LOSS_MSE) return z;
+  const float e = expf(-fabsf(z));
+  return z >= 0.0f ? 1.0f / (1.0f + e) : e / (1.0f + e);
+}
+
+template <int H, bool TRAIN>
+__global__ void __launch_bounds__(256, H == 1 ? 2 : 1) head_kernel(const HeadParams p) {
   const int lane = threadIdx.x & 31;
   const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const long long n_warps = ((long long)gridDim.x * blockDim.x) >> 5;
   constexpr int C = HEAD_KMAX / 32;
-  float w[C], dw[C];
+  float w[H][C], dw[H][C];
+  float b[H], loss[H], db[H];
 #pragma unroll
-  for (int c = 0; c < C; ++c) {
-    const int k = lane + 32 * c;
-    w[c] = k < p.K ? p.w[k] : 0.0f;
-    dw[c] = 0.0f;
+  for (int h = 0; h < H; ++h) {
+#pragma unroll
+    for (int c = 0; c < C; ++c) {
+      const int k = lane + 32 * c;
+      w[h][c] = k < p.K ? p.w[k * H + h] : 0.0f;
+      dw[h][c] = 0.0f;
+    }
+    b[h] = p.bias ? p.bias[h] : 0.0f;
+    loss[h] = db[h] = 0.0f;
   }
-  const float b = p.bias ? p.bias[0] : 0.0f;
-  float loss = 0.0f, db = 0.0f;
   for (long long m = warp; m < p.M; m += n_warps) {
     float x[C];
-    float dot = 0.0f;
+    float dot[H];
+#pragma unroll
+    for (int h = 0; h < H; ++h) dot[h] = 0.0f;
 #pragma unroll
     for (int c = 0; c < C; ++c) {
       const int k = lane + 32 * c;
       x[c] = k < p.K ? p.x[m * p.ldx + k] : 0.0f;
-      dot = fmaf(x[c], w[c], dot);
+#pragma unroll
+      for (int h = 0; h < H; ++h) dot[h] = fmaf(x[c], w[h][c], dot[h]);
     }
-    const float z = warp_sum(dot) + b;
-    const float y = load_as_f32(p.y, m, p.y_dtype);
-    const float sw = p.sample_w ? p.sample_w[m] : 1.0f;
-    const float e = expf(-fabsf(z));
-    const float l = fmaxf(z, 0.0f) - z * y + log1pf(e);
-    const float sig = z >= 0.0f ? 1.0f / (1.0f + e) : e / (1.0f + e);
-    const float dz = (sig - y) * sw * p.inv_m;
-    if (lane == 0) {
-      loss += l * sw * p.inv_m;
-      db += dz;
-      if (p.logits) p.logits[m] = z;
+    float dz[H];
+#pragma unroll
+    for (int h = 0; h < H; ++h) {
+      const float z = warp_sum(dot[h]) + b[h];
+      if (!TRAIN) {
+        if (lane == 0) p.logits[h * p.M + m] = head_pred(p.kind[h], z);
+        continue;
+      }
+      const float y = load_as_f32(p.y[h], m, p.y_dtype[h]);
+      const float sw = p.sample_w[h] ? p.sample_w[h][m] : 1.0f;
+      float l, g;
+      head_loss(p.kind[h], z, y, l, g);
+      dz[h] = g * sw * p.inv_m;
+      dz[h] *= p.lw[h];  // exact for lambda = 1
+      if (lane == 0) {
+        loss[h] += l * sw * p.inv_m;
+        db[h] += dz[h];
+        if (p.logits) p.logits[h * p.M + m] = z;
+      }
     }
+    if (!TRAIN) continue;
 #pragma unroll
     for (int c = 0; c < C; ++c) {
       const int k = lane + 32 * c;
       if (k < p.K) {
-        dw[c] = fmaf(x[c], dz, dw[c]);
-        if (p.dx) p.dx[m * p.lddx + k] = (!p.mask_relu || x[c] > 0.0f) ? dz * w[c] : 0.0f;
+        float d = dz[0] * w[0][c];
+#pragma unroll
+        for (int h = 0; h < H; ++h) {
+          dw[h][c] = fmaf(x[c], dz[h], dw[h][c]);
+          if (h > 0) d = fmaf(dz[h], w[h][c], d);
+        }
+        if (p.dx) p.dx[m * p.lddx + k] = (!p.mask_relu || x[c] > 0.0f) ? d : 0.0f;
       }
     }
   }
-  // block-level reduction of dw / db / loss before the atomics
+  if (!TRAIN) return;
+  // block-level reduction of dw / db / loss before the atomics, one head at a time
   __shared__ float red[8][HEAD_KMAX + 2];
   const int wid = threadIdx.x >> 5;
-#pragma unroll
-  for (int c = 0; c < C; ++c) red[wid][lane + 32 * c] = dw[c];
-  if (lane == 0) {
-    red[wid][HEAD_KMAX] = db;
-    red[wid][HEAD_KMAX + 1] = loss;
-  }
-  __syncthreads();
   const int nw = blockDim.x >> 5;
-  for (int k = threadIdx.x; k < HEAD_KMAX + 2; k += blockDim.x) {
-    float s = 0.0f;
-    for (int i = 0; i < nw; ++i) s += red[i][k];
-    if (k < p.K) {
-      if (p.dw) atomicAdd(p.dw + k, s);
-    } else if (k == HEAD_KMAX) {
-      if (p.db) atomicAdd(p.db, s);
-    } else if (k == HEAD_KMAX + 1) {
-      if (p.loss) atomicAdd(p.loss, s);
+#pragma unroll
+  for (int h = 0; h < H; ++h) {
+    if (h > 0) __syncthreads();  // the previous head's sums have been read
+#pragma unroll
+    for (int c = 0; c < C; ++c) red[wid][lane + 32 * c] = dw[h][c];
+    if (lane == 0) {
+      red[wid][HEAD_KMAX] = db[h];
+      red[wid][HEAD_KMAX + 1] = loss[h];
+    }
+    __syncthreads();
+    for (int k = threadIdx.x; k < HEAD_KMAX + 2; k += blockDim.x) {
+      float s = 0.0f;
+      for (int i = 0; i < nw; ++i) s += red[i][k];
+      if (k < p.K) {
+        if (p.dw) atomicAdd(p.dw + k * H + h, s);
+      } else if (k == HEAD_KMAX) {
+        if (p.db) atomicAdd(p.db + h, s);
+      } else if (k == HEAD_KMAX + 1) {
+        if (p.loss) atomicAdd(p.loss, p.lw[h] * s);
+        if (p.loss_heads) atomicAdd(p.loss_heads + h, s);
+      }
     }
   }
 }
 
 // K a multiple of 4 with 16-byte aligned rows: G = K/4 (rounded up to a power of two, <= 32) lanes own one row as
 // float4 pieces, a warp processes 32/G rows at a time (K = 32: 4 rows per warp, one 128-byte row per 8 lanes).
-template <int G>
-__global__ void __launch_bounds__(256) head_kernel_v4(const HeadParams p) {
+template <int G, int H, bool TRAIN>
+__global__ void __launch_bounds__(256, H == 1 ? 2 : 1) head_kernel_v4(const HeadParams p) {
   const int lane = threadIdx.x & 31;
   const int c = lane % G, sub = lane / G;
   constexpr int RPW = 32 / G;  // rows per warp and iteration
   const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const long long n_warps = ((long long)gridDim.x * blockDim.x) >> 5;
   const bool on = 4 * c < p.K;
-  const float4 w = on ? *reinterpret_cast<const float4*>(p.w + 4 * c) : make_float4(0.f, 0.f, 0.f, 0.f);
-  float4 dw = make_float4(0.f, 0.f, 0.f, 0.f);
-  const float b = p.bias ? p.bias[0] : 0.0f;
-  float loss = 0.0f, db = 0.0f;
+  float4 w[H], dw[H];
+  float b[H], loss[H], db[H];
+#pragma unroll
+  for (int h = 0; h < H; ++h) {
+    if (H == 1) {
+      w[h] = on ? *reinterpret_cast<const float4*>(p.w + 4 * c) : make_float4(0.f, 0.f, 0.f, 0.f);
+    } else {
+      w[h] = on ? make_float4(p.w[(4 * c) * H + h], p.w[(4 * c + 1) * H + h], p.w[(4 * c + 2) * H + h], p.w[(4 * c + 3) * H + h])
+                : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    dw[h] = make_float4(0.f, 0.f, 0.f, 0.f);
+    b[h] = p.bias ? p.bias[h] : 0.0f;
+    loss[h] = db[h] = 0.0f;
+  }
   const long long groups = (p.M + RPW - 1) / RPW;
   for (long long gi = warp; gi < groups; gi += n_warps) {
     const long long m = gi * RPW + sub;
     const bool live = m < p.M;
     float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
     if (live && on) x = __ldg(reinterpret_cast<const float4*>(p.x + m * p.ldx + 4 * c));
-    float dot = x.x * w.x + x.y * w.y + x.z * w.z + x.w * w.w;
+    float dz[H];
 #pragma unroll
-    for (int o = G / 2; o > 0; o >>= 1) dot += __shfl_xor_sync(0xffffffffu, dot, o);
-    const float z = dot + b;
-    float dz = 0.0f;
-    if (live) {
-      const float y = load_as_f32(p.y, m, p.y_dtype);
-      const float sw = p.sample_w ? p.sample_w[m] : 1.0f;
-      const float e = expf(-fabsf(z));
-      const float sig = z >= 0.0f ? 1.0f / (1.0f + e) : e / (1.0f + e);
-      dz = (sig - y) * sw * p.inv_m;
-      if (c == 0) {
-        loss += (fmaxf(z, 0.0f) - z * y + log1pf(e)) * sw * p.inv_m;
-        db += dz;
-        if (p.logits) p.logits[m] = z;
+    for (int h = 0; h < H; ++h) {
+      float dot = x.x * w[h].x + x.y * w[h].y + x.z * w[h].z + x.w * w[h].w;
+#pragma unroll
+      for (int o = G / 2; o > 0; o >>= 1) dot += __shfl_xor_sync(0xffffffffu, dot, o);
+      const float z = dot + b[h];
+      dz[h] = 0.0f;
+      if (!TRAIN) {
+        if (live && c == 0) p.logits[h * p.M + m] = head_pred(p.kind[h], z);
+        continue;
+      }
+      if (live) {
+        const float y = load_as_f32(p.y[h], m, p.y_dtype[h]);
+        const float sw = p.sample_w[h] ? p.sample_w[h][m] : 1.0f;
+        float l, g;
+        head_loss(p.kind[h], z, y, l, g);
+        dz[h] = g * sw * p.inv_m;
+        dz[h] *= p.lw[h];  // exact for lambda = 1
+        if (c == 0) {
+          loss[h] += l * sw * p.inv_m;
+          db[h] += dz[h];
+          if (p.logits) p.logits[h * p.M + m] = z;
+        }
       }
     }
-    dw.x = fmaf(x.x, dz, dw.x);
-    dw.y = fmaf(x.y, dz, dw.y);
-    dw.z = fmaf(x.z, dz, dw.z);
-    dw.w = fmaf(x.w, dz, dw.w);
+    if (!TRAIN) continue;
+#pragma unroll
+    for (int h = 0; h < H; ++h) {
+      dw[h].x = fmaf(x.x, dz[h], dw[h].x);
+      dw[h].y = fmaf(x.y, dz[h], dw[h].y);
+      dw[h].z = fmaf(x.z, dz[h], dw[h].z);
+      dw[h].w = fmaf(x.w, dz[h], dw[h].w);
+    }
     if (live && on && p.dx) {
+      float4 g = make_float4(dz[0] * w[0].x, dz[0] * w[0].y, dz[0] * w[0].z, dz[0] * w[0].w);
+#pragma unroll
+      for (int h = 1; h < H; ++h) {
+        g.x = fmaf(dz[h], w[h].x, g.x);
+        g.y = fmaf(dz[h], w[h].y, g.y);
+        g.z = fmaf(dz[h], w[h].z, g.z);
+        g.w = fmaf(dz[h], w[h].w, g.w);
+      }
       float4 d;
-      d.x = (!p.mask_relu || x.x > 0.0f) ? dz * w.x : 0.0f;
-      d.y = (!p.mask_relu || x.y > 0.0f) ? dz * w.y : 0.0f;
-      d.z = (!p.mask_relu || x.z > 0.0f) ? dz * w.z : 0.0f;
-      d.w = (!p.mask_relu || x.w > 0.0f) ? dz * w.w : 0.0f;
+      d.x = (!p.mask_relu || x.x > 0.0f) ? g.x : 0.0f;
+      d.y = (!p.mask_relu || x.y > 0.0f) ? g.y : 0.0f;
+      d.z = (!p.mask_relu || x.z > 0.0f) ? g.z : 0.0f;
+      d.w = (!p.mask_relu || x.w > 0.0f) ? g.w : 0.0f;
       *reinterpret_cast<float4*>(p.dx + m * p.lddx + 4 * c) = d;
     }
   }
+  if (!TRAIN) return;
   // lanes with the same c hold partial sums of the same columns: fold the row groups of the warp, then the block
 #pragma unroll
-  for (int o = G; o < 32; o <<= 1) {
-    dw.x += __shfl_xor_sync(0xffffffffu, dw.x, o);
-    dw.y += __shfl_xor_sync(0xffffffffu, dw.y, o);
-    dw.z += __shfl_xor_sync(0xffffffffu, dw.z, o);
-    dw.w += __shfl_xor_sync(0xffffffffu, dw.w, o);
-    loss += __shfl_xor_sync(0xffffffffu, loss, o);
-    db += __shfl_xor_sync(0xffffffffu, db, o);
+  for (int h = 0; h < H; ++h) {
+#pragma unroll
+    for (int o = G; o < 32; o <<= 1) {
+      dw[h].x += __shfl_xor_sync(0xffffffffu, dw[h].x, o);
+      dw[h].y += __shfl_xor_sync(0xffffffffu, dw[h].y, o);
+      dw[h].z += __shfl_xor_sync(0xffffffffu, dw[h].z, o);
+      dw[h].w += __shfl_xor_sync(0xffffffffu, dw[h].w, o);
+      loss[h] += __shfl_xor_sync(0xffffffffu, loss[h], o);
+      db[h] += __shfl_xor_sync(0xffffffffu, db[h], o);
+    }
   }
   __shared__ float red[8][4 * G + 2];
   const int wid = threadIdx.x >> 5;
-  if (lane < G) {
-    red[wid][4 * lane] = dw.x;
-    red[wid][4 * lane + 1] = dw.y;
-    red[wid][4 * lane + 2] = dw.z;
-    red[wid][4 * lane + 3] = dw.w;
-  }
-  if (lane == 0) {
-    red[wid][4 * G] = db;
-    red[wid][4 * G + 1] = loss;
-  }
-  __syncthreads();
   const int nw = blockDim.x >> 5;
-  for (int k = threadIdx.x; k < 4 * G + 2; k += blockDim.x) {
-    float s = 0.0f;
-    for (int i = 0; i < nw; ++i) s += red[i][k];
-    if (k < 4 * G) {
-      if (k < p.K && p.dw) atomicAdd(p.dw + k, s);
-    } else if (k == 4 * G) {
-      if (p.db) atomicAdd(p.db, s);
-    } else if (p.loss) {
-      atomicAdd(p.loss, s);
+#pragma unroll
+  for (int h = 0; h < H; ++h) {
+    if (h > 0) __syncthreads();  // the previous head's sums have been read
+    if (lane < G) {
+      red[wid][4 * lane] = dw[h].x;
+      red[wid][4 * lane + 1] = dw[h].y;
+      red[wid][4 * lane + 2] = dw[h].z;
+      red[wid][4 * lane + 3] = dw[h].w;
+    }
+    if (lane == 0) {
+      red[wid][4 * G] = db[h];
+      red[wid][4 * G + 1] = loss[h];
+    }
+    __syncthreads();
+    for (int k = threadIdx.x; k < 4 * G + 2; k += blockDim.x) {
+      float s = 0.0f;
+      for (int i = 0; i < nw; ++i) s += red[i][k];
+      if (k < 4 * G) {
+        if (k < p.K && p.dw) atomicAdd(p.dw + k * H + h, s);
+      } else if (k == 4 * G) {
+        if (p.db) atomicAdd(p.db + h, s);
+      } else {
+        if (p.loss) atomicAdd(p.loss, p.lw[h] * s);
+        if (p.loss_heads) atomicAdd(p.loss_heads + h, s);
+      }
     }
   }
+}
+
+template <int H, bool TRAIN>
+static void launch_heads(const HeadParams& p, bool vec, unsigned blocks, cudaStream_t st) {
+  if (vec) {
+    const int g = p.K / 4;
+    if (g <= 2) head_kernel_v4<2, H, TRAIN><<<blocks, 256, 0, st>>>(p);
+    else if (g <= 4) head_kernel_v4<4, H, TRAIN><<<blocks, 256, 0, st>>>(p);
+    else if (g <= 8) head_kernel_v4<8, H, TRAIN><<<blocks, 256, 0, st>>>(p);
+    else if (g <= 16) head_kernel_v4<16, H, TRAIN><<<blocks, 256, 0, st>>>(p);
+    else head_kernel_v4<32, H, TRAIN><<<blocks, 256, 0, st>>>(p);
+  } else {
+    head_kernel<H, TRAIN><<<blocks, 256, 0, st>>>(p);
+  }
+}
+
+// the instantiation for p's head count; H = 1 is mm_bce_head_fwd_bwd's kernel
+template <bool TRAIN>
+static void launch_heads(const HeadParams& p, int H, bool vec, unsigned blocks, cudaStream_t st) {
+  switch (H) {
+    case 1: launch_heads<1, TRAIN>(p, vec, blocks, st); break;
+    case 2: launch_heads<2, TRAIN>(p, vec, blocks, st); break;
+    case 3: launch_heads<3, TRAIN>(p, vec, blocks, st); break;
+    case 4: launch_heads<4, TRAIN>(p, vec, blocks, st); break;
+    case 5: launch_heads<5, TRAIN>(p, vec, blocks, st); break;
+    case 6: launch_heads<6, TRAIN>(p, vec, blocks, st); break;
+    case 7: launch_heads<7, TRAIN>(p, vec, blocks, st); break;
+    default: launch_heads<8, TRAIN>(p, vec, blocks, st); break;
+  }
+}
+
+static void run_heads(const HeadParams& p, int H, bool train, cudaStream_t st) {
+  long long blocks = (p.M + 7) / 8;
+  const long long cap = 4LL * mm::sm_count();
+  if (blocks > cap) blocks = cap;
+  // float4 weights need 16-byte aligned kernel rows: only one head's (K, 1) kernel is read as float4
+  const bool vec = (p.K & 3) == 0 && p.K <= 128 && (p.ldx & 3) == 0 && ((uintptr_t)p.x & 15) == 0 &&
+                   (H > 1 || ((uintptr_t)p.w & 15) == 0) && (!p.dx || ((p.lddx & 3) == 0 && ((uintptr_t)p.dx & 15) == 0));
+  if (train) launch_heads<true>(p, H, vec, (unsigned)blocks, st);
+  else launch_heads<false>(p, H, vec, (unsigned)blocks, st);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -654,9 +791,11 @@ int mm_bce_head_fwd_bwd(const float* x, int64_t M, int K, int64_t x_stride, cons
   p.K = K;
   p.w = w;
   p.bias = bias;
-  p.y = targets;
-  p.y_dtype = target_dtype;
-  p.sample_w = sample_weight;
+  p.y[0] = targets;
+  p.y_dtype[0] = target_dtype;
+  p.kind[0] = MM_LOSS_BCE;
+  p.lw[0] = 1.0f;
+  p.sample_w[0] = sample_weight;
   p.inv_m = 1.0f / (float)M;
   p.logits = logits;
   p.loss = loss_sum;
@@ -665,23 +804,58 @@ int mm_bce_head_fwd_bwd(const float* x, int64_t M, int K, int64_t x_stride, cons
   p.mask_relu = mask_relu;
   p.dw = dw;
   p.db = db;
-  long long blocks = (M + 7) / 8;
-  const long long cap = 4LL * mm::sm_count();
-  if (blocks > cap) blocks = cap;
-  cudaStream_t st = (cudaStream_t)stream;
-  const bool vec = (K & 3) == 0 && K <= 128 && (x_stride & 3) == 0 && ((uintptr_t)x & 15) == 0 && ((uintptr_t)w & 15) == 0 &&
-                   (!dx || ((dx_stride & 3) == 0 && ((uintptr_t)dx & 15) == 0));
-  if (vec) {
-    const int g = K / 4;
-    if (g <= 2) head_kernel_v4<2><<<(unsigned)blocks, 256, 0, st>>>(p);
-    else if (g <= 4) head_kernel_v4<4><<<(unsigned)blocks, 256, 0, st>>>(p);
-    else if (g <= 8) head_kernel_v4<8><<<(unsigned)blocks, 256, 0, st>>>(p);
-    else if (g <= 16) head_kernel_v4<16><<<(unsigned)blocks, 256, 0, st>>>(p);
-    else head_kernel_v4<32><<<(unsigned)blocks, 256, 0, st>>>(p);
-  } else {
-    head_kernel<<<(unsigned)blocks, 256, 0, st>>>(p);
-  }
+  run_heads(p, 1, true, (cudaStream_t)stream);
   return mm::check_launch("mm_bce_head_fwd_bwd");
+}
+
+int mm_heads_fwd_bwd(const float* x, int64_t M, int K, int64_t x_stride, int H, const float* w, const float* bias,
+                     const int* loss_kind, const float* loss_weight, const void* const* targets, const int* target_dtypes,
+                     const float* const* sample_weights, float* logits, float* loss, float* dx, int64_t dx_stride,
+                     int mask_relu, float* dw, float* db, void* stream) {
+  using namespace mm::trn;
+  MM_REQUIRE(x && w && loss_kind && M >= 0 && K >= 1 && x_stride >= K, MM_ERR_ARG, "mm_heads_fwd_bwd: null pointer or bad K / stride");
+  MM_REQUIRE(H >= 1 && H <= HEAD_MAX, MM_ERR_UNSUPPORTED, "mm_heads_fwd_bwd: H=%d is not in 1..%d", H, HEAD_MAX);
+  MM_REQUIRE(K <= HEAD_KMAX, MM_ERR_UNSUPPORTED, "mm_heads_fwd_bwd: K=%d > %d", K, HEAD_KMAX);
+  const bool train = targets != nullptr;
+  MM_REQUIRE(train || logits, MM_ERR_ARG, "mm_heads_fwd_bwd: forward only (targets null) needs logits");
+  MM_REQUIRE(!train || (loss_weight && target_dtypes && loss), MM_ERR_ARG,
+             "mm_heads_fwd_bwd: training needs loss_weight, target_dtypes and loss");
+  MM_REQUIRE(!train || !dx || dx_stride >= K, MM_ERR_ARG, "mm_heads_fwd_bwd: dx_stride < K");
+  HeadParams p;
+  memset(&p, 0, sizeof(p));
+  for (int h = 0; h < H; ++h) {
+    MM_REQUIRE(loss_kind[h] == MM_LOSS_BCE || loss_kind[h] == MM_LOSS_MSE, MM_ERR_ARG, "mm_heads_fwd_bwd: head %d: bad loss kind %d",
+               h, loss_kind[h]);
+    p.kind[h] = loss_kind[h];
+    if (train) {
+      MM_REQUIRE(targets[h], MM_ERR_ARG, "mm_heads_fwd_bwd: head %d: null targets", h);
+      MM_REQUIRE(target_dtypes[h] >= MM_I32 && target_dtypes[h] <= MM_F64, MM_ERR_ARG, "mm_heads_fwd_bwd: head %d: bad target dtype", h);
+      p.y[h] = targets[h];
+      p.y_dtype[h] = target_dtypes[h];
+      p.lw[h] = loss_weight[h];
+      p.sample_w[h] = sample_weights ? sample_weights[h] : nullptr;
+    }
+  }
+  if (M == 0) return MM_OK;
+  p.x = x;
+  p.ldx = x_stride;
+  p.M = M;
+  p.K = K;
+  p.w = w;
+  p.bias = bias;
+  p.inv_m = 1.0f / (float)M;
+  p.logits = logits;
+  if (train) {
+    p.loss = loss;
+    p.loss_heads = loss + 1;
+    p.dx = dx;
+    p.lddx = dx_stride;
+    p.mask_relu = mask_relu;
+    p.dw = dw;
+    p.db = db;
+  }
+  run_heads(p, H, train, (cudaStream_t)stream);
+  return mm::check_launch("mm_heads_fwd_bwd");
 }
 
 static int wgrad_dispatch(mm::trn::WgradParams p, void* stream) {

@@ -100,6 +100,7 @@ class CompiledForward:
         self.namespace = new_buffer_namespace()  # private scratch buffers: graphs may run concurrently
         self._capture()
         self.output_host = torch.empty(self.output.shape, dtype=self.output.dtype, pin_memory=True)
+        self.host_result = self._as_result(self.output_host)
         self._oob_host = torch.zeros(1, dtype=torch.int32, pin_memory=True)
         self.check_indices(sync=True)
 
@@ -129,9 +130,14 @@ class CompiledForward:
             with torch.cuda.graph(self.graph):
                 out = self._run()
             self.launches_per_replay = ops.launch_count() - n0  # kernels of libmm_b200.so inside the graph
-            if getattr(self, "output", None) is not None and (out.shape != self.output.shape or out.dtype != self.output.dtype):
+            names = None
+            if isinstance(out, dict):  # several outputs: (B, 1) views of ONE (H, B) buffer -> one D2H copy
+                names, out = list(out), _stacked_outputs(out)
+            if getattr(self, "output", None) is not None and (out.shape != self.output.shape or out.dtype != self.output.dtype
+                                                              or names != self.output_names):
                 raise RuntimeError("re-capture changed the output layout")
-            self.output = out
+            self.output, self.output_names = out, names
+            self.device_result = self._as_result(out)
             self._wv = weights_version()
         finally:
             model.defer_index_check(False)
@@ -147,6 +153,12 @@ class CompiledForward:
     def _run(self) -> torch.Tensor:
         out = self.model(self.inputs, **self.call_kwargs)
         return out.outputs if isinstance(out, Prediction) else out
+
+    def _as_result(self, buf: torch.Tensor):
+        """The output tensor of a single-output model; {name: (B, 1) view of row h} of the (H, B) buffer otherwise."""
+        if self.output_names is None:
+            return buf
+        return {n: buf[h].view(-1, 1) for h, n in enumerate(self.output_names)}
 
     def check_indices(self, sync: bool = False) -> None:
         if self._oob is None:
@@ -164,7 +176,7 @@ class CompiledForward:
     def replay(self) -> torch.Tensor:
         self._ensure_current()
         self.graph.replay()
-        return self.output
+        return self.device_result
 
     def load_device(self, packed: torch.Tensor) -> None:
         """Device-to-device refresh of the static input buffer (packed layout of `HostBatch`)."""
@@ -173,7 +185,8 @@ class CompiledForward:
     # ---- host in / host out ---------------------------------------------------------------------------
     def __call__(self, batch: HostBatch) -> torch.Tensor:
         """One H2D copy of the packed pinned batch, one graph launch, one D2H copy; returns the pinned
-        host predictions (valid until the next call)."""
+        host predictions (valid until the next call): a tensor, or {output name: (B, 1)} views of one pinned (H, B) buffer
+        for a model with several outputs."""
         if batch.spec != self.spec:
             raise ValueError("batch layout differs from the one this forward was compiled for")
         self._ensure_current()
@@ -184,7 +197,17 @@ class CompiledForward:
             self._oob_host.copy_(self._oob, non_blocking=True)
         torch.cuda.current_stream().synchronize()
         self.check_indices()
-        return self.output_host
+        return self.host_result
+
+
+def _stacked_outputs(out: Dict[str, torch.Tensor]) -> torch.Tensor:
+    """The (H, B) buffer behind a multi-output forward's {name: (B, 1)} views (models.ParallelOutputs.split)."""
+    vals = list(out.values())
+    base = vals[0]._base
+    if base is None or base.dim() != 2 or base.shape[0] != len(vals) or not base.is_contiguous() or any(
+            v._base is not base or v.data_ptr() != base[h].data_ptr() for h, v in enumerate(vals)):
+        raise RuntimeError("a multi-output forward must return views of one (H, B) buffer, in output order")
+    return base
 
 
 class PipelinedForward:
@@ -242,10 +265,10 @@ class PipelinedForward:
             torch.cuda.current_stream().wait_stream(st)
 
     def output(self, ticket: int) -> torch.Tensor:
-        return self.slots[ticket].output
+        return self.slots[ticket].device_result
 
     def result(self, ticket: int) -> torch.Tensor:
         self.done[ticket].synchronize()
         self.busy[ticket] = False
         self.slots[ticket].check_indices()
-        return self.slots[ticket].output_host
+        return self.slots[ticket].host_result

@@ -137,7 +137,7 @@ class _LazyVariables(Mapping):
 class _TensorPickler(pickle.Pickler):
     """Pickles the block structure; every torch.Tensor becomes a reference to variables/NNNN.npy."""
 
-    def __init__(self, file, var_dir: pathlib.Path, names: Dict[int, str]):
+    def __init__(self, file, var_dir: pathlib.Path, names: Dict[tuple, str]):
         super().__init__(file, protocol=pickle.HIGHEST_PROTOCOL)
         self.var_dir, self.names = var_dir, names
         self.entries, self.index_of = [], {}
@@ -145,14 +145,14 @@ class _TensorPickler(pickle.Pickler):
     def persistent_id(self, obj):
         if not isinstance(obj, torch.Tensor):
             return None
-        key = (obj.data_ptr(), tuple(obj.shape), tuple(obj.stride()), str(obj.dtype))
+        key = _tensor_key(obj)
         if key not in self.index_of:
             idx = len(self.entries)
             fname = f"{idx:04d}.npy"
             host = obj.detach().cpu()
             arr = host.view(torch.int16).numpy() if host.dtype == torch.bfloat16 else host.numpy()
             np.save(self.var_dir / fname, arr)
-            self.entries.append({"name": self.names.get(obj.data_ptr()), "file": fname, "shape": list(obj.shape),
+            self.entries.append({"name": self.names.get(key), "file": fname, "shape": list(obj.shape),
                                  "dtype": str(obj.dtype).replace("torch.", ""), "device": obj.device.type})
             self.index_of[key] = idx
         return ("mm_b200_tensor", self.index_of[key])
@@ -195,6 +195,10 @@ class _TensorUnpickler(pickle.Unpickler):
         raise pickle.UnpicklingError(f"refusing to load {module}.{name} from a model file")
 
 
+def _tensor_key(t: torch.Tensor) -> tuple:
+    return (t.data_ptr(), tuple(t.shape), tuple(t.stride()), str(t.dtype))
+
+
 def save_model(model: Block, export_path) -> None:
     """`model.save(export_path)` of the reference (models/base.py:1687-1716): variables + structure + `.merlin` metadata."""
     path = pathlib.Path(export_path)
@@ -203,10 +207,19 @@ def save_model(model: Block, export_path) -> None:
     weights = model.weights()
     if not weights:
         raise ValueError("the model has no variables yet: call model.build(device) (or run one batch) before save")
-    names = {t.data_ptr(): n for n, t in weights.items()}
+    names = {_tensor_key(t): n for n, t in weights.items()}
     buf = _io.BytesIO()
     pk = _TensorPickler(buf, var_dir, names)
     pk.dump(model)
+    # a named variable that is a view of a larger stored tensor (each output's column of a multi-output model's stacked
+    # (K, H) head kernel) gets a named file of its own, so that load_weights(export_path) finds every name
+    stored = {e["name"] for e in pk.entries if e["name"]}
+    for n, t in weights.items():
+        if n not in stored:
+            fname = f"{len(pk.entries):04d}.npy"
+            np.save(var_dir / fname, t.detach().cpu().numpy())
+            pk.entries.append({"name": n, "file": fname, "shape": list(t.shape), "dtype": str(t.dtype).replace("torch.", ""),
+                               "device": t.device.type})
     with open(path / "model.pkl", "wb") as f:
         f.write(buf.getvalue())
     with open(var_dir / "manifest.json", "w") as f:

@@ -24,11 +24,13 @@ from .schema import Schema, Tags
 class BinaryOutput(Block):
     """outputs/classification.py:72-123: Dense(1, activation="sigmoid") on the body output."""
 
+    activation, loss, suffix = "sigmoid", "binary_crossentropy", "binary_output"
+
     def __init__(self, target: Optional[Union[str, object]] = None, name: Optional[str] = None, **kwargs):
         tname = getattr(target, "name", target)
-        super().__init__(name or (f"{tname}/binary_output" if tname else unique_name("binary_output")))
+        super().__init__(name or (f"{tname}/{self.suffix}" if tname else unique_name(self.suffix)))
         self.target = tname
-        self.to_call = _Dense(1, activation="sigmoid", name=f"{self.name}/dense")
+        self.to_call = _Dense(1, activation=self.activation, name=f"{self.name}/dense")
 
     def build(self, width: Optional[int] = None, device=None):
         self.to_call.build(width, device)
@@ -50,9 +52,129 @@ class BinaryClassificationTask(BinaryOutput):
         super().__init__(target, name=task_name or (f"{target}/binary_classification_task" if target else None))
 
 
+class RegressionOutput(BinaryOutput):
+    """outputs/regression.py:35-58: Dense(1, activation="linear") on the body output, mean squared error."""
+
+    activation, loss, suffix = "linear", "mse", "regression_output"
+
+
+def _is_regression(out) -> bool:
+    return isinstance(out, RegressionOutput)
+
+
+class ParallelOutputs(Block):
+    """The ParallelBlock of ModelOutputs that OutputBlock builds for several targets (outputs/block.py:32-131): outputs keyed
+    by name ("<target>/binary_output", "<target>/regression_output"), in the order tf.nest flattens that dict (sorted by
+    name).  Owns the stacked head `to_call` = Dense(K -> H) (kernel (K, H), bias (H,)) that the fused kernels read; each
+    output's own Dense is only its initialiser.  The forward returns {name: (B, 1)}."""
+
+    def __init__(self, outputs: Sequence[Block], name: Optional[str] = None):
+        super().__init__(name or unique_name("parallel_outputs"))
+        outs = list(outputs)
+        for o in outs:
+            if not isinstance(o, BinaryOutput):
+                raise NotImplementedError(f"{getattr(o, 'name', o)!r}: only BinaryOutput / RegressionOutput heads can be combined")
+        names = [o.name for o in outs]
+        if len(set(names)) != len(names):
+            raise ValueError(f"output names must be unique, got {names}")
+        if not 2 <= len(outs) <= 8:
+            raise NotImplementedError(f"2..8 outputs are supported, got {len(outs)}")
+        self.outputs = sorted(outs, key=lambda o: o.name)
+        self.to_call = _Dense(len(outs), activation="linear", name=f"{self.name}/dense")
+
+    @property
+    def names(self) -> List[str]:
+        return [o.name for o in self.outputs]
+
+    @property
+    def losses(self) -> List[str]:
+        return [o.loss for o in self.outputs]
+
+    @property
+    def activations(self) -> List[str]:
+        return [o.activation for o in self.outputs]
+
+    def build(self, width: Optional[int] = None, device=None):
+        if width is not None and width > 256:  # mm_heads_fwd_bwd / mm_mlp_tc_heads read the body vector from registers
+            raise NotImplementedError(f"{self.name}: several outputs need a body output of at most 256 units, got {width}")
+        if self.to_call.kernel is None:
+            for o in self.outputs:
+                o.build(width, device)
+            self.to_call.build(width, device)
+            self.to_call.kernel.copy_(torch.cat([o.to_call.kernel for o in self.outputs], dim=1))
+            self.to_call.bias.copy_(torch.cat([o.to_call.bias for o in self.outputs]))
+            for o in self.outputs:  # the stacked kernel is the one variable
+                o.to_call.kernel = o.to_call.bias = None
+        self.built = True
+        return self
+
+    def weights(self):
+        """Each output's (K, 1) kernel and (1,) bias as a view of the stacked head: `<output name>/dense/{kernel,bias}`."""
+        out = {}
+        if self.to_call.kernel is None:
+            return out
+        for h, o in enumerate(self.outputs):
+            out[f"{o.name}/dense/kernel"] = self.to_call.kernel[:, h:h + 1]
+            out[f"{o.name}/dense/bias"] = self.to_call.bias[h:h + 1]
+        return out
+
+    def split(self, stacked: torch.Tensor) -> Dict[str, torch.Tensor]:
+        """(H, B) predictions -> {name: (B, 1) view}."""
+        return {n: stacked[h].view(-1, 1) for h, n in enumerate(self.names)}
+
+    def call(self, inputs: torch.Tensor, **kwargs) -> Dict[str, torch.Tensor]:
+        self.build(inputs.shape[1], inputs.device)
+        out = torch.empty((len(self.outputs), inputs.shape[0]), dtype=torch.float32, device=inputs.device)
+        ops.heads_fwd_bwd(inputs.contiguous(), self.to_call.kernel, self.to_call.bias, self.losses, None, out)
+        return self.split(out)
+
+
+def OutputBlock(schema: Schema, model_outputs=None) -> Block:
+    """outputs/block.py:32-131: one BinaryOutput / RegressionOutput per target column of the schema (continuous /
+    regression-tagged targets first, then binary ones; a categorical target with int_domain.max == 1 is binary).  One target:
+    that output itself; several: ParallelOutputs.  `model_outputs` (list or dict by name) replaces the outputs it names."""
+    targets = schema.select_by_tag(Tags.TARGET)
+    if not len(targets):
+        raise ValueError("No targets found in schema. Please tag your targets or provide them as branches.")
+    given: Dict[str, Block] = {}
+    if model_outputs is not None:
+        if isinstance(model_outputs, dict):
+            given = dict(model_outputs)
+        elif isinstance(model_outputs, (list, tuple)):
+            given = {m.name: m for m in model_outputs}
+        elif isinstance(model_outputs, Block):
+            given = {model_outputs.name: model_outputs}
+        else:
+            raise ValueError("If provided model_outputs should be either a dict or list of ModelOutput")
+    outputs = dict(given)
+    covered = {getattr(o, "target", None) for o in given.values()}
+    for col in targets:
+        if col.name in covered:  # a given output predicts this target, whatever its name
+            continue
+        if col.has_tag(Tags.CONTINUOUS) or col.has_tag(Tags.REGRESSION):
+            cls = RegressionOutput
+        elif col.has_tag(Tags.BINARY_CLASSIFICATION) or col.has_tag(Tags.BINARY):
+            cls = BinaryOutput
+        elif col.has_tag(Tags.CATEGORICAL) or col.has_tag(Tags.MULTI_CLASS_CLASSIFICATION):
+            dom = col.int_domain
+            if dom is None or dom.max != 1:
+                raise NotImplementedError(f"target {col.name!r}: CategoricalOutput (multi-class training) is not implemented")
+            cls = BinaryOutput
+        else:
+            raise ValueError(f"target {col.name!r}: tag it as regression, binary or categorical")
+        name = f"{col.name}/{cls.suffix}"
+        if name not in outputs:
+            outputs[name] = cls(col.name)
+    if len(outputs) == 1:
+        return next(iter(outputs.values()))
+    return ParallelOutputs(list(outputs.values()))
+
+
 def parse_prediction_blocks(schema: Schema, prediction_blocks=None) -> Block:
     """models/utils.py:12-31 / outputs/block.py:79-128: default = BinaryOutput for the (single)
-    binary-classification target of the schema."""
+    binary-classification target of the schema.  A schema with several binary targets, or several targets none of them
+    binary, gets OutputBlock(schema).  A schema with exactly one binary target among several keeps that one BinaryOutput
+    (the reference would build an output per target there)."""
     if prediction_blocks is None:
         targets = schema.select_by_tag(Tags.BINARY_CLASSIFICATION)
         if not len(targets):
@@ -62,16 +184,51 @@ def parse_prediction_blocks(schema: Schema, prediction_blocks=None) -> Block:
         if len(targets) > 1:
             binary = [c.name for c in targets if c.has_tag(Tags.BINARY_CLASSIFICATION)]
             if len(binary) != 1:
-                raise NotImplementedError("multi-task outputs are outside the hot path; pass one BinaryOutput")
+                return OutputBlock(schema)
             return BinaryOutput(binary[0])
         return BinaryOutput(targets.first.name)
     if isinstance(prediction_blocks, (list, tuple)):
-        if len(prediction_blocks) != 1:
-            raise NotImplementedError("multi-task outputs are outside the hot path")
+        if len(prediction_blocks) > 1:
+            return ParallelOutputs(prediction_blocks)
+        if not prediction_blocks:
+            raise ValueError("prediction_tasks is empty")
         prediction_blocks = prediction_blocks[0]
     if not isinstance(prediction_blocks, Block):
         raise ValueError(f"Unsupported prediction task {prediction_blocks!r}")
     return prediction_blocks
+
+
+_LOSS_ALIASES = {"binary_crossentropy": "binary_crossentropy", "mse": "mse", "mean_squared_error": "mse"}
+
+
+def resolve_loss_weights(outputs: Sequence[Block], loss=None, loss_weights=None) -> List[float]:
+    """Keras `compile(loss=..., loss_weights=...)` over the model's outputs: `loss` None (each output's default), one name
+    valid for every output or a dict by output name; `loss_weights` a list in output order or a dict by output name
+    (default 1).  Returns the loss weights in output order."""
+    names = [o.name for o in outputs]
+    if isinstance(loss, dict):
+        unknown = sorted(set(loss) - set(names))
+        if unknown:
+            raise ValueError(f"loss names unknown outputs {unknown}; outputs are {names}")
+        per = [loss.get(n) for n in names]
+    else:
+        per = [loss] * len(outputs)
+    for o, l in zip(outputs, per):
+        if l is None:
+            continue
+        if not isinstance(l, str) or _LOSS_ALIASES.get(l) != o.loss:
+            raise NotImplementedError(f"loss {l!r} for output {o.name!r}: only its default ({o.loss!r}) is implemented")
+    if loss_weights is None:
+        return [1.0] * len(outputs)
+    if isinstance(loss_weights, dict):
+        unknown = sorted(set(loss_weights) - set(names))
+        if unknown:
+            raise ValueError(f"loss_weights names unknown outputs {unknown}; outputs are {names}")
+        return [float(loss_weights.get(n, 1.0)) for n in names]
+    lw = [float(v) for v in loss_weights]
+    if len(lw) != len(outputs):
+        raise ValueError(f"loss_weights has {len(lw)} entries for {len(outputs)} outputs")
+    return lw
 
 
 def expected_input_columns(schema: Schema) -> List[str]:
@@ -132,6 +289,8 @@ class Model(Block):
         """One float column per prediction task (what `get_output_schema` records for the reference)."""
         from .schema import ColumnSchema
 
+        if isinstance(self.prediction, ParallelOutputs):
+            return Schema([ColumnSchema(n, dtype="float32") for n in self.prediction.names])
         target = getattr(self.prediction, "target", None) or getattr(self.prediction, "target_name", None)
         name = f"{target}/{self.prediction.name}" if target else self.prediction.name
         return Schema([ColumnSchema(name, dtype="float32")])
@@ -177,11 +336,14 @@ class Model(Block):
         return self.prediction(x, features=inputs, targets=targets, training=training, testing=testing)
 
     # -- training (models_b200/train.py; reference: models/base.py:1121-1231) ------------------
-    def _compile_training(self, optimizer, loss=None) -> None:
+    def output_blocks(self) -> List[Block]:
+        """The model's outputs in output order (one for a single-output model)."""
+        return list(self.prediction.outputs) if isinstance(self.prediction, ParallelOutputs) else [self.prediction]
+
+    def _compile_training(self, optimizer, loss=None, loss_weights=None) -> None:
         from .train import get_optimizer
 
-        if loss not in (None, "binary_crossentropy"):
-            raise NotImplementedError(f"loss {loss!r}: only the BinaryOutput default (binary cross-entropy) is implemented")
+        self.loss_weights = resolve_loss_weights(self.output_blocks(), loss, loss_weights)
         self.optimizer = get_optimizer(optimizer)
         self._trainer = None
 
@@ -212,16 +374,32 @@ class Model(Block):
             raise ValueError("train_step expects (inputs, targets) or (inputs, targets, sample_weight)")
         x, y = data[0], data[1]
         sw = data[2] if len(data) > 2 else None
-        if isinstance(y, dict):
-            if len(y) != 1:
-                raise NotImplementedError("multi-task targets are not implemented in the training step")
-            y = next(iter(y.values()))
+        outs = self.output_blocks()
         if y is None:
             raise ValueError("train_step needs targets")
+        if isinstance(y, dict):
+            if len(outs) == 1 and len(y) == 1:
+                y = next(iter(y.values()))
+            else:
+                missing = [o.target for o in outs if o.target not in y]
+                if missing:
+                    raise ValueError(f"train_step: no targets for {missing} (got keys {sorted(y)})")
+                y = [y[o.target] for o in outs]
+        elif len(outs) > 1:
+            raise ValueError(f"this model has {len(outs)} outputs: pass the targets as a dict keyed by target column")
+        else:
+            y = [y]
+        if not isinstance(y, list):
+            y = [y]
+        if isinstance(sw, dict):
+            sw = [sw.get(o.name) for o in outs]
         self._check_inputs(x)
         tr = self.trainer(batch_size_of(x))
         loss = tr.step(x, y, sw)
-        return {"loss": loss[0], "loss_batch": loss[0], "regularization_loss": torch.zeros((), device=loss.device)}
+        out = {"loss": loss[0], "loss_batch": loss[0], "regularization_loss": torch.zeros((), device=loss.device)}
+        if len(outs) > 1:
+            out.update({f"{o.name}_loss": loss[1 + h] for h, o in enumerate(outs)})
+        return out
 
     def fit(self, x=None, y=None, batch_size: Optional[int] = None, epochs: int = 1, steps_per_epoch: Optional[int] = None,
             verbose: int = 0, **kwargs):
@@ -240,13 +418,18 @@ class Model(Block):
                     self._check_inputs(inputs)
                     self.trainer(int(bs))
                 m = self.train_step((inputs, targets))
-                total = m["loss_batch"].clone() if total is None else total + m["loss_batch"]
+                # the loss-buffer views are valid until the next step: [loss_batch, per-output losses...] summed on the device
+                vec = torch.stack([m["loss_batch"]] + [v for k, v in m.items() if k not in ("loss", "loss_batch", "regularization_loss")])
+                total = vec.clone() if total is None else total + vec
                 n += 1
                 if steps_per_epoch and n >= steps_per_epoch:
                     break
             if n == 0:
                 raise ValueError("fit: the loader produced no batches")
-            history["loss"].append(float(total.item()) / n)
+            means = (total / n).tolist()
+            history["loss"].append(float(total[0].item()) / n)
+            for i, k in enumerate([k for k in m if k not in ("loss", "loss_batch", "regularization_loss")]):
+                history.setdefault(k, []).append(means[1 + i])
             self._trainer.check_indices()
         from .train import History
 
@@ -305,7 +488,8 @@ class Model(Block):
         if optimizer is not None or isinstance(example, (str, Optimizer)) or example is None:
             if example is not None and optimizer is not None:
                 raise ValueError("compile(): pass either an example batch (graph capture) or an optimizer (training)")
-            return self._compile_training(optimizer if optimizer is not None else (example or "adam"), loss)
+            return self._compile_training(optimizer if optimizer is not None else (example or "adam"), loss,
+                                          call_kwargs.pop("loss_weights", None))
         if not isinstance(example, HostBatch):
             example = HostBatch.like(example, self.input_columns())
         return CompiledForward(self, example, **call_kwargs)
@@ -363,10 +547,20 @@ class RankingModel(Model):
         self._check_inputs(inputs)
         if not self.built:
             self.build(next(iter(inputs.values())).device)
+        heads = self.prediction if isinstance(self.prediction, ParallelOutputs) else None
+        extra = [] if heads is not None else [self.prediction.to_call]
+        if heads is not None and not self.prediction.built:
+            self.prediction.build(self.body_width(), next(iter(inputs.values())).device)
+
+        def chain(x, layers, **kw):
+            if heads is None:
+                return run_dense_chain(x, layers, **kw)
+            return heads.split(run_dense_chain(x, layers, heads=heads, **kw))
+
         if isinstance(self.body, DLRM) and self.body.top_block is not None:
             # top MLP + output layer as ONE dense chain (no fp32 round trip between them)
             # top MLP (+ its normalizations, folded) + the output Dense as one chain
-            layers, tail = self.body.top_block.chain([self.prediction.to_call])
+            layers, tail = self.body.top_block.chain(extra)
             assert tail is None
             if dense_engine() != "fp32" and self.body.can_emit_split():
                 # production path: bottom vector and table rows in the interaction kernel's operand format when the
@@ -374,17 +568,17 @@ class RankingModel(Model):
                 op = self.body.use_operand_rows() and self._all_onehot(inputs)
                 bottom = self.body.bottom_forward(inputs, operand_out=op)
                 a = self.body.interaction_forward(inputs, bottom, as_split=True, operand_rows=op)
-                return run_dense_chain(None, layers, a_split=a, K=self.body.output_width_before_top())
+                return chain(None, layers, a_split=a, K=self.body.output_width_before_top())
             bottom = self.body.bottom_forward(inputs)
             x = self.body.interaction_forward(inputs, bottom)
-            return run_dense_chain(x, layers)
+            return chain(x, layers)
         if isinstance(self.body, DeepFMBody):
             return self.body.forward(inputs, out_layer=self.prediction.to_call)
         if isinstance(self.body, DCNBody) and self.body.stacked:
             x = self.body.cross(self.body.input_block(inputs))
-            layers, tail = self.body.deep.chain([self.prediction.to_call])
+            layers, tail = self.body.deep.chain(extra)
             assert tail is None
-            return run_dense_chain(x, layers)
+            return chain(x, layers)
         x = self.body(inputs, training=training)
         return self.prediction(x)
 
@@ -511,6 +705,8 @@ def DeepFMModel(schema: Schema, embedding_dim: Optional[int] = None, deep_block:
     deep_block = deep_block if deep_block is not None else MLPBlock([64])
     deep_logit_block = deep_logit_block if deep_logit_block is not None else MLPBlock([1], activation="linear", use_bias=True)
     prediction = parse_prediction_blocks(schema, prediction_tasks)
+    if isinstance(prediction, ParallelOutputs):
+        raise NotImplementedError("DeepFMModel with several outputs is not implemented: pass one BinaryOutput")
     return RankingModel(DeepFMBody(input_block, fm, deep_block, deep_logit_block), prediction, schema)
 
 

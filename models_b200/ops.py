@@ -658,14 +658,15 @@ def cross_forward(x0: torch.Tensor, kernels: Sequence[torch.Tensor], biases: Seq
     return out
 
 
-def mlp_tc_supported(K: int, widths: Sequence[int], head: bool = False) -> bool:
+def mlp_tc_supported(K: int, widths: Sequence[int], head: bool = False, heads: bool = False) -> bool:
     """True when mm_mlp_tc can run the tower (mm_mlp_tc_supported): 2..4 layers, every width <= 128, head only
-    after <= 32 units, resident weights of layers 2..n + two layer-1 pipeline stages within shared memory."""
+    after <= 32 units, resident weights of layers 2..n + two layer-1 pipeline stages within shared memory.
+    heads=True: with mm_mlp_tc_heads's multi-head epilogue."""
     n = len(widths)
     if n < 2 or n > 4:
         return False
     wd = (C.c_int * n)(*[int(w) for w in widths])
-    return bool(_lib().mm_mlp_tc_supported(int(K), n, wd, 1 if head else 0))
+    return bool(_lib().mm_mlp_tc_supported(int(K), n, wd, 2 if heads else 1 if head else 0))
 
 
 def mlp_tc(a_split: torch.Tensor, K: int, w_splits: Sequence[torch.Tensor], widths: Sequence[int],
@@ -724,6 +725,43 @@ def mlp_tc(a_split: torch.Tensor, K: int, w_splits: Sequence[torch.Tensor], widt
     return out if out is not None else head_out
 
 
+def mlp_tc_heads(a_split: torch.Tensor, K: int, w_splits: Sequence[torch.Tensor], widths: Sequence[int],
+                 biases: Sequence[Optional[torch.Tensor]], acts: Sequence[Optional[str]], heads_w: torch.Tensor,
+                 heads_b: Optional[torch.Tensor], heads_act: Sequence[Optional[str]], out: torch.Tensor) -> torch.Tensor:
+    """mm_mlp_tc_heads: the whole tower with H <= 8 fused output heads; out (H, M) with
+    out[h] = heads_act[h](tower(x) @ heads_w[:, h] + heads_b[h]).  heads_w (widths[-1], H) Keras layout, heads_b (H,) on the
+    device (read by the kernel, not copied to the host)."""
+    n = len(widths)
+    if not (len(w_splits) == len(biases) == len(acts) == n):
+        raise ValueError("mlp_tc_heads: w_splits / widths / biases / acts must have one entry per layer")
+    _dev(a_split, "a_split", torch.bfloat16), _dev(heads_w, "heads_w", torch.float32), _dev(out, "out", torch.float32)
+    M, H = a_split.shape[0], len(heads_act)
+    if a_split.dim() != 2 or a_split.shape[1] != 2 * tc_padded_k(K) or not a_split.is_contiguous():
+        raise ValueError(f"a_split must be a contiguous (M, {2 * tc_padded_k(K)}) bf16 matrix")
+    if tuple(heads_w.shape) != (int(widths[-1]), H) or not heads_w.is_contiguous():
+        raise ValueError(f"heads_w must be a contiguous ({widths[-1]}, {H}) matrix")
+    if heads_b is not None and (_dev(heads_b, "heads_b", torch.float32).numel() != H or not heads_b.is_contiguous()):
+        raise ValueError(f"heads_b must hold {H} contiguous values")
+    if tuple(out.shape) != (H, M) or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous ({H}, {M}) matrix")
+    k = K
+    for l in range(n):
+        _dev(w_splits[l], f"w_split[{l}]", torch.bfloat16)
+        if tuple(w_splits[l].shape) != (tc_padded_n(int(widths[l])), 2 * tc_padded_k(k)) or not w_splits[l].is_contiguous():
+            raise ValueError(f"w_split[{l}] must be the mm_split_weights layout of a ({k}, {widths[l]}) kernel")
+        if biases[l] is not None and (_dev(biases[l], f"bias[{l}]", torch.float32).numel() != int(widths[l])):
+            raise ValueError(f"bias[{l}] must hold {widths[l]} values")
+        k = int(widths[l])
+    wp = (C.c_void_p * n)(*[w.data_ptr() for w in w_splits])
+    bp = (C.c_void_p * n)(*[_ptr(b) for b in biases])
+    wd = (C.c_int * n)(*[int(w) for w in widths])
+    ac = (C.c_int * n)(*[ACTIVATIONS[a] for a in acts])
+    ha = (C.c_int * H)(*[ACTIVATIONS[a] for a in heads_act])
+    _cabi.check(_lib().mm_mlp_tc_heads(a_split.data_ptr(), M, K, n, wp, wd, bp, ac, H, heads_w.data_ptr(), _ptr(heads_b), ha,
+                                       out.data_ptr(), _stream()), "mm_mlp_tc_heads")
+    return out
+
+
 def dense_tc_head(a_split: torch.Tensor, K: int, w_split: torch.Tensor, N: int, bias: Optional[torch.Tensor],
                   act: Optional[str], head_w: torch.Tensor, head_b: float, head_act: Optional[str],
                   out: torch.Tensor, passes: int = 3) -> torch.Tensor:
@@ -769,6 +807,67 @@ def bce_head_fwd_bwd(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tens
                                    0 if dx is None else _row_stride(_dev(dx, "dx", torch.float32), "dx"), 1 if mask_relu else 0,
                                    dw.data_ptr(), _ptr(db), _stream()),
         "mm_bce_head_fwd_bwd")
+
+
+def heads_fwd_bwd(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], losses: Sequence[str],
+                  targets: Optional[Sequence[torch.Tensor]], out: torch.Tensor, loss: Optional[torch.Tensor] = None,
+                  dx: Optional[torch.Tensor] = None, dw: Optional[torch.Tensor] = None, db: Optional[torch.Tensor] = None,
+                  loss_weights: Optional[Sequence[float]] = None, mask_relu: bool = True, sample_weight=None) -> torch.Tensor:
+    """H <= 8 output heads Dense(K -> 1) on x (M, K), forward and backward in one pass (mm_heads_fwd_bwd).  w (K, H), bias
+    (H,); losses[h] in {"binary_crossentropy", "mse"}.  targets None: forward only, out (H, M) = the activated predictions
+    (sigmoid / linear).  Otherwise out (H, M) = the logits, loss (1 + H) += [sum_h lambda_h loss_h, loss_0, ...], dw (K, H)
+    and db (H,) are ACCUMULATED, dx (M, K) is written.  sample_weight: one (M,) fp32 tensor shared by every head, or a list
+    of H (entries may be None)."""
+    _dev(x, "x", torch.float32), _dev(w, "w", torch.float32), _dev(out, "out", torch.float32)
+    M, K = x.shape
+    H = len(losses)
+    if tuple(w.shape) != (K, H) or not w.is_contiguous():
+        raise ValueError(f"w must be a contiguous ({K}, {H}) matrix")
+    if bias is not None and (_dev(bias, "bias", torch.float32).numel() != H or not bias.is_contiguous()):
+        raise ValueError(f"bias must hold {H} contiguous values")
+    if tuple(out.shape) != (H, M) or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous ({H}, {M}) matrix")
+    if any(l not in _cabi.LOSS_KINDS for l in losses):
+        raise ValueError(f"losses must be among {sorted(_cabi.LOSS_KINDS)}, got {list(losses)}")
+    kinds = (C.c_int * H)(*[_cabi.LOSS_KINDS[l] for l in losses])
+    tp = dt = sp = lw = None
+    if targets is not None:
+        if len(targets) != H:
+            raise ValueError(f"one target tensor per head: {H} expected, got {len(targets)}")
+        for h, t in enumerate(targets):
+            _dev(t, f"targets[{h}]")
+            if t.numel() != M or not t.is_contiguous() or t.dtype not in _TARGET_DTYPES:
+                raise ValueError(f"targets[{h}] must be {M} contiguous int32 / int64 / float32 / float64 values")
+        if loss is None or dw is None:
+            raise ValueError("training needs loss and dw")
+        _dev(loss, "loss", torch.float32), _dev(dw, "dw", torch.float32)
+        if loss.numel() != 1 + H or not loss.is_contiguous():
+            raise ValueError(f"loss must hold 1 + H = {1 + H} contiguous values")
+        if tuple(dw.shape) != (K, H) or not dw.is_contiguous():
+            raise ValueError(f"dw must be a contiguous ({K}, {H}) matrix")
+        if db is not None and (_dev(db, "db", torch.float32).numel() != H or not db.is_contiguous()):
+            raise ValueError(f"db must hold {H} contiguous values")
+        sws = list(sample_weight) if isinstance(sample_weight, (list, tuple)) else [sample_weight] * H
+        if len(sws) != H:
+            raise ValueError(f"one sample-weight tensor per head: {H} expected, got {len(sws)}")
+        for h, s in enumerate(sws):
+            if s is not None and (_dev(s, f"sample_weight[{h}]", torch.float32).numel() != M or not s.is_contiguous()):
+                raise ValueError(f"sample_weight[{h}] must be ({M},) contiguous float32")
+        lws = [1.0] * H if loss_weights is None else [float(v) for v in loss_weights]
+        if len(lws) != H:
+            raise ValueError(f"one loss weight per head: {H} expected, got {len(lws)}")
+        tp = (C.c_void_p * H)(*[t.data_ptr() for t in targets])
+        dt = (C.c_int * H)(*[_TARGET_DTYPES[t.dtype] for t in targets])
+        sp = (C.c_void_p * H)(*[_ptr(s) for s in sws])
+        lw = (C.c_float * H)(*lws)
+    _cabi.check(
+        _lib().mm_heads_fwd_bwd(x.data_ptr(), M, K, _row_stride(x, "x"), H, w.data_ptr(), _ptr(bias), kinds, lw, tp, dt, sp,
+                                out.data_ptr(), _ptr(loss) if targets is not None else None,
+                                _ptr(dx) if targets is not None else None,
+                                0 if dx is None else _row_stride(_dev(dx, "dx", torch.float32), "dx"), 1 if mask_relu else 0,
+                                _ptr(dw) if targets is not None else None, _ptr(db) if targets is not None else None, _stream()),
+        "mm_heads_fwd_bwd")
+    return out
 
 
 def dense_wgrad(x: torch.Tensor, dz: torch.Tensor, dw: torch.Tensor, db: Optional[torch.Tensor]) -> None:

@@ -8,7 +8,8 @@ What a step launches (DLRM, bottom [.., D], top [...], BinaryOutput):
     forward   concat+split -> dense_tc per bottom layer (fp32 activation saved + operand of the next layer) -> fused
               lookup + interaction -> dense_tc per top layer.  D = 64 with table mirrors: the kernel reads operand-format
               rows and writes the top tower's split operand directly; otherwise fp32 rows + one split pass
-    loss      mm_bce_head_fwd_bwd: output Dense(1) + sigmoid + BCE forward AND backward in one pass
+    loss      mm_heads_fwd_bwd: the output heads (BinaryOutput: Dense(1) + sigmoid + BCE; RegressionOutput: Dense(1) + MSE;
+              up to 8 of them with loss weights) forward AND backward in one pass
     backward  per Dense layer mm_dense_wgrad[_split] (dW, db) + mm_dense_dgrad (input gradient, relu mask fused);
               mm_dlrm_interact_backward: pair gradients -> IndexedSlices per table + bottom-vector gradient
     update    mm_opt_tick, [DP: all-reduce of the dense gradient arena, all-gather of the slices], mm_dense_apply over the flat
@@ -188,13 +189,15 @@ class DLRMTrainer:
     """Static-buffer training step of a DLRM RankingModel at one batch size."""
 
     def __init__(self, model, optimizer: Optimizer, batch_size: int, device=None, group=None):
-        from .models import BinaryOutput
+        from .models import BinaryOutput, ParallelOutputs
 
         body = model.body
         if not isinstance(body, DLRM) or body.top_block is None or body.bottom_block is None:
             raise NotImplementedError("train_step is implemented for DLRMModel with bottom and top blocks")
-        if not isinstance(model.prediction, BinaryOutput):
-            raise NotImplementedError("train_step needs a BinaryOutput head (binary cross-entropy)")
+        if not isinstance(model.prediction, (BinaryOutput, ParallelOutputs)):
+            raise NotImplementedError("train_step needs BinaryOutput / RegressionOutput heads or an OutputBlock of them")
+        if group is not None and isinstance(model.prediction, ParallelOutputs):
+            raise NotImplementedError("training several outputs with a process group is not implemented")
         if body.sharded is not None:
             raise NotImplementedError("training with row-sharded tables is not implemented (forward only)")
         if not body.can_emit_split():
@@ -216,6 +219,10 @@ class DLRMTrainer:
         self.bottom = body.bottom_block.dense_layers
         self.top = body.top_block.dense_layers
         self.head = model.prediction.to_call
+        self.outputs = model.output_blocks()
+        self.H = len(self.outputs)
+        self.losses = [o.loss for o in self.outputs]
+        self.loss_weights = list(getattr(model, "loss_weights", None) or [1.0] * self.H)
         for l in self.bottom + self.top:
             if l.activation not in ("relu", "linear"):
                 raise NotImplementedError(f"{l.name}: training supports relu / linear tower activations, got {l.activation!r}")
@@ -283,8 +290,10 @@ class DLRMTrainer:
         self.t_split = [torch.zeros((B, 2 * ops.tc_padded_k(l.units)), dtype=torch.bfloat16, device=self.device) for l in self.top[:-1]]
         self.dt = [torch.zeros((B, l.units), **f32) for l in self.top]
         self.dh = [torch.zeros((B, l.units), **f32) for l in self.bottom]
-        self.logits = torch.zeros(B, **f32)
-        self.loss = torch.zeros(1, **f32)
+        self.logits = torch.zeros((self.H, B) if self.H > 1 else B, **f32)  # z of each output; (B,) for one
+        # [total, loss_0 .. loss_{H-1}]; `loss` is the (1,) total alone for one output, the whole vector for several
+        self._loss_all = torch.zeros(1 + self.H, **f32)
+        self.loss = self._loss_all if self.H > 1 else self._loss_all[:1]
         self.oob = emb.counter(self.device)
         # multi-hot features (ragged bags, (B, L) id matrices), by table position: pooled rows, their operand copy, the
         # expanded row gradients; created on the first batch that carries the feature as a bag (see _indices)
@@ -294,7 +303,7 @@ class DLRMTrainer:
         self.steps = 0
         self._graph = None
         self._static: Optional[Dict[str, torch.Tensor]] = None
-        self._static_y: Optional[torch.Tensor] = None
+        self._static_y: Optional[List[torch.Tensor]] = None
 
     # ---- one step on device tensors ------------------------------------------------------------------------------
     def _indices(self, inputs, b: Optional[int] = None) -> List[torch.Tensor]:
@@ -364,20 +373,25 @@ class DLRMTrainer:
             ops.bag_grad_rows(self._slices[t], bg["ids"], bg["offsets"], self.tables[t].table.shape[0], bg["comb"], bg["rows"],
                               out_ids=bg["apply_ids"] if bg["offsets"] is not None else None)
 
-    def forward_backward(self, inputs: Dict[str, torch.Tensor], targets: torch.Tensor, sample_weight=None) -> None:
+    def forward_backward(self, inputs: Dict[str, torch.Tensor], targets, sample_weight=None) -> None:
         """Forward (activations saved), loss and backward: fills the gradient arena and the IndexedSlices.  Batches smaller
-        than the compiled size run in the leading rows of the same buffers."""
+        than the compiled size run in the leading rows of the same buffers.  targets: one tensor per output (a bare tensor
+        for a single output); sample_weight: one (b,) tensor for every output, or a list with one per output."""
         a = self.arena
         nb, nt = len(self.bottom), len(self.top)
         D = self.D
-        self.loss.zero_()
+        self._loss_all.zero_()
         cont = self.body.continuous(inputs)
         pieces = [cont[k] for k in sorted(cont)]
         b = int(pieces[0].shape[0])
         if b > self.B or b < 1:
             raise ValueError(f"this trainer was compiled for batches of up to {self.B} samples, got {b}")
-        if targets.numel() != b:
-            raise ValueError(f"targets must hold {b} values, got {tuple(targets.shape)}")
+        targets = list(targets) if isinstance(targets, (list, tuple)) else [targets]
+        if len(targets) != self.H:
+            raise ValueError(f"{self.H} target tensors expected (one per output), got {len(targets)}")
+        for o, t in zip(self.outputs, targets):
+            if t.numel() != b:
+                raise ValueError(f"targets of {o.name!r} must hold {b} values, got {tuple(t.shape)}")
 
         def v(t):
             return t[:b]
@@ -415,9 +429,10 @@ class DLRMTrainer:
             op, K = nxt, l.units
         # -- output layer + loss, forward and backward
         hi = nb + nt
-        ops.bce_head_fwd_bwd(t_[-1], self.head.kernel.reshape(-1), self.head.bias, targets.reshape(-1), self.loss, dt[-1],
-                             a.view(a.grad, hi, "kernel").reshape(-1), a.view(a.grad, hi, "bias"),
-                             mask_relu=self.top[-1].activation == "relu", sample_weight=sample_weight, logits=v(self.logits))
+        ops.heads_fwd_bwd(t_[-1], self.head.kernel, self.head.bias, self.losses, [t.reshape(-1) for t in targets],
+                          self.logits.view(-1)[:self.H * b].view(self.H, b),
+                          self._loss_all, dt[-1], a.view(a.grad, hi, "kernel"), a.view(a.grad, hi, "bias"), loss_weights=self.loss_weights,
+                          mask_relu=self.top[-1].activation == "relu", sample_weight=sample_weight)
         # -- top tower backward
         for i in range(nt - 1, -1, -1):
             l = self.top[i]
@@ -497,8 +512,9 @@ class DLRMTrainer:
         for l, ws in zip(self.bottom + self.top, self._wsplit):
             ops.split_weights(l.kernel, out=ws)
 
-    def step(self, inputs: Dict[str, torch.Tensor], targets: torch.Tensor, sample_weight=None) -> torch.Tensor:
-        """One eager training step; returns the batch loss as a (1,) device tensor (valid until the next step)."""
+    def step(self, inputs: Dict[str, torch.Tensor], targets, sample_weight=None) -> torch.Tensor:
+        """One eager training step; returns [total loss, per-output losses...] as a (1 + H,) device tensor (valid until the
+        next step)."""
         self.forward_backward(inputs, targets, sample_weight)
         self.apply_gradients()
         self._after_step()
@@ -523,7 +539,8 @@ class DLRMTrainer:
                 raise NotImplementedError(f"graph capture with the ragged feature {f!r} is not implemented: its number of ids "
                                           "changes from batch to batch (train it eagerly, or feed it as a fixed-length (B, L) matrix)")
         self._static = {k: (v.clone() if clone else v) for k, v in inputs.items()}
-        self._static_y = targets.clone() if clone else targets
+        ys = list(targets) if isinstance(targets, (list, tuple)) else [targets]
+        self._static_y = [y.clone() if clone else y for y in ys]
         self.model.defer_index_check(True)
         try:
             s = torch.cuda.Stream(device=self.device)
@@ -578,7 +595,9 @@ class DLRMTrainer:
             for k, v in self._static.items():
                 v.copy_(inputs[k], non_blocking=True)
         if targets is not None:
-            self._static_y.copy_(targets.reshape(self._static_y.shape), non_blocking=True)
+            ys = list(targets) if isinstance(targets, (list, tuple)) else [targets]
+            for s, y in zip(self._static_y, ys):
+                s.copy_(y.reshape(s.shape), non_blocking=True)
         self._graph.replay()
         self._after_step()
         return self.loss
