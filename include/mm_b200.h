@@ -540,6 +540,31 @@ int mm_dense_apply(int opt, float* w, float* grad, float* state1, float* state2,
 int mm_opt_tick(float* hyper, void* stream);
 int mm_fill_i32(int32_t* p, int64_t n, int32_t value, void* stream);
 
+/* Added with DCN-v2 training; no existing entry point changed, except that mm_sparse_rows_apply now also takes every
+ * D with D % 4 == 0 and 4 <= D <= 128 (formerly D/4 had to divide 32; those widths run exactly as before) and returns
+ * MM_ERR_ARG for a non-null mirror when D != 64.
+ *   mm_cross_backward   one cross layer l of the backward of x_{l+1} = x0 * z_l + x_l, z_l = x_l W_l + b_l, in one pass:
+ *                       g += p (in place; p = dz_{l+1} W_{l+1}^T, null for the top layer), dz = g * x0 written as fp32 (the
+ *                       dz of mm_dense_wgrad[_split]) and as split-bf16 rows dz_split (B, 2*Kp) (mm_split_rows layout,
+ *                       Kp = mm_tc_padded_k(d), padding written as zeros: the operand of the transposed-kernel
+ *                       mm_dense_tc), and acc = g * z (acc_init) or acc += g * z.  Any d >= 1; fp32 row strides multiples
+ *                       of 4, every buffer 16-byte aligned.
+ *   mm_concat_backward  backward of a concatenated input block: for each slice t, dst_t[b, 0:width_t] = sum over the
+ *                       n_addends <= 4 (B, d) addends of addend[b, col_t : col_t + width_t].  Columns of no slice are not
+ *                       read.  col arbitrary, width a positive multiple of 4, dst 16-byte aligned with a row stride that is a
+ *                       multiple of 4; n_slices <= 64.  addends_host / addend_strides_host / slices_host are HOST arrays. */
+typedef struct {
+  float* dst;         /* (B, width) rows, dst_stride floats apart */
+  int64_t dst_stride;
+  int32_t col;        /* first column of the slice in the addends */
+  int32_t width;
+} mm_column_slice;
+int mm_cross_backward(const float* x0, int64_t x0_stride, const float* z, int64_t z_stride, float* g, int64_t g_stride,
+                      const float* p, int64_t p_stride, float* acc, int64_t acc_stride, int acc_init, int64_t B, int d, float* dz,
+                      int64_t dz_stride, void* dz_split, int Kp, void* stream);
+int mm_concat_backward(const float* const* addends_host, const int64_t* addend_strides_host, int n_addends, int64_t B, int d,
+                       const mm_column_slice* slices_host, int n_slices, void* stream);
+
 /* ---------------------------------------------------------------------------------------
  * K15  Factorization-machine heads (blocks/interaction.py:205-332; DeepFMModel models/ranking.py:171-279).
  *   mm_fm_pairwise   FMPairwiseInteraction.call: x (B, A, K) -> out (B, K) = 0.5 ((sum_a x)^2 - sum_a x^2)

@@ -83,6 +83,17 @@ class ConcatPiece(C.Structure):
     ]
 
 
+class ColumnSlice(C.Structure):
+    """mm_column_slice (include/mm_b200.h)."""
+
+    _fields_ = [
+        ("dst", C.c_void_p),
+        ("dst_stride", C.c_int64),
+        ("col", C.c_int32),
+        ("width", C.c_int32),
+    ]
+
+
 _vp, _i, _i64, _f, _u64 = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_uint64
 _tables = C.POINTER(GatherTable)
 
@@ -151,6 +162,8 @@ SIGNATURES = {
     "mm_dense_apply": (_i, [_i, _vp, _vp, _vp, _vp, _i64, _vp, _f, _vp]),
     "mm_opt_tick": (_i, [_vp, _vp]),
     "mm_fill_i32": (_i, [_vp, _i64, C.c_int32, _vp]),
+    "mm_cross_backward": (_i, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _i, _i64, _i, _vp, _i64, _vp, _i, _vp]),
+    "mm_concat_backward": (_i, [C.POINTER(C.c_void_p), C.POINTER(C.c_int64), _i, _i64, _i, C.POINTER(ColumnSlice), _i, _vp]),
 }
 
 

@@ -769,10 +769,201 @@ static int launch_dgrad(const DgradParams& p, cudaStream_t st) {
   return check_launch("mm_dense_dgrad");
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// DCN-v2 cross network backward, one launch per layer l (x_{l+1} = x0 * z_l + x_l, z_l = x_l W_l + b_l).  With g the
+// gradient flowing into x_{l+1} and p = dz_{l+1} W_{l+1}^T the dgrad of the layer above (null for the top layer):
+//   g += p (in place);  dz_l = g * x0 (fp32 for the weight gradient, split-bf16 for the transposed-kernel dgrad);
+//   acc = g * z_l (first layer) or acc += g * z_l  — the x0 terms of the product rule.
+// HBM-bound, one pass: one warp per row (8 rows per CTA, grid-stride over the rows), each lane a 4-column group at a time,
+// so no thread divides its flat index by the row width.  Groups of the split padding columns [d, Kp) write zeros.
+// ---------------------------------------------------------------------------------------------------------------
+struct CrossBwdParams {
+  const float* x0;
+  const float* z;
+  float* g;
+  const float* p;
+  float* acc;
+  float* dz;
+  __nv_bfloat16* dz_split;
+  long long ldx0, ldz, ldg, ldp, ldacc, lddz;
+  long long B;
+  int d, Kp, acc_init;
+};
+
+// n (1..4) leading floats of a 16-byte aligned group; the missing ones read as 0
+__device__ __forceinline__ float4 ld_part4(const float* p, int n) {
+  if (n >= 4) return *reinterpret_cast<const float4*>(p);
+  float4 v = make_float4(p[0], 0.f, 0.f, 0.f);
+  if (n > 1) v.y = p[1];
+  if (n > 2) v.z = p[2];
+  return v;
+}
+__device__ __forceinline__ void st_part4(float* p, const float4& v, int n) {
+  if (n >= 4) {
+    *reinterpret_cast<float4*>(p) = v;
+    return;
+  }
+  p[0] = v.x;
+  if (n > 1) p[1] = v.y;
+  if (n > 2) p[2] = v.z;
+}
+
+constexpr int CB_ROWS = 8;  // rows (warps) per CTA of cross_backward_kernel
+__global__ void __launch_bounds__(32 * CB_ROWS) cross_backward_kernel(const CrossBwdParams q) {
+  const int Q = q.Kp >> 2;
+  const int lane = threadIdx.x & 31;
+  for (long long m = (long long)blockIdx.x * CB_ROWS + (threadIdx.x >> 5); m < q.B; m += (long long)gridDim.x * CB_ROWS) {
+    for (int qi = lane; qi < Q; qi += 32) {
+      const int c = qi * 4;
+      const int n = q.d - c;
+      float4 dz = make_float4(0.f, 0.f, 0.f, 0.f);
+      if (n > 0) {
+        float* gp = q.g + m * q.ldg + c;
+        float4 g = ld_part4(gp, n);
+        if (q.p) {
+          const float4 p = ld_part4(q.p + m * q.ldp + c, n);
+          g.x += p.x;
+          g.y += p.y;
+          g.z += p.z;
+          g.w += p.w;
+          st_part4(gp, g, n);
+        }
+        const float4 x0 = ld_part4(q.x0 + m * q.ldx0 + c, n);
+        const float4 z = ld_part4(q.z + m * q.ldz + c, n);
+        dz = make_float4(g.x * x0.x, g.y * x0.y, g.z * x0.z, g.w * x0.w);
+        float* ap = q.acc + m * q.ldacc + c;
+        float4 a = make_float4(g.x * z.x, g.y * z.y, g.z * z.z, g.w * z.w);
+        if (!q.acc_init) {
+          const float4 o = ld_part4(ap, n);
+          a.x += o.x;
+          a.y += o.y;
+          a.z += o.z;
+          a.w += o.w;
+        }
+        st_part4(ap, a, n);
+        st_part4(q.dz + m * q.lddz + c, dz, n);
+      }
+      uint32_t h0, l0, h1, l1;
+      split_pair(dz.x, dz.y, h0, l0);
+      split_pair(dz.z, dz.w, h1, l1);
+      __nv_bfloat16* o = q.dz_split + m * (2ll * q.Kp) + c;
+      *reinterpret_cast<uint2*>(o) = make_uint2(h0, h1);
+      *reinterpret_cast<uint2*>(o + q.Kp) = make_uint2(l0, l1);
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Backward of the concatenated input block x0 = [.. table t's rows at columns [col_t, col_t + D_t) ..]: the sum of the
+// addends (B, d) (the cross network's running gradient, its last dgrad, the product-rule terms, a deep branch's input
+// gradient) restricted to each table's columns, written straight into that table's contiguous (B, D_t) slice buffer —
+// the IndexedSlices values.  Columns of no table (continuous features) are never read.  Offsets are arbitrary (width-1
+// continuous columns interleave by sorted name), so the addends are read as scalars; the slices are written as float4.
+// blockIdx.y = table.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int CB_MAX_ADD = 4;
+constexpr int CB_MAX_SLICES = 64;
+struct ConcatBwdParams {
+  const float* add[CB_MAX_ADD];
+  long long ld[CB_MAX_ADD];
+  mm_column_slice s[CB_MAX_SLICES];
+  long long B;
+  int n_add;
+};
+
+__global__ void __launch_bounds__(256) concat_backward_kernel(const __grid_constant__ ConcatBwdParams q) {
+  const mm_column_slice& s = q.s[blockIdx.y];
+  const int Q = s.width >> 2;
+  const long long total = q.B * Q;
+  for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
+    const long long m = e / Q;
+    const int c = (int)(e - m * Q) * 4;
+    float v[4] = {0.f, 0.f, 0.f, 0.f};
+    for (int a = 0; a < q.n_add; ++a) {
+      const float* src = q.add[a] + m * q.ld[a] + s.col + c;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) v[j] += src[j];
+    }
+    *reinterpret_cast<float4*>(s.dst + m * s.dst_stride + c) = make_float4(v[0], v[1], v[2], v[3]);
+  }
+}
+
 }  // namespace trn
 }  // namespace mm
 
 extern "C" {
+
+int mm_cross_backward(const float* x0, int64_t x0_stride, const float* z, int64_t z_stride, float* g, int64_t g_stride,
+                      const float* p, int64_t p_stride, float* acc, int64_t acc_stride, int acc_init, int64_t B, int d, float* dz,
+                      int64_t dz_stride, void* dz_split, int Kp, void* stream) {
+  using namespace mm::trn;
+  MM_REQUIRE(x0 && z && g && acc && dz && dz_split && B >= 0 && d >= 1, MM_ERR_ARG, "mm_cross_backward: null pointer or d < 1");
+  MM_REQUIRE(Kp == mm_tc_padded_k(d), MM_ERR_ARG, "mm_cross_backward: Kp must be mm_tc_padded_k(d)=%d", mm_tc_padded_k(d));
+  MM_REQUIRE(x0_stride >= d && z_stride >= d && g_stride >= d && acc_stride >= d && dz_stride >= d && (!p || p_stride >= d), MM_ERR_ARG,
+             "mm_cross_backward: a row stride is < d");
+  MM_REQUIRE(((x0_stride | z_stride | g_stride | acc_stride | dz_stride | (p ? p_stride : 0)) & 3) == 0, MM_ERR_ALIGN,
+             "mm_cross_backward: row strides must be multiples of 4");
+  MM_REQUIRE((((uintptr_t)x0 | (uintptr_t)z | (uintptr_t)g | (uintptr_t)p | (uintptr_t)acc | (uintptr_t)dz | (uintptr_t)dz_split) & 15) == 0,
+             MM_ERR_ALIGN, "mm_cross_backward: every buffer must be 16-byte aligned");
+  if (B == 0) return MM_OK;
+  CrossBwdParams q;
+  memset(&q, 0, sizeof(q));
+  q.x0 = x0;
+  q.z = z;
+  q.g = g;
+  q.p = p;
+  q.acc = acc;
+  q.dz = dz;
+  q.dz_split = (__nv_bfloat16*)dz_split;
+  q.ldx0 = x0_stride;
+  q.ldz = z_stride;
+  q.ldg = g_stride;
+  q.ldp = p_stride;
+  q.ldacc = acc_stride;
+  q.lddz = dz_stride;
+  q.B = B;
+  q.d = d;
+  q.Kp = Kp;
+  q.acc_init = acc_init ? 1 : 0;
+  long long blocks = (B + CB_ROWS - 1) / CB_ROWS;
+  const long long cap = 16LL * mm::sm_count();
+  if (blocks > cap) blocks = cap;
+  cross_backward_kernel<<<(unsigned)blocks, 32 * CB_ROWS, 0, (cudaStream_t)stream>>>(q);
+  return mm::check_launch("mm_cross_backward");
+}
+
+int mm_concat_backward(const float* const* addends_host, const int64_t* addend_strides_host, int n_addends, int64_t B, int d,
+                       const mm_column_slice* slices_host, int n_slices, void* stream) {
+  using namespace mm::trn;
+  MM_REQUIRE(addends_host && addend_strides_host && slices_host && B >= 0 && d >= 1, MM_ERR_ARG, "mm_concat_backward: null pointer or d < 1");
+  MM_REQUIRE(n_addends >= 1 && n_addends <= CB_MAX_ADD, MM_ERR_ARG, "mm_concat_backward: n_addends=%d outside [1, %d]", n_addends, CB_MAX_ADD);
+  MM_REQUIRE(n_slices >= 1 && n_slices <= CB_MAX_SLICES, MM_ERR_ARG, "mm_concat_backward: n_slices=%d outside [1, %d]", n_slices, CB_MAX_SLICES);
+  ConcatBwdParams q;
+  memset(&q, 0, sizeof(q));
+  for (int a = 0; a < n_addends; ++a) {
+    MM_REQUIRE(addends_host[a] && addend_strides_host[a] >= d, MM_ERR_ARG, "mm_concat_backward: addend %d: null or stride < d", a);
+    q.add[a] = addends_host[a];
+    q.ld[a] = addend_strides_host[a];
+  }
+  int qmax = 0;
+  for (int t = 0; t < n_slices; ++t) {
+    const mm_column_slice& s = slices_host[t];
+    MM_REQUIRE(s.dst && s.width >= 4 && (s.width & 3) == 0 && s.col >= 0 && (int64_t)s.col + s.width <= d, MM_ERR_ARG,
+               "mm_concat_backward: slice %d: null destination, width not a positive multiple of 4, or columns outside [0, d)", t);
+    MM_REQUIRE(s.dst_stride >= s.width && (s.dst_stride & 3) == 0 && ((uintptr_t)s.dst & 15) == 0, MM_ERR_ALIGN,
+               "mm_concat_backward: slice %d: destination must be 16-byte aligned with a row stride >= width and a multiple of 4", t);
+    q.s[t] = s;
+    if (s.width / 4 > qmax) qmax = s.width / 4;
+  }
+  q.B = B;
+  q.n_add = n_addends;
+  if (B == 0) return MM_OK;
+  long long blocks = (B * qmax + 255) / 256;
+  const long long cap = 4LL * mm::sm_count();
+  if (blocks > cap) blocks = cap;
+  concat_backward_kernel<<<dim3((unsigned)blocks, (unsigned)n_slices), 256, 0, (cudaStream_t)stream>>>(q);
+  return mm::check_launch("mm_concat_backward");
+}
 
 int mm_bce_head_fwd_bwd(const float* x, int64_t M, int K, int64_t x_stride, const float* w, const float* bias, const void* targets,
                         int target_dtype, const float* sample_weight, float* logits, float* loss_sum, float* dx,

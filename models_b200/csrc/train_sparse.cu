@@ -507,7 +507,7 @@ struct SparseParams {
   SparseTable t[MM_LOOKUP_MAX_ROWS];
   long long B;
   int D;
-  int lgL;  // log2(D / 4): lanes per row (a 64-bit division by a runtime value costs ~100 instructions and the XU pipe)
+  int lgL;  // ceil(log2(D / 4)): lanes per row, those past D/4 idle (a 64-bit division by a runtime value costs ~100 instructions and the XU pipe)
   int opt;
   const float* hyper;  // device: see mm_b200.h MM_HYPER_*
   int n;                                       // tables in t[]
@@ -581,10 +581,9 @@ __device__ __forceinline__ float upd(int opt, float w, float g, float& s1, float
 
 __global__ void sparse_apply_kernel(const __grid_constant__ SparseParams p) {
   const SparseTable& tb = p.t[blockIdx.y];
-  const int L = p.D >> 2;
   const long long b = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> p.lgL;
-  const int c = threadIdx.x & (L - 1);
-  if (b >= p.B) return;
+  const int c = threadIdx.x & ((1 << p.lgL) - 1);
+  if (b >= p.B || c >= (p.D >> 2)) return;
   const unsigned long long id = (unsigned long long)load_id(tb.ids, tb.idx_bytes, b);
   if (id >= (unsigned long long)tb.rows) return;
   // The row and its slots are requested TOGETHER with the map entry (one dependent round trip less: id -> {map, row});
@@ -690,8 +689,8 @@ __global__ void __launch_bounds__(256) sparse_scatter_small_kernel(const __grid_
     }
   __syncthreads();
   const int valid = cnt[rows];
-  const int L = p.D >> 2;
-  const int c = threadIdx.x & (L - 1), grp = threadIdx.x >> p.lgL, ngrp = blockDim.x >> p.lgL;
+  const int c = threadIdx.x & ((1 << p.lgL) - 1), grp = threadIdx.x >> p.lgL, ngrp = blockDim.x >> p.lgL;
+  if (c >= (p.D >> 2)) return;  // lanes past D/4 of a group (no barrier follows)
   const int per = (valid + ngrp - 1) / ngrp;
   const int k0 = grp * per, k1 = min(valid, k0 + per);
   int cur = -1;
@@ -732,10 +731,9 @@ __global__ void __launch_bounds__(256) sparse_scatter_small_kernel(const __grid_
 
 __global__ void sparse_scatter_mid_kernel(const __grid_constant__ SparseParams p) {
   const SparseTable& tb = p.t[blockIdx.y];
-  const int L = p.D >> 2;
   const long long b = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> p.lgL;
-  const int c = threadIdx.x & (L - 1);
-  if (b >= p.B) return;
+  const int c = threadIdx.x & ((1 << p.lgL) - 1);
+  if (b >= p.B || c >= (p.D >> 2)) return;
   const unsigned long long id = (unsigned long long)load_id(tb.ids, tb.idx_bytes, b);
   if (id >= (unsigned long long)tb.rows) return;
   const float4 v = *reinterpret_cast<const float4*>(tb.grad + b * p.D + 4 * c);
@@ -746,10 +744,9 @@ __global__ void sparse_scatter_mid_kernel(const __grid_constant__ SparseParams p
 // one group of D/4 lanes per ROW of a dense-path table (rows of all such tables form one flattened index space: row_start
 // holds the prefix sums): touched rows are updated from the accumulator, which is cleared
 __global__ void sparse_apply_dense_kernel(const __grid_constant__ SparseParams p) {
-  const int L = p.D >> 2;
   const long long fr = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> p.lgL;
-  const int c = threadIdx.x & (L - 1);
-  if (fr >= p.row_start[p.n]) return;
+  const int c = threadIdx.x & ((1 << p.lgL) - 1);
+  if (fr >= p.row_start[p.n] || c >= (p.D >> 2)) return;
   int t = 0;
   while (fr >= p.row_start[t + 1]) ++t;
   const SparseTable& tb = p.t[t];
@@ -969,7 +966,8 @@ int mm_sparse_rows_apply(const mm_sparse_table* tables_host, int n_tables, int64
   using namespace mm::trs;
   MM_REQUIRE(tables_host && n_tables > 0 && n_tables <= MM_LOOKUP_MAX_ROWS && hyper && B >= 0, MM_ERR_ARG,
              "mm_sparse_rows_apply: null pointer or n_tables outside [1, %d]", MM_LOOKUP_MAX_ROWS);
-  MM_REQUIRE(D >= 4 && D <= 128 && (D & 3) == 0 && (32 % (D / 4)) == 0, MM_ERR_UNSUPPORTED, "mm_sparse_rows_apply: D=%d (needs D %% 4 == 0, D/4 a divisor of 32)", D);
+  // a row is a group of L = next power of two >= D/4 lanes (one float4 each) inside one warp; lanes past D/4 are idle
+  MM_REQUIRE(D >= 4 && D <= 128 && (D & 3) == 0, MM_ERR_UNSUPPORTED, "mm_sparse_rows_apply: D=%d (needs D %% 4 == 0, 4 <= D <= 128)", D);
   MM_REQUIRE(opt == MM_OPT_SGD || opt == MM_OPT_ADAGRAD || opt == MM_OPT_ADAM, MM_ERR_ARG, "mm_sparse_rows_apply: unknown optimizer %d", opt);
   MM_REQUIRE(B < (int64_t)INT_MAX, MM_ERR_UNSUPPORTED, "mm_sparse_rows_apply: batch too large for the int32 representative map");
   if (B == 0) return MM_OK;
@@ -985,6 +983,7 @@ int mm_sparse_rows_apply(const mm_sparse_table* tables_host, int n_tables, int64
     MM_REQUIRE(s.weights && s.indices && s.grad_rows && s.rep_map && s.rows > 0, MM_ERR_ARG, "mm_sparse_rows_apply: table %d: null pointer", i);
     MM_REQUIRE(opt == MM_OPT_SGD || s.state1, MM_ERR_ARG, "mm_sparse_rows_apply: table %d: optimizer state missing", i);
     MM_REQUIRE(opt != MM_OPT_ADAM || s.state2, MM_ERR_ARG, "mm_sparse_rows_apply: table %d: second optimizer state missing", i);
+    MM_REQUIRE(!s.mirror || D == 64, MM_ERR_ARG, "mm_sparse_rows_apply: table %d: an operand mirror needs D = 64", i);
     MM_REQUIRE((((uintptr_t)s.weights | (uintptr_t)s.grad_rows | (uintptr_t)s.state1 | (uintptr_t)s.state2 | (uintptr_t)s.dense_grad) & 15) == 0,
                MM_ERR_ALIGN, "mm_sparse_rows_apply: table %d: 16-byte alignment", i);
     if (const int rc = check_id_column("mm_sparse_rows_apply", i, s.indices, s.idx_bytes, s.rows)) return rc;
@@ -1021,7 +1020,7 @@ int mm_sparse_rows_apply(const mm_sparse_table* tables_host, int n_tables, int64
     q->hyper = hyper;
   }
   cudaStream_t st = (cudaStream_t)stream;
-  const int L = D / 4;
+  const int L = 1 << pb.lgL;
   const unsigned bx1 = (unsigned)((B + 255) / 256), bxl = (unsigned)((B * L + 255) / 256);
   int rc = MM_OK;
   if (ns) {

@@ -348,8 +348,9 @@ class Model(Block):
         self._trainer = None
 
     def trainer(self, batch_size: int, group=None):
-        """The static-buffer training engine for batches of (up to) `batch_size` samples (train.DLRMTrainer)."""
-        from .train import DLRMTrainer
+        """The static-buffer training engine for batches of (up to) `batch_size` samples (train.DLRMTrainer or
+        train.DCNTrainer, by the body)."""
+        from .train import trainer_for
 
         if getattr(self, "optimizer", None) is None:
             raise RuntimeError("compile() the model with an optimizer before training it")
@@ -361,7 +362,7 @@ class Model(Block):
                 raise NotImplementedError("the training batch size grew after the first step: create the engine for the largest "
                                           "batch first (model.trainer(batch_size) before the first train_step)")
             return tr
-        tr = self._trainer = DLRMTrainer(self, self.optimizer, batch_size, group=group)
+        tr = self._trainer = trainer_for(self, self.optimizer, batch_size, group=group)
         return tr
 
     def train_step(self, data) -> Dict[str, torch.Tensor]:

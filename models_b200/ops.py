@@ -816,7 +816,7 @@ def heads_fwd_bwd(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor]
     """H <= 8 output heads Dense(K -> 1) on x (M, K), forward and backward in one pass (mm_heads_fwd_bwd).  w (K, H), bias
     (H,); losses[h] in {"binary_crossentropy", "mse"}.  targets None: forward only, out (H, M) = the activated predictions
     (sigmoid / linear).  Otherwise out (H, M) = the logits, loss (1 + H) += [sum_h lambda_h loss_h, loss_0, ...], dw (K, H)
-    and db (H,) are ACCUMULATED, dx (M, K) is written.  sample_weight: one (M,) fp32 tensor shared by every head, or a list
+    and db (H,) are ACCUMULATED (each nullable), dx (M, K) is written.  sample_weight: one (M,) fp32 tensor shared by every head, or a list
     of H (entries may be None)."""
     _dev(x, "x", torch.float32), _dev(w, "w", torch.float32), _dev(out, "out", torch.float32)
     M, K = x.shape
@@ -838,12 +838,12 @@ def heads_fwd_bwd(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor]
             _dev(t, f"targets[{h}]")
             if t.numel() != M or not t.is_contiguous() or t.dtype not in _TARGET_DTYPES:
                 raise ValueError(f"targets[{h}] must be {M} contiguous int32 / int64 / float32 / float64 values")
-        if loss is None or dw is None:
-            raise ValueError("training needs loss and dw")
-        _dev(loss, "loss", torch.float32), _dev(dw, "dw", torch.float32)
+        if loss is None:
+            raise ValueError("training needs loss")
+        _dev(loss, "loss", torch.float32)
         if loss.numel() != 1 + H or not loss.is_contiguous():
             raise ValueError(f"loss must hold 1 + H = {1 + H} contiguous values")
-        if tuple(dw.shape) != (K, H) or not dw.is_contiguous():
+        if dw is not None and (_dev(dw, "dw", torch.float32).shape != (K, H) or not dw.is_contiguous()):
             raise ValueError(f"dw must be a contiguous ({K}, {H}) matrix")
         if db is not None and (_dev(db, "db", torch.float32).numel() != H or not db.is_contiguous()):
             raise ValueError(f"db must hold {H} contiguous values")
@@ -1035,6 +1035,50 @@ def bag_grad_rows(g: torch.Tensor, ids: torch.Tensor, offsets: Optional[torch.Te
                                         L, nnz, int(rows), COMBINERS[combiner], out.data_ptr(), _ptr(out_ids), _stream()),
                 "mm_bag_grad_rows")
     return out
+
+
+def cross_backward(x0: torch.Tensor, z: torch.Tensor, g: torch.Tensor, p: Optional[torch.Tensor], acc: torch.Tensor, acc_init: bool,
+                   dz: torch.Tensor, dz_split: torch.Tensor) -> None:
+    """One DCN-v2 cross layer of the backward (mm_cross_backward): g += p (in place; p None for the top layer),
+    dz = g * x0 as fp32 and as the split-bf16 operand dz_split (B, 2*Kp), acc = g * z (acc_init) or acc += g * z.
+    All fp32 operands (B, d) with row strides that are multiples of 4."""
+    fs = [("x0", x0), ("z", z), ("g", g), ("acc", acc), ("dz", dz)] + ([("p", p)] if p is not None else [])
+    for n_, t_ in fs:
+        _dev(t_, n_, torch.float32)
+    B, d = x0.shape
+    for n_, t_ in fs:
+        if tuple(t_.shape) != (B, d):
+            raise ValueError(f"{n_} must be ({B}, {d}), got {tuple(t_.shape)}")
+    _dev(dz_split, "dz_split", torch.bfloat16)
+    Kp = tc_padded_k(d)
+    if tuple(dz_split.shape) != (B, 2 * Kp) or not dz_split.is_contiguous():
+        raise ValueError(f"dz_split must be a contiguous bf16 ({B}, {2 * Kp}) matrix")
+    _cabi.check(_lib().mm_cross_backward(x0.data_ptr(), _row_stride(x0, "x0"), z.data_ptr(), _row_stride(z, "z"), g.data_ptr(),
+                                         _row_stride(g, "g"), _ptr(p), 0 if p is None else _row_stride(p, "p"), acc.data_ptr(),
+                                         _row_stride(acc, "acc"), 1 if acc_init else 0, B, d, dz.data_ptr(), _row_stride(dz, "dz"),
+                                         dz_split.data_ptr(), Kp, _stream()), "mm_cross_backward")
+
+
+def concat_backward(addends: Sequence[torch.Tensor], slices: Sequence[tuple]) -> None:
+    """Backward of a concatenated input block (mm_concat_backward): for each (dst (B, w), col) in `slices`,
+    dst = sum of the (B, d) addends' columns [col, col + w)."""
+    if not addends:
+        raise ValueError("concat_backward needs at least one addend")
+    B, d = addends[0].shape
+    n = len(addends)
+    ap, st = (C.c_void_p * n)(), (C.c_int64 * n)()
+    for i, a in enumerate(addends):
+        _dev(a, f"addends[{i}]", torch.float32)
+        if tuple(a.shape) != (B, d):
+            raise ValueError(f"addends[{i}] must be ({B}, {d}), got {tuple(a.shape)}")
+        ap[i], st[i] = a.data_ptr(), _row_stride(a, f"addends[{i}]")
+    arr = (_cabi.ColumnSlice * max(len(slices), 1))()
+    for t, (dst, col) in enumerate(slices):
+        _dev(dst, f"slices[{t}].dst", torch.float32)
+        if dst.dim() != 2 or dst.shape[0] != B:
+            raise ValueError(f"slices[{t}].dst must be ({B}, width), got {tuple(dst.shape)}")
+        arr[t].dst, arr[t].dst_stride, arr[t].col, arr[t].width = dst.data_ptr(), _row_stride(dst, f"slices[{t}].dst"), int(col), dst.shape[1]
+    _cabi.check(_lib().mm_concat_backward(ap, st, n, B, d, arr, len(slices), _stream()), "mm_concat_backward")
 
 
 def dense_apply(opt: str, w: torch.Tensor, grad: torch.Tensor, state1: Optional[torch.Tensor], state2: Optional[torch.Tensor],

@@ -22,6 +22,9 @@ at ids 0..B-1, so those kernels serve them unchanged; the backward's slice of th
 mm_bag_grad_rows expands to one scaled row per id for one mm_sparse_rows_apply call per multi-hot table.  Ragged features are
 trained eagerly (their number of ids changes per batch); fixed-length ones can be captured like one-hot features.
 
+DCNModel trains through DCNTrainer (below): the cross network's backward (mm_cross_backward per layer), the input block's
+backward straight into per-table slices (mm_concat_backward) and one sparse update per distinct embedding width.
+
 All Dense variables of the model are re-homed into ONE flat fp32 arena (gradients and optimizer slots mirror its layout), so
 the dense update is one launch and data-parallel training needs one all-reduce.  Every buffer is static: a step can be
 captured into a CUDA graph (`DLRMTrainer.capture()` / `replay()`), the learning rate lives in device memory.
@@ -39,6 +42,8 @@ from .core import batch_size_of, default_device, get_feature
 
 INT32_MAX = 2**31 - 1
 DENSE_PATH_MAX_ROWS = 131072  # tables up to this size accumulate duplicate ids in a dense (rows, D) gradient
+SPARSE_MAX_TABLES = 32  # tables per mm_sparse_rows_apply call (MM_LOOKUP_MAX_ROWS)
+CONCAT_MAX_SLICES = 64  # tables per mm_concat_backward call
 
 
 class History:
@@ -185,7 +190,229 @@ def gather_slices(ids: torch.Tensor, slices: torch.Tensor, group) -> tuple:
             all_sl.permute(1, 0, 2, 3).reshape(T, world * B, slices.shape[2]).contiguous())
 
 
-class DLRMTrainer:
+class _StepTrainer:
+    """What every static-buffer training step shares: the output heads, the dgrad of Dense layers, the update of the
+    dense arena and the embedding tables, CUDA-graph capture / replay, and the host-side bookkeeping.  A subclass sets
+    the attributes below in its __init__ and implements forward_backward / apply_gradients:
+      model, body, opt, device, B, group, world, arena, hyper, head, outputs, H, losses, loss_weights,
+      _tc_layers / _wsplit (Dense layers whose split operand copies follow the updates), _wide (see _init_wide),
+      feats / tables / tstate1 / tstate2 / rep / tdense, oob, logits / _loss_all / loss."""
+
+    def _init_common(self, model, optimizer: Optimizer, batch_size: int, device, group) -> None:
+        self.model, self.body, self.opt = model, model.body, optimizer
+        self.device = torch.device(device) if device is not None else default_device()
+        self.B = int(batch_size)
+        self.group = group
+        self.world = 1
+        if group is not None:
+            import torch.distributed as dist
+
+            self.world = dist.get_world_size(group)
+        if not model.built:
+            model.build(self.device)
+
+    def _init_heads(self) -> None:
+        self.head = self.model.prediction.to_call
+        self.outputs = self.model.output_blocks()
+        self.H = len(self.outputs)
+        self.losses = [o.loss for o in self.outputs]
+        self.loss_weights = list(getattr(self.model, "loss_weights", None) or [1.0] * self.H)
+
+    def _init_wide(self, needs_dgrad, dz_split_given=lambda li: False) -> None:
+        """Layers wider than mm_dense_dgrad's 128 units take dX = dZ W^T through the tensor-core forward GEMM on the
+        transposed kernel: per such layer of _tc_layers (index li with needs_dgrad(li)) a transposed copy, its split
+        operand and, unless the caller passes dZ's split to _dgrad (dz_split_given(li)), the split of dZ."""
+        self._wide: Dict[int, dict] = {}
+        for li, l in enumerate(self._tc_layers):
+            if l.units > 128 and needs_dgrad(li):
+                K, N = l.kernel.shape
+                wT = torch.empty((N, K), dtype=torch.float32, device=self.device)
+                dzs = None if dz_split_given(li) else torch.zeros((self.B, 2 * ops.tc_padded_k(N)), dtype=torch.bfloat16, device=self.device)
+                self._wide[li] = dict(wT=wT, wT_split=torch.zeros((ops.tc_padded_n(K), 2 * ops.tc_padded_k(N)), dtype=torch.bfloat16, device=self.device),
+                                      dz_split=dzs)
+
+    def _init_table_state(self, optimizer: Optimizer) -> None:
+        self.rep = [ops.fill_i32(torch.empty(t.table.shape[0], dtype=torch.int32, device=self.device), INT32_MAX) for t in self.tables]
+        self.tstate1 = [torch.full_like(t.table, optimizer.initial_accumulator_value) if optimizer.slots >= 1 else None for t in self.tables]
+        self.tstate2 = [torch.zeros_like(t.table) if optimizer.slots >= 2 else None for t in self.tables]
+        # tables with few rows (every id repeats many times per batch) sum their slices into a dense accumulator
+        self.tdense = [torch.zeros_like(t.table) if t.table.shape[0] <= DENSE_PATH_MAX_ROWS else None for t in self.tables]
+
+    def _init_loss(self, B: int) -> None:
+        f32 = dict(dtype=torch.float32, device=self.device)
+        self.logits = torch.zeros((self.H, B) if self.H > 1 else B, **f32)  # z of each output; (B,) for one
+        # [total, loss_0 .. loss_{H-1}]; `loss` is the (1,) total alone for one output, the whole vector for several
+        self._loss_all = torch.zeros(1 + self.H, **f32)
+        self.loss = self._loss_all if self.H > 1 else self._loss_all[:1]
+        self.steps = 0
+        self._graph = None
+        self._static: Optional[Dict[str, torch.Tensor]] = None
+        self._static_y: Optional[List[torch.Tensor]] = None
+
+    def _check_targets(self, targets, b: int) -> list:
+        if b > self.B or b < 1:
+            raise ValueError(f"this trainer was compiled for batches of up to {self.B} samples, got {b}")
+        targets = list(targets) if isinstance(targets, (list, tuple)) else [targets]
+        if len(targets) != self.H:
+            raise ValueError(f"{self.H} target tensors expected (one per output), got {len(targets)}")
+        for o, t in zip(self.outputs, targets):
+            if t.numel() != b:
+                raise ValueError(f"targets of {o.name!r} must hold {b} values, got {tuple(t.shape)}")
+        return targets
+
+    def _heads(self, x: torch.Tensor, targets, dx: torch.Tensor, mask_relu: bool, sample_weight, b: int) -> None:
+        """The output heads' forward, loss and backward: logits, loss, dx and the head's gradients in the arena."""
+        a, hi = self.arena, len(self.arena.layers) - 1
+        ops.heads_fwd_bwd(x, self.head.kernel, self.head.bias, self.losses, [t.reshape(-1) for t in targets],
+                          self.logits.view(-1)[:self.H * b].view(self.H, b),
+                          self._loss_all, dx, a.view(a.grad, hi, "kernel"), a.view(a.grad, hi, "bias"), loss_weights=self.loss_weights,
+                          mask_relu=mask_relu, sample_weight=sample_weight)
+
+    def _dgrad(self, li: int, layer: _Dense, dz: torch.Tensor, dx: torch.Tensor, mask: Optional[torch.Tensor],
+               dz_split: Optional[torch.Tensor] = None) -> None:
+        """dx = dz W^T (zeroed where mask <= 0) for layer `li` of _tc_layers.  dz_split: dz's split operand when it exists
+        already (wide layers only)."""
+        wide = self._wide.get(li)
+        if wide is None:
+            ops.dense_dgrad(dz, layer.kernel, dx, mask=mask)
+            return
+        K, N = layer.kernel.shape
+        b = dz.shape[0]
+        wide["wT"].copy_(layer.kernel.t())
+        ops.split_weights(wide["wT"], out=wide["wT_split"])
+        if dz_split is None:
+            dz_split = wide["dz_split"][:b]
+            ops.split_rows(dz, out=dz_split)
+        ops.dense_tc(dz_split, N, wide["wT_split"], K, None, None, out_f32=dx)
+        if mask is not None:
+            ops.relu_mask(dx, mask)
+
+    def _table_args(self, t: int, indices: torch.Tensor, grad_rows: torch.Tensor) -> dict:
+        tb = self.tables[t]
+        mirror = tb._mirror if (tb._mirror is not None and tb._mirror.shape[0] == tb.table.shape[0]) else None
+        return dict(weights=tb.table, indices=indices, grad_rows=grad_rows, rep_map=self.rep[t], state1=self.tstate1[t],
+                    state2=self.tstate2[t], mirror=mirror, dense_grad=self.tdense[t])
+
+    def _refresh_operands(self) -> None:
+        for l, ws in zip(self._tc_layers, self._wsplit):
+            ops.split_weights(l.kernel, out=ws)
+
+    def step(self, inputs: Dict[str, torch.Tensor], targets, sample_weight=None) -> torch.Tensor:
+        """One eager training step; returns [total loss, per-output losses...] as a (1 + H,) device tensor (valid until the
+        next step)."""
+        self.forward_backward(inputs, targets, sample_weight)
+        self.apply_gradients()
+        self._after_step()
+        return self.loss
+
+    def _after_step(self) -> None:
+        from .core import bump_weights_version
+
+        self.steps += 1
+        self.head._bias_host = None
+        bump_weights_version()  # forward graphs captured earlier hold scalars / operand copies of the old variables
+
+    # ---- CUDA-graph replay over static input buffers ------------------------------------------------------------
+    def capture(self, inputs: Dict[str, torch.Tensor], targets: torch.Tensor, clone: bool = True) -> None:
+        """Capture forward + backward + update into ONE CUDA graph over copies of `inputs` / `targets` (single GPU; with a
+        process group the collectives stay eager between two graphs).  clone=False: the given tensors ARE the static
+        buffers (e.g. views of one packed device buffer that a single H2D copy refreshes before replay())."""
+        if self.world > 1:
+            raise NotImplementedError("graph capture of the data-parallel step is not implemented")
+        for f in self.feats:
+            if isinstance(get_feature(inputs, f), tuple):
+                raise NotImplementedError(f"graph capture with the ragged feature {f!r} is not implemented: its number of ids "
+                                          "changes from batch to batch (train it eagerly, or feed it as a fixed-length (B, L) matrix)")
+        self._static = {k: (v.clone() if clone else v) for k, v in inputs.items()}
+        ys = list(targets) if isinstance(targets, (list, tuple)) else [targets]
+        self._static_y = [y.clone() if clone else y for y in ys]
+        self.model.defer_index_check(True)
+        try:
+            s = torch.cuda.Stream(device=self.device)
+            s.wait_stream(torch.cuda.current_stream())
+            # warm-up steps DO train: snapshot and restore every variable so that capture has no side effect
+            snap = self._snapshot()
+            with torch.cuda.stream(s):
+                for _ in range(2):
+                    self.forward_backward(self._static, self._static_y)
+                    self.apply_gradients()
+            torch.cuda.current_stream().wait_stream(s)
+            torch.cuda.synchronize()
+            self._graph = torch.cuda.CUDAGraph()
+            n0 = ops.launch_count()
+            with torch.cuda.graph(self._graph):
+                self.forward_backward(self._static, self._static_y)
+                self.apply_gradients()
+            self.launches_per_step = ops.launch_count() - n0
+            self._restore(snap)
+        finally:
+            self.model.defer_index_check(False)
+
+    def _snapshot(self):
+        return dict(w=self.arena.w.clone(), s1=None if self.arena.state1 is None else self.arena.state1.clone(),
+                    s2=None if self.arena.state2 is None else self.arena.state2.clone(), hyper=self.hyper.clone(),
+                    tables=[t.table.clone() for t in self.tables],
+                    ts1=[None if s is None else s.clone() for s in self.tstate1], ts2=[None if s is None else s.clone() for s in self.tstate2])
+
+    def _restore(self, snap) -> None:
+        self.arena.w.copy_(snap["w"])
+        self.arena.grad.zero_()
+        if snap["s1"] is not None:
+            self.arena.state1.copy_(snap["s1"])
+        if snap["s2"] is not None:
+            self.arena.state2.copy_(snap["s2"])
+        self.hyper.copy_(snap["hyper"])
+        for t, w, s1, s2, a1, a2 in zip(self.tables, snap["tables"], snap["ts1"], snap["ts2"], self.tstate1, self.tstate2):
+            t.table.copy_(w)
+            if s1 is not None:
+                a1.copy_(s1)
+            if s2 is not None:
+                a2.copy_(s2)
+            if t._mirror is not None and t._mirror.shape[0] == t.table.shape[0]:
+                ops.split_rows(t.table, out=t._mirror)
+        self._refresh_operands()
+
+    def replay(self, inputs: Optional[Dict[str, torch.Tensor]] = None, targets: Optional[torch.Tensor] = None) -> torch.Tensor:
+        if self._graph is None:
+            raise RuntimeError("capture() first")
+        if inputs is not None:
+            for k, v in self._static.items():
+                v.copy_(inputs[k], non_blocking=True)
+        if targets is not None:
+            ys = list(targets) if isinstance(targets, (list, tuple)) else [targets]
+            for s, y in zip(self._static_y, ys):
+                s.copy_(y.reshape(s.shape), non_blocking=True)
+        self._graph.replay()
+        self._after_step()
+        return self.loss
+
+    def check_indices(self) -> None:
+        """Raise IndexError if any batch since the last check carried an id outside its table (the forward read a zero
+        row for it and its gradient was dropped).  One device-to-host read: `fit` calls it once per epoch, not per step."""
+        if self.oob is None:
+            return
+        n = int(self.oob.item())
+        if n:
+            self.oob.zero_()
+            raise IndexError(f"{n} indices out of range for the embedding tables "
+                             "(TF raises InvalidArgumentError: indices[...] is not in [0, rows))")
+
+    def set_learning_rate(self, lr: float) -> None:
+        self.opt.learning_rate = float(lr)
+        self.hyper[_cabi.HYPER_LR] = float(lr)
+
+    def gradients(self) -> Dict[str, torch.Tensor]:
+        """Dense gradients by variable name (after forward_backward, before apply_gradients) — for parity tests."""
+        out = {}
+        for i, l in enumerate(self.arena.layers):
+            out[f"{l.name}/kernel"] = self.arena.view(self.arena.grad, i, "kernel")
+            b = self.arena.view(self.arena.grad, i, "bias")
+            if b is not None:
+                out[f"{l.name}/bias"] = b
+        return out
+
+
+class DLRMTrainer(_StepTrainer):
     """Static-buffer training step of a DLRM RankingModel at one batch size."""
 
     def __init__(self, model, optimizer: Optimizer, batch_size: int, device=None, group=None):
@@ -202,47 +429,25 @@ class DLRMTrainer:
             raise NotImplementedError("training with row-sharded tables is not implemented (forward only)")
         if not body.can_emit_split():
             raise NotImplementedError("training needs <= 32 interaction features and embedding_dim in {16, 32, 64, 128}")
-        self.model, self.body, self.opt = model, body, optimizer
-        self.device = torch.device(device) if device is not None else default_device()
-        self.B = int(batch_size)
-        self.group = group
-        self.world = 1
-        if group is not None:
-            import torch.distributed as dist
-
-            self.world = dist.get_world_size(group)
-        if not model.built:
-            model.build(self.device)
+        self._init_common(model, optimizer, batch_size, device, group)
         for blk in (body.bottom_block, body.top_block):
             if not isinstance(blk, MLP) or blk.has_normalization or blk.dropout:
                 raise NotImplementedError("training supports MLPBlock towers without normalization / dropout")
         self.bottom = body.bottom_block.dense_layers
         self.top = body.top_block.dense_layers
-        self.head = model.prediction.to_call
-        self.outputs = model.output_blocks()
-        self.H = len(self.outputs)
-        self.losses = [o.loss for o in self.outputs]
-        self.loss_weights = list(getattr(model, "loss_weights", None) or [1.0] * self.H)
+        self._init_heads()
         for l in self.bottom + self.top:
             if l.activation not in ("relu", "linear"):
                 raise NotImplementedError(f"{l.name}: training supports relu / linear tower activations, got {l.activation!r}")
         if self.head.input_dim > 256:
             raise NotImplementedError("the output layer's input must be <= 256 wide")
         self.arena = DenseArena(self.bottom + self.top + [self.head], optimizer, self.device)
-        nb, nt = len(self.bottom), len(self.top)
-        self._wsplit = [ops.split_weights(l.kernel) for l in self.bottom + self.top]
-        for l, ws in zip(self.bottom + self.top, self._wsplit):
+        self._tc_layers = self.bottom + self.top
+        self._wsplit = [ops.split_weights(l.kernel) for l in self._tc_layers]
+        for l, ws in zip(self._tc_layers, self._wsplit):
             l._w_split = ws  # the forward path of this model keeps reading the refreshed operand copies
         self.hyper = torch.from_numpy(optimizer.hyper()).to(self.device)
-        # layers wider than mm_dense_dgrad's 128 units take dX = dZ W^T through the tensor-core forward GEMM on the transposed
-        # kernel: per such layer a transposed copy, its split operand and the split of dZ
-        self._wide: Dict[int, dict] = {}
-        for li, l in enumerate(self.bottom + self.top):
-            if l.units > 128 and li != 0:  # the first bottom layer needs no input gradient
-                K, N = l.kernel.shape
-                wT = torch.empty((N, K), dtype=torch.float32, device=self.device)
-                self._wide[li] = dict(wT=wT, wT_split=torch.zeros((ops.tc_padded_n(K), 2 * ops.tc_padded_k(N)), dtype=torch.bfloat16, device=self.device),
-                                      dz_split=torch.zeros((self.B, 2 * ops.tc_padded_k(N)), dtype=torch.bfloat16, device=self.device))
+        self._init_wide(lambda li: li != 0)  # the first bottom layer needs no input gradient
 
         # ---- tables
         emb = body.embeddings
@@ -259,11 +464,7 @@ class DLRMTrainer:
                 raise NotImplementedError("frozen embedding tables are not implemented in the training step")
         T, B, D = len(self.tables), self.B, self.D
         self.slices = torch.zeros((T, B, D), dtype=torch.float32, device=self.device)
-        self.rep = [ops.fill_i32(torch.empty(t.table.shape[0], dtype=torch.int32, device=self.device), INT32_MAX) for t in self.tables]
-        self.tstate1 = [torch.full_like(t.table, optimizer.initial_accumulator_value) if optimizer.slots >= 1 else None for t in self.tables]
-        self.tstate2 = [torch.zeros_like(t.table) if optimizer.slots >= 2 else None for t in self.tables]
-        # tables with few rows (every id repeats many times per batch) sum their slices into a dense accumulator
-        self.tdense = [torch.zeros_like(t.table) if t.table.shape[0] <= DENSE_PATH_MAX_ROWS else None for t in self.tables]
+        self._init_table_state(optimizer)
 
         # ---- activations and gradients
         # operand-format rows for the lookup + interaction kernels (forward and backward) (D = 64, mirrors enabled): the tables' mirrors (the
@@ -290,20 +491,13 @@ class DLRMTrainer:
         self.t_split = [torch.zeros((B, 2 * ops.tc_padded_k(l.units)), dtype=torch.bfloat16, device=self.device) for l in self.top[:-1]]
         self.dt = [torch.zeros((B, l.units), **f32) for l in self.top]
         self.dh = [torch.zeros((B, l.units), **f32) for l in self.bottom]
-        self.logits = torch.zeros((self.H, B) if self.H > 1 else B, **f32)  # z of each output; (B,) for one
-        # [total, loss_0 .. loss_{H-1}]; `loss` is the (1,) total alone for one output, the whole vector for several
-        self._loss_all = torch.zeros(1 + self.H, **f32)
-        self.loss = self._loss_all if self.H > 1 else self._loss_all[:1]
+        self._init_loss(B)
         self.oob = emb.counter(self.device)
         # multi-hot features (ragged bags, (B, L) id matrices), by table position: pooled rows, their operand copy, the
         # expanded row gradients; created on the first batch that carries the feature as a bag (see _indices)
         self._bag_bufs: Dict[int, dict] = {}
         self._iota: Optional[torch.Tensor] = None
         self._bags: Dict[int, dict] = {}
-        self.steps = 0
-        self._graph = None
-        self._static: Optional[Dict[str, torch.Tensor]] = None
-        self._static_y: Optional[List[torch.Tensor]] = None
 
     # ---- one step on device tensors ------------------------------------------------------------------------------
     def _indices(self, inputs, b: Optional[int] = None) -> List[torch.Tensor]:
@@ -384,14 +578,7 @@ class DLRMTrainer:
         cont = self.body.continuous(inputs)
         pieces = [cont[k] for k in sorted(cont)]
         b = int(pieces[0].shape[0])
-        if b > self.B or b < 1:
-            raise ValueError(f"this trainer was compiled for batches of up to {self.B} samples, got {b}")
-        targets = list(targets) if isinstance(targets, (list, tuple)) else [targets]
-        if len(targets) != self.H:
-            raise ValueError(f"{self.H} target tensors expected (one per output), got {len(targets)}")
-        for o, t in zip(self.outputs, targets):
-            if t.numel() != b:
-                raise ValueError(f"targets of {o.name!r} must hold {b} values, got {tuple(t.shape)}")
+        targets = self._check_targets(targets, b)
 
         def v(t):
             return t[:b]
@@ -428,11 +615,7 @@ class DLRMTrainer:
             ops.dense_tc(op, K, self._wsplit[nb + i], l.units, l.bias, l.activation, out_f32=t_[i], out_split=nxt)
             op, K = nxt, l.units
         # -- output layer + loss, forward and backward
-        hi = nb + nt
-        ops.heads_fwd_bwd(t_[-1], self.head.kernel, self.head.bias, self.losses, [t.reshape(-1) for t in targets],
-                          self.logits.view(-1)[:self.H * b].view(self.H, b),
-                          self._loss_all, dt[-1], a.view(a.grad, hi, "kernel"), a.view(a.grad, hi, "bias"), loss_weights=self.loss_weights,
-                          mask_relu=self.top[-1].activation == "relu", sample_weight=sample_weight)
+        self._heads(t_[-1], targets, dt[-1], self.top[-1].activation == "relu", sample_weight, b)
         # -- top tower backward
         for i in range(nt - 1, -1, -1):
             l = self.top[i]
@@ -464,21 +647,6 @@ class DLRMTrainer:
                 self._dgrad(i, l, dh[i], dh[i - 1], h[i - 1] if self.bottom[i - 1].activation == "relu" else None)
         self._idx, self._b = idx, b
 
-    def _dgrad(self, li: int, layer: _Dense, dz: torch.Tensor, dx: torch.Tensor, mask: Optional[torch.Tensor]) -> None:
-        """dx = dz W^T (zeroed where mask <= 0) for layer `li` of bottom + top."""
-        wide = self._wide.get(li)
-        if wide is None:
-            ops.dense_dgrad(dz, layer.kernel, dx, mask=mask)
-            return
-        K, N = layer.kernel.shape
-        b = dz.shape[0]
-        wide["wT"].copy_(layer.kernel.t())
-        ops.split_weights(wide["wT"], out=wide["wT_split"])
-        ops.split_rows(dz, out=wide["dz_split"][:b])
-        ops.dense_tc(wide["dz_split"][:b], N, wide["wT_split"], K, None, None, out_f32=dx)
-        if mask is not None:
-            ops.relu_mask(dx, mask)
-
     def apply_gradients(self) -> None:
         a = self.arena
         ops.opt_tick(self.hyper)
@@ -497,10 +665,8 @@ class DLRMTrainer:
             Bt = self._b * self.world
         ops.dense_apply(self.opt.kind, a.w, a.grad, a.state1, a.state2, self.hyper, grad_scale=scale)
         tabs = []
-        for t, tb in enumerate(self.tables):
-            mirror = tb._mirror if (tb._mirror is not None and tb._mirror.shape[0] == tb.table.shape[0]) else None
-            tab = dict(weights=tb.table, indices=idx[t], grad_rows=slices[t], rep_map=self.rep[t], state1=self.tstate1[t],
-                       state2=self.tstate2[t], mirror=mirror, dense_grad=self.tdense[t])
+        for t in range(len(self.tables)):
+            tab = self._table_args(t, idx[t], slices[t])
             bag = self._bags.get(t)
             if bag is None:
                 tabs.append(tab)
@@ -509,120 +675,254 @@ class DLRMTrainer:
                 ops.sparse_rows_apply(self.opt.kind, [tab], bag["rows"].shape[0], self.D, self.hyper)
         if tabs:
             ops.sparse_rows_apply(self.opt.kind, tabs, Bt, self.D, self.hyper)
-        for l, ws in zip(self.bottom + self.top, self._wsplit):
-            ops.split_weights(l.kernel, out=ws)
+        self._refresh_operands()
 
-    def step(self, inputs: Dict[str, torch.Tensor], targets, sample_weight=None) -> torch.Tensor:
-        """One eager training step; returns [total loss, per-output losses...] as a (1 + H,) device tensor (valid until the
-        next step)."""
-        self.forward_backward(inputs, targets, sample_weight)
-        self.apply_gradients()
-        self._after_step()
-        return self.loss
 
-    def _after_step(self) -> None:
-        from .core import bump_weights_version
+class DCNTrainer(_StepTrainer):
+    """Static-buffer training step of a DCN-v2 RankingModel (DCNModel, stacked or parallel body) at one batch size.
 
-        self.steps += 1
-        self.head._bias_host = None
-        bump_weights_version()  # forward graphs captured earlier hold scalars / operand copies of the old variables
+    forward   gather of every table's rows + the continuous columns into x0 (B, d) at their sorted-name offsets, its split
+              operand; per cross layer mm_dense_tc (z_l = x_l W_l + b_l, fp32 saved) -> mm_cross_combine
+              (x_{l+1} = x0 z_l + x_l) -> mm_split_rows (the next operand); the deep tower as in DLRM's towers
+    loss      mm_heads_fwd_bwd on the deep output (stacked) or on [cross | deep] in DCNBody.branch_order() (parallel)
+    backward  deep tower as DLRM's towers; per cross layer (top down) mm_cross_backward (g += p, dz = g x0 fp32 + split,
+              acc += g z_l), mm_dense_wgrad_split on x_l's saved operand, p = dz W_l^T (transposed-kernel mm_dense_tc for
+              d > 128); mm_concat_backward sums g + p + acc (+ the deep branch's input gradient) = dx0 into each table's
+              (B, D_t) IndexedSlices buffer
+    update    mm_opt_tick, mm_dense_apply over the arena [cross layers, deep layers, head], one mm_sparse_rows_apply per
+              distinct embedding width, mm_split_weights refresh of the operand copies the model's forward reads."""
 
-    # ---- CUDA-graph replay over static input buffers ------------------------------------------------------------
-    def capture(self, inputs: Dict[str, torch.Tensor], targets: torch.Tensor, clone: bool = True) -> None:
-        """Capture forward + backward + update into ONE CUDA graph over copies of `inputs` / `targets` (single GPU; with a
-        process group the collectives stay eager between two graphs).  clone=False: the given tensors ARE the static
-        buffers (e.g. views of one packed device buffer that a single H2D copy refreshes before replay())."""
-        if self.world > 1:
-            raise NotImplementedError("graph capture of the data-parallel step is not implemented")
-        for f in self.feats:
-            if isinstance(get_feature(inputs, f), tuple):
-                raise NotImplementedError(f"graph capture with the ragged feature {f!r} is not implemented: its number of ids "
-                                          "changes from batch to batch (train it eagerly, or feed it as a fixed-length (B, L) matrix)")
-        self._static = {k: (v.clone() if clone else v) for k, v in inputs.items()}
-        ys = list(targets) if isinstance(targets, (list, tuple)) else [targets]
-        self._static_y = [y.clone() if clone else y for y in ys]
-        self.model.defer_index_check(True)
-        try:
-            s = torch.cuda.Stream(device=self.device)
-            s.wait_stream(torch.cuda.current_stream())
-            # warm-up steps DO train: snapshot and restore every variable so that capture has no side effect
-            snap = self._snapshot()
-            with torch.cuda.stream(s):
-                for _ in range(2):
-                    self.forward_backward(self._static, self._static_y)
-                    self.apply_gradients()
-            torch.cuda.current_stream().wait_stream(s)
-            torch.cuda.synchronize()
-            self._graph = torch.cuda.CUDAGraph()
-            n0 = ops.launch_count()
-            with torch.cuda.graph(self._graph):
-                self.forward_backward(self._static, self._static_y)
-                self.apply_gradients()
-            self.launches_per_step = ops.launch_count() - n0
-            self._restore(snap)
-        finally:
-            self.model.defer_index_check(False)
+    def __init__(self, model, optimizer: Optimizer, batch_size: int, device=None, group=None):
+        from .blocks import Cross
+        from .models import BinaryOutput, DCNBody, ParallelOutputs
 
-    def _snapshot(self):
-        return dict(w=self.arena.w.clone(), s1=None if self.arena.state1 is None else self.arena.state1.clone(),
-                    s2=None if self.arena.state2 is None else self.arena.state2.clone(), hyper=self.hyper.clone(),
-                    tables=[t.table.clone() for t in self.tables],
-                    ts1=[None if s is None else s.clone() for s in self.tstate1], ts2=[None if s is None else s.clone() for s in self.tstate2])
+        body = model.body
+        if not isinstance(body, DCNBody):
+            raise NotImplementedError("DCNTrainer trains DCNModel bodies")
+        if not isinstance(model.prediction, (BinaryOutput, ParallelOutputs)):
+            raise NotImplementedError("train_step needs BinaryOutput / RegressionOutput heads or an OutputBlock of them")
+        if group is not None:
+            raise NotImplementedError("training DCNModel with a process group is not implemented")
+        cross_layers = body.cross.cross_layers
+        for c in cross_layers:
+            if not isinstance(c, Cross) or c.low_rank_dim is not None:
+                raise NotImplementedError(f"{c.name}: training a low-rank cross layer (low_rank_dim) is not implemented")
+        if body.cross.inputs is not None:
+            raise NotImplementedError("training a CrossBlock with its own `inputs` block is not implemented")
+        deep = body.deep
+        if not isinstance(deep, MLP) or deep.has_normalization or deep.dropout:
+            raise NotImplementedError("training DCNModel supports a deep_block without normalization / dropout")
+        ib = body.input_block
+        if getattr(ib, "aggregation", "concat") != "concat":
+            raise NotImplementedError("training DCNModel needs the concatenating input block")
+        self._init_common(model, optimizer, batch_size, device, None)
+        self.stacked = bool(body.stacked)
+        self.cross = [c.dense for c in cross_layers]
+        self.deep = deep.dense_layers
+        self._init_heads()
+        for l in self.deep:
+            if l.activation not in ("relu", "linear"):
+                raise NotImplementedError(f"{l.name}: training supports relu / linear deep-layer activations, got {l.activation!r}")
 
-    def _restore(self, snap) -> None:
-        self.arena.w.copy_(snap["w"])
-        self.arena.grad.zero_()
-        if snap["s1"] is not None:
-            self.arena.state1.copy_(snap["s1"])
-        if snap["s2"] is not None:
-            self.arena.state2.copy_(snap["s2"])
-        self.hyper.copy_(snap["hyper"])
-        for t, w, s1, s2, a1, a2 in zip(self.tables, snap["tables"], snap["ts1"], snap["ts2"], self.tstate1, self.tstate2):
-            t.table.copy_(w)
-            if s1 is not None:
-                a1.copy_(s1)
-            if s2 is not None:
-                a2.copy_(s2)
-            if t._mirror is not None and t._mirror.shape[0] == t.table.shape[0]:
-                ops.split_rows(t.table, out=t._mirror)
-        for l, ws in zip(self.bottom + self.top, self._wsplit):
-            ops.split_weights(l.kernel, out=ws)
+        # ---- input block layout and tables
+        emb = ib.embeddings
+        self.cols, widths, d = ib.layout()
+        self.d = d
+        self.feats = list(emb.feature_names) if emb is not None else []
+        self.tables = [emb.feature_to_table[f] for f in self.feats]
+        seen = set()
+        for f, t in zip(self.feats, self.tables):
+            if id(t) in seen:
+                raise NotImplementedError(f"feature {f!r}: training with a table shared between features is not implemented")
+            seen.add(id(t))
+            if not t.trainable:
+                raise NotImplementedError(f"feature {f!r}: frozen embedding tables are not implemented in the training step")
+            D = t.table.shape[1]
+            if D % 4 or D > 128:
+                raise NotImplementedError(f"table {t.table_name!r}: embedding width {D} is not supported by the sparse update "
+                                          "(it needs a multiple of 4 no larger than 128)")
+        self.cont = sorted(ib.continuous.features) if ib.continuous is not None else []
 
-    def replay(self, inputs: Optional[Dict[str, torch.Tensor]] = None, targets: Optional[torch.Tensor] = None) -> torch.Tensor:
-        if self._graph is None:
-            raise RuntimeError("capture() first")
-        if inputs is not None:
-            for k, v in self._static.items():
-                v.copy_(inputs[k], non_blocking=True)
-        if targets is not None:
-            ys = list(targets) if isinstance(targets, (list, tuple)) else [targets]
-            for s, y in zip(self._static_y, ys):
-                s.copy_(y.reshape(s.shape), non_blocking=True)
-        self._graph.replay()
-        self._after_step()
-        return self.loss
+        self.arena = DenseArena(self.cross + self.deep + [self.head], optimizer, self.device)
+        self._tc_layers = self.cross + self.deep
+        self._wsplit = [ops.split_weights(l.kernel) for l in self._tc_layers]
+        for l, ws in zip(self._tc_layers, self._wsplit):
+            l._w_split = ws  # the model's forward keeps reading the refreshed operand copies
+        self.hyper = torch.from_numpy(optimizer.hyper()).to(self.device)
+        # every layer needs its input gradient (x0 is the tables' rows); mm_cross_backward writes the split of a cross
+        # layer's dz itself
+        L = len(self.cross)
+        self._init_wide(lambda li: True, dz_split_given=lambda li: li < L)
+        self._init_table_state(optimizer)
+        self._by_width: Dict[int, List[int]] = {}
+        for t, tb in enumerate(self.tables):
+            self._by_width.setdefault(tb.table.shape[1], []).append(t)
 
-    def check_indices(self) -> None:
-        """Raise IndexError if any batch since the last check carried an id outside its table (the forward read a zero
-        row for it and its gradient was dropped).  One device-to-host read: `fit` calls it once per epoch, not per step."""
-        if self.oob is None:
+        # ---- activations and gradients (fp32 (B, d) buffers with a row stride that is a multiple of 4)
+        B = self.B
+        self.ld = (d + 3) // 4 * 4
+        f32 = dict(dtype=torch.float32, device=self.device)
+        bf = dict(dtype=torch.bfloat16, device=self.device)
+        Kp = ops.tc_padded_k(d)
+
+        def mat():
+            return torch.zeros((B, self.ld), **f32)
+
+        self.x0 = mat()
+        self.xs = [torch.zeros((B, 2 * Kp), **bf) for _ in range(L + (1 if self.stacked else 0))]  # operands of x_0 .. x_L
+        self.z = [mat() for _ in range(L)]
+        self.xf = [mat() for _ in range(min(L, 2))]  # fp32 x_1 .. x_L, alternating (only the residual of the next layer)
+        self.h = [torch.zeros((B, l.units), **f32) for l in self.deep]
+        self.h_split = [torch.zeros((B, 2 * ops.tc_padded_k(l.units)), **bf) for l in self.deep[:-1]]
+        self.dh = [torch.zeros((B, l.units), **f32) for l in self.deep]
+        self.g, self.p, self.acc, self.dz = mat(), mat(), mat(), mat()
+        self.dz_split = torch.zeros((B, 2 * Kp), **bf)
+        self.slices = [torch.zeros((B, tb.table.shape[1]), **f32) for tb in self.tables]
+        if not self.stacked:
+            # the head reads [cross | deep] (or [deep | cross]): x_L and the deep output are written straight into it
+            u = self.deep[-1].units
+            self.order = body.branch_order()
+            self.coff, self.doff = (0, d) if self.order == ("cross", "deep") else (u, 0)
+            self.cat = torch.zeros((B, d + u), **f32)
+            self.dcat = torch.zeros((B, d + u), **f32)
+            self.ddeep = mat()  # input gradient of the deep branch (an addend of dx0)
+        # mm_heads_fwd_bwd reads at most 256 inputs per row.  A wider head input (a parallel body's [cross | deep] at
+        # realistic d, or a wide last deep layer) takes its logits from the tensor-core GEMM; the loss kernel then runs on
+        # those logits with an identity kernel (dz out, db accumulated), and dW / dX come from mm_dense_wgrad_split /
+        # mm_dense_dgrad on dz.
+        self.wide_head = self.head.input_dim > 256
+        if self.wide_head:
+            Kh = self.head.input_dim
+            self._head_x_split = torch.zeros((B, 2 * ops.tc_padded_k(Kh)), **bf)
+            self._head_w_split = torch.zeros((ops.tc_padded_n(self.H), 2 * ops.tc_padded_k(Kh)), **bf)
+            self._head_z = torch.zeros((B, self.H), **f32)
+            self._head_dz = torch.zeros((B, self.H), **f32)
+            self._head_eye = torch.eye(self.H, **f32)
+        self._init_loss(B)
+        self.oob = emb.counter(self.device) if emb is not None else None
+
+    def _ids(self, inputs) -> List[torch.Tensor]:
+        idx = []
+        for f, tb in zip(self.feats, self.tables):
+            x = get_feature(inputs, f)
+            if tb.lookup_kind(x) != "onehot":
+                raise NotImplementedError(f"feature {f!r}: training DCNModel on multi-hot / ragged features is not implemented")
+            idx.append(ops.as_index(x).reshape(-1))
+        if len({i.dtype for i in idx}) > 1:
+            idx = [i.to(torch.int64) for i in idx]
+        return idx
+
+    def forward_backward(self, inputs: Dict[str, torch.Tensor], targets, sample_weight=None) -> None:
+        """Forward (activations saved), loss and backward: fills the gradient arena and the IndexedSlices.  Batches smaller
+        than the compiled size run in the leading rows of the same buffers."""
+        a = self.arena
+        d, L, nd = self.d, len(self.cross), len(self.deep)
+        self._loss_all.zero_()
+        b = batch_size_of(inputs)
+        targets = self._check_targets(targets, b)
+        idx = self._ids(inputs)
+
+        def v(t):
+            return t[:b]
+
+        def vd(t):
+            return t[:b, :d]
+
+        # -- input block: x0 = [embeddings | continuous] in sorted-name order
+        x0 = vd(self.x0)
+        if self.tables:
+            ops.gather_multi([tb.table for tb in self.tables], idx, [self.cols[f] for f in self.feats], x0, self.oob)
+        if self.cont:
+            ops.concat_columns([inputs[n] for n in self.cont], x0, [self.cols[n] for n in self.cont])
+        ops.split_rows(x0, out=v(self.xs[0]))
+        # -- cross network
+        x = x0
+        cat = v(self.cat) if not self.stacked else None
+        for l, layer in enumerate(self.cross):
+            ops.dense_tc(v(self.xs[l]), d, self._wsplit[l], d, layer.bias, "linear", out_f32=vd(self.z[l]))
+            last = l == L - 1
+            out = cat[:, self.coff:self.coff + d] if (last and cat is not None) else vd(self.xf[l % len(self.xf)])
+            ops.cross_combine(x0, vd(self.z[l]), x, out)
+            if l + 1 < len(self.xs):
+                ops.split_rows(out, out=v(self.xs[l + 1]))
+            x = out
+        # -- deep tower on x_L (stacked) or x0 (parallel)
+        op0 = v(self.xs[L] if self.stacked else self.xs[0])
+        h, dh = [v(t) for t in self.h], [v(t) for t in self.dh]
+        if cat is not None:
+            h[-1] = cat[:, self.doff:self.doff + self.deep[-1].units]
+        op, K = op0, d
+        for i, l in enumerate(self.deep):
+            nxt = v(self.h_split[i]) if i < nd - 1 else None
+            ops.dense_tc(op, K, self._wsplit[L + i], l.units, l.bias, l.activation, out_f32=h[i], out_split=nxt)
+            op, K = nxt, l.units
+        # -- output layer + loss, forward and backward
+        relu_last = self.deep[-1].activation == "relu"
+        g = vd(self.g)
+        if cat is None:
+            self._dcn_heads(h[-1], targets, dh[-1], relu_last, sample_weight, b)
+        else:
+            dcat = v(self.dcat)
+            self._dcn_heads(cat, targets, dcat, False, sample_weight, b)
+            dh[-1] = dcat[:, self.doff:self.doff + self.deep[-1].units]
+            if relu_last:
+                ops.relu_mask(dh[-1], h[-1])
+            ops.concat_columns([dcat[:, self.coff:self.coff + d]], g, [0])  # the cross branch's output gradient
+        # -- deep tower backward
+        for i in range(nd - 1, -1, -1):
+            l = self.deep[i]
+            if i > 0:
+                ops.dense_wgrad(h[i - 1], dh[i], a.view(a.grad, L + i, "kernel"), a.view(a.grad, L + i, "bias"))
+                self._dgrad(L + i, l, dh[i], dh[i - 1], h[i - 1] if self.deep[i - 1].activation == "relu" else None)
+            else:
+                ops.dense_wgrad_split(op0, d, dh[0], a.view(a.grad, L, "kernel"), a.view(a.grad, L, "bias"))
+                self._dgrad(L, l, dh[0], g if self.stacked else vd(self.ddeep), None)
+        # -- cross network backward (g: gradient into x_{l+1}; p: dgrad of the layer above)
+        p, acc, dz, dzs = vd(self.p), vd(self.acc), vd(self.dz), v(self.dz_split)
+        for l in range(L - 1, -1, -1):
+            ops.cross_backward(x0, vd(self.z[l]), g, p if l < L - 1 else None, acc, l == L - 1, dz, dzs)
+            ops.dense_wgrad_split(v(self.xs[l]), d, dz, a.view(a.grad, l, "kernel"), a.view(a.grad, l, "bias"))
+            self._dgrad(l, self.cross[l], dz, p, None, dz_split=dzs)
+        # -- input block backward: dx0 = g_1 + p_0 + acc (+ the deep branch's input gradient), the tables' columns only
+        self._slices = [v(s) for s in self.slices]
+        addends = [g, p, acc] + ([vd(self.ddeep)] if not self.stacked else [])
+        slices = [(s, self.cols[f]) for s, f in zip(self._slices, self.feats)]
+        for s in range(0, len(slices), CONCAT_MAX_SLICES):
+            ops.concat_backward(addends, slices[s:s + CONCAT_MAX_SLICES])
+        self._idx, self._b = idx, b
+
+    def _dcn_heads(self, x: torch.Tensor, targets, dx: torch.Tensor, mask_relu: bool, sample_weight, b: int) -> None:
+        """The output heads on x (b, K): the fused loss kernel for K <= 256, otherwise the wide-head composition."""
+        if not self.wide_head:
+            self._heads(x, targets, dx, mask_relu, sample_weight, b)
             return
-        n = int(self.oob.item())
-        if n:
-            self.oob.zero_()
-            raise IndexError(f"{n} indices out of range for the embedding tables "
-                             "(TF raises InvalidArgumentError: indices[...] is not in [0, rows))")
+        a, hi, K = self.arena, len(self.arena.layers) - 1, x.shape[1]
+        xs, z, dz = self._head_x_split[:b], self._head_z[:b], self._head_dz[:b]
+        ops.split_rows(x, out=xs)
+        ops.split_weights(self.head.kernel, out=self._head_w_split)
+        ops.dense_tc(xs, K, self._head_w_split, self.H, None, "linear", out_f32=z)  # x W: the logits without the bias
+        ops.heads_fwd_bwd(z, self._head_eye, self.head.bias, self.losses, [t.reshape(-1) for t in targets],
+                          self.logits.view(-1)[:self.H * b].view(self.H, b), self._loss_all, dz, None,
+                          a.view(a.grad, hi, "bias"), loss_weights=self.loss_weights, mask_relu=False, sample_weight=sample_weight)
+        ops.dense_wgrad_split(xs, K, dz, a.view(a.grad, hi, "kernel"), None)
+        ops.dense_dgrad(dz, self.head.kernel, dx, mask=x if mask_relu else None)
 
-    def set_learning_rate(self, lr: float) -> None:
-        self.opt.learning_rate = float(lr)
-        self.hyper[_cabi.HYPER_LR] = float(lr)
+    def apply_gradients(self) -> None:
+        a = self.arena
+        ops.opt_tick(self.hyper)
+        ops.dense_apply(self.opt.kind, a.w, a.grad, a.state1, a.state2, self.hyper)
+        for D, ts in self._by_width.items():
+            for s in range(0, len(ts), SPARSE_MAX_TABLES):
+                chunk = ts[s:s + SPARSE_MAX_TABLES]
+                ops.sparse_rows_apply(self.opt.kind, [self._table_args(t, self._idx[t], self._slices[t]) for t in chunk], self._b, D,
+                                      self.hyper)
+        self._refresh_operands()
 
-    def gradients(self) -> Dict[str, torch.Tensor]:
-        """Dense gradients by variable name (after forward_backward, before apply_gradients) — for parity tests."""
-        out = {}
-        for i, l in enumerate(self.arena.layers):
-            out[f"{l.name}/kernel"] = self.arena.view(self.arena.grad, i, "kernel")
-            b = self.arena.view(self.arena.grad, i, "bias")
-            if b is not None:
-                out[f"{l.name}/bias"] = b
-        return out
+
+def trainer_for(model, optimizer: Optimizer, batch_size: int, group=None):
+    """The training engine of `model`'s body: DLRMTrainer or DCNTrainer."""
+    from .models import DCNBody
+
+    if isinstance(getattr(model, "body", None), DCNBody):
+        return DCNTrainer(model, optimizer, batch_size, group=group)
+    return DLRMTrainer(model, optimizer, batch_size, group=group)
