@@ -1,17 +1,21 @@
 // Narrow-input two-layer tower in one launch:  h = act2(act1(concat(columns) W1 + b1) W2 + b2)
 //
 // The DLRM bottom tower (13 continuous columns -> 128 -> 64) is 1.3 GFLOP and 20 MB of traffic per 65 536-sample
-// batch — far too small for the TMA/wgmma tower kernel, whose per-tile latency chain (plus the separate
-// concat+split launch in front of it) cost 34 us of a 147 us step.  Here one warp owns 16 samples:
+// batch — far too small for the TMA/wgmma tower kernel, whose per-tile latency chain (plus a separate concat+split
+// launch in front of it) would dominate at these widths.  Here one warp owns 16 samples:
 //   * the <= 16 input columns are read straight from their column arrays (ContinuousFeatures + ConcatFeatures:
 //     sorted-name order, cast to fp32; merlin/models/tf/inputs/continuous.py:117-138, core/aggregation.py:54-66)
-//     into the m16k16 A fragment — no concatenated matrix, no bf16 operand in HBM;
+//     into the m16k16 A fragment — no concatenated matrix, no bf16 operand in HBM.  Each lane cp.asyncs its 8 values
+//     of the warp's NEXT tile into a per-warp stage before the MMAs of the current one (the first tile's values are
+//     in flight during the weight fill); all-fp32 inputs take an instantiation without any dtype handling;
 //   * layer 1 and layer 2 run on mma.sync.m16n8k16 with the same 3-pass bf16 split as every other dense layer
 //     (hi*lo + lo*hi + hi*hi, fp32 accumulate); the layer-1 accumulator fragment IS the layer-2 A fragment
 //     (row/column ownership coincides), so the hidden activations never leave registers;
 //   * both weight matrices sit in shared memory (pre-split K-major rows, padded against bank conflicts) and are
 //     fetched as B fragments by ldmatrix.x4 (hi and lo of one n-tile per instruction);
-//   * the last epilogue writes fp32 rows and/or split-bf16 rows [hi | lo] (the interaction kernel's operand format).
+//   * the last epilogue stages the tile's fp32 rows and/or split-bf16 rows [hi | lo] (the interaction kernel's
+//     operand format) in a per-warp shared-memory area and writes them out with 16-byte stores, so every store
+//     instruction covers whole 32-byte sectors.
 // Replaces MLPBlock([N1, N2]) over a dict of <= 16 scalar features (blocks/mlp.py:97-139, :275-280).
 #include <cuda_bf16.h>
 
@@ -24,7 +28,7 @@ namespace mm {
 namespace tsm {
 
 constexpr int MAX_COLS = 16;
-constexpr int WARPS = 16;  // 512 threads x <= 128 registers: the hidden layer is processed in halves to fit
+constexpr int WARPS = 16;  // 512 threads x <= 128 registers: the hidden layer is processed in chunks to fit
 
 struct Cols {  // one entry per input COLUMN (a width-w piece contributes w entries)
   const void* src[MAX_COLS];
@@ -45,9 +49,38 @@ struct Params {
   float* out_f32;
   long long out_stride;
   __nv_bfloat16* out_split;  // (B, 2*N2) [hi | lo]
+  int out_f32_v16;           // out_f32 rows can be written with 16-byte stores (else 8-byte)
+  int out_split_v16;         // out_split is 16-byte aligned (else 4-byte stores)
+};
+
+struct ColS {  // one input column as the kernel reads it, in shared memory
+  const uint8_t* base;  // row 0
+  long long pitch;      // bytes between consecutive rows
+  int dtype;
+  int pad;
 };
 
 constexpr int W1_STRIDE = 80;  // bytes per n-row of W1 in shared memory: [hi k0..15 | lo k0..15] = 64 B + 16 B pad
+
+// Shared memory of one CTA (byte offsets)
+template <int N1T, int N2T, bool F32>
+struct Layout {
+  static constexpr int N1 = 8 * N1T, N2 = 8 * N2T;
+  static constexpr int W2_STRIDE = N1 * 4 + 16;  // [hi k0..N1 | lo k0..N1] + pad
+  static constexpr int SLOT = F32 ? 4 : 8;        // bytes per staged input value (8: raw int64 / fp64 bits)
+  static constexpr int SPLIT_PITCH = 4 * N2 + 16;  // staged split row [hi | lo] + pad: rows g land 16 B apart in the banks
+  static constexpr int F32_PITCH = 4 * N2 + 32;    // staged fp32 row + pad: the float2 writes of 4 rows are conflict-free
+  static constexpr int W1 = 0;
+  static constexpr int W2 = W1 + N1 * W1_STRIDE;
+  static constexpr int B1 = W2 + N2 * W2_STRIDE;
+  static constexpr int B2 = B1 + 4 * N1;
+  static constexpr int COLS = B2 + 4 * N2;
+  static constexpr int XIN = COLS + MAX_COLS * (int)sizeof(ColS);
+  static constexpr int XIN_WARP = 2 * 8 * 32 * SLOT;  // two tiles x [value v][lane] slots
+  static constexpr int OUT = XIN + WARPS * XIN_WARP;
+  static constexpr int OUT_WARP = 16 * F32_PITCH;  // also holds 16 split rows (SPLIT_PITCH < F32_PITCH)
+  static constexpr int BYTES = OUT + WARPS * OUT_WARP;
+};
 
 // N1T / N2T: number of 8-column n-tiles of layer 1 / layer 2 (N1 = 8*N1T is also the K of layer 2, a multiple of 16)
 template <bool RELU>
@@ -55,91 +88,146 @@ __device__ __forceinline__ float act_fn(float v, int act) {
   return RELU ? fmaxf(v, 0.0f) : apply_act(v, act);
 }
 
-// RELU: both activations are relu (compile-time fast path: no per-element dispatch)
-template <int N1T, int N2T, bool RELU>
+// A staged input value (raw bits as copied; the high word only for 8-byte dtypes) -> fp32, as load_as_f32 converts it
+__device__ __forceinline__ float raw_to_f32(uint2 raw, int dt) {
+  const long long i64 = (long long)(((unsigned long long)raw.y << 32) | raw.x);
+  float f = __uint_as_float(raw.x);  // MM_F32
+  f = dt == MM_I32 ? (float)(int)raw.x : f;
+  f = dt == MM_I64 ? (float)i64 : f;
+  f = dt == MM_F64 ? (float)__longlong_as_double(i64) : f;
+  return f;
+}
+
+// 16 staged rows of ROW_BYTES -> global rows dst + r * dst_pitch (r < rows), sizeof(V) bytes per lane and store:
+// consecutive lanes write consecutive pieces of a row
+template <int ROW_BYTES, typename V>
+__device__ __forceinline__ void store_rows(const uint8_t* st, int pitch, uint8_t* dst, long long dst_pitch, int rows, int lane) {
+  constexpr int PER_ROW = ROW_BYTES / (int)sizeof(V), N = 16 * PER_ROW;
+#pragma unroll
+  for (int i = 0; i < (N + 31) / 32; ++i) {
+    const int c = i * 32 + lane;
+    const int r = c / PER_ROW, q = c % PER_ROW;
+    if ((N % 32 == 0 || c < N) && r < rows)
+      *reinterpret_cast<V*>(dst + r * dst_pitch + q * (int)sizeof(V)) = *reinterpret_cast<const V*>(st + r * pitch + q * (int)sizeof(V));
+  }
+}
+
+// RELU: both activations are relu (compile-time fast path: no per-element dispatch).  F32: every column is fp32.
+template <int N1T, int N2T, bool RELU, bool F32>
 __global__ void __launch_bounds__(32 * WARPS)
 tower_small_kernel(const __grid_constant__ Cols cols, const Params p) {
   extern __shared__ __align__(16) uint8_t smem[];
-  constexpr int N1 = 8 * N1T, N2 = 8 * N2T;
-  constexpr int W2_STRIDE = N1 * 4 + 16;  // [hi k0..N1 | lo k0..N1] + pad
-  uint8_t* w1s = smem;
-  uint8_t* w2s = w1s + N1 * W1_STRIDE;
-  float* b1s = reinterpret_cast<float*>(w2s + N2 * W2_STRIDE);
-  float* b2s = b1s + N1;
-  // ---- weights -> shared memory (once per CTA), 16 bytes per load
+  using L = Layout<N1T, N2T, F32>;
+  constexpr int N1 = L::N1, N2 = L::N2, W2_STRIDE = L::W2_STRIDE, SLOT = L::SLOT;
+  uint8_t* w1s = smem + L::W1;
+  uint8_t* w2s = smem + L::W2;
+  float* b1s = reinterpret_cast<float*>(smem + L::B1);
+  float* b2s = reinterpret_cast<float*>(smem + L::B2);
+  ColS* cs = reinterpret_cast<ColS*>(smem + L::COLS);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int g = lane >> 2, t = lane & 3;
+  uint8_t* xin = smem + L::XIN + warp * L::XIN_WARP;
+  uint8_t* ost = smem + L::OUT + warp * L::OUT_WARP;
+
+  if (threadIdx.x < MAX_COLS) {  // columns past K read column 0's address with zero fill
+    const int k = threadIdx.x < cols.K ? threadIdx.x : 0;
+    const int dt = cols.dtype[k];
+    const int esz = (dt == MM_I64 || dt == MM_F64) ? 8 : 4;
+    cs[threadIdx.x] = ColS{reinterpret_cast<const uint8_t*>(cols.src[k]) + (long long)cols.off[k] * esz, cols.stride[k] * esz, dt, 0};
+  }
+  __syncthreads();
+
+  // this lane's values of tile `tile` -> stage `buf`: columns k = 2t, 2t+1, 2t+8, 2t+9 (j = 0..3) of rows g and g+8
+  // (h = 0, 1) as value v = 2j + h; rows at or past B and columns at or past K are zero-filled
+  const long long tiles = (p.B + 15) >> 4;
+  const long long tstep = (long long)gridDim.x * WARPS;
+  auto issue = [&](long long tile, int buf) {
+    const uint32_t dst0 = (uint32_t)__cvta_generic_to_shared(xin) + (uint32_t)(buf * 8 * 32 * SLOT + lane * SLOT);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int k = 2 * t + (j & 1) + ((j >> 1) << 3);
+      const ColS c = cs[k];
+      const bool on = k < cols.K;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const long long r = tile * 16 + g + 8 * h;
+        const bool valid = on && r < p.B;
+        const uint8_t* src = c.base + (valid ? r * c.pitch : 0);
+        const uint32_t dst = dst0 + (uint32_t)((2 * j + h) * 32 * SLOT);
+        if (F32 || !(c.dtype == MM_I64 || c.dtype == MM_F64))
+          cp_async4_zfill(dst, src, valid);
+        else
+          cp_async8_zfill(dst, src, valid);
+      }
+    }
+    cp_async_commit();
+  };
+  long long tile = (long long)blockIdx.x * WARPS + warp;
+  issue(tile, 0);  // in flight during the weight fill
+
+  // ---- weights -> shared memory (once per CTA), 16-byte cp.async: every chunk of a thread in flight at once
   for (int e = threadIdx.x; e < N1 * 4; e += blockDim.x) {  // W1 row n: hi k0..15 (2 x 16 B) | lo k0..15 (2 x 16 B)
     const int n = e >> 2, c = e & 3;
-    const uint4 v = *reinterpret_cast<const uint4*>(p.w1 + (long long)n * 2 * p.K1p + (c < 2 ? c * 8 : p.K1p + (c - 2) * 8));
-    *reinterpret_cast<uint4*>(w1s + n * W1_STRIDE + c * 16) = v;
+    cp_async16_if(true, (uint32_t)__cvta_generic_to_shared(w1s + n * W1_STRIDE + c * 16),
+                  p.w1 + (long long)n * 2 * p.K1p + (c < 2 ? c * 8 : p.K1p + (c - 2) * 8));
   }
   constexpr int C2 = N1 / 8;  // 16-byte chunks per half row of W2
   for (int e = threadIdx.x; e < N2 * 2 * C2; e += blockDim.x) {
     const int n = e / (2 * C2), c = e % (2 * C2);
-    const uint4 v = *reinterpret_cast<const uint4*>(p.w2 + (long long)n * 2 * p.K2p + (c < C2 ? c * 8 : p.K2p + (c - C2) * 8));
-    *reinterpret_cast<uint4*>(w2s + n * W2_STRIDE + c * 16) = v;
+    cp_async16_if(true, (uint32_t)__cvta_generic_to_shared(w2s + n * W2_STRIDE + c * 16),
+                  p.w2 + (long long)n * 2 * p.K2p + (c < C2 ? c * 8 : p.K2p + (c - C2) * 8));
   }
+  cp_async_commit();
   for (int e = threadIdx.x; e < N1; e += blockDim.x) b1s[e] = p.b1 ? p.b1[e] : 0.0f;
   for (int e = threadIdx.x; e < N2; e += blockDim.x) b2s[e] = p.b2 ? p.b2[e] : 0.0f;
+  cp_async_wait<0>();  // (also the first tile's values, issued before the weights)
   __syncthreads();
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int g = lane >> 2, t = lane & 3;
   const uint32_t w1_lane = (uint32_t)__cvta_generic_to_shared(w1s) + (uint32_t)(lane & 7) * W1_STRIDE + (uint32_t)(lane >> 3) * 16u;
   // W2: matrices (hi, chunk 2ks) (hi, 2ks+1) (lo, 2ks) (lo, 2ks+1) of rows 8nt + (lane & 7)
   const uint32_t w2_lane = (uint32_t)__cvta_generic_to_shared(w2s) + (uint32_t)(lane & 7) * W2_STRIDE +
                            (uint32_t)((lane >> 3) & 1) * 16u + (uint32_t)(lane >> 4) * (N1 * 2);
-  // this lane's four input columns k = 2t, 2t+1, 2t+8, 2t+9 as running byte pointers (row g of the warp's first tile)
-  const long long tiles = (p.B + 15) >> 4;
-  const long long tile0 = (long long)blockIdx.x * WARPS + warp, tstep = (long long)gridDim.x * WARPS;
-  const uint8_t* cptr[4];
-  int cstep[4];  // bytes between consecutive rows of the column
-  uint32_t cdts = 0;
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const int k = 2 * t + (j & 1) + ((j >> 1) << 3);
-    const bool on = k < cols.K;
-    const int kk = on ? k : 0;
-    const int dt = cols.dtype[kk];
-    const int esz = (dt == MM_I64 || dt == MM_F64) ? 8 : 4;
-    cstep[j] = (int)(cols.stride[kk] * esz);
-    cptr[j] = on ? reinterpret_cast<const uint8_t*>(cols.src[kk]) + (long long)cols.off[kk] * esz + (tile0 * 16 + g) * (long long)cstep[j]
-                 : nullptr;
-    cdts |= (uint32_t)dt << (8 * j);
-  }
-  for (long long tile = tile0; tile < tiles; tile += tstep) {
-    const long long r0 = tile * 16 + g, r1 = r0 + 8;
-    const bool v0 = r0 < p.B, v1 = r1 < p.B;
-    // ---- A fragment of layer 1 from the column arrays: rows {g, g+8} x k {2t, 2t+1, 2t+8, 2t+9}
+  for (int buf = 0; tile < tiles; tile += tstep, buf ^= 1) {
+    issue(tile + tstep, buf ^ 1);  // zero-filled past the last tile
+    cp_async_wait<1>();            // this tile's values (each lane reads only the slots it copied itself)
+    // ---- A fragment of layer 1: rows {g, g+8} x k {2t, 2t+1, 2t+8, 2t+9}
     float x[2][4];
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      const int dt = (int)((cdts >> (8 * j)) & 0xff);
-      x[0][j] = (cptr[j] && v0) ? load_as_f32<true>(cptr[j], 0, dt) : 0.0f;
-      x[1][j] = (cptr[j] && v1) ? load_as_f32<true>(cptr[j] + 8 * (long long)cstep[j], 0, dt) : 0.0f;
-      if (cptr[j]) cptr[j] += tstep * 16 * (long long)cstep[j];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint8_t* s = xin + buf * 8 * 32 * SLOT + (2 * j + h) * 32 * SLOT + lane * SLOT;
+        if (F32) {
+          x[h][j] = *reinterpret_cast<const float*>(s);
+        } else {
+          const int k = 2 * t + (j & 1) + ((j >> 1) << 3);
+          x[h][j] = raw_to_f32(*reinterpret_cast<const uint2*>(s), k < cols.K ? cols.dtype[k] : cs[0].dtype);
+        }
+      }
     }
     uint32_t ah[4], al[4];
     split_pair(x[0][0], x[0][1], ah[0], al[0]);
     split_pair(x[1][0], x[1][1], ah[1], al[1]);
     split_pair(x[0][2], x[0][3], ah[2], al[2]);
     split_pair(x[1][2], x[1][3], ah[3], al[3]);
-    // ---- the hidden layer in halves of HT n-tiles: layer 1 computes HT*8 hidden units, which are at once consumed as
-    // HT/2 k-steps of layer 2 (the accumulator fragment of n-tiles (2k, 2k+1) IS the A fragment of k-step k), so only half
-    // of the hidden activations is live at a time.  Groups of 4 n-tiles, pass-major: four independent accumulators
-    // between dependent MMAs.
-    constexpr int HT = N1T >= 8 ? N1T / 2 : N1T;
+    // ---- the hidden layer in chunks of HT = 4 n-tiles: layer 1 computes 32 hidden units, which are at once consumed as
+    // 2 k-steps of layer 2 (the accumulator fragment of n-tiles (2k, 2k+1) IS the A fragment of k-step k), so only 32
+    // hidden activations per row are live at a time.  Groups of 4 n-tiles, pass-major: four independent accumulators
+    // between dependent MMAs.  The chunk loop stays rolled for the wide relu shapes: unrolled, ptxas hoists the next
+    // chunk's fragment loads and spills.
+    constexpr int HT = 4;
     float acc2[N2T][4];
 #pragma unroll
     for (int nt = 0; nt < N2T; ++nt) acc2[nt][0] = acc2[nt][1] = acc2[nt][2] = acc2[nt][3] = 0.0f;
-#pragma unroll
-    for (int half = 0; half < N1T / HT; ++half) {
+#pragma unroll (RELU && N1T * N2T >= 64 ? 1 : N1T / HT)
+    for (int ch = 0; ch < N1T / HT; ++ch) {
       float acc1[HT][4];
 #pragma unroll
       for (int n0 = 0; n0 < HT; n0 += 4) {
         uint32_t bh[4][2], bl[4][2];
 #pragma unroll
         for (int u = 0; u < 4; ++u) {
-          ldsm_x4(w1_lane + (uint32_t)(half * HT + n0 + u) * (8 * W1_STRIDE), bh[u][0], bh[u][1], bl[u][0], bl[u][1]);
+          ldsm_x4(w1_lane + (uint32_t)(ch * HT + n0 + u) * (8 * W1_STRIDE), bh[u][0], bh[u][1], bl[u][0], bl[u][1]);
           acc1[n0 + u][0] = acc1[n0 + u][1] = acc1[n0 + u][2] = acc1[n0 + u][3] = 0.0f;
         }
 #pragma unroll
@@ -151,7 +239,7 @@ tower_small_kernel(const __grid_constant__ Cols cols, const Params p) {
       }
 #pragma unroll
       for (int nt = 0; nt < HT; ++nt) {
-        const float2 b = *reinterpret_cast<const float2*>(b1s + 8 * (half * HT + nt) + 2 * t);
+        const float2 b = *reinterpret_cast<const float2*>(b1s + 8 * (ch * HT + nt) + 2 * t);
         acc1[nt][0] = act_fn<RELU>(acc1[nt][0] + b.x, p.act1);
         acc1[nt][1] = act_fn<RELU>(acc1[nt][1] + b.y, p.act1);
         acc1[nt][2] = act_fn<RELU>(acc1[nt][2] + b.x, p.act1);
@@ -159,7 +247,7 @@ tower_small_kernel(const __grid_constant__ Cols cols, const Params p) {
       }
 #pragma unroll
       for (int kq = 0; kq < HT / 2; ++kq) {
-        const int ks = half * (HT / 2) + kq;
+        const int ks = ch * (HT / 2) + kq;
         uint32_t a2h[4], a2l[4];
         split_pair(acc1[2 * kq][0], acc1[2 * kq][1], a2h[0], a2l[0]);
         split_pair(acc1[2 * kq][2], acc1[2 * kq][3], a2h[1], a2l[1]);
@@ -181,39 +269,60 @@ tower_small_kernel(const __grid_constant__ Cols cols, const Params p) {
         }
       }
     }
-    // ---- epilogue: bias + activation, fp32 rows and / or split-bf16 rows
+    // ---- epilogue: bias + activation; fp32 rows and / or split-bf16 rows, each staged and then stored row-contiguous
 #pragma unroll
     for (int nt = 0; nt < N2T; ++nt) {
-      const int n = 8 * nt + 2 * t;
-      const float2 b = *reinterpret_cast<const float2*>(b2s + n);
-      const float y00 = act_fn<RELU>(acc2[nt][0] + b.x, p.act2), y01 = act_fn<RELU>(acc2[nt][1] + b.y, p.act2);
-      const float y10 = act_fn<RELU>(acc2[nt][2] + b.x, p.act2), y11 = act_fn<RELU>(acc2[nt][3] + b.y, p.act2);
-      if (p.out_f32) {
-        if (v0) *reinterpret_cast<float2*>(p.out_f32 + r0 * p.out_stride + n) = make_float2(y00, y01);
-        if (v1) *reinterpret_cast<float2*>(p.out_f32 + r1 * p.out_stride + n) = make_float2(y10, y11);
-      }
-      if (p.out_split) {
+      const float2 b = *reinterpret_cast<const float2*>(b2s + 8 * nt + 2 * t);
+      acc2[nt][0] = act_fn<RELU>(acc2[nt][0] + b.x, p.act2);
+      acc2[nt][1] = act_fn<RELU>(acc2[nt][1] + b.y, p.act2);
+      acc2[nt][2] = act_fn<RELU>(acc2[nt][2] + b.x, p.act2);
+      acc2[nt][3] = act_fn<RELU>(acc2[nt][3] + b.y, p.act2);
+    }
+    const int rows = (int)min(16LL, p.B - tile * 16);
+    if (p.out_split) {
+#pragma unroll
+      for (int nt = 0; nt < N2T; ++nt) {
+        const int n = 8 * nt + 2 * t;
         uint32_t h0, l0, h1, l1;
-        split_pair(y00, y01, h0, l0);
-        split_pair(y10, y11, h1, l1);
-        if (v0) {
-          *reinterpret_cast<uint32_t*>(p.out_split + r0 * (2 * N2) + n) = h0;
-          *reinterpret_cast<uint32_t*>(p.out_split + r0 * (2 * N2) + N2 + n) = l0;
-        }
-        if (v1) {
-          *reinterpret_cast<uint32_t*>(p.out_split + r1 * (2 * N2) + n) = h1;
-          *reinterpret_cast<uint32_t*>(p.out_split + r1 * (2 * N2) + N2 + n) = l1;
-        }
+        split_pair(acc2[nt][0], acc2[nt][1], h0, l0);
+        split_pair(acc2[nt][2], acc2[nt][3], h1, l1);
+        *reinterpret_cast<uint32_t*>(ost + g * L::SPLIT_PITCH + 2 * n) = h0;
+        *reinterpret_cast<uint32_t*>(ost + g * L::SPLIT_PITCH + 2 * (N2 + n)) = l0;
+        *reinterpret_cast<uint32_t*>(ost + (g + 8) * L::SPLIT_PITCH + 2 * n) = h1;
+        *reinterpret_cast<uint32_t*>(ost + (g + 8) * L::SPLIT_PITCH + 2 * (N2 + n)) = l1;
       }
+      __syncwarp();
+      uint8_t* dst = reinterpret_cast<uint8_t*>(p.out_split) + tile * 16 * (4 * N2);
+      if (p.out_split_v16)
+        store_rows<4 * N2, uint4>(ost, L::SPLIT_PITCH, dst, 4 * N2, rows, lane);
+      else
+        store_rows<4 * N2, uint32_t>(ost, L::SPLIT_PITCH, dst, 4 * N2, rows, lane);
+      __syncwarp();
+    }
+    if (p.out_f32) {
+#pragma unroll
+      for (int nt = 0; nt < N2T; ++nt) {
+        const int n = 8 * nt + 2 * t;
+        *reinterpret_cast<float2*>(ost + g * L::F32_PITCH + 4 * n) = make_float2(acc2[nt][0], acc2[nt][1]);
+        *reinterpret_cast<float2*>(ost + (g + 8) * L::F32_PITCH + 4 * n) = make_float2(acc2[nt][2], acc2[nt][3]);
+      }
+      __syncwarp();
+      const long long pitch = p.out_stride * 4;
+      uint8_t* dst = reinterpret_cast<uint8_t*>(p.out_f32) + tile * 16 * pitch;
+      if (p.out_f32_v16)
+        store_rows<4 * N2, uint4>(ost, L::F32_PITCH, dst, pitch, rows, lane);
+      else
+        store_rows<4 * N2, uint2>(ost, L::F32_PITCH, dst, pitch, rows, lane);
+      __syncwarp();
     }
   }
+  cp_async_wait<0>();
 }
 
-template <int N1T, int N2T, bool RELU>
+template <int N1T, int N2T, bool RELU, bool F32>
 static int launch(const Cols& c, const Params& p, cudaStream_t st) {
-  constexpr int N1 = 8 * N1T, N2 = 8 * N2T;
-  const size_t smem = (size_t)N1 * W1_STRIDE + (size_t)N2 * (N1 * 4 + 16) + (size_t)(N1 + N2) * sizeof(float);
-  auto kern = tower_small_kernel<N1T, N2T, RELU>;
+  const size_t smem = (size_t)Layout<N1T, N2T, F32>::BYTES;
+  auto kern = tower_small_kernel<N1T, N2T, RELU, F32>;
   if (smem > 48 * 1024) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) {
@@ -227,6 +336,12 @@ static int launch(const Cols& c, const Params& p, cudaStream_t st) {
   if (blocks > cap) blocks = cap;
   kern<<<(unsigned)blocks, 32 * WARPS, smem, st>>>(c, p);
   return check_launch("mm_tower2_small");
+}
+
+template <int N1T, int N2T>
+static int launch(const Cols& c, const Params& p, bool relu, bool f32, cudaStream_t st) {
+  if (f32) return relu ? launch<N1T, N2T, true, true>(c, p, st) : launch<N1T, N2T, false, true>(c, p, st);
+  return relu ? launch<N1T, N2T, true, false>(c, p, st) : launch<N1T, N2T, false, false>(c, p, st);
 }
 
 }  // namespace tsm
@@ -247,11 +362,13 @@ int mm_tower2_small(const mm_concat_piece* pieces_host, int n_pieces, int64_t B,
   Cols c;
   memset(&c, 0, sizeof(c));
   int K = 0;
+  bool f32 = true;
   for (int i = 0; i < n_pieces; ++i) {
     const mm_concat_piece& pc = pieces_host[i];
     MM_REQUIRE(pc.src && pc.width >= 1 && pc.src_stride >= pc.width && pc.dtype >= MM_I32 && pc.dtype <= MM_F64, MM_ERR_ARG,
                "mm_tower2_small: piece %d: null source, bad width / stride / dtype", i);
     MM_REQUIRE(pc.out_col == K, MM_ERR_ARG, "mm_tower2_small: pieces must be listed in column order without gaps (piece %d)", i);
+    f32 = f32 && pc.dtype == MM_F32;
     for (int w = 0; w < pc.width; ++w) {
       MM_REQUIRE(K < MAX_COLS, MM_ERR_UNSUPPORTED, "mm_tower2_small: more than %d input columns", MAX_COLS);
       c.src[K] = pc.src;
@@ -284,10 +401,12 @@ int mm_tower2_small(const mm_concat_piece* pieces_host, int n_pieces, int64_t B,
   p.out_f32 = out;
   p.out_stride = out_stride;
   p.out_split = (__nv_bfloat16*)out_split;
+  p.out_f32_v16 = ((uintptr_t)out % 16) == 0 && (out_stride % 4) == 0;
+  p.out_split_v16 = ((uintptr_t)out_split % 16) == 0;
   cudaStream_t st = (cudaStream_t)stream;
   const bool relu = act1 == MM_ACT_RELU && act2 == MM_ACT_RELU;
 #define MM_TSM(a, b) \
-  if (N1 == 8 * a && N2 == 8 * b) return relu ? launch<a, b, true>(c, p, st) : launch<a, b, false>(c, p, st);
+  if (N1 == 8 * a && N2 == 8 * b) return launch<a, b>(c, p, relu, f32, st);
   MM_TSM(16, 8) MM_TSM(16, 4) MM_TSM(16, 2) MM_TSM(8, 8) MM_TSM(8, 4) MM_TSM(8, 2) MM_TSM(4, 8) MM_TSM(4, 4) MM_TSM(4, 2)
 #undef MM_TSM
   return MM_ERR_UNSUPPORTED;

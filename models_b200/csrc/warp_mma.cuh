@@ -56,6 +56,13 @@ __device__ __forceinline__ void cp_async4_if(bool pred, uint32_t dst, const void
       "l"(src), "r"((uint32_t)pred)
       : "memory");
 }
+// 4- / 8-byte cp.async that writes zeros instead of copying when !valid (src-size 0: nothing is read from src)
+__device__ __forceinline__ void cp_async4_zfill(uint32_t dst, const void* src, bool valid) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(src), "r"(valid ? 4u : 0u) : "memory");
+}
+__device__ __forceinline__ void cp_async8_zfill(uint32_t dst, const void* src, bool valid) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 8, %2;" ::"r"(dst), "l"(src), "r"(valid ? 8u : 0u) : "memory");
+}
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() {
