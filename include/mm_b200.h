@@ -585,6 +585,36 @@ int mm_deepfm_head(const mm_lookup_table* tables_host, const int64_t* wide_offse
                    const float* wide_kernel, const float* wide_bias, const float* addend, int64_t addend_stride,
                    const float* out_w, const float* out_b, int out_act, float* out, int32_t* oob_count, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * K16  Training step of the two-tower path (TwoTowerModel + ItemRetrievalTask, prediction_tasks/retrieval.py:33-191;
+ * CategoricalCrossentropy(from_logits=True) against the one-hot on column 0, losses/listwise.py:38-50).  Added with
+ * two-tower training; no existing entry point changed.
+ *   mm_inbatch_softmax_ce_backward  backward of mm_inbatch_softmax_ce without the (B, 1+N) logits.  With s the logits of
+ *       that call (s[b,0] = pos_logit[b]; s[b,1+n] = masked ? false_neg_score/T : (q_b.neg_n - log(neg_prob[n]+1e-16))/T,
+ *       masked = downscore && pos_ids[b] == neg_ids[n]), lse[b] = stats[b,1] and p = exp(s - lse)
+ *       (false_neg_score is taken for symmetry with the forward and not read: a masked logit is a constant):
+ *         g[b,0] = c[b] (p[b,0] - 1) / T;  g[b,1+n] = masked ? 0 : c[b] p[b,1+n] / T   (the masked logits are constants)
+ *         dq[b] = g[b,0] pos[b] + sum_n g[b,1+n] neg[n];  dpos[b] = g[b,0] q[b];  dneg[n] = sum_b g[b,1+n] q[b]
+ *         *loss += sum_b c[b] (lse[b] - s[b,0])        (loss nullable; accumulated: zero it first)
+ *       c = row_scale: (B,) device floats, or ONE device float when row_scale_is_scalar (1/B: Keras' mean).
+ *       q_split / neg_split: the operands the forward read (mm_split_rows, Kp = mm_tc_padded_k(D) <= 128, 16-B aligned);
+ *       stats (B,3): mm_inbatch_softmax_ce's output; q, pos (B, D), dq, dpos (B, D), dneg (N, D): contiguous fp32.
+ *       dpos may alias dneg when the negatives are the positives (in-batch, N == B): the sum is written.  dq aliases
+ *       neither.  Two wgmma kernels recompute the logits tile by tile (inbatch_ce_dq_kernel: one CTA per 128 queries;
+ *       inbatch_ce_dn_kernel: one CTA per 128 negatives), each output row is written by one CTA: deterministic.
+ *       Errors before any launch: MM_ERR_ARG (null pointer, T <= 0, N <= 0, ids missing for down-scoring, dpos == dneg with
+ *       N != B), MM_ERR_UNSUPPORTED (D > 128, sizes >= 2^31), MM_ERR_ALIGN (split operands not 16-B aligned).
+ *   mm_l2_normalize_backward  backward of mm_l2_normalize from its INPUT x: s = sum(x^2), n = sqrt(s), y = x / n;
+ *       s >= 1e-12: dx = (dy - y (y.dy)) / n, else dx = dy / 1e-6 (TF's gradient of maximum(s, 1e-12) flows to s only
+ *       where s >= 1e-12).  dx may alias x or dy.
+ * ------------------------------------------------------------------------------------- */
+int mm_inbatch_softmax_ce_backward(const void* q_split, const void* neg_split, int64_t B, int64_t N, int D, const void* pos_ids,
+                                   const void* neg_ids, int id_dtype, int downscore, float false_neg_score, const float* neg_prob,
+                                   float temperature, const float* stats, const float* q, const float* pos, const float* row_scale,
+                                   int row_scale_is_scalar, float* dq, float* dpos, float* dneg, float* loss, void* stream);
+int mm_l2_normalize_backward(const float* x, const float* dy, int64_t B, int D, int64_t x_stride, int64_t dy_stride, float* dx,
+                             int64_t dx_stride, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -164,6 +164,9 @@ SIGNATURES = {
     "mm_fill_i32": (_i, [_vp, _i64, C.c_int32, _vp]),
     "mm_cross_backward": (_i, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _i, _i64, _i, _vp, _i64, _vp, _i, _vp]),
     "mm_concat_backward": (_i, [C.POINTER(C.c_void_p), C.POINTER(C.c_int64), _i, _i64, _i, C.POINTER(ColumnSlice), _i, _vp]),
+    "mm_inbatch_softmax_ce_backward": (_i, [_vp, _vp, _i64, _i64, _i, _vp, _vp, _i, _i, _f, _vp, _f, _vp, _vp, _vp, _vp, _i,
+                                            _vp, _vp, _vp, _vp, _vp]),
+    "mm_l2_normalize_backward": (_i, [_vp, _vp, _i64, _i, _i64, _i64, _vp, _i64, _vp]),
 }
 
 

@@ -108,6 +108,33 @@ __global__ void l2_normalize_kernel(const float* __restrict__ x, long long B, in
   }
 }
 
+// Backward of l2_normalize_kernel, y = x / sqrt(max(sum(x^2), 1e-12)) (transforms/regularization.py:27-82).  TF's gradient
+// of tf.math.maximum(s, eps) flows to s where s >= eps, so: s >= 1e-12: dx = (dy - y (y . dy)) / n, n = sqrt(s);
+// otherwise the denominator is the constant 1e-6 and dx = dy / 1e-6.  Each lane reads x[d], dy[d] before it writes dx[d]:
+// dx may alias x or dy.
+__global__ void l2_normalize_backward_kernel(const float* x, const float* dy, long long B, int D, long long x_stride,
+                                             long long dy_stride, float* dx, long long dx_stride) {
+  const int lane = threadIdx.x & 31;
+  const long long warp0 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const long long n_warps = ((long long)gridDim.x * blockDim.x) >> 5;
+  for (long long b = warp0; b < B; b += n_warps) {
+    float ss = 0.0f, xg = 0.0f;
+    for (int d = lane; d < D; d += 32) {
+      const float v = x[b * x_stride + d], g = dy[b * dy_stride + d];
+      ss = fmaf(v, v, ss);
+      xg = fmaf(v, g, xg);
+    }
+    ss = warp_sum(ss);
+    xg = warp_sum(xg);
+    const bool on = ss >= 1e-12f;
+    const float nrm = on ? sqrtf(ss) : 1e-6f;
+    const float yg = on ? xg / nrm : 0.0f;  // y . dy
+    for (int d = lane; d < D; d += 32) {
+      const float y = x[b * x_stride + d] / nrm;
+      dx[b * dx_stride + d] = (dy[b * dy_stride + d] - y * yg) / nrm;
+    }
+  }
+}
 
 // out[b, c] = x[b, c] * scale[c] + shift[c]: tf.keras.layers.BatchNormalization at inference with
 // scale = gamma / sqrt(moving_var + eps), shift = beta - moving_mean * scale (blocks/mlp.py:131-135).
@@ -220,6 +247,20 @@ int mm_l2_normalize(const float* x, int64_t B, int D, int64_t x_stride, float* o
   mm::l2_normalize_kernel<<<(unsigned)blocks, threads, 0, (cudaStream_t)stream>>>(x, B, D, x_stride, out,
                                                                                 out_stride);
   return mm::check_launch("mm_l2_normalize");
+}
+
+int mm_l2_normalize_backward(const float* x, const float* dy, int64_t B, int D, int64_t x_stride, int64_t dy_stride, float* dx,
+                             int64_t dx_stride, void* stream) {
+  MM_REQUIRE(x && dy && dx && B >= 0 && D > 0 && x_stride >= D && dy_stride >= D && dx_stride >= D, MM_ERR_ARG,
+             "mm_l2_normalize_backward: null pointer, D<=0 or stride < D");
+  if (B == 0) return MM_OK;
+  const int threads = 256;
+  long long blocks = (B * 32 + threads - 1) / threads;
+  const long long cap = (long long)mm::sm_count() * 32;
+  if (blocks > cap) blocks = cap;
+  mm::l2_normalize_backward_kernel<<<(unsigned)blocks, threads, 0, (cudaStream_t)stream>>>(x, dy, B, D, x_stride, dy_stride, dx,
+                                                                                         dx_stride);
+  return mm::check_launch("mm_l2_normalize_backward");
 }
 
 int mm_scale_shift(const float* x, int64_t B, int D, int64_t x_stride, const float* scale, const float* shift,

@@ -198,7 +198,8 @@ def parse_prediction_blocks(schema: Schema, prediction_blocks=None) -> Block:
     return prediction_blocks
 
 
-_LOSS_ALIASES = {"binary_crossentropy": "binary_crossentropy", "mse": "mse", "mean_squared_error": "mse"}
+_LOSS_ALIASES = {"binary_crossentropy": "binary_crossentropy", "mse": "mse", "mean_squared_error": "mse",
+                 "categorical_crossentropy": "categorical_crossentropy"}
 
 
 def resolve_loss_weights(outputs: Sequence[Block], loss=None, loss_weights=None) -> List[float]:
@@ -728,9 +729,42 @@ def _brute_force(k: int):
 
 
 class RetrievalModel(Model):
-    """models/base.py:2259-2489, forward only."""
+    """models/base.py:2259-2489.  `compile(optimizer=...)` / `train_step` / `fit` train a v1 TwoTowerModel with its
+    ItemRetrievalTask's in-batch soft-max cross-entropy (models_b200/train.py: TwoTowerTrainer)."""
 
     _TRANSIENT = {"pre_eval_topk": None}
+
+    def train_step(self, data) -> Dict[str, torch.Tensor]:
+        """One optimizer step on `data` = (inputs,) or (inputs, targets); the targets are ignored, because the retrieval task
+        builds its own one-hot targets (the positive item on column 0).  Returns {"loss", "loss_batch",
+        "regularization_loss"} as device scalars, views of the engine's loss buffer valid until the next step."""
+        if getattr(self, "optimizer", None) is None:
+            raise RuntimeError("compile() the model with an optimizer before training it")
+        if isinstance(data, dict):
+            data = (data,)
+        if not isinstance(data, (tuple, list)) or not data:
+            raise ValueError("train_step expects (inputs,) or (inputs, targets)")
+        if len(data) > 2 and data[2] is not None:
+            raise NotImplementedError("sample_weight is not implemented in the two-tower training step")
+        x = data[0]
+        self._check_inputs(x)
+        tr = self.trainer(batch_size_of(x))
+        loss = tr.step(x, None)
+        return {"loss": loss[0], "loss_batch": loss[0], "regularization_loss": torch.zeros((), device=loss.device)}
+
+    def fit(self, x=None, y=None, batch_size: Optional[int] = None, epochs: int = 1, steps_per_epoch: Optional[int] = None,
+            verbose: int = 0, **kwargs):
+        """Keras `fit` over a Loader or an iterable of batches, each a feature dict or (inputs, targets) (targets ignored)."""
+        if x is None:
+            raise ValueError("fit needs a loader / iterable of batches")
+        bs = batch_size or getattr(x, "batch_size", None)
+
+        class _Pairs:
+            def __iter__(self_):
+                for item in x:
+                    yield (item, None) if isinstance(item, dict) else (item[0], None)
+
+        return super().fit(_Pairs(), y, batch_size=bs, epochs=epochs, steps_per_epoch=steps_per_epoch, verbose=verbose, **kwargs)
 
     def build(self, device=None):
         self.body.build(device)

@@ -393,6 +393,80 @@ def inbatch_softmax_ce(q, pos, neg, pos_ids=None, neg_ids=None, downscore=True, 
     return stats
 
 
+def positive_scores(q: torch.Tensor, pos: torch.Tensor, out: torch.Tensor, pos_prob=None, temperature: float = 1.0) -> torch.Tensor:
+    """out (B,) = (q . pos - log(pos_prob + 1e-16)) / T, row-wise (mm_positive_scores): column 0 of the in-batch logits."""
+    for n_, t_ in (("q", q), ("pos", pos), ("out", out)):
+        _dev(t_, n_, torch.float32)
+    if not (q.is_contiguous() and pos.is_contiguous()) or q.shape != pos.shape or out.numel() != q.shape[0]:
+        raise ValueError("q and pos must be contiguous (B, D) and out hold B values")
+    _cabi.check(_lib().mm_positive_scores(q.data_ptr(), pos.data_ptr(), q.shape[0], q.shape[1], _ptr(pos_prob), float(temperature),
+                                          out.data_ptr(), 1, _stream()), "mm_positive_scores")
+    return out
+
+
+def inbatch_softmax_ce_split(q_split, neg_split, D: int, pos_logit, stats, workspace, pos_ids=None, neg_ids=None, downscore=True,
+                             false_neg_score: float = -655.04, neg_prob=None, temperature: float = 1.0) -> torch.Tensor:
+    """inbatch_softmax_ce on split operands the caller owns (mm_inbatch_softmax_ce): stats (B, 3) from q_split (B, 2*Kp),
+    neg_split (N, 2*Kp) and pos_logit (B,); workspace: uint8 of at least catalog_workspace_bytes(B, N) bytes.  Nothing is
+    allocated, so a training step can be captured into a CUDA graph."""
+    _dev(q_split, "q_split", torch.bfloat16), _dev(neg_split, "neg_split", torch.bfloat16)
+    _dev(pos_logit, "pos_logit", torch.float32), _dev(stats, "stats", torch.float32), _dev(workspace, "workspace", torch.uint8)
+    B, N = q_split.shape[0], neg_split.shape[0]
+    if stats.numel() != 3 * B or not stats.is_contiguous() or pos_logit.numel() != B:
+        raise ValueError(f"stats must be contiguous ({B}, 3) and pos_logit hold {B} values")
+    pos_ids, neg_ids, id_dt = _item_ids(pos_ids, neg_ids, downscore)
+    _cabi.check(
+        _lib().mm_inbatch_softmax_ce(q_split.data_ptr(), neg_split.data_ptr(), B, N, int(D), _ptr(pos_ids) if downscore else None,
+                                     _ptr(neg_ids) if downscore else None, id_dt, int(bool(downscore)), float(false_neg_score),
+                                     pos_logit.data_ptr(), _ptr(neg_prob), float(temperature), stats.data_ptr(), workspace.data_ptr(),
+                                     workspace.numel(), _stream()),
+        "mm_inbatch_softmax_ce")
+    return stats
+
+
+def catalog_workspace_bytes(B: int, N: int, k: int = 0) -> int:
+    return int(_lib().mm_catalog_workspace_bytes(int(B), int(N), int(k)))
+
+
+def inbatch_softmax_ce_backward(q_split, neg_split, D: int, stats, q, pos, row_scale, dq, dpos, dneg, loss=None, pos_ids=None,
+                                neg_ids=None, downscore=True, false_neg_score: float = -655.04, neg_prob=None,
+                                temperature: float = 1.0) -> None:
+    """Backward of inbatch_softmax_ce (mm_inbatch_softmax_ce_backward): from the split operands the forward read
+    (q_split (B, 2*Kp), neg_split (N, 2*Kp)) and its stats (B, 3), writes dq, dpos (B, D) and dneg (N, D) of
+    sum_b c[b] (lse[b] - s[b,0]) and adds that loss to `loss` (nullable).  row_scale: (B,) or (1,) fp32 c.  dpos may be
+    dneg (in-batch negatives, N == B): the sum is written."""
+    _dev(q_split, "q_split", torch.bfloat16), _dev(neg_split, "neg_split", torch.bfloat16)
+    for n_, t_ in (("stats", stats), ("q", q), ("pos", pos), ("row_scale", row_scale), ("dq", dq), ("dpos", dpos), ("dneg", dneg)):
+        _dev(t_, n_, torch.float32)
+        if not t_.is_contiguous():
+            raise ValueError(f"{n_} must be contiguous")
+    if loss is not None:
+        _dev(loss, "loss", torch.float32)
+    B, N = q_split.shape[0], neg_split.shape[0]
+    Kp = tc_padded_k(D)
+    for n_, t_, shape in (("q_split", q_split, (B, 2 * Kp)), ("neg_split", neg_split, (N, 2 * Kp)), ("stats", stats, (B, 3)),
+                          ("q", q, (B, D)), ("pos", pos, (B, D)), ("dq", dq, (B, D)), ("dpos", dpos, (B, D)), ("dneg", dneg, (N, D))):
+        if tuple(t_.shape) != shape:
+            raise ValueError(f"{n_} must be {shape}, got {tuple(t_.shape)}")
+    if not (q_split.is_contiguous() and neg_split.is_contiguous()):
+        raise ValueError("q_split and neg_split must be contiguous")
+    if neg_prob is not None and (_dev(neg_prob, "neg_prob", torch.float32).numel() != N or not neg_prob.is_contiguous()):
+        raise ValueError(f"neg_prob must hold {N} contiguous values")
+    if loss is not None and loss.numel() < 1:
+        raise ValueError("loss must hold at least one value")
+    if row_scale.numel() not in (1, B):
+        raise ValueError(f"row_scale must hold 1 or {B} values, got {row_scale.numel()}")
+    scalar = row_scale.numel() == 1 and B != 1
+    pos_ids, neg_ids, id_dt = _item_ids(pos_ids, neg_ids, downscore)
+    _cabi.check(
+        _lib().mm_inbatch_softmax_ce_backward(q_split.data_ptr(), neg_split.data_ptr(), B, N, int(D),
+                                              _ptr(pos_ids) if downscore else None, _ptr(neg_ids) if downscore else None, id_dt,
+                                              int(bool(downscore)), float(false_neg_score), _ptr(neg_prob), float(temperature),
+                                              stats.data_ptr(), q.data_ptr(), pos.data_ptr(), row_scale.data_ptr(), int(scalar),
+                                              dq.data_ptr(), dpos.data_ptr(), dneg.data_ptr(), _ptr(loss), _stream()),
+        "mm_inbatch_softmax_ce_backward")
+
+
 _CONCAT_DTYPES = {torch.int32: _cabi.MM_I32, torch.int64: _cabi.MM_I64, torch.float32: _cabi.MM_F32,
                   torch.float64: _cabi.MM_F64}
 
@@ -507,6 +581,20 @@ def l2_normalize(x: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.T
     _cabi.check(_lib().mm_l2_normalize(x.data_ptr(), x.shape[0], x.shape[1], _row_stride(x, "x"), out.data_ptr(),
                                        _row_stride(out, "out"), _stream()), "mm_l2_normalize")
     return out
+
+
+def l2_normalize_backward(x: torch.Tensor, dy: torch.Tensor, dx: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Gradient of l2_normalize at its input x (mm_l2_normalize_backward); dx may be x or dy."""
+    _dev(x, "x", torch.float32), _dev(dy, "dy", torch.float32)
+    if dx is None:
+        dx = torch.empty_like(dy)
+    _dev(dx, "dx", torch.float32)
+    if x.shape != dy.shape or dx.shape != dy.shape:
+        raise ValueError("x, dy and dx must have the same shape")
+    _cabi.check(_lib().mm_l2_normalize_backward(x.data_ptr(), dy.data_ptr(), x.shape[0], x.shape[1], _row_stride(x, "x"),
+                                                _row_stride(dy, "dy"), dx.data_ptr(), _row_stride(dx, "dx"), _stream()),
+                "mm_l2_normalize_backward")
+    return dx
 
 
 # ---------------------------------------------------------------------------------------------

@@ -386,7 +386,10 @@ def _sampled_negatives(samplers, table, pos_emb, pos_ids, logq: bool):
 
 class ItemRetrievalTask(Block):
     """prediction_tasks/retrieval.py:33-191: ItemRetrievalScorer (+ LogitsTemperatureScaler when
-    T != 1, applied only in training/testing — transforms/bias.py:44-52)."""
+    T != 1, applied only in training/testing — transforms/bias.py:44-52).  Its loss is the v1 default,
+    CategoricalCrossentropy(from_logits=True) against the one-hot on column 0 (:69)."""
+
+    loss = "categorical_crossentropy"
 
     def __init__(self, schema: Schema, samplers: Sequence = (), target_name: Optional[str] = None,
                  task_name: Optional[str] = None, post_logits=None, logits_temperature: float = 1.0,

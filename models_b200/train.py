@@ -24,6 +24,8 @@ trained eagerly (their number of ids changes per batch); fixed-length ones can b
 
 DCNModel trains through DCNTrainer (below): the cross network's backward (mm_cross_backward per layer), the input block's
 backward straight into per-table slices (mm_concat_backward) and one sparse update per distinct embedding width.
+The v1 TwoTowerModel trains through TwoTowerTrainer: both towers as DCN's input block + deep tower, the in-batch soft-max
+cross-entropy forward and backward without the (B, 1+B) logits (mm_inbatch_softmax_ce[_backward]).
 
 All Dense variables of the model are re-homed into ONE flat fp32 arena (gradients and optimizer slots mirror its layout), so
 the dense update is one launch and data-parallel training needs one all-reduce.  Every buffer is static: a step can be
@@ -919,10 +921,340 @@ class DCNTrainer(_StepTrainer):
         self._refresh_operands()
 
 
-def trainer_for(model, optimizer: Optimizer, batch_size: int, group=None):
-    """The training engine of `model`'s body: DLRMTrainer or DCNTrainer."""
-    from .models import DCNBody
+class TwoTowerTrainer(_StepTrainer):
+    """Static-buffer training step of a v1 TwoTowerModel (RetrievalModel over a TwoTowerBlock, ItemRetrievalTask with
+    in-batch negatives and false negatives down-scored by the item-id column) at one batch size; a smaller batch b runs in
+    the leading rows with its own b items as the negatives.
 
+    forward   per tower: gather of its tables' rows (mm_gather_multi; ragged bags mm_gather_bag, (B, L) ids mm_gather_seq)
+              and its continuous columns (mm_concat_columns) into x0 at their sorted-name offsets, its split operand, one
+              mm_dense_tc per layer (fp32 activation saved + the next layer's operand); mm_l2_normalize (post="l2-norm");
+              mm_split_rows of both outputs; mm_positive_scores + mm_inbatch_softmax_ce (no (b, 1+b) logits)
+    backward  mm_inbatch_softmax_ce_backward (c = 1/b: Keras' mean; dpos and dneg summed into one item gradient, the loss
+              accumulated on the device); mm_l2_normalize_backward; per tower mm_dense_wgrad[_split] + mm_dense_dgrad down to
+              x0; mm_concat_backward into each table's (b, D) IndexedSlices buffer; mm_bag_grad_rows for multi-hot features
+    update    mm_opt_tick, mm_dense_apply over ONE arena holding both towers, one mm_sparse_rows_apply per embedding width
+              (and per multi-hot table), mm_split_weights refresh of the operand copies the model's forward reads."""
+
+    def __init__(self, model, optimizer: Optimizer, batch_size: int, device=None, group=None):
+        from .blocks import dense_engine
+        from .models import RetrievalModel
+        from .retrieval import InBatchSampler, ItemRetrievalTask, L2Norm, TwoTowerBlock
+
+        if not isinstance(model, RetrievalModel) or not isinstance(model.body, TwoTowerBlock):
+            raise NotImplementedError("TwoTowerTrainer trains the v1 TwoTowerModel (a RetrievalModel over a TwoTowerBlock)")
+        task = model.prediction
+        if not isinstance(task, ItemRetrievalTask):
+            raise NotImplementedError("training a TwoTowerModel needs the default ItemRetrievalTask")
+        scorer = task.scorer
+        if scorer.sampled_softmax_mode:
+            raise NotImplementedError("training with sampled_softmax_mode is not implemented")
+        if len(scorer.samplers) != 1 or not isinstance(scorer.samplers[0], InBatchSampler):
+            raise NotImplementedError("training supports the in-batch sampler only (other samplers are not implemented)")
+        if getattr(task, "logq_sampling_correction", False):
+            raise NotImplementedError("the logQ sampling correction is not implemented in the training step")
+        if group is not None:
+            raise NotImplementedError("training a TwoTowerModel with a process group (data parallel) is not implemented")
+        if dense_engine() == "fp32":
+            raise NotImplementedError("training a TwoTowerModel runs on the tensor-core engine (dense_engine() == 'fp32')")
+        body = model.body
+        if body.post is not None and not isinstance(body.post, L2Norm):
+            raise NotImplementedError(f"post block {type(body.post).__name__}: only post='l2-norm' is implemented in training")
+        self._init_common(model, optimizer, batch_size, device, None)
+        self.task = task
+        self.temperature = float(task.logits_temperature)
+        self.downscore = bool(scorer.downscore_false_negatives)
+        self.false_neg_score = float(scorer.false_negatives_score)
+        self.item_id = scorer.item_id_feature_name
+        self.l2 = body.post is not None
+        self.H = 1
+        self.towers = []
+        self.feats, self.tables = [], []
+        seen = set()
+        for tb in (body.query, body.item):
+            mlp = tb.mlp
+            if not isinstance(mlp, MLP) or mlp.has_normalization or mlp.dropout:
+                raise NotImplementedError(f"{tb.name} tower: training supports MLPBlock towers without normalization / dropout")
+            for l in mlp.dense_layers:
+                if l.activation not in ("relu", "linear"):
+                    raise NotImplementedError(f"{l.name}: training supports relu / linear tower activations, got {l.activation!r}")
+            ib = tb.inputs
+            cols, widths, d = ib.layout()
+            emb = ib.embeddings
+            feats = list(emb.feature_names) if emb is not None else []
+            first = len(self.tables)
+            for f in feats:
+                t = emb.feature_to_table[f]
+                if id(t) in seen:
+                    raise NotImplementedError(f"feature {f!r}: training with a table shared between features is not implemented")
+                seen.add(id(t))
+                if not t.trainable:
+                    raise NotImplementedError(f"feature {f!r}: frozen embedding tables are not implemented in the training step")
+                D = t.table.shape[1]
+                if D % 4 or D > 128:
+                    raise NotImplementedError(f"table {t.table_name!r}: embedding width {D} is not supported by the sparse update "
+                                              "(it needs a multiple of 4 no larger than 128)")
+                self.feats.append(f)
+                self.tables.append(t)
+            cont = sorted(ib.continuous.features) if ib.continuous is not None else []
+            self.towers.append(dict(name=tb.name, layers=mlp.dense_layers, cols=cols, d=d, feats=feats, tidx=list(range(first, len(self.tables))),
+                                    cont=cont, oob=emb.counter(self.device) if emb is not None else None))
+        out_w = {t["layers"][-1].units for t in self.towers}
+        if len(out_w) != 1:
+            raise ValueError(f"the query and item towers must end in the same width, got {sorted(out_w)}")
+        self.D = out_w.pop()
+        if ops.tc_padded_k(self.D) > 128:
+            raise NotImplementedError(f"tower output width {self.D}: the in-batch soft-max kernels take up to 128")
+
+        layers = [l for t in self.towers for l in t["layers"]]
+        self.arena = DenseArena(layers, optimizer, self.device)
+        self._tc_layers = layers
+        self._wsplit = [ops.split_weights(l.kernel) for l in layers]
+        for l, ws in zip(layers, self._wsplit):
+            l._w_split = ws  # the model's forward keeps reading the refreshed operand copies
+        self.hyper = torch.from_numpy(optimizer.hyper()).to(self.device)
+        first_layer = {}
+        li = 0
+        for t in self.towers:
+            t["li0"] = li
+            first_layer[li] = bool(t["feats"])  # the first layer needs its input gradient only when the tower has tables
+            li += len(t["layers"])
+        self._init_wide(lambda i: first_layer.get(i, True))
+        self._init_table_state(optimizer)
+        self._by_width: Dict[int, List[int]] = {}
+        for t, tb in enumerate(self.tables):
+            self._by_width.setdefault(tb.table.shape[1], []).append(t)
+
+        # ---- activations and gradients
+        B = self.B
+        f32 = dict(dtype=torch.float32, device=self.device)
+        bf = dict(dtype=torch.bfloat16, device=self.device)
+        for t in self.towers:
+            d = t["d"]
+            t["ld"] = (d + 3) // 4 * 4
+            t["x0"] = torch.zeros((B, t["ld"]), **f32)
+            t["xs"] = torch.zeros((B, 2 * ops.tc_padded_k(d)), **bf)
+            t["h"] = [torch.zeros((B, l.units), **f32) for l in t["layers"]]
+            t["h_split"] = [torch.zeros((B, 2 * ops.tc_padded_k(l.units)), **bf) for l in t["layers"][:-1]]
+            t["dh"] = [torch.zeros((B, l.units), **f32) for l in t["layers"]]
+            t["dx0"] = torch.zeros((B, t["ld"]), **f32) if t["feats"] else None
+            t["y"] = torch.zeros((B, self.D), **f32) if self.l2 else None  # the normalised output
+            t["split"] = torch.zeros((B, 2 * ops.tc_padded_k(self.D)), **bf)
+        self.slices = [torch.zeros((B, tb.table.shape[1]), **f32) for tb in self.tables]
+        self.pos_logit = torch.zeros(B, **f32)
+        self.stats = torch.zeros((B, 3), **f32)
+        ws = max(ops.catalog_workspace_bytes(min(128 * m, B), min(128 * m, B)) for m in range(1, (B + 127) // 128 + 1))
+        self.ws = torch.zeros(ws, dtype=torch.uint8, device=self.device)
+        self._inv_b: Dict[int, torch.Tensor] = {}  # c = 1/b per batch size, one device float each
+        self._init_loss(B)
+        self.logits = self.stats  # [max, log-sum-exp, positive logit] of every row of the last step
+        # one counter for both towers (every gather receives it), so check_indices sees every table
+        self.oob = next((t["oob"] for t in self.towers if t["oob"] is not None), None)
+        self._bag_bufs: Dict[int, dict] = {}
+        self._bags: Dict[int, dict] = {}
+
+    # ---- the parts of _StepTrainer that concern output heads do not apply: the retrieval task builds its own targets
+    def _init_heads(self) -> None:
+        raise NotImplementedError
+
+    def _check_targets(self, targets, b: int) -> list:
+        if b > self.B or b < 1:
+            raise ValueError(f"this trainer was compiled for batches of up to {self.B} samples, got {b}")
+        return []
+
+    def _after_step(self) -> None:
+        from .core import bump_weights_version
+
+        self.steps += 1
+        bump_weights_version()
+
+    def capture(self, inputs: Dict[str, torch.Tensor], targets=None, clone: bool = True) -> None:
+        """As _StepTrainer.capture; the targets are ignored (the task's targets are the one-hot column 0)."""
+        super().capture(inputs, [], clone=clone)
+
+    def replay(self, inputs: Optional[Dict[str, torch.Tensor]] = None, targets=None) -> torch.Tensor:
+        return super().replay(inputs, None)
+
+    def gradients(self) -> Dict[str, torch.Tensor]:
+        """Dense gradients by tower-qualified variable name (after forward_backward, before apply_gradients)."""
+        out = {}
+        for t in self.towers:
+            for j, l in enumerate(t["layers"]):
+                i = t["li0"] + j
+                out[f"{t['name']}/{l.name}/kernel"] = self.arena.view(self.arena.grad, i, "kernel")
+                bv = self.arena.view(self.arena.grad, i, "bias")
+                if bv is not None:
+                    out[f"{t['name']}/{l.name}/bias"] = bv
+        return out
+
+    def table_gradients(self) -> Dict[str, tuple]:
+        """{feature: (ids, rows)} of the last forward_backward: the IndexedSlices of every table before duplicates are
+        summed (multi-hot features: one row per id)."""
+        out = {}
+        for t, f in enumerate(self.feats):
+            bag = self._bags.get(t)
+            if bag is None:
+                out[f] = (self._idx[t], self._slices[t])
+            else:
+                out[f] = (bag["apply_ids"], bag["rows"])
+        return out
+
+    # ---- one step on device tensors ------------------------------------------------------------------------------
+    def _scale(self, b: int) -> torch.Tensor:
+        c = self._inv_b.get(b)
+        if c is None:
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError("the loss scale of a new batch size cannot be created during graph capture")
+            c = self._inv_b[b] = torch.full((1,), 1.0 / b, dtype=torch.float32, device=self.device)
+        return c
+
+    def _lookup(self, t: int, f: str, x, x0: torch.Tensor, col: int, b: int):
+        """Rows of feature f into x0[:, col:col+D]; returns the update's ids of a one-hot feature (None for a bag, whose
+        pooled-row gradient _bag_grads expands)."""
+        tb = self.tables[t]
+        kind = tb.lookup_kind(x)
+        if kind == "onehot":
+            return ops.as_index(x).reshape(-1)
+        comb = tb.sequence_combiner or "mean"
+        if comb == "max":
+            raise NotImplementedError(f"feature {f!r}: training with the 'max' sequence combiner is not implemented")
+        buf = self._bag_bufs.setdefault(t, dict(rows=None, ids=None))
+        D = tb.table.shape[1]
+        if kind == "bag":
+            values, offsets = x
+            ids, offs = ops.as_index(values).reshape(-1), ops.as_index(offsets)
+            ops.gather_bag(tb.table, ids, offs, comb, x0, col, self.oob)
+        else:
+            if comb == "sqrtn":
+                raise ValueError(f"feature {f!r}: sequence_combiner 'sqrtn' is only defined for ragged inputs")
+            ids, offs = ops.as_index(x).reshape(x.shape[0], -1).contiguous(), None
+            ops.gather_seq(tb.table, ids, comb, x0, col, self.oob)
+        nnz = ids.numel()
+        if buf["rows"] is None or buf["rows"].shape[0] < nnz:  # ragged: grows to the largest batch; fixed length: b * L
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError(f"feature {f!r}: the expanded gradient buffer cannot grow during graph capture")
+            buf["rows"] = torch.empty((nnz, D), dtype=torch.float32, device=self.device)
+        if kind == "bag" and (buf["ids"] is None or buf["ids"].shape[0] < nnz or buf["ids"].dtype != ids.dtype):
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError(f"feature {f!r}: the expanded id buffer cannot grow during graph capture")
+            buf["ids"] = torch.empty(max(nnz, 1), dtype=ids.dtype, device=self.device)
+        self._bags[t] = dict(ids=ids, offsets=offs, comb=comb, rows=buf["rows"][:nnz],
+                             apply_ids=buf["ids"][:nnz] if kind == "bag" else ids.reshape(-1))
+        return None
+
+    def _tower_forward(self, tw: dict, inputs, b: int) -> torch.Tensor:
+        d = tw["d"]
+        x0 = tw["x0"][:b, :d]
+        one_w, one_i, one_c = [], [], []
+        for t, f in zip(tw["tidx"], tw["feats"]):
+            ids = self._lookup(t, f, get_feature(inputs, f), x0, tw["cols"][f], b)
+            self._idx[t] = ids
+            if ids is not None:
+                one_w.append(self.tables[t].table)
+                one_i.append(ids)
+                one_c.append(tw["cols"][f])
+        if one_w:
+            if len({i.dtype for i in one_i}) > 1:
+                one_i = [i.to(torch.int64) for i in one_i]
+                for t, i in zip([t for t in tw["tidx"] if self._idx[t] is not None], one_i):
+                    self._idx[t] = i
+            ops.gather_multi(one_w, one_i, one_c, x0, self.oob)
+        if tw["cont"]:
+            ops.concat_columns([inputs[n] for n in tw["cont"]], x0, [tw["cols"][n] for n in tw["cont"]])
+        ops.split_rows(x0, out=tw["xs"][:b])
+        op, K = tw["xs"][:b], d
+        n = len(tw["layers"])
+        for i, l in enumerate(tw["layers"]):
+            nxt = tw["h_split"][i][:b] if i < n - 1 else None
+            ops.dense_tc(op, K, self._wsplit[tw["li0"] + i], l.units, l.bias, l.activation, out_f32=tw["h"][i][:b], out_split=nxt)
+            op, K = nxt, l.units
+        out = tw["h"][-1][:b]
+        if self.l2:
+            out = ops.l2_normalize(out, out=tw["y"][:b])
+        ops.split_rows(out, out=tw["split"][:b])
+        return out
+
+    def _tower_backward(self, tw: dict, dout: torch.Tensor, b: int) -> None:
+        """dout: gradient of the tower's (normalised) output, overwritten by the pre-activation gradient of the last layer."""
+        a = self.arena
+        h, dh, layers = [x[:b] for x in tw["h"]], [x[:b] for x in tw["dh"]], tw["layers"]
+        n = len(layers)
+        if self.l2:
+            ops.l2_normalize_backward(h[-1], dout, dout)
+        if layers[-1].activation == "relu":
+            ops.relu_mask(dout, h[-1])
+        dh[-1] = dout
+        for i in range(n - 1, -1, -1):
+            li = tw["li0"] + i
+            if i > 0:
+                ops.dense_wgrad(h[i - 1], dh[i], a.view(a.grad, li, "kernel"), a.view(a.grad, li, "bias"))
+                self._dgrad(li, layers[i], dh[i], dh[i - 1], h[i - 1] if layers[i - 1].activation == "relu" else None)
+            else:
+                ops.dense_wgrad_split(tw["xs"][:b], tw["d"], dh[0], a.view(a.grad, li, "kernel"), a.view(a.grad, li, "bias"))
+                if tw["dx0"] is not None:
+                    dx0 = tw["dx0"][:b, :tw["d"]]
+                    self._dgrad(li, layers[0], dh[0], dx0, None)
+                    slices = [(self._slices[t], tw["cols"][f]) for t, f in zip(tw["tidx"], tw["feats"])]
+                    for s in range(0, len(slices), CONCAT_MAX_SLICES):
+                        ops.concat_backward([dx0], slices[s:s + CONCAT_MAX_SLICES])
+
+    def forward_backward(self, inputs: Dict[str, torch.Tensor], targets=None, sample_weight=None) -> None:
+        """Forward (activations saved), in-batch soft-max cross-entropy and backward: fills the gradient arena and the
+        IndexedSlices.  `targets` are ignored: the task's target is the positive on column 0 of every row."""
+        if sample_weight is not None and not (isinstance(sample_weight, (list, tuple)) and all(s is None for s in sample_weight)):
+            raise NotImplementedError("sample_weight is not implemented in the two-tower training step")
+        b = batch_size_of(inputs)
+        self._check_targets(targets, b)
+        self._loss_all.zero_()
+        self._idx: List[Optional[torch.Tensor]] = [None] * len(self.tables)
+        self._bags = {}
+        self._slices = [s[:b] for s in self.slices]
+        q = self._tower_forward(self.towers[0], inputs, b)
+        it = self._tower_forward(self.towers[1], inputs, b)
+        qs, its = self.towers[0]["split"][:b], self.towers[1]["split"][:b]
+        ids = inputs[self.item_id].reshape(-1) if self.downscore else None
+        T = self.temperature
+        ops.positive_scores(q, it, self.pos_logit[:b], temperature=T)
+        ops.inbatch_softmax_ce_split(qs, its, self.D, self.pos_logit[:b], self.stats[:b], self.ws, pos_ids=ids, neg_ids=ids,
+                                     downscore=self.downscore, false_neg_score=self.false_neg_score, temperature=T)
+        # dq -> the query tower's last dh, d_item = dpos + dneg (the negatives are the positives) -> the item tower's
+        dq, di = self.towers[0]["dh"][-1][:b], self.towers[1]["dh"][-1][:b]
+        ops.inbatch_softmax_ce_backward(qs, its, self.D, self.stats[:b], q, it, self._scale(b), dq, di, di, loss=self._loss_all[:1],
+                                        pos_ids=ids, neg_ids=ids, downscore=self.downscore, false_neg_score=self.false_neg_score,
+                                        temperature=T)
+        for tw, dout in zip(self.towers, (dq, di)):
+            self._tower_backward(tw, dout, b)
+        for t, bg in self._bags.items():
+            ops.bag_grad_rows(self._slices[t], bg["ids"], bg["offsets"], self.tables[t].table.shape[0], bg["comb"], bg["rows"],
+                              out_ids=bg["apply_ids"] if bg["offsets"] is not None else None)
+        self._b = b
+
+    def apply_gradients(self) -> None:
+        a = self.arena
+        ops.opt_tick(self.hyper)
+        ops.dense_apply(self.opt.kind, a.w, a.grad, a.state1, a.state2, self.hyper)
+        for D, ts in self._by_width.items():
+            onehot = [t for t in ts if t not in self._bags]
+            for s in range(0, len(onehot), SPARSE_MAX_TABLES):
+                chunk = onehot[s:s + SPARSE_MAX_TABLES]
+                ops.sparse_rows_apply(self.opt.kind, [self._table_args(t, self._idx[t], self._slices[t]) for t in chunk], self._b, D,
+                                      self.hyper)
+            for t in ts:
+                bag = self._bags.get(t)
+                if bag is not None and bag["rows"].shape[0] > 0:
+                    tab = self._table_args(t, bag["apply_ids"], bag["rows"])
+                    ops.sparse_rows_apply(self.opt.kind, [tab], bag["rows"].shape[0], D, self.hyper)
+        self._refresh_operands()
+
+
+def trainer_for(model, optimizer: Optimizer, batch_size: int, group=None):
+    """The training engine of `model`: DLRMTrainer or DCNTrainer by the ranking body, TwoTowerTrainer for a RetrievalModel."""
+    from .models import DCNBody, RetrievalModel, RetrievalModelV2
+
+    if isinstance(model, RetrievalModelV2):
+        raise NotImplementedError("training TwoTowerModelV2 / ContrastiveOutput is not implemented: train the v1 TwoTowerModel")
+    if isinstance(model, RetrievalModel):
+        return TwoTowerTrainer(model, optimizer, batch_size, group=group)
     if isinstance(getattr(model, "body", None), DCNBody):
         return DCNTrainer(model, optimizer, batch_size, group=group)
     return DLRMTrainer(model, optimizer, batch_size, group=group)
