@@ -18,6 +18,7 @@ from models_b200 import datasets, ops
 from oracle import oracle_train
 from tests import helpers as H
 from tests.golden import replay
+from tests.test_gpu_lookup_v2 import pack_ids
 
 pytestmark = pytest.mark.gpu
 G = Path(__file__).parent / "golden"
@@ -194,14 +195,17 @@ def test_interact_backward_out_of_range_ids_read_zero_rows(device):
 @pytest.mark.parametrize("D", [16, 64, 128])
 @pytest.mark.parametrize("dense_path", [False, True])
 def test_sparse_rows_apply_sums_duplicates_and_updates_once(device, opt, D, dense_path):
-    """Election path (dense_grad = None) and dense-accumulator path (sort + run sums for the 7- and 300-row tables, vector
-    reds for the 5 000-row one) give the same update."""
+    """Election path (dense_grad = None) and dense-accumulator path (sort + run sums for the 7-, 300- and 200-row tables,
+    vector reds for the 5 000-row ones) give the same update, at every id width (int32, int64, uint16, and the packed
+    uint8 and 3-byte columns of a host batch) in one call."""
     rng = np.random.default_rng(5)
     B = 3000
-    rows = [7, 5000, 300]  # 7 rows: every id repeats hundreds of times
+    rows = [7, 5000, 300, 200, 5000, 300]  # 7 rows: every id repeats hundreds of times
     W = [rng.normal(size=(r, D)).astype(np.float32) for r in rows]
     ids = [rng.integers(0, r, B) for r in rows]
     ids[1][:10] = [-3, 5000, 6000, 1, 1, 1, 2, 2, 4999, 0]  # out of range ids are dropped
+    ids[4][:10] = [(1 << 24) - 3, 5000, 6000, 1, 1, 1, 2, 2, 4999, 0]  # (-3 as a 3-byte id)
+    ids[3][:3] = [200, 255, 199]  # 1-byte ids past the table's 200 rows
     vals = [rng.normal(size=(B, D)).astype(np.float32) for _ in rows]
     hyper_cfg = dict(lr=0.05, beta_1=0.9, beta_2=0.999, epsilon=1e-7)
     o = {"sgd": mm.SGD(0.05), "adagrad": mm.Adagrad(0.05), "adam": mm.Adam(0.05)}[opt]
@@ -212,16 +216,19 @@ def test_sparse_rows_apply_sums_duplicates_and_updates_once(device, opt, D, dens
     rep = [ops.fill_i32(torch.empty(r, dtype=torch.int32, device=device), 2**31 - 1) for r in rows]
     mirror = [ops.split_rows(w) if D == 64 else None for w in dev_w]
     dense = [torch.zeros_like(w) if dense_path else None for w in dev_w]
-    dt = [torch.int32, torch.int64, torch.uint16]
+    widths = [4, 8, 2, 1, 3, 3]  # id bytes per table
     st = [{"a": np.full(w.shape, o.initial_accumulator_value), "m": np.zeros(w.shape), "v": np.zeros(w.shape)} for w in W]
     st = [{k: v for k, v in s.items() if (opt == "adagrad" and k == "a") or (opt == "adam" and k in "mv")} for s in st]
     ref = [w.astype(np.float64) for w in W]
+    n = len(rows)
     for step in (1, 2):
         ops.opt_tick(hyper)
-        tabs = [dict(weights=dev_w[t], indices=torch.from_numpy(ids[t]).to(dt[t]).to(device), grad_rows=torch.from_numpy(vals[t].copy()).to(device),
-                     rep_map=rep[t], state1=s1[t], state2=s2[t], mirror=mirror[t], dense_grad=dense[t]) for t in range(3)]
+        tabs = [dict(weights=dev_w[t], indices=torch.from_numpy(pack_ids(ids[t], widths[t])).to(device),
+                     grad_rows=torch.from_numpy(vals[t].copy()).to(device), rep_map=rep[t], state1=s1[t], state2=s2[t], mirror=mirror[t],
+                     dense_grad=dense[t]) for t in range(n)]
+        assert [ops.index_bytes_of(tb["indices"]) for tb in tabs] == widths
         ops.sparse_rows_apply(opt, tabs, B, D, hyper)
-        for t in range(3):
+        for t in range(n):
             kw = dict(hyper_cfg, step=step)
             lr = kw.pop("lr")
             ref[t] = oracle_train.sparse_update(opt, ref[t], ids[t], vals[t], st[t], lr, **kw)
