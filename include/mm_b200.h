@@ -585,6 +585,48 @@ int mm_deepfm_head(const mm_lookup_table* tables_host, const int64_t* wide_offse
                    const float* wide_kernel, const float* wide_bias, const float* addend, int64_t addend_stride,
                    const float* out_w, const float* out_b, int out_act, float* out, int32_t* oob_count, void* stream);
 
+/* Added with DeepFM training; no existing entry point changed.  With the forward's notation, u = h.w_dl + b_dl the deep
+ * logit's pre-activation, s = pairwise + wide + act_dl(u), z = s * out_w + out_b and delta = dloss/dz (as
+ * mm_heads_fwd_bwd: BCE sw (sigmoid(z) - y) / B, MSE sw 2 (z - y) / B):
+ *   mm_deepfm_head_fwd_bwd  forward, loss and backward of the head in one pass over the batch.  The embedding rows are read
+ *       from the gathered x0 (B, x0_stride) at emb_cols_host[f] (no second lookup); tables_host[f] gives feature f's ids
+ *       (idx_bytes 1, 2, 3, 4, 8), its rows and its block's first row in the wide kernel.  Writes logits (B,) = z,
+ *       ds (B,) = delta out_w, dh (B, units) = du w_dl (zeroed where h <= 0 when mask_h), du = ds act_dl'(u);
+ *       ACCUMULATES loss (2,) += [loss, loss] (total and the one output's), *dw_out += sum delta s, *db_out += sum delta,
+ *       dw_dl (units,) += sum du h, *db_dl += sum du, *d_wide_bias += sum ds, d_cont (n_cont,) += sum ds x_c (each of
+ *       these nullable).  An id outside [0, rows) adds no wide term and bumps *oob_count (its x0 row is the gather's zero
+ *       row).  out_w / out_b / wide_bias / b_dl: DEVICE scalars.  units <= 512; act_dl linear or relu.
+ *   mm_fm_concat_backward   the FM term's gradient into the embedding rows, added to mm_concat_backward's sum:
+ *       dst_t[b, :] = sum_a addend_a[b, col_t : col_t + D] + ds[b] (S_t,b - x0[b, col_t : col_t + D]), S_t,b the sum of
+ *       that x0 slice.  Every slice has the same width D (1..128); 0..4 addends; no alignment beyond fp32.
+ *   mm_wide_rows_apply      optimizer step of DeepFM's wide kernel (wide_rows, 1) by the rule of mm_sparse_rows_apply:
+ *       block i covers rows [offset, offset + rows) and is addressed by the batch's ids of feature i; every block's gradient
+ *       values are grad (B,) (the ds of mm_deepfm_head_fwd_bwd).  Duplicates are summed, each touched row gets one
+ *       update, untouched rows and their slots do not move (LazyAdam), ids outside [0, rows) are dropped.  acc (wide_rows,)
+ *       fp32 all zero and rep_map (wide_rows,) int32 all INT32_MAX between calls.  The n_dense rows at dense_offsets_host
+ *       (the continuous columns' rows) and the bias (nullable; its slots bias_state1 / bias_state2) take the dense rule
+ *       with the gradients dense_grad (n_dense [+ 1],), which are then cleared.  Blocks must not overlap. */
+typedef struct {
+  const void* indices; /* (B,) ids, idx_bytes each (1, 2, 3, 4, 8) */
+  int64_t rows;
+  int64_t offset;      /* first row of the block in the wide kernel */
+  int32_t idx_bytes;
+  int32_t reserved;
+} mm_wide_block;
+int mm_deepfm_head_fwd_bwd(const float* x0, int64_t x0_stride, const int64_t* emb_cols_host, int D, const mm_wide_block* tables_host,
+                           int n_tables, const mm_concat_piece* cont_host, const int64_t* cont_offsets_host, int n_cont,
+                           const float* wide_kernel, const float* wide_bias, const float* h, int64_t h_stride, int units, int mask_h,
+                           const float* w_dl, const float* b_dl, int act_dl, const float* out_w, const float* out_b, int loss_kind,
+                           const void* targets, int target_dtype, const float* sample_weight, int64_t B, float* logits, float* loss,
+                           float* ds, float* dh, int64_t dh_stride, float* dw_out, float* db_out, float* dw_dl, float* db_dl,
+                           float* d_wide_bias, float* d_cont, int32_t* oob_count, void* stream);
+int mm_fm_concat_backward(const float* const* addends_host, const int64_t* addend_strides_host, int n_addends, int64_t B, int d,
+                          const float* x0, int64_t x0_stride, const float* ds, const mm_column_slice* slices_host, int n_slices,
+                          void* stream);
+int mm_wide_rows_apply(float* wide, float* state1, float* state2, int64_t wide_rows, const mm_wide_block* blocks_host, int n_blocks,
+                       int64_t B, const float* grad, float* acc, int32_t* rep_map, const int64_t* dense_offsets_host, int n_dense,
+                       float* dense_grad, float* bias, float* bias_state1, float* bias_state2, int opt, const float* hyper, void* stream);
+
 /* ---------------------------------------------------------------------------------------
  * K16  Training step of the two-tower path (TwoTowerModel + ItemRetrievalTask, prediction_tasks/retrieval.py:33-191;
  * CategoricalCrossentropy(from_logits=True) against the one-hot on column 0, losses/listwise.py:38-50).  Added with

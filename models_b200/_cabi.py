@@ -65,6 +65,18 @@ class SparseTable(C.Structure):
     ]
 
 
+class WideBlock(C.Structure):
+    """mm_wide_block (include/mm_b200.h)."""
+
+    _fields_ = [
+        ("indices", C.c_void_p),
+        ("rows", C.c_int64),
+        ("offset", C.c_int64),
+        ("idx_bytes", C.c_int32),
+        ("reserved", C.c_int32),
+    ]
+
+
 OPTIMIZERS = {"sgd": 0, "adagrad": 1, "adam": 2}
 LOSS_KINDS = {"binary_crossentropy": 0, "mse": 1}  # MM_LOSS_BCE / MM_LOSS_MSE
 HYPER_LR, HYPER_BETA1, HYPER_BETA2, HYPER_EPS, HYPER_STEP, HYPER_LR_T, HYPER_COUNT = 0, 1, 2, 3, 4, 5, 8
@@ -167,6 +179,13 @@ SIGNATURES = {
     "mm_inbatch_softmax_ce_backward": (_i, [_vp, _vp, _i64, _i64, _i, _vp, _vp, _i, _i, _f, _vp, _f, _vp, _vp, _vp, _vp, _i,
                                             _vp, _vp, _vp, _vp, _vp]),
     "mm_l2_normalize_backward": (_i, [_vp, _vp, _i64, _i, _i64, _i64, _vp, _i64, _vp]),
+    "mm_deepfm_head_fwd_bwd": (_i, [_vp, _i64, C.POINTER(C.c_int64), _i, C.POINTER(WideBlock), _i, C.POINTER(ConcatPiece),
+                                    C.POINTER(C.c_int64), _i, _vp, _vp, _vp, _i64, _i, _i, _vp, _vp, _i, _vp, _vp, _i, _vp, _i, _vp,
+                                    _i64, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "mm_fm_concat_backward": (_i, [C.POINTER(C.c_void_p), C.POINTER(C.c_int64), _i, _i64, _i, _vp, _i64, _vp, C.POINTER(ColumnSlice),
+                                   _i, _vp]),
+    "mm_wide_rows_apply": (_i, [_vp, _vp, _vp, _i64, C.POINTER(WideBlock), _i, _i64, _vp, _vp, _vp, C.POINTER(C.c_int64), _i, _vp,
+                                _vp, _vp, _vp, _i, _vp, _vp]),
 }
 
 

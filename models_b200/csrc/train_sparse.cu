@@ -886,6 +886,144 @@ static void launch_bag_grad(unsigned blocks, cudaStream_t st, const float* g, lo
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Wide kernel of DeepFM (mm_wide_rows_apply): a (sum of cardinalities + n_cont, 1) Keras kernel whose feature blocks are
+// disjoint row ranges; every block's gradient values are the one (B,) vector g (dloss/ds), so no (B, T) slice array exists.
+// Scatter (blockIdx.y = block, CTAs stride chunks of WIDE_CHUNK samples): the lanes of a warp holding the same row are
+// found with match.any and summed by their leader, which adds ONE value per row and warp:
+//   small blocks (rows <= WIDE_SMALL_ROWS): into a per-CTA shared accumulator, flushed with one global add per touched row
+//     and CTA at the end (a 4-row Criteo feature is hit 16 000 times per batch);
+//   other blocks: straight into the (rows,) accumulator `acc`, and atomicMin(rep[row], b) elects the smallest sample.
+// Apply: blocks of <= WIDE_DENSE_ROWS rows walk their rows (rep != INT_MAX marks a touched row); larger blocks walk the
+// samples and the elected sample updates its row.  Either clears acc and rep.  The continuous rows and the bias are
+// touched by every step and take the dense rule (wide_dense_apply_kernel).
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int WIDE_MAX_BLOCKS = 64;
+constexpr int WIDE_CHUNK = 2048;
+constexpr int WIDE_SMALL_ROWS = 2048;
+constexpr long long WIDE_DENSE_ROWS = 131072;
+constexpr int WIDE_MAX_DENSE = 64;
+struct WideBlock {
+  const void* ids;
+  long long rows;
+  long long off;
+  int idx_bytes;
+};
+struct WideParams {
+  WideBlock blk[WIDE_MAX_BLOCKS];
+  long long dense_off[WIDE_MAX_DENSE];
+  int n_dense;
+  float* w;
+  float* s1;
+  float* s2;
+  float* acc;
+  int* rep;
+  const float* g;
+  float* dgrad;  // (n_dense [+ 1 for the bias],)
+  float* bias;
+  float* bs1;
+  float* bs2;
+  long long B;
+  int opt;
+  const float* hyper;
+};
+
+__global__ void __launch_bounds__(256) wide_scatter_kernel(const __grid_constant__ WideParams p) {
+  __shared__ float sacc[WIDE_SMALL_ROWS];
+  __shared__ int stouch[WIDE_SMALL_ROWS];
+  const WideBlock& bk = p.blk[blockIdx.y];
+  const bool small = bk.rows <= WIDE_SMALL_ROWS;
+  const int lane = threadIdx.x & 31;
+  if (small) {
+    for (int r = threadIdx.x; r < bk.rows; r += blockDim.x) {
+      sacc[r] = 0.0f;
+      stouch[r] = 0;
+    }
+    __syncthreads();
+  }
+  const long long n_chunks = (p.B + WIDE_CHUNK - 1) / WIDE_CHUNK;
+  for (long long ch = blockIdx.x; ch < n_chunks; ch += gridDim.x) {
+    for (int i = 0; i < WIDE_CHUNK; i += 256) {  // uniform trip count: every lane reaches match.any
+      const long long b = ch * WIDE_CHUNK + i + threadIdx.x;
+      long long row = -1;
+      float v = 0.0f;
+      if (b < p.B) {
+        const unsigned long long id = (unsigned long long)load_id(bk.ids, bk.idx_bytes, b);
+        if (id < (unsigned long long)bk.rows) {
+          row = (long long)id;
+          v = p.g[b];
+        }
+      }
+      const unsigned grp = __match_any_sync(0xffffffffu, (unsigned long long)row);
+      if (row < 0) continue;
+      float s = 0.0f;
+      for (unsigned m = grp; m; m &= m - 1) s += __shfl_sync(grp, v, __ffs(m) - 1);
+      if (lane != __ffs(grp) - 1) continue;
+      if (small) {
+        atomicAdd(&sacc[row], s);
+        stouch[row] = 1;
+      } else {
+        atomicAdd(p.acc + bk.off + row, s);
+        atomicMin(p.rep + bk.off + row, (int)b);  // the leader is the group's smallest sample
+      }
+    }
+  }
+  if (small) {
+    __syncthreads();
+    for (int r = threadIdx.x; r < bk.rows; r += blockDim.x)
+      if (stouch[r]) {
+        atomicAdd(p.acc + bk.off + r, sacc[r]);
+        atomicMin(p.rep + bk.off + r, 0);
+      }
+  }
+}
+
+__device__ __forceinline__ void wide_update(int opt, float* w, float* s1, float* s2, float g, const Hyper& hy) {
+  float a = opt != MM_OPT_SGD ? *s1 : 0.0f, v = opt == MM_OPT_ADAM ? *s2 : 0.0f;
+  *w = upd(opt, *w, g, a, v, hy);
+  if (opt != MM_OPT_SGD) *s1 = a;
+  if (opt == MM_OPT_ADAM) *s2 = v;
+}
+
+__global__ void __launch_bounds__(256) wide_apply_kernel(const __grid_constant__ WideParams p) {
+  const WideBlock& bk = p.blk[blockIdx.y];
+  const Hyper hy = load_hyper(p.hyper);
+  const long long t0 = (long long)blockIdx.x * blockDim.x + threadIdx.x, stride = (long long)gridDim.x * blockDim.x;
+  if (bk.rows <= WIDE_DENSE_ROWS) {
+    for (long long r = t0; r < bk.rows; r += stride) {
+      const long long i = bk.off + r;
+      if (p.rep[i] == INT_MAX) continue;
+      wide_update(p.opt, p.w + i, p.s1 + i, p.s2 + i, p.acc[i], hy);
+      p.acc[i] = 0.0f;
+      p.rep[i] = INT_MAX;
+    }
+  } else {
+    for (long long b = t0; b < p.B; b += stride) {
+      const unsigned long long id = (unsigned long long)load_id(bk.ids, bk.idx_bytes, b);
+      if (id >= (unsigned long long)bk.rows) continue;
+      const long long i = bk.off + (long long)id;
+      if (p.rep[i] != (int)b) continue;  // another sample holds the row (or already updated it: INT_MAX)
+      wide_update(p.opt, p.w + i, p.s1 + i, p.s2 + i, p.acc[i], hy);
+      p.acc[i] = 0.0f;
+      p.rep[i] = INT_MAX;
+    }
+  }
+}
+
+// the continuous columns' rows and the bias: one thread each
+__global__ void wide_dense_apply_kernel(const __grid_constant__ WideParams p) {
+  const int t = threadIdx.x;
+  const Hyper hy = load_hyper(p.hyper);
+  if (t < p.n_dense) {
+    const long long i = p.dense_off[t];
+    wide_update(p.opt, p.w + i, p.s1 + i, p.s2 + i, p.dgrad[t], hy);
+    p.dgrad[t] = 0.0f;
+  } else if (t == p.n_dense && p.bias) {
+    wide_update(p.opt, p.bias, p.bs1, p.bs2, p.dgrad[t], hy);
+    p.dgrad[t] = 0.0f;
+  }
+}
+
 __global__ void opt_tick_kernel(float* hyper) {
   const float t = hyper[MM_HYPER_STEP] + 1.0f;
   hyper[MM_HYPER_STEP] = t;
@@ -1100,6 +1238,80 @@ int mm_bag_grad_rows(const float* g, int64_t B, int D, int64_t g_stride, const v
   else if (o64) launch_bag_grad<int, long long>((unsigned)blocks, st, g, g_stride, ids, offsets, L, B, nnz, rows, combiner, D, out, out_ids);
   else launch_bag_grad<int, int>((unsigned)blocks, st, g, g_stride, ids, offsets, L, B, nnz, rows, combiner, D, out, out_ids);
   return mm::check_launch("mm_bag_grad_rows");
+}
+
+int mm_wide_rows_apply(float* wide, float* state1, float* state2, int64_t wide_rows, const mm_wide_block* blocks_host, int n_blocks,
+                       int64_t B, const float* grad, float* acc, int32_t* rep_map, const int64_t* dense_offsets_host, int n_dense,
+                       float* dense_grad, float* bias, float* bias_state1, float* bias_state2, int opt, const float* hyper, void* stream) {
+  using namespace mm;
+  using namespace mm::trs;
+  MM_REQUIRE(wide && blocks_host && grad && acc && rep_map && hyper && B >= 0 && wide_rows > 0, MM_ERR_ARG,
+             "mm_wide_rows_apply: null pointer or bad size");
+  MM_REQUIRE(n_blocks >= 1 && n_blocks <= WIDE_MAX_BLOCKS && n_dense >= 0 && n_dense <= WIDE_MAX_DENSE, MM_ERR_UNSUPPORTED,
+             "mm_wide_rows_apply: 1..%d feature blocks and 0..%d dense rows", WIDE_MAX_BLOCKS, WIDE_MAX_DENSE);
+  MM_REQUIRE(opt == MM_OPT_SGD || opt == MM_OPT_ADAGRAD || opt == MM_OPT_ADAM, MM_ERR_ARG, "mm_wide_rows_apply: unknown optimizer %d", opt);
+  MM_REQUIRE(opt == MM_OPT_SGD || (state1 && (!bias || bias_state1)), MM_ERR_ARG, "mm_wide_rows_apply: optimizer state missing");
+  MM_REQUIRE(opt != MM_OPT_ADAM || (state2 && (!bias || bias_state2)), MM_ERR_ARG, "mm_wide_rows_apply: second optimizer state missing");
+  MM_REQUIRE((n_dense == 0 && !bias) || (dense_grad && (n_dense == 0 || dense_offsets_host)), MM_ERR_ARG,
+             "mm_wide_rows_apply: dense rows or a bias without dense_grad / offsets");
+  MM_REQUIRE(B < (int64_t)INT_MAX, MM_ERR_UNSUPPORTED, "mm_wide_rows_apply: batch too large for the int32 representative map");
+  WideParams p;
+  memset(&p, 0, sizeof(p));
+  for (int i = 0; i < n_blocks; ++i) {
+    const mm_wide_block& s = blocks_host[i];
+    if (const int rc = check_id_column("mm_wide_rows_apply", i, s.indices, s.idx_bytes, s.rows)) return rc;
+    MM_REQUIRE(s.offset >= 0 && s.offset + s.rows <= wide_rows, MM_ERR_ARG, "mm_wide_rows_apply: block %d: rows outside the wide kernel", i);
+    for (int j = 0; j < i; ++j)
+      MM_REQUIRE(s.offset >= blocks_host[j].offset + blocks_host[j].rows || blocks_host[j].offset >= s.offset + s.rows, MM_ERR_ARG,
+                 "mm_wide_rows_apply: blocks %d and %d overlap", j, i);
+    p.blk[i].ids = s.indices;
+    p.blk[i].rows = s.rows;
+    p.blk[i].off = s.offset;
+    p.blk[i].idx_bytes = s.idx_bytes;
+  }
+  for (int c = 0; c < n_dense; ++c) {
+    MM_REQUIRE(dense_offsets_host[c] >= 0 && dense_offsets_host[c] < wide_rows, MM_ERR_ARG, "mm_wide_rows_apply: dense row %d outside the wide kernel", c);
+    for (int i = 0; i < n_blocks; ++i)
+      MM_REQUIRE(dense_offsets_host[c] < blocks_host[i].offset || dense_offsets_host[c] >= blocks_host[i].offset + blocks_host[i].rows,
+                 MM_ERR_ARG, "mm_wide_rows_apply: dense row %d lies in block %d", c, i);
+    p.dense_off[c] = dense_offsets_host[c];
+  }
+  p.n_dense = n_dense;
+  p.w = wide;
+  p.s1 = state1;
+  p.s2 = state2;
+  p.acc = acc;
+  p.rep = rep_map;
+  p.g = grad;
+  p.dgrad = dense_grad;
+  p.bias = bias;
+  p.bs1 = bias_state1;
+  p.bs2 = bias_state2;
+  p.B = B;
+  p.opt = opt;
+  p.hyper = hyper;
+  cudaStream_t st = (cudaStream_t)stream;
+  long long sx = (B + WIDE_CHUNK - 1) / WIDE_CHUNK;
+  long long scap = 2LL * sm_count() / n_blocks;
+  if (scap < 1) scap = 1;
+  if (sx > scap) sx = scap;
+  if (sx >= 1) {
+    wide_scatter_kernel<<<dim3((unsigned)sx, (unsigned)n_blocks), 256, 0, st>>>(p);
+    if (const int rc = check_launch("mm_wide_rows_apply(scatter)")) return rc;
+  }
+  long long span = B;
+  for (int i = 0; i < n_blocks; ++i)
+    if (blocks_host[i].rows <= WIDE_DENSE_ROWS && blocks_host[i].rows > span) span = blocks_host[i].rows;
+  long long ax = (span + 255) / 256;
+  long long acap = 4LL * sm_count() / n_blocks;
+  if (acap < 1) acap = 1;
+  if (ax > acap) ax = acap;
+  if (ax < 1) ax = 1;
+  wide_apply_kernel<<<dim3((unsigned)ax, (unsigned)n_blocks), 256, 0, st>>>(p);
+  if (const int rc = check_launch("mm_wide_rows_apply(apply)")) return rc;
+  if (n_dense == 0 && !bias) return MM_OK;
+  wide_dense_apply_kernel<<<1, 96, 0, st>>>(p);
+  return check_launch("mm_wide_rows_apply(dense rows)");
 }
 
 int mm_fill_i32(int32_t* p, int64_t n, int32_t value, void* stream) {

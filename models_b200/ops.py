@@ -1230,3 +1230,136 @@ def deepfm_head(weights, indices, wide_offsets, cont, cont_offsets, wide_kernel:
                               _ptr(out_w), _ptr(out_b), ACTIVATIONS[out_act], out.data_ptr(), _ptr(oob), _stream()),
         "mm_deepfm_head")
     return out
+
+
+# ---- DeepFM training (include/mm_b200.h, added with DeepFM training) ------------------------------------------------
+def _wide_blocks(indices, rows, offsets, B: int):
+    n = len(indices)
+    if not (len(rows) == n and len(offsets) == n):
+        raise ValueError("indices / rows / offsets length mismatch")
+    arr = (_cabi.WideBlock * max(n, 1))()
+    for t in range(n):
+        ix = _dev(indices[t], f"indices[{t}]")
+        w = index_bytes_of(ix)
+        if ix.shape[0] != B or not ix.is_contiguous() or (ix.numel() != B * (3 if w == 3 else 1)):
+            raise ValueError(f"indices[{t}] must be {B} contiguous ids, got {tuple(ix.shape)}")
+        arr[t].indices, arr[t].rows, arr[t].offset, arr[t].idx_bytes = ix.data_ptr(), int(rows[t]), int(offsets[t]), w
+    return arr, n
+
+
+def deepfm_head_fwd_bwd(x0: torch.Tensor, emb_cols, D: int, indices, rows, wide_offsets, cont, cont_offsets,
+                        wide_kernel: torch.Tensor, wide_bias: Optional[torch.Tensor], h: torch.Tensor, mask_h: bool,
+                        w_dl: torch.Tensor, b_dl: Optional[torch.Tensor], act_dl: str, out_w: torch.Tensor,
+                        out_b: Optional[torch.Tensor], loss: str, targets: torch.Tensor, sample_weight: Optional[torch.Tensor],
+                        logits: torch.Tensor, loss_buf: torch.Tensor, ds: torch.Tensor, dh: torch.Tensor,
+                        dw_out: Optional[torch.Tensor] = None, db_out: Optional[torch.Tensor] = None,
+                        dw_dl: Optional[torch.Tensor] = None, db_dl: Optional[torch.Tensor] = None,
+                        d_wide_bias: Optional[torch.Tensor] = None, d_cont: Optional[torch.Tensor] = None,
+                        oob: Optional[torch.Tensor] = None) -> None:
+    """The DeepFM head's forward, loss and backward in one pass (mm_deepfm_head_fwd_bwd).  x0 (B, d) holds the gathered
+    rows at emb_cols; indices[f] (B,) ids of any width of index_bytes_of, rows[f] its table's rows, wide_offsets[f] its
+    block in the wide kernel; cont (B,) columns at cont_offsets.  Writes logits, ds (B,) and dh (B, U); ACCUMULATES
+    loss_buf (2,) and the gradients (each nullable)."""
+    for n_, t_ in (("x0", x0), ("wide_kernel", wide_kernel), ("h", h), ("w_dl", w_dl), ("out_w", out_w), ("logits", logits),
+                   ("loss_buf", loss_buf), ("ds", ds), ("dh", dh)):
+        _dev(t_, n_, torch.float32)
+    B = x0.shape[0]
+    U = h.shape[1]
+    if h.shape[0] != B or tuple(dh.shape) != (B, U):
+        raise ValueError(f"h and dh must be ({B}, units)")
+    if not wide_kernel.is_contiguous() or w_dl.numel() != U or not w_dl.is_contiguous():
+        raise ValueError(f"wide_kernel must be contiguous and w_dl hold {U} contiguous values")
+    for n_, t_, k in (("out_w", out_w, 1), ("out_b", out_b, 1), ("b_dl", b_dl, 1), ("wide_bias", wide_bias, 1),
+                      ("dw_out", dw_out, 1), ("db_out", db_out, 1), ("db_dl", db_dl, 1), ("d_wide_bias", d_wide_bias, 1),
+                      ("dw_dl", dw_dl, U), ("d_cont", d_cont, len(cont))):
+        if t_ is not None and (_dev(t_, n_, torch.float32).numel() != k or not t_.is_contiguous()):
+            raise ValueError(f"{n_} must hold {k} contiguous float32 values")
+    if logits.numel() != B or ds.numel() != B or not logits.is_contiguous() or not ds.is_contiguous():
+        raise ValueError(f"logits and ds must hold {B} contiguous values")
+    if loss_buf.numel() != 2 or not loss_buf.is_contiguous():
+        raise ValueError("loss_buf must hold 2 contiguous values")
+    if loss not in _cabi.LOSS_KINDS:
+        raise ValueError(f"loss must be among {sorted(_cabi.LOSS_KINDS)}, got {loss!r}")
+    if act_dl not in ("linear", "relu"):
+        raise ValueError(f"the deep logit's activation must be linear or relu, got {act_dl!r}")
+    _dev(targets, "targets")
+    if targets.numel() != B or not targets.is_contiguous() or targets.dtype not in _TARGET_DTYPES:
+        raise ValueError(f"targets must be {B} contiguous int32 / int64 / float32 / float64 values")
+    if sample_weight is not None and (_dev(sample_weight, "sample_weight", torch.float32).numel() != B or not sample_weight.is_contiguous()):
+        raise ValueError(f"sample_weight must be ({B},) contiguous float32")
+    n = len(indices)
+    if len(emb_cols) != n:
+        raise ValueError("emb_cols / indices length mismatch")
+    arr, _ = _wide_blocks(indices, rows, wide_offsets, B)
+    cols = (C.c_int64 * max(n, 1))(*[int(c) for c in emb_cols])
+    m = len(cont)
+    if len(cont_offsets) != m:
+        raise ValueError("cont / cont_offsets length mismatch")
+    for c, t in enumerate(cont):
+        if _dev(t, f"cont[{c}]").numel() != B:
+            raise ValueError(f"cont[{c}] must hold {B} values")
+    carr, _, _ = _concat_pieces([t.reshape(-1) for t in cont], B, "cont")
+    coff = (C.c_int64 * max(m, 1))(*[int(o) for o in cont_offsets])
+    _cabi.check(
+        _lib().mm_deepfm_head_fwd_bwd(x0.data_ptr(), _row_stride(x0, "x0"), cols, int(D), arr, n, carr, coff, m, wide_kernel.data_ptr(),
+                                      _ptr(wide_bias), h.data_ptr(), _row_stride(h, "h"), U, 1 if mask_h else 0, w_dl.data_ptr(),
+                                      _ptr(b_dl), ACTIVATIONS[act_dl], out_w.data_ptr(), _ptr(out_b), _cabi.LOSS_KINDS[loss],
+                                      targets.data_ptr(), _TARGET_DTYPES[targets.dtype], _ptr(sample_weight), B, logits.data_ptr(),
+                                      loss_buf.data_ptr(), ds.data_ptr(), dh.data_ptr(), _row_stride(dh, "dh"), _ptr(dw_out),
+                                      _ptr(db_out), _ptr(dw_dl), _ptr(db_dl), _ptr(d_wide_bias), _ptr(d_cont), _ptr(oob), _stream()),
+        "mm_deepfm_head_fwd_bwd")
+
+
+def fm_concat_backward(addends: Sequence[torch.Tensor], x0: torch.Tensor, ds: torch.Tensor, slices: Sequence[tuple]) -> None:
+    """concat_backward plus the FM term (mm_fm_concat_backward): for each (dst (B, D), col) in `slices`,
+    dst = sum of the addends' columns [col, col + D) + ds[:, None] * (S - x0[:, col:col + D]), S the row sum of that slice."""
+    _dev(x0, "x0", torch.float32), _dev(ds, "ds", torch.float32)
+    B, d = x0.shape
+    if ds.numel() != B or not ds.is_contiguous():
+        raise ValueError(f"ds must hold {B} contiguous values")
+    n = len(addends)
+    ap, st = (C.c_void_p * max(n, 1))(), (C.c_int64 * max(n, 1))()
+    for i, a in enumerate(addends):
+        _dev(a, f"addends[{i}]", torch.float32)
+        if tuple(a.shape) != (B, d):
+            raise ValueError(f"addends[{i}] must be ({B}, {d}), got {tuple(a.shape)}")
+        ap[i], st[i] = a.data_ptr(), _row_stride(a, f"addends[{i}]")
+    arr = (_cabi.ColumnSlice * max(len(slices), 1))()
+    for t, (dst, col) in enumerate(slices):
+        _dev(dst, f"slices[{t}].dst", torch.float32)
+        if dst.dim() != 2 or dst.shape[0] != B:
+            raise ValueError(f"slices[{t}].dst must be ({B}, width), got {tuple(dst.shape)}")
+        arr[t].dst, arr[t].dst_stride, arr[t].col, arr[t].width = dst.data_ptr(), _row_stride(dst, f"slices[{t}].dst"), int(col), dst.shape[1]
+    _cabi.check(_lib().mm_fm_concat_backward(ap, st, n, B, d, x0.data_ptr(), _row_stride(x0, "x0"), ds.data_ptr(), arr, len(slices),
+                                             _stream()), "mm_fm_concat_backward")
+
+
+def wide_rows_apply(opt: str, wide: torch.Tensor, state1: Optional[torch.Tensor], state2: Optional[torch.Tensor], indices, rows,
+                    offsets, grad: torch.Tensor, acc: torch.Tensor, rep_map: torch.Tensor, dense_offsets, dense_grad: Optional[torch.Tensor],
+                    bias: Optional[torch.Tensor], bias_state1: Optional[torch.Tensor], bias_state2: Optional[torch.Tensor],
+                    hyper: torch.Tensor) -> None:
+    """Optimizer step of a wide kernel (mm_wide_rows_apply): block f = rows [offsets[f], offsets[f] + rows[f]) addressed by
+    indices[f], gradient values grad (B,) for every block; the rows at dense_offsets and the bias take the dense rule with
+    dense_grad (len(dense_offsets) [+ 1],), which is cleared."""
+    W = wide.numel()
+    for n_, t_ in (("wide", wide), ("grad", grad), ("acc", acc), ("hyper", hyper)):
+        _dev(t_, n_, torch.float32)
+    _dev(rep_map, "rep_map", torch.int32)
+    for n_, t_ in (("wide", wide), ("acc", acc), ("rep_map", rep_map), ("state1", state1), ("state2", state2)):
+        if t_ is not None and (t_.numel() != W or not t_.is_contiguous()):
+            raise ValueError(f"{n_} must hold {W} contiguous values (one per row of the wide kernel)")
+    for n_, t_ in (("state1", state1), ("state2", state2), ("bias", bias), ("bias_state1", bias_state1), ("bias_state2", bias_state2)):
+        if t_ is not None:
+            _dev(t_, n_, torch.float32)
+    B = grad.numel()
+    if not grad.is_contiguous():
+        raise ValueError("grad must be contiguous")
+    arr, n = _wide_blocks(indices, rows, offsets, B)
+    m = len(dense_offsets)
+    k = m + (1 if bias is not None else 0)
+    if k and (dense_grad is None or _dev(dense_grad, "dense_grad", torch.float32).numel() != k or not dense_grad.is_contiguous()):
+        raise ValueError(f"dense_grad must hold {k} contiguous values")
+    doff = (C.c_int64 * max(m, 1))(*[int(o) for o in dense_offsets])
+    _cabi.check(_lib().mm_wide_rows_apply(wide.data_ptr(), _ptr(state1), _ptr(state2), W, arr, n, B, grad.data_ptr(), acc.data_ptr(),
+                                          rep_map.data_ptr(), doff, m, _ptr(dense_grad), _ptr(bias), _ptr(bias_state1), _ptr(bias_state2),
+                                          _cabi.OPTIMIZERS[opt], hyper.data_ptr(), _stream()), "mm_wide_rows_apply")

@@ -26,6 +26,9 @@ DCNModel trains through DCNTrainer (below): the cross network's backward (mm_cro
 backward straight into per-table slices (mm_concat_backward) and one sparse update per distinct embedding width.
 The v1 TwoTowerModel trains through TwoTowerTrainer: both towers as DCN's input block + deep tower, the in-batch soft-max
 cross-entropy forward and backward without the (B, 1+B) logits (mm_inbatch_softmax_ce[_backward]).
+DeepFMModel trains through DeepFMTrainer: DCN's input block and deep tower, the FM / wide / output head forward and
+backward in one kernel (mm_deepfm_head_fwd_bwd), the FM term's input gradient (mm_fm_concat_backward) and the wide
+kernel's sparse update (mm_wide_rows_apply).
 
 All Dense variables of the model are re-homed into ONE flat fp32 arena (gradients and optimizer slots mirror its layout), so
 the dense update is one launch and data-parallel training needs one all-reduce.  Every buffer is static: a step can be
@@ -1247,9 +1250,234 @@ class TwoTowerTrainer(_StepTrainer):
         self._refresh_operands()
 
 
+class DeepFMTrainer(_StepTrainer):
+    """Static-buffer training step of a DeepFMModel (one BinaryOutput or RegressionOutput) at one batch size.
+
+    forward   mm_gather_multi of every table's rows + mm_concat_columns of the continuous columns into x0 (B, d) at their
+              sorted-name offsets, its split operand; mm_dense_tc per deep layer and per deep-logit layer but the last
+    head      mm_deepfm_head_fwd_bwd: FM pairwise term from x0, wide lookup, the last Dense(1) of the deep logit, the output
+              layer and the loss, forward and backward: logits, ds = dloss/ds (B,), dh, and the gradients of the deep logit,
+              the output layer (arena), the wide bias and the continuous rows of the wide kernel
+    backward  mm_dense_wgrad[_split] + dgrad per tower layer down to dx0; mm_fm_concat_backward: dx0 + ds (S_f - e_f) into
+              each table's (B, D) IndexedSlices buffer
+    update    mm_opt_tick, mm_dense_apply over the arena [deep, deep logit, output layer], mm_sparse_rows_apply (tables),
+              mm_wide_rows_apply (the wide kernel's rows: one (B,) gradient vector for every feature block; continuous rows
+              and bias by the dense rule), mm_split_weights refresh of the operand copies the model's forward reads.
+    The wide kernel (one row per category of every feature) stays where it is, its optimizer slots beside it."""
+
+    def __init__(self, model, optimizer: Optimizer, batch_size: int, device=None, group=None):
+        from .blocks import dense_engine
+        from .models import BinaryOutput, DeepFMBody
+
+        body = model.body
+        if not isinstance(body, DeepFMBody):
+            raise NotImplementedError("DeepFMTrainer trains DeepFMModel bodies")
+        if not isinstance(model.prediction, BinaryOutput):
+            raise NotImplementedError("training DeepFMModel needs one BinaryOutput or RegressionOutput")
+        if group is not None:
+            raise NotImplementedError("training DeepFMModel with a process group is not implemented")
+        if dense_engine() == "fp32":
+            raise NotImplementedError("training DeepFMModel runs on the tensor-core engine (dense_engine() == 'fp32')")
+        ib, fm = body.input_block, body.fm
+        emb = ib.embeddings
+        if getattr(emb, "sharded", None) is not None:
+            raise NotImplementedError("training DeepFMModel with row-sharded tables is not implemented")
+        if fm.embeddings is not emb:
+            raise NotImplementedError("training DeepFMModel needs the FM term to read the input block's tables")
+        for blk in (body.deep, body.deep_logit):
+            if not isinstance(blk, MLP) or blk.has_normalization or blk.dropout:
+                raise NotImplementedError("training DeepFMModel supports deep / deep-logit MLPBlocks without normalization / dropout")
+        self._init_common(model, optimizer, batch_size, device, None)
+        self._init_heads()
+        self.chain = body.deep.dense_layers + body.deep_logit.dense_layers[:-1]  # tower layers run by mm_dense_tc
+        self.last = body.deep_logit.dense_layers[-1]  # Dense(1), fused into the head kernel
+        for l in self.chain + [self.last]:
+            if l.activation not in ("relu", "linear"):
+                raise NotImplementedError(f"{l.name}: training supports relu / linear deep activations, got {l.activation!r}")
+        self.U = self.chain[-1].units
+        if self.U > 512:
+            raise NotImplementedError(f"{self.chain[-1].name}: the head kernel reads at most 512 units of the last deep layer, got {self.U}")
+
+        # ---- input block layout, tables, wide kernel
+        self.cols, widths, d = ib.layout()
+        self.d = d
+        self.feats = list(fm.cat_names)
+        self.tables = [emb.feature_to_table[f] for f in self.feats]
+        seen = set()
+        for f, t in zip(self.feats, self.tables):
+            if id(t) in seen:
+                raise NotImplementedError(f"feature {f!r}: training with a table shared between features is not implemented")
+            seen.add(id(t))
+            if not t.trainable:
+                raise NotImplementedError(f"feature {f!r}: frozen embedding tables are not implemented in the training step")
+        self.D = fm.dim
+        if self.D % 4 or self.D > 128:
+            raise NotImplementedError(f"embedding width {self.D} is not supported by the sparse update (it needs a multiple of 4 no "
+                                      "larger than 128)")
+        if len(self.feats) > 32 or len(fm.cont_names) > 32:
+            raise NotImplementedError("the DeepFM head kernel takes up to 32 categorical and 32 continuous features")
+        self.cont = list(fm.cont_names)
+        self.wk = fm.wide  # _Dense(1) over [one-hot | continuous]: kernel (W, 1), bias (1,)
+        self.woff = [fm.wide_offsets[f] for f in self.feats]
+        self.coff = [fm.wide_offsets[n] for n in self.cont]
+
+        self.arena = DenseArena(self.chain + [self.last, self.head], optimizer, self.device)
+        self._tc_layers = self.chain + [self.last]  # the last one's operand copy is what the model's forward reads
+        self._wsplit = [ops.split_weights(l.kernel) for l in self._tc_layers]
+        for l, ws in zip(self._tc_layers, self._wsplit):
+            l._w_split = ws
+        self.hyper = torch.from_numpy(optimizer.hyper()).to(self.device)
+        n = len(self.chain)
+        self._init_wide(lambda li: li < n)
+        self._init_table_state(optimizer)
+        f32 = dict(dtype=torch.float32, device=self.device)
+        W = self.wk.kernel.numel()
+        self.wk_s1 = torch.full((W,), optimizer.initial_accumulator_value, **f32) if optimizer.slots >= 1 else None
+        self.wk_s2 = torch.zeros(W, **f32) if optimizer.slots >= 2 else None
+        nb = 1 if self.wk.bias is not None else 0
+        self.wb_s1 = torch.full((nb,), optimizer.initial_accumulator_value, **f32) if optimizer.slots >= 1 and nb else None
+        self.wb_s2 = torch.zeros(nb, **f32) if optimizer.slots >= 2 and nb else None
+        self.wk_acc = torch.zeros(W, **f32)
+        self.wk_rep = ops.fill_i32(torch.empty(W, dtype=torch.int32, device=self.device), INT32_MAX)
+        self.wk_grad = torch.zeros(len(self.cont) + nb, **f32)  # [continuous rows..., bias]
+
+        # ---- activations and gradients
+        B = self.B
+        self.ld = (d + 3) // 4 * 4
+        self.x0 = torch.zeros((B, self.ld), **f32)
+        self.xs = torch.zeros((B, 2 * ops.tc_padded_k(d)), dtype=torch.bfloat16, device=self.device)
+        self.h = [torch.zeros((B, l.units), **f32) for l in self.chain]
+        self.h_split = [torch.zeros((B, 2 * ops.tc_padded_k(l.units)), dtype=torch.bfloat16, device=self.device) for l in self.chain[:-1]]
+        self.dh = [torch.zeros((B, l.units), **f32) for l in self.chain]
+        self.dx0 = torch.zeros((B, self.ld), **f32)
+        self.ds = torch.zeros(B, **f32)
+        self.slices = [torch.zeros((B, self.D), **f32) for _ in self.tables]
+        self._init_loss(B)
+        self.oob = emb.counter(self.device)
+
+    def _ids(self, inputs):
+        """(gather ids: int32 / int64, one dtype; fused ids: packed widths as given) per table."""
+        gather, fused = [], []
+        for f, tb in zip(self.feats, self.tables):
+            x = get_feature(inputs, f)
+            if tb.lookup_kind(x) != "onehot":
+                raise NotImplementedError(f"feature {f!r}: training DeepFMModel on multi-hot / ragged features is not implemented")
+            gather.append(ops.as_index(x).reshape(-1))
+            fused.append(ops.fused_ids(x))
+        if len({i.dtype for i in gather}) > 1:
+            gather = [i.to(torch.int64) for i in gather]
+        return gather, fused
+
+    def forward_backward(self, inputs: Dict[str, torch.Tensor], targets, sample_weight=None) -> None:
+        """Forward (activations saved), loss and backward: fills the gradient arena, the IndexedSlices of the tables, ds (the
+        wide kernel's gradient values) and the gradients of the wide kernel's continuous rows and bias.  Batches smaller
+        than the compiled size run in the leading rows of the same buffers."""
+        a = self.arena
+        d, n = self.d, len(self.chain)
+        self._loss_all.zero_()
+        b = batch_size_of(inputs)
+        targets = self._check_targets(targets, b)
+        if isinstance(sample_weight, (list, tuple)):
+            sample_weight = sample_weight[0]
+        gidx, fidx = self._ids(inputs)
+
+        def v(t):
+            return t[:b]
+
+        x0 = self.x0[:b, :d]
+        ops.gather_multi([tb.table for tb in self.tables], gidx, [self.cols[f] for f in self.feats], x0, self.oob)
+        conts = [inputs[c] for c in self.cont]
+        if conts:
+            ops.concat_columns(conts, x0, [self.cols[c] for c in self.cont])
+        xs = v(self.xs)
+        ops.split_rows(x0, out=xs)
+        h, dh = [v(t) for t in self.h], [v(t) for t in self.dh]
+        op, K = xs, d
+        for i, l in enumerate(self.chain):
+            nxt = v(self.h_split[i]) if i < n - 1 else None
+            ops.dense_tc(op, K, self._wsplit[i], l.units, l.bias, l.activation, out_f32=h[i], out_split=nxt)
+            op, K = nxt, l.units
+        # -- FM + wide + deep logit + output layer + loss, forward and backward
+        hi = len(a.layers) - 1
+        ds = v(self.ds)
+        nc = len(self.cont)
+        ops.deepfm_head_fwd_bwd(
+            x0, [self.cols[f] for f in self.feats], self.D, fidx, [tb.table.shape[0] for tb in self.tables], self.woff, conts,
+            self.coff, self.wk.kernel.reshape(-1), self.wk.bias, h[-1], self.chain[-1].activation == "relu", self.last.kernel.reshape(-1),
+            self.last.bias, self.last.activation, self.head.kernel.reshape(-1), self.head.bias, self.losses[0], targets[0].reshape(-1),
+            sample_weight, v(self.logits), self._loss_all, ds, dh[-1], dw_out=a.view(a.grad, hi, "kernel"), db_out=a.view(a.grad, hi, "bias"),
+            dw_dl=a.view(a.grad, n, "kernel"), db_dl=a.view(a.grad, n, "bias"),
+            d_wide_bias=self.wk_grad[nc:] if self.wk.bias is not None else None, d_cont=self.wk_grad[:nc] if nc else None, oob=self.oob)
+        # -- deep tower backward down to dx0
+        dx0 = self.dx0[:b, :d]
+        for i in range(n - 1, -1, -1):
+            l = self.chain[i]
+            if i > 0:
+                ops.dense_wgrad(h[i - 1], dh[i], a.view(a.grad, i, "kernel"), a.view(a.grad, i, "bias"))
+                self._dgrad(i, l, dh[i], dh[i - 1], h[i - 1] if self.chain[i - 1].activation == "relu" else None)
+            else:
+                ops.dense_wgrad_split(xs, d, dh[0], a.view(a.grad, 0, "kernel"), a.view(a.grad, 0, "bias"))
+                self._dgrad(0, l, dh[0], dx0, None)
+        # -- input block backward: the deep tower's dx0 + the FM term, the tables' columns only
+        self._slices = [v(s) for s in self.slices]
+        slices = [(s, self.cols[f]) for s, f in zip(self._slices, self.feats)]
+        for s in range(0, len(slices), CONCAT_MAX_SLICES):
+            ops.fm_concat_backward([dx0], x0, ds, slices[s:s + CONCAT_MAX_SLICES])
+        self._idx, self._fidx, self._b = gidx, fidx, b
+
+    def apply_gradients(self) -> None:
+        a = self.arena
+        ops.opt_tick(self.hyper)
+        ops.dense_apply(self.opt.kind, a.w, a.grad, a.state1, a.state2, self.hyper)
+        T = len(self.tables)
+        for s in range(0, T, SPARSE_MAX_TABLES):
+            ops.sparse_rows_apply(self.opt.kind, [self._table_args(t, self._fidx[t], self._slices[t]) for t in range(s, min(T, s + SPARSE_MAX_TABLES))],
+                                  self._b, self.D, self.hyper)
+        ops.wide_rows_apply(self.opt.kind, self.wk.kernel.reshape(-1), self.wk_s1, self.wk_s2, self._fidx,
+                            [tb.table.shape[0] for tb in self.tables], self.woff, self.ds[:self._b], self.wk_acc, self.wk_rep, self.coff,
+                            self.wk_grad if self.wk_grad.numel() else None, None if self.wk.bias is None else self.wk.bias.reshape(-1),
+                            self.wb_s1, self.wb_s2, self.hyper)
+        self._refresh_operands()
+
+    def wide_gradients(self) -> Dict[str, torch.Tensor]:
+        """The wide kernel's gradient (W,) and its bias' (after forward_backward, before apply_gradients), assembled in float64
+        from ds, the ids and the continuous rows' sums — for parity tests."""
+        W = self.wk.kernel.numel()
+        g = torch.zeros(W, dtype=torch.float64, device=self.device)
+        ds = self.ds[:self._b].double()
+        for f, ids, tb in zip(self.feats, self._fidx, self.tables):
+            i = ops.widen_index(ids).reshape(-1).long()
+            ok = (i >= 0) & (i < tb.table.shape[0])
+            g.index_add_(0, i[ok] + self.woff[self.feats.index(f)], ds[ok])
+        nc = len(self.cont)
+        for c in range(nc):
+            g[self.coff[c]] += self.wk_grad[c].double()
+        out = {"wide/kernel": g.reshape(W, 1)}
+        if self.wk.bias is not None:
+            out["wide/bias"] = self.wk_grad[nc:].double().clone()
+        return out
+
+    def _snapshot(self):
+        snap = super()._snapshot()
+        snap.update(wk=self.wk.kernel.clone(), wb=None if self.wk.bias is None else self.wk.bias.clone(),
+                    wk_s=[None if s is None else s.clone() for s in (self.wk_s1, self.wk_s2, self.wb_s1, self.wb_s2)])
+        return snap
+
+    def _restore(self, snap) -> None:
+        super()._restore(snap)
+        self.wk.kernel.copy_(snap["wk"])
+        if snap["wb"] is not None:
+            self.wk.bias.copy_(snap["wb"])
+        for dst, src in zip((self.wk_s1, self.wk_s2, self.wb_s1, self.wb_s2), snap["wk_s"]):
+            if src is not None:
+                dst.copy_(src)
+        self.wk_grad.zero_()
+
+
 def trainer_for(model, optimizer: Optimizer, batch_size: int, group=None):
-    """The training engine of `model`: DLRMTrainer or DCNTrainer by the ranking body, TwoTowerTrainer for a RetrievalModel."""
-    from .models import DCNBody, RetrievalModel, RetrievalModelV2
+    """The training engine of `model`: DLRMTrainer, DCNTrainer or DeepFMTrainer by the ranking body, TwoTowerTrainer for a
+    RetrievalModel."""
+    from .models import DCNBody, DeepFMBody, RetrievalModel, RetrievalModelV2
 
     if isinstance(model, RetrievalModelV2):
         raise NotImplementedError("training TwoTowerModelV2 / ContrastiveOutput is not implemented: train the v1 TwoTowerModel")
@@ -1257,4 +1485,6 @@ def trainer_for(model, optimizer: Optimizer, batch_size: int, group=None):
         return TwoTowerTrainer(model, optimizer, batch_size, group=group)
     if isinstance(getattr(model, "body", None), DCNBody):
         return DCNTrainer(model, optimizer, batch_size, group=group)
+    if isinstance(getattr(model, "body", None), DeepFMBody):
+        return DeepFMTrainer(model, optimizer, batch_size, group=group)
     return DLRMTrainer(model, optimizer, batch_size, group=group)
