@@ -9,6 +9,8 @@ host predictions out (`Model.compile(example_batch)`), and what bench.py reports
 """
 from __future__ import annotations
 
+import contextlib
+import gc
 from typing import Dict, Optional
 
 import numpy as np
@@ -17,6 +19,23 @@ import torch
 from .core import Prediction, default_device, new_buffer_namespace, set_buffer_namespace
 
 _ALIGN = 256
+
+
+@contextlib.contextmanager
+def graph_capture(graph: torch.cuda.CUDAGraph):
+    """torch.cuda.graph(graph) with Python's cyclic garbage collector kept out of the capture.  A CUDA graph that sits in
+    an unreachable reference cycle (a dropped model, trainer or compiled forward) is destroyed whenever the collector
+    runs; destroying a graph while a stream is capturing invalidates that capture.  So pending garbage is collected
+    first and the collector stays off until the capture ends."""
+    enabled = gc.isenabled()
+    gc.collect()
+    gc.disable()
+    try:
+        with torch.cuda.graph(graph):
+            yield
+    finally:
+        if enabled:
+            gc.enable()
 
 
 class HostBatch:
@@ -127,7 +146,7 @@ class CompiledForward:
             torch.cuda.synchronize()
             self.graph = torch.cuda.CUDAGraph()
             n0 = ops.launch_count()
-            with torch.cuda.graph(self.graph):
+            with graph_capture(self.graph):
                 out = self._run()
             self.launches_per_replay = ops.launch_count() - n0  # kernels of libmm_b200.so inside the graph
             names = None

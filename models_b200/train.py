@@ -44,6 +44,7 @@ import torch
 from . import _cabi, ops
 from .blocks import DLRM, MLP, _Dense
 from .core import batch_size_of, default_device, get_feature
+from .graph import graph_capture
 
 INT32_MAX = 2**31 - 1
 DENSE_PATH_MAX_ROWS = 131072  # tables up to this size accumulate duplicate ids in a dense (rows, D) gradient
@@ -345,7 +346,7 @@ class _StepTrainer:
             torch.cuda.synchronize()
             self._graph = torch.cuda.CUDAGraph()
             n0 = ops.launch_count()
-            with torch.cuda.graph(self._graph):
+            with graph_capture(self._graph):
                 self.forward_backward(self._static, self._static_y)
                 self.apply_gradients()
             self.launches_per_step = ops.launch_count() - n0
@@ -1215,7 +1216,7 @@ class TwoTowerTrainer(_StepTrainer):
         q = self._tower_forward(self.towers[0], inputs, b)
         it = self._tower_forward(self.towers[1], inputs, b)
         qs, its = self.towers[0]["split"][:b], self.towers[1]["split"][:b]
-        ids = inputs[self.item_id].reshape(-1) if self.downscore else None
+        ids = ops.as_index(inputs[self.item_id]).reshape(-1) if self.downscore else None  # packed host-batch ids widened
         T = self.temperature
         ops.positive_scores(q, it, self.pos_logit[:b], temperature=T)
         ops.inbatch_softmax_ce_split(qs, its, self.D, self.pos_logit[:b], self.stats[:b], self.ws, pos_ids=ids, neg_ids=ids,
