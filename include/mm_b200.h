@@ -657,6 +657,57 @@ int mm_inbatch_softmax_ce_backward(const void* q_split, const void* neg_split, i
 int mm_l2_normalize_backward(const float* x, const float* dy, int64_t B, int D, int64_t x_stride, int64_t dy_stride, float* dx,
                              int64_t dx_stride, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * K17  Evaluation metrics of the ranking outputs (Keras metrics of BinaryOutput / RegressionOutput: AUC, Precision,
+ * Recall, BinaryAccuracy, RootMeanSquaredError, and the compiled loss), accumulated on the device.  Added with
+ * RankingModel.evaluate; no existing entry point changed.
+ *   mm_metrics_update  reads the LOGITS z (H, M) of H <= 8 heads (the (H, M) layout of mm_heads_fwd_bwd / mm_mlp_tc_heads)
+ *       and ADDS this batch into state, H blocks of MM_METRICS_SCALARS + 4 * num_buckets fp64 values (zero it first):
+ *         [MM_METRICS_LOSS]    sum sample_weight * l,  l = BCE max(z,0) - z y + log(1 + e^-|z|) | MSE (z - y)^2
+ *         [MM_METRICS_COUNT]   samples;   [MM_METRICS_INVALID]  samples with a NaN z / y or a binary target outside {0, 1}
+ *                              (they add nothing else)
+ *         metric set s (0, 1 < n_sets) at MM_METRICS_SET0 + s * MM_METRICS_SET_STRIDE, w = metric_weights[s][i] or 1:
+ *           binary heads: +POS / +NEG sum w of y = 1 / y = 0, +TP + t / +FP + t sum w of y = 1 / y = 0 with p > thresholds[t];
+ *           regression heads: +SQ_ERR sum w (z - y)^2, +W_SUM sum w
+ *         binary heads, after the scalars: per set [pos | neg] num_buckets each: sum w of y = 1 / y = 0 in bucket
+ *           max(ceil(fp32(p) * fp32(num_buckets - 1)) - 1, 0)   (the evenly spaced thresholds of Keras' AUC)
+ *       p = sigmoid(z) by pred_form: MM_PRED_ACT 1 / (1 + expf(-z)) (the epilogues that take MM_ACT_SIGMOID) or MM_PRED_HEAD
+ *       the |z|-stable form of mm_heads_fwd_bwd; either is bit-identical to the forward that produced z.  heads_host is a HOST
+ *       array.  workspace: mm_metrics_workspace_bytes(M, H) bytes of device scratch (one partial per CTA, added in CTA order:
+ *       with null metric weights the result does not depend on scheduling; weighted buckets use fp64 atomics).
+ *       2 <= num_buckets <= MM_METRICS_MAX_BUCKETS, n_sets 1 or 2.
+ * ------------------------------------------------------------------------------------- */
+#define MM_METRICS_MAX_HEADS 8
+#define MM_METRICS_MAX_THRESHOLDS 4
+#define MM_METRICS_MAX_BUCKETS 1024
+#define MM_METRICS_LOSS 0
+#define MM_METRICS_COUNT 1
+#define MM_METRICS_INVALID 2
+#define MM_METRICS_SET0 3
+#define MM_METRICS_SET_STRIDE 12
+#define MM_METRICS_POS 0
+#define MM_METRICS_NEG 1
+#define MM_METRICS_SQ_ERR 2
+#define MM_METRICS_W_SUM 3
+#define MM_METRICS_TP 4
+#define MM_METRICS_FP 8
+#define MM_METRICS_SCALARS 27
+#define MM_PRED_ACT 0
+#define MM_PRED_HEAD 1
+typedef struct {
+  const void* targets;              /* (M,) of target_dtype (MM_I32 .. MM_F64) */
+  const float* sample_weight;       /* (M,) weights of the loss, nullable */
+  const float* metric_weights[2];   /* (M,) weights of metric set 0 / 1, nullable */
+  int32_t target_dtype;
+  int32_t loss_kind;                /* MM_LOSS_BCE / MM_LOSS_MSE */
+  int32_t pred_form;                /* MM_PRED_ACT / MM_PRED_HEAD */
+  int32_t n_thresholds;             /* 0 .. MM_METRICS_MAX_THRESHOLDS */
+  float thresholds[4];
+} mm_metrics_head;
+int64_t mm_metrics_workspace_bytes(int64_t M, int H);
+int mm_metrics_update(const float* logits, int64_t M, int H, const mm_metrics_head* heads_host, int num_buckets, int n_sets,
+                      double* state, void* workspace, int64_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -106,6 +106,28 @@ class ColumnSlice(C.Structure):
     ]
 
 
+class MetricsHead(C.Structure):
+    """mm_metrics_head (include/mm_b200.h)."""
+
+    _fields_ = [
+        ("targets", C.c_void_p),
+        ("sample_weight", C.c_void_p),
+        ("metric_weights", C.c_void_p * 2),
+        ("target_dtype", C.c_int32),
+        ("loss_kind", C.c_int32),
+        ("pred_form", C.c_int32),
+        ("n_thresholds", C.c_int32),
+        ("thresholds", C.c_float * 4),
+    ]
+
+
+# mm_metrics_update state layout (include/mm_b200.h, K17)
+METRICS_MAX_HEADS, METRICS_MAX_THRESHOLDS, METRICS_MAX_BUCKETS = 8, 4, 1024
+METRICS_LOSS, METRICS_COUNT, METRICS_INVALID, METRICS_SET0, METRICS_SET_STRIDE = 0, 1, 2, 3, 12
+METRICS_POS, METRICS_NEG, METRICS_SQ_ERR, METRICS_W_SUM, METRICS_TP, METRICS_FP = 0, 1, 2, 3, 4, 8
+METRICS_SCALARS = 27
+PRED_ACT, PRED_HEAD = 0, 1
+
 _vp, _i, _i64, _f, _u64 = C.c_void_p, C.c_int, C.c_int64, C.c_float, C.c_uint64
 _tables = C.POINTER(GatherTable)
 
@@ -186,6 +208,8 @@ SIGNATURES = {
                                    _i, _vp]),
     "mm_wide_rows_apply": (_i, [_vp, _vp, _vp, _i64, C.POINTER(WideBlock), _i, _i64, _vp, _vp, _vp, C.POINTER(C.c_int64), _i, _vp,
                                 _vp, _vp, _vp, _i, _vp, _vp]),
+    "mm_metrics_workspace_bytes": (_i64, [_i64, _i]),
+    "mm_metrics_update": (_i, [_vp, _i64, _i, C.POINTER(MetricsHead), _i, _i, _vp, _vp, _i64, _vp]),
 }
 
 

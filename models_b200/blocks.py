@@ -43,6 +43,11 @@ def last_dense_path() -> str:
     return _LAST_PATH[0]
 
 
+# "mlp_tc" (mm_mlp_tc_heads) | "heads" (mm_heads_fwd_bwd): which kernel computed the most recent multi-output heads.  The
+# two apply the sigmoid in different (each exact) forms; RankingModel.logits reports the one its forward took.
+_LAST_HEADS = ["none"]
+
+
 _SMALL_TOWER = [True]  # mm_tower2_small for narrow-input two-layer towers (tests switch it off to reach the TMA tower kernel)
 _TABLE_MIRROR = [None]  # None: decide from MM_TABLE_MIRROR (default on); True / False: forced
 
@@ -63,7 +68,7 @@ def table_mirror() -> bool:
 
 
 def run_dense_chain(x: Optional[torch.Tensor], layers: "List[_Dense]", a_split: Optional[torch.Tensor] = None,
-                    K: Optional[int] = None, operand_out: bool = False, heads=None) -> torch.Tensor:
+                    K: Optional[int] = None, operand_out: bool = False, heads=None, logits: bool = False) -> torch.Tensor:
     """A chain of Dense layers on one input matrix.  operand_out=True: the result rows come back as bf16 split rows
     (B, 2*Kp) = [hi | lo] (the interaction kernel's operand format) — directly from the whole-tower kernel's last
     epilogue when it applies, by one mm_split_rows pass over the fp32 result otherwise.
@@ -75,7 +80,11 @@ def run_dense_chain(x: Optional[torch.Tensor], layers: "List[_Dense]", a_split: 
 
     heads (models.ParallelOutputs): the chain is followed by H output heads; the result is their (H, B) activated
     predictions — from the whole-tower kernel's multi-head epilogue (mm_mlp_tc_heads) when it applies, else by
-    mm_heads_fwd_bwd (forward only) over the last layer's fp32 rows."""
+    mm_heads_fwd_bwd (forward only) over the last layer's fp32 rows.
+
+    logits=True: the output (the heads, or else the chain's last layer) skips its activation, through the same kernels with
+    the activation argument linear: the result is the logits the activation would have read.  _LAST_HEADS records which
+    kernel computed the heads."""
     if heads is not None:
         hl = heads.to_call
         dev = (x if x is not None else a_split).device
@@ -86,15 +95,15 @@ def run_dense_chain(x: Optional[torch.Tensor], layers: "List[_Dense]", a_split: 
             width = l.units
         out = torch.empty((len(heads.outputs), B), dtype=torch.float32, device=dev)
         if _use_tc() and width <= 32 and ops.mlp_tc_supported(K if a_split is not None else x.shape[1], [l.units for l in layers], heads=True):
-            _LAST_PATH[0] = "mlp_tc"
+            _LAST_PATH[0] = _LAST_HEADS[0] = "mlp_tc"
             a = a_split if a_split is not None else ops.split_rows(x)
             return ops.mlp_tc_heads(a, K if a_split is not None else x.shape[1], [l.split_kernel() for l in layers],
                                     [l.units for l in layers], [l.bias for l in layers], [l.activation for l in layers],
-                                    hl.kernel, hl.bias, heads.activations, out)
+                                    hl.kernel, hl.bias, ["linear"] * len(heads.outputs) if logits else heads.activations, out)
         if a_split is not None and not _use_tc():
             raise ValueError("the fp32 dense engine needs an fp32 input")
         h = run_dense_chain(x, layers, a_split=a_split, K=K)
-        return ops.heads_fwd_bwd(h.contiguous(), hl.kernel, hl.bias, heads.losses, None, out)
+        return heads.stacked_forward(h, out, logits=logits)
     if a_split is not None:  # producer (interaction kernel) already emitted the split-bf16 operand
         device, B, a = a_split.device, a_split.shape[0], a_split
     else:
@@ -103,11 +112,14 @@ def run_dense_chain(x: Optional[torch.Tensor], layers: "List[_Dense]", a_split: 
     for l in layers:
         l.build(width, device)
         width = l.units
+    acts = [l.activation for l in layers]
+    if logits:
+        acts[-1] = "linear"
     if not _use_tc():
         if x is None:
             raise ValueError("the fp32 dense engine needs an fp32 input")
-        for l in layers:
-            x = l(x)
+        for l, act in zip(layers, acts):
+            x = l(x, activation=act)
         _LAST_PATH[0] = "fp32"
         return ops.split_rows(x.contiguous()) if operand_out else x
     if a_split is None:
@@ -118,7 +130,7 @@ def run_dense_chain(x: Optional[torch.Tensor], layers: "List[_Dense]", a_split: 
     fuse_head = (len(layers) >= 2 and layers[-1].units == 1 and layers[-2].units <= 32
                  and layers[-1].input_dim == layers[-2].units)
     if fuse_head:
-        head, layers = layers[-1], layers[:-1]
+        (head, layers), (head_act, acts) = (layers[-1], layers[:-1]), (acts[-1], acts[:-1])
     if K != layers[0].input_dim:
         raise ValueError(f"{layers[0].name}: input width {K} != kernel rows {layers[0].input_dim}")
     widths = [l.units for l in layers]
@@ -128,7 +140,7 @@ def run_dense_chain(x: Optional[torch.Tensor], layers: "List[_Dense]", a_split: 
         kw = {}
         if fuse_head:
             out = torch.empty((B, 1), dtype=torch.float32, device=device)
-            kw = dict(head_w=head.kernel.reshape(-1), head_b=head.bias_value(), head_act=head.activation, head_out=out)
+            kw = dict(head_w=head.kernel.reshape(-1), head_b=head.bias_value(), head_act=head_act, head_out=out)
         elif operand_out and widths[-1] % 64 == 0:
             out = torch.empty((B, 2 * widths[-1]), dtype=torch.bfloat16, device=device)  # split rows [hi | lo]
             kw = dict(out_operand=out)
@@ -136,25 +148,24 @@ def run_dense_chain(x: Optional[torch.Tensor], layers: "List[_Dense]", a_split: 
         else:
             out = torch.empty((B, widths[-1]), dtype=torch.float32, device=device)
             kw = dict(out=out)
-        ops.mlp_tc(a, K, [l.split_kernel() for l in layers], widths, [l.bias for l in layers],
-                   [l.activation for l in layers], **kw)
+        ops.mlp_tc(a, K, [l.split_kernel() for l in layers], widths, [l.bias for l in layers], acts, **kw)
         return ops.split_rows(out) if operand_out else out
     _LAST_PATH[0] = "dense_tc"
-    for i, l in enumerate(layers):
+    for i, (l, act) in enumerate(zip(layers, acts)):
         last = i == len(layers) - 1
         if K != l.input_dim:
             raise ValueError(f"{l.name}: input width {K} != kernel rows {l.input_dim}")
         nxt = None
         if last and fuse_head:
             out = torch.empty((B, 1), dtype=torch.float32, device=device)
-            ops.dense_tc_head(a, K, l.split_kernel(), l.units, l.bias, l.activation, head.kernel.reshape(-1),
-                              head.bias_value(), head.activation, out)
+            ops.dense_tc_head(a, K, l.split_kernel(), l.units, l.bias, act, head.kernel.reshape(-1),
+                              head.bias_value(), head_act, out)
             return out
         if last:
             out = torch.empty((B, l.units), dtype=torch.float32, device=device)
         else:
             nxt = l.split_buffer(B, device)
-        ops.dense_tc(a, K, l.split_kernel(), l.units, l.bias, l.activation, passes=3, out_f32=out, out_split=nxt)
+        ops.dense_tc(a, K, l.split_kernel(), l.units, l.bias, act, passes=3, out_f32=out, out_split=nxt)
         a, K = nxt, l.units
     return ops.split_rows(out) if operand_out else out
 
@@ -247,7 +258,9 @@ class _Dense(Block):
             out["bias"] = self.bias
         return out
 
-    def call(self, inputs, x0: Optional[torch.Tensor] = None, **kwargs) -> torch.Tensor:
+    def call(self, inputs, x0: Optional[torch.Tensor] = None, activation: Optional[str] = None, **kwargs) -> torch.Tensor:
+        """activation: replaces the layer's own for this call (the logits of an output layer: "linear")."""
+        act = activation or self.activation
         x = concat_sorted(inputs) if isinstance(inputs, dict) else inputs
         if x.dim() != 2:
             raise ValueError(f"{self.name}: expected a 2-D input, got shape {tuple(x.shape)}")
@@ -256,12 +269,11 @@ class _Dense(Block):
             raise ValueError(f"{self.name}: input width {x.shape[1]} != kernel rows {self.input_dim}")
         out = torch.empty((x.shape[0], self.units), dtype=torch.float32, device=x.device)
         if x0 is None and not _use_tc():
-            return ops.dense_fp32(x, self.kernel, self.bias, self.activation, out)
+            return ops.dense_fp32(x, self.kernel, self.bias, act, out)
         if x0 is None:
-            ops.dense_tc(ops.split_rows(x), self.input_dim, self.split_kernel(), self.units, self.bias, self.activation,
-                         out_f32=out)
+            ops.dense_tc(ops.split_rows(x), self.input_dim, self.split_kernel(), self.units, self.bias, act, out_f32=out)
             return out
-        return ops.dense_fp32(x, self.kernel, self.bias, self.activation, out, x0=x0)
+        return ops.dense_fp32(x, self.kernel, self.bias, act, out, x0=x0)
 
 
 class BatchNormalization(Block):
@@ -537,8 +549,10 @@ class FM(Block):
     def weights(self):
         return {f"wide/{k}": v for k, v in self.wide.weights().items()}
 
-    def head(self, inputs: TabularData, addend: Optional[torch.Tensor] = None, out_layer: Optional["_Dense"] = None) -> torch.Tensor:
-        """(B, 1) = [out_layer](wide + pairwise [+ addend]) in one kernel (ops.deepfm_head)."""
+    def head(self, inputs: TabularData, addend: Optional[torch.Tensor] = None, out_layer: Optional["_Dense"] = None,
+             logits: bool = False) -> torch.Tensor:
+        """(B, 1) = [out_layer](wide + pairwise [+ addend]) in one kernel (ops.deepfm_head); logits=True: out_layer without
+        its activation."""
         from .core import get_feature
 
         dev = next(iter(inputs.values())).device
@@ -557,7 +571,7 @@ class FM(Block):
         ow = ob = act = None
         if out_layer is not None:
             out_layer.build(1, dev)
-            ow, ob, act = out_layer.kernel.reshape(-1), out_layer.bias, out_layer.activation
+            ow, ob, act = out_layer.kernel.reshape(-1), out_layer.bias, "linear" if logits else out_layer.activation
         ops.deepfm_head(tabs, idx, [self.wide_offsets[f] for f in self.cat_names], cont, [self.wide_offsets[n] for n in self.cont_names],
                         self.wide.kernel.reshape(-1), self.wide.bias, None if addend is None else addend.reshape(-1), ow, ob, act,
                         out.reshape(-1), oob)

@@ -70,6 +70,14 @@ __device__ __forceinline__ float apply_act(float v, int act) {
   return apply_act_slow(v, act);
 }
 
+// Prediction of an output head from its logit z, as mm_heads_fwd_bwd writes it: z (MM_LOSS_MSE) or the |z|-stable sigmoid
+// (MM_LOSS_BCE).  mm_metrics_update evaluates the same code, so its sigmoid is bit-identical to that forward's.
+__device__ __forceinline__ float head_pred(int kind, float z) {
+  if (kind == MM_LOSS_MSE) return z;
+  const float e = expf(-fabsf(z));
+  return z >= 0.0f ? 1.0f / (1.0f + e) : e / (1.0f + e);
+}
+
 // per-launch table list, passed by value in kernel parameter space (2 KB)
 struct GatherParams {
   mm_gather_table t[MM_MAX_TABLES];

@@ -73,12 +73,6 @@ __device__ __forceinline__ void head_loss(int kind, float z, float y, float& l, 
   }
 }
 
-__device__ __forceinline__ float head_pred(int kind, float z) {
-  if (kind == MM_LOSS_MSE) return z;
-  const float e = expf(-fabsf(z));
-  return z >= 0.0f ? 1.0f / (1.0f + e) : e / (1.0f + e);
-}
-
 template <int H, bool TRAIN>
 __global__ void __launch_bounds__(256, H == 1 ? 2 : 1) head_kernel(const HeadParams p) {
   const int lane = threadIdx.x & 31;

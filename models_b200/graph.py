@@ -291,3 +291,94 @@ class PipelinedForward:
         self.busy[ticket] = False
         self.slots[ticket].check_indices()
         return self.slots[ticket].host_result
+
+
+def _uniq_clones(ts):
+    """Clones of a list of tensors (entries may be None or repeat: a repeated tensor is cloned once)."""
+    seen = {}
+    return [None if t is None else seen.setdefault(id(t), t.clone()) for t in ts]
+
+
+class EvalGraph:
+    """One evaluation step of a ranking model — the logits forward (RankingModel.logits) and the metric update
+    (metrics.MetricsState.update) — captured into a CUDA graph over static device buffers, for batches of one layout.
+    `replay` refreshes the static buffers (device-to-device, all columns in a few multi-tensor copies) and launches the graph.  Re-captured when a
+    model variable was reassigned or trained since the capture (core.weights_version), as CompiledForward is."""
+
+    def __init__(self, model, state, inputs: Dict[str, torch.Tensor], targets, sample_weight):
+        self.model, self.state = model, state
+        self.key = self.layout(inputs, targets, sample_weight, state.device)
+        self.inputs = {k: v.clone() for k, v in inputs.items()}
+        self.targets = _uniq_clones(targets)
+        self.sample_weight = None if sample_weight is None else _uniq_clones(sample_weight)
+        self.namespace = new_buffer_namespace()  # private scratch buffers of the captured forward
+        self._capture()
+
+    @staticmethod
+    def layout(inputs, targets, sample_weight, device) -> Optional[tuple]:
+        """Shapes and dtypes of a batch, or None when it cannot be replayed: a ragged feature (its number of ids changes from
+        batch to batch) or a column that is not a tensor on `device`."""
+        cols = list(inputs.items()) + [(f"#y{h}", t) for h, t in enumerate(targets)]
+        cols += [(f"#w{h}", w) for h, w in enumerate(sample_weight or []) if w is not None]
+        key = []
+        for k, v in cols:
+            if not isinstance(v, torch.Tensor) or v.device != device or k.endswith("__values") or k.endswith("__offsets"):
+                return None
+            key.append((k, tuple(v.shape), v.dtype))
+        shared = list(targets) + list(sample_weight or [])  # which entries are one tensor (one static copy)
+        key.append(tuple(next(i for i, u in enumerate(shared) if u is t) for t in shared if t is not None))
+        return tuple(key)
+
+    def _step(self) -> None:
+        z, form = self.model.logits(self.inputs)
+        self.state.update(z, self.targets, form, self.sample_weight)
+
+    def _capture(self) -> None:
+        from . import ops
+        from .core import weights_version
+
+        st = self.state
+        saved = (st.state.clone(), st.before_last.clone())
+        old_ns = set_buffer_namespace(self.namespace)
+        try:
+            # warm-up on a side stream (split kernels, scratch buffers, the fused head's host bias, the metric workspace);
+            # it adds two batches into the state, which is restored afterwards
+            s = torch.cuda.Stream(device=st.device)
+            s.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(s):
+                for _ in range(2):
+                    self._step()
+            torch.cuda.current_stream().wait_stream(s)
+            torch.cuda.synchronize()
+            st.state.copy_(saved[0])
+            st.before_last.copy_(saved[1])
+            self.workspace = st.workspace  # the graph holds its address: keep it alive
+            self.graph = torch.cuda.CUDAGraph()
+            n0 = ops.launch_count()
+            with graph_capture(self.graph):
+                self._step()
+            self.launches_per_replay = ops.launch_count() - n0
+            self._wv = weights_version()
+        finally:
+            set_buffer_namespace(old_ns)
+
+    def replay(self, inputs: Dict[str, torch.Tensor], targets, sample_weight) -> None:
+        from .core import weights_version
+
+        if weights_version() != self._wv:
+            torch.cuda.synchronize()
+            self._capture()
+        dst, src, done = list(self.inputs.values()), [inputs[k] for k in self.inputs], set()
+        for mine, theirs in zip(self.targets + (self.sample_weight or []), list(targets) + list(sample_weight or [])):
+            if mine is not None and id(mine) not in done:
+                dst.append(mine)
+                src.append(theirs)
+                done.add(id(mine))
+        groups: Dict[torch.dtype, tuple] = {}
+        for d, s_ in zip(dst, src):
+            g = groups.setdefault(d.dtype, ([], []))
+            g[0].append(d)
+            g[1].append(s_)
+        for d, s_ in groups.values():  # one multi-tensor copy per dtype instead of one launch per column
+            torch._foreach_copy_(d, s_, non_blocking=True)
+        self.graph.replay()

@@ -2,8 +2,8 @@
 
 Reference: merlin/models/tf/models/ranking.py:23-168, models/retrieval.py:106-203,
 models/base.py:1805-1854 (Model.call protocol), outputs/classification.py:72-123 (BinaryOutput),
-prediction_tasks/classification.py:59-116 (BinaryClassificationTask).  Only construction and the
-forward call are in scope — fit/compile/optimizers/metrics are not (SURVEY.md §8).
+prediction_tasks/classification.py:59-116 (BinaryClassificationTask).  Construction, the forward call, compile / fit /
+train_step (models_b200/train.py) and, for ranking models, evaluate and the compiled metrics (models_b200/metrics.py).
 """
 from __future__ import annotations
 
@@ -40,8 +40,8 @@ class BinaryOutput(Block):
     def weights(self):
         return {f"dense/{k}": v for k, v in self.to_call.weights().items()}
 
-    def call(self, inputs: torch.Tensor, **kwargs) -> torch.Tensor:
-        return self.to_call(inputs)
+    def call(self, inputs: torch.Tensor, logits: bool = False, **kwargs) -> torch.Tensor:
+        return self.to_call(inputs, activation="linear" if logits else None)
 
 
 class BinaryClassificationTask(BinaryOutput):
@@ -122,11 +122,19 @@ class ParallelOutputs(Block):
         """(H, B) predictions -> {name: (B, 1) view}."""
         return {n: stacked[h].view(-1, 1) for h, n in enumerate(self.names)}
 
-    def call(self, inputs: torch.Tensor, **kwargs) -> Dict[str, torch.Tensor]:
+    def stacked_forward(self, x: torch.Tensor, out: torch.Tensor, logits: bool = False) -> torch.Tensor:
+        """out (H, B) = the heads on the body output x by mm_heads_fwd_bwd (forward only): the activated predictions, or with
+        logits=True the logits (every head run as a linear regression head)."""
+        from .blocks import _LAST_HEADS
+
+        _LAST_HEADS[0] = "heads"
+        return ops.heads_fwd_bwd(x.contiguous(), self.to_call.kernel, self.to_call.bias,
+                                 ["mse"] * len(self.outputs) if logits else self.losses, None, out)
+
+    def call(self, inputs: torch.Tensor, logits: bool = False, **kwargs) -> Dict[str, torch.Tensor]:
         self.build(inputs.shape[1], inputs.device)
         out = torch.empty((len(self.outputs), inputs.shape[0]), dtype=torch.float32, device=inputs.device)
-        ops.heads_fwd_bwd(inputs.contiguous(), self.to_call.kernel, self.to_call.bias, self.losses, None, out)
-        return self.split(out)
+        return self.split(self.stacked_forward(inputs, out, logits=logits))
 
 
 def OutputBlock(schema: Schema, model_outputs=None) -> Block:
@@ -341,12 +349,28 @@ class Model(Block):
         """The model's outputs in output order (one for a single-output model)."""
         return list(self.prediction.outputs) if isinstance(self.prediction, ParallelOutputs) else [self.prediction]
 
-    def _compile_training(self, optimizer, loss=None, loss_weights=None) -> None:
+    def _compile_training(self, optimizer, loss=None, loss_weights=None, metrics=None, weighted_metrics=None) -> None:
         from .train import get_optimizer
 
         self.loss_weights = resolve_loss_weights(self.output_blocks(), loss, loss_weights)
         self.optimizer = get_optimizer(optimizer)
         self._trainer = None
+
+    def _targets_by_output(self, y) -> list:
+        """Targets as given to train_step / evaluate (a tensor, or a dict keyed by target column) -> one per output."""
+        outs = self.output_blocks()
+        if y is None:
+            raise ValueError("targets are needed")
+        if isinstance(y, dict):
+            if len(outs) == 1 and len(y) == 1:
+                return [next(iter(y.values()))]
+            missing = [o.target for o in outs if o.target not in y]
+            if missing:
+                raise ValueError(f"no targets for {missing} (got keys {sorted(y)})")
+            return [y[o.target] for o in outs]
+        if len(outs) > 1:
+            raise ValueError(f"this model has {len(outs)} outputs: pass the targets as a dict keyed by target column")
+        return [y]
 
     def trainer(self, batch_size: int, group=None):
         """The static-buffer training engine for batches of (up to) `batch_size` samples (train.DLRMTrainer or
@@ -379,20 +403,10 @@ class Model(Block):
         outs = self.output_blocks()
         if y is None:
             raise ValueError("train_step needs targets")
-        if isinstance(y, dict):
-            if len(outs) == 1 and len(y) == 1:
-                y = next(iter(y.values()))
-            else:
-                missing = [o.target for o in outs if o.target not in y]
-                if missing:
-                    raise ValueError(f"train_step: no targets for {missing} (got keys {sorted(y)})")
-                y = [y[o.target] for o in outs]
-        elif len(outs) > 1:
-            raise ValueError(f"this model has {len(outs)} outputs: pass the targets as a dict keyed by target column")
-        else:
-            y = [y]
-        if not isinstance(y, list):
-            y = [y]
+        try:
+            y = self._targets_by_output(y)
+        except ValueError as e:
+            raise ValueError(f"train_step: {e}") from None
         if isinstance(sw, dict):
             sw = [sw.get(o.name) for o in outs]
         self._check_inputs(x)
@@ -413,13 +427,18 @@ class Model(Block):
             raise NotImplementedError("fit(x, y): pass a Loader or an iterable of (inputs, targets) batches")
         bs = batch_size or getattr(x, "batch_size", None)
         history = {"loss": []}
-        for _ in range(int(epochs)):
+        train_metrics, every = self._fit_train_metrics(kwargs)
+        for epoch in range(int(epochs)):
             total, n = None, 0
+            if train_metrics is not None:
+                train_metrics.reset()
             for inputs, targets in x:
                 if getattr(self, "_trainer", None) is None and bs:
                     self._check_inputs(inputs)
                     self.trainer(int(bs))
                 m = self.train_step((inputs, targets))
+                if train_metrics is not None and n % every == 0:
+                    self._update_train_metrics(train_metrics, targets)
                 # the loss-buffer views are valid until the next step: [loss_batch, per-output losses...] summed on the device
                 vec = torch.stack([m["loss_batch"]] + [v for k, v in m.items() if k not in ("loss", "loss_batch", "regularization_loss")])
                 total = vec.clone() if total is None else total + vec
@@ -433,10 +452,18 @@ class Model(Block):
             for i, k in enumerate([k for k in m if k not in ("loss", "loss_batch", "regularization_loss")]):
                 history.setdefault(k, []).append(means[1 + i])
             self._trainer.check_indices()
+            self._fit_epoch_end(epoch, history, train_metrics, kwargs)
         from .train import History
 
         self.history = History(history)
         return self.history
+
+    def _fit_train_metrics(self, fit_kwargs):
+        """(state, every): the device state of the training metrics and the batch interval of their updates (None: off)."""
+        return None, 0
+
+    def _fit_epoch_end(self, epoch: int, history: Dict[str, List[float]], train_metrics, fit_kwargs) -> None:
+        pass
 
     # -- CUDA-graph runtime (models_b200/graph.py) ---------------------------------------------
     def embedding_blocks(self) -> List[EmbeddingsBlock]:
@@ -479,8 +506,9 @@ class Model(Block):
 
         * `compile(optimizer="adam")` / `compile("adagrad")` / `compile(optimizer=mm.Adagrad(0.01))` — Keras `compile`
           (models/base.py: the reference's models are compiled before `fit`): picks the optimizer of the training step
-          (models_b200/train.py).  The loss is the prediction task's default (binary cross-entropy for BinaryOutput);
-          `metrics` / `run_eagerly` are accepted for signature parity.
+          (models_b200/train.py).  The loss is the prediction task's default (binary cross-entropy for BinaryOutput).
+          Ranking models take `metrics` / `weighted_metrics` (models_b200/metrics.py: None = each output's reference
+          defaults) for `evaluate` and `fit`; `run_eagerly` is accepted for signature parity.
         * `compile(example_batch, **call_kwargs)` — capture this model's forward for `example`'s batch layout into a CUDA
           graph; the result maps a packed pinned HostBatch to pinned host predictions with one H2D, one graph launch and
           one D2H (models_b200/graph.py)."""
@@ -491,7 +519,7 @@ class Model(Block):
             if example is not None and optimizer is not None:
                 raise ValueError("compile(): pass either an example batch (graph capture) or an optimizer (training)")
             return self._compile_training(optimizer if optimizer is not None else (example or "adam"), loss,
-                                          call_kwargs.pop("loss_weights", None))
+                                          call_kwargs.pop("loss_weights", None), metrics, call_kwargs.pop("weighted_metrics", None))
         if not isinstance(example, HostBatch):
             example = HostBatch.like(example, self.input_columns())
         return CompiledForward(self, example, **call_kwargs)
@@ -523,8 +551,169 @@ class Model(Block):
         return pred.cpu()
 
 
+_EVAL_GRAPH = [True]  # evaluate replays full-size fixed-shape batches as a CUDA graph (tests switch it off for the eager path)
+
+
 class RankingModel(Model):
-    """DLRM / DCN: body -> (B, h) -> BinaryOutput (B,1)."""
+    """DLRM / DCN / DeepFM: body -> (B, h) -> BinaryOutput (B,1) (or an OutputBlock's heads).  `evaluate` and
+    `fit(validation_data=...)` report the compiled metrics (models_b200/metrics.py), accumulated on the device."""
+
+    _TRANSIENT = {"_pinned": {}, "_trainer": None, "_eval_state": None, "_fit_state": None, "_eval_graph": None}
+
+    def _distributed(self) -> bool:
+        """Row-sharded tables or a data-parallel training engine: each rank sees only its share of the data."""
+        return getattr(self.body, "sharded", None) is not None or getattr(getattr(self, "_trainer", None), "group", None) is not None
+
+    def _compile_training(self, optimizer, loss=None, loss_weights=None, metrics=None, weighted_metrics=None) -> None:
+        from .metrics import MetricsSpec
+
+        super()._compile_training(optimizer, loss, loss_weights)
+        self.metrics_spec = MetricsSpec(self.output_blocks(), self.loss_weights, metrics, weighted_metrics)
+        self._eval_state = self._fit_state = None
+
+    @property
+    def metrics_names(self) -> List[str]:
+        """The keys of `evaluate(return_dict=True)`, in the order of `evaluate`'s list."""
+        return self._compiled_metrics().result_names()
+
+    def _compiled_metrics(self):
+        spec = getattr(self, "metrics_spec", None)
+        if spec is None:
+            raise RuntimeError("You must compile your model before training/testing. Use `model.compile(optimizer, loss)`.")
+        return spec
+
+    def _metrics_state(self, attr: str, device):
+        from .metrics import MetricsState
+
+        st = getattr(self, attr, None)
+        if st is None or st.spec is not self.metrics_spec or st.device != device:
+            st = MetricsState(self.metrics_spec, device)
+            setattr(self, attr, st)
+        st.reset()
+        return st
+
+    def predict(self, *args, **kwargs):
+        raise NotImplementedError("predict is not implemented: call the model on a batch, or compile(example_batch) for a "
+                                  "CUDA-graph forward")
+
+    def evaluate(self, x, y=None, batch_size: Optional[int] = None, steps: Optional[int] = None, return_dict: bool = False,
+                 verbose: int = 0, callbacks=None, **kwargs):
+        """Keras `evaluate` (models/base.py:1176-1310) over a Loader or an iterable of (inputs, targets[, sample_weight])
+        batches; targets a tensor or a dict keyed by target column, sample_weight a tensor or a dict by output name.  Each
+        batch is the forward up to the logits (RankingModel.logits) plus one mm_metrics_update launch.  Batches of the first
+        batch's size whose columns all have a fixed shape replay that step as one CUDA graph over static buffers
+        (graph.EvalGraph); a smaller last batch and ragged features run eagerly.  Nothing is read back until the end: then
+        one copy of the metric state and one read of the out-of-range id counter.  Returns the values in `metrics_names`
+        order, or a dict with return_dict=True.  Variables, optimizer slots and captured training graphs are not touched."""
+        from .graph import EvalGraph
+
+        spec = self._compiled_metrics()
+        if y is not None:
+            raise NotImplementedError("evaluate(x, y): pass a Loader or an iterable of (inputs, targets[, sample_weight]) batches")
+        if callbacks:
+            raise NotImplementedError("evaluate(callbacks=...) is not implemented")
+        if self._distributed():
+            raise NotImplementedError("evaluate of a sharded or data-parallel model is not implemented (each rank would need "
+                                      "the metric states of every other rank)")
+        outs = self.output_blocks()
+        for o in outs:
+            if not isinstance(o, BinaryOutput):
+                raise NotImplementedError(f"evaluate: output {o.name!r} is not a BinaryOutput / RegressionOutput")
+        state, n, dev, oob, full = None, 0, None, None, None
+        it = iter(x)
+        self.defer_index_check(True)
+        try:
+            while steps is None or n < int(steps):
+                try:
+                    batch = next(it)
+                except StopIteration:
+                    break
+                if not isinstance(batch, (tuple, list)) or len(batch) < 2:
+                    raise ValueError("evaluate expects batches of (inputs, targets) or (inputs, targets, sample_weight)")
+                inputs, targets = batch[0], batch[1]
+                sw = batch[2] if len(batch) > 2 else None
+                self._check_inputs(inputs)
+                if state is None:
+                    dev = next(iter(inputs.values())).device
+                    state = self._metrics_state("_eval_state", dev)
+                    oob = self.index_error_counter(dev)  # one counter shared by every table, read once at the end
+                    full = batch_size_of(inputs)
+                ys = [torch.as_tensor(t, device=dev) for t in self._targets_by_output(targets)]
+                if isinstance(sw, dict):
+                    sw = [sw.get(o.name) for o in outs]
+                elif sw is not None and not isinstance(sw, (list, tuple)):
+                    sw = [sw] * len(outs)
+                key = EvalGraph.layout(inputs, ys, sw, dev) if _EVAL_GRAPH[0] and batch_size_of(inputs) == full else None
+                if key is None:
+                    z, form = self.logits(inputs)
+                    state.update(z, ys, form, sw)
+                else:
+                    g = getattr(self, "_eval_graph", None)
+                    if g is None or g.key != key or g.state is not state:
+                        g = self._eval_graph = None  # drop the old graph before capturing the new one
+                        g = self._eval_graph = EvalGraph(self, state, inputs, ys, sw)
+                    g.replay(inputs, ys, sw)
+                n += 1
+        finally:
+            self.defer_index_check(False)
+        if n == 0:
+            raise ValueError("evaluate: the data produced no batches")
+        res = state.result()
+        if oob is not None:
+            from .inputs import _raise_on_oob
+
+            _raise_on_oob(oob, "evaluate")
+        return res if return_dict else [res[k] for k in spec.result_names()]
+
+    def fit(self, x=None, y=None, batch_size: Optional[int] = None, epochs: int = 1, steps_per_epoch: Optional[int] = None,
+            verbose: int = 0, validation_data=None, validation_steps: Optional[int] = None, validation_freq=1,
+            train_metrics_steps: int = 1, callbacks=None, **kwargs):
+        """Model.fit plus the compiled metrics: on the training batches (from the step's logits, on the first batch and
+        every `train_metrics_steps` batches of each epoch, 0: off) under their own names, and with `validation_data`
+        `evaluate` after every epoch that `validation_freq` names (an interval, or a list of 1-based epochs) under
+        `val_<name>`.  The metric launches happen between steps, outside the training step and its captured graph."""
+        if callbacks:
+            raise NotImplementedError("fit(callbacks=...) is not implemented")
+        freqs = list(validation_freq) if isinstance(validation_freq, (list, tuple, set, range)) else [validation_freq]
+        if any(int(f) < 1 for f in freqs):
+            raise ValueError(f"validation_freq must be a positive interval or a list of positive epochs, got {validation_freq!r}")
+        return super().fit(x, y, batch_size=batch_size, epochs=epochs, steps_per_epoch=steps_per_epoch, verbose=verbose,
+                           validation_data=validation_data, validation_steps=validation_steps, validation_freq=validation_freq,
+                           train_metrics_steps=train_metrics_steps, **kwargs)
+
+    def _fit_train_metrics(self, fit_kwargs):
+        every = int(fit_kwargs.get("train_metrics_steps", 1))
+        if every < 0:
+            raise ValueError("train_metrics_steps must be >= 0")
+        # with sharded tables or a data-parallel engine each rank would report its own, unaveraged metrics: off
+        if (every == 0 or getattr(self, "metrics_spec", None) is None or not self._compiled_metrics().metric_keys()
+                or self._distributed()):
+            return None, 0
+        return self._metrics_state("_fit_state", default_device()), every
+
+    def _update_train_metrics(self, state, targets) -> None:
+        from ._cabi import PRED_HEAD
+
+        tr = self._trainer
+        ys = [t if isinstance(t, torch.Tensor) and t.device == state.device else torch.as_tensor(t, device=state.device)
+              for t in self._targets_by_output(targets)]
+        b = ys[0].numel()
+        state.update(tr.logits.view(-1)[:tr.H * b].view(tr.H, b), ys, PRED_HEAD)
+
+    def _fit_epoch_end(self, epoch: int, history, train_metrics, fit_kwargs) -> None:
+        if train_metrics is not None:
+            res = train_metrics.result()
+            for k in self.metrics_spec.metric_keys():
+                history.setdefault(k, []).append(res[k])
+        data = fit_kwargs.get("validation_data")
+        if data is None:
+            return
+        freq = fit_kwargs.get("validation_freq", 1)
+        due = (epoch + 1) in freq if isinstance(freq, (list, tuple, set, range)) else (epoch + 1) % int(freq) == 0
+        if due:
+            res = self.evaluate(data, steps=fit_kwargs.get("validation_steps"), return_dict=True)
+            for k, v in res.items():
+                history.setdefault(f"val_{k}", []).append(v)
 
     def build(self, device=None):
         self.body.build(device)
@@ -546,6 +735,25 @@ class RankingModel(Model):
         return self.body.output_width()
 
     def call(self, inputs: TabularData, targets=None, training: bool = False, testing: bool = False, **kwargs):
+        return self._forward(inputs, training=training)
+
+    def logits(self, inputs: TabularData):
+        """The forward of `call` stopped before the output activation: (z, pred_form) with z the (H, B) logits of the H
+        outputs (output order) and pred_form the _cabi.PRED_* form in which that forward applies the sigmoid (the
+        multi-head kernel mm_heads_fwd_bwd has its own), so that a metric recomputing sigmoid(z) gets `call`'s
+        predictions bit for bit."""
+        from ._cabi import PRED_ACT, PRED_HEAD
+        from .blocks import _LAST_HEADS
+
+        _LAST_HEADS[0] = "none"
+        out = self._forward(inputs, logits=True)
+        if isinstance(out, dict):
+            from .graph import _stacked_outputs
+
+            return _stacked_outputs(out), PRED_HEAD if _LAST_HEADS[0] == "heads" else PRED_ACT
+        return out.reshape(1, -1), PRED_ACT
+
+    def _forward(self, inputs: TabularData, training: bool = False, logits: bool = False):
         self._check_inputs(inputs)
         if not self.built:
             self.build(next(iter(inputs.values())).device)
@@ -556,8 +764,8 @@ class RankingModel(Model):
 
         def chain(x, layers, **kw):
             if heads is None:
-                return run_dense_chain(x, layers, **kw)
-            return heads.split(run_dense_chain(x, layers, heads=heads, **kw))
+                return run_dense_chain(x, layers, logits=logits, **kw)
+            return heads.split(run_dense_chain(x, layers, heads=heads, logits=logits, **kw))
 
         if isinstance(self.body, DLRM) and self.body.top_block is not None:
             # top MLP + output layer as ONE dense chain (no fp32 round trip between them)
@@ -575,14 +783,14 @@ class RankingModel(Model):
             x = self.body.interaction_forward(inputs, bottom)
             return chain(x, layers)
         if isinstance(self.body, DeepFMBody):
-            return self.body.forward(inputs, out_layer=self.prediction.to_call)
+            return self.body.forward(inputs, out_layer=self.prediction.to_call, logits=logits)
         if isinstance(self.body, DCNBody) and self.body.stacked:
             x = self.body.cross(self.body.input_block(inputs))
             layers, tail = self.body.deep.chain(extra)
             assert tail is None
             return chain(x, layers)
         x = self.body(inputs, training=training)
-        return self.prediction(x)
+        return self.prediction(x, logits=True) if logits else self.prediction(x)
 
 
 def DLRMModel(schema: Schema, *, embeddings: Optional[EmbeddingsBlock] = None, embedding_dim: Optional[int] = None,
@@ -679,12 +887,12 @@ class DeepFMBody(Block):
         out.update({f"deep_logit/{k}": v for k, v in self.deep_logit.weights().items()})
         return out
 
-    def forward(self, inputs: TabularData, out_layer: Optional[_Dense] = None) -> torch.Tensor:
+    def forward(self, inputs: TabularData, out_layer: Optional[_Dense] = None, logits: bool = False) -> torch.Tensor:
         if not self.built:
             self.build(next(iter(inputs.values())).device)
         x0 = self.input_block(inputs)
         deep = run_dense_chain(x0, self.deep.dense_layers + self.deep_logit.dense_layers)
-        return self.fm.head(inputs, addend=deep, out_layer=out_layer)
+        return self.fm.head(inputs, addend=deep, out_layer=out_layer, logits=logits)
 
     def call(self, inputs: TabularData, **kwargs) -> torch.Tensor:
         return self.forward(inputs)

@@ -1363,3 +1363,70 @@ def wide_rows_apply(opt: str, wide: torch.Tensor, state1: Optional[torch.Tensor]
     _cabi.check(_lib().mm_wide_rows_apply(wide.data_ptr(), _ptr(state1), _ptr(state2), W, arr, n, B, grad.data_ptr(), acc.data_ptr(),
                                           rep_map.data_ptr(), doff, m, _ptr(dense_grad), _ptr(bias), _ptr(bias_state1), _ptr(bias_state2),
                                           _cabi.OPTIMIZERS[opt], hyper.data_ptr(), _stream()), "mm_wide_rows_apply")
+
+
+def metrics_workspace_bytes(M: int, H: int) -> int:
+    return int(_lib().mm_metrics_workspace_bytes(int(M), int(H)))
+
+
+def metrics_update(z: torch.Tensor, losses: Sequence[str], targets: Sequence[torch.Tensor], state: torch.Tensor,
+                   workspace: torch.Tensor, num_buckets: int, pred_forms: Sequence[int],
+                   thresholds: Sequence[Sequence[float]], sample_weight: Optional[Sequence[Optional[torch.Tensor]]] = None,
+                   metric_weights: Optional[Sequence[Sequence[Optional[torch.Tensor]]]] = None) -> torch.Tensor:
+    """Add one batch of H <= 8 heads' logits z (H, M) into the fp64 metric state (mm_metrics_update): loss sums, AUC
+    histograms of num_buckets, confusion counts at each head's thresholds (<= 4) and squared-error sums, per metric set.
+    losses[h] in {"binary_crossentropy", "mse"}; targets[h] (M,) int32 / int64 / float32 / float64; pred_forms[h]
+    _cabi.PRED_ACT / PRED_HEAD; sample_weight[h] the loss weights (or None); metric_weights[s][h] the weights of metric set s
+    (1 or 2 sets; entries None: unweighted; default one unweighted set).  state (H, METRICS_SCALARS + 4 num_buckets)
+    float64, accumulated."""
+    _dev(z, "z", torch.float32)
+    H = len(losses)
+    if not 1 <= H <= _cabi.METRICS_MAX_HEADS:
+        raise ValueError(f"1..{_cabi.METRICS_MAX_HEADS} heads, got {H}")
+    if z.dim() != 2 or z.shape[0] != H or not z.is_contiguous():
+        raise ValueError(f"z must be a contiguous ({H}, M) matrix, got {tuple(z.shape)}")
+    M = z.shape[1]
+    T = int(num_buckets)
+    if not 2 <= T <= _cabi.METRICS_MAX_BUCKETS:
+        raise ValueError(f"num_buckets must lie in [2, {_cabi.METRICS_MAX_BUCKETS}], got {T}")
+    _dev(state, "state", torch.float64)
+    if tuple(state.shape) != (H, _cabi.METRICS_SCALARS + 4 * T) or not state.is_contiguous():
+        raise ValueError(f"state must be a contiguous ({H}, {_cabi.METRICS_SCALARS + 4 * T}) float64 matrix")
+    sets = [[None] * H] if metric_weights is None else [list(s) for s in metric_weights]
+    if len(sets) not in (1, 2) or any(len(s) != H for s in sets):
+        raise ValueError(f"one or two metric sets of {H} weight entries each")
+    sws = list(sample_weight) if sample_weight is not None else [None] * H
+    for name, seq in (("targets", targets), ("pred_forms", pred_forms), ("thresholds", thresholds), ("sample_weight", sws)):
+        if len(seq) != H:
+            raise ValueError(f"{name}: one entry per head ({H}), got {len(seq)}")
+    arr = (_cabi.MetricsHead * H)()
+    for h in range(H):
+        if losses[h] not in _cabi.LOSS_KINDS:
+            raise ValueError(f"losses must be among {sorted(_cabi.LOSS_KINDS)}, got {losses[h]!r}")
+        t = _dev(targets[h], f"targets[{h}]")
+        if t.numel() != M or not t.is_contiguous() or t.dtype not in _TARGET_DTYPES:
+            raise ValueError(f"targets[{h}] must be {M} contiguous int32 / int64 / float32 / float64 values")
+        ws = [sws[h]] + [s[h] for s in sets]
+        for i, w in enumerate(ws):
+            if w is not None and (_dev(w, "weights", torch.float32).numel() != M or not w.is_contiguous()):
+                raise ValueError(f"head {h}: sample / metric weights must be ({M},) contiguous float32")
+        thr = [float(v) for v in thresholds[h]]
+        if len(thr) > _cabi.METRICS_MAX_THRESHOLDS:
+            raise ValueError(f"head {h}: at most {_cabi.METRICS_MAX_THRESHOLDS} thresholds, got {len(thr)}")
+        arr[h].targets = t.data_ptr()
+        arr[h].sample_weight = _ptr(sws[h])
+        for s in range(len(sets)):
+            arr[h].metric_weights[s] = _ptr(sets[s][h])
+        arr[h].target_dtype = _TARGET_DTYPES[t.dtype]
+        arr[h].loss_kind = _cabi.LOSS_KINDS[losses[h]]
+        arr[h].pred_form = int(pred_forms[h])
+        arr[h].n_thresholds = len(thr)
+        for i, v in enumerate(thr):
+            arr[h].thresholds[i] = v
+    _dev(workspace, "workspace")
+    need = metrics_workspace_bytes(M, H)
+    if workspace.numel() * workspace.element_size() < need or not workspace.is_contiguous():
+        raise ValueError(f"workspace must hold {need} contiguous bytes")
+    _cabi.check(_lib().mm_metrics_update(z.data_ptr(), M, H, arr, T, len(sets), state.data_ptr(), workspace.data_ptr(),
+                                         workspace.numel() * workspace.element_size(), _stream()), "mm_metrics_update")
+    return state
