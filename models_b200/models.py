@@ -373,8 +373,8 @@ class Model(Block):
         return [y]
 
     def trainer(self, batch_size: int, group=None):
-        """The static-buffer training engine for batches of (up to) `batch_size` samples (train.DLRMTrainer or
-        train.DCNTrainer, by the body)."""
+        """The static-buffer training engine for batches of (up to) `batch_size` samples (train.trainer_for picks it by
+        the body: DLRMTrainer, DCNTrainer or DeepFMTrainer)."""
         from .train import trainer_for
 
         if getattr(self, "optimizer", None) is None:

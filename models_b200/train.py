@@ -1,7 +1,10 @@
-"""Training step of the DLRM path (SURVEY §8(f)-4): forward with saved activations, binary cross-entropy, backward and
-optimizer update as hand-written CUDA (include/mm_b200.h K14), behind the reference's `compile` / `fit` / `train_step`
+"""Training steps (SURVEY §8(f)-4): forward with saved activations, loss, backward and optimizer update as hand-written
+CUDA (include/mm_b200.h K14), behind the reference's `compile` / `fit` / `train_step`
 (merlin/models/tf/models/base.py:1121-1231; optimizers: tf.keras.optimizers.{SGD, Adagrad, Adam}, LazyAdam
-blocks/optimizer.py:342).
+blocks/optimizer.py:342).  One trainer per model (DLRMTrainer, DCNTrainer, TwoTowerTrainer, DeepFMTrainer; trainer_for picks)
+holds what is particular to it; the parts they share are methods of _StepTrainer: the dense arena, the table checks and
+optimizer state, a chain of Dense layers forward and backward, the concatenating input block, multi-hot pooling, the output
+heads, the update (apply_gradients), capture / replay.
 
 What a step launches (DLRM, bottom [.., D], top [...], BinaryOutput):
 
@@ -17,10 +20,11 @@ What a step launches (DLRM, bottom [.., D], top [...], BinaryOutput):
               refresh of the tensor-core operand copies (in place)
 
 Multi-hot features (ragged `name__values` + `name__offsets`, or (B, L) id matrices; combiners mean / sum / sqrtn) are pooled
-by mm_gather_bag / mm_gather_seq into a (B, D) buffer that the lookup + interaction kernels read as one more table of B rows
-at ids 0..B-1, so those kernels serve them unchanged; the backward's slice of that "table" is the pooled-row gradient, which
-mm_bag_grad_rows expands to one scaled row per id for one mm_sparse_rows_apply call per multi-hot table.  Ragged features are
-trained eagerly (their number of ids changes per batch); fixed-length ones can be captured like one-hot features.
+by mm_gather_bag / mm_gather_seq (_pool_bag), in DLRM into a (B, D) buffer that the lookup + interaction kernels read as one
+more table of B rows at ids 0..B-1, so those kernels serve them unchanged; the backward's slice of that "table" is the
+pooled-row gradient, which mm_bag_grad_rows expands to one scaled row per id for one mm_sparse_rows_apply call per multi-hot
+table.  Ragged features are trained eagerly (their number of ids changes per batch); fixed-length ones can be captured like
+one-hot features.
 
 DCNModel trains through DCNTrainer (below): the cross network's backward (mm_cross_backward per layer), the input block's
 backward straight into per-table slices (mm_concat_backward) and one sparse update per distinct embedding width.
@@ -32,7 +36,7 @@ kernel's sparse update (mm_wide_rows_apply).
 
 All Dense variables of the model are re-homed into ONE flat fp32 arena (gradients and optimizer slots mirror its layout), so
 the dense update is one launch and data-parallel training needs one all-reduce.  Every buffer is static: a step can be
-captured into a CUDA graph (`DLRMTrainer.capture()` / `replay()`), the learning rate lives in device memory.
+captured into a CUDA graph (`capture()` / `replay()`), the learning rate lives in device memory.
 """
 from __future__ import annotations
 
@@ -139,6 +143,11 @@ def _align(n: int, a: int = 64) -> int:
     return (n + a - 1) // a * a
 
 
+def _ld4(d: int) -> int:
+    """Row stride (a multiple of 4) of the fp32 buffer behind a (B, d) view."""
+    return (d + 3) // 4 * 4
+
+
 class DenseArena:
     """All Dense variables of a chain of layers in one flat fp32 buffer (kernel then bias per layer, 256-byte aligned);
     `grad`, `state1`, `state2` share the layout.  The layers' `kernel` / `bias` become views of it."""
@@ -197,12 +206,17 @@ def gather_slices(ids: torch.Tensor, slices: torch.Tensor, group) -> tuple:
 
 
 class _StepTrainer:
-    """What every static-buffer training step shares: the output heads, the dgrad of Dense layers, the update of the
-    dense arena and the embedding tables, CUDA-graph capture / replay, and the host-side bookkeeping.  A subclass sets
-    the attributes below in its __init__ and implements forward_backward / apply_gradients:
+    """What every static-buffer training step shares: the dense arena and its operand copies, the table checks and
+    optimizer state, a chain of Dense layers forward and backward, the concatenating input block forward and backward,
+    multi-hot pooling and its gradient expansion, the output heads, the update, CUDA-graph capture / replay, and the
+    host-side bookkeeping.  A subclass sets the attributes below in its __init__ (through the _init_* methods) and
+    implements forward_backward, which leaves _idx / _slices / _bags / _b for apply_gradients:
       model, body, opt, device, B, group, world, arena, hyper, head, outputs, H, losses, loss_weights,
       _tc_layers / _wsplit (Dense layers whose split operand copies follow the updates), _wide (see _init_wide),
       feats / tables / tstate1 / tstate2 / rep / tdense, oob, logits / _loss_all / loss."""
+
+    head: Optional[_Dense] = None  # the output layer; a trainer whose task builds its own targets has none
+    _multihot_refused: Optional[str] = None  # the model's name when its input block trains one-hot features only
 
     def _init_common(self, model, optimizer: Optimizer, batch_size: int, device, group) -> None:
         self.model, self.body, self.opt = model, model.body, optimizer
@@ -237,12 +251,54 @@ class _StepTrainer:
                 self._wide[li] = dict(wT=wT, wT_split=torch.zeros((ops.tc_padded_n(K), 2 * ops.tc_padded_k(N)), dtype=torch.bfloat16, device=self.device),
                                       dz_split=dzs)
 
-    def _init_table_state(self, optimizer: Optimizer) -> None:
+    def _init_dense(self, tc_layers: Sequence[_Dense], fused_layers: Sequence[_Dense]) -> None:
+        """One arena over tc_layers (run by mm_dense_tc: each gets a split operand copy that follows the updates) and
+        fused_layers (read as fp32 by a fused kernel), and the optimizer's hyper-parameters in device memory."""
+        self.arena = DenseArena(list(tc_layers) + list(fused_layers), self.opt, self.device)
+        self._tc_layers = list(tc_layers)
+        self._wsplit = [ops.split_weights(l.kernel) for l in self._tc_layers]
+        for l, ws in zip(self._tc_layers, self._wsplit):
+            l._w_split = ws  # the model's forward keeps reading the refreshed operand copies
+        self.hyper = torch.from_numpy(self.opt.hyper()).to(self.device)
+
+    def _init_tables(self, feats: Sequence[str], tables: Sequence, check_width: bool = True) -> None:
+        """feats / tables (one table per feature, by position) after the checks every sparse update needs, their
+        optimizer state, and the table positions of every embedding width."""
+        seen = set()
+        for f, t in zip(feats, tables):
+            if id(t) in seen:
+                raise NotImplementedError(f"feature {f!r}: training with a table shared between features is not implemented")
+            seen.add(id(t))
+            if not t.trainable:
+                raise NotImplementedError(f"feature {f!r}: frozen embedding tables are not implemented in the training step")
+            D = t.table.shape[1]
+            if check_width and (D % 4 or D > 128):
+                raise NotImplementedError(f"table {t.table_name!r}: embedding width {D} is not supported by the sparse update "
+                                          "(it needs a multiple of 4 no larger than 128)")
+        self.feats, self.tables = list(feats), list(tables)
+        opt = self.opt
         self.rep = [ops.fill_i32(torch.empty(t.table.shape[0], dtype=torch.int32, device=self.device), INT32_MAX) for t in self.tables]
-        self.tstate1 = [torch.full_like(t.table, optimizer.initial_accumulator_value) if optimizer.slots >= 1 else None for t in self.tables]
-        self.tstate2 = [torch.zeros_like(t.table) if optimizer.slots >= 2 else None for t in self.tables]
+        self.tstate1 = [torch.full_like(t.table, opt.initial_accumulator_value) if opt.slots >= 1 else None for t in self.tables]
+        self.tstate2 = [torch.zeros_like(t.table) if opt.slots >= 2 else None for t in self.tables]
         # tables with few rows (every id repeats many times per batch) sum their slices into a dense accumulator
         self.tdense = [torch.zeros_like(t.table) if t.table.shape[0] <= DENSE_PATH_MAX_ROWS else None for t in self.tables]
+        self._by_width: Dict[int, List[int]] = {}
+        for t, tb in enumerate(self.tables):
+            self._by_width.setdefault(tb.table.shape[1], []).append(t)
+        # multi-hot features (ragged bags, (B, L) id matrices), by table position: the expanded row gradients and the
+        # update's ids, created on the first batch that carries the feature as a bag (see _pool_bag)
+        self._bag_bufs: Dict[int, dict] = {}
+        self._bags: Dict[int, dict] = {}
+
+    def _chain_buffers(self, layers: Sequence[_Dense], split_last: bool = False) -> tuple:
+        """(h, h_split, dh) of a chain of Dense layers: the fp32 activations, the split operand every layer but the last
+        (split_last: every layer) emits for the layer that reads it, and the pre-activation gradients."""
+        f32 = dict(dtype=torch.float32, device=self.device)
+        h = [torch.zeros((self.B, l.units), **f32) for l in layers]
+        h_split = [torch.zeros((self.B, 2 * ops.tc_padded_k(l.units)), dtype=torch.bfloat16, device=self.device)
+                   for l in (layers if split_last else layers[:-1])]
+        dh = [torch.zeros((self.B, l.units), **f32) for l in layers]
+        return h, h_split, dh
 
     def _init_loss(self, B: int) -> None:
         f32 = dict(dtype=torch.float32, device=self.device)
@@ -255,9 +311,12 @@ class _StepTrainer:
         self._static: Optional[Dict[str, torch.Tensor]] = None
         self._static_y: Optional[List[torch.Tensor]] = None
 
-    def _check_targets(self, targets, b: int) -> list:
+    def _check_batch(self, b: int) -> None:
         if b > self.B or b < 1:
             raise ValueError(f"this trainer was compiled for batches of up to {self.B} samples, got {b}")
+
+    def _check_targets(self, targets, b: int) -> list:
+        self._check_batch(b)
         targets = list(targets) if isinstance(targets, (list, tuple)) else [targets]
         if len(targets) != self.H:
             raise ValueError(f"{self.H} target tensors expected (one per output), got {len(targets)}")
@@ -299,6 +358,132 @@ class _StepTrainer:
         return dict(weights=tb.table, indices=indices, grad_rows=grad_rows, rep_map=self.rep[t], state1=self.tstate1[t],
                     state2=self.tstate2[t], mirror=mirror, dense_grad=self.tdense[t])
 
+    # ---- a chain of Dense layers (layers li0 .. of _tc_layers) on b-row views of _chain_buffers -----------------------
+    def _chain_forward(self, op: torch.Tensor, K: int, li0: int, layers, h, h_split) -> None:
+        """The chain on the split operand `op` of its (b, K) input: fp32 activations into h, each layer's split output
+        (where h_split has one) into the operand of the next."""
+        for i, l in enumerate(layers):
+            nxt = h_split[i] if i < len(h_split) else None
+            ops.dense_tc(op, K, self._wsplit[li0 + i], l.units, l.bias, l.activation, out_f32=h[i], out_split=nxt)
+            op, K = nxt, l.units
+
+    def _chain_backward(self, li0: int, layers, h, dh, first_in, dx: Optional[torch.Tensor]) -> None:
+        """From dh[-1] (the pre-activation gradient of the last layer) down: per layer dW, db into the arena and the input
+        gradient with the relu mask of the layer below.  first_in: the chain's input, as (split operand, K) or as an fp32
+        matrix; dx: where the first layer's input gradient goes (None: nothing below needs it)."""
+        a = self.arena
+        for i in range(len(layers) - 1, 0, -1):
+            ops.dense_wgrad(h[i - 1], dh[i], a.view(a.grad, li0 + i, "kernel"), a.view(a.grad, li0 + i, "bias"))
+            self._dgrad(li0 + i, layers[i], dh[i], dh[i - 1], h[i - 1] if layers[i - 1].activation == "relu" else None)
+        if isinstance(first_in, tuple):
+            ops.dense_wgrad_split(first_in[0], first_in[1], dh[0], a.view(a.grad, li0, "kernel"), a.view(a.grad, li0, "bias"))
+        else:
+            ops.dense_wgrad(first_in, dh[0], a.view(a.grad, li0, "kernel"), a.view(a.grad, li0, "bias"))
+        if dx is not None:
+            self._dgrad(li0, layers[0], dh[0], dx, None)
+
+    # ---- the concatenating input block: x0 = [embedding rows | continuous columns] at their sorted-name offsets ------
+    def _input_forward(self, feats, tidx, cols: Dict[str, int], cont, inputs, x0: torch.Tensor, xs: torch.Tensor) -> None:
+        """Rows of the features `feats` (tables at positions `tidx`) and the continuous columns `cont` into x0 (b, d) at
+        the offsets `cols`, and x0's split operand xs.  One-hot features share one mm_gather_multi, a multi-hot feature is
+        pooled straight into its columns (_pool_bag).  Leaves the update's ids in _idx (None for a multi-hot feature)."""
+        ts, ids = [], []
+        for t, f in zip(tidx, feats):
+            x = get_feature(inputs, f)
+            kind = self.tables[t].lookup_kind(x)
+            if kind == "onehot":
+                ts.append(t)
+                ids.append(ops.as_index(x).reshape(-1))
+            elif self._multihot_refused:
+                raise NotImplementedError(f"feature {f!r}: training {self._multihot_refused} on multi-hot / ragged features "
+                                          "is not implemented")
+            else:
+                self._pool_bag(t, f, x, kind, x0, cols[f])
+        if ts:
+            if len({i.dtype for i in ids}) > 1:  # one launch reads one index dtype
+                ids = [i.to(torch.int64) for i in ids]
+            ops.gather_multi([self.tables[t].table for t in ts], ids, [cols[self.feats[t]] for t in ts], x0, self.oob)
+            for t, i in zip(ts, ids):
+                self._idx[t] = i
+        if cont:
+            ops.concat_columns([inputs[n] for n in cont], x0, [cols[n] for n in cont])
+        ops.split_rows(x0, out=xs)
+
+    def _input_backward(self, addends, feats, tidx, cols: Dict[str, int], fm: Optional[tuple] = None) -> None:
+        """The tables' columns of the summed (b, d) addends into each table's slice of _slices; fm = (x0, ds) adds the FM
+        term's input gradient (mm_fm_concat_backward)."""
+        slices = [(self._slices[t], cols[f]) for t, f in zip(tidx, feats)]
+        for s in range(0, len(slices), CONCAT_MAX_SLICES):
+            if fm is None:
+                ops.concat_backward(addends, slices[s:s + CONCAT_MAX_SLICES])
+            else:
+                ops.fm_concat_backward(addends, fm[0], fm[1], slices[s:s + CONCAT_MAX_SLICES])
+
+    # ---- multi-hot features -----------------------------------------------------------------------------------------
+    def _pool_bag(self, t: int, f: str, x, kind: str, out: torch.Tensor, col: int) -> None:
+        """The forward's combiner over the rows of multi-hot feature f (table t) into out[:, col:col+D], and in _bags[t]
+        what the backward needs: the ids, the buffer of the expanded row gradients and the update's ids."""
+        tb = self.tables[t]
+        D = tb.table.shape[1]
+        comb = tb.sequence_combiner or "mean"
+        if comb == "max":
+            raise NotImplementedError(f"feature {f!r}: training with the 'max' sequence combiner is not implemented")
+        buf = self._bag_bufs.setdefault(t, dict(rows=None, ids=None))
+        if kind == "bag":
+            values, offsets = x
+            ids, offs = ops.as_index(values).reshape(-1), ops.as_index(offsets)
+            ops.gather_bag(tb.table, ids, offs, comb, out, col, self.oob)
+        else:
+            if comb == "sqrtn":
+                raise ValueError(f"feature {f!r}: sequence_combiner 'sqrtn' is only defined for ragged inputs")
+            ids, offs = ops.as_index(x).reshape(x.shape[0], -1).contiguous(), None
+            ops.gather_seq(tb.table, ids, comb, out, col, self.oob)
+        nnz = ids.numel()
+        if buf["rows"] is None or buf["rows"].shape[0] < nnz:  # ragged: grows to the largest batch; fixed length: b * L
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError(f"feature {f!r}: the expanded gradient buffer cannot grow during graph capture")
+            buf["rows"] = torch.empty((nnz, D), dtype=torch.float32, device=self.device)
+        if kind == "bag" and (buf["ids"] is None or buf["ids"].shape[0] < nnz or buf["ids"].dtype != ids.dtype):
+            # the update's indices: a ragged batch's offsets need not cover every value (offsets[0] > 0, offsets[B] < nnz);
+            # the expansion marks such positions -1 so that no row the batch does not hold is updated
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError(f"feature {f!r}: the expanded id buffer cannot grow during graph capture")
+            buf["ids"] = torch.empty(max(nnz, 1), dtype=ids.dtype, device=self.device)
+        self._bags[t] = dict(ids=ids, offsets=offs, comb=comb, rows=buf["rows"][:nnz],
+                             apply_ids=buf["ids"][:nnz] if kind == "bag" else ids.reshape(-1))
+
+    def _bag_grads(self) -> None:
+        """Pooled-row gradient (the feature's slice of the backward) -> one scaled row per id."""
+        for t, bg in self._bags.items():
+            ops.bag_grad_rows(self._slices[t], bg["ids"], bg["offsets"], self.tables[t].table.shape[0], bg["comb"], bg["rows"],
+                              out_ids=bg["apply_ids"] if bg["offsets"] is not None else None)
+
+    # ---- the update ---------------------------------------------------------------------------------------------------
+    def _gradients_to_apply(self) -> tuple:
+        """(ids per table, slices per table, rows per slice, scale of the dense gradient) of the last forward_backward."""
+        return self._idx, self._slices, self._b, 1.0
+
+    def _apply_more(self) -> None:
+        """Variables outside the arena and the tables."""
+
+    def apply_gradients(self) -> None:
+        a = self.arena
+        ops.opt_tick(self.hyper)
+        idx, slices, rows, scale = self._gradients_to_apply()
+        ops.dense_apply(self.opt.kind, a.w, a.grad, a.state1, a.state2, self.hyper, grad_scale=scale)
+        for D, ts in self._by_width.items():
+            onehot = [t for t in ts if t not in self._bags]
+            for s in range(0, len(onehot), SPARSE_MAX_TABLES):
+                chunk = onehot[s:s + SPARSE_MAX_TABLES]
+                ops.sparse_rows_apply(self.opt.kind, [self._table_args(t, idx[t], slices[t]) for t in chunk], rows, D, self.hyper)
+            for t in ts:
+                bag = self._bags.get(t)
+                if bag is not None and bag["rows"].shape[0] > 0:  # a multi-hot table: its own call over the nnz expanded rows
+                    tab = self._table_args(t, bag["apply_ids"], bag["rows"])
+                    ops.sparse_rows_apply(self.opt.kind, [tab], bag["rows"].shape[0], D, self.hyper)
+        self._apply_more()
+        self._refresh_operands()
+
     def _refresh_operands(self) -> None:
         for l, ws in zip(self._tc_layers, self._wsplit):
             ops.split_weights(l.kernel, out=ws)
@@ -315,7 +500,8 @@ class _StepTrainer:
         from .core import bump_weights_version
 
         self.steps += 1
-        self.head._bias_host = None
+        if self.head is not None:
+            self.head._bias_host = None
         bump_weights_version()  # forward graphs captured earlier hold scalars / operand copies of the old variables
 
     # ---- CUDA-graph replay over static input buffers ------------------------------------------------------------
@@ -447,30 +633,16 @@ class DLRMTrainer(_StepTrainer):
                 raise NotImplementedError(f"{l.name}: training supports relu / linear tower activations, got {l.activation!r}")
         if self.head.input_dim > 256:
             raise NotImplementedError("the output layer's input must be <= 256 wide")
-        self.arena = DenseArena(self.bottom + self.top + [self.head], optimizer, self.device)
-        self._tc_layers = self.bottom + self.top
-        self._wsplit = [ops.split_weights(l.kernel) for l in self._tc_layers]
-        for l, ws in zip(self._tc_layers, self._wsplit):
-            l._w_split = ws  # the forward path of this model keeps reading the refreshed operand copies
-        self.hyper = torch.from_numpy(optimizer.hyper()).to(self.device)
+        self._init_dense(self.bottom + self.top, [self.head])
         self._init_wide(lambda li: li != 0)  # the first bottom layer needs no input gradient
 
-        # ---- tables
+        # ---- tables (their width is one of can_emit_split's)
         emb = body.embeddings
-        self.feats = list(emb.feature_names)
         self.slots = body.slots()
         self.D = body.embedding_dim
-        self.tables = [emb.feature_to_table[f] for f in self.feats]
-        seen = set()
-        for t in self.tables:
-            if id(t) in seen:
-                raise NotImplementedError("training with a table shared between features is not implemented")
-            seen.add(id(t))
-            if not t.trainable:
-                raise NotImplementedError("frozen embedding tables are not implemented in the training step")
+        self._init_tables(emb.feature_names, [emb.feature_to_table[f] for f in emb.feature_names], check_width=False)
         T, B, D = len(self.tables), self.B, self.D
         self.slices = torch.zeros((T, B, D), dtype=torch.float32, device=self.device)
-        self._init_table_state(optimizer)
 
         # ---- activations and gradients
         # operand-format rows for the lookup + interaction kernels (forward and backward) (D = 64, mirrors enabled): the tables' mirrors (the
@@ -484,32 +656,25 @@ class DLRMTrainer(_StepTrainer):
         f32 = dict(dtype=torch.float32, device=self.device)
         self.K0 = len(body.continuous.features)
         self.x0_split = torch.zeros((B, 2 * ops.tc_padded_k(self.K0)), dtype=torch.bfloat16, device=self.device)
-        self.h = [torch.zeros((B, l.units), **f32) for l in self.bottom]
-        n_split = len(self.bottom) if self.operand_rows else len(self.bottom) - 1
-        self.h_split = [torch.zeros((B, 2 * ops.tc_padded_k(l.units)), dtype=torch.bfloat16, device=self.device) for l in self.bottom[:n_split]]
+        self.h, self.h_split, self.dh = self._chain_buffers(self.bottom, split_last=self.operand_rows)
         F = len(self.slots)
         self.OW = D + F * (F - 1) // 2
-        self.ldA = (self.OW + 3) // 4 * 4
+        self.ldA = _ld4(self.OW)
         self.A = None if self.operand_rows else torch.zeros((B, self.ldA), **f32)
         self.dA = torch.zeros((B, self.ldA), **f32)
         self.A_split = torch.zeros((B, 2 * ops.tc_padded_k(self.OW)), dtype=torch.bfloat16, device=self.device)
-        self.t = [torch.zeros((B, l.units), **f32) for l in self.top]
-        self.t_split = [torch.zeros((B, 2 * ops.tc_padded_k(l.units)), dtype=torch.bfloat16, device=self.device) for l in self.top[:-1]]
-        self.dt = [torch.zeros((B, l.units), **f32) for l in self.top]
-        self.dh = [torch.zeros((B, l.units), **f32) for l in self.bottom]
+        self.t, self.t_split, self.dt = self._chain_buffers(self.top)
         self._init_loss(B)
         self.oob = emb.counter(self.device)
-        # multi-hot features (ragged bags, (B, L) id matrices), by table position: pooled rows, their operand copy, the
-        # expanded row gradients; created on the first batch that carries the feature as a bag (see _indices)
-        self._bag_bufs: Dict[int, dict] = {}
+        # multi-hot features, by table position: the pooled rows and their operand copy, created with the first bag
+        self._pooled: Dict[int, dict] = {}
         self._iota: Optional[torch.Tensor] = None
-        self._bags: Dict[int, dict] = {}
 
     # ---- one step on device tensors ------------------------------------------------------------------------------
     def _indices(self, inputs, b: Optional[int] = None) -> List[torch.Tensor]:
-        """Ids the lookup + interaction kernels read per table.  A multi-hot feature is pooled first (gather_bag /
-        gather_seq, the forward's combiner) into a (B, D) buffer that those kernels then read as one more table of b rows
-        at ids 0..b-1; its backward returns the pooled-row gradient, which _bag_grads expands to one row per id."""
+        """Ids the lookup + interaction kernels read per table.  A multi-hot feature is pooled first (_pool_bag, the
+        forward's combiner) into a (B, D) buffer that those kernels then read as one more table of b rows at ids 0..b-1;
+        its backward returns the pooled-row gradient, which _bag_grads expands to one row per id."""
         idx: List[torch.Tensor] = []
         self._bags = {}
         for t, f in enumerate(self.feats):
@@ -518,85 +683,42 @@ class DLRMTrainer(_StepTrainer):
             if kind == "onehot":
                 idx.append(ops.fused_ids(x))
                 continue
+            if self.group is not None:  # gather_slices exchanges (T, B, D) slices: one row per sample and table
+                raise NotImplementedError(f"feature {f!r}: training multi-hot features with a process group is not implemented")
             if b is None:  # the pooled rows and the ids that read them must agree on the batch size
                 b = batch_size_of(inputs)
-            self._bags[t] = self._pool(t, f, x, kind, b)
+            buf = self._pooled.get(t)
+            if buf is None:
+                if self._iota is None:
+                    self._iota = torch.arange(self.B, dtype=torch.int32, device=self.device)
+                buf = self._pooled[t] = dict(
+                    pooled=torch.zeros((self.B, self.D), dtype=torch.float32, device=self.device),
+                    split=torch.zeros((self.B, 2 * ops.tc_padded_k(self.D)), dtype=torch.bfloat16, device=self.device) if self.operand_rows else None)
+            pooled, split = buf["pooled"][:b], None
+            self._pool_bag(t, f, x, kind, pooled, 0)
+            if self.operand_rows:
+                split = buf["split"][:b]
+                ops.split_rows(pooled, out=split)
+            self._bags[t].update(pooled=pooled, split=split)
             idx.append(self._iota[:b])
         return idx
-
-    def _pool(self, t: int, f: str, x, kind: str, b: int) -> dict:
-        tb, D = self.tables[t], self.D
-        comb = tb.sequence_combiner or "mean"
-        if comb == "max":
-            raise NotImplementedError(f"feature {f!r}: training with the 'max' sequence combiner is not implemented")
-        if self.group is not None:  # gather_slices exchanges (T, B, D) slices: one row per sample and table
-            raise NotImplementedError(f"feature {f!r}: training multi-hot features with a process group is not implemented")
-        buf = self._bag_bufs.get(t)
-        if buf is None:
-            if self._iota is None:
-                self._iota = torch.arange(self.B, dtype=torch.int32, device=self.device)
-            buf = self._bag_bufs[t] = dict(
-                pooled=torch.zeros((self.B, D), dtype=torch.float32, device=self.device),
-                split=torch.zeros((self.B, 2 * ops.tc_padded_k(D)), dtype=torch.bfloat16, device=self.device) if self.operand_rows else None,
-                rows=None, ids=None)
-        pooled = buf["pooled"][:b]
-        if kind == "bag":
-            values, offsets = x
-            ids, offs = ops.as_index(values).reshape(-1), ops.as_index(offsets)
-            ops.gather_bag(tb.table, ids, offs, comb, pooled, 0, self.oob)
-        else:
-            if comb == "sqrtn":
-                raise ValueError(f"feature {f!r}: sequence_combiner 'sqrtn' is only defined for ragged inputs")
-            ids, offs = ops.as_index(x).reshape(x.shape[0], -1).contiguous(), None
-            ops.gather_seq(tb.table, ids, comb, pooled, 0, self.oob)
-        nnz = ids.numel()
-        if buf["rows"] is None or buf["rows"].shape[0] < nnz:  # ragged: grows to the largest batch; fixed length: b * L
-            if torch.cuda.is_current_stream_capturing():
-                raise RuntimeError(f"feature {f!r}: the expanded gradient buffer cannot grow during graph capture")
-            buf["rows"] = torch.empty((nnz, D), dtype=torch.float32, device=self.device)
-        if kind == "bag" and (buf["ids"] is None or buf["ids"].shape[0] < nnz or buf["ids"].dtype != ids.dtype):
-            # the update's indices: a ragged batch's offsets need not cover every value (offsets[0] > 0, offsets[B] < nnz);
-            # the expansion marks such positions -1 so that no row the batch does not hold is updated
-            if torch.cuda.is_current_stream_capturing():
-                raise RuntimeError(f"feature {f!r}: the expanded id buffer cannot grow during graph capture")
-            buf["ids"] = torch.empty(max(nnz, 1), dtype=ids.dtype, device=self.device)
-        split = None
-        if self.operand_rows:
-            split = buf["split"][:b]
-            ops.split_rows(pooled, out=split)
-        return dict(ids=ids, offsets=offs, comb=comb, pooled=pooled, split=split, rows=buf["rows"][:nnz],
-                    apply_ids=buf["ids"][:nnz] if kind == "bag" else ids.reshape(-1))
-
-    def _bag_grads(self) -> None:
-        """Pooled-row gradient (the feature's slice of the interaction backward) -> one scaled row per id."""
-        for t, bg in self._bags.items():
-            ops.bag_grad_rows(self._slices[t], bg["ids"], bg["offsets"], self.tables[t].table.shape[0], bg["comb"], bg["rows"],
-                              out_ids=bg["apply_ids"] if bg["offsets"] is not None else None)
 
     def forward_backward(self, inputs: Dict[str, torch.Tensor], targets, sample_weight=None) -> None:
         """Forward (activations saved), loss and backward: fills the gradient arena and the IndexedSlices.  Batches smaller
         than the compiled size run in the leading rows of the same buffers.  targets: one tensor per output (a bare tensor
         for a single output); sample_weight: one (b,) tensor for every output, or a list with one per output."""
-        a = self.arena
-        nb, nt = len(self.bottom), len(self.top)
+        nb = len(self.bottom)
         D = self.D
         self._loss_all.zero_()
         cont = self.body.continuous(inputs)
         pieces = [cont[k] for k in sorted(cont)]
         b = int(pieces[0].shape[0])
         targets = self._check_targets(targets, b)
-
-        def v(t):
-            return t[:b]
-
-        h, t_, dt, dh = [v(x) for x in self.h], [v(x) for x in self.t], [v(x) for x in self.dt], [v(x) for x in self.dh]
-        ops.concat_split(pieces, out=v(self.x0_split))  # the concatenated continuous columns exist only as this operand
-        # -- bottom tower
-        op, K = v(self.x0_split), self.K0
-        for i, l in enumerate(self.bottom):
-            nxt = v(self.h_split[i]) if i < len(self.h_split) else None
-            ops.dense_tc(op, K, self._wsplit[i], l.units, l.bias, l.activation, out_f32=h[i], out_split=nxt)
-            op, K = nxt, l.units
+        h, t_, dt, dh = ([x[:b] for x in bufs] for bufs in (self.h, self.t, self.dt, self.dh))
+        h_split, x0_split, A_split = [x[:b] for x in self.h_split], self.x0_split[:b], self.A_split[:b]
+        ops.concat_split(pieces, out=x0_split)  # the concatenated continuous columns exist only as this operand
+        # -- bottom tower (operand_rows: its last layer emits the split bottom vector too)
+        self._chain_forward(x0_split, self.K0, 0, self.bottom, h, h_split)
         # -- lookup + interaction (fp32 rows)
         idx = self._indices(inputs, b)
         tabs = [self._bags[t]["pooled"] if t in self._bags else tb.table for t, tb in enumerate(self.tables)]
@@ -608,80 +730,43 @@ class DLRMTrainer(_StepTrainer):
         if self.operand_rows:
             # operand-format rows in, split-bf16 operand of the top tower out: no fp32 copy of [bottom | interactions] exists
             A_view = None
-            ops.dlrm_lookup_interact(mirrors, idx, tslots, rows, D, v(self.h_split[-1]), bslot,
-                                     v(self.A_split), self.oob, operand_rows=True)
+            ops.dlrm_lookup_interact(mirrors, idx, tslots, rows, D, h_split[-1], bslot, A_split, self.oob, operand_rows=True)
         else:
             A_view = self.A[:b, :self.OW]
             ops.dlrm_lookup_interact(tabs, idx, tslots, rows, D, h[-1], bslot, A_view, self.oob)
-            ops.split_rows(A_view, out=v(self.A_split))
+            ops.split_rows(A_view, out=A_split)
         # -- top tower
-        op, K = v(self.A_split), self.OW
-        for i, l in enumerate(self.top):
-            nxt = v(self.t_split[i]) if i < nt - 1 else None
-            ops.dense_tc(op, K, self._wsplit[nb + i], l.units, l.bias, l.activation, out_f32=t_[i], out_split=nxt)
-            op, K = nxt, l.units
+        self._chain_forward(A_split, self.OW, nb, self.top, t_, [x[:b] for x in self.t_split])
         # -- output layer + loss, forward and backward
         self._heads(t_[-1], targets, dt[-1], self.top[-1].activation == "relu", sample_weight, b)
-        # -- top tower backward
-        for i in range(nt - 1, -1, -1):
-            l = self.top[i]
-            if i == 0 and A_view is None:
-                ops.dense_wgrad_split(v(self.A_split), self.OW, dt[0], a.view(a.grad, nb, "kernel"), a.view(a.grad, nb, "bias"))
-            else:
-                ops.dense_wgrad(t_[i - 1] if i > 0 else A_view, dt[i], a.view(a.grad, nb + i, "kernel"), a.view(a.grad, nb + i, "bias"))
-            if i > 0:
-                self._dgrad(nb + i, l, dt[i], dt[i - 1], t_[i - 1] if self.top[i - 1].activation == "relu" else None)
-            else:
-                self._dgrad(nb, l, dt[0], dA_view, None)
+        # -- top tower backward: its input exists as fp32 only without operand_rows
+        self._chain_backward(nb, self.top, t_, dt, (A_split, self.OW) if A_view is None else A_view, dA_view)
         # -- interaction + lookup backward
-        self._slices = [self.slices[t][:b] for t in range(len(tabs))]
+        self._slices = [s[:b] for s in self.slices]
         if self.operand_rows:
-            ops.dlrm_interact_backward(mirrors, idx, tslots, rows, D, v(self.h_split[-1]), bslot, dA_view,
+            ops.dlrm_interact_backward(mirrors, idx, tslots, rows, D, h_split[-1], bslot, dA_view,
                                        self._slices, dh[-1], mask_bottom=self.bottom[-1].activation == "relu", operand_rows=True)
         else:
             ops.dlrm_interact_backward(tabs, idx, tslots, rows, D, h[-1], bslot, dA_view, self._slices, dh[-1],
                                        mask_bottom=self.bottom[-1].activation == "relu")
         self._bag_grads()
         # -- bottom tower backward
-        for i in range(nb - 1, -1, -1):
-            l = self.bottom[i]
-            if i > 0:
-                ops.dense_wgrad(h[i - 1], dh[i], a.view(a.grad, i, "kernel"), a.view(a.grad, i, "bias"))
-            else:
-                ops.dense_wgrad_split(v(self.x0_split), self.K0, dh[0], a.view(a.grad, 0, "kernel"), a.view(a.grad, 0, "bias"))
-            if i > 0:
-                self._dgrad(i, l, dh[i], dh[i - 1], h[i - 1] if self.bottom[i - 1].activation == "relu" else None)
+        self._chain_backward(0, self.bottom, h, dh, (x0_split, self.K0), None)
         self._idx, self._b = idx, b
 
-    def apply_gradients(self) -> None:
-        a = self.arena
-        ops.opt_tick(self.hyper)
-        idx, slices, Bt = self._idx, self._slices, self._b
-        scale = 1.0
-        if self.world > 1:
-            import torch.distributed as dist
+    def _gradients_to_apply(self) -> tuple:
+        """Data parallel: the dense gradients are summed over the ranks (and scaled by 1 / world in the update), every
+        rank applies every rank's IndexedSlices."""
+        if self.world == 1:
+            return super()._gradients_to_apply()
+        import torch.distributed as dist
 
-            dist.all_reduce(a.grad, group=self.group)
-            scale = 1.0 / self.world
-            ids32 = torch.stack([ops.widen_index(i).to(torch.int32) for i in idx])
-            all_ids, all_sl = gather_slices(ids32, torch.stack(slices), self.group)
-            all_sl.mul_(scale)
-            idx = [all_ids[t] for t in range(all_ids.shape[0])]
-            slices = [all_sl[t] for t in range(all_sl.shape[0])]
-            Bt = self._b * self.world
-        ops.dense_apply(self.opt.kind, a.w, a.grad, a.state1, a.state2, self.hyper, grad_scale=scale)
-        tabs = []
-        for t in range(len(self.tables)):
-            tab = self._table_args(t, idx[t], slices[t])
-            bag = self._bags.get(t)
-            if bag is None:
-                tabs.append(tab)
-            elif bag["rows"].shape[0] > 0:  # a multi-hot table: its own call over the nnz expanded rows
-                tab.update(indices=bag["apply_ids"], grad_rows=bag["rows"])
-                ops.sparse_rows_apply(self.opt.kind, [tab], bag["rows"].shape[0], self.D, self.hyper)
-        if tabs:
-            ops.sparse_rows_apply(self.opt.kind, tabs, Bt, self.D, self.hyper)
-        self._refresh_operands()
+        dist.all_reduce(self.arena.grad, group=self.group)
+        scale = 1.0 / self.world
+        ids32 = torch.stack([ops.widen_index(i).to(torch.int32) for i in self._idx])
+        all_ids, all_sl = gather_slices(ids32, torch.stack(self._slices), self.group)
+        all_sl.mul_(scale)
+        return list(all_ids), list(all_sl), self._b * self.world, scale
 
 
 class DCNTrainer(_StepTrainer):
@@ -697,6 +782,8 @@ class DCNTrainer(_StepTrainer):
               (B, D_t) IndexedSlices buffer
     update    mm_opt_tick, mm_dense_apply over the arena [cross layers, deep layers, head], one mm_sparse_rows_apply per
               distinct embedding width, mm_split_weights refresh of the operand copies the model's forward reads."""
+
+    _multihot_refused = "DCNModel"
 
     def __init__(self, model, optimizer: Optimizer, batch_size: int, device=None, group=None):
         from .blocks import Cross
@@ -734,39 +821,19 @@ class DCNTrainer(_StepTrainer):
         emb = ib.embeddings
         self.cols, widths, d = ib.layout()
         self.d = d
-        self.feats = list(emb.feature_names) if emb is not None else []
-        self.tables = [emb.feature_to_table[f] for f in self.feats]
-        seen = set()
-        for f, t in zip(self.feats, self.tables):
-            if id(t) in seen:
-                raise NotImplementedError(f"feature {f!r}: training with a table shared between features is not implemented")
-            seen.add(id(t))
-            if not t.trainable:
-                raise NotImplementedError(f"feature {f!r}: frozen embedding tables are not implemented in the training step")
-            D = t.table.shape[1]
-            if D % 4 or D > 128:
-                raise NotImplementedError(f"table {t.table_name!r}: embedding width {D} is not supported by the sparse update "
-                                          "(it needs a multiple of 4 no larger than 128)")
+        feats = list(emb.feature_names) if emb is not None else []
+        self._init_tables(feats, [emb.feature_to_table[f] for f in feats])
         self.cont = sorted(ib.continuous.features) if ib.continuous is not None else []
 
-        self.arena = DenseArena(self.cross + self.deep + [self.head], optimizer, self.device)
-        self._tc_layers = self.cross + self.deep
-        self._wsplit = [ops.split_weights(l.kernel) for l in self._tc_layers]
-        for l, ws in zip(self._tc_layers, self._wsplit):
-            l._w_split = ws  # the model's forward keeps reading the refreshed operand copies
-        self.hyper = torch.from_numpy(optimizer.hyper()).to(self.device)
+        self._init_dense(self.cross + self.deep, [self.head])
         # every layer needs its input gradient (x0 is the tables' rows); mm_cross_backward writes the split of a cross
         # layer's dz itself
         L = len(self.cross)
         self._init_wide(lambda li: True, dz_split_given=lambda li: li < L)
-        self._init_table_state(optimizer)
-        self._by_width: Dict[int, List[int]] = {}
-        for t, tb in enumerate(self.tables):
-            self._by_width.setdefault(tb.table.shape[1], []).append(t)
 
         # ---- activations and gradients (fp32 (B, d) buffers with a row stride that is a multiple of 4)
         B = self.B
-        self.ld = (d + 3) // 4 * 4
+        self.ld = _ld4(d)
         f32 = dict(dtype=torch.float32, device=self.device)
         bf = dict(dtype=torch.bfloat16, device=self.device)
         Kp = ops.tc_padded_k(d)
@@ -778,9 +845,7 @@ class DCNTrainer(_StepTrainer):
         self.xs = [torch.zeros((B, 2 * Kp), **bf) for _ in range(L + (1 if self.stacked else 0))]  # operands of x_0 .. x_L
         self.z = [mat() for _ in range(L)]
         self.xf = [mat() for _ in range(min(L, 2))]  # fp32 x_1 .. x_L, alternating (only the residual of the next layer)
-        self.h = [torch.zeros((B, l.units), **f32) for l in self.deep]
-        self.h_split = [torch.zeros((B, 2 * ops.tc_padded_k(l.units)), **bf) for l in self.deep[:-1]]
-        self.dh = [torch.zeros((B, l.units), **f32) for l in self.deep]
+        self.h, self.h_split, self.dh = self._chain_buffers(self.deep)
         self.g, self.p, self.acc, self.dz = mat(), mat(), mat(), mat()
         self.dz_split = torch.zeros((B, 2 * Kp), **bf)
         self.slices = [torch.zeros((B, tb.table.shape[1]), **f32) for tb in self.tables]
@@ -807,26 +872,17 @@ class DCNTrainer(_StepTrainer):
         self._init_loss(B)
         self.oob = emb.counter(self.device) if emb is not None else None
 
-    def _ids(self, inputs) -> List[torch.Tensor]:
-        idx = []
-        for f, tb in zip(self.feats, self.tables):
-            x = get_feature(inputs, f)
-            if tb.lookup_kind(x) != "onehot":
-                raise NotImplementedError(f"feature {f!r}: training DCNModel on multi-hot / ragged features is not implemented")
-            idx.append(ops.as_index(x).reshape(-1))
-        if len({i.dtype for i in idx}) > 1:
-            idx = [i.to(torch.int64) for i in idx]
-        return idx
-
     def forward_backward(self, inputs: Dict[str, torch.Tensor], targets, sample_weight=None) -> None:
         """Forward (activations saved), loss and backward: fills the gradient arena and the IndexedSlices.  Batches smaller
         than the compiled size run in the leading rows of the same buffers."""
         a = self.arena
-        d, L, nd = self.d, len(self.cross), len(self.deep)
+        d, L = self.d, len(self.cross)
         self._loss_all.zero_()
         b = batch_size_of(inputs)
         targets = self._check_targets(targets, b)
-        idx = self._ids(inputs)
+        tidx = range(len(self.tables))
+        self._idx: List[Optional[torch.Tensor]] = [None] * len(self.tables)
+        self._slices = [s[:b] for s in self.slices]
 
         def v(t):
             return t[:b]
@@ -836,11 +892,7 @@ class DCNTrainer(_StepTrainer):
 
         # -- input block: x0 = [embeddings | continuous] in sorted-name order
         x0 = vd(self.x0)
-        if self.tables:
-            ops.gather_multi([tb.table for tb in self.tables], idx, [self.cols[f] for f in self.feats], x0, self.oob)
-        if self.cont:
-            ops.concat_columns([inputs[n] for n in self.cont], x0, [self.cols[n] for n in self.cont])
-        ops.split_rows(x0, out=v(self.xs[0]))
+        self._input_forward(self.feats, tidx, self.cols, self.cont, inputs, x0, v(self.xs[0]))
         # -- cross network
         x = x0
         cat = v(self.cat) if not self.stacked else None
@@ -857,11 +909,7 @@ class DCNTrainer(_StepTrainer):
         h, dh = [v(t) for t in self.h], [v(t) for t in self.dh]
         if cat is not None:
             h[-1] = cat[:, self.doff:self.doff + self.deep[-1].units]
-        op, K = op0, d
-        for i, l in enumerate(self.deep):
-            nxt = v(self.h_split[i]) if i < nd - 1 else None
-            ops.dense_tc(op, K, self._wsplit[L + i], l.units, l.bias, l.activation, out_f32=h[i], out_split=nxt)
-            op, K = nxt, l.units
+        self._chain_forward(op0, d, L, self.deep, h, [v(t) for t in self.h_split])
         # -- output layer + loss, forward and backward
         relu_last = self.deep[-1].activation == "relu"
         g = vd(self.g)
@@ -874,15 +922,8 @@ class DCNTrainer(_StepTrainer):
             if relu_last:
                 ops.relu_mask(dh[-1], h[-1])
             ops.concat_columns([dcat[:, self.coff:self.coff + d]], g, [0])  # the cross branch's output gradient
-        # -- deep tower backward
-        for i in range(nd - 1, -1, -1):
-            l = self.deep[i]
-            if i > 0:
-                ops.dense_wgrad(h[i - 1], dh[i], a.view(a.grad, L + i, "kernel"), a.view(a.grad, L + i, "bias"))
-                self._dgrad(L + i, l, dh[i], dh[i - 1], h[i - 1] if self.deep[i - 1].activation == "relu" else None)
-            else:
-                ops.dense_wgrad_split(op0, d, dh[0], a.view(a.grad, L, "kernel"), a.view(a.grad, L, "bias"))
-                self._dgrad(L, l, dh[0], g if self.stacked else vd(self.ddeep), None)
+        # -- deep tower backward: its input gradient adds to x_L's (stacked) or is an addend of dx0 (parallel)
+        self._chain_backward(L, self.deep, h, dh, (op0, d), g if self.stacked else vd(self.ddeep))
         # -- cross network backward (g: gradient into x_{l+1}; p: dgrad of the layer above)
         p, acc, dz, dzs = vd(self.p), vd(self.acc), vd(self.dz), v(self.dz_split)
         for l in range(L - 1, -1, -1):
@@ -890,12 +931,9 @@ class DCNTrainer(_StepTrainer):
             ops.dense_wgrad_split(v(self.xs[l]), d, dz, a.view(a.grad, l, "kernel"), a.view(a.grad, l, "bias"))
             self._dgrad(l, self.cross[l], dz, p, None, dz_split=dzs)
         # -- input block backward: dx0 = g_1 + p_0 + acc (+ the deep branch's input gradient), the tables' columns only
-        self._slices = [v(s) for s in self.slices]
         addends = [g, p, acc] + ([vd(self.ddeep)] if not self.stacked else [])
-        slices = [(s, self.cols[f]) for s, f in zip(self._slices, self.feats)]
-        for s in range(0, len(slices), CONCAT_MAX_SLICES):
-            ops.concat_backward(addends, slices[s:s + CONCAT_MAX_SLICES])
-        self._idx, self._b = idx, b
+        self._input_backward(addends, self.feats, tidx, self.cols)
+        self._b = b
 
     def _dcn_heads(self, x: torch.Tensor, targets, dx: torch.Tensor, mask_relu: bool, sample_weight, b: int) -> None:
         """The output heads on x (b, K): the fused loss kernel for K <= 256, otherwise the wide-head composition."""
@@ -912,17 +950,6 @@ class DCNTrainer(_StepTrainer):
                           a.view(a.grad, hi, "bias"), loss_weights=self.loss_weights, mask_relu=False, sample_weight=sample_weight)
         ops.dense_wgrad_split(xs, K, dz, a.view(a.grad, hi, "kernel"), None)
         ops.dense_dgrad(dz, self.head.kernel, dx, mask=x if mask_relu else None)
-
-    def apply_gradients(self) -> None:
-        a = self.arena
-        ops.opt_tick(self.hyper)
-        ops.dense_apply(self.opt.kind, a.w, a.grad, a.state1, a.state2, self.hyper)
-        for D, ts in self._by_width.items():
-            for s in range(0, len(ts), SPARSE_MAX_TABLES):
-                chunk = ts[s:s + SPARSE_MAX_TABLES]
-                ops.sparse_rows_apply(self.opt.kind, [self._table_args(t, self._idx[t], self._slices[t]) for t in chunk], self._b, D,
-                                      self.hyper)
-        self._refresh_operands()
 
 
 class TwoTowerTrainer(_StepTrainer):
@@ -973,8 +1000,7 @@ class TwoTowerTrainer(_StepTrainer):
         self.l2 = body.post is not None
         self.H = 1
         self.towers = []
-        self.feats, self.tables = [], []
-        seen = set()
+        feats_all, tables = [], []
         for tb in (body.query, body.item):
             mlp = tb.mlp
             if not isinstance(mlp, MLP) or mlp.has_normalization or mlp.dropout:
@@ -986,22 +1012,11 @@ class TwoTowerTrainer(_StepTrainer):
             cols, widths, d = ib.layout()
             emb = ib.embeddings
             feats = list(emb.feature_names) if emb is not None else []
-            first = len(self.tables)
-            for f in feats:
-                t = emb.feature_to_table[f]
-                if id(t) in seen:
-                    raise NotImplementedError(f"feature {f!r}: training with a table shared between features is not implemented")
-                seen.add(id(t))
-                if not t.trainable:
-                    raise NotImplementedError(f"feature {f!r}: frozen embedding tables are not implemented in the training step")
-                D = t.table.shape[1]
-                if D % 4 or D > 128:
-                    raise NotImplementedError(f"table {t.table_name!r}: embedding width {D} is not supported by the sparse update "
-                                              "(it needs a multiple of 4 no larger than 128)")
-                self.feats.append(f)
-                self.tables.append(t)
+            first = len(tables)
+            feats_all += feats
+            tables += [emb.feature_to_table[f] for f in feats]
             cont = sorted(ib.continuous.features) if ib.continuous is not None else []
-            self.towers.append(dict(name=tb.name, layers=mlp.dense_layers, cols=cols, d=d, feats=feats, tidx=list(range(first, len(self.tables))),
+            self.towers.append(dict(name=tb.name, layers=mlp.dense_layers, cols=cols, d=d, feats=feats, tidx=list(range(first, len(tables))),
                                     cont=cont, oob=emb.counter(self.device) if emb is not None else None))
         out_w = {t["layers"][-1].units for t in self.towers}
         if len(out_w) != 1:
@@ -1010,13 +1025,8 @@ class TwoTowerTrainer(_StepTrainer):
         if ops.tc_padded_k(self.D) > 128:
             raise NotImplementedError(f"tower output width {self.D}: the in-batch soft-max kernels take up to 128")
 
-        layers = [l for t in self.towers for l in t["layers"]]
-        self.arena = DenseArena(layers, optimizer, self.device)
-        self._tc_layers = layers
-        self._wsplit = [ops.split_weights(l.kernel) for l in layers]
-        for l, ws in zip(layers, self._wsplit):
-            l._w_split = ws  # the model's forward keeps reading the refreshed operand copies
-        self.hyper = torch.from_numpy(optimizer.hyper()).to(self.device)
+        self._init_tables(feats_all, tables)
+        self._init_dense([l for t in self.towers for l in t["layers"]], [])
         first_layer = {}
         li = 0
         for t in self.towers:
@@ -1024,10 +1034,6 @@ class TwoTowerTrainer(_StepTrainer):
             first_layer[li] = bool(t["feats"])  # the first layer needs its input gradient only when the tower has tables
             li += len(t["layers"])
         self._init_wide(lambda i: first_layer.get(i, True))
-        self._init_table_state(optimizer)
-        self._by_width: Dict[int, List[int]] = {}
-        for t, tb in enumerate(self.tables):
-            self._by_width.setdefault(tb.table.shape[1], []).append(t)
 
         # ---- activations and gradients
         B = self.B
@@ -1035,12 +1041,10 @@ class TwoTowerTrainer(_StepTrainer):
         bf = dict(dtype=torch.bfloat16, device=self.device)
         for t in self.towers:
             d = t["d"]
-            t["ld"] = (d + 3) // 4 * 4
+            t["ld"] = _ld4(d)
             t["x0"] = torch.zeros((B, t["ld"]), **f32)
             t["xs"] = torch.zeros((B, 2 * ops.tc_padded_k(d)), **bf)
-            t["h"] = [torch.zeros((B, l.units), **f32) for l in t["layers"]]
-            t["h_split"] = [torch.zeros((B, 2 * ops.tc_padded_k(l.units)), **bf) for l in t["layers"][:-1]]
-            t["dh"] = [torch.zeros((B, l.units), **f32) for l in t["layers"]]
+            t["h"], t["h_split"], t["dh"] = self._chain_buffers(t["layers"])
             t["dx0"] = torch.zeros((B, t["ld"]), **f32) if t["feats"] else None
             t["y"] = torch.zeros((B, self.D), **f32) if self.l2 else None  # the normalised output
             t["split"] = torch.zeros((B, 2 * ops.tc_padded_k(self.D)), **bf)
@@ -1054,24 +1058,8 @@ class TwoTowerTrainer(_StepTrainer):
         self.logits = self.stats  # [max, log-sum-exp, positive logit] of every row of the last step
         # one counter for both towers (every gather receives it), so check_indices sees every table
         self.oob = next((t["oob"] for t in self.towers if t["oob"] is not None), None)
-        self._bag_bufs: Dict[int, dict] = {}
-        self._bags: Dict[int, dict] = {}
 
     # ---- the parts of _StepTrainer that concern output heads do not apply: the retrieval task builds its own targets
-    def _init_heads(self) -> None:
-        raise NotImplementedError
-
-    def _check_targets(self, targets, b: int) -> list:
-        if b > self.B or b < 1:
-            raise ValueError(f"this trainer was compiled for batches of up to {self.B} samples, got {b}")
-        return []
-
-    def _after_step(self) -> None:
-        from .core import bump_weights_version
-
-        self.steps += 1
-        bump_weights_version()
-
     def capture(self, inputs: Dict[str, torch.Tensor], targets=None, clone: bool = True) -> None:
         """As _StepTrainer.capture; the targets are ignored (the task's targets are the one-hot column 0)."""
         super().capture(inputs, [], clone=clone)
@@ -1112,67 +1100,13 @@ class TwoTowerTrainer(_StepTrainer):
             c = self._inv_b[b] = torch.full((1,), 1.0 / b, dtype=torch.float32, device=self.device)
         return c
 
-    def _lookup(self, t: int, f: str, x, x0: torch.Tensor, col: int, b: int):
-        """Rows of feature f into x0[:, col:col+D]; returns the update's ids of a one-hot feature (None for a bag, whose
-        pooled-row gradient _bag_grads expands)."""
-        tb = self.tables[t]
-        kind = tb.lookup_kind(x)
-        if kind == "onehot":
-            return ops.as_index(x).reshape(-1)
-        comb = tb.sequence_combiner or "mean"
-        if comb == "max":
-            raise NotImplementedError(f"feature {f!r}: training with the 'max' sequence combiner is not implemented")
-        buf = self._bag_bufs.setdefault(t, dict(rows=None, ids=None))
-        D = tb.table.shape[1]
-        if kind == "bag":
-            values, offsets = x
-            ids, offs = ops.as_index(values).reshape(-1), ops.as_index(offsets)
-            ops.gather_bag(tb.table, ids, offs, comb, x0, col, self.oob)
-        else:
-            if comb == "sqrtn":
-                raise ValueError(f"feature {f!r}: sequence_combiner 'sqrtn' is only defined for ragged inputs")
-            ids, offs = ops.as_index(x).reshape(x.shape[0], -1).contiguous(), None
-            ops.gather_seq(tb.table, ids, comb, x0, col, self.oob)
-        nnz = ids.numel()
-        if buf["rows"] is None or buf["rows"].shape[0] < nnz:  # ragged: grows to the largest batch; fixed length: b * L
-            if torch.cuda.is_current_stream_capturing():
-                raise RuntimeError(f"feature {f!r}: the expanded gradient buffer cannot grow during graph capture")
-            buf["rows"] = torch.empty((nnz, D), dtype=torch.float32, device=self.device)
-        if kind == "bag" and (buf["ids"] is None or buf["ids"].shape[0] < nnz or buf["ids"].dtype != ids.dtype):
-            if torch.cuda.is_current_stream_capturing():
-                raise RuntimeError(f"feature {f!r}: the expanded id buffer cannot grow during graph capture")
-            buf["ids"] = torch.empty(max(nnz, 1), dtype=ids.dtype, device=self.device)
-        self._bags[t] = dict(ids=ids, offsets=offs, comb=comb, rows=buf["rows"][:nnz],
-                             apply_ids=buf["ids"][:nnz] if kind == "bag" else ids.reshape(-1))
-        return None
-
     def _tower_forward(self, tw: dict, inputs, b: int) -> torch.Tensor:
         d = tw["d"]
-        x0 = tw["x0"][:b, :d]
-        one_w, one_i, one_c = [], [], []
-        for t, f in zip(tw["tidx"], tw["feats"]):
-            ids = self._lookup(t, f, get_feature(inputs, f), x0, tw["cols"][f], b)
-            self._idx[t] = ids
-            if ids is not None:
-                one_w.append(self.tables[t].table)
-                one_i.append(ids)
-                one_c.append(tw["cols"][f])
-        if one_w:
-            if len({i.dtype for i in one_i}) > 1:
-                one_i = [i.to(torch.int64) for i in one_i]
-                for t, i in zip([t for t in tw["tidx"] if self._idx[t] is not None], one_i):
-                    self._idx[t] = i
-            ops.gather_multi(one_w, one_i, one_c, x0, self.oob)
-        if tw["cont"]:
-            ops.concat_columns([inputs[n] for n in tw["cont"]], x0, [tw["cols"][n] for n in tw["cont"]])
-        ops.split_rows(x0, out=tw["xs"][:b])
-        op, K = tw["xs"][:b], d
-        n = len(tw["layers"])
-        for i, l in enumerate(tw["layers"]):
-            nxt = tw["h_split"][i][:b] if i < n - 1 else None
-            ops.dense_tc(op, K, self._wsplit[tw["li0"] + i], l.units, l.bias, l.activation, out_f32=tw["h"][i][:b], out_split=nxt)
-            op, K = nxt, l.units
-        out = tw["h"][-1][:b]
+        xs = tw["xs"][:b]
+        self._input_forward(tw["feats"], tw["tidx"], tw["cols"], tw["cont"], inputs, tw["x0"][:b, :d], xs)
+        h = [x[:b] for x in tw["h"]]
+        self._chain_forward(xs, d, tw["li0"], tw["layers"], h, [x[:b] for x in tw["h_split"]])
+        out = h[-1]
         if self.l2:
             out = ops.l2_normalize(out, out=tw["y"][:b])
         ops.split_rows(out, out=tw["split"][:b])
@@ -1180,27 +1114,16 @@ class TwoTowerTrainer(_StepTrainer):
 
     def _tower_backward(self, tw: dict, dout: torch.Tensor, b: int) -> None:
         """dout: gradient of the tower's (normalised) output, overwritten by the pre-activation gradient of the last layer."""
-        a = self.arena
         h, dh, layers = [x[:b] for x in tw["h"]], [x[:b] for x in tw["dh"]], tw["layers"]
-        n = len(layers)
         if self.l2:
             ops.l2_normalize_backward(h[-1], dout, dout)
         if layers[-1].activation == "relu":
             ops.relu_mask(dout, h[-1])
         dh[-1] = dout
-        for i in range(n - 1, -1, -1):
-            li = tw["li0"] + i
-            if i > 0:
-                ops.dense_wgrad(h[i - 1], dh[i], a.view(a.grad, li, "kernel"), a.view(a.grad, li, "bias"))
-                self._dgrad(li, layers[i], dh[i], dh[i - 1], h[i - 1] if layers[i - 1].activation == "relu" else None)
-            else:
-                ops.dense_wgrad_split(tw["xs"][:b], tw["d"], dh[0], a.view(a.grad, li, "kernel"), a.view(a.grad, li, "bias"))
-                if tw["dx0"] is not None:
-                    dx0 = tw["dx0"][:b, :tw["d"]]
-                    self._dgrad(li, layers[0], dh[0], dx0, None)
-                    slices = [(self._slices[t], tw["cols"][f]) for t, f in zip(tw["tidx"], tw["feats"])]
-                    for s in range(0, len(slices), CONCAT_MAX_SLICES):
-                        ops.concat_backward([dx0], slices[s:s + CONCAT_MAX_SLICES])
+        dx0 = tw["dx0"][:b, :tw["d"]] if tw["dx0"] is not None else None  # a tower without tables has nothing below it
+        self._chain_backward(tw["li0"], layers, h, dh, (tw["xs"][:b], tw["d"]), dx0)
+        if dx0 is not None:
+            self._input_backward([dx0], tw["feats"], tw["tidx"], tw["cols"])
 
     def forward_backward(self, inputs: Dict[str, torch.Tensor], targets=None, sample_weight=None) -> None:
         """Forward (activations saved), in-batch soft-max cross-entropy and backward: fills the gradient arena and the
@@ -1208,7 +1131,7 @@ class TwoTowerTrainer(_StepTrainer):
         if sample_weight is not None and not (isinstance(sample_weight, (list, tuple)) and all(s is None for s in sample_weight)):
             raise NotImplementedError("sample_weight is not implemented in the two-tower training step")
         b = batch_size_of(inputs)
-        self._check_targets(targets, b)
+        self._check_batch(b)
         self._loss_all.zero_()
         self._idx: List[Optional[torch.Tensor]] = [None] * len(self.tables)
         self._bags = {}
@@ -1228,27 +1151,8 @@ class TwoTowerTrainer(_StepTrainer):
                                         temperature=T)
         for tw, dout in zip(self.towers, (dq, di)):
             self._tower_backward(tw, dout, b)
-        for t, bg in self._bags.items():
-            ops.bag_grad_rows(self._slices[t], bg["ids"], bg["offsets"], self.tables[t].table.shape[0], bg["comb"], bg["rows"],
-                              out_ids=bg["apply_ids"] if bg["offsets"] is not None else None)
+        self._bag_grads()
         self._b = b
-
-    def apply_gradients(self) -> None:
-        a = self.arena
-        ops.opt_tick(self.hyper)
-        ops.dense_apply(self.opt.kind, a.w, a.grad, a.state1, a.state2, self.hyper)
-        for D, ts in self._by_width.items():
-            onehot = [t for t in ts if t not in self._bags]
-            for s in range(0, len(onehot), SPARSE_MAX_TABLES):
-                chunk = onehot[s:s + SPARSE_MAX_TABLES]
-                ops.sparse_rows_apply(self.opt.kind, [self._table_args(t, self._idx[t], self._slices[t]) for t in chunk], self._b, D,
-                                      self.hyper)
-            for t in ts:
-                bag = self._bags.get(t)
-                if bag is not None and bag["rows"].shape[0] > 0:
-                    tab = self._table_args(t, bag["apply_ids"], bag["rows"])
-                    ops.sparse_rows_apply(self.opt.kind, [tab], bag["rows"].shape[0], D, self.hyper)
-        self._refresh_operands()
 
 
 class DeepFMTrainer(_StepTrainer):
@@ -1265,6 +1169,8 @@ class DeepFMTrainer(_StepTrainer):
               mm_wide_rows_apply (the wide kernel's rows: one (B,) gradient vector for every feature block; continuous rows
               and bias by the dense rule), mm_split_weights refresh of the operand copies the model's forward reads.
     The wide kernel (one row per category of every feature) stays where it is, its optimizer slots beside it."""
+
+    _multihot_refused = "DeepFMModel"
 
     def __init__(self, model, optimizer: Optimizer, batch_size: int, device=None, group=None):
         from .blocks import dense_engine
@@ -1302,35 +1208,19 @@ class DeepFMTrainer(_StepTrainer):
         # ---- input block layout, tables, wide kernel
         self.cols, widths, d = ib.layout()
         self.d = d
-        self.feats = list(fm.cat_names)
-        self.tables = [emb.feature_to_table[f] for f in self.feats]
-        seen = set()
-        for f, t in zip(self.feats, self.tables):
-            if id(t) in seen:
-                raise NotImplementedError(f"feature {f!r}: training with a table shared between features is not implemented")
-            seen.add(id(t))
-            if not t.trainable:
-                raise NotImplementedError(f"feature {f!r}: frozen embedding tables are not implemented in the training step")
-        self.D = fm.dim
-        if self.D % 4 or self.D > 128:
-            raise NotImplementedError(f"embedding width {self.D} is not supported by the sparse update (it needs a multiple of 4 no "
-                                      "larger than 128)")
-        if len(self.feats) > 32 or len(fm.cont_names) > 32:
+        if len(fm.cat_names) > 32 or len(fm.cont_names) > 32:
             raise NotImplementedError("the DeepFM head kernel takes up to 32 categorical and 32 continuous features")
+        self._init_tables(fm.cat_names, [emb.feature_to_table[f] for f in fm.cat_names])
+        self.D = fm.dim
         self.cont = list(fm.cont_names)
         self.wk = fm.wide  # _Dense(1) over [one-hot | continuous]: kernel (W, 1), bias (1,)
         self.woff = [fm.wide_offsets[f] for f in self.feats]
         self.coff = [fm.wide_offsets[n] for n in self.cont]
 
-        self.arena = DenseArena(self.chain + [self.last, self.head], optimizer, self.device)
-        self._tc_layers = self.chain + [self.last]  # the last one's operand copy is what the model's forward reads
-        self._wsplit = [ops.split_weights(l.kernel) for l in self._tc_layers]
-        for l, ws in zip(self._tc_layers, self._wsplit):
-            l._w_split = ws
-        self.hyper = torch.from_numpy(optimizer.hyper()).to(self.device)
+        # the step reads self.last as fp32 (the head kernel); its operand copy is what the model's forward reads
+        self._init_dense(self.chain + [self.last], [self.head])
         n = len(self.chain)
         self._init_wide(lambda li: li < n)
-        self._init_table_state(optimizer)
         f32 = dict(dtype=torch.float32, device=self.device)
         W = self.wk.kernel.numel()
         self.wk_s1 = torch.full((W,), optimizer.initial_accumulator_value, **f32) if optimizer.slots >= 1 else None
@@ -1344,30 +1234,15 @@ class DeepFMTrainer(_StepTrainer):
 
         # ---- activations and gradients
         B = self.B
-        self.ld = (d + 3) // 4 * 4
+        self.ld = _ld4(d)
         self.x0 = torch.zeros((B, self.ld), **f32)
         self.xs = torch.zeros((B, 2 * ops.tc_padded_k(d)), dtype=torch.bfloat16, device=self.device)
-        self.h = [torch.zeros((B, l.units), **f32) for l in self.chain]
-        self.h_split = [torch.zeros((B, 2 * ops.tc_padded_k(l.units)), dtype=torch.bfloat16, device=self.device) for l in self.chain[:-1]]
-        self.dh = [torch.zeros((B, l.units), **f32) for l in self.chain]
+        self.h, self.h_split, self.dh = self._chain_buffers(self.chain)
         self.dx0 = torch.zeros((B, self.ld), **f32)
         self.ds = torch.zeros(B, **f32)
         self.slices = [torch.zeros((B, self.D), **f32) for _ in self.tables]
         self._init_loss(B)
         self.oob = emb.counter(self.device)
-
-    def _ids(self, inputs):
-        """(gather ids: int32 / int64, one dtype; fused ids: packed widths as given) per table."""
-        gather, fused = [], []
-        for f, tb in zip(self.feats, self.tables):
-            x = get_feature(inputs, f)
-            if tb.lookup_kind(x) != "onehot":
-                raise NotImplementedError(f"feature {f!r}: training DeepFMModel on multi-hot / ragged features is not implemented")
-            gather.append(ops.as_index(x).reshape(-1))
-            fused.append(ops.fused_ids(x))
-        if len({i.dtype for i in gather}) > 1:
-            gather = [i.to(torch.int64) for i in gather]
-        return gather, fused
 
     def forward_backward(self, inputs: Dict[str, torch.Tensor], targets, sample_weight=None) -> None:
         """Forward (activations saved), loss and backward: fills the gradient arena, the IndexedSlices of the tables, ds (the
@@ -1380,65 +1255,42 @@ class DeepFMTrainer(_StepTrainer):
         targets = self._check_targets(targets, b)
         if isinstance(sample_weight, (list, tuple)):
             sample_weight = sample_weight[0]
-        gidx, fidx = self._ids(inputs)
-
-        def v(t):
-            return t[:b]
-
-        x0 = self.x0[:b, :d]
-        ops.gather_multi([tb.table for tb in self.tables], gidx, [self.cols[f] for f in self.feats], x0, self.oob)
+        tidx = range(len(self.tables))
+        self._idx: List[Optional[torch.Tensor]] = [None] * len(self.tables)
+        self._slices = [s[:b] for s in self.slices]
+        x0, xs = self.x0[:b, :d], self.xs[:b]
+        self._input_forward(self.feats, tidx, self.cols, self.cont, inputs, x0, xs)
+        # the head kernel and the updates read the ids at the width they came in (packed host-batch ids are not widened)
+        fidx = [ops.fused_ids(get_feature(inputs, f)) for f in self.feats]
         conts = [inputs[c] for c in self.cont]
-        if conts:
-            ops.concat_columns(conts, x0, [self.cols[c] for c in self.cont])
-        xs = v(self.xs)
-        ops.split_rows(x0, out=xs)
-        h, dh = [v(t) for t in self.h], [v(t) for t in self.dh]
-        op, K = xs, d
-        for i, l in enumerate(self.chain):
-            nxt = v(self.h_split[i]) if i < n - 1 else None
-            ops.dense_tc(op, K, self._wsplit[i], l.units, l.bias, l.activation, out_f32=h[i], out_split=nxt)
-            op, K = nxt, l.units
+        h, dh = [t[:b] for t in self.h], [t[:b] for t in self.dh]
+        self._chain_forward(xs, d, 0, self.chain, h, [t[:b] for t in self.h_split])
         # -- FM + wide + deep logit + output layer + loss, forward and backward
         hi = len(a.layers) - 1
-        ds = v(self.ds)
+        ds = self.ds[:b]
         nc = len(self.cont)
         ops.deepfm_head_fwd_bwd(
             x0, [self.cols[f] for f in self.feats], self.D, fidx, [tb.table.shape[0] for tb in self.tables], self.woff, conts,
             self.coff, self.wk.kernel.reshape(-1), self.wk.bias, h[-1], self.chain[-1].activation == "relu", self.last.kernel.reshape(-1),
             self.last.bias, self.last.activation, self.head.kernel.reshape(-1), self.head.bias, self.losses[0], targets[0].reshape(-1),
-            sample_weight, v(self.logits), self._loss_all, ds, dh[-1], dw_out=a.view(a.grad, hi, "kernel"), db_out=a.view(a.grad, hi, "bias"),
+            sample_weight, self.logits[:b], self._loss_all, ds, dh[-1], dw_out=a.view(a.grad, hi, "kernel"), db_out=a.view(a.grad, hi, "bias"),
             dw_dl=a.view(a.grad, n, "kernel"), db_dl=a.view(a.grad, n, "bias"),
             d_wide_bias=self.wk_grad[nc:] if self.wk.bias is not None else None, d_cont=self.wk_grad[:nc] if nc else None, oob=self.oob)
         # -- deep tower backward down to dx0
         dx0 = self.dx0[:b, :d]
-        for i in range(n - 1, -1, -1):
-            l = self.chain[i]
-            if i > 0:
-                ops.dense_wgrad(h[i - 1], dh[i], a.view(a.grad, i, "kernel"), a.view(a.grad, i, "bias"))
-                self._dgrad(i, l, dh[i], dh[i - 1], h[i - 1] if self.chain[i - 1].activation == "relu" else None)
-            else:
-                ops.dense_wgrad_split(xs, d, dh[0], a.view(a.grad, 0, "kernel"), a.view(a.grad, 0, "bias"))
-                self._dgrad(0, l, dh[0], dx0, None)
+        self._chain_backward(0, self.chain, h, dh, (xs, d), dx0)
         # -- input block backward: the deep tower's dx0 + the FM term, the tables' columns only
-        self._slices = [v(s) for s in self.slices]
-        slices = [(s, self.cols[f]) for s, f in zip(self._slices, self.feats)]
-        for s in range(0, len(slices), CONCAT_MAX_SLICES):
-            ops.fm_concat_backward([dx0], x0, ds, slices[s:s + CONCAT_MAX_SLICES])
-        self._idx, self._fidx, self._b = gidx, fidx, b
+        self._input_backward([dx0], self.feats, tidx, self.cols, fm=(x0, ds))
+        self._fidx, self._b = fidx, b
 
-    def apply_gradients(self) -> None:
-        a = self.arena
-        ops.opt_tick(self.hyper)
-        ops.dense_apply(self.opt.kind, a.w, a.grad, a.state1, a.state2, self.hyper)
-        T = len(self.tables)
-        for s in range(0, T, SPARSE_MAX_TABLES):
-            ops.sparse_rows_apply(self.opt.kind, [self._table_args(t, self._fidx[t], self._slices[t]) for t in range(s, min(T, s + SPARSE_MAX_TABLES))],
-                                  self._b, self.D, self.hyper)
+    def _gradients_to_apply(self) -> tuple:
+        return self._fidx, self._slices, self._b, 1.0
+
+    def _apply_more(self) -> None:
         ops.wide_rows_apply(self.opt.kind, self.wk.kernel.reshape(-1), self.wk_s1, self.wk_s2, self._fidx,
                             [tb.table.shape[0] for tb in self.tables], self.woff, self.ds[:self._b], self.wk_acc, self.wk_rep, self.coff,
                             self.wk_grad if self.wk_grad.numel() else None, None if self.wk.bias is None else self.wk.bias.reshape(-1),
                             self.wb_s1, self.wb_s2, self.hyper)
-        self._refresh_operands()
 
     def wide_gradients(self) -> Dict[str, torch.Tensor]:
         """The wide kernel's gradient (W,) and its bias' (after forward_backward, before apply_gradients), assembled in float64
