@@ -15,10 +15,12 @@
 // fp32 parity: all operands are split-bf16 pairs (x = hi + lo), every layer accumulates
 // hi*lo + lo*hi + hi*hi into one fp32 accumulator (same arithmetic as mm_dense_tc, passes = 3).
 //
-// CTA = 9 warps, persistent over 128-row tiles: warps 0-7 are two consumer warpgroups (64 rows of the
-// tile each: layer-1 MMAs, every epilogue and every chain MMA of those rows), warp 8 is the TMA producer
-// (layer-1 operands; the chain weights once).  The accumulator fragment of a layer maps register for
-// register onto the A fragment of the next layer's MMA (columns 16 s .. 16 s + 15 of D are k-step s of A).
+// CTA = 9 warps, persistent over 64-row tiles: warps 0-7 are two consumer warpgroups that ping-pong, warp 8 is
+// the TMA producer (layer-1 operands; the chain weights once).  Warpgroup w takes the tiles 2 i + w of the CTA's
+// sequence and runs every layer of them: the layer-1 MMAs, every epilogue and every chain MMA.  The layer-1
+// k-loops go to one warpgroup at a time, in tile order, so one tile's epilogue and chain layers run under the
+// other warpgroup's layer-1 MMAs.  The accumulator fragment of a layer maps register for register onto the A
+// fragment of the next layer's MMA (columns 16 s .. 16 s + 15 of D are k-step s of A).
 #include <cuda.h>
 #include <cuda_bf16.h>
 
@@ -32,14 +34,15 @@ namespace mlp {
 
 using namespace mm::tc;
 
-constexpr int BLOCK_M = 128;
+constexpr int BLOCK_M = 64;  // one tile = the M of one warpgroup's wgmma
 constexpr int BLOCK_K = 64;
 constexpr int MMA_K = 16;
 constexpr int kConsumerWarps = 8;
 constexpr int kThreads = 32 * (kConsumerWarps + 1);
 constexpr int kMaxChain = 3;
 constexpr int kMaxHeads = 8;
-constexpr uint32_t A_TILE_BYTES = BLOCK_M * BLOCK_K * 2;  // 16 KB
+constexpr int kTurnBar = 1;  // named barriers kTurnBar + w (256 threads): warpgroup w may start its layer-1 k-loop
+constexpr uint32_t A_TILE_BYTES = BLOCK_M * BLOCK_K * 2;  // 8 KB
 
 struct ChainLayer {
   int N, Np;        // true / padded (multiple of 16) width of this layer
@@ -123,14 +126,14 @@ mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
               const __grid_constant__ CUtensorMap tmC2, const Params p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // keeps the shared state space
-  // layer-1 ring: each slot holds ONE half of a k-block, {A_hi, W1_hi} or {A_lo, W1_lo} (32 KB at N1 = 128):
-  // finer slots keep more bytes in flight than whole {hi, lo} stages in the same shared memory
+  // layer-1 ring: each slot holds ONE half of a k-block of one tile, {A_hi, W1_hi} or {A_lo, W1_lo} (24 KB at
+  // N1 = 128): finer slots keep more bytes in flight than whole {hi, lo} stages in the same shared memory
   constexpr uint32_t B_TILE_BYTES = (uint32_t)N1P * BLOCK_K * 2;
   constexpr uint32_t STAGE_BYTES = A_TILE_BYTES + B_TILE_BYTES;
   uint8_t* wres = smem + (size_t)p.stages * STAGE_BYTES;  // resident chain weights (1024-B aligned tiles)
   uint64_t* bars = reinterpret_cast<uint64_t*>(wres + p.w_bytes);
   uint64_t* full_bar = bars;                        // [stages]
-  uint64_t* empty_bar = bars + p.stages;            // [stages] one arrive per consumer warp
+  uint64_t* empty_bar = bars + p.stages;            // [stages] one arrive per warp of the consuming warpgroup
   uint64_t* w_full = bars + 2 * p.stages;           // resident weights landed
   float* bias_s = reinterpret_cast<float*>(bars + 2 * p.stages + 2);  // [kMaxChain + 1][128], zero padded
   float* head_s = bias_s + (kMaxChain + 1) * 128;                     // [128] ([kMaxHeads][128] + [kMaxHeads] biases: HEADS), zero padded
@@ -144,7 +147,7 @@ mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmW1) : "memory");
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(smem_u32(full_bar + s), 1);
-      mbar_init(smem_u32(empty_bar + s), kConsumerWarps);
+      mbar_init(smem_u32(empty_bar + s), kConsumerWarps / 2);
     }
     mbar_init(smem_u32(w_full), 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -185,6 +188,7 @@ mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
           }
         }
       }
+      // tiles in the CTA's order, which is the order the two warpgroups' k-loops take turns in
       int stage = 0;
       uint32_t phase = 0;
       for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
@@ -205,18 +209,24 @@ mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
       }
     }
   } else {
-    // ===================== consumer warpgroups: 64 rows each, every layer =====================
+    // ===================== consumer warpgroups: every other tile each, every layer =====================
     const int wg = warp >> 2;
     const int c2 = 2 * (lane & 3);  // fragment column offset inside an 8-column block
-    const int frow = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // tile row of fragment row 0 (row 1 is 8 further)
-    const uint32_t a_off = (uint32_t)wg * (A_TILE_BYTES / 2);
-    int stage = 0;
-    uint32_t phase = 0;
+    const int frow = 16 * (warp & 3) + (lane >> 2);  // tile row of fragment row 0 (row 1 is 8 further)
     bool weights_ready = p.n_chain == 0;
-    for (long long tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    for (long long tile = blockIdx.x + (long long)wg * gridDim.x; tile < tiles; tile += 2ll * gridDim.x) {
+      // this tile's first ring slot: the producer fills 2 KB slots per tile, in the CTA's tile order
+      const long long pos = (tile - blockIdx.x) / gridDim.x * (2 * KB);
+      int stage = (int)(pos % p.stages);
+      uint32_t phase = (uint32_t)(pos / p.stages) & 1u;
       float acc[64];
 #pragma unroll
       for (int i = 0; i < 64; ++i) acc[i] = 0.0f;
+      // The layer-1 k-loops take turns in tile order: wait until the other warpgroup's k-loop of the previous tile
+      // is done.  Then every slot before this tile's has been filled, so the parity waits below cannot match a
+      // phase of a slot that is one lap behind.  Each tile with a successor arrives once and each tile with a
+      // predecessor waits once, so the two barriers balance for any tile count.
+      if (tile >= (long long)blockIdx.x + gridDim.x) named_bar(kTurnBar + wg, 256);
       for (int kb = 0; kb < KB; ++kb) {
         // hi slot: the dominant hi*hi product starts as soon as it lands
         const int s_hi = stage;
@@ -226,7 +236,7 @@ mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < BLOCK_K / MMA_K; ++k)
-          wgmma_ss(N1P, acc, make_desc_sw128(a_hi + a_off + k * 32), make_desc_sw128(b_hi + k * 32));
+          wgmma_ss(N1P, acc, make_desc_sw128(a_hi + k * 32), make_desc_sw128(b_hi + k * 32));
         wgmma_commit();
         if (++stage == p.stages) {
           stage = 0;
@@ -239,10 +249,10 @@ mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < BLOCK_K / MMA_K; ++k)
-          wgmma_ss(N1P, acc, make_desc_sw128(a_hi + a_off + k * 32), make_desc_sw128(b_lo + k * 32));
+          wgmma_ss(N1P, acc, make_desc_sw128(a_hi + k * 32), make_desc_sw128(b_lo + k * 32));
 #pragma unroll
         for (int k = 0; k < BLOCK_K / MMA_K; ++k)
-          wgmma_ss(N1P, acc, make_desc_sw128(a_lo + a_off + k * 32), make_desc_sw128(b_hi + k * 32));
+          wgmma_ss(N1P, acc, make_desc_sw128(a_lo + k * 32), make_desc_sw128(b_hi + k * 32));
         wgmma_commit();
         wgmma_wait_all();
         wgmma_fence_acc(acc);
@@ -256,6 +266,7 @@ mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
           phase ^= 1;
         }
       }
+      if (tile + gridDim.x < tiles) named_bar_arrive(kTurnBar + (wg ^ 1), 256);  // the next tile's k-loop may start
 
       for (int layer = 0; layer <= p.n_chain; ++layer) {
         const bool last = layer == p.n_chain;
@@ -263,16 +274,29 @@ mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
         const int Np = layer == 0 ? N1P : p.c[layer - 1].Np;
         const int act = layer == 0 ? p.act1 : p.c[layer - 1].act;
         const float* bs = bias_s + layer * 128;
-        // bias + activation on the fragment; padding columns (>= N) become exact zeros
+        // bias + activation on the fragment; padding columns (>= N) become exact zeros.  Every column block is
+        // processed: the ones past Np hold zeros (no MMA wrote them) and zero biases, so they stay zero.  The relu
+        // path is straight-line code: a test of `act` per element made each element its own basic block, and the
+        // epilogue then ran one dependent chain at a time.
+        if (act == MM_ACT_RELU) {
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          if (8 * j < Np) {
+          for (int j = 0; j < 16; ++j) {
+            const float2 b = *reinterpret_cast<const float2*>(bs + 8 * j + c2);
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+              const int col = 8 * j + c2 + (e & 1);
+              const float v = fmaxf(acc[4 * j + e] + ((e & 1) ? b.y : b.x), 0.0f);
+              acc[4 * j + e] = col < N ? v : 0.0f;
+            }
+          }
+        } else {
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
               const int col = 8 * j + c2 + (e & 1);
               float v = acc[4 * j + e] + bs[col];
-              if (act == MM_ACT_RELU) v = fmaxf(v, 0.0f);
-              else if (act != MM_ACT_LINEAR && col < N) v = apply_act_slow(v, act);
+              if (act != MM_ACT_LINEAR && col < N) v = apply_act_slow(v, act);
               acc[4 * j + e] = col < N ? v : 0.0f;
             }
           }

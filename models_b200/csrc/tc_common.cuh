@@ -55,6 +55,10 @@ __device__ __forceinline__ void wgmma_fence_acc(float (&d)[64]) {
 __device__ __forceinline__ void named_bar(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
+// counts this warp's threads towards named barrier `id` without waiting for it
+__device__ __forceinline__ void named_bar_arrive(int id, int threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
 
 __device__ __forceinline__ void wgmma_ss_n16(float (&d)[64], uint64_t a, uint64_t b) {
   asm volatile(
