@@ -459,10 +459,12 @@ def _variables(tr):
     return out
 
 
-def _reference_step(tr, inputs, y, B, chunk=8192):
+def _reference_step(tr, inputs, y, B, chunk=8192, rows_of=None):
     """float64 autograd on the device of the trainer's forward (bottom MLP, lookup, pairwise dots, top MLP, head, mean BCE)
     over the looked-up rows, in sample chunks.  Returns the loss, the dense gradients by variable name, the slices per
-    table, and per sample whether a relu unit is on in one implementation and off in the other."""
+    table, and per sample whether a relu unit is on in one implementation and off in the other.  rows_of(t, s, e): the
+    float64 rows of table t for samples [s, e) (default: the table's rows at the trainer's ids; a multi-hot feature passes
+    its pooled rows)."""
     layers = tr.bottom + tr.top + [tr.head]
     P = [(l.kernel.double().requires_grad_(True), None if l.bias is None else l.bias.double().requires_grad_(True)) for l in layers]
     cont = tr.body.continuous(inputs)
@@ -498,7 +500,8 @@ def _reference_step(tr, inputs, y, B, chunk=8192):
         h = x0[s:e]
         for li in range(nb):
             h = dense(h, li, flip, s, e)
-        rows = [tr.tables[t].table[ids[t][s:e]].double().requires_grad_(True) for t in range(len(ids))]
+        rows = [(tr.tables[t].table[ids[t][s:e]].double() if rows_of is None else rows_of(t, s, e)).requires_grad_(True)
+                for t in range(len(ids))]
         seq = [None] * F
         for t, sl in enumerate(order):
             seq[sl] = rows[t]
