@@ -308,24 +308,6 @@ int mm_tower2_small(const mm_concat_piece* pieces_host, int n_pieces, int64_t B,
                     const float* bias1, int act1, const void* w2_split, int N2, const float* bias2, int act2, float* out,
                     int64_t out_stride, void* out_split, void* stream);
 
-/* Whole-op entry points over fp32 Keras-layout weights (kernel (in, out) row-major, bias (out,) or
- * NULL) and a caller-provided workspace — for callers outside this package's Python host; nothing is
- * allocated, no pre-split weights are needed (the bf16 splits live in the workspace).
- *   mm_mlp_forward: MLPBlock, h_l = act_l(h_{l-1} W_l + b_l), 1..8 layers (blocks/mlp.py:97-139,
- *     :275-280); the whole-tower kernel when mm_mlp_tc_supported, else one wgmma launch per layer.
- *   mm_cross_forward: CrossBlock, x_{l+1} = x0 * (x_l W_l + b_l) + x_l, W_l (d, d)
- *     (blocks/cross.py:29-109, :188-202); depth > 1 needs x_stride == d.
- * workspace: 256-B aligned device memory of at least mm_*_workspace_bytes(...) (-1 on bad arguments). */
-int64_t mm_mlp_workspace_bytes(int64_t M, int K, int n_layers, const int* widths);
-int mm_mlp_forward(const float* x, int64_t M, int K, int64_t x_stride, int n_layers,
-                   const float* const* kernels, const float* const* biases, const int* widths,
-                   const int* acts, float* out, int64_t out_stride, void* workspace,
-                   int64_t workspace_bytes, void* stream);
-int64_t mm_cross_workspace_bytes(int64_t M, int d, int depth);
-int mm_cross_forward(const float* x0, int64_t M, int d, int64_t x_stride, int depth,
-                     const float* const* kernels, const float* const* biases, float* out,
-                     int64_t out_stride, void* workspace, int64_t workspace_bytes, void* stream);
-
 /* ---------------------------------------------------------------------------------------
  * K8/K9  Two-tower scoring.
  * mm_rowwise_dot: inference scorer  s[b] = sum_d q[b,d]*i[b,d]
@@ -416,12 +398,8 @@ int mm_init_uniform_hash_rows(float* w, int64_t local_rows, int D, uint64_t seed
  * i.e. what `Model.train_step` (merlin/models/tf/models/base.py:1121-1231) obtains from tf.GradientTape +
  * `optimizer.apply_gradients` for DLRMBlock (blocks/dlrm.py:32-133) + BinaryOutput (outputs/classification.py:114):
  *
- *   mm_bce_head_fwd_bwd       Dense(K -> 1) + sigmoid + binary cross-entropy (Keras evaluates it on the logits),
- *                             forward AND backward in one pass over x (M, K), K <= 256:
- *                               z = x.w + b;  *loss_sum += sum_i sw_i (max(z,0) - z y + log(1 + e^-|z|)) / M;
- *                               dz = sw_i (sigmoid(z) - y) / M;  dx = dz w (zeroed where x <= 0 when mask_relu);
- *                               dw += x^T dz;  *db += sum dz.      loss_sum / dw / db are ACCUMULATED (zero them first).
- *   mm_heads_fwd_bwd          the same for H <= 8 BinaryOutput / RegressionOutput heads with loss weights (see below).
+ *   mm_heads_fwd_bwd          H <= 8 BinaryOutput / RegressionOutput heads Dense(K -> 1) with loss weights, forward AND
+ *                             backward in one pass over x (M, K), K <= 256 (see below).
  *   mm_dense_wgrad            dW (K, N) += X^T dZ,  db (N) += column sums of dZ   (db nullable; accumulated)
  *   mm_dense_dgrad            dX (M, K) = dZ (M, N) W^T, W the Keras kernel (K, N), N <= 128; `mask` (M, K) nullable:
  *                             dX is zeroed where mask <= 0 (mask = the layer's input = the previous layer's relu
@@ -490,9 +468,6 @@ typedef struct {
                       * flags the touched rows, and the update walks the rows.  Null: the election path (rows >> batch: duplicates are rare). */
 } mm_sparse_table;
 
-int mm_bce_head_fwd_bwd(const float* x, int64_t M, int K, int64_t x_stride, const float* w, const float* bias,
-                        const void* targets, int target_dtype, const float* sample_weight, float* logits,
-                        float* loss_sum, float* dx, int64_t dx_stride, int mask_relu, float* dw, float* db, void* stream);
 /* Loss kinds of mm_heads_fwd_bwd: BinaryOutput (sigmoid + binary cross-entropy on the logits) and RegressionOutput
  * (linear + squared error). */
 #define MM_LOSS_BCE 0
@@ -509,8 +484,7 @@ int mm_bce_head_fwd_bwd(const float* x, int64_t M, int K, int64_t x_stride, cons
  * loss_kind, loss_weight, targets, target_dtypes, sample_weights are HOST arrays of H entries; targets[h] is (M,) of
  * target_dtypes[h] (MM_I32 .. MM_F64); sample_weights (nullable array, entries nullable) holds (M,) fp32 per head — the
  * same pointer for every head when the weights are shared.  targets == NULL: forward only — logits (H, M) receives the
- * activated predictions (sigmoid(z) / z) and nothing else is read or written.  mm_bce_head_fwd_bwd is H = 1 with one
- * BCE head and loss_weight 1 (its loss_sum is the total alone). */
+ * activated predictions (sigmoid(z) / z) and nothing else is read or written. */
 int mm_heads_fwd_bwd(const float* x, int64_t M, int K, int64_t x_stride, int H, const float* w, const float* bias,
                      const int* loss_kind, const float* loss_weight, const void* const* targets, const int* target_dtypes,
                      const float* const* sample_weights, float* logits, float* loss, float* dx, int64_t dx_stride,

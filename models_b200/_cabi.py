@@ -155,11 +155,6 @@ SIGNATURES = {
     "mm_dense_tc": (_i, [_vp, _i64, _i, _i, _vp, _i, _i, _vp, _i, _i, _vp, _vp, _i64, _vp, _i64,
                          _vp, _i, _vp]),
     "mm_dense_tc_head": (_i, [_vp, _i64, _i, _i, _vp, _i, _i, _vp, _i, _i, _vp, _f, _i, _vp, _vp]),
-    "mm_mlp_workspace_bytes": (_i64, [_i64, _i, _i, C.POINTER(C.c_int)]),
-    "mm_mlp_forward": (_i, [_vp, _i64, _i, _i64, _i, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_int),
-                            C.POINTER(C.c_int), _vp, _i64, _vp, _i64, _vp]),
-    "mm_cross_workspace_bytes": (_i64, [_i64, _i, _i]),
-    "mm_cross_forward": (_i, [_vp, _i64, _i, _i64, _i, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), _vp, _i64, _vp, _i64, _vp]),
     "mm_mlp_tc_supported": (_i, [_i, _i, C.POINTER(C.c_int), _i]),
     "mm_mlp_tc": (_i, [_vp, _i64, _i, _i, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_void_p), C.POINTER(C.c_int),
                        _vp, _i64, _vp, _f, _i, _vp, _vp]),
@@ -182,7 +177,6 @@ SIGNATURES = {
     "mm_fm_pairwise": (_i, [_vp, _i64, _i, _i, _vp, _vp]),
     "mm_deepfm_head": (_i, [C.POINTER(LookupTable), C.POINTER(C.c_int64), _i, _i64, _i, C.POINTER(ConcatPiece), C.POINTER(C.c_int64), _i,
                             _vp, _vp, _vp, _i64, _vp, _vp, _i, _vp, _vp, _vp]),
-    "mm_bce_head_fwd_bwd": (_i, [_vp, _i64, _i, _i64, _vp, _vp, _vp, _i, _vp, _vp, _vp, _vp, _i64, _i, _vp, _vp, _vp]),
     "mm_heads_fwd_bwd": (_i, [_vp, _i64, _i, _i64, _i, _vp, _vp, C.POINTER(C.c_int), C.POINTER(C.c_float), C.POINTER(C.c_void_p),
                               C.POINTER(C.c_int), C.POINTER(C.c_void_p), _vp, _vp, _vp, _i64, _i, _vp, _vp, _vp]),
     "mm_dense_wgrad": (_i, [_vp, _i64, _i, _i64, _vp, _i, _i64, _vp, _vp, _vp]),

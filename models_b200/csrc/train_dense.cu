@@ -4,8 +4,8 @@
 // batch: the whole backward is 19 GFLOP against ~1 GB of activations per 65 536 samples, so every kernel
 // here is organised around streaming the activations once.
 //
-//   mm_bce_head_fwd_bwd  z = x.w + b, loss += sum BCE(z, y), dz = (sigmoid(z) - y) * w_i / M,
-//                        dx = dz * w [x > 0], dw += x^T dz, db += sum dz        (one warp per row, no GEMM)
+//   mm_heads_fwd_bwd     z_h = x.W[:, h] + b_h, loss += sum BCE / MSE(z_h, y_h), dz_h = lambda_h sw_i l'_h / M,
+//                        dx = sum_h dz_h W[:, h]^T [x > 0], dW += x^T dz, db += sum dz   (one warp per row, no GEMM)
 //   mm_dense_wgrad       dW += X^T dZ, db += column sums of dZ                  (reduction over the batch)
 //   mm_dense_dgrad       dX = (dZ W^T) [mask > 0]                                (mask: the layer input = the
 //                        previous layer's relu output, so the result is that layer's pre-activation gradient)
@@ -29,8 +29,8 @@ namespace trn {
 //     l_i = max(z,0) - z*y + log(1 + exp(-|z|)),   dl/dz = sigmoid(z) - y
 //   MSE (RegressionOutput, linear):  l_i = (z - y)^2,   dl/dz = 2 (z - y)
 // loss_h = sum_i sw_i l_h,i / M (Keras "sum_over_batch_size"), total = sum_h lambda_h loss_h, dz_h = lambda_h sw_i l'_h / M.
-// H and TRAIN are template parameters; the loss kind of a head is a uniform runtime branch.  H = 1 with one BCE head and
-// lambda = 1 is mm_bce_head_fwd_bwd: the same products and sums in the same order (the products by lambda = 1 are exact).
+// H and TRAIN are template parameters; the loss kind of a head is a uniform runtime branch.  H = 1 (a model with one
+// output head) is its own instantiation, so the single-head step pays for no loop over unused heads.
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int HEAD_MAX = 8;
 
@@ -310,7 +310,7 @@ static void launch_heads(const HeadParams& p, bool vec, unsigned blocks, cudaStr
   }
 }
 
-// the instantiation for p's head count; H = 1 is mm_bce_head_fwd_bwd's kernel
+// the instantiation for p's head count
 template <bool TRAIN>
 static void launch_heads(const HeadParams& p, int H, bool vec, unsigned blocks, cudaStream_t st) {
   switch (H) {
@@ -957,40 +957,6 @@ int mm_concat_backward(const float* const* addends_host, const int64_t* addend_s
   if (blocks > cap) blocks = cap;
   concat_backward_kernel<<<dim3((unsigned)blocks, (unsigned)n_slices), 256, 0, (cudaStream_t)stream>>>(q);
   return mm::check_launch("mm_concat_backward");
-}
-
-int mm_bce_head_fwd_bwd(const float* x, int64_t M, int K, int64_t x_stride, const float* w, const float* bias, const void* targets,
-                        int target_dtype, const float* sample_weight, float* logits, float* loss_sum, float* dx,
-                        int64_t dx_stride, int mask_relu, float* dw, float* db, void* stream) {
-  using namespace mm::trn;
-  MM_REQUIRE(x && w && targets && M >= 0 && K >= 1 && x_stride >= K, MM_ERR_ARG, "mm_bce_head_fwd_bwd: null pointer or bad K / stride");
-  MM_REQUIRE(K <= HEAD_KMAX, MM_ERR_UNSUPPORTED, "mm_bce_head_fwd_bwd: K=%d > %d", K, HEAD_KMAX);
-  MM_REQUIRE(target_dtype >= MM_I32 && target_dtype <= MM_F64, MM_ERR_ARG, "mm_bce_head_fwd_bwd: bad target dtype");
-  MM_REQUIRE(!dx || dx_stride >= K, MM_ERR_ARG, "mm_bce_head_fwd_bwd: dx_stride < K");
-  if (M == 0) return MM_OK;
-  HeadParams p;
-  memset(&p, 0, sizeof(p));
-  p.x = x;
-  p.ldx = x_stride;
-  p.M = M;
-  p.K = K;
-  p.w = w;
-  p.bias = bias;
-  p.y[0] = targets;
-  p.y_dtype[0] = target_dtype;
-  p.kind[0] = MM_LOSS_BCE;
-  p.lw[0] = 1.0f;
-  p.sample_w[0] = sample_weight;
-  p.inv_m = 1.0f / (float)M;
-  p.logits = logits;
-  p.loss = loss_sum;
-  p.dx = dx;
-  p.lddx = dx_stride;
-  p.mask_relu = mask_relu;
-  p.dw = dw;
-  p.db = db;
-  run_heads(p, 1, true, (cudaStream_t)stream);
-  return mm::check_launch("mm_bce_head_fwd_bwd");
 }
 
 int mm_heads_fwd_bwd(const float* x, int64_t M, int K, int64_t x_stride, int H, const float* w, const float* bias,

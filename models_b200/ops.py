@@ -39,6 +39,12 @@ def _ptr(t: Optional[torch.Tensor]) -> Optional[int]:
     return None if t is None else t.data_ptr()
 
 
+def _vec(t: Optional[torch.Tensor], n: int, name: str, what: str = "hold {n} contiguous values") -> None:
+    """Checks that t is None or an fp32 vector of n contiguous values; the error says f"{name} must {what}"."""
+    if t is not None and (_dev(t, name, torch.float32).numel() != n or not t.is_contiguous()):
+        raise ValueError(f"{name} must " + what.format(n=n))
+
+
 def _idx_dtype(t: torch.Tensor, name: str) -> int:
     if t.dtype == torch.int32:
         return MM_I32
@@ -231,19 +237,26 @@ def fused_ids(t: torch.Tensor) -> torch.Tensor:
     return t if t.dtype in (torch.uint8, torch.uint16) else as_index(t).reshape(-1)
 
 
+def _id_column(ix: torch.Tensor, B: int, name: str, leading: bool = False) -> int:
+    """index_bytes_of a column of B contiguous ids (a uint8 (B, 3) column holds B ids).  leading: its first dimension must
+    also be B."""
+    _dev(ix, name)
+    wb = index_bytes_of(ix)
+    if ix.numel() != B * (3 if wb == 3 else 1) or not ix.is_contiguous() or (leading and ix.shape[0] != B):
+        raise ValueError(f"{name} must be {B} contiguous ids, got {tuple(ix.shape)}")
+    return wb
+
+
 def _lookup_tables(weights, indices, B: int, wdt: torch.dtype, wcols: int, slots=None, rows=None):
     """mm_lookup_table array: table t is weights[t], a contiguous (rows, wcols) wdt matrix, read at the B ids indices[t]
     (any width of index_bytes_of), staged at slots[t] (default t), with rows[t] rows (default weights[t].shape[0])."""
     arr = (_cabi.LookupTable * len(weights))()
     for t in range(len(weights)):
         w = _dev(weights[t], f"weights[{t}]", wdt)
-        ix = _dev(indices[t], f"indices[{t}]")
         if w.dim() != 2 or w.shape[1] != wcols or not w.is_contiguous():
             raise ValueError(f"weights[{t}] must be a contiguous (rows, {wcols}) {wdt} matrix")
-        wb = index_bytes_of(ix)
-        if ix.numel() != B * (3 if wb == 3 else 1) or not ix.is_contiguous():
-            raise ValueError(f"indices[{t}] must be contiguous with {B} ids, got {tuple(ix.shape)}")
-        arr[t].weights, arr[t].indices, arr[t].idx_bytes = w.data_ptr(), ix.data_ptr(), wb
+        arr[t].idx_bytes = _id_column(indices[t], B, f"indices[{t}]")
+        arr[t].weights, arr[t].indices = w.data_ptr(), indices[t].data_ptr()
         arr[t].rows = w.shape[0] if rows is None else int(rows[t])
         arr[t].slot = t if slots is None else int(slots[t])
     return arr
@@ -316,9 +329,10 @@ def rowwise_dot(q: torch.Tensor, items: torch.Tensor, out: torch.Tensor) -> torc
 
 def _item_ids(pos_ids, neg_ids, downscore: bool):
     """(pos_ids, neg_ids, id dtype code) for the false-negative mask of the in-batch kernels: with downscore, both as
-    contiguous (B,) / (N,) vectors of the negative ids' dtype (utils/tf_utils.py:136 casts the positive ids to it)."""
+    contiguous (B,) / (N,) vectors of the negative ids' dtype (utils/tf_utils.py:136 casts the positive ids to it);
+    without, None (the kernels read no ids)."""
     if not downscore:
-        return pos_ids, neg_ids, MM_I64
+        return None, None, MM_I64
     if pos_ids is None or neg_ids is None:
         raise ValueError("downscore_false_negatives requires positive and negative item ids")
     neg_ids = neg_ids.reshape(-1).contiguous()
@@ -374,23 +388,14 @@ def inbatch_softmax_ce(q, pos, neg, pos_ids=None, neg_ids=None, downscore=True, 
     N = neg.shape[0]
     if N == 0 or B == 0:
         raise ValueError("in-batch softmax needs at least one query and one negative")
-    pos_ids, neg_ids, id_dt = _item_ids(pos_ids, neg_ids, downscore)
-    dev = q.device
-    pos_logit = torch.empty((B, 1), dtype=torch.float32, device=dev)
-    _cabi.check(_lib().mm_positive_scores(q.data_ptr(), pos.data_ptr(), B, D, _ptr(pos_prob), float(temperature),
-                                          pos_logit.data_ptr(), 1, _stream()), "mm_positive_scores")
+    pos_logit = torch.empty((B, 1), dtype=torch.float32, device=q.device)
+    stats = torch.empty((B, 3), dtype=torch.float32, device=q.device)
+    ws = _catalog_workspace(B, N, 0, q.device)
+    positive_scores(q, pos, pos_logit, pos_prob, temperature)
     qs = split_rows(q)
     ns = qs if neg.data_ptr() == q.data_ptr() else split_rows(neg)
-    stats = torch.empty((B, 3), dtype=torch.float32, device=dev)
-    nbytes = int(_lib().mm_catalog_workspace_bytes(B, N, 0))
-    ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=dev)
-    _cabi.check(
-        _lib().mm_inbatch_softmax_ce(qs.data_ptr(), ns.data_ptr(), B, N, D, _ptr(pos_ids) if downscore else None,
-                                     _ptr(neg_ids) if downscore else None, id_dt, int(bool(downscore)), float(false_neg_score),
-                                     pos_logit.data_ptr(), _ptr(neg_prob), float(temperature), stats.data_ptr(), ws.data_ptr(),
-                                     nbytes, _stream()),
-        "mm_inbatch_softmax_ce")
-    return stats
+    return inbatch_softmax_ce_split(qs, ns, D, pos_logit, stats, ws, pos_ids, neg_ids, downscore, false_neg_score, neg_prob,
+                                    temperature)
 
 
 def positive_scores(q: torch.Tensor, pos: torch.Tensor, out: torch.Tensor, pos_prob=None, temperature: float = 1.0) -> torch.Tensor:
@@ -416,16 +421,20 @@ def inbatch_softmax_ce_split(q_split, neg_split, D: int, pos_logit, stats, works
         raise ValueError(f"stats must be contiguous ({B}, 3) and pos_logit hold {B} values")
     pos_ids, neg_ids, id_dt = _item_ids(pos_ids, neg_ids, downscore)
     _cabi.check(
-        _lib().mm_inbatch_softmax_ce(q_split.data_ptr(), neg_split.data_ptr(), B, N, int(D), _ptr(pos_ids) if downscore else None,
-                                     _ptr(neg_ids) if downscore else None, id_dt, int(bool(downscore)), float(false_neg_score),
-                                     pos_logit.data_ptr(), _ptr(neg_prob), float(temperature), stats.data_ptr(), workspace.data_ptr(),
-                                     workspace.numel(), _stream()),
+        _lib().mm_inbatch_softmax_ce(q_split.data_ptr(), neg_split.data_ptr(), B, N, int(D), _ptr(pos_ids), _ptr(neg_ids), id_dt,
+                                     int(bool(downscore)), float(false_neg_score), pos_logit.data_ptr(), _ptr(neg_prob),
+                                     float(temperature), stats.data_ptr(), workspace.data_ptr(), workspace.numel(), _stream()),
         "mm_inbatch_softmax_ce")
     return stats
 
 
 def catalog_workspace_bytes(B: int, N: int, k: int = 0) -> int:
     return int(_lib().mm_catalog_workspace_bytes(int(B), int(N), int(k)))
+
+
+def _catalog_workspace(B: int, N: int, k: int, device) -> torch.Tensor:
+    """uint8 workspace of the catalog-scoring kernel for B queries, N items and top-k (at least 16 bytes)."""
+    return torch.empty(max(catalog_workspace_bytes(B, N, k), 16), dtype=torch.uint8, device=device)
 
 
 def inbatch_softmax_ce_backward(q_split, neg_split, D: int, stats, q, pos, row_scale, dq, dpos, dneg, loss=None, pos_ids=None,
@@ -450,8 +459,7 @@ def inbatch_softmax_ce_backward(q_split, neg_split, D: int, stats, q, pos, row_s
             raise ValueError(f"{n_} must be {shape}, got {tuple(t_.shape)}")
     if not (q_split.is_contiguous() and neg_split.is_contiguous()):
         raise ValueError("q_split and neg_split must be contiguous")
-    if neg_prob is not None and (_dev(neg_prob, "neg_prob", torch.float32).numel() != N or not neg_prob.is_contiguous()):
-        raise ValueError(f"neg_prob must hold {N} contiguous values")
+    _vec(neg_prob, N, "neg_prob")
     if loss is not None and loss.numel() < 1:
         raise ValueError("loss must hold at least one value")
     if row_scale.numel() not in (1, B):
@@ -459,9 +467,8 @@ def inbatch_softmax_ce_backward(q_split, neg_split, D: int, stats, q, pos, row_s
     scalar = row_scale.numel() == 1 and B != 1
     pos_ids, neg_ids, id_dt = _item_ids(pos_ids, neg_ids, downscore)
     _cabi.check(
-        _lib().mm_inbatch_softmax_ce_backward(q_split.data_ptr(), neg_split.data_ptr(), B, N, int(D),
-                                              _ptr(pos_ids) if downscore else None, _ptr(neg_ids) if downscore else None, id_dt,
-                                              int(bool(downscore)), float(false_neg_score), _ptr(neg_prob), float(temperature),
+        _lib().mm_inbatch_softmax_ce_backward(q_split.data_ptr(), neg_split.data_ptr(), B, N, int(D), _ptr(pos_ids), _ptr(neg_ids),
+                                              id_dt, int(bool(downscore)), float(false_neg_score), _ptr(neg_prob), float(temperature),
                                               stats.data_ptr(), q.data_ptr(), pos.data_ptr(), row_scale.data_ptr(), int(scalar),
                                               dq.data_ptr(), dpos.data_ptr(), dneg.data_ptr(), _ptr(loss), _stream()),
         "mm_inbatch_softmax_ce_backward")
@@ -494,6 +501,18 @@ def _concat_pieces(pieces: Sequence[torch.Tensor], B: int, name: str = "pieces",
     for i, (ptr, sstride, w, dt, oc) in enumerate(flat):
         arr[i].src, arr[i].src_stride, arr[i].width, arr[i].dtype, arr[i].out_col = ptr, sstride, w, dt, oc
     return arr, len(flat), col
+
+
+def _cont_columns(cont, cont_offsets, B: int):
+    """(mm_concat_piece array, offsets array, count) of the continuous columns cont, B values each, at cont_offsets."""
+    m = len(cont)
+    if len(cont_offsets) != m:
+        raise ValueError("cont / cont_offsets length mismatch")
+    for c, t in enumerate(cont):
+        if _dev(t, f"cont[{c}]").numel() != B:
+            raise ValueError(f"cont[{c}] must hold {B} values")
+    carr, _, _ = _concat_pieces([t.reshape(-1) for t in cont], B, "cont")
+    return carr, (C.c_int64 * max(m, 1))(*[int(o) for o in cont_offsets]), m
 
 
 def concat_columns(pieces: Sequence[torch.Tensor], out: torch.Tensor, out_cols: Optional[Sequence[int]] = None,
@@ -683,67 +702,12 @@ def catalog_score(q: torch.Tensor, e_split: torch.Tensor, n_items: int, bias: Op
     if targets is not None:
         targets = targets.reshape(-1).contiguous()
         id_dt = _idx_dtype(targets, "targets")
-    nbytes = int(_lib().mm_catalog_workspace_bytes(B, n_items, k))
-    ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=dev)
+    ws = _catalog_workspace(B, n_items, k, dev)
     _cabi.check(
         _lib().mm_catalog_score(split_rows(q).data_ptr(), B, D, e_split.data_ptr(), n_items, _ptr(bias), _ptr(targets), id_dt,
-                                _ptr(stats), k, _ptr(scores), _ptr(ids), ws.data_ptr(), nbytes, _stream()),
+                                _ptr(stats), k, _ptr(scores), _ptr(ids), ws.data_ptr(), ws.numel(), _stream()),
         "mm_catalog_score")
     return stats, scores, ids
-
-
-def mlp_forward(x: torch.Tensor, kernels: Sequence[torch.Tensor], biases: Sequence[Optional[torch.Tensor]],
-                acts: Sequence[Optional[str]], out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """MLPBlock in ONE C call over fp32 Keras-layout kernels (mm_mlp_forward): the bf16 splits of the input,
-    the weights and the intermediate activations live in a workspace allocated here."""
-    _dev(x, "x", torch.float32)
-    M, K = x.shape
-    n = len(kernels)
-    widths = [int(k.shape[1]) for k in kernels]
-    kk = K
-    for l, kern in enumerate(kernels):
-        _dev(kern, f"kernels[{l}]", torch.float32)
-        if kern.dim() != 2 or kern.shape[0] != kk or not kern.is_contiguous():
-            raise ValueError(f"kernels[{l}] must be a contiguous ({kk}, units) matrix, got {tuple(kern.shape)}")
-        if biases[l] is not None:
-            _dev(biases[l], f"biases[{l}]", torch.float32)
-        kk = widths[l]
-    if out is None:
-        out = torch.empty((M, widths[-1]), dtype=torch.float32, device=x.device)
-    wd = (C.c_int * n)(*widths)
-    need = int(_lib().mm_mlp_workspace_bytes(M, K, n, wd))
-    if need < 0:
-        raise ValueError("mm_mlp_workspace_bytes rejected the tower (1..8 layers, positive widths)")
-    ws = torch.empty(max(need, 256), dtype=torch.uint8, device=x.device)
-    kp = (C.c_void_p * n)(*[k.data_ptr() for k in kernels])
-    bp = (C.c_void_p * n)(*[_ptr(b) for b in biases])
-    ac = (C.c_int * n)(*[ACTIVATIONS[a] for a in acts])
-    _cabi.check(_lib().mm_mlp_forward(x.data_ptr(), M, K, _row_stride(x, "x"), n, kp, bp, wd, ac, out.data_ptr(),
-                                      _row_stride(out, "out"), ws.data_ptr(), need, _stream()), "mm_mlp_forward")
-    return out
-
-
-def cross_forward(x0: torch.Tensor, kernels: Sequence[torch.Tensor], biases: Sequence[Optional[torch.Tensor]],
-                  out: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """CrossBlock stack in ONE C call (mm_cross_forward): x_{l+1} = x0 * (x_l W_l + b_l) + x_l."""
-    _dev(x0, "x0", torch.float32)
-    M, d = x0.shape
-    depth = len(kernels)
-    for l, kern in enumerate(kernels):
-        _dev(kern, f"kernels[{l}]", torch.float32)
-        if tuple(kern.shape) != (d, d) or not kern.is_contiguous():
-            raise ValueError(f"kernels[{l}] must be a contiguous ({d}, {d}) matrix")
-    if out is None:
-        out = torch.empty((M, d), dtype=torch.float32, device=x0.device)
-    need = int(_lib().mm_cross_workspace_bytes(M, d, depth))
-    if need < 0:
-        raise ValueError(f"Number of cross layers (depth) should be positive but is {depth}.")
-    ws = torch.empty(max(need, 256), dtype=torch.uint8, device=x0.device)
-    kp = (C.c_void_p * depth)(*[k.data_ptr() for k in kernels])
-    bp = (C.c_void_p * depth)(*[_ptr(b) for b in biases])
-    _cabi.check(_lib().mm_cross_forward(x0.data_ptr(), M, d, _row_stride(x0, "x0"), depth, kp, bp, out.data_ptr(),
-                                        _row_stride(out, "out"), ws.data_ptr(), need, _stream()), "mm_cross_forward")
-    return out
 
 
 def mlp_tc_supported(K: int, widths: Sequence[int], head: bool = False, heads: bool = False) -> bool:
@@ -757,18 +721,15 @@ def mlp_tc_supported(K: int, widths: Sequence[int], head: bool = False, heads: b
     return bool(_lib().mm_mlp_tc_supported(int(K), n, wd, 2 if heads else 1 if head else 0))
 
 
-def mlp_tc(a_split: torch.Tensor, K: int, w_splits: Sequence[torch.Tensor], widths: Sequence[int],
-           biases: Sequence[Optional[torch.Tensor]], acts: Sequence[Optional[str]], out: Optional[torch.Tensor] = None,
-           head_w: Optional[torch.Tensor] = None, head_b: float = 0.0, head_act: Optional[str] = None,
-           head_out: Optional[torch.Tensor] = None, out_operand: Optional[torch.Tensor] = None):
-    """Whole MLP tower in one launch (mm_mlp_tc): layer 1 from the split-bf16 rows `a_split`, layers 2..n on
-    chip (activations stay in registers).  out: (M, widths[-1]) fp32 and/or head_out: (M, 1); out_operand:
-    (M, 2*widths[-1]) bf16 split rows [hi | lo] for the interaction kernel (mm_mlp_tc_operand_out)."""
+def _tower(who: str, a_split: torch.Tensor, K: int, w_splits: Sequence[torch.Tensor], widths: Sequence[int],
+           biases: Sequence[Optional[torch.Tensor]], acts: Sequence[Optional[str]]):
+    """(M, n, weight pointers, widths, bias pointers, activation codes) of a tower over the split-bf16 rows a_split
+    (M, 2*Kp): layer l is w_splits[l], the mm_split_weights layout of a (k, widths[l]) kernel, biases[l] None or
+    widths[l] fp32 values, acts[l] its activation."""
     n = len(widths)
     if not (len(w_splits) == len(biases) == len(acts) == n):
-        raise ValueError("mlp_tc: w_splits / widths / biases / acts must have one entry per layer")
+        raise ValueError(f"{who}: w_splits / widths / biases / acts must have one entry per layer")
     _dev(a_split, "a_split", torch.bfloat16)
-    M = a_split.shape[0]
     if a_split.dim() != 2 or a_split.shape[1] != 2 * tc_padded_k(K) or not a_split.is_contiguous():
         raise ValueError(f"a_split must be a contiguous (M, {2 * tc_padded_k(K)}) bf16 matrix")
     k = K
@@ -776,11 +737,24 @@ def mlp_tc(a_split: torch.Tensor, K: int, w_splits: Sequence[torch.Tensor], widt
         _dev(w_splits[l], f"w_split[{l}]", torch.bfloat16)
         if tuple(w_splits[l].shape) != (tc_padded_n(int(widths[l])), 2 * tc_padded_k(k)) or not w_splits[l].is_contiguous():
             raise ValueError(f"w_split[{l}] must be the mm_split_weights layout of a ({k}, {widths[l]}) kernel")
-        if biases[l] is not None:
-            _dev(biases[l], f"bias[{l}]", torch.float32)
-            if biases[l].numel() != int(widths[l]):
-                raise ValueError(f"bias[{l}] must hold {widths[l]} values")
+        if biases[l] is not None and _dev(biases[l], f"bias[{l}]", torch.float32).numel() != int(widths[l]):
+            raise ValueError(f"bias[{l}] must hold {widths[l]} values")
         k = int(widths[l])
+    wp = (C.c_void_p * n)(*[w.data_ptr() for w in w_splits])
+    wd = (C.c_int * n)(*[int(w) for w in widths])
+    bp = (C.c_void_p * n)(*[_ptr(b) for b in biases])
+    ac = (C.c_int * n)(*[ACTIVATIONS[a] for a in acts])
+    return a_split.shape[0], n, wp, wd, bp, ac
+
+
+def mlp_tc(a_split: torch.Tensor, K: int, w_splits: Sequence[torch.Tensor], widths: Sequence[int],
+           biases: Sequence[Optional[torch.Tensor]], acts: Sequence[Optional[str]], out: Optional[torch.Tensor] = None,
+           head_w: Optional[torch.Tensor] = None, head_b: float = 0.0, head_act: Optional[str] = None,
+           head_out: Optional[torch.Tensor] = None, out_operand: Optional[torch.Tensor] = None):
+    """Whole MLP tower in one launch (mm_mlp_tc): layer 1 from the split-bf16 rows `a_split`, layers 2..n on
+    chip (activations stay in registers).  out: (M, widths[-1]) fp32 and/or head_out: (M, 1); out_operand:
+    (M, 2*widths[-1]) bf16 split rows [hi | lo] for the interaction kernel (mm_mlp_tc_operand_out)."""
+    M, n, wp, wd, bp, ac = _tower("mlp_tc", a_split, K, w_splits, widths, biases, acts)
     if out is not None:
         _dev(out, "out", torch.float32)
         if out.dim() != 2 or tuple(out.shape) != (M, int(widths[-1])) or out.stride(1) != 1:
@@ -791,10 +765,6 @@ def mlp_tc(a_split: torch.Tensor, K: int, w_splits: Sequence[torch.Tensor], widt
         _dev(head_w, "head_w", torch.float32), _dev(head_out, "head_out", torch.float32)
         if head_w.numel() != int(widths[-1]) or not head_w.is_contiguous() or head_out.numel() != M or not head_out.is_contiguous():
             raise ValueError("head_w must hold widths[-1] weights and head_out M contiguous values")
-    wp = (C.c_void_p * n)(*[w.data_ptr() for w in w_splits])
-    bp = (C.c_void_p * n)(*[_ptr(b) for b in biases])
-    wd = (C.c_int * n)(*[int(w) for w in widths])
-    ac = (C.c_int * n)(*[ACTIVATIONS[a] for a in acts])
     if out_operand is not None:
         if head_w is not None:
             raise ValueError("out_operand and the fused head exclude each other")
@@ -819,31 +789,14 @@ def mlp_tc_heads(a_split: torch.Tensor, K: int, w_splits: Sequence[torch.Tensor]
     """mm_mlp_tc_heads: the whole tower with H <= 8 fused output heads; out (H, M) with
     out[h] = heads_act[h](tower(x) @ heads_w[:, h] + heads_b[h]).  heads_w (widths[-1], H) Keras layout, heads_b (H,) on the
     device (read by the kernel, not copied to the host)."""
-    n = len(widths)
-    if not (len(w_splits) == len(biases) == len(acts) == n):
-        raise ValueError("mlp_tc_heads: w_splits / widths / biases / acts must have one entry per layer")
-    _dev(a_split, "a_split", torch.bfloat16), _dev(heads_w, "heads_w", torch.float32), _dev(out, "out", torch.float32)
-    M, H = a_split.shape[0], len(heads_act)
-    if a_split.dim() != 2 or a_split.shape[1] != 2 * tc_padded_k(K) or not a_split.is_contiguous():
-        raise ValueError(f"a_split must be a contiguous (M, {2 * tc_padded_k(K)}) bf16 matrix")
+    M, n, wp, wd, bp, ac = _tower("mlp_tc_heads", a_split, K, w_splits, widths, biases, acts)
+    _dev(heads_w, "heads_w", torch.float32), _dev(out, "out", torch.float32)
+    H = len(heads_act)
     if tuple(heads_w.shape) != (int(widths[-1]), H) or not heads_w.is_contiguous():
         raise ValueError(f"heads_w must be a contiguous ({widths[-1]}, {H}) matrix")
-    if heads_b is not None and (_dev(heads_b, "heads_b", torch.float32).numel() != H or not heads_b.is_contiguous()):
-        raise ValueError(f"heads_b must hold {H} contiguous values")
+    _vec(heads_b, H, "heads_b")
     if tuple(out.shape) != (H, M) or not out.is_contiguous():
         raise ValueError(f"out must be a contiguous ({H}, {M}) matrix")
-    k = K
-    for l in range(n):
-        _dev(w_splits[l], f"w_split[{l}]", torch.bfloat16)
-        if tuple(w_splits[l].shape) != (tc_padded_n(int(widths[l])), 2 * tc_padded_k(k)) or not w_splits[l].is_contiguous():
-            raise ValueError(f"w_split[{l}] must be the mm_split_weights layout of a ({k}, {widths[l]}) kernel")
-        if biases[l] is not None and (_dev(biases[l], f"bias[{l}]", torch.float32).numel() != int(widths[l])):
-            raise ValueError(f"bias[{l}] must hold {widths[l]} values")
-        k = int(widths[l])
-    wp = (C.c_void_p * n)(*[w.data_ptr() for w in w_splits])
-    bp = (C.c_void_p * n)(*[_ptr(b) for b in biases])
-    wd = (C.c_int * n)(*[int(w) for w in widths])
-    ac = (C.c_int * n)(*[ACTIVATIONS[a] for a in acts])
     ha = (C.c_int * H)(*[ACTIVATIONS[a] for a in heads_act])
     _cabi.check(_lib().mm_mlp_tc_heads(a_split.data_ptr(), M, K, n, wp, wd, bp, ac, H, heads_w.data_ptr(), _ptr(heads_b), ha,
                                        out.data_ptr(), _stream()), "mm_mlp_tc_heads")
@@ -870,31 +823,15 @@ def dense_tc_head(a_split: torch.Tensor, K: int, w_split: torch.Tensor, N: int, 
 
 # ---- training step (include/mm_b200.h K14) -----------------------------------------------------------------------
 _TARGET_DTYPES = {torch.int32: MM_I32, torch.int64: MM_I64, torch.float32: _cabi.MM_F32, torch.float64: _cabi.MM_F64}
+_SAMPLE_WEIGHT = "be ({n},) contiguous float32"  # _vec's error for a sample-weight column
 
 
-def bce_head_fwd_bwd(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], targets: torch.Tensor,
-                     loss_sum: torch.Tensor, dx: Optional[torch.Tensor], dw: torch.Tensor, db: Optional[torch.Tensor],
-                     mask_relu: bool = True, sample_weight: Optional[torch.Tensor] = None,
-                     logits: Optional[torch.Tensor] = None) -> None:
-    """Dense(K -> 1) + sigmoid + binary cross-entropy, forward and backward (mm_bce_head_fwd_bwd).  loss_sum (1,), dw (K,),
-    db (1,) are ACCUMULATED; dx (M, K) is written (zeroed where x <= 0 when mask_relu)."""
-    _dev(x, "x", torch.float32), _dev(w, "w", torch.float32), _dev(targets, "targets"), _dev(loss_sum, "loss_sum", torch.float32)
-    _dev(dw, "dw", torch.float32)
-    M, K = x.shape
-    if w.numel() != K or dw.numel() != K or not w.is_contiguous() or not dw.is_contiguous():
-        raise ValueError(f"w and dw must hold {K} contiguous values")
-    if targets.numel() != M or not targets.is_contiguous() or targets.dtype not in _TARGET_DTYPES:
-        raise ValueError(f"targets must be {M} contiguous int32 / int64 / float32 / float64 values")
-    if sample_weight is not None and (sample_weight.numel() != M or sample_weight.dtype != torch.float32 or not sample_weight.is_contiguous()):
-        raise ValueError("sample_weight must be (M,) contiguous float32")
-    if logits is not None and (logits.numel() != M or logits.dtype != torch.float32 or not logits.is_contiguous()):
-        raise ValueError("logits must be (M,) contiguous float32")
-    _cabi.check(
-        _lib().mm_bce_head_fwd_bwd(x.data_ptr(), M, K, _row_stride(x, "x"), w.data_ptr(), _ptr(bias), targets.data_ptr(),
-                                   _TARGET_DTYPES[targets.dtype], _ptr(sample_weight), _ptr(logits), loss_sum.data_ptr(), _ptr(dx),
-                                   0 if dx is None else _row_stride(_dev(dx, "dx", torch.float32), "dx"), 1 if mask_relu else 0,
-                                   dw.data_ptr(), _ptr(db), _stream()),
-        "mm_bce_head_fwd_bwd")
+def _target(t: torch.Tensor, M: int, name: str) -> int:
+    """Dtype code of a target column: M contiguous int32 / int64 / float32 / float64 values."""
+    _dev(t, name)
+    if t.numel() != M or not t.is_contiguous() or t.dtype not in _TARGET_DTYPES:
+        raise ValueError(f"{name} must be {M} contiguous int32 / int64 / float32 / float64 values")
+    return _TARGET_DTYPES[t.dtype]
 
 
 def heads_fwd_bwd(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], losses: Sequence[str],
@@ -911,8 +848,7 @@ def heads_fwd_bwd(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor]
     H = len(losses)
     if tuple(w.shape) != (K, H) or not w.is_contiguous():
         raise ValueError(f"w must be a contiguous ({K}, {H}) matrix")
-    if bias is not None and (_dev(bias, "bias", torch.float32).numel() != H or not bias.is_contiguous()):
-        raise ValueError(f"bias must hold {H} contiguous values")
+    _vec(bias, H, "bias")
     if tuple(out.shape) != (H, M) or not out.is_contiguous():
         raise ValueError(f"out must be a contiguous ({H}, {M}) matrix")
     if any(l not in _cabi.LOSS_KINDS for l in losses):
@@ -922,10 +858,7 @@ def heads_fwd_bwd(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor]
     if targets is not None:
         if len(targets) != H:
             raise ValueError(f"one target tensor per head: {H} expected, got {len(targets)}")
-        for h, t in enumerate(targets):
-            _dev(t, f"targets[{h}]")
-            if t.numel() != M or not t.is_contiguous() or t.dtype not in _TARGET_DTYPES:
-                raise ValueError(f"targets[{h}] must be {M} contiguous int32 / int64 / float32 / float64 values")
+        dt = (C.c_int * H)(*[_target(t, M, f"targets[{h}]") for h, t in enumerate(targets)])
         if loss is None:
             raise ValueError("training needs loss")
         _dev(loss, "loss", torch.float32)
@@ -933,19 +866,16 @@ def heads_fwd_bwd(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor]
             raise ValueError(f"loss must hold 1 + H = {1 + H} contiguous values")
         if dw is not None and (_dev(dw, "dw", torch.float32).shape != (K, H) or not dw.is_contiguous()):
             raise ValueError(f"dw must be a contiguous ({K}, {H}) matrix")
-        if db is not None and (_dev(db, "db", torch.float32).numel() != H or not db.is_contiguous()):
-            raise ValueError(f"db must hold {H} contiguous values")
+        _vec(db, H, "db")
         sws = list(sample_weight) if isinstance(sample_weight, (list, tuple)) else [sample_weight] * H
         if len(sws) != H:
             raise ValueError(f"one sample-weight tensor per head: {H} expected, got {len(sws)}")
         for h, s in enumerate(sws):
-            if s is not None and (_dev(s, f"sample_weight[{h}]", torch.float32).numel() != M or not s.is_contiguous()):
-                raise ValueError(f"sample_weight[{h}] must be ({M},) contiguous float32")
+            _vec(s, M, f"sample_weight[{h}]", _SAMPLE_WEIGHT)
         lws = [1.0] * H if loss_weights is None else [float(v) for v in loss_weights]
         if len(lws) != H:
             raise ValueError(f"one loss weight per head: {H} expected, got {len(lws)}")
         tp = (C.c_void_p * H)(*[t.data_ptr() for t in targets])
-        dt = (C.c_int * H)(*[_TARGET_DTYPES[t.dtype] for t in targets])
         sp = (C.c_void_p * H)(*[_ptr(s) for s in sws])
         lw = (C.c_float * H)(*lws)
     _cabi.check(
@@ -958,31 +888,33 @@ def heads_fwd_bwd(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor]
     return out
 
 
-def dense_wgrad(x: torch.Tensor, dz: torch.Tensor, dw: torch.Tensor, db: Optional[torch.Tensor]) -> None:
-    """dw (K, N) += x^T dz;  db (N,) += column sums of dz  (mm_dense_wgrad; accumulated)."""
-    _dev(x, "x", torch.float32), _dev(dz, "dz", torch.float32), _dev(dw, "dw", torch.float32)
-    M, K = x.shape
+def _wgrad_n(M: int, K: int, dz: torch.Tensor, dw: torch.Tensor, db: Optional[torch.Tensor]) -> int:
+    """N of the gradients of a Dense layer with M rows of K inputs: dz (M, N), dw a contiguous (K, N) matrix, db (N,) or None."""
+    _dev(dz, "dz", torch.float32), _dev(dw, "dw", torch.float32)
     N = dz.shape[1]
     if dz.shape[0] != M or tuple(dw.shape) != (K, N) or not dw.is_contiguous():
         raise ValueError(f"dz must be ({M}, N) and dw a contiguous ({K}, {N}) matrix")
-    if db is not None and (_dev(db, "db", torch.float32).numel() != N or not db.is_contiguous()):
-        raise ValueError(f"db must hold {N} contiguous values")
+    _vec(db, N, "db")
+    return N
+
+
+def dense_wgrad(x: torch.Tensor, dz: torch.Tensor, dw: torch.Tensor, db: Optional[torch.Tensor]) -> None:
+    """dw (K, N) += x^T dz;  db (N,) += column sums of dz  (mm_dense_wgrad; accumulated)."""
+    _dev(x, "x", torch.float32)
+    M, K = x.shape
+    N = _wgrad_n(M, K, dz, dw, db)
     _cabi.check(_lib().mm_dense_wgrad(x.data_ptr(), M, K, _row_stride(x, "x"), dz.data_ptr(), N, _row_stride(dz, "dz"), dw.data_ptr(),
                                       _ptr(db), _stream()), "mm_dense_wgrad")
 
 
 def dense_wgrad_split(x_split: torch.Tensor, K: int, dz: torch.Tensor, dw: torch.Tensor, db: Optional[torch.Tensor]) -> None:
     """dense_wgrad with x given as the split-bf16 operand (M, 2*Kp) the forward layer consumed (mm_dense_wgrad_split)."""
-    _dev(x_split, "x_split", torch.bfloat16), _dev(dz, "dz", torch.float32), _dev(dw, "dw", torch.float32)
+    _dev(x_split, "x_split", torch.bfloat16)
     M = x_split.shape[0]
     Kp = tc_padded_k(K)
-    N = dz.shape[1]
     if tuple(x_split.shape) != (M, 2 * Kp) or not x_split.is_contiguous():
         raise ValueError(f"x_split must be a contiguous bf16 ({M}, {2 * Kp}) matrix")
-    if dz.shape[0] != M or tuple(dw.shape) != (K, N) or not dw.is_contiguous():
-        raise ValueError(f"dz must be ({M}, N) and dw a contiguous ({K}, {N}) matrix")
-    if db is not None and (_dev(db, "db", torch.float32).numel() != N or not db.is_contiguous()):
-        raise ValueError(f"db must hold {N} contiguous values")
+    N = _wgrad_n(M, K, dz, dw, db)
     _cabi.check(_lib().mm_dense_wgrad_split(x_split.data_ptr(), M, K, Kp, dz.data_ptr(), N, _row_stride(dz, "dz"), dw.data_ptr(), _ptr(db),
                                             _stream()), "mm_dense_wgrad_split")
 
@@ -1147,14 +1079,11 @@ def cross_backward(x0: torch.Tensor, z: torch.Tensor, g: torch.Tensor, p: Option
                                          dz_split.data_ptr(), Kp, _stream()), "mm_cross_backward")
 
 
-def concat_backward(addends: Sequence[torch.Tensor], slices: Sequence[tuple]) -> None:
-    """Backward of a concatenated input block (mm_concat_backward): for each (dst (B, w), col) in `slices`,
-    dst = sum of the (B, d) addends' columns [col, col + w)."""
-    if not addends:
-        raise ValueError("concat_backward needs at least one addend")
-    B, d = addends[0].shape
+def _addends_slices(addends: Sequence[torch.Tensor], slices: Sequence[tuple], B: int, d: int):
+    """(pointers, row strides, mm_column_slice array) of a concat backward's (B, d) fp32 addends and its (dst (B, width), col)
+    slices."""
     n = len(addends)
-    ap, st = (C.c_void_p * n)(), (C.c_int64 * n)()
+    ap, st = (C.c_void_p * max(n, 1))(), (C.c_int64 * max(n, 1))()
     for i, a in enumerate(addends):
         _dev(a, f"addends[{i}]", torch.float32)
         if tuple(a.shape) != (B, d):
@@ -1166,7 +1095,17 @@ def concat_backward(addends: Sequence[torch.Tensor], slices: Sequence[tuple]) ->
         if dst.dim() != 2 or dst.shape[0] != B:
             raise ValueError(f"slices[{t}].dst must be ({B}, width), got {tuple(dst.shape)}")
         arr[t].dst, arr[t].dst_stride, arr[t].col, arr[t].width = dst.data_ptr(), _row_stride(dst, f"slices[{t}].dst"), int(col), dst.shape[1]
-    _cabi.check(_lib().mm_concat_backward(ap, st, n, B, d, arr, len(slices), _stream()), "mm_concat_backward")
+    return ap, st, arr
+
+
+def concat_backward(addends: Sequence[torch.Tensor], slices: Sequence[tuple]) -> None:
+    """Backward of a concatenated input block (mm_concat_backward): for each (dst (B, w), col) in `slices`,
+    dst = sum of the (B, d) addends' columns [col, col + w)."""
+    if not addends:
+        raise ValueError("concat_backward needs at least one addend")
+    B, d = addends[0].shape
+    ap, st, arr = _addends_slices(addends, slices, B, d)
+    _cabi.check(_lib().mm_concat_backward(ap, st, len(addends), B, d, arr, len(slices), _stream()), "mm_concat_backward")
 
 
 def dense_apply(opt: str, w: torch.Tensor, grad: torch.Tensor, state1: Optional[torch.Tensor], state2: Optional[torch.Tensor],
@@ -1214,14 +1153,7 @@ def deepfm_head(weights, indices, wide_offsets, cont, cont_offsets, wide_kernel:
     D = weights[0].shape[1]
     arr = _lookup_tables(weights, indices, B, torch.float32, D)
     woff = (C.c_int64 * n)(*[int(o) for o in wide_offsets])
-    m = len(cont)
-    if len(cont_offsets) != m:
-        raise ValueError("cont / cont_offsets length mismatch")
-    for c, t in enumerate(cont):
-        if _dev(t, f"cont[{c}]").numel() != B:
-            raise ValueError(f"cont[{c}] must hold {B} values")
-    carr, _, _ = _concat_pieces([t.reshape(-1) for t in cont], B, "cont")
-    coff = (C.c_int64 * max(m, 1))(*[int(o) for o in cont_offsets])
+    carr, coff, m = _cont_columns(cont, cont_offsets, B)
     if addend is not None and (_dev(addend, "addend", torch.float32).numel() != B):
         raise ValueError(f"addend must hold {B} values")
     a_stride = 0 if addend is None else (addend.stride(0) if addend.dim() >= 1 else 1)
@@ -1239,10 +1171,8 @@ def _wide_blocks(indices, rows, offsets, B: int):
         raise ValueError("indices / rows / offsets length mismatch")
     arr = (_cabi.WideBlock * max(n, 1))()
     for t in range(n):
-        ix = _dev(indices[t], f"indices[{t}]")
-        w = index_bytes_of(ix)
-        if ix.shape[0] != B or not ix.is_contiguous() or (ix.numel() != B * (3 if w == 3 else 1)):
-            raise ValueError(f"indices[{t}] must be {B} contiguous ids, got {tuple(ix.shape)}")
+        ix = indices[t]
+        w = _id_column(ix, B, f"indices[{t}]", leading=True)
         arr[t].indices, arr[t].rows, arr[t].offset, arr[t].idx_bytes = ix.data_ptr(), int(rows[t]), int(offsets[t]), w
     return arr, n
 
@@ -1272,8 +1202,7 @@ def deepfm_head_fwd_bwd(x0: torch.Tensor, emb_cols, D: int, indices, rows, wide_
     for n_, t_, k in (("out_w", out_w, 1), ("out_b", out_b, 1), ("b_dl", b_dl, 1), ("wide_bias", wide_bias, 1),
                       ("dw_out", dw_out, 1), ("db_out", db_out, 1), ("db_dl", db_dl, 1), ("d_wide_bias", d_wide_bias, 1),
                       ("dw_dl", dw_dl, U), ("d_cont", d_cont, len(cont))):
-        if t_ is not None and (_dev(t_, n_, torch.float32).numel() != k or not t_.is_contiguous()):
-            raise ValueError(f"{n_} must hold {k} contiguous float32 values")
+        _vec(t_, k, n_, "hold {n} contiguous float32 values")
     if logits.numel() != B or ds.numel() != B or not logits.is_contiguous() or not ds.is_contiguous():
         raise ValueError(f"logits and ds must hold {B} contiguous values")
     if loss_buf.numel() != 2 or not loss_buf.is_contiguous():
@@ -1282,29 +1211,19 @@ def deepfm_head_fwd_bwd(x0: torch.Tensor, emb_cols, D: int, indices, rows, wide_
         raise ValueError(f"loss must be among {sorted(_cabi.LOSS_KINDS)}, got {loss!r}")
     if act_dl not in ("linear", "relu"):
         raise ValueError(f"the deep logit's activation must be linear or relu, got {act_dl!r}")
-    _dev(targets, "targets")
-    if targets.numel() != B or not targets.is_contiguous() or targets.dtype not in _TARGET_DTYPES:
-        raise ValueError(f"targets must be {B} contiguous int32 / int64 / float32 / float64 values")
-    if sample_weight is not None and (_dev(sample_weight, "sample_weight", torch.float32).numel() != B or not sample_weight.is_contiguous()):
-        raise ValueError(f"sample_weight must be ({B},) contiguous float32")
+    target_dtype = _target(targets, B, "targets")
+    _vec(sample_weight, B, "sample_weight", _SAMPLE_WEIGHT)
     n = len(indices)
     if len(emb_cols) != n:
         raise ValueError("emb_cols / indices length mismatch")
     arr, _ = _wide_blocks(indices, rows, wide_offsets, B)
     cols = (C.c_int64 * max(n, 1))(*[int(c) for c in emb_cols])
-    m = len(cont)
-    if len(cont_offsets) != m:
-        raise ValueError("cont / cont_offsets length mismatch")
-    for c, t in enumerate(cont):
-        if _dev(t, f"cont[{c}]").numel() != B:
-            raise ValueError(f"cont[{c}] must hold {B} values")
-    carr, _, _ = _concat_pieces([t.reshape(-1) for t in cont], B, "cont")
-    coff = (C.c_int64 * max(m, 1))(*[int(o) for o in cont_offsets])
+    carr, coff, m = _cont_columns(cont, cont_offsets, B)
     _cabi.check(
         _lib().mm_deepfm_head_fwd_bwd(x0.data_ptr(), _row_stride(x0, "x0"), cols, int(D), arr, n, carr, coff, m, wide_kernel.data_ptr(),
                                       _ptr(wide_bias), h.data_ptr(), _row_stride(h, "h"), U, 1 if mask_h else 0, w_dl.data_ptr(),
                                       _ptr(b_dl), ACTIVATIONS[act_dl], out_w.data_ptr(), _ptr(out_b), _cabi.LOSS_KINDS[loss],
-                                      targets.data_ptr(), _TARGET_DTYPES[targets.dtype], _ptr(sample_weight), B, logits.data_ptr(),
+                                      targets.data_ptr(), target_dtype, _ptr(sample_weight), B, logits.data_ptr(),
                                       loss_buf.data_ptr(), ds.data_ptr(), dh.data_ptr(), _row_stride(dh, "dh"), _ptr(dw_out),
                                       _ptr(db_out), _ptr(dw_dl), _ptr(db_dl), _ptr(d_wide_bias), _ptr(d_cont), _ptr(oob), _stream()),
         "mm_deepfm_head_fwd_bwd")
@@ -1317,21 +1236,9 @@ def fm_concat_backward(addends: Sequence[torch.Tensor], x0: torch.Tensor, ds: to
     B, d = x0.shape
     if ds.numel() != B or not ds.is_contiguous():
         raise ValueError(f"ds must hold {B} contiguous values")
-    n = len(addends)
-    ap, st = (C.c_void_p * max(n, 1))(), (C.c_int64 * max(n, 1))()
-    for i, a in enumerate(addends):
-        _dev(a, f"addends[{i}]", torch.float32)
-        if tuple(a.shape) != (B, d):
-            raise ValueError(f"addends[{i}] must be ({B}, {d}), got {tuple(a.shape)}")
-        ap[i], st[i] = a.data_ptr(), _row_stride(a, f"addends[{i}]")
-    arr = (_cabi.ColumnSlice * max(len(slices), 1))()
-    for t, (dst, col) in enumerate(slices):
-        _dev(dst, f"slices[{t}].dst", torch.float32)
-        if dst.dim() != 2 or dst.shape[0] != B:
-            raise ValueError(f"slices[{t}].dst must be ({B}, width), got {tuple(dst.shape)}")
-        arr[t].dst, arr[t].dst_stride, arr[t].col, arr[t].width = dst.data_ptr(), _row_stride(dst, f"slices[{t}].dst"), int(col), dst.shape[1]
-    _cabi.check(_lib().mm_fm_concat_backward(ap, st, n, B, d, x0.data_ptr(), _row_stride(x0, "x0"), ds.data_ptr(), arr, len(slices),
-                                             _stream()), "mm_fm_concat_backward")
+    ap, st, arr = _addends_slices(addends, slices, B, d)
+    _cabi.check(_lib().mm_fm_concat_backward(ap, st, len(addends), B, d, x0.data_ptr(), _row_stride(x0, "x0"), ds.data_ptr(), arr,
+                                             len(slices), _stream()), "mm_fm_concat_backward")
 
 
 def wide_rows_apply(opt: str, wide: torch.Tensor, state1: Optional[torch.Tensor], state2: Optional[torch.Tensor], indices, rows,
@@ -1403,9 +1310,7 @@ def metrics_update(z: torch.Tensor, losses: Sequence[str], targets: Sequence[tor
     for h in range(H):
         if losses[h] not in _cabi.LOSS_KINDS:
             raise ValueError(f"losses must be among {sorted(_cabi.LOSS_KINDS)}, got {losses[h]!r}")
-        t = _dev(targets[h], f"targets[{h}]")
-        if t.numel() != M or not t.is_contiguous() or t.dtype not in _TARGET_DTYPES:
-            raise ValueError(f"targets[{h}] must be {M} contiguous int32 / int64 / float32 / float64 values")
+        arr[h].target_dtype = _target(targets[h], M, f"targets[{h}]")
         ws = [sws[h]] + [s[h] for s in sets]
         for i, w in enumerate(ws):
             if w is not None and (_dev(w, "weights", torch.float32).numel() != M or not w.is_contiguous()):
@@ -1413,11 +1318,10 @@ def metrics_update(z: torch.Tensor, losses: Sequence[str], targets: Sequence[tor
         thr = [float(v) for v in thresholds[h]]
         if len(thr) > _cabi.METRICS_MAX_THRESHOLDS:
             raise ValueError(f"head {h}: at most {_cabi.METRICS_MAX_THRESHOLDS} thresholds, got {len(thr)}")
-        arr[h].targets = t.data_ptr()
+        arr[h].targets = targets[h].data_ptr()
         arr[h].sample_weight = _ptr(sws[h])
         for s in range(len(sets)):
             arr[h].metric_weights[s] = _ptr(sets[s][h])
-        arr[h].target_dtype = _TARGET_DTYPES[t.dtype]
         arr[h].loss_kind = _cabi.LOSS_KINDS[losses[h]]
         arr[h].pred_form = int(pred_forms[h])
         arr[h].n_thresholds = len(thr)

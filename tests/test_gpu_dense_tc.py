@@ -7,7 +7,7 @@ import pytest
 import torch
 
 import models_b200 as mm
-from models_b200 import datasets, ops
+from models_b200 import blocks, datasets, ops
 from oracle import oracle
 from tests import helpers as H
 
@@ -65,29 +65,46 @@ def test_dense_tc_split_output_feeds_next_layer(device):
     assert torch.equal(ops.split_rows(out), nxt)  # identical to splitting the fp32 output
 
 
-def test_dense_chain_tc_vs_fp32_engine(device):
+def _dense_chain_vs_oracle(device, K, widths, use_bias, strided, path, tol):
+    """MLPBlock(widths) on both dense engines against the oracle; `path` is the tensor-core path the tower must take."""
     mm.set_seed(3)
     rng = np.random.default_rng(3)
-    x = dev(rng.standard_normal((2000, 415)).astype(np.float32), device)
-    mlp = mm.MLPBlock([128, 64, 32])
+    x = dev(rng.standard_normal((2000, K)).astype(np.float32), device)
+    if strided:
+        x = torch.zeros((2000, K + 5), device=device)[:, :K].copy_(x)
+    mlp = mm.MLPBlock(widths, use_bias=use_bias)
     mm.set_dense_engine("tc")
     try:
         y_tc = mlp(x).cpu().numpy()
+        assert blocks.last_dense_path() == path
         mm.set_dense_engine("fp32")
         y_32 = mlp(x).cpu().numpy()
     finally:
         mm.set_dense_engine("auto")
     ref = oracle.mlp(x.cpu().numpy(), H.mlp_layers(mlp))
     assert H.rel_err(y_32, ref) < 2e-5
-    assert H.rel_err(y_tc, ref) < 5e-5
+    assert H.rel_err(y_tc, ref) < tol
 
 
-def test_cross_block_tc_matches_oracle(device):
+def test_dense_chain_tc_vs_fp32_engine(device):
+    _dense_chain_vs_oracle(device, 415, [128, 64, 32], True, False, "mlp_tc", 5e-5)
+
+
+@pytest.mark.parametrize("K,widths,use_bias,strided,tol", [
+    (13, [512, 256, 64], False, True, 1.5e-4),      # width > 128, no biases, input a strided view
+    (200, [100, 50, 20, 7, 3], True, False, 2.5e-4),  # more than 4 layers
+])
+def test_dense_chain_per_layer_tc_vs_fp32_engine(device, K, widths, use_bias, strided, tol):
+    """Towers the whole-tower kernel does not take: one mm_dense_tc launch per layer."""
+    _dense_chain_vs_oracle(device, K, widths, use_bias, strided, "dense_tc", tol)
+
+
+def _cross_block_vs_oracle(device, d, depth, tol):
     mm.set_seed(4)
     rng = np.random.default_rng(4)
-    B, d = 700, 1037
+    B = 700
     x0 = rng.standard_normal((B, d)).astype(np.float32)
-    cross = mm.CrossBlock(3)
+    cross = mm.CrossBlock(depth)
     for eng in ("tc", "fp32"):
         mm.set_dense_engine(eng)
         try:
@@ -96,7 +113,17 @@ def test_cross_block_tc_matches_oracle(device):
             mm.set_dense_engine("auto")
         layers = [{"kernel": H.to_numpy(l.dense.kernel), "bias": H.to_numpy(l.dense.bias)} for l in cross.cross_layers]
         ref = oracle.cross_layers(x0, layers)
-        assert H.rel_err(y, ref) < 5e-5, eng
+        assert H.rel_err(y, ref) < tol, eng
+
+
+def test_cross_block_tc_matches_oracle(device):
+    _cross_block_vs_oracle(device, 1037, 3, 5e-5)
+
+
+@pytest.mark.parametrize("d,depth,tol", [(100, 4, 1e-4), (415, 1, 1e-4)])
+def test_cross_block_depths_tc_matches_oracle(device, d, depth, tol):
+    """CrossBlock at depth 1, and deeper with d not a multiple of 64."""
+    _cross_block_vs_oracle(device, d, depth, tol)
 
 
 def test_dense_tc_argument_errors(device):

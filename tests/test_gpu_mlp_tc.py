@@ -189,43 +189,6 @@ def test_mlp_block_on_feature_dict_uses_concat_split(device):
     assert H.rel_err(got.cpu().numpy(), ref) < 1e-4
 
 
-@pytest.mark.parametrize("K,widths", [(415, [128, 64, 32]), (13, [512, 256, 64]), (69, [256, 128]), (200, [100, 50, 20, 7, 3]),
-                                      (64, [16])])
-def test_mm_mlp_forward_whole_op_matches_oracle(device, K, widths):
-    """mm_mlp_forward: fp32 Keras-layout kernels in, one C call, workspace-backed (fused tower when the widths
-    allow it, per-layer wgmma otherwise) == oracle.dense chain."""
-    rng = np.random.default_rng(18)
-    M = 1537
-    x = rng.standard_normal((M, K)).astype(np.float32)
-    Ws, bs = _tower(rng, K, widths)
-    acts = (["relu", "tanh", "relu", "sigmoid", "linear"] * 2)[: len(widths)]
-    bs[0] = None  # use_bias=False layer
-    out = ops.mlp_forward(dev(x, device), [dev(W, device) for W in Ws], [None if b is None else dev(b, device) for b in bs], acts)
-    ref = _oracle_chain(x, Ws, [np.zeros(widths[0], np.float32)] + bs[1:], acts)
-    assert H.rel_err(out.cpu().numpy(), ref) < 5e-5 * len(widths)
-    # strided input / output views
-    big = torch.zeros((M, K + 5), device=device)
-    big[:, :K] = dev(x, device)
-    wide = torch.full((M, widths[-1] + 3), 9.0, device=device)
-    ops.mlp_forward(big[:, :K], [dev(W, device) for W in Ws], [None if b is None else dev(b, device) for b in bs], acts,
-                    out=wide[:, : widths[-1]])
-    assert torch.equal(wide[:, : widths[-1]], out) and float(wide[:, widths[-1]:].min()) == 9.0
-
-
-@pytest.mark.parametrize("d,depth", [(1037, 3), (64, 2), (100, 4), (415, 1)])
-def test_mm_cross_forward_whole_op_matches_oracle(device, d, depth):
-    rng = np.random.default_rng(19)
-    M = 700
-    x0 = rng.standard_normal((M, d)).astype(np.float32)
-    Ws = [(rng.standard_normal((d, d)) * 0.05 / np.sqrt(d) * 10).astype(np.float32) for _ in range(depth)]
-    bs = [(rng.standard_normal(d) * 0.1).astype(np.float32) for _ in range(depth)]
-    out = ops.cross_forward(dev(x0, device), [dev(W, device) for W in Ws], [dev(b, device) for b in bs])
-    ref = oracle.cross_layers(x0, [{"kernel": W, "bias": b} for W, b in zip(Ws, bs)])
-    assert H.rel_err(out.cpu().numpy(), ref) < 1e-4
-    with pytest.raises(ValueError, match="should be positive"):
-        ops.cross_forward(dev(x0, device), [], [])
-
-
 @pytest.mark.parametrize("dims,K,acts", [([128, 64], 13, "relu"), ([64, 32], 5, ["tanh", "linear"]), ([32, 16], 16, ["gelu", "sigmoid"]),
                                          ([128, 16], 1, "relu")])
 @pytest.mark.parametrize("B", [1, 17, 4099])

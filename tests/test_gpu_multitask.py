@@ -123,39 +123,6 @@ def test_heads_forward_only_touches_no_gradient_buffer(device, K):
         assert float(t.min()) == 5.0 and float(t.max()) == 5.0
 
 
-@pytest.mark.parametrize("M,K", [(8, 32), (8, 200), (1000, 32), (4099, 8), (513, 200), (37, 24)])
-def test_one_bce_head_is_bit_identical_to_bce_head_fwd_bwd(device, M, K):
-    """One BCE head with loss weight 1 through mm_heads_fwd_bwd and through mm_bce_head_fwd_bwd.  Per row (logits, dx) the
-    two run the same instructions: bit-identical.  The sums (loss, dw, db) are per-block partial sums added with fp32
-    atomics in whatever order the blocks finish, so two runs of the SAME entry point already differ in the last bits once
-    there are several blocks; with M <= 8 there is one block, one atomic per element, and they are bit-identical too."""
-    g = torch.Generator().manual_seed(M + K)
-    x = torch.randn((M, K), generator=g).clamp_min(0).to(device)
-    w = torch.randn(K, generator=g).to(device)
-    b = torch.randn(1, generator=g).to(device)
-    y = (torch.rand(M, generator=g) < 0.3).to(torch.int64).to(device)
-    out = []
-    for fn in ("bce", "heads"):
-        loss = torch.zeros(2, device=device)
-        dx = torch.zeros((M, K), device=device)
-        dw = torch.zeros(K, device=device)
-        db = torch.zeros(1, device=device)
-        lg = torch.zeros(M, device=device)
-        if fn == "bce":
-            ops.bce_head_fwd_bwd(x, w, b, y, loss[:1], dx, dw, db, logits=lg)
-        else:
-            ops.heads_fwd_bwd(x, w.view(K, 1), b, ["binary_crossentropy"], [y], lg.view(1, M), loss, dx, dw.view(K, 1), db)
-        out.append((loss[0].clone(), dx, lg, dw, db))
-    assert torch.equal(out[0][2], out[1][2]) and torch.equal(out[0][1], out[1][1])
-    if M <= 8:
-        for a, b in zip(out[0], out[1]):
-            assert torch.equal(a, b)
-    else:
-        np.testing.assert_allclose(out[0][0].item(), out[1][0].item(), rtol=1e-6)
-        np.testing.assert_allclose(out[0][3].cpu().numpy(), out[1][3].cpu().numpy(), rtol=1e-5, atol=1e-9)
-        np.testing.assert_allclose(out[0][4].cpu().numpy(), out[1][4].cpu().numpy(), rtol=1e-5, atol=1e-9)
-
-
 @pytest.mark.parametrize("H_", [1, 2, 8])
 @pytest.mark.parametrize("widths", [(128, 64, 32), (64, 16), (128, 64, 32, 8)])
 def test_mlp_tc_heads_matches_float64(device, H_, widths):

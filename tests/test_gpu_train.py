@@ -77,7 +77,8 @@ def test_dense_dgrad_rejects_wide_layers(device):
 
 @pytest.mark.parametrize("M,K", [(1, 32), (1000, 32), (4099, 8), (513, 200), (37, 24), (100, 128), (65, 64), (9, 16)])
 @pytest.mark.parametrize("tdtype", [torch.int64, torch.float32])
-def test_bce_head_forward_backward(device, M, K, tdtype):
+def test_one_bce_head_forward_backward(device, M, K, tdtype):
+    """BinaryOutput's Dense(1) + BCE as the training step runs it: heads_fwd_bwd with H = 1, against float64 autograd."""
     g = torch.Generator().manual_seed(M + K)
     x = torch.randn((M, K), generator=g).clamp_min(0.0).to(device)
     w = (torch.randn(K, generator=g) * 0.5).to(device)
@@ -85,12 +86,13 @@ def test_bce_head_forward_backward(device, M, K, tdtype):
     y = torch.randint(0, 2, (M,), generator=g).to(tdtype).to(device)
     sw = (torch.rand(M, generator=g) + 0.5).to(device)
     for weights in (None, sw):
-        loss = torch.zeros(1, device=device)
+        loss = torch.zeros(2, device=device)
         dx = torch.empty((M, K), device=device)
         dw = torch.zeros(K, device=device)
         db = torch.zeros(1, device=device)
         logits = torch.empty(M, device=device)
-        ops.bce_head_fwd_bwd(x, w, b, y, loss, dx, dw, db, mask_relu=True, sample_weight=weights, logits=logits)
+        ops.heads_fwd_bwd(x, w.view(K, 1), b, ["binary_crossentropy"], [y], logits.view(1, M), loss, dx, dw.view(K, 1), db,
+                          mask_relu=True, sample_weight=weights)
         xd = x.double().requires_grad_(True)
         wd = w.double().requires_grad_(True)
         bd = b.double().requires_grad_(True)
@@ -98,7 +100,7 @@ def test_bce_head_forward_backward(device, M, K, tdtype):
         per = torch.nn.functional.binary_cross_entropy_with_logits(z, y.double(), reduction="none")
         ref = (per * (1.0 if weights is None else weights.double())).sum() / M
         ref.backward()
-        np.testing.assert_allclose(loss.item(), ref.item(), rtol=1e-5)
+        np.testing.assert_allclose(loss[0].item(), ref.item(), rtol=1e-5)
         close(logits, z, 1e-5, "logits")
         close(dx, xd.grad * (x > 0), 1e-5, "dx")
         close(dw, wd.grad, 1e-5, "dw")
