@@ -682,6 +682,55 @@ int64_t mm_metrics_workspace_bytes(int64_t M, int H);
 int mm_metrics_update(const float* logits, int64_t M, int H, const mm_metrics_head* heads_host, int num_buckets, int n_sets,
                       double* state, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * K18  Wide&Deep head (WideAndDeepModel, models/ranking.py:276-570; CategoryEncoding, transforms/features.py:473-612).
+ * Added with WideAndDeepModel; no existing entry point changed.  The wide branch is Dense(1) over the concatenated
+ * CategoryEncoding of each wide feature: a block of (int_domain.max + 1) rows of the wide kernel per feature.
+ *   mm_wide_bag: one bag (list) feature of the wide branch.  values (nnz,) ids of idx_bytes (1, 2, 3, 4, 8); offsets
+ *       (B + 1,) of off_dtype (MM_I32 / MM_I64): bag b = positions [offsets[b], offsets[b+1]) clamped to [0, nnz] (an end
+ *       below the start is an empty bag; positions no bag covers are ignored), or offsets null: fixed length, bag b =
+ *       [b length, (b + 1) length) and nnz = B length.  mode MM_WIDE_MULTI_HOT: each distinct id of a bag counts once
+ *       (Keras bincount(binary_output=True)); MM_WIDE_COUNT: every occurrence counts.  Deduplication compares each
+ *       position with the earlier positions of its bag (quadratic in the bag length).  The gradient matches the forward
+ *       when the offsets are non-decreasing; other offsets are never read or written outside their arrays.
+ *   mm_wide_deep_head_fwd_bwd  one pass over the batch:
+ *       wide = sum over one-hot blocks wide_kernel[offset + id] + sum over bags (by mode) wide_kernel[offset + id] + *wide_bias
+ *       u = h . w_dl + *b_dl;  s = wide + act_dl(u);  z = s *out_w + *out_b
+ *       h null: no deep part (s = wide); no blocks: no wide part (s = act_dl(u) + *wide_bias).
+ *     targets null: forward only, out (B,) = out_act(z); loss_kind, ds, dh and the gradients are not read.
+ *     otherwise out (B,) = z, delta = dloss/dz as mm_heads_fwd_bwd (BCE sw (sigmoid(z) - y) / B | MSE sw 2 (z - y) / B),
+ *       ds (B,) = delta *out_w, du = ds act_dl'(u), dh (B, units) = du w_dl (zeroed where h <= 0 when mask_h);
+ *       ACCUMULATES loss (2,) += [loss, loss], *dw_out += sum delta s, *db_out += sum delta, dw_dl (units,) += sum du h,
+ *       *db_dl += sum du, *d_wide_bias += sum ds (each nullable).
+ *     Ids outside [0, rows) add nothing and bump *oob_count.  out_w / out_b / wide_bias / b_dl: DEVICE scalars (nullable
+ *     but out_w).  units <= 512; act_dl linear or relu; <= 64 one-hot blocks and <= 32 bags.
+ *   mm_wide_bag_grad  one bag feature's gradient as nnz pairs: out_ids[i] = values[i] and out_values[i] = ds[bag(i)] for
+ *       every position that adds a term in the forward (MM_WIDE_COUNT: every in-range id; MM_WIDE_MULTI_HOT: the first
+ *       occurrence of each id in its bag), out_ids[i] = -1 and out_values[i] = 0 for repeated occurrences, ids outside
+ *       [0, rows) and positions no bag covers.  Passed to mm_wide_rows_apply as one block of B = nnz samples with int64
+ *       ids (idx_bytes 8), the block's rows / offset and grad = out_values.
+ * ------------------------------------------------------------------------------------- */
+#define MM_WIDE_MULTI_HOT 0
+#define MM_WIDE_COUNT 1
+typedef struct {
+  const void* values;  /* (nnz,) ids, idx_bytes each */
+  const void* offsets; /* (B + 1,) or null: fixed length */
+  int64_t rows;
+  int64_t offset;      /* first row of the block in the wide kernel */
+  int64_t nnz;
+  int32_t idx_bytes;
+  int32_t off_dtype;
+  int32_t length;      /* ids per sample when offsets is null */
+  int32_t mode;        /* MM_WIDE_MULTI_HOT / MM_WIDE_COUNT */
+} mm_wide_bag;
+int mm_wide_deep_head_fwd_bwd(const mm_wide_block* onehot_host, int n_onehot, const mm_wide_bag* bags_host, int n_bags,
+                              const float* wide_kernel, const float* wide_bias, const float* h, int64_t h_stride, int units,
+                              int mask_h, const float* w_dl, const float* b_dl, int act_dl, const float* out_w, const float* out_b,
+                              int out_act, int loss_kind, const void* targets, int target_dtype, const float* sample_weight,
+                              int64_t B, float* out, float* loss, float* ds, float* dh, int64_t dh_stride, float* dw_out,
+                              float* db_out, float* dw_dl, float* db_dl, float* d_wide_bias, int32_t* oob_count, void* stream);
+int mm_wide_bag_grad(const mm_wide_bag* bag_host, int64_t B, const float* ds, int64_t* out_ids, float* out_values, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

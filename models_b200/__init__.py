@@ -15,12 +15,12 @@ from .inputs import (ContinuousFeatures, EmbeddingOptions, Embeddings, Embedding
                      InputBlockV2, infer_embedding_dim)
 from .blocks import (CrossBlock, DLRMBlock, DotProductInteraction, MLPBlock, dense_engine,  # noqa: F401
                      set_dense_engine)
-from .blocks import BatchNormalization, FMBlock, FMPairwiseInteraction  # noqa: F401
+from .blocks import BatchNormalization, CategoryEncoding, FMBlock, FMPairwiseInteraction, HashedCross, HashedCrossAll  # noqa: F401
 from .retrieval import (CategoricalOutput, ContrastiveOutput, Encoder, InBatchSampler, InBatchSamplerV2,  # noqa: F401
                         ItemRetrievalScorer, ItemRetrievalTask, L2Norm, PopularityBasedSamplerV2, TwoTowerBlock,
                         log_uniform_sampling_probs)
 from .models import (BinaryClassificationTask, BinaryOutput, DCNModel, DeepFMModel, DLRMModel, Model, OutputBlock,  # noqa: F401
-                     ParallelOutputs, RegressionOutput,
+                     ParallelOutputs, RegressionOutput, WideAndDeepModel,
                      RetrievalModel, RetrievalModelV2, TwoTowerModel, TwoTowerModelV2)
 from .topk import (AvgPrecisionAt, BruteForce, MRRAt, NDCGAt, PrecisionAt, RecallAt, TopKEncoder,  # noqa: F401
                    TopKIndexBlock, TopKPrediction, encode_candidates, unique_rows_by_features)

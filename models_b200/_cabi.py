@@ -77,6 +77,23 @@ class WideBlock(C.Structure):
     ]
 
 
+class WideBag(C.Structure):
+    """mm_wide_bag (include/mm_b200.h)."""
+
+    _fields_ = [
+        ("values", C.c_void_p),
+        ("offsets", C.c_void_p),
+        ("rows", C.c_int64),
+        ("offset", C.c_int64),
+        ("nnz", C.c_int64),
+        ("idx_bytes", C.c_int32),
+        ("off_dtype", C.c_int32),
+        ("length", C.c_int32),
+        ("mode", C.c_int32),
+    ]
+
+
+WIDE_MODES = {"multi_hot": 0, "count": 1}  # MM_WIDE_MULTI_HOT / MM_WIDE_COUNT
 OPTIMIZERS = {"sgd": 0, "adagrad": 1, "adam": 2}
 LOSS_KINDS = {"binary_crossentropy": 0, "mse": 1}  # MM_LOSS_BCE / MM_LOSS_MSE
 HYPER_LR, HYPER_BETA1, HYPER_BETA2, HYPER_EPS, HYPER_STEP, HYPER_LR_T, HYPER_COUNT = 0, 1, 2, 3, 4, 5, 8
@@ -203,6 +220,9 @@ SIGNATURES = {
     "mm_wide_rows_apply": (_i, [_vp, _vp, _vp, _i64, C.POINTER(WideBlock), _i, _i64, _vp, _vp, _vp, C.POINTER(C.c_int64), _i, _vp,
                                 _vp, _vp, _vp, _i, _vp, _vp]),
     "mm_metrics_workspace_bytes": (_i64, [_i64, _i]),
+    "mm_wide_deep_head_fwd_bwd": (_i, [C.POINTER(WideBlock), _i, C.POINTER(WideBag), _i, _vp, _vp, _vp, _i64, _i, _i, _vp, _vp, _i, _vp,
+                                       _vp, _i, _i, _vp, _i, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "mm_wide_bag_grad": (_i, [C.POINTER(WideBag), _i64, _vp, _vp, _vp, _vp]),
     "mm_metrics_update": (_i, [_vp, _i64, _i, C.POINTER(MetricsHead), _i, _i, _vp, _vp, _i64, _vp]),
 }
 

@@ -601,6 +601,114 @@ def FMBlock(schema: Schema, fm_input_block=None, wide_input_block=None, wide_log
     return FM(schema, emb)
 
 
+_ENCODING_MODES = ("one_hot", "multi_hot", "count")
+
+
+class CategoryEncoding(Block):
+    """transforms/features.py:473-612: each CATEGORICAL column of `schema` encoded as a (B, int_domain.max + 1) vector —
+    "one_hot" (the input must squeeze to one id per sample), "multi_hot" (1 at every distinct id of the sample's list) or
+    "count" (the number of occurrences of each id).  Other columns produce no output.  Here the encoding is never
+    materialized: the wide branch of WideAndDeepModel multiplies it with its Dense(1) kernel inside the head kernel
+    (ops.wide_deep_head_fwd_bwd), as a sum of kernel rows.  `sparse` selects a SparseTensor output in the reference and
+    changes nothing here."""
+
+    def __init__(self, schema: Schema = None, output_mode: str = "one_hot", sparse: bool = False, count_weights=None,
+                 name: Optional[str] = None, **kwargs):
+        super().__init__(name or unique_name("category_encoding"))
+        if output_mode not in _ENCODING_MODES:
+            raise ValueError(f"CategoryEncoding: output_mode must be one of {list(_ENCODING_MODES)}, got {output_mode!r}")
+        if count_weights is not None:
+            if output_mode != "count":
+                raise ValueError("`count_weights` is not used when `output_mode` is not `'count'`. "
+                                 f"Received `count_weights={count_weights}`.")
+            raise NotImplementedError("CategoryEncoding(count_weights=...): weighted counts are not implemented")
+        self.schema = schema.select_by_tag(Tags.CATEGORICAL) if schema is not None else Schema([])
+        self.output_mode, self.sparse = output_mode, sparse
+        self.cardinalities: Dict[str, int] = {c.name: int(c.int_domain.max) + 1 for c in self.schema}
+
+    def call(self, inputs, **kwargs):
+        raise NotImplementedError("CategoryEncoding runs fused into WideAndDeepModel's wide Dense(1) (the encoded vectors "
+                                  "are never built); pass it as `wide_preprocess`")
+
+
+class WideLinear(Block):
+    """The wide branch of WideAndDeepModel (models/ranking.py:504-535): Dense(1) with bias over the concatenation, in
+    sorted-name order (ConcatFeatures), of each encoded wide feature.  The Keras kernel is (sum_f cardinality_f, 1): one
+    block of rows per feature (`offsets`), and the product with an encoding is a sum of kernel rows.  A feature fed as a
+    list ((B, L) ids or ragged `__values` / `__offsets`) takes the encoding's mode; a one-hot encoding accepts one id per
+    sample only.  A uint8 (B, 3) matrix is the package's packed 24-bit id of one sample (graph.HostBatch) for a column the
+    schema does not mark as a list; for a list column it is ambiguous (the deep input block would read packed ids) and is
+    refused: pass such a list's ids as uint16 / int32 / int64."""
+
+    def __init__(self, encoding: CategoryEncoding, exclude: Sequence[str] = (), name: Optional[str] = None):
+        super().__init__(name or unique_name("wide"))
+        self.encoding = encoding
+        # this branch's own copy: the encoding the caller passed in is not modified (another model may share it)
+        self.cardinalities: Dict[str, int] = {n: c for n, c in encoding.cardinalities.items() if n not in set(exclude)}
+        self.lists = {c.name for c in encoding.schema if c.is_list and c.name in self.cardinalities}
+        self.names = sorted(self.cardinalities)
+        if not self.names:
+            raise ValueError("the wide branch needs categorical features")
+        self.offsets: Dict[str, int] = {}
+        off = 0
+        for n in self.names:
+            self.offsets[n] = off
+            off += self.cardinalities[n]
+        self.width = off
+        self.dense = _Dense(1, activation="linear", use_bias=True, name=f"{self.name}/wide_logit")
+        # holds no table: the out-of-range id counter this branch shares with the model's embedding tables
+        self.ids = EmbeddingsBlock({}, encoding.schema, name=f"{self.name}/ids")
+
+    @property
+    def mode(self) -> str:
+        return self.encoding.output_mode
+
+    def build(self, device=None):
+        self.dense.build(self.width, device)
+        self.built = True
+        return self
+
+    def weights(self):
+        return dict(self.dense.weights())
+
+    def blocks(self, inputs: TabularData):
+        """(one-hot blocks [(ids, rows, offset)], bag blocks [(values, offsets, rows, offset, mode)]) of this batch."""
+        from .core import get_feature
+
+        onehot, bags = [], []
+        mode = "multi_hot" if self.mode == "one_hot" else self.mode
+        for n in self.names:
+            x = get_feature(inputs, n)
+            rows, off = self.cardinalities[n], self.offsets[n]
+            if n in self.lists and not isinstance(x, tuple) and x.dtype == torch.uint8 and x.dim() == 2 and x.shape[1] == 3:
+                raise ValueError(f"list feature {n!r}: a uint8 (B, 3) id matrix reads as packed 24-bit ids; pass the list's ids "
+                                 "as uint16, int32 or int64")
+            if isinstance(x, tuple):
+                if self.mode == "one_hot":
+                    raise ValueError(f"{n!r}: One-hot accepts input tensors that are squeezable to 1D, but received a ragged list")
+                bags.append((ops.as_index(x[0]).reshape(-1), ops.as_index(x[1]).reshape(-1), rows, off, mode))
+            elif (x.dtype == torch.uint8 and x.dim() == 2 and x.shape[1] == 3) or x.dim() == 1 or (x.dim() == 2 and x.shape[1] == 1):
+                onehot.append((ops.fused_ids(x), rows, off))
+            elif x.dim() == 2 or (x.dim() == 3 and x.shape[2] == 1):
+                if self.mode == "one_hot":
+                    raise ValueError("One-hot accepts input tensors that are squeezable to 1D, but received a tensor with shape: "
+                                     f"{tuple(x.shape)}")
+                bags.append((ops.as_index(x).reshape(x.shape[0], -1).contiguous(), None, rows, off, mode))
+            else:
+                raise ValueError(f"{n!r}: unsupported categorical input shape {tuple(x.shape)}")
+        return onehot, bags
+
+
+def HashedCross(*args, **kwargs):
+    """transforms/features.py HashedCross: crosses hashed with TF's FarmHash; not implemented."""
+    raise NotImplementedError("HashedCross is not implemented: its feature crosses are hashed with TensorFlow's FarmHash")
+
+
+def HashedCrossAll(*args, **kwargs):
+    """transforms/features.py HashedCrossAll: crosses hashed with TF's FarmHash; not implemented."""
+    raise NotImplementedError("HashedCrossAll is not implemented: its feature crosses are hashed with TensorFlow's FarmHash")
+
+
 _INTERACTION_TYPES = (None, "field_all", "field_each", "field_interaction")
 
 

@@ -13,8 +13,8 @@ import numpy as np
 import torch
 
 from . import ops
-from .blocks import (FM, MLP, CrossBlock, CrossBlockSeq, DLRM, DLRMBlock, FMBlock, MLPBlock, _Dense, dense_engine,
-                     run_dense_chain)
+from .blocks import (FM, MLP, CategoryEncoding, CrossBlock, CrossBlockSeq, DLRM, DLRMBlock, FMBlock, MLPBlock, WideLinear, _Dense,
+                     dense_engine, run_dense_chain)
 from .core import Block, Prediction, TabularData, batch_size_of, default_device, to_device, unique_name
 from .inputs import EmbeddingOptions, EmbeddingsBlock, InputBlockV2
 from .retrieval import ItemRetrievalTask, TwoTowerBlock
@@ -784,6 +784,8 @@ class RankingModel(Model):
             return chain(x, layers)
         if isinstance(self.body, DeepFMBody):
             return self.body.forward(inputs, out_layer=self.prediction.to_call, logits=logits)
+        if isinstance(self.body, WideAndDeepBody):
+            return self.body.forward(inputs, out_layer=self.prediction.to_call, logits=logits)
         if isinstance(self.body, DCNBody) and self.body.stacked:
             x = self.body.cross(self.body.input_block(inputs))
             layers, tail = self.body.deep.chain(extra)
@@ -918,6 +920,150 @@ def DeepFMModel(schema: Schema, embedding_dim: Optional[int] = None, deep_block:
     if isinstance(prediction, ParallelOutputs):
         raise NotImplementedError("DeepFMModel with several outputs is not implemented: pass one BinaryOutput")
     return RankingModel(DeepFMBody(input_block, fm, deep_block, deep_logit_block), prediction, schema)
+
+
+class WideAndDeepBody(Block):
+    """ParallelBlock({"deep": input_block -> deep_block -> MLPBlock([1]), "wide": CategoryEncoding -> Dense(1)},
+    "element-wise-sum") (models/ranking.py:504-570): (B, 1).  The deep tower's hidden layers are the usual dense chain;
+    the deep logit's Dense(1), the wide Dense(1) over the encoded wide features, the sum and (from RankingModel) the output
+    layer are ONE kernel (ops.wide_deep_head_fwd_bwd).  Either branch may be absent (input_block / wide None)."""
+
+    def __init__(self, input_block: Optional[InputBlockV2], deep: Optional[MLP], deep_logit: Optional[MLP], wide: Optional[WideLinear],
+                 regularized: bool = False):
+        super().__init__(unique_name("wide_and_deep_body"))
+        self.input_block, self.deep, self.deep_logit, self.wide = input_block, deep, deep_logit, wide
+        self.regularized = regularized  # a deep / wide regularizer was given (it only changes training)
+        if deep is not None:
+            if deep.has_normalization:
+                raise NotImplementedError("WideAndDeepModel: normalization inside deep_block is not implemented")
+            if deep.dense_layers[-1].units > 512:
+                raise NotImplementedError(f"WideAndDeepModel: the head kernel reads at most 512 units of the deep block's last "
+                                          f"layer, got {deep.dense_layers[-1].units}")
+
+    def build(self, device=None):
+        if self.input_block is not None:
+            self.input_block.build(device)
+            _, _, d = self.input_block.layout()
+            self.deep.build_from_width(d, device)
+            self.deep_logit.build_from_width(self.deep.dense_layers[-1].units, device)
+        if self.wide is not None:
+            self.wide.build(device)
+        self.built = True
+        return self
+
+    def output_width(self) -> int:
+        return 1
+
+    def weights(self):
+        out = {}
+        if self.input_block is not None:
+            out.update({f"input/{k}": v for k, v in self.input_block.weights().items()})
+            out.update({f"deep/{k}": v for k, v in self.deep.weights().items()})
+            out.update({f"deep_logit/{k}": v for k, v in self.deep_logit.weights().items()})
+        if self.wide is not None:
+            out.update({f"wide/{k}": v for k, v in self.wide.weights().items()})
+        return out
+
+    def oob_counter(self, device):
+        """The out-of-range id counter of the model's tables and wide features (one shared counter) and its owner; (None,
+        None) for a model without ids (a deep branch over continuous columns only and no wide branch)."""
+        if self.input_block is not None and self.input_block.embeddings is not None:
+            owner = self.input_block.embeddings
+        elif self.wide is not None:
+            owner = self.wide.ids
+        else:
+            return None, None
+        return owner.counter(device), owner
+
+    def forward(self, inputs: TabularData, out_layer: _Dense, logits: bool = False) -> torch.Tensor:
+        dev = next(iter(inputs.values())).device
+        if not self.built:
+            self.build(dev)
+        B = batch_size_of(inputs)
+        h = dl = None
+        if self.input_block is not None:
+            h = run_dense_chain(self.input_block(inputs), self.deep.dense_layers)
+            dl = self.deep_logit.dense_layers[-1]
+        onehot, bags = self.wide.blocks(inputs) if self.wide is not None else ([], [])
+        wd = self.wide.dense if self.wide is not None else None
+        out_layer.build(1, dev)
+        out = torch.empty((B, 1), dtype=torch.float32, device=dev)
+        oob, owner = self.oob_counter(dev)
+        ops.wide_deep_head_fwd_bwd(onehot, bags, None if wd is None else wd.kernel.reshape(-1), None if wd is None else wd.bias, h, False,
+                                   None if dl is None else dl.kernel.reshape(-1), None if dl is None else dl.bias,
+                                   "linear" if dl is None else dl.activation, out_layer.kernel.reshape(-1), out_layer.bias,
+                                   out.reshape(-1), out_act="linear" if logits else out_layer.activation, oob=oob)
+        if owner is not None:
+            owner.finish_check(oob)
+        return out
+
+    def call(self, inputs: TabularData, **kwargs) -> torch.Tensor:
+        raise NotImplementedError("WideAndDeepBody runs inside its RankingModel (the output layer is fused into its head)")
+
+
+def WideAndDeepModel(schema: Schema, deep_block: Optional[MLP] = None, wide_schema: Optional[Schema] = None,
+                     deep_schema: Optional[Schema] = None, wide_preprocess=None, deep_input_block: Optional[InputBlockV2] = None,
+                     wide_input_block=None, deep_regularizer=None, wide_regularizer=None, deep_dropout: Optional[float] = None,
+                     wide_dropout: Optional[float] = None, prediction_tasks=None, pre=None, **wide_body_kwargs) -> RankingModel:
+    """models/ranking.py:276-570: Dense(1)(deep(x)) + Dense(1)(CategoryEncoding(wide features)), then the prediction task.
+
+    deep   deep_input_block, default InputBlockV2(deep_schema, categorical=Embeddings(categorical part of deep_schema,
+           sequence_combiner="mean")) at inferred widths, deep_schema defaulting to schema; then deep_block and
+           MLPBlock([1], no_activation_last_layer=True).  No deep part when deep_block is None or deep_schema has no
+           input features (the reference needs a deep_block).
+    wide   wide_preprocess (a CategoryEncoding; default CategoryEncoding(wide_schema, output_mode="one_hot")) over the
+           categorical columns of wide_schema in sorted-name order, then Dense(1) with bias.  Continuous columns of
+           wide_schema add nothing (CategoryEncoding emits categorical columns only).  No wide_schema: pure deep, with the
+           reference's warning.
+    A list feature given ragged (`__values` / `__offsets`) contributes only its own ids to the wide term; the reference
+    pads it to a dense (B, L) matrix with id 0 first (ToDense).  Dropout is the identity in the forward; regularizers do
+    not change the forward."""
+    import warnings
+
+    if pre is not None:
+        raise NotImplementedError("WideAndDeepModel(pre=...) is not implemented")
+    if wide_input_block is not None:
+        raise NotImplementedError("WideAndDeepModel: a custom wide_input_block is not implemented (pass wide_schema and a "
+                                  "CategoryEncoding as wide_preprocess)")
+    if wide_body_kwargs:
+        raise NotImplementedError(f"WideAndDeepModel: options {sorted(wide_body_kwargs)} of the wide Dense are not implemented")
+    prediction = parse_prediction_blocks(schema, prediction_tasks)
+    if isinstance(prediction, ParallelOutputs):
+        raise NotImplementedError("WideAndDeepModel with several outputs is not implemented: pass one BinaryOutput or RegressionOutput")
+    if not wide_schema:
+        warnings.warn("If not specify wide_schema, NO feature would be sent to wide model")
+    if not deep_schema:
+        deep_schema = schema
+    deep = deep_logit = None
+    if deep_block is not None:
+        if deep_input_block is None:
+            feats = deep_schema.excluding_by_tag(Tags.TARGET)
+            if len(feats):
+                from .inputs import Embeddings
+
+                cat = feats.select_by_tag(Tags.CATEGORICAL)
+                deep_input_block = InputBlockV2(feats, categorical=Embeddings(cat, sequence_combiner="mean")) if len(cat) else InputBlockV2(feats)
+        if deep_input_block is not None:
+            deep = deep_block
+            deep_logit = MLPBlock([1], no_activation_last_layer=True, dropout=deep_dropout)
+    else:
+        deep_input_block = None
+    wide = None
+    if wide_schema is not None and len(wide_schema) > 0:
+        enc = wide_preprocess if wide_preprocess is not None else CategoryEncoding(wide_schema, output_mode="one_hot", sparse=True)
+        if isinstance(enc, (tuple, list)) and len(enc) == 1:
+            enc = enc[0]
+        if not isinstance(enc, CategoryEncoding):
+            raise NotImplementedError(f"WideAndDeepModel: wide_preprocess {type(enc).__name__} is not implemented (CategoryEncoding only)")
+        outside = [n for n in enc.cardinalities if n not in wide_schema.column_names]
+        if outside:
+            raise ValueError(f"wide_preprocess encodes {outside}, which are not in wide_schema")
+        wide = WideLinear(enc, exclude=wide_schema.select_by_tag(Tags.TARGET).column_names)
+        wide.dropout = wide_dropout
+    if deep is None and wide is None:
+        raise ValueError("At least the deep part (deep_schema/deep_input_block) or wide part (wide_schema/wide_input_block) must be provided.")
+    body = WideAndDeepBody(deep_input_block, deep, deep_logit, wide, regularized=deep_regularizer is not None or wide_regularizer is not None)
+    return RankingModel(body, prediction, schema)
 
 
 def DCNModel(schema: Schema, depth: int, deep_block: Optional[MLP] = None, stacked: bool = True,

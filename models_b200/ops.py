@@ -1334,3 +1334,113 @@ def metrics_update(z: torch.Tensor, losses: Sequence[str], targets: Sequence[tor
     _cabi.check(_lib().mm_metrics_update(z.data_ptr(), M, H, arr, T, len(sets), state.data_ptr(), workspace.data_ptr(),
                                          workspace.numel() * workspace.element_size(), _stream()), "mm_metrics_update")
     return state
+
+
+# ---- Wide&Deep head (include/mm_b200.h K18) -------------------------------------------------------------------------
+_BAG_ID_BYTES = {torch.uint8: 1, torch.uint16: 2, torch.int32: 4, torch.int64: 8}
+
+
+def _wide_bags(bags, B: int):
+    """mm_wide_bag array of bag blocks (values, offsets, rows, offset, mode): values (nnz,) ids with offsets (B + 1,)
+    int32 / int64, or a (B, L) id matrix with offsets None; ids uint8 / uint16 / int32 / int64; mode "multi_hot" or
+    "count"."""
+    arr = (_cabi.WideBag * max(len(bags), 1))()
+    for i, (values, offsets, rows, offset, mode) in enumerate(bags):
+        v = _dev(values, f"bags[{i}].values")
+        if v.dtype not in _BAG_ID_BYTES or not v.is_contiguous():
+            raise ValueError(f"bags[{i}].values must be contiguous uint8 / uint16 / int32 / int64 ids, got {v.dtype}")
+        if mode not in _cabi.WIDE_MODES:
+            raise ValueError(f"bags[{i}]: mode must be one of {sorted(_cabi.WIDE_MODES)}, got {mode!r}")
+        if offsets is None:
+            if v.dim() != 2 or v.shape[0] != B:
+                raise ValueError(f"bags[{i}]: fixed-length ids must be a (B={B}, L) matrix, got {tuple(v.shape)}")
+            arr[i].length, arr[i].offsets, arr[i].off_dtype = v.shape[1], None, MM_I32
+        else:
+            o = _dev(offsets, f"bags[{i}].offsets")
+            if o.numel() != B + 1 or not o.is_contiguous():
+                raise ValueError(f"bags[{i}].offsets must be contiguous with B+1={B + 1} elements, got {tuple(o.shape)}")
+            arr[i].length, arr[i].offsets, arr[i].off_dtype = 0, o.data_ptr(), _idx_dtype(o, f"bags[{i}].offsets")
+        arr[i].values, arr[i].nnz, arr[i].idx_bytes = v.data_ptr(), v.numel(), _BAG_ID_BYTES[v.dtype]
+        arr[i].rows, arr[i].offset, arr[i].mode = int(rows), int(offset), _cabi.WIDE_MODES[mode]
+    return arr, len(bags)
+
+
+def wide_deep_head_fwd_bwd(onehot, bags, wide_kernel: Optional[torch.Tensor], wide_bias: Optional[torch.Tensor],
+                           h: Optional[torch.Tensor], mask_h: bool, w_dl: Optional[torch.Tensor], b_dl: Optional[torch.Tensor],
+                           act_dl: str, out_w: torch.Tensor, out_b: Optional[torch.Tensor], out: torch.Tensor,
+                           out_act: Optional[str] = "linear", loss: Optional[str] = None, targets: Optional[torch.Tensor] = None,
+                           sample_weight: Optional[torch.Tensor] = None, loss_buf: Optional[torch.Tensor] = None,
+                           ds: Optional[torch.Tensor] = None, dh: Optional[torch.Tensor] = None,
+                           dw_out: Optional[torch.Tensor] = None, db_out: Optional[torch.Tensor] = None,
+                           dw_dl: Optional[torch.Tensor] = None, db_dl: Optional[torch.Tensor] = None,
+                           d_wide_bias: Optional[torch.Tensor] = None, oob: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The Wide&Deep head in one pass (mm_wide_deep_head_fwd_bwd).  onehot: (ids (B,) of any width of index_bytes_of, rows,
+    offset) per one-hot wide feature; bags: see _wide_bags; h (B, U) the deep tower's last hidden layer and w_dl (U,) /
+    b_dl the deep logit's Dense(1), or h None for a model without a deep part.  targets None: out (B,) = out_act(z).
+    Otherwise out = z, ds (B,) and dh (B, U) are written and loss_buf (2,) and the gradients (each nullable) ACCUMULATED."""
+    _dev(out, "out", torch.float32), _dev(out_w, "out_w", torch.float32)
+    B = out.numel()
+    if not out.is_contiguous():
+        raise ValueError("out must be contiguous")
+    if wide_kernel is not None and (not _dev(wide_kernel, "wide_kernel", torch.float32).is_contiguous()):
+        raise ValueError("wide_kernel must be contiguous")
+    for n_, t_ in (("out_w", out_w), ("out_b", out_b), ("b_dl", b_dl), ("wide_bias", wide_bias), ("dw_out", dw_out),
+                   ("db_out", db_out), ("db_dl", db_dl), ("d_wide_bias", d_wide_bias)):
+        _vec(t_, 1, n_, "hold {n} contiguous float32 values")
+    U, hs, dhs = 0, 0, 0
+    if h is not None:
+        _dev(h, "h", torch.float32)
+        U = h.shape[1]
+        hs = _row_stride(h, "h")
+        if h.shape[0] != B or w_dl is None:
+            raise ValueError(f"h must be ({B}, units) with the deep logit's kernel w_dl")
+        _vec(w_dl, U, "w_dl", "hold {n} contiguous float32 values")
+        _vec(dw_dl, U, "dw_dl", "hold {n} contiguous float32 values")
+        if act_dl not in ("linear", "relu"):
+            raise ValueError(f"the deep logit's activation must be linear or relu, got {act_dl!r}")
+    target_dtype = 0
+    if targets is not None:
+        if loss not in _cabi.LOSS_KINDS:
+            raise ValueError(f"loss must be among {sorted(_cabi.LOSS_KINDS)}, got {loss!r}")
+        target_dtype = _target(targets, B, "targets")
+        _vec(sample_weight, B, "sample_weight", _SAMPLE_WEIGHT)
+        _vec(ds, B, "ds", "hold {n} contiguous float32 values")
+        if ds is None:
+            raise ValueError("training needs ds")
+        if loss_buf is not None and (_dev(loss_buf, "loss_buf", torch.float32).numel() != 2 or not loss_buf.is_contiguous()):
+            raise ValueError("loss_buf must hold 2 contiguous values")
+        if h is not None:
+            if dh is None or tuple(_dev(dh, "dh", torch.float32).shape) != (B, U):
+                raise ValueError(f"training with a deep part needs dh ({B}, {U})")
+            dhs = _row_stride(dh, "dh")
+    n_oh = len(onehot)
+    oh = (_cabi.WideBlock * max(n_oh, 1))()
+    for i, (ix, rows, off) in enumerate(onehot):
+        oh[i].idx_bytes = _id_column(ix, B, f"onehot[{i}]", leading=True)
+        oh[i].indices, oh[i].rows, oh[i].offset = ix.data_ptr(), int(rows), int(off)
+    barr, n_bag = _wide_bags(bags, B)
+    train = targets is not None
+    _cabi.check(
+        _lib().mm_wide_deep_head_fwd_bwd(oh, n_oh, barr, n_bag, _ptr(wide_kernel), _ptr(wide_bias), _ptr(h), hs, U, 1 if mask_h else 0,
+                                         _ptr(w_dl), _ptr(b_dl), ACTIVATIONS[act_dl], out_w.data_ptr(), _ptr(out_b),
+                                         ACTIVATIONS[out_act], _cabi.LOSS_KINDS[loss] if train else 0, _ptr(targets), target_dtype,
+                                         _ptr(sample_weight) if train else None, B, out.data_ptr(), _ptr(loss_buf) if train else None,
+                                         _ptr(ds) if train else None, _ptr(dh) if train else None, dhs,
+                                         *[_ptr(t) if train else None for t in (dw_out, db_out, dw_dl, db_dl, d_wide_bias)], _ptr(oob),
+                                         _stream()),
+        "mm_wide_deep_head_fwd_bwd")
+    return out
+
+
+def wide_bag_grad(bag, B: int, ds: torch.Tensor, out_ids: torch.Tensor, out_values: torch.Tensor) -> None:
+    """One bag block's gradient as nnz (id, value) pairs for wide_rows_apply (mm_wide_bag_grad): out_ids (nnz,) int64, -1
+    where no term of the forward sits; out_values (nnz,) fp32."""
+    _dev(ds, "ds", torch.float32)
+    if ds.numel() < B or not ds.is_contiguous():
+        raise ValueError(f"ds must hold {B} contiguous values")
+    arr, _ = _wide_bags([bag], B)
+    nnz = arr[0].nnz
+    if _dev(out_ids, "out_ids", torch.int64).numel() != nnz or not out_ids.is_contiguous():
+        raise ValueError(f"out_ids must hold {nnz} contiguous int64 values")
+    _vec(out_values, nnz, "out_values", "hold {n} contiguous float32 values")
+    _cabi.check(_lib().mm_wide_bag_grad(arr, B, ds.data_ptr(), out_ids.data_ptr(), out_values.data_ptr(), _stream()), "mm_wide_bag_grad")

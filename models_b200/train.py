@@ -1327,10 +1327,212 @@ class DeepFMTrainer(_StepTrainer):
         self.wk_grad.zero_()
 
 
+class WideAndDeepTrainer(_StepTrainer):
+    """Static-buffer training step of a WideAndDeepModel (one BinaryOutput or RegressionOutput) at one batch size.
+
+    forward   the deep input block as DCN's (one-hot features gathered, multi-hot features pooled by their combiner) into x0
+              and its split operand; mm_dense_tc per deep layer
+    head      mm_wide_deep_head_fwd_bwd: the wide term over the one-hot and bag features, the deep logit's Dense(1), the
+              sum, the output layer and the loss, forward and backward: logits, ds = dloss/ds (B,), dh and the gradients of
+              the deep logit, the output layer (arena) and the wide bias; mm_wide_bag_grad per wide bag feature
+    backward  mm_dense_wgrad[_split] + dgrad per deep layer down to dx0; mm_concat_backward into each table's IndexedSlices
+              buffer, mm_bag_grad_rows for multi-hot deep features
+    update    mm_opt_tick, mm_dense_apply over the arena [deep, deep logit, output layer], mm_sparse_rows_apply (tables),
+              mm_wide_rows_apply over the wide kernel's one-hot blocks (gradient values ds, with the bias) and once per wide
+              bag feature (its nnz expanded pairs), mm_split_weights refresh of the operand copies the model's forward reads.
+    The wide kernel stays where it is, its optimizer slots beside it.  Fixed-length list features can be captured into one
+    CUDA graph; ragged ones train eagerly (their number of ids changes from batch to batch)."""
+
+    def __init__(self, model, optimizer: Optimizer, batch_size: int, device=None, group=None):
+        from .blocks import dense_engine
+        from .models import BinaryOutput, WideAndDeepBody
+
+        body = model.body
+        if not isinstance(body, WideAndDeepBody):
+            raise NotImplementedError("WideAndDeepTrainer trains WideAndDeepModel bodies")
+        if not isinstance(model.prediction, BinaryOutput):
+            raise NotImplementedError("training WideAndDeepModel needs one BinaryOutput or RegressionOutput")
+        if group is not None:
+            raise NotImplementedError("training WideAndDeepModel with a process group is not implemented")
+        if dense_engine() == "fp32":
+            raise NotImplementedError("training WideAndDeepModel runs on the tensor-core engine (dense_engine() == 'fp32')")
+        if body.regularized:
+            raise NotImplementedError("training WideAndDeepModel with deep / wide regularizers is not implemented")
+        if body.wide is not None and getattr(body.wide, "dropout", None):
+            raise NotImplementedError("training WideAndDeepModel with wide_dropout is not implemented")
+        ib = body.input_block
+        self.deep = ib is not None
+        if self.deep:
+            if getattr(ib.embeddings, "sharded", None) is not None:
+                raise NotImplementedError("training WideAndDeepModel with row-sharded tables is not implemented")
+            for blk in (body.deep, body.deep_logit):
+                if not isinstance(blk, MLP) or blk.has_normalization or blk.dropout:
+                    raise NotImplementedError("training WideAndDeepModel supports a deep_block without normalization / dropout "
+                                              "(and no deep_dropout)")
+        self._init_common(model, optimizer, batch_size, device, None)
+        self._init_heads()
+        f32 = dict(dtype=torch.float32, device=self.device)
+        B = self.B
+        self.chain, self.last = [], None
+        feats, tables = [], []
+        if self.deep:
+            self.chain = body.deep.dense_layers  # run by mm_dense_tc
+            self.last = body.deep_logit.dense_layers[-1]  # Dense(1), fused into the head kernel
+            for l in self.chain + [self.last]:
+                if l.activation not in ("relu", "linear"):
+                    raise NotImplementedError(f"{l.name}: training supports relu / linear deep activations, got {l.activation!r}")
+            self.cols, _, self.d = ib.layout()
+            emb = ib.embeddings
+            feats = list(emb.feature_names) if emb is not None else []
+            tables = [emb.feature_to_table[f] for f in feats]
+            for f, t in zip(feats, tables):
+                col = model.schema.get(f)
+                if col is not None and col.is_list and t.dim not in (16, 32, 64, 128):
+                    raise NotImplementedError(f"feature {f!r}: training a multi-hot deep feature needs an embedding width of 16, "
+                                              f"32, 64 or 128, got {t.dim} (pass deep_input_block with Embeddings(dim=...))")
+            self.cont = sorted(ib.continuous.features) if ib.continuous is not None else []
+        self._init_tables(feats, tables)
+        self._init_dense(self.chain + ([self.last] if self.deep else []), [self.head])
+        n = len(self.chain)
+        self._init_wide(lambda li: li < n)
+        if self.deep:
+            self.ld = _ld4(self.d)
+            self.x0 = torch.zeros((B, self.ld), **f32)
+            self.xs = torch.zeros((B, 2 * ops.tc_padded_k(self.d)), dtype=torch.bfloat16, device=self.device)
+            self.h, self.h_split, self.dh = self._chain_buffers(self.chain)
+            self.dx0 = torch.zeros((B, self.ld), **f32)
+            self.slices = [torch.zeros((B, t.table.shape[1]), **f32) for t in self.tables]
+        # ---- the wide kernel (W, 1) and its bias, outside the arena
+        self.wl = body.wide
+        self.ds = torch.zeros(B, **f32)
+        if self.wl is not None:
+            self.wk = self.wl.dense
+            W = self.wk.kernel.numel()
+            slots = optimizer.slots
+            self.wk_s1 = torch.full((W,), optimizer.initial_accumulator_value, **f32) if slots >= 1 else None
+            self.wk_s2 = torch.zeros(W, **f32) if slots >= 2 else None
+            self.wb_s1 = torch.full((1,), optimizer.initial_accumulator_value, **f32) if slots >= 1 else None
+            self.wb_s2 = torch.zeros(1, **f32) if slots >= 2 else None
+            self.wk_acc = torch.zeros(W, **f32)
+            self.wk_rep = ops.fill_i32(torch.empty(W, dtype=torch.int32, device=self.device), INT32_MAX)
+            self.wk_grad = torch.zeros(1, **f32)  # the bias' gradient
+            self._wbag_bufs: Dict[int, dict] = {}
+        self._init_loss(B)
+        self.oob = body.oob_counter(self.device)[0]
+
+    def forward_backward(self, inputs: Dict[str, torch.Tensor], targets, sample_weight=None) -> None:
+        """Forward (activations saved), loss and backward: fills the gradient arena, the tables' IndexedSlices, ds and the
+        expanded (id, value) pairs of the wide bag features, and the wide bias' gradient.  Batches smaller than the
+        compiled size run in the leading rows of the same buffers."""
+        a = self.arena
+        n = len(self.chain)
+        self._loss_all.zero_()
+        b = batch_size_of(inputs)
+        targets = self._check_targets(targets, b)
+        if isinstance(sample_weight, (list, tuple)):
+            sample_weight = sample_weight[0]
+        tidx = range(len(self.tables))
+        self._idx: List[Optional[torch.Tensor]] = [None] * len(self.tables)
+        self._slices: List[torch.Tensor] = []  # no tables without a deep part
+        self._bags = {}
+        h = dh = None
+        if self.deep:
+            self._slices = [s[:b] for s in self.slices]
+            x0, xs = self.x0[:b, :self.d], self.xs[:b]
+            self._input_forward(self.feats, tidx, self.cols, self.cont, inputs, x0, xs)
+            h, dh = [t[:b] for t in self.h], [t[:b] for t in self.dh]
+            self._chain_forward(xs, self.d, 0, self.chain, h, [t[:b] for t in self.h_split])
+        onehot, bags = self.wl.blocks(inputs) if self.wl is not None else ([], [])
+        ds = self.ds[:b]
+        hi = len(a.layers) - 1
+        wk = self.wk if self.wl is not None else None
+        ops.wide_deep_head_fwd_bwd(
+            onehot, bags, None if wk is None else wk.kernel.reshape(-1), None if wk is None else wk.bias, None if h is None else h[-1],
+            self.deep and self.chain[-1].activation == "relu", None if not self.deep else self.last.kernel.reshape(-1),
+            None if not self.deep else self.last.bias, "linear" if not self.deep else self.last.activation, self.head.kernel.reshape(-1),
+            self.head.bias, self.logits[:b], loss=self.losses[0], targets=targets[0].reshape(-1), sample_weight=sample_weight,
+            loss_buf=self._loss_all, ds=ds, dh=None if dh is None else dh[-1], dw_out=a.view(a.grad, hi, "kernel"),
+            db_out=a.view(a.grad, hi, "bias"), dw_dl=a.view(a.grad, n, "kernel") if self.deep else None,
+            db_dl=a.view(a.grad, n, "bias") if self.deep else None, d_wide_bias=None if wk is None else self.wk_grad, oob=self.oob)
+        self._wpairs = []
+        for q, bag in enumerate(bags):  # each wide bag feature's gradient as (id, value) pairs
+            nnz = bag[0].numel()
+            buf = self._wbag_bufs.setdefault(q, dict(ids=None, vals=None))
+            if buf["ids"] is None or buf["ids"].shape[0] < nnz:
+                if torch.cuda.is_current_stream_capturing():
+                    raise RuntimeError("the wide bag gradient buffers cannot grow during graph capture")
+                buf["ids"] = torch.empty(max(nnz, 1), dtype=torch.int64, device=self.device)
+                buf["vals"] = torch.empty(max(nnz, 1), dtype=torch.float32, device=self.device)
+            ids, vals = buf["ids"][:nnz], buf["vals"][:nnz]
+            ops.wide_bag_grad(bag, b, ds, ids, vals)
+            self._wpairs.append((ids, vals, bag[2], bag[3]))
+        if self.deep:
+            dx0 = self.dx0[:b, :self.d] if self.tables else None
+            self._chain_backward(0, self.chain, h, dh, (xs, self.d), dx0)
+            if self.tables:
+                self._input_backward([dx0], self.feats, tidx, self.cols)
+                self._bag_grads()
+        self._onehot, self._b = onehot, b
+
+    def _apply_more(self) -> None:
+        if self.wl is None:
+            return
+        wk, first = self.wk.kernel.reshape(-1), True
+        calls = []
+        if self._onehot:
+            calls.append(([i for i, _, _ in self._onehot], [r for _, r, _ in self._onehot], [o for _, _, o in self._onehot], self.ds[:self._b]))
+        calls += [([ids], [rows], [off], vals) for ids, vals, rows, off in self._wpairs]
+        for ids, rows, offs, g in calls:  # the bias takes its step with the first call
+            ops.wide_rows_apply(self.opt.kind, wk, self.wk_s1, self.wk_s2, ids, rows, offs, g, self.wk_acc, self.wk_rep, [],
+                                self.wk_grad if first else None, self.wk.bias.reshape(-1) if first else None,
+                                self.wb_s1 if first else None, self.wb_s2 if first else None, self.hyper)
+            first = False
+
+    def wide_gradients(self) -> Dict[str, torch.Tensor]:
+        """The wide kernel's gradient (W, 1) and its bias' (after forward_backward, before apply_gradients), assembled in
+        float64 from ds, the one-hot ids and the bag features' expanded pairs — for parity tests."""
+        W = self.wk.kernel.numel()
+        g = torch.zeros(W, dtype=torch.float64, device=self.device)
+        ds = self.ds[:self._b].double()
+        for ids, rows, off in self._onehot:
+            i = ops.widen_index(ids).reshape(-1).long()
+            ok = (i >= 0) & (i < rows)
+            g.index_add_(0, i[ok] + off, ds[ok])
+        for ids, vals, rows, off in self._wpairs:
+            ok = ids >= 0
+            g.index_add_(0, ids[ok] + off, vals[ok].double())
+        return {"wide/kernel": g.reshape(W, 1), "wide/bias": self.wk_grad.double().clone()}
+
+    def capture(self, inputs: Dict[str, torch.Tensor], targets: torch.Tensor, clone: bool = True) -> None:
+        for f in (self.wl.names if self.wl is not None else []):
+            if isinstance(get_feature(inputs, f), tuple):
+                raise NotImplementedError(f"graph capture with the ragged wide feature {f!r} is not implemented: its number of ids "
+                                          "changes from batch to batch (train it eagerly, or feed it as a fixed-length (B, L) matrix)")
+        super().capture(inputs, targets, clone)
+
+    def _snapshot(self):
+        snap = super()._snapshot()
+        if self.wl is not None:
+            snap.update(wk=self.wk.kernel.clone(), wb=self.wk.bias.clone(),
+                        wk_s=[None if s is None else s.clone() for s in (self.wk_s1, self.wk_s2, self.wb_s1, self.wb_s2)])
+        return snap
+
+    def _restore(self, snap) -> None:
+        super()._restore(snap)
+        if self.wl is None:
+            return
+        self.wk.kernel.copy_(snap["wk"])
+        self.wk.bias.copy_(snap["wb"])
+        for dst, src in zip((self.wk_s1, self.wk_s2, self.wb_s1, self.wb_s2), snap["wk_s"]):
+            if src is not None:
+                dst.copy_(src)
+        self.wk_grad.zero_()
+
+
 def trainer_for(model, optimizer: Optimizer, batch_size: int, group=None):
-    """The training engine of `model`: DLRMTrainer, DCNTrainer or DeepFMTrainer by the ranking body, TwoTowerTrainer for a
-    RetrievalModel."""
-    from .models import DCNBody, DeepFMBody, RetrievalModel, RetrievalModelV2
+    """The training engine of `model`: DLRMTrainer, DCNTrainer, DeepFMTrainer or WideAndDeepTrainer by the ranking body,
+    TwoTowerTrainer for a RetrievalModel."""
+    from .models import DCNBody, DeepFMBody, RetrievalModel, RetrievalModelV2, WideAndDeepBody
 
     if isinstance(model, RetrievalModelV2):
         raise NotImplementedError("training TwoTowerModelV2 / ContrastiveOutput is not implemented: train the v1 TwoTowerModel")
@@ -1340,4 +1542,6 @@ def trainer_for(model, optimizer: Optimizer, batch_size: int, group=None):
         return DCNTrainer(model, optimizer, batch_size, group=group)
     if isinstance(getattr(model, "body", None), DeepFMBody):
         return DeepFMTrainer(model, optimizer, batch_size, group=group)
+    if isinstance(getattr(model, "body", None), WideAndDeepBody):
+        return WideAndDeepTrainer(model, optimizer, batch_size, group=group)
     return DLRMTrainer(model, optimizer, batch_size, group=group)
