@@ -731,6 +731,50 @@ int mm_wide_deep_head_fwd_bwd(const mm_wide_block* onehot_host, int n_onehot, co
                               float* db_out, float* dw_dl, float* db_dl, float* d_wide_bias, int32_t* oob_count, void* stream);
 int mm_wide_bag_grad(const mm_wide_bag* bag_host, int64_t B, const float* ds, int64_t* out_ids, float* out_values, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * K19  MMoE gates, expert mixture and output heads (MMOEBlock, blocks/experts.py:37-208; OutputBlock, outputs/block.py).
+ * Added with MMOEBlock; no existing entry point changed.
+ *   mm_mmoe_heads_fwd_bwd  one pass over the batch.  x (B, E U): the E experts' last-layer outputs side by side (expert e
+ *       at columns [e U, (e + 1) U)); gate_logits_host[t] (B, E) with row stride gate_strides_host[t]: task t's gate logits
+ *       (host arrays of H device pointers / strides).  w (U, H) Keras layout, bias (H,) nullable; losses, loss weights,
+ *       targets, sample weights and the loss vector as mm_heads_fwd_bwd.
+ *       p_t = softmax(L_t / temperature),  m_t = sum_e p_t,e x_e,  z_t = m_t . w[:, t] + bias[t]   (m_t is never stored)
+ *     targets null: forward only, logits (H, B) = the activated predictions (mm_heads_fwd_bwd's sigmoid form, or z for MSE);
+ *       loss_weight, dx, the gate-logit gradients and dw / db are not read.
+ *     otherwise logits (H, B) = z, delta_t = dloss/dz_t as mm_heads_fwd_bwd, dm_t = delta_t w[:, t];
+ *       dx (B, E U) = sum_t p_t,e dm_t (zeroed where x <= 0 when mask_relu), d_gate_logits_host[t] (B, E) =
+ *       p_t (dg_t - <p_t, dg_t>) / temperature with dg_t,e = <dm_t, x_e>; ACCUMULATES loss (1 + H), dw (U, H) += m_t delta_t,
+ *       db (H,) += delta_t (dw / db nullable).
+ *     E <= 16, U <= 256, 1 <= H <= 8, temperature > 0.
+ * ------------------------------------------------------------------------------------- */
+int mm_mmoe_heads_fwd_bwd(const float* x, int64_t B, int E, int U, int64_t x_stride, const float* const* gate_logits_host,
+                          const int64_t* gate_strides_host, int H, float temperature, const float* w, const float* bias,
+                          const int* loss_kind, const float* loss_weight, const void* const* targets, const int* target_dtypes,
+                          const float* const* sample_weights, float* logits, float* loss, float* dx, int64_t dx_stride,
+                          int mask_relu, float* const* d_gate_logits_host, const int64_t* d_gate_strides_host, float* dw,
+                          float* db, void* stream);
+/* The task-tower path: the gates and mixture alone, then H heads with one input per task.
+ *   mm_mmoe_mix_fwd  p (B, H E) = the gate weights softmax(L_t / temperature) side by side (saved for the backward);
+ *       m (H, B, U) contiguous: m[t] = sum_e p_t,e x_e; m_split (H, B, 2 Kp) nullable: m[t]'s split-bf16 operand
+ *       (mm_split_rows layout, Kp = mm_tc_padded_k(U), padding written as zeros).
+ *   mm_mmoe_mix_bwd  from dm (H, B, U): dx (B, E U) = sum_t p_t,e dm_t (zeroed where x <= 0 when mask_relu) and
+ *       d_gate_logits_host[t] (B, E) = p_t (dg_t - <p_t, dg_t>) / temperature with dg_t,e = <dm_t, x_e>.
+ *   mm_mmoe_task_heads_fwd_bwd  head t reads x_host[t] (B, K) (row stride x_strides_host[t]): z_t = x_t . w[:, t] + bias[t],
+ *       w (K, H); losses, targets, sample weights, the loss vector, dw / db (accumulated) and the forward-only form as
+ *       mm_heads_fwd_bwd; training writes dx_host[t] (B, K) = delta_t w[:, t] (zeroed where x_t <= 0 when mask_relu).
+ *     E <= 16, U <= 256, K <= 256, 1 <= H <= 8, temperature > 0. */
+int mm_mmoe_mix_fwd(const float* x, int64_t B, int E, int U, int64_t x_stride, const float* const* gate_logits_host,
+                    const int64_t* gate_strides_host, int H, float temperature, float* p, float* m, void* m_split, int Kp,
+                    void* stream);
+int mm_mmoe_mix_bwd(const float* x, int64_t B, int E, int U, int64_t x_stride, const float* p, int H, float temperature,
+                    const float* dm, float* dx, int64_t dx_stride, int mask_relu, float* const* d_gate_logits_host,
+                    const int64_t* d_gate_strides_host, void* stream);
+int mm_mmoe_task_heads_fwd_bwd(const float* const* x_host, const int64_t* x_strides_host, int64_t B, int K, int H, const float* w,
+                               const float* bias, const int* loss_kind, const float* loss_weight, const void* const* targets,
+                               const int* target_dtypes, const float* const* sample_weights, float* logits, float* loss,
+                               float* const* dx_host, const int64_t* dx_strides_host, int mask_relu, float* dw, float* db,
+                               void* stream);
+
 #ifdef __cplusplus
 }
 #endif

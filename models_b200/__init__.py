@@ -16,6 +16,7 @@ from .inputs import (ContinuousFeatures, EmbeddingOptions, Embeddings, Embedding
 from .blocks import (CrossBlock, DLRMBlock, DotProductInteraction, MLPBlock, dense_engine,  # noqa: F401
                      set_dense_engine)
 from .blocks import BatchNormalization, CategoryEncoding, FMBlock, FMPairwiseInteraction, HashedCross, HashedCrossAll  # noqa: F401
+from .experts import CGCBlock, MMOEBlock, PLEBlock  # noqa: F401
 from .retrieval import (CategoricalOutput, ContrastiveOutput, Encoder, InBatchSampler, InBatchSamplerV2,  # noqa: F401
                         ItemRetrievalScorer, ItemRetrievalTask, L2Norm, PopularityBasedSamplerV2, TwoTowerBlock,
                         log_uniform_sampling_probs)

@@ -224,6 +224,16 @@ SIGNATURES = {
                                        _vp, _i, _i, _vp, _i, _vp, _i64, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "mm_wide_bag_grad": (_i, [C.POINTER(WideBag), _i64, _vp, _vp, _vp, _vp]),
     "mm_metrics_update": (_i, [_vp, _i64, _i, C.POINTER(MetricsHead), _i, _i, _vp, _vp, _i64, _vp]),
+    "mm_mmoe_heads_fwd_bwd": (_i, [_vp, _i64, _i, _i, _i64, C.POINTER(C.c_void_p), C.POINTER(C.c_int64), _i, _f, _vp, _vp,
+                                   C.POINTER(C.c_int), C.POINTER(C.c_float), C.POINTER(C.c_void_p), C.POINTER(C.c_int),
+                                   C.POINTER(C.c_void_p), _vp, _vp, _vp, _i64, _i, C.POINTER(C.c_void_p), C.POINTER(C.c_int64),
+                                   _vp, _vp, _vp]),
+    "mm_mmoe_mix_fwd": (_i, [_vp, _i64, _i, _i, _i64, C.POINTER(C.c_void_p), C.POINTER(C.c_int64), _i, _f, _vp, _vp, _vp, _i, _vp]),
+    "mm_mmoe_mix_bwd": (_i, [_vp, _i64, _i, _i, _i64, _vp, _i, _f, _vp, _vp, _i64, _i, C.POINTER(C.c_void_p), C.POINTER(C.c_int64),
+                             _vp]),
+    "mm_mmoe_task_heads_fwd_bwd": (_i, [C.POINTER(C.c_void_p), C.POINTER(C.c_int64), _i64, _i, _i, _vp, _vp, C.POINTER(C.c_int),
+                                        C.POINTER(C.c_float), C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_void_p),
+                                        _vp, _vp, C.POINTER(C.c_void_p), C.POINTER(C.c_int64), _i, _vp, _vp, _vp]),
 }
 
 

@@ -32,13 +32,22 @@ class BinaryOutput(Block):
         self.target = tname
         self.to_call = _Dense(1, activation=self.activation, name=f"{self.name}/dense")
 
+    task_blocks = None  # {name: tower} when OutputBlock(task_blocks=...) gave this output a tower
+
     def build(self, width: Optional[int] = None, device=None):
+        if self.task_blocks and width is not None:
+            tower = self.task_blocks[self.name]
+            tower.build_from_width(width, device)
+            width = tower.dense_layers[-1].units
         self.to_call.build(width, device)
         self.built = True
         return self
 
     def weights(self):
-        return {f"dense/{k}": v for k, v in self.to_call.weights().items()}
+        out = {f"dense/{k}": v for k, v in self.to_call.weights().items()}
+        if self.task_blocks:
+            out.update({f"task_block/{k}": v for k, v in self.task_blocks[self.name].weights().items()})
+        return out
 
     def call(self, inputs: torch.Tensor, logits: bool = False, **kwargs) -> torch.Tensor:
         return self.to_call(inputs, activation="linear" if logits else None)
@@ -81,6 +90,7 @@ class ParallelOutputs(Block):
             raise NotImplementedError(f"2..8 outputs are supported, got {len(outs)}")
         self.outputs = sorted(outs, key=lambda o: o.name)
         self.to_call = _Dense(len(outs), activation="linear", name=f"{self.name}/dense")
+        self.task_blocks: Optional[Dict[str, MLP]] = None  # {output name: tower} (OutputBlock(task_blocks=...))
 
     @property
     def names(self) -> List[str]:
@@ -95,6 +105,10 @@ class ParallelOutputs(Block):
         return [o.activation for o in self.outputs]
 
     def build(self, width: Optional[int] = None, device=None):
+        if self.task_blocks and width is not None and self.to_call.kernel is None:
+            for o in self.outputs:
+                self.task_blocks[o.name].build_from_width(width, device)
+            width = self.task_blocks[self.outputs[0].name].dense_layers[-1].units
         if width is not None and width > 256:  # mm_heads_fwd_bwd / mm_mlp_tc_heads read the body vector from registers
             raise NotImplementedError(f"{self.name}: several outputs need a body output of at most 256 units, got {width}")
         if self.to_call.kernel is None:
@@ -116,6 +130,8 @@ class ParallelOutputs(Block):
         for h, o in enumerate(self.outputs):
             out[f"{o.name}/dense/kernel"] = self.to_call.kernel[:, h:h + 1]
             out[f"{o.name}/dense/bias"] = self.to_call.bias[h:h + 1]
+            if self.task_blocks:
+                out.update({f"{o.name}/task_block/{k}": v for k, v in self.task_blocks[o.name].weights().items()})
         return out
 
     def split(self, stacked: torch.Tensor) -> Dict[str, torch.Tensor]:
@@ -137,10 +153,13 @@ class ParallelOutputs(Block):
         return self.split(self.stacked_forward(inputs, out, logits=logits))
 
 
-def OutputBlock(schema: Schema, model_outputs=None) -> Block:
+def OutputBlock(schema: Schema, model_outputs=None, task_blocks=None) -> Block:
     """outputs/block.py:32-131: one BinaryOutput / RegressionOutput per target column of the schema (continuous /
     regression-tagged targets first, then binary ones; a categorical target with int_domain.max == 1 is binary).  One target:
-    that output itself; several: ParallelOutputs.  `model_outputs` (list or dict by name) replaces the outputs it names."""
+    that output itself; several: ParallelOutputs.  `model_outputs` (list or dict by name) replaces the outputs it names.
+    `task_blocks` (outputs/block.py:133-190): one MLPBlock cloned for every output, or a dict keyed by output name or target
+    column; output t then reads Dense(1)(task_block_t(body)).  The towers must end in the same width (the outputs' heads stay
+    one stacked (K, H) Dense)."""
     targets = schema.select_by_tag(Tags.TARGET)
     if not len(targets):
         raise ValueError("No targets found in schema. Please tag your targets or provide them as branches.")
@@ -173,9 +192,49 @@ def OutputBlock(schema: Schema, model_outputs=None) -> Block:
         name = f"{col.name}/{cls.suffix}"
         if name not in outputs:
             outputs[name] = cls(col.name)
-    if len(outputs) == 1:
-        return next(iter(outputs.values()))
-    return ParallelOutputs(list(outputs.values()))
+    out = next(iter(outputs.values())) if len(outputs) == 1 else ParallelOutputs(list(outputs.values()))
+    if task_blocks is not None:
+        _attach_towers(out, task_blocks)
+    return out
+
+
+def _attach_towers(out: Block, task_blocks) -> None:
+    """out.task_blocks = {output name: its tower} from task_blocks (a Layer cloned per output, or a dict by output name or
+    target column)."""
+    outs = out.outputs if isinstance(out, ParallelOutputs) else [out]
+    towers = {}
+    for o in outs:
+        if isinstance(task_blocks, dict):
+            blk = task_blocks.get(o.name, task_blocks.get(o.target))
+            if blk is None:
+                continue
+        else:
+            blk = task_blocks.copy()  # an independent copy per output
+        if not isinstance(blk, MLP) or blk.has_normalization:
+            raise NotImplementedError(f"task block of {o.name!r}: MLPBlock towers without normalization are implemented, got "
+                                      f"{type(blk).__name__}")
+        towers[o.name] = blk
+    if isinstance(task_blocks, dict):
+        unknown = sorted(set(task_blocks) - {o.name for o in outs} - {o.target for o in outs})
+        if unknown:
+            raise ValueError(f"task_blocks names unknown outputs / targets {unknown}")
+    if towers and len(towers) != len(outs):
+        raise NotImplementedError("OutputBlock(task_blocks=...): every output needs a tower (the heads read towers of one width)")
+    widths = {t.dense_layers[-1].units for t in towers.values()}
+    if len(widths) > 1:
+        raise NotImplementedError(f"OutputBlock(task_blocks=...): the towers must end in the same width, got {sorted(widths)}")
+    if widths and widths.pop() > 256:
+        raise NotImplementedError("OutputBlock(task_blocks=...): a tower's last layer must be at most 256 wide")
+    out.task_blocks = towers or None
+
+
+def output_towers(prediction: Block) -> Optional[List[MLP]]:
+    """The output towers of an output block in output order, or None."""
+    towers = getattr(prediction, "task_blocks", None)
+    if not towers:
+        return None
+    outs = prediction.outputs if isinstance(prediction, ParallelOutputs) else [prediction]
+    return [towers[o.name] for o in outs]
 
 
 def parse_prediction_blocks(schema: Schema, prediction_blocks=None) -> Block:
@@ -195,6 +254,10 @@ def parse_prediction_blocks(schema: Schema, prediction_blocks=None) -> Block:
                 return OutputBlock(schema)
             return BinaryOutput(binary[0])
         return BinaryOutput(targets.first.name)
+    for b in (prediction_blocks if isinstance(prediction_blocks, (list, tuple)) else [prediction_blocks]):
+        if getattr(b, "task_blocks", None):
+            raise NotImplementedError("per-task towers (OutputBlock(task_blocks=...)) are implemented for the sequential "
+                                      "Model(InputBlockV2, ..., output) only")
     if isinstance(prediction_blocks, (list, tuple)):
         if len(prediction_blocks) > 1:
             return ParallelOutputs(prediction_blocks)
@@ -251,9 +314,56 @@ def expected_input_columns(schema: Schema) -> List[str]:
     return cols
 
 
-class Model(Block):
+def _is_sequential(args, kwargs) -> bool:
+    """Model(*blocks) (the reference's form) rather than Model(body, prediction, schema): no Schema argument and an
+    InputBlockV2 first."""
+    return (not kwargs and len(args) >= 2 and isinstance(args[0], InputBlockV2)
+            and not any(isinstance(a, Schema) for a in args))
+
+
+def _sequential_model(*blocks) -> "RankingModel":
+    """Model(InputBlockV2, [MLPBlock], [MMOEBlock], output): the concatenating input block, optionally one MLPBlock as a
+    shared bottom, optionally one MMOEBlock, then a BinaryOutput / RegressionOutput or the result of OutputBlock."""
+    from .blocks import MLP
+    from .experts import MMOEBlock
+
+    ib, mid, out = blocks[0], list(blocks[1:-1]), blocks[-1]
+    order = "Model(*blocks) takes InputBlockV2, then optionally one MLPBlock, then optionally one MMOEBlock, then the output"
+    if ib.aggregation != "concat":
+        raise NotImplementedError("Model(*blocks): the input block must concatenate its features (aggregation='concat')")
+    if not isinstance(out, (BinaryOutput, ParallelOutputs)):
+        raise NotImplementedError(f"{order} (BinaryOutput, RegressionOutput or OutputBlock(schema)); got {type(out).__name__} last")
+    bottom = mmoe = None
+    for blk in mid:
+        if isinstance(blk, MLP) and bottom is None and mmoe is None:
+            bottom = blk
+        elif isinstance(blk, MMOEBlock) and mmoe is None:
+            mmoe = blk
+        else:
+            raise NotImplementedError(f"{order}; got {[type(b).__name__ for b in blocks]}")
+    if bottom is None and mmoe is None and not getattr(out, "task_blocks", None):
+        raise NotImplementedError(f"{order}: an MLPBlock, an MMOEBlock or task towers are needed between the input and the output")
+    if mmoe is not None:
+        mmoe.bind(out.names if isinstance(out, ParallelOutputs) else [out.name])
+    return RankingModel(MMoEBody(ib, bottom, mmoe), out, ib.schema)
+
+
+class _ModelMeta(type):
+    """`Model(*blocks)` (the reference's sequential form) builds through _sequential_model; every other call constructs the
+    class as usual, so `Model(body, prediction, schema)` keeps its exact signature."""
+
+    def __call__(cls, *args, **kwargs):
+        if cls is Model and _is_sequential(args, kwargs):
+            return _sequential_model(*args)
+        return super().__call__(*args, **kwargs)
+
+
+class Model(Block, metaclass=_ModelMeta):
     """models/base.py:1621-2245: model(inputs, targets=None, training=False, testing=False) with `inputs` a dict keyed by
-    schema column names; `compile(optimizer)` / `fit` / `train_step` for the DLRM path (models_b200/train.py)."""
+    schema column names; `compile(optimizer)` / `fit` / `train_step` for the DLRM path (models_b200/train.py).
+
+    `Model(body, prediction, schema)` wraps a body and its prediction block; `Model(InputBlockV2, *blocks)` (no schema
+    argument) is the reference's sequential form and returns a RankingModel (_sequential_model)."""
 
     def __init__(self, body: Block, prediction: Block, schema: Schema):
         super().__init__(unique_name("model"))
@@ -751,7 +861,7 @@ class RankingModel(Model):
             from .graph import _stacked_outputs
 
             return _stacked_outputs(out), PRED_HEAD if _LAST_HEADS[0] == "heads" else PRED_ACT
-        return out.reshape(1, -1), PRED_ACT
+        return out.reshape(1, -1), PRED_HEAD if _LAST_HEADS[0] == "heads" else PRED_ACT
 
     def _forward(self, inputs: TabularData, training: bool = False, logits: bool = False):
         self._check_inputs(inputs)
@@ -786,6 +896,15 @@ class RankingModel(Model):
             return self.body.forward(inputs, out_layer=self.prediction.to_call, logits=logits)
         if isinstance(self.body, WideAndDeepBody):
             return self.body.forward(inputs, out_layer=self.prediction.to_call, logits=logits)
+        if isinstance(self.body, MMoEBody) and (self.body.mmoe is not None or output_towers(self.prediction)):
+            out = self.body.forward(inputs, self.output_blocks(), self.prediction.to_call, output_towers(self.prediction),
+                                    logits=logits)
+            return heads.split(out) if heads is not None else out.view(-1, 1)
+        if isinstance(self.body, MMoEBody):
+            x = self.body.input_block(inputs)
+            layers, tail = self.body.bottom.chain(extra)
+            assert tail is None
+            return chain(x, layers)
         if isinstance(self.body, DCNBody) and self.body.stacked:
             x = self.body.cross(self.body.input_block(inputs))
             layers, tail = self.body.deep.chain(extra)
@@ -793,6 +912,87 @@ class RankingModel(Model):
             return chain(x, layers)
         x = self.body(inputs, training=training)
         return self.prediction(x, logits=True) if logits else self.prediction(x)
+
+
+class MMoEBody(Block):
+    """The body of Model(InputBlockV2, [MLPBlock], [MMOEBlock], output): input block -> shared bottom -> experts and gates.
+    Without an MMOEBlock the output heads read the bottom's output as in the other ranking models; with one, the gates,
+    the mixture and the heads are one kernel (ops.mmoe_heads_fwd_bwd) after the stacked expert and gate layers."""
+
+    def __init__(self, input_block: InputBlockV2, bottom: Optional[MLP], mmoe):
+        super().__init__(unique_name("mmoe_body"))
+        self.input_block, self.bottom, self.mmoe = input_block, bottom, mmoe
+        if bottom is not None and bottom.has_normalization and mmoe is not None:
+            raise NotImplementedError("Model(*blocks): normalization in the shared bottom before an MMOEBlock is not implemented")
+
+    def input_width(self) -> int:
+        """Width of what the experts and gates (or the heads) read."""
+        return self.bottom.dense_layers[-1].units if self.bottom is not None else self.input_block.layout()[2]
+
+    def build(self, device=None):
+        self.input_block.build(device)
+        _, _, d = self.input_block.layout()
+        if self.bottom is not None:
+            self.bottom.build_from_width(d, device)
+        if self.mmoe is not None:
+            self.mmoe.build(self.input_width(), device)
+        self.built = True
+        return self
+
+    def output_width(self) -> int:
+        return self.mmoe.units if self.mmoe is not None else self.input_width()
+
+    def weights(self):
+        out = {f"input/{k}": v for k, v in self.input_block.weights().items()}
+        if self.bottom is not None:
+            out.update({f"bottom/{k}": v for k, v in self.bottom.weights().items()})
+        if self.mmoe is not None:
+            out.update({f"mmoe/{k}": v for k, v in self.mmoe.weights().items()})
+        return out
+
+    def forward(self, inputs: TabularData, outputs: Sequence[Block], head: _Dense, towers: Optional[List[MLP]],
+                logits: bool = False) -> torch.Tensor:
+        """(H, B): the activated predictions of the outputs, or their logits with logits=True (each head run as a linear
+        regression head, as ParallelOutputs.stacked_forward does).  Without towers the gates, the mixture and the heads are
+        mm_mmoe_heads_fwd_bwd; with towers mm_mmoe_mix_fwd, one tower chain per output and mm_mmoe_task_heads_fwd_bwd."""
+        from .blocks import _LAST_HEADS
+
+        if not self.built:
+            self.build(next(iter(inputs.values())).device)
+        mo = self.mmoe
+        x = self.input_block(inputs)
+        if self.bottom is not None:
+            x = run_dense_chain(x, self.bottom.dense_layers)
+        B, K = x.shape
+        H = len(outputs)
+        dev = x.device
+        out = torch.empty((H, B), dtype=torch.float32, device=dev)
+        losses = ["mse"] * H if logits else [o.loss for o in outputs]
+        _LAST_HEADS[0] = "heads"
+        if mo is None:  # towers on the shared vector
+            ts = [run_dense_chain(x, t.dense_layers) for t in towers]
+            return ops.mmoe_task_heads_fwd_bwd(ts, head.kernel, head.bias, losses, None, out)
+        xs = ops.split_rows(x)
+        X = torch.empty((B, mo.experts.units), dtype=torch.float32, device=dev)
+        ops.dense_tc(xs, K, mo.experts.split_kernel(), mo.experts.units, mo.experts.bias, mo.experts.activation, out_f32=X)
+        if mo.gates is not None:
+            L = torch.empty((B, mo.gates.units), dtype=torch.float32, device=dev)
+            ops.dense_tc(xs, K, mo.gates.split_kernel(), mo.gates.units, None, "linear", out_f32=L)
+            gl = mo.gate_logits(L)
+        else:
+            gl = [run_dense_chain(x, mo.gate_chain(t)) for t in range(H)]
+        if towers is None:
+            return ops.mmoe_heads_fwd_bwd(X, mo.num_experts, gl, mo.temperature, head.kernel, head.bias, losses, None, out)
+        U = mo.units
+        m = torch.empty((H, B, U), dtype=torch.float32, device=dev)
+        m_split = torch.empty((H, B, 2 * ops.tc_padded_k(U)), dtype=torch.bfloat16, device=dev)
+        p = torch.empty((B, H * mo.num_experts), dtype=torch.float32, device=dev)
+        ops.mmoe_mix_fwd(X, mo.num_experts, gl, mo.temperature, p, m, m_split)
+        ts = [run_dense_chain(None, t.dense_layers, a_split=m_split[i], K=U) for i, t in enumerate(towers)]
+        return ops.mmoe_task_heads_fwd_bwd(ts, head.kernel, head.bias, losses, None, out)
+
+    def call(self, inputs: TabularData, **kwargs):
+        raise NotImplementedError("MMoEBody runs inside its RankingModel (the output heads are fused with the mixture)")
 
 
 def DLRMModel(schema: Schema, *, embeddings: Optional[EmbeddingsBlock] = None, embedding_dim: Optional[int] = None,

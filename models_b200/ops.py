@@ -888,6 +888,198 @@ def heads_fwd_bwd(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor]
     return out
 
 
+MMOE_MAX_EXPERTS, MMOE_MAX_UNITS, MMOE_MAX_TASKS = 16, 256, 8  # mm_mmoe_heads_fwd_bwd
+
+
+def mmoe_heads_fwd_bwd(x: torch.Tensor, E: int, gate_logits: Sequence[torch.Tensor], temperature: float, w: torch.Tensor,
+                       bias: Optional[torch.Tensor], losses: Sequence[str], targets: Optional[Sequence[torch.Tensor]],
+                       out: torch.Tensor, loss: Optional[torch.Tensor] = None, dx: Optional[torch.Tensor] = None,
+                       d_gate_logits: Optional[Sequence[torch.Tensor]] = None, dw: Optional[torch.Tensor] = None,
+                       db: Optional[torch.Tensor] = None, loss_weights: Optional[Sequence[float]] = None, mask_relu: bool = True,
+                       sample_weight=None) -> torch.Tensor:
+    """H <= 8 tasks, each the soft-max gate of its (M, E) logits gate_logits[t] over the E experts' outputs x (M, E U)
+    followed by its Dense(U -> 1), forward and backward in one pass (mm_mmoe_heads_fwd_bwd).  w (U, H), bias (H,), losses,
+    targets, out, loss, dw, db, loss_weights and sample_weight as heads_fwd_bwd.  Training writes dx (M, E U) and
+    d_gate_logits[t] (M, E)."""
+    _dev(x, "x", torch.float32), _dev(w, "w", torch.float32), _dev(out, "out", torch.float32)
+    M, EU = x.shape
+    H = len(losses)
+    if not (1 <= E <= MMOE_MAX_EXPERTS) or EU % E:
+        raise ValueError(f"x must hold E = {E} experts (1..{MMOE_MAX_EXPERTS}) of equal width, got {EU} columns")
+    U = EU // E
+    if not (1 <= U <= MMOE_MAX_UNITS) or not (1 <= H <= MMOE_MAX_TASKS):
+        raise ValueError(f"expert width {U} must be in 1..{MMOE_MAX_UNITS} and the task count {H} in 1..{MMOE_MAX_TASKS}")
+    if not temperature > 0:
+        raise ValueError(f"the gate temperature must be > 0, got {temperature}")
+    if tuple(w.shape) != (U, H) or not w.is_contiguous():
+        raise ValueError(f"w must be a contiguous ({U}, {H}) matrix")
+    _vec(bias, H, "bias")
+    if tuple(out.shape) != (H, M) or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous ({H}, {M}) matrix")
+    if any(l not in _cabi.LOSS_KINDS for l in losses):
+        raise ValueError(f"losses must be among {sorted(_cabi.LOSS_KINDS)}, got {list(losses)}")
+
+    def gates(ts, name):
+        if len(ts) != H:
+            raise ValueError(f"{name}: one (M, E) matrix per task: {H} expected, got {len(ts)}")
+        for t, g in enumerate(ts):
+            if _dev(g, f"{name}[{t}]", torch.float32).shape != (M, E):
+                raise ValueError(f"{name}[{t}] must be ({M}, {E}), got {tuple(g.shape)}")
+        return ((C.c_void_p * H)(*[g.data_ptr() for g in ts]),
+                (C.c_int64 * H)(*[_row_stride(g, f"{name}[{t}]") for t, g in enumerate(ts)]))
+
+    gp, gs = gates(gate_logits, "gate_logits")
+    kinds = (C.c_int * H)(*[_cabi.LOSS_KINDS[l] for l in losses])
+    tp = dt = sp = lw = dgp = dgs = None
+    dxs = 0
+    if targets is not None:
+        if len(targets) != H:
+            raise ValueError(f"one target tensor per task: {H} expected, got {len(targets)}")
+        dt = (C.c_int * H)(*[_target(t, M, f"targets[{h}]") for h, t in enumerate(targets)])
+        if loss is None or dx is None or d_gate_logits is None:
+            raise ValueError("training needs loss, dx and d_gate_logits")
+        _vec(loss, 1 + H, "loss")
+        if _dev(dx, "dx", torch.float32).shape != (M, EU):
+            raise ValueError(f"dx must be ({M}, {EU})")
+        dxs = _row_stride(dx, "dx")
+        dgp, dgs = gates(d_gate_logits, "d_gate_logits")
+        if dw is not None and (_dev(dw, "dw", torch.float32).shape != (U, H) or not dw.is_contiguous()):
+            raise ValueError(f"dw must be a contiguous ({U}, {H}) matrix")
+        _vec(db, H, "db")
+        sws = list(sample_weight) if isinstance(sample_weight, (list, tuple)) else [sample_weight] * H
+        if len(sws) != H:
+            raise ValueError(f"one sample-weight tensor per task: {H} expected, got {len(sws)}")
+        for h, s in enumerate(sws):
+            _vec(s, M, f"sample_weight[{h}]", _SAMPLE_WEIGHT)
+        lws = [1.0] * H if loss_weights is None else [float(v) for v in loss_weights]
+        if len(lws) != H:
+            raise ValueError(f"one loss weight per task: {H} expected, got {len(lws)}")
+        tp = (C.c_void_p * H)(*[t.data_ptr() for t in targets])
+        sp = (C.c_void_p * H)(*[_ptr(s) for s in sws])
+        lw = (C.c_float * H)(*lws)
+    train = targets is not None
+    _cabi.check(
+        _lib().mm_mmoe_heads_fwd_bwd(x.data_ptr(), M, E, U, _row_stride(x, "x"), gp, gs, H, float(temperature), w.data_ptr(),
+                                     _ptr(bias), kinds, lw, tp, dt, sp, out.data_ptr(), _ptr(loss) if train else None,
+                                     _ptr(dx) if train else None, dxs, 1 if mask_relu else 0, dgp, dgs,
+                                     _ptr(dw) if train else None, _ptr(db) if train else None, _stream()),
+        "mm_mmoe_heads_fwd_bwd")
+    return out
+
+
+def _ptr_array(ts: Sequence[torch.Tensor], name: str, H: int, shape: tuple):
+    """(device pointers, row strides) of H fp32 matrices of the given shape, as the ctypes arrays the K19 calls take."""
+    if len(ts) != H:
+        raise ValueError(f"{name}: one matrix per task: {H} expected, got {len(ts)}")
+    for t, g in enumerate(ts):
+        if tuple(_dev(g, f"{name}[{t}]", torch.float32).shape) != shape:
+            raise ValueError(f"{name}[{t}] must be {shape}, got {tuple(g.shape)}")
+    return ((C.c_void_p * H)(*[g.data_ptr() for g in ts]),
+            (C.c_int64 * H)(*[_row_stride(g, f"{name}[{t}]") for t, g in enumerate(ts)]))
+
+
+def _mixture_shape(x: torch.Tensor, E: int, temperature: float):
+    _dev(x, "x", torch.float32)
+    M, EU = x.shape
+    if not (1 <= E <= MMOE_MAX_EXPERTS) or EU % E or not (1 <= EU // E <= MMOE_MAX_UNITS):
+        raise ValueError(f"x must hold E = {E} experts (1..{MMOE_MAX_EXPERTS}) of 1..{MMOE_MAX_UNITS} units, got {EU} columns")
+    if not temperature > 0:
+        raise ValueError(f"the gate temperature must be > 0, got {temperature}")
+    return M, EU // E
+
+
+def mmoe_mix_fwd(x: torch.Tensor, E: int, gate_logits: Sequence[torch.Tensor], temperature: float, p: torch.Tensor,
+                 m: torch.Tensor, m_split: Optional[torch.Tensor] = None) -> None:
+    """The gates and the mixture alone (mm_mmoe_mix_fwd): p (M, H E) = the gate weights, m (H, M, U) the mixtures, m_split
+    (H, M, 2 Kp) their split-bf16 operands (optional)."""
+    M, U = _mixture_shape(x, E, temperature)
+    H = len(gate_logits)
+    if not 1 <= H <= MMOE_MAX_TASKS:
+        raise ValueError(f"1..{MMOE_MAX_TASKS} tasks, got {H}")
+    gp, gs = _ptr_array(gate_logits, "gate_logits", H, (M, E))
+    if tuple(_dev(p, "p", torch.float32).shape) != (M, H * E) or not p.is_contiguous():
+        raise ValueError(f"p must be a contiguous ({M}, {H * E}) matrix")
+    if tuple(_dev(m, "m", torch.float32).shape) != (H, M, U) or not m.is_contiguous():
+        raise ValueError(f"m must be a contiguous ({H}, {M}, {U}) tensor")
+    Kp = tc_padded_k(U)
+    if m_split is not None and (tuple(_dev(m_split, "m_split", torch.bfloat16).shape) != (H, M, 2 * Kp) or not m_split.is_contiguous()):
+        raise ValueError(f"m_split must be a contiguous bf16 ({H}, {M}, {2 * Kp}) tensor")
+    _cabi.check(_lib().mm_mmoe_mix_fwd(x.data_ptr(), M, E, U, _row_stride(x, "x"), gp, gs, H, float(temperature), p.data_ptr(),
+                                       m.data_ptr(), _ptr(m_split), Kp, _stream()), "mm_mmoe_mix_fwd")
+
+
+def mmoe_mix_bwd(x: torch.Tensor, E: int, p: torch.Tensor, temperature: float, dm: torch.Tensor, dx: torch.Tensor,
+                 d_gate_logits: Sequence[torch.Tensor], mask_relu: bool = True) -> None:
+    """Backward of mmoe_mix_fwd (mm_mmoe_mix_bwd): dm (H, M, U) -> dx (M, E U) and d_gate_logits[t] (M, E)."""
+    M, U = _mixture_shape(x, E, temperature)
+    H = len(d_gate_logits)
+    if not 1 <= H <= MMOE_MAX_TASKS:
+        raise ValueError(f"1..{MMOE_MAX_TASKS} tasks, got {H}")
+    dgp, dgs = _ptr_array(d_gate_logits, "d_gate_logits", H, (M, E))
+    if tuple(_dev(p, "p", torch.float32).shape) != (M, H * E) or not p.is_contiguous():
+        raise ValueError(f"p must be a contiguous ({M}, {H * E}) matrix")
+    if tuple(_dev(dm, "dm", torch.float32).shape) != (H, M, U) or not dm.is_contiguous():
+        raise ValueError(f"dm must be a contiguous ({H}, {M}, {U}) tensor")
+    if tuple(_dev(dx, "dx", torch.float32).shape) != (M, E * U):
+        raise ValueError(f"dx must be ({M}, {E * U})")
+    _cabi.check(_lib().mm_mmoe_mix_bwd(x.data_ptr(), M, E, U, _row_stride(x, "x"), p.data_ptr(), H, float(temperature), dm.data_ptr(),
+                                       dx.data_ptr(), _row_stride(dx, "dx"), 1 if mask_relu else 0, dgp, dgs, _stream()),
+                "mm_mmoe_mix_bwd")
+
+
+def mmoe_task_heads_fwd_bwd(xs: Sequence[torch.Tensor], w: torch.Tensor, bias: Optional[torch.Tensor], losses: Sequence[str],
+                            targets: Optional[Sequence[torch.Tensor]], out: torch.Tensor, loss: Optional[torch.Tensor] = None,
+                            dxs: Optional[Sequence[torch.Tensor]] = None, dw: Optional[torch.Tensor] = None,
+                            db: Optional[torch.Tensor] = None, loss_weights: Optional[Sequence[float]] = None,
+                            mask_relu: bool = True, sample_weight=None) -> torch.Tensor:
+    """H output heads where head t reads its own input xs[t] (M, K) (mm_mmoe_task_heads_fwd_bwd); w (K, H), bias, losses,
+    targets, out, loss, dw, db, loss_weights and sample_weight as heads_fwd_bwd; training writes dxs[t] (M, K)."""
+    H = len(losses)
+    if not 1 <= H <= MMOE_MAX_TASKS or not xs:
+        raise ValueError(f"1..{MMOE_MAX_TASKS} heads, got {H}")
+    M, K = xs[0].shape
+    if not 1 <= K <= MMOE_MAX_UNITS:
+        raise ValueError(f"the heads read at most {MMOE_MAX_UNITS} inputs, got {K}")
+    xp, xst = _ptr_array(xs, "xs", H, (M, K))
+    if tuple(_dev(w, "w", torch.float32).shape) != (K, H) or not w.is_contiguous():
+        raise ValueError(f"w must be a contiguous ({K}, {H}) matrix")
+    _vec(bias, H, "bias")
+    if tuple(_dev(out, "out", torch.float32).shape) != (H, M) or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous ({H}, {M}) matrix")
+    if any(l not in _cabi.LOSS_KINDS for l in losses):
+        raise ValueError(f"losses must be among {sorted(_cabi.LOSS_KINDS)}, got {list(losses)}")
+    kinds = (C.c_int * H)(*[_cabi.LOSS_KINDS[l] for l in losses])
+    tp = dt = sp = lw = dxp = dxst = None
+    train = targets is not None
+    if train:
+        if len(targets) != H:
+            raise ValueError(f"one target tensor per head: {H} expected, got {len(targets)}")
+        dt = (C.c_int * H)(*[_target(t, M, f"targets[{h}]") for h, t in enumerate(targets)])
+        if loss is None or dxs is None:
+            raise ValueError("training needs loss and dxs")
+        _vec(loss, 1 + H, "loss")
+        dxp, dxst = _ptr_array(dxs, "dxs", H, (M, K))
+        if dw is not None and (_dev(dw, "dw", torch.float32).shape != (K, H) or not dw.is_contiguous()):
+            raise ValueError(f"dw must be a contiguous ({K}, {H}) matrix")
+        _vec(db, H, "db")
+        sws = list(sample_weight) if isinstance(sample_weight, (list, tuple)) else [sample_weight] * H
+        if len(sws) != H:
+            raise ValueError(f"one sample-weight tensor per head: {H} expected, got {len(sws)}")
+        for h, s_ in enumerate(sws):
+            _vec(s_, M, f"sample_weight[{h}]", _SAMPLE_WEIGHT)
+        lws = [1.0] * H if loss_weights is None else [float(v) for v in loss_weights]
+        if len(lws) != H:
+            raise ValueError(f"one loss weight per head: {H} expected, got {len(lws)}")
+        tp = (C.c_void_p * H)(*[t.data_ptr() for t in targets])
+        sp = (C.c_void_p * H)(*[_ptr(s_) for s_ in sws])
+        lw = (C.c_float * H)(*lws)
+    _cabi.check(_lib().mm_mmoe_task_heads_fwd_bwd(xp, xst, M, K, H, w.data_ptr(), _ptr(bias), kinds, lw, tp, dt, sp, out.data_ptr(),
+                                                  _ptr(loss) if train else None, dxp, dxst, 1 if mask_relu else 0,
+                                                  _ptr(dw) if train else None, _ptr(db) if train else None, _stream()),
+                "mm_mmoe_task_heads_fwd_bwd")
+    return out
+
+
 def _wgrad_n(M: int, K: int, dz: torch.Tensor, dw: torch.Tensor, db: Optional[torch.Tensor]) -> int:
     """N of the gradients of a Dense layer with M rows of K inputs: dz (M, N), dw a contiguous (K, N) matrix, db (N,) or None."""
     _dev(dz, "dz", torch.float32), _dev(dw, "dw", torch.float32)

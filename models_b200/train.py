@@ -1529,10 +1529,242 @@ class WideAndDeepTrainer(_StepTrainer):
         self.wk_grad.zero_()
 
 
+class MMoETrainer(_StepTrainer):
+    """Static-buffer training step of Model(InputBlockV2, [MLPBlock], [MMOEBlock], output) at one batch size, the output
+    optionally with per-task towers (OutputBlock(task_blocks=...)).
+
+    forward   the input block as DCN's (one-hot features gathered, multi-hot features pooled by their combiner) into x0 and
+              its split operand; mm_dense_tc per shared-bottom layer (the last one emits its split operand too); with an
+              MMOEBlock, mm_dense_tc of the stacked expert layer (B, E U) and the gates on that same operand (one stacked
+              bias-free layer, or one chain per gate with a gate_block)
+    head      without towers mm_mmoe_heads_fwd_bwd: gate soft-max, mixture, heads and loss, forward and backward; with
+              towers mm_mmoe_mix_fwd (the mixtures and their split operands) -> one tower chain per output ->
+              mm_mmoe_task_heads_fwd_bwd -> each tower's backward down to dm -> mm_mmoe_mix_bwd; without an MMOEBlock the
+              towers (or, without them, mm_heads_fwd_bwd) read the bottom's output
+    backward  every layer that reads the shared vector (experts, gates or towers) writes its pre-activation gradient into
+              its columns of one buffer G; mm_dense_wgrad_split per such layer, then their summed input gradient as ONE
+              transposed-kernel GEMM G [W_0 | W_1 | ..]^T; the bottom's backward; mm_concat_backward into each table's
+              IndexedSlices buffer, mm_bag_grad_rows for multi-hot features
+    update    mm_opt_tick, mm_dense_apply over the arena, mm_sparse_rows_apply per embedding width, mm_split_weights refresh
+              of the operand copies the model's forward reads.
+    Fixed-length list features can be captured into one CUDA graph; ragged ones train eagerly."""
+
+    def __init__(self, model, optimizer: Optimizer, batch_size: int, device=None, group=None):
+        from .blocks import dense_engine
+        from .models import BinaryOutput, MMoEBody, ParallelOutputs, output_towers
+
+        body = model.body
+        if not isinstance(body, MMoEBody):
+            raise NotImplementedError("MMoETrainer trains Model(InputBlockV2, [MLPBlock], [MMOEBlock], output) bodies")
+        if not isinstance(model.prediction, (BinaryOutput, ParallelOutputs)):
+            raise NotImplementedError("train_step needs BinaryOutput / RegressionOutput heads or an OutputBlock of them")
+        if group is not None:
+            raise NotImplementedError("training a multi-task Model(*blocks) with a process group is not implemented")
+        if dense_engine() == "fp32":
+            raise NotImplementedError("training a multi-task Model(*blocks) runs on the tensor-core engine (dense_engine() == 'fp32')")
+        ib, mo = body.input_block, body.mmoe
+        if getattr(ib.embeddings, "sharded", None) is not None:
+            raise NotImplementedError("training a multi-task Model(*blocks) with row-sharded tables is not implemented")
+        towers = output_towers(model.prediction) or []
+        blocks = ([body.bottom] if body.bottom is not None else []) + towers + (list(mo.gate_blocks.values()) if mo is not None and mo.gate_blocks else [])
+        for blk in blocks:
+            if blk.has_normalization or blk.dropout:
+                raise NotImplementedError("training supports bottom, gate and task blocks without normalization / dropout")
+        if mo is not None and mo.dropout:
+            raise NotImplementedError("training MMOEBlock experts with dropout is not implemented")
+        self._init_common(model, optimizer, batch_size, device, None)
+        self._init_heads()
+        self.bottom = body.bottom.dense_layers if body.bottom is not None else []
+        self.mmoe = mo
+        self.towers = [t.dense_layers for t in towers]
+        self.gate_chains = [mo.gate_chain(t) for t in range(mo.num_gates)] if mo is not None and mo.gate_blocks else []
+        chain_layers = [l for c in self.gate_chains + self.towers for l in c]
+        for l in self.bottom + chain_layers + ([mo.experts] if mo is not None else []):
+            if l.activation not in ("relu", "linear"):
+                raise NotImplementedError(f"{l.name}: training supports relu / linear activations, got {l.activation!r}")
+        if self.head.input_dim > 256:
+            raise NotImplementedError("the output layer's input must be <= 256 wide")
+        self.cols, _, self.d = ib.layout()
+        emb = ib.embeddings
+        feats = list(emb.feature_names) if emb is not None else []
+        tables = [emb.feature_to_table[f] for f in feats]
+        for f, t in zip(feats, tables):
+            col = model.schema.get(f)
+            if col is not None and col.is_list and t.dim not in (16, 32, 64, 128):
+                raise NotImplementedError(f"feature {f!r}: training a multi-hot feature needs an embedding width of 16, 32, 64 or "
+                                          f"128, got {t.dim} (pass an InputBlockV2 with Embeddings(dim=...))")
+        self.cont = sorted(ib.continuous.features) if ib.continuous is not None else []
+        self._init_tables(feats, tables)
+        # arena order: bottom, [experts, stacked gates], gate chains, towers, heads; li0 of each chain
+        tc = list(self.bottom)
+        if mo is not None:
+            self.li_experts = len(tc)
+            tc.append(mo.experts)
+            if mo.gates is not None:
+                self.li_gates = len(tc)
+                tc.append(mo.gates)
+        self.gate_li0 = []
+        for c in self.gate_chains:
+            self.gate_li0.append(len(tc))
+            tc += c
+        self.tower_li0 = []
+        for c in self.towers:
+            self.tower_li0.append(len(tc))
+            tc += c
+        self._init_dense(tc, [self.head])
+        nb = len(self.bottom)
+        firsts = set(self.gate_li0) | (set() if mo is not None else set(self.tower_li0))
+        # layers whose input gradient _dgrad computes (> 128 units: through the transposed kernel); the layers reading the
+        # shared vector take theirs together, and a tower's first layer reading the mixture takes it alone
+        self._init_wide(lambda li: (li < nb and (li > 0 or bool(self.tables))) or (li >= nb + (2 if mo is not None and mo.gates is not None else 1 if mo is not None else 0) and li not in firsts))
+
+        B, d = self.B, self.d
+        f32 = dict(dtype=torch.float32, device=self.device)
+        bf = dict(dtype=torch.bfloat16, device=self.device)
+        self.x0 = torch.zeros((B, _ld4(d)), **f32)
+        self.xs = torch.zeros((B, 2 * ops.tc_padded_k(d)), **bf)
+        self.dx0 = torch.zeros((B, _ld4(d)), **f32)
+        fanout = mo is not None or bool(self.towers)
+        if nb:
+            self.h, self.h_split, self.dh = self._chain_buffers(self.bottom, split_last=fanout)
+        # the layers that read the shared vector, and their columns in G
+        readers = ([mo.experts] + ([mo.gates] if mo.gates is not None else [c[0] for c in self.gate_chains])) if mo is not None \
+            else [c[0] for c in self.towers]
+        self.readers = readers
+        self.G = self.G_split = self.wT = self.wT_split = None
+        if fanout:
+            K = body.input_width()
+            N = sum(l.units for l in readers)
+            self.G = torch.zeros((B, N), **f32)
+            self.G_split = torch.zeros((B, 2 * ops.tc_padded_k(N)), **bf)
+            self.wT = torch.zeros((N, K), **f32)  # [W_0 | W_1 | ..]^T
+            self.wT_split = torch.zeros((ops.tc_padded_n(K), 2 * ops.tc_padded_k(N)), **bf)
+            self.G_cols, c = [], 0
+            for l in readers:
+                self.G_cols.append((c, c + l.units))
+                c += l.units
+        if mo is not None:
+            self.EU = mo.experts.units
+            self.X = torch.zeros((B, self.EU), **f32)
+            if mo.gates is not None:
+                self.L = torch.zeros((B, mo.gates.units), **f32)
+        self.gbufs = [self._chain_buffers(c) for c in self.gate_chains]
+        self.tbufs = [self._chain_buffers(c) for c in self.towers]
+        if self.towers and mo is not None:
+            H, U = self.H, mo.units
+            self.P = torch.zeros((B, H * mo.num_experts), **f32)
+            self.M = torch.zeros((H, B, U), **f32)
+            self.M_split = torch.zeros((H, B, 2 * ops.tc_padded_k(U)), **bf)
+            self.dM = torch.zeros((H, B, U), **f32)
+        self.slices = [torch.zeros((B, t.table.shape[1]), **f32) for t in self.tables]
+        self._init_loss(B)
+        self.oob = emb.counter(self.device) if emb is not None else None
+
+    def _g(self, i: int, b: int) -> torch.Tensor:
+        """Reader i's columns of G (its pre-activation gradient)."""
+        c0, c1 = self.G_cols[i]
+        return self.G[:b, c0:c1]
+
+    def forward_backward(self, inputs: Dict[str, torch.Tensor], targets, sample_weight=None) -> None:
+        """Forward (activations saved), loss and backward: fills the gradient arena and the tables' IndexedSlices.  Batches
+        smaller than the compiled size run in the leading rows of the same buffers."""
+        a = self.arena
+        nb, d, mo = len(self.bottom), self.d, self.mmoe
+        self._loss_all.zero_()
+        b = batch_size_of(inputs)
+        targets = self._check_targets(targets, b)
+        ys = [t.reshape(-1) for t in targets]
+        hi = len(a.layers) - 1
+        logits = self.logits.view(-1)[:self.H * b].view(self.H, b)
+        tidx = range(len(self.tables))
+        self._idx: List[Optional[torch.Tensor]] = [None] * len(self.tables)
+        self._slices = [s[:b] for s in self.slices]
+        self._bags = {}
+        v = lambda ts: [t[:b] for t in ts]
+        x0, xs, dx0 = self.x0[:b, :d], self.xs[:b], self.dx0[:b, :d]
+        self._input_forward(self.feats, tidx, self.cols, self.cont, inputs, x0, xs)
+        op, K = xs, d
+        if nb:
+            h, h_split, dh = v(self.h), v(self.h_split), v(self.dh)
+            self._chain_forward(xs, d, 0, self.bottom, h, h_split)
+            if self.G is not None:
+                op, K = h_split[-1], self.bottom[-1].units
+        heads_kw = dict(loss_weights=self.loss_weights, sample_weight=sample_weight)
+        if self.G is None:  # shared bottom -> heads
+            self._heads(h[-1], targets, dh[-1], self.bottom[-1].activation == "relu", sample_weight, b)
+        elif mo is None:  # towers on the shared vector
+            tb = [[v(x) for x in bufs] for bufs in self.tbufs]
+            for i, (c, (th, ths, tdh)) in enumerate(zip(self.towers, tb)):
+                tdh[0] = self._g(i, b)
+                self._chain_forward(op, K, self.tower_li0[i], c, th, ths)
+            ops.mmoe_task_heads_fwd_bwd([t[0][-1] for t in tb], self.head.kernel, self.head.bias, self.losses, ys, logits,
+                                        self._loss_all, [t[2][-1] for t in tb], a.view(a.grad, hi, "kernel"), a.view(a.grad, hi, "bias"),
+                                        mask_relu=self.towers[0][-1].activation == "relu", **heads_kw)
+            for i, (c, (th, ths, tdh)) in enumerate(zip(self.towers, tb)):
+                self._chain_backward(self.tower_li0[i], c, th, tdh, (op, K), None)
+        else:
+            X = self.X[:b]
+            ops.dense_tc(op, K, self._wsplit[self.li_experts], self.EU, mo.experts.bias, mo.experts.activation, out_f32=X)
+            gb = [[v(x) for x in bufs] for bufs in self.gbufs]
+            if mo.gates is not None:
+                L = self.L[:b]
+                ops.dense_tc(op, K, self._wsplit[self.li_gates], mo.gates.units, None, "linear", out_f32=L)
+                gl, dgl = mo.gate_logits(L), mo.gate_logits(self._g(1, b))
+            else:
+                for i, (c, (gh, ghs, gdh)) in enumerate(zip(self.gate_chains, gb)):
+                    gdh[0] = self._g(1 + i, b)
+                    self._chain_forward(op, K, self.gate_li0[i], c, gh, ghs)
+                gl, dgl = [g[0][-1] for g in gb], [g[2][-1] for g in gb]
+            dX = self._g(0, b)
+            relu_x = mo.experts.activation == "relu"
+            if not self.towers:
+                ops.mmoe_heads_fwd_bwd(X, mo.num_experts, gl, mo.temperature, self.head.kernel, self.head.bias, self.losses, ys,
+                                       logits, self._loss_all, dx=dX, d_gate_logits=dgl, dw=a.view(a.grad, hi, "kernel"),
+                                       db=a.view(a.grad, hi, "bias"), mask_relu=relu_x, **heads_kw)
+            else:
+                U = mo.units
+                H = self.H
+                # (H, b, ...) views of the leading H b rows, contiguous like the kernels write them
+                M, Ms, dM = (t.view(-1)[:H * b * t.shape[2]].view(H, b, t.shape[2]) for t in (self.M, self.M_split, self.dM))
+                P = self.P[:b]
+                ops.mmoe_mix_fwd(X, mo.num_experts, gl, mo.temperature, P, M, Ms)
+                tb = [[v(x) for x in bufs] for bufs in self.tbufs]
+                for i, (c, (th, ths, tdh)) in enumerate(zip(self.towers, tb)):
+                    self._chain_forward(Ms[i], U, self.tower_li0[i], c, th, ths)
+                ops.mmoe_task_heads_fwd_bwd([t[0][-1] for t in tb], self.head.kernel, self.head.bias, self.losses, ys, logits,
+                                            self._loss_all, [t[2][-1] for t in tb], a.view(a.grad, hi, "kernel"),
+                                            a.view(a.grad, hi, "bias"), mask_relu=self.towers[0][-1].activation == "relu", **heads_kw)
+                for i, (c, (th, ths, tdh)) in enumerate(zip(self.towers, tb)):
+                    self._chain_backward(self.tower_li0[i], c, th, tdh, (Ms[i], U), dM[i])
+                ops.mmoe_mix_bwd(X, mo.num_experts, P, mo.temperature, dM, dX, dgl, mask_relu=relu_x)
+            ops.dense_wgrad_split(op, K, dX, a.view(a.grad, self.li_experts, "kernel"), a.view(a.grad, self.li_experts, "bias"))
+            if mo.gates is not None:
+                ops.dense_wgrad_split(op, K, self._g(1, b), a.view(a.grad, self.li_gates, "kernel"), None)
+            else:
+                for i, (c, (gh, ghs, gdh)) in enumerate(zip(self.gate_chains, gb)):
+                    self._chain_backward(self.gate_li0[i], c, gh, gdh, (op, K), None)
+        dx_in = dh[-1] if nb else (dx0 if self.tables else None)
+        if self.G is not None and dx_in is not None:  # G [W_0 | W_1 | ..]^T: the readers' input gradients summed by one GEMM
+            for (c0, c1), l in zip(self.G_cols, self.readers):
+                self.wT[c0:c1].copy_(l.kernel.t())
+            ops.split_weights(self.wT, out=self.wT_split)
+            Gs = self.G_split[:b]
+            ops.split_rows(self.G[:b], out=Gs)
+            ops.dense_tc(Gs, self.G.shape[1], self.wT_split, K, None, None, out_f32=dx_in)
+            if nb and self.bottom[-1].activation == "relu":
+                ops.relu_mask(dx_in, h[-1])
+        if nb:
+            self._chain_backward(0, self.bottom, h, dh, (xs, d), dx0 if self.tables else None)
+        if self.tables:
+            self._input_backward([dx0], self.feats, tidx, self.cols)
+            self._bag_grads()
+        self._b = b
+
+
 def trainer_for(model, optimizer: Optimizer, batch_size: int, group=None):
-    """The training engine of `model`: DLRMTrainer, DCNTrainer, DeepFMTrainer or WideAndDeepTrainer by the ranking body,
-    TwoTowerTrainer for a RetrievalModel."""
-    from .models import DCNBody, DeepFMBody, RetrievalModel, RetrievalModelV2, WideAndDeepBody
+    """The training engine of `model`: DLRMTrainer, DCNTrainer, DeepFMTrainer, WideAndDeepTrainer or MMoETrainer by the
+    ranking body, TwoTowerTrainer for a RetrievalModel."""
+    from .models import DCNBody, DeepFMBody, MMoEBody, RetrievalModel, RetrievalModelV2, WideAndDeepBody
 
     if isinstance(model, RetrievalModelV2):
         raise NotImplementedError("training TwoTowerModelV2 / ContrastiveOutput is not implemented: train the v1 TwoTowerModel")
@@ -1544,4 +1776,6 @@ def trainer_for(model, optimizer: Optimizer, batch_size: int, group=None):
         return DeepFMTrainer(model, optimizer, batch_size, group=group)
     if isinstance(getattr(model, "body", None), WideAndDeepBody):
         return WideAndDeepTrainer(model, optimizer, batch_size, group=group)
+    if isinstance(getattr(model, "body", None), MMoEBody):
+        return MMoETrainer(model, optimizer, batch_size, group=group)
     return DLRMTrainer(model, optimizer, batch_size, group=group)
