@@ -182,15 +182,16 @@ __global__ void __launch_bounds__(32 * WARPS, 1) mmoe_heads_kernel(const Params 
       continue;
     }
     __syncwarp();
-    // gate backward: lane t < H, dg_t,e = dz_t <w_t, X_e>
+    // gate backward: lane t < H, dg_t,e = dz_t <w_t, X_e>.  dg is rounded once (__fmul_rn, never contracted into an FMA)
+    // so that s and dg - s see the same value: with one expert dg - s is then exactly 0, as the soft-max's gradient is.
     if (lane < H) {
       const float dz = s_dz[wid][lane];
       const float* q = sp + lane * E;
       const float* a = sa + lane * E;
       float s = 0.0f;
-      for (int e = 0; e < E; ++e) s = fmaf(q[e], dz * a[e], s);
+      for (int e = 0; e < E; ++e) s = fmaf(q[e], __fmul_rn(dz, a[e]), s);
       float* o = p.dgl[lane] + m * p.lddgl[lane];
-      for (int e = 0; e < E; ++e) o[e] = q[e] * (dz * a[e] - s) * p.inv_t;
+      for (int e = 0; e < E; ++e) o[e] = q[e] * (__fmul_rn(dz, a[e]) - s) * p.inv_t;
     }
     // expert backward: dX_e = sum_t p_t,e dz_t w_t
     float dzr[NH];

@@ -31,16 +31,20 @@ def gate_mix(X: torch.Tensor, L: torch.Tensor, E: int, T: float) -> torch.Tensor
 
 
 def heads_loss(zs: Sequence[torch.Tensor], losses: Sequence[str], targets, loss_weights=None, sample_weight=None):
-    """(total, [loss_t]) of the logits zs[t] (B,)."""
+    """(total, [loss_t]) of the logits zs[t] (B,); targets and sample weights as numpy arrays or tensors (on any device)."""
     H = len(zs)
     lws = [1.0] * H if loss_weights is None else [float(v) for v in loss_weights]
     sws = list(sample_weight) if isinstance(sample_weight, (list, tuple)) else [sample_weight] * H
+    like = lambda v, z: (v.reshape(-1).to(z) if isinstance(v, torch.Tensor)  # noqa: E731
+                         else torch.as_tensor(np.asarray(v, dtype=np.float64).reshape(-1)).to(z))
     total, per = None, []
     for z, l, y_np, sw, lw in zip(zs, losses, targets, sws, lws):
-        y = torch.as_tensor(np.asarray(y_np, dtype=np.float64).reshape(-1)).to(z.dtype)
-        term = torch.clamp(z, min=0) - z * y + torch.log1p(torch.exp(-z.abs())) if l == BCE else (z - y) ** 2
+        y = like(y_np, z)
+        # max(z, 0) as (z + |z|) / 2: the same value, and at z = 0 (a dead tower's output times the head kernel plus a zero
+        # bias) the derivative sigmoid(0) - y the kernels compute, where clamp's sub-gradient would give 1 - y
+        term = (z + z.abs()) / 2 - z * y + torch.log1p(torch.exp(-z.abs())) if l == BCE else (z - y) ** 2
         if sw is not None:
-            term = term * torch.as_tensor(np.asarray(sw, dtype=np.float64).reshape(-1)).to(z.dtype)
+            term = term * like(sw, z)
         lt = term.sum() / y.shape[0]
         total = lw * lt if total is None else total + lw * lt
         per.append(lt)

@@ -103,14 +103,15 @@ def _targets(model, targs, device):
     return {o.target: torch.from_numpy(np.asarray(targs[o.target])).to(device) for o in model.output_blocks()}
 
 
-def _check_gradients(model, tr, feats, targs):
+def _check_gradients(model, tr, feats, targs, sample_weight=None):
     """One forward_backward against the restatement (with the device's relu decisions): loss, every dense gradient and the
-    tables' dense gradients."""
+    tables' dense gradients.  sample_weight: one (B,) numpy array or None per output."""
     arr = model_arrays(model)
     outs = model.output_blocks()
     ys = [np.asarray(targs[o.target]) for o in outs]
     dev = tr.device
-    tr.forward_backward(H.device_batch(feats, dev), [torch.from_numpy(y).to(dev) for y in ys])
+    sw = None if sample_weight is None else [None if w is None else torch.from_numpy(w).to(dev) for w in sample_weight]
+    tr.forward_backward(H.device_batch(feats, dev), [torch.from_numpy(y).to(dev) for y in ys], sample_weight=sw)
     b = len(ys[0])
     masks = {f"bottom_{i}": (tr.h[i][:b] > 0).cpu().numpy() for i in range(len(tr.bottom))}
     if tr.mmoe is not None:
@@ -119,8 +120,8 @@ def _check_gradients(model, tr, feats, targs):
         for t, (h_, _, _) in enumerate(bufs):
             masks.update({f"{tag}_{t}_{i}": (x[:b] > 0).cpu().numpy() for i, x in enumerate(h_)})
     total, per, zs, g = mmoe_loss_and_grads(feats, arr["tables"], arr["continuous"], arr["bottom"], arr["experts"], arr["gates"],
-                                            arr["temperature"], arr["heads"], ys, loss_weights=model.loss_weights, masks=masks,
-                                            towers=arr["towers"])
+                                            arr["temperature"], arr["heads"], ys, loss_weights=model.loss_weights,
+                                            sample_weight=sample_weight, masks=masks, towers=arr["towers"])
     close(tr._loss_all[0], total, 1e-5, "loss")
     if len(outs) > 1:
         close(tr._loss_all[1:], np.array(per), 1e-5, "per-task losses")

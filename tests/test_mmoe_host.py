@@ -213,3 +213,11 @@ def test_task_blocks_as_a_layer_and_as_dicts_by_name_and_by_column():
     o3 = mm.OutputBlock(s, task_blocks=mm.MLPBlock([8]))
     shared = mm.Model(mm.InputBlockV2(s), mm.MLPBlock([16]), o3)
     assert shared.body.mmoe is None and shared.prediction.task_blocks
+
+
+def test_kernel_cases_reach_every_instantiation():
+    """tests/test_gpu_mmoe_kernels.py's CASES reach every (tasks rounded up to a power of two, columns per lane) pair the
+    MMoE mixture and task-head kernels are compiled for."""
+    from tests.test_gpu_mmoe_kernels import CASES, _dispatch
+
+    assert sorted({_dispatch(c[0], c[1]) for c in CASES}) == [(nh, c) for nh in (1, 2, 4, 8) for c in (1, 2, 4, 8)]

@@ -9,7 +9,7 @@ import pytest
 import models_b200 as mm
 from models_b200.models import WideAndDeepBody
 from models_b200.schema import ColumnSchema, Schema, Tags
-from tests.wide_deep_train_oracle import BCE, MSE, bags_of, encode, wide_deep_forward, wide_deep_loss_and_grads
+from tests.wide_deep_train_oracle import BCE, MSE, bags_of, encode, encode_sparse, wide_deep_forward, wide_deep_loss_and_grads
 
 CATS = [("C1", 30), ("C3", 3), ("C5", 400), ("C7", 7)]
 LISTS = [("L2", 50), ("L4", 9)]
@@ -201,3 +201,43 @@ def test_packed_uint8_list_is_refused():
         m.body.wide.blocks(x)
     onehot, bags = m.body.wide.blocks({"C1": x["C1"], "L2": x["L2"].to(torch.int32)})
     assert len(onehot) == 1 and onehot[0][0].dtype == torch.uint8 and len(bags) == 1 and bags[0][0].shape == (4, 3)
+
+
+@pytest.mark.parametrize("mode", ["one_hot", "multi_hot", "count"])
+def test_sparse_encoding_equals_the_dense_one(mode):
+    """encode_sparse against encode on one-hot ids, fixed bags with repeats and ragged bags whose offsets leave values
+    uncovered, go backwards and run past the end (clamped as bags_of does); out-of-range and negative ids encode to nothing."""
+    g = np.random.default_rng(5)
+    card = 11
+    one = g.integers(-1, card + 2, 40)
+    fixed = g.integers(-1, card + 2, (40, 6))
+    fixed[0] = 4
+    offs = np.array([2, 2, 5, 4, 9, 9, 13, 30])
+    vals = g.integers(-1, card + 2, 20)
+    for x in (one, fixed, (vals, offs)):
+        if mode == "one_hot" and not (isinstance(x, np.ndarray) and x.ndim == 1):
+            continue
+        np.testing.assert_array_equal(encode_sparse(x, card, mode).toarray(), encode(x, card, mode))
+
+
+@pytest.mark.parametrize("mode", ["multi_hot", "count"])
+@pytest.mark.parametrize("ragged", [False, True])
+@pytest.mark.parametrize("loss", [BCE, MSE])
+def test_sparse_restatement_equals_the_dense_one(mode, ragged, loss):
+    """wide_deep_loss_and_grads(sparse=True) (CSR encodings and mean pools, closed-form wide and pooled-table gradients)
+    gives the dense path's loss, logits and every gradient."""
+    g = np.random.default_rng(11)
+    wide, deep, head = _state(g, mode)
+    head["loss"] = loss
+    B = 37
+    batch = _batch(g, B, ragged)
+    batch["L2"] = batch["L2"] if ragged else np.where(g.random((B, 4)) < 0.1, 12, batch["L2"])  # out-of-range ids in bags
+    y = g.integers(0, 2, B) if loss == BCE else g.standard_normal(B)
+    sw = g.random(B) * 2
+    L, z, grads = wide_deep_loss_and_grads(batch, wide, deep, head, y, sample_weight=sw)
+    Ls, zs, gs = wide_deep_loss_and_grads(batch, wide, deep, head, y, sample_weight=sw, sparse=True)
+    assert abs(Ls - L) <= 1e-12 * max(1.0, abs(L))
+    np.testing.assert_allclose(zs, z, rtol=1e-12, atol=1e-12)
+    assert sorted(gs) == sorted(grads)
+    for k in grads:
+        np.testing.assert_allclose(gs[k], grads[k], rtol=1e-10, atol=1e-12, err_msg=k)

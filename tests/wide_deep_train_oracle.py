@@ -14,6 +14,7 @@ from __future__ import annotations
 from typing import Dict, List, Optional
 
 import numpy as np
+import scipy.sparse as sp
 import torch
 
 from oracle.oracle_train import _act
@@ -44,6 +45,49 @@ def encode(x, card: int, mode: str) -> np.ndarray:
         c = np.bincount(ids, minlength=card).astype(np.float64)
         out[b] = np.minimum(c, 1.0) if mode in ("one_hot", "multi_hot") else c
     return out
+
+
+def _positions(x):
+    """(sample, id, bag length) of every position of a feature given as (B,), (B, L) or (values, offsets), vectorised:
+    positions outside [offsets[b], offsets[b + 1]) (clamped as bags_of does) belong to no sample and are dropped."""
+    if isinstance(x, tuple):
+        v, o = np.asarray(x[0]).reshape(-1).astype(np.int64), np.asarray(x[1]).reshape(-1).astype(np.int64)
+        n = v.shape[0]
+        s = np.clip(o[:-1], 0, n)
+        e = np.maximum(np.clip(o[1:], 0, n), s)
+        lens = e - s
+        b = np.repeat(np.arange(lens.shape[0]), lens)
+        pos = np.arange(int(lens.sum())) - np.repeat(np.cumsum(lens) - lens, lens) + np.repeat(s, lens)
+        return b, v[pos], lens
+    x = np.asarray(x)
+    x = x.reshape(x.shape[0], -1)
+    B, L = x.shape
+    return np.repeat(np.arange(B), L), x.reshape(-1).astype(np.int64), np.full(B, L)
+
+
+def encode_sparse(x, card: int, mode: str) -> sp.csr_matrix:
+    """encode() as a (B, card) CSR matrix, built without a per-sample loop."""
+    b, ids, lens = _positions(x)
+    ok = (ids >= 0) & (ids < card)
+    m = sp.csr_matrix((np.ones(int(ok.sum())), (b[ok], ids[ok])), shape=(lens.shape[0], card))
+    m.sum_duplicates()
+    if mode in ("one_hot", "multi_hot"):
+        m.data = np.minimum(m.data, 1.0)
+    return m
+
+
+def _mean_pool_sparse(x, rows: int, ragged: bool) -> sp.csr_matrix:
+    """The (B, rows) weights of the deep mean over a bag: 1 / L per in-range position for fixed bags, 1 / (in-range count)
+    for ragged ones, as _pooled."""
+    b, ids, lens = _positions(x)
+    ok = (ids >= 0) & (ids < rows)
+    if ragged:
+        n = np.maximum(np.bincount(b[ok], minlength=lens.shape[0]), 1)
+    else:
+        n = np.maximum(lens, 1)
+    m = sp.csr_matrix((1.0 / n[b[ok]], (b[ok], ids[ok])), shape=(lens.shape[0], rows))
+    m.sum_duplicates()
+    return m
 
 
 def _pooled(x, table: np.ndarray) -> np.ndarray:
@@ -87,20 +131,35 @@ def wide_deep_forward(batch: Dict[str, object], wide: Optional[dict], deep: Opti
 
 
 def wide_deep_loss_and_grads(batch: Dict[str, object], wide: Optional[dict], deep: Optional[dict], head: dict, targets: np.ndarray,
-                             sample_weight=None):
+                             sample_weight=None, sparse: bool = False, masks: Optional[Dict[str, np.ndarray]] = None):
     """The forward of wide_deep_forward in float64 torch, the loss of head["loss"] and autograd.  Returns (loss, z (B,), grads)
     with grads keyed "wide/kernel", "wide/bias", "table/<f>", "deep/kernel_i", "deep/bias_i", "deep_logit/kernel",
-    "deep_logit/bias", "head/kernel", "head/bias"."""
+    "deep_logit/bias", "head/kernel", "head/bias".
+
+    sparse: the encodings and the multi-hot mean pools as scipy CSR matrices built without a per-sample loop (sizes where
+    a dense (B, card) matrix does not fit): the wide term enc @ wk and each pooled input enter autograd as leaves, and
+    their parameters' gradients are the closed forms enc^T ds and pool^T d(pooled).
+
+    masks {"deep_i": (B, units)} (optional): where deep layer i's relu passes its input, as the device decided it.  A
+    pre-activation within float32 rounding of 0 can take either side of the kink; with the device's decisions the
+    restatement's gradients follow the same branch (relu(y) and y * mask differ only at such values)."""
 
     def var(x):
         return torch.tensor(np.asarray(x, dtype=np.float64), requires_grad=True)
 
     P = {"head/kernel": var(head["kernel"]), "head/bias": var(head["bias"])}
+    leaves = {}  # name: (leaf tensor, CSR matrix, parameter key) for the sparse path
     s = 0.0
     if wide is not None:
         P["wide/kernel"], P["wide/bias"] = var(wide["kernel"]), var(wide["bias"])
-        enc = np.concatenate([encode(batch[n], wide["cards"][n], wide["mode"]) for n in sorted(wide["cards"])], axis=1)
-        s = torch.from_numpy(enc) @ P["wide/kernel"].reshape(-1) + P["wide/bias"].reshape(())
+        if sparse:
+            enc = sp.hstack([encode_sparse(batch[n], wide["cards"][n], wide["mode"]) for n in sorted(wide["cards"])], format="csr")
+            t = torch.tensor(enc @ np.asarray(wide["kernel"], np.float64).reshape(-1), requires_grad=True)
+            leaves["wide"] = (t, enc, "wide/kernel")
+            s = t + P["wide/bias"].reshape(())
+        else:
+            enc = np.concatenate([encode(batch[n], wide["cards"][n], wide["mode"]) for n in sorted(wide["cards"])], axis=1)
+            s = torch.from_numpy(enc) @ P["wide/kernel"].reshape(-1) + P["wide/bias"].reshape(())
     if deep is not None:
         cols = {}
         for n, t in deep["tables"].items():
@@ -111,6 +170,10 @@ def wide_deep_loss_and_grads(batch: Dict[str, object], wide: Optional[dict], dee
                 ids = torch.from_numpy(np.asarray(x).reshape(-1).astype(np.int64))
                 ok = ((ids >= 0) & (ids < rows)).double()
                 cols[n] = P[f"table/{n}"][ids.clamp(0, rows - 1)] * ok[:, None]
+            elif sparse:
+                M = _mean_pool_sparse(x, rows, isinstance(x, tuple))
+                cols[n] = torch.tensor(M @ np.asarray(t, np.float64), requires_grad=True)
+                leaves[f"pool/{n}"] = (cols[n], M, f"table/{n}")
             else:  # mean over the bag as a (B, rows) weight matrix
                 bags = bags_of(x)
                 M = np.zeros((len(bags), rows))
@@ -124,7 +187,11 @@ def wide_deep_loss_and_grads(batch: Dict[str, object], wide: Optional[dict], dee
         h = torch.cat([cols[n] for n in sorted(cols)], dim=1)
         for i, l in enumerate(deep["layers"]):
             P[f"deep/kernel_{i}"], P[f"deep/bias_{i}"] = var(l["kernel"]), var(l["bias"])
-            h = _act(h @ P[f"deep/kernel_{i}"] + P[f"deep/bias_{i}"], l.get("activation"))
+            h = h @ P[f"deep/kernel_{i}"] + P[f"deep/bias_{i}"]
+            if l.get("activation") == "relu" and f"deep_{i}" in (masks or {}):
+                h = h * torch.from_numpy(np.asarray(masks[f"deep_{i}"], dtype=np.float64))
+            else:
+                h = _act(h, l.get("activation"))
         lg = deep["logit"]
         P["deep_logit/kernel"], P["deep_logit/bias"] = var(lg["kernel"]), var(lg["bias"])
         s = s + _act(h @ P["deep_logit/kernel"] + P["deep_logit/bias"], lg.get("activation")).reshape(-1)
@@ -139,4 +206,6 @@ def wide_deep_loss_and_grads(batch: Dict[str, object], wide: Optional[dict], dee
     loss = per.sum() / y.shape[0]
     loss.backward()
     grads = {k: (v.grad.numpy().copy() if v.grad is not None else np.zeros(tuple(v.shape))) for k, v in P.items()}
+    for leaf, M, key in leaves.values():  # the sparse path's closed forms
+        grads[key] = np.asarray(M.T @ leaf.grad.numpy()).reshape(grads[key].shape)
     return float(loss.item()), z.detach().numpy().copy(), grads
