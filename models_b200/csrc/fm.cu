@@ -137,21 +137,6 @@ struct HeadBwdParams {
   int D;
 };
 
-// loss term and d loss / dz (before sw and 1/M): BCE on the logit (BinaryOutput), squared error (RegressionOutput); the
-// same expressions as mm_heads_fwd_bwd
-__device__ __forceinline__ void fm_head_loss(int kind, float z, float y, float& l, float& g) {
-  if (kind == MM_LOSS_MSE) {
-    const float d = z - y;
-    l = d * d;
-    g = 2.0f * d;
-  } else {
-    const float e = expf(-fabsf(z));
-    l = fmaxf(z, 0.0f) - z * y + log1pf(e);
-    const float sig = z >= 0.0f ? 1.0f / (1.0f + e) : e / (1.0f + e);
-    g = sig - y;
-  }
-}
-
 __global__ void __launch_bounds__(256) deepfm_head_fwd_bwd_kernel(const __grid_constant__ HeadBwdParams p) {
   constexpr int UC = HB_MAX_U / 32;
   const int lane = threadIdx.x & 31;
@@ -208,7 +193,7 @@ __global__ void __launch_bounds__(256) deepfm_head_fwd_bwd_kernel(const __grid_c
     const float y = load_as_f32(p.y, b, p.y_dtype);
     const float sw = p.sw ? p.sw[b] : 1.0f;
     float l, g;
-    fm_head_loss(p.kind, z, y, l, g);
+    head_loss(p.kind, z, y, l, g);
     const float delta = g * sw * p.inv_m;
     const float dsv = delta * wo;
     const float du = (relu_dl && !(u > 0.0f)) ? 0.0f : dsv;

@@ -78,6 +78,22 @@ __device__ __forceinline__ float head_pred(int kind, float z) {
   return z >= 0.0f ? 1.0f / (1.0f + e) : e / (1.0f + e);
 }
 
+// Loss term l and dloss/dz g of an output head from its logit z and target y, before the loss weight, the sample weight
+// and 1/B: BCE on the logit (MM_LOSS_BCE, BinaryOutput) or squared error (MM_LOSS_MSE, RegressionOutput).  Every kernel
+// that fuses a head's loss (mm_heads_fwd_bwd, the DeepFM, Wide&Deep and MMoE heads) evaluates this one code.
+__device__ __forceinline__ void head_loss(int kind, float z, float y, float& l, float& g) {
+  if (kind == MM_LOSS_MSE) {
+    const float d = z - y;
+    l = d * d;
+    g = 2.0f * d;
+  } else {
+    const float e = expf(-fabsf(z));
+    l = fmaxf(z, 0.0f) - z * y + log1pf(e);
+    const float sig = z >= 0.0f ? 1.0f / (1.0f + e) : e / (1.0f + e);
+    g = sig - y;
+  }
+}
+
 // per-launch table list, passed by value in kernel parameter space (2 KB)
 struct GatherParams {
   mm_gather_table t[MM_MAX_TABLES];

@@ -57,20 +57,6 @@ struct Params {
   float* db;  // (H,) accumulated
 };
 
-// loss term and d loss / dz (before lambda, sw and 1/M), the expressions of mm_heads_fwd_bwd
-__device__ __forceinline__ void head_loss(int kind, float z, float y, float& l, float& g) {
-  if (kind == MM_LOSS_MSE) {
-    const float d = z - y;
-    l = d * d;
-    g = 2.0f * d;
-  } else {
-    const float e = expf(-fabsf(z));
-    l = fmaxf(z, 0.0f) - z * y + log1pf(e);
-    const float sig = z >= 0.0f ? 1.0f / (1.0f + e) : e / (1.0f + e);
-    g = sig - y;
-  }
-}
-
 // the gate soft-max of sample m into sp[t E + e] (the warp's shared row); ends with the row visible to the whole warp
 __device__ __forceinline__ void gate_softmax(const float* const* gl, const long long* ldgl, long long m, int E, int H, float inv_t,
                                              float* sp, int lane) {

@@ -59,20 +59,6 @@ struct HeadParams {
 
 constexpr int HEAD_KMAX = 256;  // 8 columns per lane
 
-// loss term and d loss / dz (before lambda, sw and 1/M) of one head
-__device__ __forceinline__ void head_loss(int kind, float z, float y, float& l, float& g) {
-  if (kind == MM_LOSS_MSE) {
-    const float d = z - y;
-    l = d * d;
-    g = 2.0f * d;
-  } else {
-    const float e = expf(-fabsf(z));
-    l = fmaxf(z, 0.0f) - z * y + log1pf(e);
-    const float sig = z >= 0.0f ? 1.0f / (1.0f + e) : e / (1.0f + e);
-    g = sig - y;
-  }
-}
-
 template <int H, bool TRAIN>
 __global__ void __launch_bounds__(256, H == 1 ? 2 : 1) head_kernel(const HeadParams p) {
   const int lane = threadIdx.x & 31;

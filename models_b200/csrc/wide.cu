@@ -110,20 +110,6 @@ __device__ __forceinline__ float group_sum(float v) {
   return v;
 }
 
-// loss term and dloss/dz before sw and 1/B: BCE on the logit (BinaryOutput), squared error (RegressionOutput)
-__device__ __forceinline__ void head_loss(int kind, float z, float y, float& l, float& g) {
-  if (kind == MM_LOSS_MSE) {
-    const float d = z - y;
-    l = d * d;
-    g = 2.0f * d;
-  } else {
-    const float e = expf(-fabsf(z));
-    l = fmaxf(z, 0.0f) - z * y + log1pf(e);
-    const float sig = z >= 0.0f ? 1.0f / (1.0f + e) : e / (1.0f + e);
-    g = sig - y;
-  }
-}
-
 __device__ __forceinline__ float4 load4(const float* row, int k, int U, bool vec) {
   if (vec) return k < U ? *reinterpret_cast<const float4*>(row + k) : make_float4(0.f, 0.f, 0.f, 0.f);
   return make_float4(k < U ? row[k] : 0.f, k + 1 < U ? row[k + 1] : 0.f, k + 2 < U ? row[k + 2] : 0.f, k + 3 < U ? row[k + 3] : 0.f);

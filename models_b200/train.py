@@ -1,10 +1,12 @@
 """Training steps (SURVEY §8(f)-4): forward with saved activations, loss, backward and optimizer update as hand-written
 CUDA (include/mm_b200.h K14), behind the reference's `compile` / `fit` / `train_step`
 (merlin/models/tf/models/base.py:1121-1231; optimizers: tf.keras.optimizers.{SGD, Adagrad, Adam}, LazyAdam
-blocks/optimizer.py:342).  One trainer per model (DLRMTrainer, DCNTrainer, TwoTowerTrainer, DeepFMTrainer; trainer_for picks)
-holds what is particular to it; the parts they share are methods of _StepTrainer: the dense arena, the table checks and
-optimizer state, a chain of Dense layers forward and backward, the concatenating input block, multi-hot pooling, the output
-heads, the update (apply_gradients), capture / replay.
+blocks/optimizer.py:342).  One trainer per model (DLRMTrainer, DCNTrainer, TwoTowerTrainer, DeepFMTrainer,
+WideAndDeepTrainer, MMoETrainer; trainer_for picks) holds what is particular to it; the parts they share are methods of
+_StepTrainer (the construction checks, the dense arena, the table checks and optimizer state, a chain of Dense layers forward
+and backward, multi-hot pooling, the output heads, the step's prologue, the update (apply_gradients), snapshot / restore,
+capture / replay) and two parts a trainer owns: the concatenating input block (_ConcatInput) and a wide kernel trained
+outside the arena (_WideKernel).
 
 What a step launches (DLRM, bottom [.., D], top [...], BinaryOutput):
 
@@ -210,13 +212,43 @@ class _StepTrainer:
     optimizer state, a chain of Dense layers forward and backward, the concatenating input block forward and backward,
     multi-hot pooling and its gradient expansion, the output heads, the update, CUDA-graph capture / replay, and the
     host-side bookkeeping.  A subclass sets the attributes below in its __init__ (through the _init_* methods) and
-    implements forward_backward, which leaves _idx / _slices / _bags / _b for apply_gradients:
+    implements forward_backward, which starts with _begin_step and leaves _idx / _slices / _bags / _b for apply_gradients:
       model, body, opt, device, B, group, world, arena, hyper, head, outputs, H, losses, loss_weights,
       _tc_layers / _wsplit (Dense layers whose split operand copies follow the updates), _wide (see _init_wide),
-      feats / tables / tstate1 / tstate2 / rep / tdense, oob, logits / _loss_all / loss."""
+      feats / tables / tstate1 / tstate2 / rep / tdense / slices, oob, logits / _loss_all / loss, wk (_WideKernel)."""
 
     head: Optional[_Dense] = None  # the output layer; a trainer whose task builds its own targets has none
-    _multihot_refused: Optional[str] = None  # the model's name when its input block trains one-hot features only
+    _model_name = "this model"  # how the construction checks' messages name the model
+    _onehot_only = False  # the model's input block trains one-hot features only
+    wk: Optional["_WideKernel"] = None  # a wide kernel trained outside the arena (DeepFM, Wide&Deep)
+
+    # ---- construction checks ------------------------------------------------------------------------------------------
+    def _refuse_group(self, group) -> None:
+        if group is not None:
+            raise NotImplementedError(f"training {self._model_name} with a process group is not implemented")
+
+    def _require_tc_engine(self) -> None:
+        from .blocks import dense_engine
+
+        if dense_engine() == "fp32":
+            raise NotImplementedError(f"training {self._model_name} runs on the tensor-core engine (dense_engine() == 'fp32')")
+
+    def _refuse_sharded(self, owner) -> None:
+        """owner: the embeddings (or the body) that would hold a row-sharded placement."""
+        if getattr(owner, "sharded", None) is not None:
+            raise NotImplementedError(f"training {self._model_name} with row-sharded tables is not implemented")
+
+    def _check_mlps(self, blocks) -> None:
+        for blk in blocks:
+            if not isinstance(blk, MLP) or blk.has_normalization or blk.dropout:
+                raise NotImplementedError(f"{blk.name}: training {self._model_name} supports MLPBlocks without normalization / "
+                                          "dropout")
+
+    @staticmethod
+    def _check_activations(layers: Sequence[_Dense]) -> None:
+        for l in layers:
+            if l.activation not in ("relu", "linear"):
+                raise NotImplementedError(f"{l.name}: training supports relu / linear activations, got {l.activation!r}")
 
     def _init_common(self, model, optimizer: Optimizer, batch_size: int, device, group) -> None:
         self.model, self.body, self.opt = model, model.body, optimizer
@@ -290,6 +322,17 @@ class _StepTrainer:
         self._bag_bufs: Dict[int, dict] = {}
         self._bags: Dict[int, dict] = {}
 
+    def _init_inputs(self, parts: Sequence["_ConcatInput"]) -> None:
+        """_init_tables over the features of the input parts, in order (each part learns its features' table
+        positions), and every table's (B, D) IndexedSlices buffer."""
+        feats, tables = [], []
+        for p in parts:
+            p.tidx = list(range(len(feats), len(feats) + len(p.feats)))
+            feats += p.feats
+            tables += [p.emb.feature_to_table[f] for f in p.feats]
+        self._init_tables(feats, tables)
+        self.slices = [torch.zeros((self.B, t.table.shape[1]), dtype=torch.float32, device=self.device) for t in self.tables]
+
     def _chain_buffers(self, layers: Sequence[_Dense], split_last: bool = False) -> tuple:
         """(h, h_split, dh) of a chain of Dense layers: the fp32 activations, the split operand every layer but the last
         (split_last: every layer) emits for the layer that reads it, and the pre-activation gradients."""
@@ -324,6 +367,23 @@ class _StepTrainer:
             if t.numel() != b:
                 raise ValueError(f"targets of {o.name!r} must hold {b} values, got {tuple(t.shape)}")
         return targets
+
+    def _begin_step(self, inputs, targets, sample_weight) -> tuple:
+        """What every forward_backward starts with: the loss zeroed, the batch size b checked (and the targets against it,
+        unless the task builds its own), the step's ids / slices / bags reset.  Returns (b, targets as a list,
+        sample_weight), a single output's sample_weight taken out of its list."""
+        self._loss_all.zero_()
+        b = batch_size_of(inputs)
+        if self.head is None:
+            self._check_batch(b)
+        else:
+            targets = self._check_targets(targets, b)
+        if self.H == 1 and isinstance(sample_weight, (list, tuple)):
+            sample_weight = sample_weight[0]
+        self._idx: List[Optional[torch.Tensor]] = [None] * len(self.tables)
+        self._slices = [s[:b] for s in self.slices]
+        self._bags = {}
+        return b, targets, sample_weight
 
     def _heads(self, x: torch.Tensor, targets, dx: torch.Tensor, mask_relu: bool, sample_weight, b: int) -> None:
         """The output heads' forward, loss and backward: logits, loss, dx and the head's gradients in the arena."""
@@ -382,43 +442,6 @@ class _StepTrainer:
         if dx is not None:
             self._dgrad(li0, layers[0], dh[0], dx, None)
 
-    # ---- the concatenating input block: x0 = [embedding rows | continuous columns] at their sorted-name offsets ------
-    def _input_forward(self, feats, tidx, cols: Dict[str, int], cont, inputs, x0: torch.Tensor, xs: torch.Tensor) -> None:
-        """Rows of the features `feats` (tables at positions `tidx`) and the continuous columns `cont` into x0 (b, d) at
-        the offsets `cols`, and x0's split operand xs.  One-hot features share one mm_gather_multi, a multi-hot feature is
-        pooled straight into its columns (_pool_bag).  Leaves the update's ids in _idx (None for a multi-hot feature)."""
-        ts, ids = [], []
-        for t, f in zip(tidx, feats):
-            x = get_feature(inputs, f)
-            kind = self.tables[t].lookup_kind(x)
-            if kind == "onehot":
-                ts.append(t)
-                ids.append(ops.as_index(x).reshape(-1))
-            elif self._multihot_refused:
-                raise NotImplementedError(f"feature {f!r}: training {self._multihot_refused} on multi-hot / ragged features "
-                                          "is not implemented")
-            else:
-                self._pool_bag(t, f, x, kind, x0, cols[f])
-        if ts:
-            if len({i.dtype for i in ids}) > 1:  # one launch reads one index dtype
-                ids = [i.to(torch.int64) for i in ids]
-            ops.gather_multi([self.tables[t].table for t in ts], ids, [cols[self.feats[t]] for t in ts], x0, self.oob)
-            for t, i in zip(ts, ids):
-                self._idx[t] = i
-        if cont:
-            ops.concat_columns([inputs[n] for n in cont], x0, [cols[n] for n in cont])
-        ops.split_rows(x0, out=xs)
-
-    def _input_backward(self, addends, feats, tidx, cols: Dict[str, int], fm: Optional[tuple] = None) -> None:
-        """The tables' columns of the summed (b, d) addends into each table's slice of _slices; fm = (x0, ds) adds the FM
-        term's input gradient (mm_fm_concat_backward)."""
-        slices = [(self._slices[t], cols[f]) for t, f in zip(tidx, feats)]
-        for s in range(0, len(slices), CONCAT_MAX_SLICES):
-            if fm is None:
-                ops.concat_backward(addends, slices[s:s + CONCAT_MAX_SLICES])
-            else:
-                ops.fm_concat_backward(addends, fm[0], fm[1], slices[s:s + CONCAT_MAX_SLICES])
-
     # ---- multi-hot features -----------------------------------------------------------------------------------------
     def _pool_bag(self, t: int, f: str, x, kind: str, out: torch.Tensor, col: int) -> None:
         """The forward's combiner over the rows of multi-hot feature f (table t) into out[:, col:col+D], and in _bags[t]
@@ -463,9 +486,6 @@ class _StepTrainer:
         """(ids per table, slices per table, rows per slice, scale of the dense gradient) of the last forward_backward."""
         return self._idx, self._slices, self._b, 1.0
 
-    def _apply_more(self) -> None:
-        """Variables outside the arena and the tables."""
-
     def apply_gradients(self) -> None:
         a = self.arena
         ops.opt_tick(self.hyper)
@@ -481,7 +501,8 @@ class _StepTrainer:
                 if bag is not None and bag["rows"].shape[0] > 0:  # a multi-hot table: its own call over the nnz expanded rows
                     tab = self._table_args(t, bag["apply_ids"], bag["rows"])
                     ops.sparse_rows_apply(self.opt.kind, [tab], bag["rows"].shape[0], D, self.hyper)
-        self._apply_more()
+        if self.wk is not None:
+            self.wk.apply()
         self._refresh_operands()
 
     def _refresh_operands(self) -> None:
@@ -540,26 +561,28 @@ class _StepTrainer:
         finally:
             self.model.defer_index_check(False)
 
-    def _snapshot(self):
-        return dict(w=self.arena.w.clone(), s1=None if self.arena.state1 is None else self.arena.state1.clone(),
-                    s2=None if self.arena.state2 is None else self.arena.state2.clone(), hyper=self.hyper.clone(),
-                    tables=[t.table.clone() for t in self.tables],
-                    ts1=[None if s is None else s.clone() for s in self.tstate1], ts2=[None if s is None else s.clone() for s in self.tstate2])
+    def _state(self) -> Dict[str, Optional[torch.Tensor]]:
+        """Every variable a step changes, by name: the arena's w / s1 / s2, the hyper-parameters (the step counter), each
+        table and its optimizer slots, and the wide kernel's; None where an optimizer has no such slot."""
+        a = self.arena
+        state = dict(w=a.w, s1=a.state1, s2=a.state2, hyper=self.hyper)
+        for t, (tb, s1, s2) in enumerate(zip(self.tables, self.tstate1, self.tstate2)):
+            state.update({f"table{t}": tb.table, f"table{t}/s1": s1, f"table{t}/s2": s2})
+        if self.wk is not None:
+            state.update(self.wk.state())
+        return state
+
+    def _snapshot(self) -> Dict[str, Optional[torch.Tensor]]:
+        return {k: None if v is None else v.clone() for k, v in self._state().items()}
 
     def _restore(self, snap) -> None:
-        self.arena.w.copy_(snap["w"])
+        for k, dst in self._state().items():
+            if dst is not None:
+                dst.copy_(snap[k])
         self.arena.grad.zero_()
-        if snap["s1"] is not None:
-            self.arena.state1.copy_(snap["s1"])
-        if snap["s2"] is not None:
-            self.arena.state2.copy_(snap["s2"])
-        self.hyper.copy_(snap["hyper"])
-        for t, w, s1, s2, a1, a2 in zip(self.tables, snap["tables"], snap["ts1"], snap["ts2"], self.tstate1, self.tstate2):
-            t.table.copy_(w)
-            if s1 is not None:
-                a1.copy_(s1)
-            if s2 is not None:
-                a2.copy_(s2)
+        if self.wk is not None:
+            self.wk.grad.zero_()
+        for t in self.tables:
             if t._mirror is not None and t._mirror.shape[0] == t.table.shape[0]:
                 ops.split_rows(t.table, out=t._mirror)
         self._refresh_operands()
@@ -604,8 +627,143 @@ class _StepTrainer:
         return out
 
 
+class _ConcatInput:
+    """A trainer's concatenating input block (InputBlockV2): x0 (B, d) = [embedding rows | continuous columns] at their
+    sorted-name offsets `cols`, its split operand xs and, for a caller that needs the input gradient, dx0 (None without
+    tables).  feats: the features it gathers, by default every feature of the block's embeddings, at the trainer's table
+    positions tidx (set by _init_inputs); cont: its continuous columns, by default in sorted-name order."""
+
+    def __init__(self, tr: _StepTrainer, ib, dx0: bool = False, feats: Optional[Sequence[str]] = None,
+                 cont: Optional[Sequence[str]] = None):
+        self.tr = tr
+        self.emb = ib.embeddings
+        self.cols, _, self.d = ib.layout()
+        if feats is None:
+            feats = self.emb.feature_names if self.emb is not None else []
+        if cont is None:
+            cont = sorted(ib.continuous.features) if ib.continuous is not None else []
+        self.feats, self.cont = list(feats), list(cont)
+        self.tidx: List[int] = []
+        self.oob = self.emb.counter(tr.device) if self.emb is not None else None
+        f32 = dict(dtype=torch.float32, device=tr.device)
+        self.x0 = torch.zeros((tr.B, _ld4(self.d)), **f32)
+        self.xs = torch.zeros((tr.B, 2 * ops.tc_padded_k(self.d)), dtype=torch.bfloat16, device=tr.device)
+        self.dx0 = torch.zeros((tr.B, _ld4(self.d)), **f32) if dx0 and self.feats else None
+
+    def check_multihot_widths(self, schema) -> None:
+        """Refuse a list feature whose table the multi-hot gradient expansion (mm_bag_grad_rows) cannot serve."""
+        for f in self.feats:
+            col, t = schema.get(f), self.emb.feature_to_table[f]
+            if col is not None and col.is_list and t.dim not in (16, 32, 64, 128):
+                raise NotImplementedError(f"feature {f!r}: training a multi-hot feature needs an embedding width of 16, 32, 64 "
+                                          f"or 128, got {t.dim} (give its table one with Embeddings(dim=...))")
+
+    def views(self, b: int) -> tuple:
+        """(x0, xs, dx0) on the leading b rows."""
+        return self.x0[:b, :self.d], self.xs[:b], None if self.dx0 is None else self.dx0[:b, :self.d]
+
+    def forward(self, inputs, b: int) -> tuple:
+        """The features' rows and the continuous columns into x0, and x0's split operand xs; returns views(b).  One-hot
+        features share one mm_gather_multi, a multi-hot feature is pooled straight into its columns (_pool_bag).  Leaves
+        the update's ids in the trainer's _idx (None for a multi-hot feature)."""
+        tr = self.tr
+        x0, xs, dx0 = self.views(b)
+        ts, ids = [], []
+        for t, f in zip(self.tidx, self.feats):
+            x = get_feature(inputs, f)
+            kind = tr.tables[t].lookup_kind(x)
+            if kind == "onehot":
+                ts.append(t)
+                ids.append(ops.as_index(x).reshape(-1))
+            elif tr._onehot_only:
+                raise NotImplementedError(f"feature {f!r}: training {tr._model_name} on multi-hot / ragged features "
+                                          "is not implemented")
+            else:
+                tr._pool_bag(t, f, x, kind, x0, self.cols[f])
+        if ts:
+            if len({i.dtype for i in ids}) > 1:  # one launch reads one index dtype
+                ids = [i.to(torch.int64) for i in ids]
+            ops.gather_multi([tr.tables[t].table for t in ts], ids, [self.cols[tr.feats[t]] for t in ts], x0, tr.oob)
+            for t, i in zip(ts, ids):
+                tr._idx[t] = i
+        if self.cont:
+            ops.concat_columns([inputs[n] for n in self.cont], x0, [self.cols[n] for n in self.cont])
+        ops.split_rows(x0, out=xs)
+        return x0, xs, dx0
+
+    def backward(self, addends, b: int, fm: Optional[torch.Tensor] = None) -> None:
+        """The tables' columns of the summed (b, d) addends into each table's slice of the trainer's _slices; fm: the FM
+        term's ds (b,), whose input gradient from x0 is added (mm_fm_concat_backward)."""
+        tr = self.tr
+        slices = [(tr._slices[t], self.cols[f]) for t, f in zip(self.tidx, self.feats)]
+        for s in range(0, len(slices), CONCAT_MAX_SLICES):
+            if fm is None:
+                ops.concat_backward(addends, slices[s:s + CONCAT_MAX_SLICES])
+            else:
+                ops.fm_concat_backward(addends, self.x0[:b, :self.d], fm, slices[s:s + CONCAT_MAX_SLICES])
+
+
+class _WideKernel:
+    """A wide Dense(1) (DeepFM's FM wide term, Wide&Deep's wide branch) trained outside the arena: its kernel (W, 1) stays
+    where it is, one row per category of every feature (and per continuous column), with its bias' and its own optimizer
+    slots beside it, the accumulator and representative map of mm_wide_rows_apply, and `grad` = [the continuous rows'
+    gradients..., the bias' gradient] that the head kernel accumulates.  The trainer's forward_backward leaves in `calls`
+    the step's gradient as (ids per block, rows per block, kernel offset per block, gradient values) groups."""
+
+    def __init__(self, tr: _StepTrainer, dense: _Dense, cont_offsets: Sequence[int] = ()):
+        self.tr, self.dense = tr, dense
+        self.cont_offsets = list(cont_offsets)
+        opt = tr.opt
+        f32 = dict(dtype=torch.float32, device=tr.device)
+        W = dense.kernel.numel()
+        nb = 1 if dense.bias is not None else 0
+        self.wk_s1 = torch.full((W,), opt.initial_accumulator_value, **f32) if opt.slots >= 1 else None
+        self.wk_s2 = torch.zeros(W, **f32) if opt.slots >= 2 else None
+        self.wb_s1 = torch.full((nb,), opt.initial_accumulator_value, **f32) if opt.slots >= 1 and nb else None
+        self.wb_s2 = torch.zeros(nb, **f32) if opt.slots >= 2 and nb else None
+        self.acc = torch.zeros(W, **f32)
+        self.rep = ops.fill_i32(torch.empty(W, dtype=torch.int32, device=tr.device), INT32_MAX)
+        self.grad = torch.zeros(len(self.cont_offsets) + nb, **f32)
+        self.calls: List[tuple] = []
+
+    def state(self) -> Dict[str, Optional[torch.Tensor]]:
+        return {"wide/kernel": self.dense.kernel, "wide/bias": self.dense.bias, "wide/kernel/s1": self.wk_s1,
+                "wide/kernel/s2": self.wk_s2, "wide/bias/s1": self.wb_s1, "wide/bias/s2": self.wb_s2}
+
+    def apply(self) -> None:
+        """One mm_wide_rows_apply per group of `calls`; the continuous rows and the bias take their step with the first."""
+        wk, bias = self.dense.kernel.reshape(-1), self.dense.bias
+        for i, (ids, rows, offs, g) in enumerate(self.calls):
+            first = i == 0
+            ops.wide_rows_apply(self.tr.opt.kind, wk, self.wk_s1, self.wk_s2, ids, rows, offs, g, self.acc, self.rep,
+                                self.cont_offsets if first else [], self.grad if first and self.grad.numel() else None,
+                                bias.reshape(-1) if first and bias is not None else None, self.wb_s1 if first else None,
+                                self.wb_s2 if first else None, self.tr.hyper)
+
+    def gradients(self) -> Dict[str, torch.Tensor]:
+        """The kernel's gradient (W, 1) and the bias' (after forward_backward, before apply_gradients), assembled in float64
+        from `calls` and `grad` — for parity tests."""
+        W = self.dense.kernel.numel()
+        g = torch.zeros(W, dtype=torch.float64, device=self.tr.device)
+        for ids, rows, offs, vals in self.calls:
+            v = vals.double()
+            for i, r, o in zip(ids, rows, offs):
+                i = ops.widen_index(i).reshape(-1).long()
+                ok = (i >= 0) & (i < r)
+                g.index_add_(0, i[ok] + o, v[ok])
+        nc = len(self.cont_offsets)
+        for c, o in enumerate(self.cont_offsets):
+            g[o] += self.grad[c].double()
+        out = {"wide/kernel": g.reshape(W, 1)}
+        if self.dense.bias is not None:
+            out["wide/bias"] = self.grad[nc:].double().clone()
+        return out
+
+
 class DLRMTrainer(_StepTrainer):
     """Static-buffer training step of a DLRM RankingModel at one batch size."""
+
+    _model_name = "DLRMModel"
 
     def __init__(self, model, optimizer: Optimizer, batch_size: int, device=None, group=None):
         from .models import BinaryOutput, ParallelOutputs
@@ -617,20 +775,15 @@ class DLRMTrainer(_StepTrainer):
             raise NotImplementedError("train_step needs BinaryOutput / RegressionOutput heads or an OutputBlock of them")
         if group is not None and isinstance(model.prediction, ParallelOutputs):
             raise NotImplementedError("training several outputs with a process group is not implemented")
-        if body.sharded is not None:
-            raise NotImplementedError("training with row-sharded tables is not implemented (forward only)")
+        self._refuse_sharded(body)
         if not body.can_emit_split():
             raise NotImplementedError("training needs <= 32 interaction features and embedding_dim in {16, 32, 64, 128}")
         self._init_common(model, optimizer, batch_size, device, group)
-        for blk in (body.bottom_block, body.top_block):
-            if not isinstance(blk, MLP) or blk.has_normalization or blk.dropout:
-                raise NotImplementedError("training supports MLPBlock towers without normalization / dropout")
+        self._check_mlps((body.bottom_block, body.top_block))
         self.bottom = body.bottom_block.dense_layers
         self.top = body.top_block.dense_layers
         self._init_heads()
-        for l in self.bottom + self.top:
-            if l.activation not in ("relu", "linear"):
-                raise NotImplementedError(f"{l.name}: training supports relu / linear tower activations, got {l.activation!r}")
+        self._check_activations(self.bottom + self.top)
         if self.head.input_dim > 256:
             raise NotImplementedError("the output layer's input must be <= 256 wide")
         self._init_dense(self.bottom + self.top, [self.head])
@@ -709,11 +862,9 @@ class DLRMTrainer(_StepTrainer):
         for a single output); sample_weight: one (b,) tensor for every output, or a list with one per output."""
         nb = len(self.bottom)
         D = self.D
-        self._loss_all.zero_()
+        b, targets, sample_weight = self._begin_step(inputs, targets, sample_weight)
         cont = self.body.continuous(inputs)
         pieces = [cont[k] for k in sorted(cont)]
-        b = int(pieces[0].shape[0])
-        targets = self._check_targets(targets, b)
         h, t_, dt, dh = ([x[:b] for x in bufs] for bufs in (self.h, self.t, self.dt, self.dh))
         h_split, x0_split, A_split = [x[:b] for x in self.h_split], self.x0_split[:b], self.A_split[:b]
         ops.concat_split(pieces, out=x0_split)  # the concatenated continuous columns exist only as this operand
@@ -742,7 +893,6 @@ class DLRMTrainer(_StepTrainer):
         # -- top tower backward: its input exists as fp32 only without operand_rows
         self._chain_backward(nb, self.top, t_, dt, (A_split, self.OW) if A_view is None else A_view, dA_view)
         # -- interaction + lookup backward
-        self._slices = [s[:b] for s in self.slices]
         if self.operand_rows:
             ops.dlrm_interact_backward(mirrors, idx, tslots, rows, D, h_split[-1], bslot, dA_view,
                                        self._slices, dh[-1], mask_bottom=self.bottom[-1].activation == "relu", operand_rows=True)
@@ -783,7 +933,8 @@ class DCNTrainer(_StepTrainer):
     update    mm_opt_tick, mm_dense_apply over the arena [cross layers, deep layers, head], one mm_sparse_rows_apply per
               distinct embedding width, mm_split_weights refresh of the operand copies the model's forward reads."""
 
-    _multihot_refused = "DCNModel"
+    _model_name = "DCNModel"
+    _onehot_only = True
 
     def __init__(self, model, optimizer: Optimizer, batch_size: int, device=None, group=None):
         from .blocks import Cross
@@ -794,36 +945,26 @@ class DCNTrainer(_StepTrainer):
             raise NotImplementedError("DCNTrainer trains DCNModel bodies")
         if not isinstance(model.prediction, (BinaryOutput, ParallelOutputs)):
             raise NotImplementedError("train_step needs BinaryOutput / RegressionOutput heads or an OutputBlock of them")
-        if group is not None:
-            raise NotImplementedError("training DCNModel with a process group is not implemented")
+        self._refuse_group(group)
         cross_layers = body.cross.cross_layers
         for c in cross_layers:
             if not isinstance(c, Cross) or c.low_rank_dim is not None:
                 raise NotImplementedError(f"{c.name}: training a low-rank cross layer (low_rank_dim) is not implemented")
         if body.cross.inputs is not None:
             raise NotImplementedError("training a CrossBlock with its own `inputs` block is not implemented")
-        deep = body.deep
-        if not isinstance(deep, MLP) or deep.has_normalization or deep.dropout:
-            raise NotImplementedError("training DCNModel supports a deep_block without normalization / dropout")
+        self._check_mlps([body.deep])
         ib = body.input_block
         if getattr(ib, "aggregation", "concat") != "concat":
             raise NotImplementedError("training DCNModel needs the concatenating input block")
         self._init_common(model, optimizer, batch_size, device, None)
         self.stacked = bool(body.stacked)
         self.cross = [c.dense for c in cross_layers]
-        self.deep = deep.dense_layers
+        self.deep = body.deep.dense_layers
         self._init_heads()
-        for l in self.deep:
-            if l.activation not in ("relu", "linear"):
-                raise NotImplementedError(f"{l.name}: training supports relu / linear deep-layer activations, got {l.activation!r}")
-
-        # ---- input block layout and tables
-        emb = ib.embeddings
-        self.cols, widths, d = ib.layout()
-        self.d = d
-        feats = list(emb.feature_names) if emb is not None else []
-        self._init_tables(feats, [emb.feature_to_table[f] for f in feats])
-        self.cont = sorted(ib.continuous.features) if ib.continuous is not None else []
+        self._check_activations(self.deep)
+        self.inp = _ConcatInput(self, ib)
+        self._init_inputs([self.inp])
+        d = self.inp.d
 
         self._init_dense(self.cross + self.deep, [self.head])
         # every layer needs its input gradient (x0 is the tables' rows); mm_cross_backward writes the split of a cross
@@ -833,22 +974,20 @@ class DCNTrainer(_StepTrainer):
 
         # ---- activations and gradients (fp32 (B, d) buffers with a row stride that is a multiple of 4)
         B = self.B
-        self.ld = _ld4(d)
         f32 = dict(dtype=torch.float32, device=self.device)
         bf = dict(dtype=torch.bfloat16, device=self.device)
         Kp = ops.tc_padded_k(d)
 
         def mat():
-            return torch.zeros((B, self.ld), **f32)
+            return torch.zeros((B, _ld4(d)), **f32)
 
-        self.x0 = mat()
-        self.xs = [torch.zeros((B, 2 * Kp), **bf) for _ in range(L + (1 if self.stacked else 0))]  # operands of x_0 .. x_L
+        # operands of x_0 (the input block's) .. x_L
+        self.xs = [self.inp.xs] + [torch.zeros((B, 2 * Kp), **bf) for _ in range(L - 1 + (1 if self.stacked else 0))]
         self.z = [mat() for _ in range(L)]
         self.xf = [mat() for _ in range(min(L, 2))]  # fp32 x_1 .. x_L, alternating (only the residual of the next layer)
         self.h, self.h_split, self.dh = self._chain_buffers(self.deep)
         self.g, self.p, self.acc, self.dz = mat(), mat(), mat(), mat()
         self.dz_split = torch.zeros((B, 2 * Kp), **bf)
-        self.slices = [torch.zeros((B, tb.table.shape[1]), **f32) for tb in self.tables]
         if not self.stacked:
             # the head reads [cross | deep] (or [deep | cross]): x_L and the deep output are written straight into it
             u = self.deep[-1].units
@@ -870,19 +1009,14 @@ class DCNTrainer(_StepTrainer):
             self._head_dz = torch.zeros((B, self.H), **f32)
             self._head_eye = torch.eye(self.H, **f32)
         self._init_loss(B)
-        self.oob = emb.counter(self.device) if emb is not None else None
+        self.oob = self.inp.oob
 
     def forward_backward(self, inputs: Dict[str, torch.Tensor], targets, sample_weight=None) -> None:
         """Forward (activations saved), loss and backward: fills the gradient arena and the IndexedSlices.  Batches smaller
         than the compiled size run in the leading rows of the same buffers."""
         a = self.arena
-        d, L = self.d, len(self.cross)
-        self._loss_all.zero_()
-        b = batch_size_of(inputs)
-        targets = self._check_targets(targets, b)
-        tidx = range(len(self.tables))
-        self._idx: List[Optional[torch.Tensor]] = [None] * len(self.tables)
-        self._slices = [s[:b] for s in self.slices]
+        d, L = self.inp.d, len(self.cross)
+        b, targets, sample_weight = self._begin_step(inputs, targets, sample_weight)
 
         def v(t):
             return t[:b]
@@ -890,9 +1024,8 @@ class DCNTrainer(_StepTrainer):
         def vd(t):
             return t[:b, :d]
 
-        # -- input block: x0 = [embeddings | continuous] in sorted-name order
-        x0 = vd(self.x0)
-        self._input_forward(self.feats, tidx, self.cols, self.cont, inputs, x0, v(self.xs[0]))
+        # -- input block: x0 = [embeddings | continuous] in sorted-name order, its operand xs[0]
+        x0, _, _ = self.inp.forward(inputs, b)
         # -- cross network
         x = x0
         cat = v(self.cat) if not self.stacked else None
@@ -932,7 +1065,7 @@ class DCNTrainer(_StepTrainer):
             self._dgrad(l, self.cross[l], dz, p, None, dz_split=dzs)
         # -- input block backward: dx0 = g_1 + p_0 + acc (+ the deep branch's input gradient), the tables' columns only
         addends = [g, p, acc] + ([vd(self.ddeep)] if not self.stacked else [])
-        self._input_backward(addends, self.feats, tidx, self.cols)
+        self.inp.backward(addends, b)
         self._b = b
 
     def _dcn_heads(self, x: torch.Tensor, targets, dx: torch.Tensor, mask_relu: bool, sample_weight, b: int) -> None:
@@ -967,8 +1100,9 @@ class TwoTowerTrainer(_StepTrainer):
     update    mm_opt_tick, mm_dense_apply over ONE arena holding both towers, one mm_sparse_rows_apply per embedding width
               (and per multi-hot table), mm_split_weights refresh of the operand copies the model's forward reads."""
 
+    _model_name = "a TwoTowerModel"
+
     def __init__(self, model, optimizer: Optimizer, batch_size: int, device=None, group=None):
-        from .blocks import dense_engine
         from .models import RetrievalModel
         from .retrieval import InBatchSampler, ItemRetrievalTask, L2Norm, TwoTowerBlock
 
@@ -984,10 +1118,8 @@ class TwoTowerTrainer(_StepTrainer):
             raise NotImplementedError("training supports the in-batch sampler only (other samplers are not implemented)")
         if getattr(task, "logq_sampling_correction", False):
             raise NotImplementedError("the logQ sampling correction is not implemented in the training step")
-        if group is not None:
-            raise NotImplementedError("training a TwoTowerModel with a process group (data parallel) is not implemented")
-        if dense_engine() == "fp32":
-            raise NotImplementedError("training a TwoTowerModel runs on the tensor-core engine (dense_engine() == 'fp32')")
+        self._refuse_group(group)
+        self._require_tc_engine()
         body = model.body
         if body.post is not None and not isinstance(body.post, L2Norm):
             raise NotImplementedError(f"post block {type(body.post).__name__}: only post='l2-norm' is implemented in training")
@@ -999,25 +1131,12 @@ class TwoTowerTrainer(_StepTrainer):
         self.item_id = scorer.item_id_feature_name
         self.l2 = body.post is not None
         self.H = 1
-        self.towers = []
-        feats_all, tables = [], []
+        self.towers, self.inps = [], []  # per tower: its layers and buffers, its input block
         for tb in (body.query, body.item):
-            mlp = tb.mlp
-            if not isinstance(mlp, MLP) or mlp.has_normalization or mlp.dropout:
-                raise NotImplementedError(f"{tb.name} tower: training supports MLPBlock towers without normalization / dropout")
-            for l in mlp.dense_layers:
-                if l.activation not in ("relu", "linear"):
-                    raise NotImplementedError(f"{l.name}: training supports relu / linear tower activations, got {l.activation!r}")
-            ib = tb.inputs
-            cols, widths, d = ib.layout()
-            emb = ib.embeddings
-            feats = list(emb.feature_names) if emb is not None else []
-            first = len(tables)
-            feats_all += feats
-            tables += [emb.feature_to_table[f] for f in feats]
-            cont = sorted(ib.continuous.features) if ib.continuous is not None else []
-            self.towers.append(dict(name=tb.name, layers=mlp.dense_layers, cols=cols, d=d, feats=feats, tidx=list(range(first, len(tables))),
-                                    cont=cont, oob=emb.counter(self.device) if emb is not None else None))
+            self._check_mlps([tb.mlp])
+            self._check_activations(tb.mlp.dense_layers)
+            self.towers.append(dict(name=tb.name, layers=tb.mlp.dense_layers))
+            self.inps.append(_ConcatInput(self, tb.inputs, dx0=True))  # a tower without tables has nothing below x0
         out_w = {t["layers"][-1].units for t in self.towers}
         if len(out_w) != 1:
             raise ValueError(f"the query and item towers must end in the same width, got {sorted(out_w)}")
@@ -1025,13 +1144,13 @@ class TwoTowerTrainer(_StepTrainer):
         if ops.tc_padded_k(self.D) > 128:
             raise NotImplementedError(f"tower output width {self.D}: the in-batch soft-max kernels take up to 128")
 
-        self._init_tables(feats_all, tables)
+        self._init_inputs(self.inps)
         self._init_dense([l for t in self.towers for l in t["layers"]], [])
         first_layer = {}
         li = 0
-        for t in self.towers:
+        for t, inp in zip(self.towers, self.inps):
             t["li0"] = li
-            first_layer[li] = bool(t["feats"])  # the first layer needs its input gradient only when the tower has tables
+            first_layer[li] = bool(inp.feats)  # the first layer needs its input gradient only when the tower has tables
             li += len(t["layers"])
         self._init_wide(lambda i: first_layer.get(i, True))
 
@@ -1040,15 +1159,9 @@ class TwoTowerTrainer(_StepTrainer):
         f32 = dict(dtype=torch.float32, device=self.device)
         bf = dict(dtype=torch.bfloat16, device=self.device)
         for t in self.towers:
-            d = t["d"]
-            t["ld"] = _ld4(d)
-            t["x0"] = torch.zeros((B, t["ld"]), **f32)
-            t["xs"] = torch.zeros((B, 2 * ops.tc_padded_k(d)), **bf)
             t["h"], t["h_split"], t["dh"] = self._chain_buffers(t["layers"])
-            t["dx0"] = torch.zeros((B, t["ld"]), **f32) if t["feats"] else None
             t["y"] = torch.zeros((B, self.D), **f32) if self.l2 else None  # the normalised output
             t["split"] = torch.zeros((B, 2 * ops.tc_padded_k(self.D)), **bf)
-        self.slices = [torch.zeros((B, tb.table.shape[1]), **f32) for tb in self.tables]
         self.pos_logit = torch.zeros(B, **f32)
         self.stats = torch.zeros((B, 3), **f32)
         ws = max(ops.catalog_workspace_bytes(min(128 * m, B), min(128 * m, B)) for m in range(1, (B + 127) // 128 + 1))
@@ -1057,7 +1170,7 @@ class TwoTowerTrainer(_StepTrainer):
         self._init_loss(B)
         self.logits = self.stats  # [max, log-sum-exp, positive logit] of every row of the last step
         # one counter for both towers (every gather receives it), so check_indices sees every table
-        self.oob = next((t["oob"] for t in self.towers if t["oob"] is not None), None)
+        self.oob = next((p.oob for p in self.inps if p.oob is not None), None)
 
     # ---- the parts of _StepTrainer that concern output heads do not apply: the retrieval task builds its own targets
     def capture(self, inputs: Dict[str, torch.Tensor], targets=None, clone: bool = True) -> None:
@@ -1100,19 +1213,17 @@ class TwoTowerTrainer(_StepTrainer):
             c = self._inv_b[b] = torch.full((1,), 1.0 / b, dtype=torch.float32, device=self.device)
         return c
 
-    def _tower_forward(self, tw: dict, inputs, b: int) -> torch.Tensor:
-        d = tw["d"]
-        xs = tw["xs"][:b]
-        self._input_forward(tw["feats"], tw["tidx"], tw["cols"], tw["cont"], inputs, tw["x0"][:b, :d], xs)
+    def _tower_forward(self, tw: dict, inp: _ConcatInput, inputs, b: int) -> torch.Tensor:
+        _, xs, _ = inp.forward(inputs, b)
         h = [x[:b] for x in tw["h"]]
-        self._chain_forward(xs, d, tw["li0"], tw["layers"], h, [x[:b] for x in tw["h_split"]])
+        self._chain_forward(xs, inp.d, tw["li0"], tw["layers"], h, [x[:b] for x in tw["h_split"]])
         out = h[-1]
         if self.l2:
             out = ops.l2_normalize(out, out=tw["y"][:b])
         ops.split_rows(out, out=tw["split"][:b])
         return out
 
-    def _tower_backward(self, tw: dict, dout: torch.Tensor, b: int) -> None:
+    def _tower_backward(self, tw: dict, inp: _ConcatInput, dout: torch.Tensor, b: int) -> None:
         """dout: gradient of the tower's (normalised) output, overwritten by the pre-activation gradient of the last layer."""
         h, dh, layers = [x[:b] for x in tw["h"]], [x[:b] for x in tw["dh"]], tw["layers"]
         if self.l2:
@@ -1120,24 +1231,18 @@ class TwoTowerTrainer(_StepTrainer):
         if layers[-1].activation == "relu":
             ops.relu_mask(dout, h[-1])
         dh[-1] = dout
-        dx0 = tw["dx0"][:b, :tw["d"]] if tw["dx0"] is not None else None  # a tower without tables has nothing below it
-        self._chain_backward(tw["li0"], layers, h, dh, (tw["xs"][:b], tw["d"]), dx0)
+        _, xs, dx0 = inp.views(b)
+        self._chain_backward(tw["li0"], layers, h, dh, (xs, inp.d), dx0)
         if dx0 is not None:
-            self._input_backward([dx0], tw["feats"], tw["tidx"], tw["cols"])
+            inp.backward([dx0], b)
 
     def forward_backward(self, inputs: Dict[str, torch.Tensor], targets=None, sample_weight=None) -> None:
         """Forward (activations saved), in-batch soft-max cross-entropy and backward: fills the gradient arena and the
         IndexedSlices.  `targets` are ignored: the task's target is the positive on column 0 of every row."""
         if sample_weight is not None and not (isinstance(sample_weight, (list, tuple)) and all(s is None for s in sample_weight)):
             raise NotImplementedError("sample_weight is not implemented in the two-tower training step")
-        b = batch_size_of(inputs)
-        self._check_batch(b)
-        self._loss_all.zero_()
-        self._idx: List[Optional[torch.Tensor]] = [None] * len(self.tables)
-        self._bags = {}
-        self._slices = [s[:b] for s in self.slices]
-        q = self._tower_forward(self.towers[0], inputs, b)
-        it = self._tower_forward(self.towers[1], inputs, b)
+        b, _, _ = self._begin_step(inputs, targets, sample_weight)
+        q, it = (self._tower_forward(tw, inp, inputs, b) for tw, inp in zip(self.towers, self.inps))
         qs, its = self.towers[0]["split"][:b], self.towers[1]["split"][:b]
         ids = ops.as_index(inputs[self.item_id]).reshape(-1) if self.downscore else None  # packed host-batch ids widened
         T = self.temperature
@@ -1149,8 +1254,8 @@ class TwoTowerTrainer(_StepTrainer):
         ops.inbatch_softmax_ce_backward(qs, its, self.D, self.stats[:b], q, it, self._scale(b), dq, di, di, loss=self._loss_all[:1],
                                         pos_ids=ids, neg_ids=ids, downscore=self.downscore, false_neg_score=self.false_neg_score,
                                         temperature=T)
-        for tw, dout in zip(self.towers, (dq, di)):
-            self._tower_backward(tw, dout, b)
+        for tw, inp, dout in zip(self.towers, self.inps, (dq, di)):
+            self._tower_backward(tw, inp, dout, b)
         self._bag_grads()
         self._b = b
 
@@ -1170,10 +1275,10 @@ class DeepFMTrainer(_StepTrainer):
               and bias by the dense rule), mm_split_weights refresh of the operand copies the model's forward reads.
     The wide kernel (one row per category of every feature) stays where it is, its optimizer slots beside it."""
 
-    _multihot_refused = "DeepFMModel"
+    _model_name = "DeepFMModel"
+    _onehot_only = True
 
     def __init__(self, model, optimizer: Optimizer, batch_size: int, device=None, group=None):
-        from .blocks import dense_engine
         from .models import BinaryOutput, DeepFMBody
 
         body = model.body
@@ -1181,150 +1286,83 @@ class DeepFMTrainer(_StepTrainer):
             raise NotImplementedError("DeepFMTrainer trains DeepFMModel bodies")
         if not isinstance(model.prediction, BinaryOutput):
             raise NotImplementedError("training DeepFMModel needs one BinaryOutput or RegressionOutput")
-        if group is not None:
-            raise NotImplementedError("training DeepFMModel with a process group is not implemented")
-        if dense_engine() == "fp32":
-            raise NotImplementedError("training DeepFMModel runs on the tensor-core engine (dense_engine() == 'fp32')")
+        self._refuse_group(group)
+        self._require_tc_engine()
         ib, fm = body.input_block, body.fm
-        emb = ib.embeddings
-        if getattr(emb, "sharded", None) is not None:
-            raise NotImplementedError("training DeepFMModel with row-sharded tables is not implemented")
-        if fm.embeddings is not emb:
+        self._refuse_sharded(ib.embeddings)
+        if fm.embeddings is not ib.embeddings:
             raise NotImplementedError("training DeepFMModel needs the FM term to read the input block's tables")
-        for blk in (body.deep, body.deep_logit):
-            if not isinstance(blk, MLP) or blk.has_normalization or blk.dropout:
-                raise NotImplementedError("training DeepFMModel supports deep / deep-logit MLPBlocks without normalization / dropout")
+        self._check_mlps((body.deep, body.deep_logit))
         self._init_common(model, optimizer, batch_size, device, None)
         self._init_heads()
         self.chain = body.deep.dense_layers + body.deep_logit.dense_layers[:-1]  # tower layers run by mm_dense_tc
         self.last = body.deep_logit.dense_layers[-1]  # Dense(1), fused into the head kernel
-        for l in self.chain + [self.last]:
-            if l.activation not in ("relu", "linear"):
-                raise NotImplementedError(f"{l.name}: training supports relu / linear deep activations, got {l.activation!r}")
+        self._check_activations(self.chain + [self.last])
         self.U = self.chain[-1].units
         if self.U > 512:
             raise NotImplementedError(f"{self.chain[-1].name}: the head kernel reads at most 512 units of the last deep layer, got {self.U}")
 
-        # ---- input block layout, tables, wide kernel
-        self.cols, widths, d = ib.layout()
-        self.d = d
+        # ---- input block, tables (the FM term's features, in its order), wide kernel
         if len(fm.cat_names) > 32 or len(fm.cont_names) > 32:
             raise NotImplementedError("the DeepFM head kernel takes up to 32 categorical and 32 continuous features")
-        self._init_tables(fm.cat_names, [emb.feature_to_table[f] for f in fm.cat_names])
+        self.inp = _ConcatInput(self, ib, dx0=True, feats=fm.cat_names, cont=fm.cont_names)
+        self._init_inputs([self.inp])
         self.D = fm.dim
-        self.cont = list(fm.cont_names)
-        self.wk = fm.wide  # _Dense(1) over [one-hot | continuous]: kernel (W, 1), bias (1,)
         self.woff = [fm.wide_offsets[f] for f in self.feats]
-        self.coff = [fm.wide_offsets[n] for n in self.cont]
+        self.coff = [fm.wide_offsets[n] for n in self.inp.cont]
 
         # the step reads self.last as fp32 (the head kernel); its operand copy is what the model's forward reads
         self._init_dense(self.chain + [self.last], [self.head])
         n = len(self.chain)
         self._init_wide(lambda li: li < n)
-        f32 = dict(dtype=torch.float32, device=self.device)
-        W = self.wk.kernel.numel()
-        self.wk_s1 = torch.full((W,), optimizer.initial_accumulator_value, **f32) if optimizer.slots >= 1 else None
-        self.wk_s2 = torch.zeros(W, **f32) if optimizer.slots >= 2 else None
-        nb = 1 if self.wk.bias is not None else 0
-        self.wb_s1 = torch.full((nb,), optimizer.initial_accumulator_value, **f32) if optimizer.slots >= 1 and nb else None
-        self.wb_s2 = torch.zeros(nb, **f32) if optimizer.slots >= 2 and nb else None
-        self.wk_acc = torch.zeros(W, **f32)
-        self.wk_rep = ops.fill_i32(torch.empty(W, dtype=torch.int32, device=self.device), INT32_MAX)
-        self.wk_grad = torch.zeros(len(self.cont) + nb, **f32)  # [continuous rows..., bias]
+        self.wk = _WideKernel(self, fm.wide, self.coff)  # _Dense(1) over [one-hot | continuous]: kernel (W, 1), bias (1,)
 
         # ---- activations and gradients
         B = self.B
-        self.ld = _ld4(d)
-        self.x0 = torch.zeros((B, self.ld), **f32)
-        self.xs = torch.zeros((B, 2 * ops.tc_padded_k(d)), dtype=torch.bfloat16, device=self.device)
         self.h, self.h_split, self.dh = self._chain_buffers(self.chain)
-        self.dx0 = torch.zeros((B, self.ld), **f32)
-        self.ds = torch.zeros(B, **f32)
-        self.slices = [torch.zeros((B, self.D), **f32) for _ in self.tables]
+        self.ds = torch.zeros(B, dtype=torch.float32, device=self.device)
         self._init_loss(B)
-        self.oob = emb.counter(self.device)
+        self.oob = self.inp.oob
 
     def forward_backward(self, inputs: Dict[str, torch.Tensor], targets, sample_weight=None) -> None:
         """Forward (activations saved), loss and backward: fills the gradient arena, the IndexedSlices of the tables, ds (the
         wide kernel's gradient values) and the gradients of the wide kernel's continuous rows and bias.  Batches smaller
         than the compiled size run in the leading rows of the same buffers."""
         a = self.arena
-        d, n = self.d, len(self.chain)
-        self._loss_all.zero_()
-        b = batch_size_of(inputs)
-        targets = self._check_targets(targets, b)
-        if isinstance(sample_weight, (list, tuple)):
-            sample_weight = sample_weight[0]
-        tidx = range(len(self.tables))
-        self._idx: List[Optional[torch.Tensor]] = [None] * len(self.tables)
-        self._slices = [s[:b] for s in self.slices]
-        x0, xs = self.x0[:b, :d], self.xs[:b]
-        self._input_forward(self.feats, tidx, self.cols, self.cont, inputs, x0, xs)
+        d, n = self.inp.d, len(self.chain)
+        b, targets, sample_weight = self._begin_step(inputs, targets, sample_weight)
+        x0, xs, dx0 = self.inp.forward(inputs, b)
         # the head kernel and the updates read the ids at the width they came in (packed host-batch ids are not widened)
         fidx = [ops.fused_ids(get_feature(inputs, f)) for f in self.feats]
-        conts = [inputs[c] for c in self.cont]
+        conts = [inputs[c] for c in self.inp.cont]
         h, dh = [t[:b] for t in self.h], [t[:b] for t in self.dh]
         self._chain_forward(xs, d, 0, self.chain, h, [t[:b] for t in self.h_split])
         # -- FM + wide + deep logit + output layer + loss, forward and backward
         hi = len(a.layers) - 1
         ds = self.ds[:b]
-        nc = len(self.cont)
+        nc = len(self.coff)
+        rows = [tb.table.shape[0] for tb in self.tables]
+        wk, wg = self.wk.dense, self.wk.grad
         ops.deepfm_head_fwd_bwd(
-            x0, [self.cols[f] for f in self.feats], self.D, fidx, [tb.table.shape[0] for tb in self.tables], self.woff, conts,
-            self.coff, self.wk.kernel.reshape(-1), self.wk.bias, h[-1], self.chain[-1].activation == "relu", self.last.kernel.reshape(-1),
+            x0, [self.inp.cols[f] for f in self.feats], self.D, fidx, rows, self.woff, conts,
+            self.coff, wk.kernel.reshape(-1), wk.bias, h[-1], self.chain[-1].activation == "relu", self.last.kernel.reshape(-1),
             self.last.bias, self.last.activation, self.head.kernel.reshape(-1), self.head.bias, self.losses[0], targets[0].reshape(-1),
             sample_weight, self.logits[:b], self._loss_all, ds, dh[-1], dw_out=a.view(a.grad, hi, "kernel"), db_out=a.view(a.grad, hi, "bias"),
             dw_dl=a.view(a.grad, n, "kernel"), db_dl=a.view(a.grad, n, "bias"),
-            d_wide_bias=self.wk_grad[nc:] if self.wk.bias is not None else None, d_cont=self.wk_grad[:nc] if nc else None, oob=self.oob)
+            d_wide_bias=wg[nc:] if wk.bias is not None else None, d_cont=wg[:nc] if nc else None, oob=self.oob)
         # -- deep tower backward down to dx0
-        dx0 = self.dx0[:b, :d]
         self._chain_backward(0, self.chain, h, dh, (xs, d), dx0)
         # -- input block backward: the deep tower's dx0 + the FM term, the tables' columns only
-        self._input_backward([dx0], self.feats, tidx, self.cols, fm=(x0, ds))
+        self.inp.backward([dx0], b, fm=ds)
+        self.wk.calls = [(fidx, rows, self.woff, ds)]  # one gradient value per sample for every feature's block
         self._fidx, self._b = fidx, b
 
     def _gradients_to_apply(self) -> tuple:
         return self._fidx, self._slices, self._b, 1.0
 
-    def _apply_more(self) -> None:
-        ops.wide_rows_apply(self.opt.kind, self.wk.kernel.reshape(-1), self.wk_s1, self.wk_s2, self._fidx,
-                            [tb.table.shape[0] for tb in self.tables], self.woff, self.ds[:self._b], self.wk_acc, self.wk_rep, self.coff,
-                            self.wk_grad if self.wk_grad.numel() else None, None if self.wk.bias is None else self.wk.bias.reshape(-1),
-                            self.wb_s1, self.wb_s2, self.hyper)
-
     def wide_gradients(self) -> Dict[str, torch.Tensor]:
-        """The wide kernel's gradient (W,) and its bias' (after forward_backward, before apply_gradients), assembled in float64
-        from ds, the ids and the continuous rows' sums — for parity tests."""
-        W = self.wk.kernel.numel()
-        g = torch.zeros(W, dtype=torch.float64, device=self.device)
-        ds = self.ds[:self._b].double()
-        for f, ids, tb in zip(self.feats, self._fidx, self.tables):
-            i = ops.widen_index(ids).reshape(-1).long()
-            ok = (i >= 0) & (i < tb.table.shape[0])
-            g.index_add_(0, i[ok] + self.woff[self.feats.index(f)], ds[ok])
-        nc = len(self.cont)
-        for c in range(nc):
-            g[self.coff[c]] += self.wk_grad[c].double()
-        out = {"wide/kernel": g.reshape(W, 1)}
-        if self.wk.bias is not None:
-            out["wide/bias"] = self.wk_grad[nc:].double().clone()
-        return out
-
-    def _snapshot(self):
-        snap = super()._snapshot()
-        snap.update(wk=self.wk.kernel.clone(), wb=None if self.wk.bias is None else self.wk.bias.clone(),
-                    wk_s=[None if s is None else s.clone() for s in (self.wk_s1, self.wk_s2, self.wb_s1, self.wb_s2)])
-        return snap
-
-    def _restore(self, snap) -> None:
-        super()._restore(snap)
-        self.wk.kernel.copy_(snap["wk"])
-        if snap["wb"] is not None:
-            self.wk.bias.copy_(snap["wb"])
-        for dst, src in zip((self.wk_s1, self.wk_s2, self.wb_s1, self.wb_s2), snap["wk_s"]):
-            if src is not None:
-                dst.copy_(src)
-        self.wk_grad.zero_()
+        """The wide kernel's gradient (W, 1) and its bias' (after forward_backward, before apply_gradients) — for parity tests."""
+        return self.wk.gradients()
 
 
 class WideAndDeepTrainer(_StepTrainer):
@@ -1343,8 +1381,9 @@ class WideAndDeepTrainer(_StepTrainer):
     The wide kernel stays where it is, its optimizer slots beside it.  Fixed-length list features can be captured into one
     CUDA graph; ragged ones train eagerly (their number of ids changes from batch to batch)."""
 
+    _model_name = "WideAndDeepModel"
+
     def __init__(self, model, optimizer: Optimizer, batch_size: int, device=None, group=None):
-        from .blocks import dense_engine
         from .models import BinaryOutput, WideAndDeepBody
 
         body = model.body
@@ -1352,10 +1391,8 @@ class WideAndDeepTrainer(_StepTrainer):
             raise NotImplementedError("WideAndDeepTrainer trains WideAndDeepModel bodies")
         if not isinstance(model.prediction, BinaryOutput):
             raise NotImplementedError("training WideAndDeepModel needs one BinaryOutput or RegressionOutput")
-        if group is not None:
-            raise NotImplementedError("training WideAndDeepModel with a process group is not implemented")
-        if dense_engine() == "fp32":
-            raise NotImplementedError("training WideAndDeepModel runs on the tensor-core engine (dense_engine() == 'fp32')")
+        self._refuse_group(group)
+        self._require_tc_engine()
         if body.regularized:
             raise NotImplementedError("training WideAndDeepModel with deep / wide regularizers is not implemented")
         if body.wide is not None and getattr(body.wide, "dropout", None):
@@ -1363,60 +1400,30 @@ class WideAndDeepTrainer(_StepTrainer):
         ib = body.input_block
         self.deep = ib is not None
         if self.deep:
-            if getattr(ib.embeddings, "sharded", None) is not None:
-                raise NotImplementedError("training WideAndDeepModel with row-sharded tables is not implemented")
-            for blk in (body.deep, body.deep_logit):
-                if not isinstance(blk, MLP) or blk.has_normalization or blk.dropout:
-                    raise NotImplementedError("training WideAndDeepModel supports a deep_block without normalization / dropout "
-                                              "(and no deep_dropout)")
+            self._refuse_sharded(ib.embeddings)
+            self._check_mlps((body.deep, body.deep_logit))
         self._init_common(model, optimizer, batch_size, device, None)
         self._init_heads()
-        f32 = dict(dtype=torch.float32, device=self.device)
         B = self.B
-        self.chain, self.last = [], None
-        feats, tables = [], []
+        self.chain, self.last, self.inp = [], None, None
         if self.deep:
             self.chain = body.deep.dense_layers  # run by mm_dense_tc
             self.last = body.deep_logit.dense_layers[-1]  # Dense(1), fused into the head kernel
-            for l in self.chain + [self.last]:
-                if l.activation not in ("relu", "linear"):
-                    raise NotImplementedError(f"{l.name}: training supports relu / linear deep activations, got {l.activation!r}")
-            self.cols, _, self.d = ib.layout()
-            emb = ib.embeddings
-            feats = list(emb.feature_names) if emb is not None else []
-            tables = [emb.feature_to_table[f] for f in feats]
-            for f, t in zip(feats, tables):
-                col = model.schema.get(f)
-                if col is not None and col.is_list and t.dim not in (16, 32, 64, 128):
-                    raise NotImplementedError(f"feature {f!r}: training a multi-hot deep feature needs an embedding width of 16, "
-                                              f"32, 64 or 128, got {t.dim} (pass deep_input_block with Embeddings(dim=...))")
-            self.cont = sorted(ib.continuous.features) if ib.continuous is not None else []
-        self._init_tables(feats, tables)
+            self._check_activations(self.chain + [self.last])
+            self.inp = _ConcatInput(self, ib, dx0=True)
+            self.inp.check_multihot_widths(model.schema)
+        self._init_inputs([self.inp] if self.deep else [])
         self._init_dense(self.chain + ([self.last] if self.deep else []), [self.head])
         n = len(self.chain)
         self._init_wide(lambda li: li < n)
         if self.deep:
-            self.ld = _ld4(self.d)
-            self.x0 = torch.zeros((B, self.ld), **f32)
-            self.xs = torch.zeros((B, 2 * ops.tc_padded_k(self.d)), dtype=torch.bfloat16, device=self.device)
             self.h, self.h_split, self.dh = self._chain_buffers(self.chain)
-            self.dx0 = torch.zeros((B, self.ld), **f32)
-            self.slices = [torch.zeros((B, t.table.shape[1]), **f32) for t in self.tables]
         # ---- the wide kernel (W, 1) and its bias, outside the arena
         self.wl = body.wide
-        self.ds = torch.zeros(B, **f32)
+        self.ds = torch.zeros(B, dtype=torch.float32, device=self.device)
         if self.wl is not None:
-            self.wk = self.wl.dense
-            W = self.wk.kernel.numel()
-            slots = optimizer.slots
-            self.wk_s1 = torch.full((W,), optimizer.initial_accumulator_value, **f32) if slots >= 1 else None
-            self.wk_s2 = torch.zeros(W, **f32) if slots >= 2 else None
-            self.wb_s1 = torch.full((1,), optimizer.initial_accumulator_value, **f32) if slots >= 1 else None
-            self.wb_s2 = torch.zeros(1, **f32) if slots >= 2 else None
-            self.wk_acc = torch.zeros(W, **f32)
-            self.wk_rep = ops.fill_i32(torch.empty(W, dtype=torch.int32, device=self.device), INT32_MAX)
-            self.wk_grad = torch.zeros(1, **f32)  # the bias' gradient
-            self._wbag_bufs: Dict[int, dict] = {}
+            self.wk = _WideKernel(self, self.wl.dense)
+        self._wbag_bufs: Dict[int, dict] = {}
         self._init_loss(B)
         self.oob = body.oob_counter(self.device)[0]
 
@@ -1426,26 +1433,16 @@ class WideAndDeepTrainer(_StepTrainer):
         compiled size run in the leading rows of the same buffers."""
         a = self.arena
         n = len(self.chain)
-        self._loss_all.zero_()
-        b = batch_size_of(inputs)
-        targets = self._check_targets(targets, b)
-        if isinstance(sample_weight, (list, tuple)):
-            sample_weight = sample_weight[0]
-        tidx = range(len(self.tables))
-        self._idx: List[Optional[torch.Tensor]] = [None] * len(self.tables)
-        self._slices: List[torch.Tensor] = []  # no tables without a deep part
-        self._bags = {}
+        b, targets, sample_weight = self._begin_step(inputs, targets, sample_weight)  # no tables without a deep part
         h = dh = None
         if self.deep:
-            self._slices = [s[:b] for s in self.slices]
-            x0, xs = self.x0[:b, :self.d], self.xs[:b]
-            self._input_forward(self.feats, tidx, self.cols, self.cont, inputs, x0, xs)
+            _, xs, dx0 = self.inp.forward(inputs, b)
             h, dh = [t[:b] for t in self.h], [t[:b] for t in self.dh]
-            self._chain_forward(xs, self.d, 0, self.chain, h, [t[:b] for t in self.h_split])
+            self._chain_forward(xs, self.inp.d, 0, self.chain, h, [t[:b] for t in self.h_split])
         onehot, bags = self.wl.blocks(inputs) if self.wl is not None else ([], [])
         ds = self.ds[:b]
         hi = len(a.layers) - 1
-        wk = self.wk if self.wl is not None else None
+        wk = self.wk.dense if self.wk is not None else None
         ops.wide_deep_head_fwd_bwd(
             onehot, bags, None if wk is None else wk.kernel.reshape(-1), None if wk is None else wk.bias, None if h is None else h[-1],
             self.deep and self.chain[-1].activation == "relu", None if not self.deep else self.last.kernel.reshape(-1),
@@ -1453,9 +1450,10 @@ class WideAndDeepTrainer(_StepTrainer):
             self.head.bias, self.logits[:b], loss=self.losses[0], targets=targets[0].reshape(-1), sample_weight=sample_weight,
             loss_buf=self._loss_all, ds=ds, dh=None if dh is None else dh[-1], dw_out=a.view(a.grad, hi, "kernel"),
             db_out=a.view(a.grad, hi, "bias"), dw_dl=a.view(a.grad, n, "kernel") if self.deep else None,
-            db_dl=a.view(a.grad, n, "bias") if self.deep else None, d_wide_bias=None if wk is None else self.wk_grad, oob=self.oob)
-        self._wpairs = []
-        for q, bag in enumerate(bags):  # each wide bag feature's gradient as (id, value) pairs
+            db_dl=a.view(a.grad, n, "bias") if self.deep else None, d_wide_bias=None if wk is None else self.wk.grad, oob=self.oob)
+        # the wide kernel's gradient: ds for the one-hot blocks, each bag feature's as (id, value) pairs
+        calls = [([i for i, _, _ in onehot], [r for _, r, _ in onehot], [o for _, _, o in onehot], ds)] if onehot else []
+        for q, bag in enumerate(bags):
             nnz = bag[0].numel()
             buf = self._wbag_bufs.setdefault(q, dict(ids=None, vals=None))
             if buf["ids"] is None or buf["ids"].shape[0] < nnz:
@@ -1465,43 +1463,19 @@ class WideAndDeepTrainer(_StepTrainer):
                 buf["vals"] = torch.empty(max(nnz, 1), dtype=torch.float32, device=self.device)
             ids, vals = buf["ids"][:nnz], buf["vals"][:nnz]
             ops.wide_bag_grad(bag, b, ds, ids, vals)
-            self._wpairs.append((ids, vals, bag[2], bag[3]))
+            calls.append(([ids], [bag[2]], [bag[3]], vals))
+        if self.wk is not None:
+            self.wk.calls = calls
         if self.deep:
-            dx0 = self.dx0[:b, :self.d] if self.tables else None
-            self._chain_backward(0, self.chain, h, dh, (xs, self.d), dx0)
+            self._chain_backward(0, self.chain, h, dh, (xs, self.inp.d), dx0)
             if self.tables:
-                self._input_backward([dx0], self.feats, tidx, self.cols)
+                self.inp.backward([dx0], b)
                 self._bag_grads()
-        self._onehot, self._b = onehot, b
-
-    def _apply_more(self) -> None:
-        if self.wl is None:
-            return
-        wk, first = self.wk.kernel.reshape(-1), True
-        calls = []
-        if self._onehot:
-            calls.append(([i for i, _, _ in self._onehot], [r for _, r, _ in self._onehot], [o for _, _, o in self._onehot], self.ds[:self._b]))
-        calls += [([ids], [rows], [off], vals) for ids, vals, rows, off in self._wpairs]
-        for ids, rows, offs, g in calls:  # the bias takes its step with the first call
-            ops.wide_rows_apply(self.opt.kind, wk, self.wk_s1, self.wk_s2, ids, rows, offs, g, self.wk_acc, self.wk_rep, [],
-                                self.wk_grad if first else None, self.wk.bias.reshape(-1) if first else None,
-                                self.wb_s1 if first else None, self.wb_s2 if first else None, self.hyper)
-            first = False
+        self._b = b
 
     def wide_gradients(self) -> Dict[str, torch.Tensor]:
-        """The wide kernel's gradient (W, 1) and its bias' (after forward_backward, before apply_gradients), assembled in
-        float64 from ds, the one-hot ids and the bag features' expanded pairs — for parity tests."""
-        W = self.wk.kernel.numel()
-        g = torch.zeros(W, dtype=torch.float64, device=self.device)
-        ds = self.ds[:self._b].double()
-        for ids, rows, off in self._onehot:
-            i = ops.widen_index(ids).reshape(-1).long()
-            ok = (i >= 0) & (i < rows)
-            g.index_add_(0, i[ok] + off, ds[ok])
-        for ids, vals, rows, off in self._wpairs:
-            ok = ids >= 0
-            g.index_add_(0, ids[ok] + off, vals[ok].double())
-        return {"wide/kernel": g.reshape(W, 1), "wide/bias": self.wk_grad.double().clone()}
+        """The wide kernel's gradient (W, 1) and its bias' (after forward_backward, before apply_gradients) — for parity tests."""
+        return self.wk.gradients()
 
     def capture(self, inputs: Dict[str, torch.Tensor], targets: torch.Tensor, clone: bool = True) -> None:
         for f in (self.wl.names if self.wl is not None else []):
@@ -1509,24 +1483,6 @@ class WideAndDeepTrainer(_StepTrainer):
                 raise NotImplementedError(f"graph capture with the ragged wide feature {f!r} is not implemented: its number of ids "
                                           "changes from batch to batch (train it eagerly, or feed it as a fixed-length (B, L) matrix)")
         super().capture(inputs, targets, clone)
-
-    def _snapshot(self):
-        snap = super()._snapshot()
-        if self.wl is not None:
-            snap.update(wk=self.wk.kernel.clone(), wb=self.wk.bias.clone(),
-                        wk_s=[None if s is None else s.clone() for s in (self.wk_s1, self.wk_s2, self.wb_s1, self.wb_s2)])
-        return snap
-
-    def _restore(self, snap) -> None:
-        super()._restore(snap)
-        if self.wl is None:
-            return
-        self.wk.kernel.copy_(snap["wk"])
-        self.wk.bias.copy_(snap["wb"])
-        for dst, src in zip((self.wk_s1, self.wk_s2, self.wb_s1, self.wb_s2), snap["wk_s"]):
-            if src is not None:
-                dst.copy_(src)
-        self.wk_grad.zero_()
 
 
 class MMoETrainer(_StepTrainer):
@@ -1549,8 +1505,9 @@ class MMoETrainer(_StepTrainer):
               of the operand copies the model's forward reads.
     Fixed-length list features can be captured into one CUDA graph; ragged ones train eagerly."""
 
+    _model_name = "a multi-task Model(*blocks)"
+
     def __init__(self, model, optimizer: Optimizer, batch_size: int, device=None, group=None):
-        from .blocks import dense_engine
         from .models import BinaryOutput, MMoEBody, ParallelOutputs, output_towers
 
         body = model.body
@@ -1558,18 +1515,14 @@ class MMoETrainer(_StepTrainer):
             raise NotImplementedError("MMoETrainer trains Model(InputBlockV2, [MLPBlock], [MMOEBlock], output) bodies")
         if not isinstance(model.prediction, (BinaryOutput, ParallelOutputs)):
             raise NotImplementedError("train_step needs BinaryOutput / RegressionOutput heads or an OutputBlock of them")
-        if group is not None:
-            raise NotImplementedError("training a multi-task Model(*blocks) with a process group is not implemented")
-        if dense_engine() == "fp32":
-            raise NotImplementedError("training a multi-task Model(*blocks) runs on the tensor-core engine (dense_engine() == 'fp32')")
+        self._refuse_group(group)
+        self._require_tc_engine()
         ib, mo = body.input_block, body.mmoe
-        if getattr(ib.embeddings, "sharded", None) is not None:
-            raise NotImplementedError("training a multi-task Model(*blocks) with row-sharded tables is not implemented")
+        self._refuse_sharded(ib.embeddings)
         towers = output_towers(model.prediction) or []
-        blocks = ([body.bottom] if body.bottom is not None else []) + towers + (list(mo.gate_blocks.values()) if mo is not None and mo.gate_blocks else [])
-        for blk in blocks:
-            if blk.has_normalization or blk.dropout:
-                raise NotImplementedError("training supports bottom, gate and task blocks without normalization / dropout")
+        # the bottom, the task towers and the gate blocks
+        self._check_mlps(([body.bottom] if body.bottom is not None else []) + towers
+                         + (list(mo.gate_blocks.values()) if mo is not None and mo.gate_blocks else []))
         if mo is not None and mo.dropout:
             raise NotImplementedError("training MMOEBlock experts with dropout is not implemented")
         self._init_common(model, optimizer, batch_size, device, None)
@@ -1579,22 +1532,12 @@ class MMoETrainer(_StepTrainer):
         self.towers = [t.dense_layers for t in towers]
         self.gate_chains = [mo.gate_chain(t) for t in range(mo.num_gates)] if mo is not None and mo.gate_blocks else []
         chain_layers = [l for c in self.gate_chains + self.towers for l in c]
-        for l in self.bottom + chain_layers + ([mo.experts] if mo is not None else []):
-            if l.activation not in ("relu", "linear"):
-                raise NotImplementedError(f"{l.name}: training supports relu / linear activations, got {l.activation!r}")
+        self._check_activations(self.bottom + chain_layers + ([mo.experts] if mo is not None else []))
         if self.head.input_dim > 256:
             raise NotImplementedError("the output layer's input must be <= 256 wide")
-        self.cols, _, self.d = ib.layout()
-        emb = ib.embeddings
-        feats = list(emb.feature_names) if emb is not None else []
-        tables = [emb.feature_to_table[f] for f in feats]
-        for f, t in zip(feats, tables):
-            col = model.schema.get(f)
-            if col is not None and col.is_list and t.dim not in (16, 32, 64, 128):
-                raise NotImplementedError(f"feature {f!r}: training a multi-hot feature needs an embedding width of 16, 32, 64 or "
-                                          f"128, got {t.dim} (pass an InputBlockV2 with Embeddings(dim=...))")
-        self.cont = sorted(ib.continuous.features) if ib.continuous is not None else []
-        self._init_tables(feats, tables)
+        self.inp = _ConcatInput(self, ib, dx0=True)
+        self.inp.check_multihot_widths(model.schema)
+        self._init_inputs([self.inp])
         # arena order: bottom, [experts, stacked gates], gate chains, towers, heads; li0 of each chain
         tc = list(self.bottom)
         if mo is not None:
@@ -1618,12 +1561,9 @@ class MMoETrainer(_StepTrainer):
         # shared vector take theirs together, and a tower's first layer reading the mixture takes it alone
         self._init_wide(lambda li: (li < nb and (li > 0 or bool(self.tables))) or (li >= nb + (2 if mo is not None and mo.gates is not None else 1 if mo is not None else 0) and li not in firsts))
 
-        B, d = self.B, self.d
+        B = self.B
         f32 = dict(dtype=torch.float32, device=self.device)
         bf = dict(dtype=torch.bfloat16, device=self.device)
-        self.x0 = torch.zeros((B, _ld4(d)), **f32)
-        self.xs = torch.zeros((B, 2 * ops.tc_padded_k(d)), **bf)
-        self.dx0 = torch.zeros((B, _ld4(d)), **f32)
         fanout = mo is not None or bool(self.towers)
         if nb:
             self.h, self.h_split, self.dh = self._chain_buffers(self.bottom, split_last=fanout)
@@ -1656,9 +1596,8 @@ class MMoETrainer(_StepTrainer):
             self.M = torch.zeros((H, B, U), **f32)
             self.M_split = torch.zeros((H, B, 2 * ops.tc_padded_k(U)), **bf)
             self.dM = torch.zeros((H, B, U), **f32)
-        self.slices = [torch.zeros((B, t.table.shape[1]), **f32) for t in self.tables]
         self._init_loss(B)
-        self.oob = emb.counter(self.device) if emb is not None else None
+        self.oob = self.inp.oob
 
     def _g(self, i: int, b: int) -> torch.Tensor:
         """Reader i's columns of G (its pre-activation gradient)."""
@@ -1669,20 +1608,13 @@ class MMoETrainer(_StepTrainer):
         """Forward (activations saved), loss and backward: fills the gradient arena and the tables' IndexedSlices.  Batches
         smaller than the compiled size run in the leading rows of the same buffers."""
         a = self.arena
-        nb, d, mo = len(self.bottom), self.d, self.mmoe
-        self._loss_all.zero_()
-        b = batch_size_of(inputs)
-        targets = self._check_targets(targets, b)
+        nb, d, mo = len(self.bottom), self.inp.d, self.mmoe
+        b, targets, sample_weight = self._begin_step(inputs, targets, sample_weight)
         ys = [t.reshape(-1) for t in targets]
         hi = len(a.layers) - 1
         logits = self.logits.view(-1)[:self.H * b].view(self.H, b)
-        tidx = range(len(self.tables))
-        self._idx: List[Optional[torch.Tensor]] = [None] * len(self.tables)
-        self._slices = [s[:b] for s in self.slices]
-        self._bags = {}
         v = lambda ts: [t[:b] for t in ts]
-        x0, xs, dx0 = self.x0[:b, :d], self.xs[:b], self.dx0[:b, :d]
-        self._input_forward(self.feats, tidx, self.cols, self.cont, inputs, x0, xs)
+        _, xs, dx0 = self.inp.forward(inputs, b)  # dx0: None without tables
         op, K = xs, d
         if nb:
             h, h_split, dh = v(self.h), v(self.h_split), v(self.dh)
@@ -1743,7 +1675,7 @@ class MMoETrainer(_StepTrainer):
             else:
                 for i, (c, (gh, ghs, gdh)) in enumerate(zip(self.gate_chains, gb)):
                     self._chain_backward(self.gate_li0[i], c, gh, gdh, (op, K), None)
-        dx_in = dh[-1] if nb else (dx0 if self.tables else None)
+        dx_in = dh[-1] if nb else dx0
         if self.G is not None and dx_in is not None:  # G [W_0 | W_1 | ..]^T: the readers' input gradients summed by one GEMM
             for (c0, c1), l in zip(self.G_cols, self.readers):
                 self.wT[c0:c1].copy_(l.kernel.t())
@@ -1754,9 +1686,9 @@ class MMoETrainer(_StepTrainer):
             if nb and self.bottom[-1].activation == "relu":
                 ops.relu_mask(dx_in, h[-1])
         if nb:
-            self._chain_backward(0, self.bottom, h, dh, (xs, d), dx0 if self.tables else None)
+            self._chain_backward(0, self.bottom, h, dh, (xs, d), dx0)
         if self.tables:
-            self._input_backward([dx0], self.feats, tidx, self.cols)
+            self.inp.backward([dx0], b)
             self._bag_grads()
         self._b = b
 
@@ -1770,12 +1702,7 @@ def trainer_for(model, optimizer: Optimizer, batch_size: int, group=None):
         raise NotImplementedError("training TwoTowerModelV2 / ContrastiveOutput is not implemented: train the v1 TwoTowerModel")
     if isinstance(model, RetrievalModel):
         return TwoTowerTrainer(model, optimizer, batch_size, group=group)
-    if isinstance(getattr(model, "body", None), DCNBody):
-        return DCNTrainer(model, optimizer, batch_size, group=group)
-    if isinstance(getattr(model, "body", None), DeepFMBody):
-        return DeepFMTrainer(model, optimizer, batch_size, group=group)
-    if isinstance(getattr(model, "body", None), WideAndDeepBody):
-        return WideAndDeepTrainer(model, optimizer, batch_size, group=group)
-    if isinstance(getattr(model, "body", None), MMoEBody):
-        return MMoETrainer(model, optimizer, batch_size, group=group)
-    return DLRMTrainer(model, optimizer, batch_size, group=group)
+    by_body = {DCNBody: DCNTrainer, DeepFMBody: DeepFMTrainer, WideAndDeepBody: WideAndDeepTrainer, MMoEBody: MMoETrainer}
+    body = getattr(model, "body", None)
+    cls = next((c for t, c in by_body.items() if isinstance(body, t)), DLRMTrainer)
+    return cls(model, optimizer, batch_size, group=group)

@@ -510,12 +510,12 @@ def _dcn_reference(tr, inputs, y, B, chunk=4096):
     yd = y.reshape(-1).double()
     loss, slices, flips = 0.0, [[] for _ in ids], []
     for s, e in _chunks(B, chunk):
-        x0 = torch.zeros((e - s, tr.d), dtype=torch.float64, device=yd.device)
+        x0 = torch.zeros((e - s, tr.inp.d), dtype=torch.float64, device=yd.device)
         for t, f in enumerate(tr.feats):
-            c, w = tr.cols[f], tr.tables[t].table.shape[1]
+            c, w = tr.inp.cols[f], tr.tables[t].table.shape[1]
             x0[:, c:c + w] = tr.tables[t].table[ids[t][s:e]].double()
-        for n in tr.cont:
-            x0[:, tr.cols[n]] = inputs[n].reshape(-1)[s:e].double()
+        for n in tr.inp.cont:
+            x0[:, tr.inp.cols[n]] = inputs[n].reshape(-1)[s:e].double()
         x0.requires_grad_(True)
         flip = []
         x = x0
@@ -531,7 +531,7 @@ def _dcn_reference(tr, inputs, y, B, chunk=4096):
         part.backward()
         loss += float(part.detach())
         for t, f in enumerate(tr.feats):
-            c, w = tr.cols[f], tr.tables[t].table.shape[1]
+            c, w = tr.inp.cols[f], tr.tables[t].table.shape[1]
             slices[t].append(x0.grad[:, c:c + w])
         flips.append(torch.stack(flip).any(0))
         ref.collect()
@@ -539,7 +539,7 @@ def _dcn_reference(tr, inputs, y, B, chunk=4096):
     return loss, grads, terms, [torch.cat(s) for s in slices], torch.cat(flips)
 
 
-def test_dcn_train_step_as_the_benchmark_runs_it(device):
+def test_dcn_train_step_at_benchmark_size(device):
     """DCNModel(Criteo schema capped at 400 000 rows, depth 3, deep [256, 128]) with the uncapped schema's widths
     (d = 1037), Adagrad, B = 65 536, packed 1/2/3-byte ids through HostBatch into one CUDA graph.  The tables cover every
     sparse path: counting sort (<= 1024 rows), the dense accumulator (<= DENSE_PATH_MAX_ROWS) and the election at widths
@@ -557,7 +557,7 @@ def test_dcn_train_step_as_the_benchmark_runs_it(device):
     _, mb = _dcn_bench_model(device, 41)
     label, hosts, packed, static, inputs, y = _dcn_packed(schema, ma, B, (5150, 5151, 5152), device)
     ta, tb = ma.trainer(B), mb.trainer(B)
-    assert ta.d == D_DCN and ta.stacked and sorted(ta._wide) == [0, 1, 2, 3]  # the cross layers and the 256-unit layer
+    assert ta.inp.d == D_DCN and ta.stacked and sorted(ta._wide) == [0, 1, 2, 3]  # the cross layers and the 256-unit layer
     rows = {f: t.table.shape[0] for f, t in zip(ta.feats, ta.tables)}
     widths = {f: t.table.shape[1] for f, t in zip(ta.feats, ta.tables)}
     assert min(rows.values()) <= COUNTING_SORT_MAX_ROWS and any(COUNTING_SORT_MAX_ROWS < r <= DENSE_PATH_MAX_ROWS for r in rows.values())
@@ -585,7 +585,7 @@ def test_dcn_train_step_as_the_benchmark_runs_it(device):
     _check_operands(ta, transposed=False)
 
 
-def test_dcn_parallel_gradients_at_scale(device):
+def test_dcn_parallel_step_gradients_at_scale(device):
     """The parallel body at B = 65 573: the deep tower on x0, the head on [cross | deep] of 1037 + 128 = 1165 inputs,
     beyond the fused loss kernel's 256 (the wide-head composition: tensor-core logits, mm_heads_fwd_bwd with an
     identity kernel, mm_dense_wgrad_split and mm_dense_dgrad of the head).  forward_backward on packed ids against
@@ -646,13 +646,13 @@ def _tt_reference(tr, inputs, B):
     ref = _Ref([l for tw in tr.towers for l in tw["layers"]])
     names = {id(l): f"{tw['name']}/" for tw in tr.towers for l in tw["layers"]}
     outs, x0s, flips = [], [], []
-    for tw in tr.towers:
-        x0 = torch.zeros((B, tw["d"]), dtype=torch.float64, device=tr.device)
-        for t, f in zip(tw["tidx"], tw["feats"]):
-            c, w = tw["cols"][f], tr.tables[t].table.shape[1]
+    for tw, inp in zip(tr.towers, tr.inps):
+        x0 = torch.zeros((B, inp.d), dtype=torch.float64, device=tr.device)
+        for t, f in zip(inp.tidx, inp.feats):
+            c, w = inp.cols[f], tr.tables[t].table.shape[1]
             x0[:, c:c + w] = tr.tables[t].table[ops.widen_index(tr._idx[t]).long()].double()
-        for n in tw["cont"]:
-            x0[:, tw["cols"][n]] = inputs[n].reshape(-1).double()
+        for n in inp.cont:
+            x0[:, inp.cols[n]] = inputs[n].reshape(-1).double()
         x0.requires_grad_(True)
         h = x0
         for i in range(len(tw["layers"])):
@@ -667,7 +667,7 @@ def _tt_reference(tr, inputs, B):
     pre = {li: (hin, z.detach()) for li, hin, z in ref.pre}
     terms, slice_terms = {}, [None] * len(tr.tables)
     with torch.no_grad():
-        for tw, dz in zip(tr.towers, _ce_terms(q.detach(), it.detach(), ids, tr.temperature, 1.0 / B)):
+        for tw, inp, dz in zip(tr.towers, tr.inps, _ce_terms(q.detach(), it.detach(), ids, tr.temperature, 1.0 / B)):
             for i in range(len(tw["layers"]) - 1, -1, -1):
                 l = tw["layers"][i]
                 hin, z = pre[tw["li0"] + i]
@@ -677,18 +677,18 @@ def _tt_reference(tr, inputs, B):
                 if l.bias is not None:
                     terms[f"{tw['name']}/{l.name}/bias"] = dz.sum(0)
                 dz = dz @ l.kernel.double().abs().t()
-            for t, f in zip(tw["tidx"], tw["feats"]):
-                c, w = tw["cols"][f], tr.tables[t].table.shape[1]
+            for t, f in zip(inp.tidx, inp.feats):
+                c, w = inp.cols[f], tr.tables[t].table.shape[1]
                 slice_terms[t] = dz[:, c:c + w]
     slices = [None] * len(tr.tables)
-    for tw, x0 in zip(tr.towers, x0s):
-        for t, f in zip(tw["tidx"], tw["feats"]):
-            c, w = tw["cols"][f], tr.tables[t].table.shape[1]
+    for inp, x0 in zip(tr.inps, x0s):
+        for t, f in zip(inp.tidx, inp.feats):
+            c, w = inp.cols[f], tr.tables[t].table.shape[1]
             slices[t] = x0.grad[:, c:c + w]
     return loss, grads, terms, slices, torch.stack(flips).any(0), slice_terms
 
 
-def test_twotower_train_step_as_the_benchmark_runs_it(device):
+def test_twotower_train_step_at_benchmark_size(device):
     """TwoTowerModel(retrieval_10m_schema(): 10 M-row item table, 1 M-row user table; towers [256, 128]) at full size,
     Adagrad, B = 16 384, Zipf ids (generate_batch's law of the benchmark), packed through HostBatch: user_id and item_id
     as 3-byte ids.  Adagrad rather than Adam: Adam divides every update by sqrt(v), so an element whose gradient

@@ -74,9 +74,9 @@ def main():
     tr = model.trainer(B)
     tr.capture(*batches[0])
     rows = sum(tb.table.shape[0] for tb in tr.tables)
-    print(f"batch {B}, d = {tr.d}, embedding_dim {DIM}, deep {DEEP}, {rows} table rows, wide kernel {tr.wk.kernel.shape[0]} rows, "
+    print(f"batch {B}, d = {tr.inp.d}, embedding_dim {DIM}, deep {DEEP}, {rows} table rows, wide kernel {tr.wk.dense.kernel.shape[0]} rows, "
           f"launches per step: {tr.launches_per_step}")
-    T, C, U = len(tr.feats), len(tr.cont), tr.U
+    T, C, U = len(tr.feats), len(tr.inp.cont), tr.U
     hb = head_bytes(B, T, C, DIM, U)
     floor_us = sum(hb.values()) / HBM_BYTES_PER_S * 1e6
     print("head kernel bytes per step (computed): " + ", ".join(f"{k} {v / 1e6:.1f} MB" for k, v in hb.items())

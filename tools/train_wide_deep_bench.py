@@ -91,8 +91,8 @@ def main():
     tr.capture(*batches[0])
     ids = sum(bag.values())
     U = DEEP[-1]
-    print(f"{'multi-hot' if args.multihot else 'one-hot'} Wide&Deep train step, batch {B}, {ids} ids per sample, d = {tr.d}, "
-          f"deep {DEEP}, wide kernel {tr.wk.kernel.shape[0]} rows, launches per step: {tr.launches_per_step}")
+    print(f"{'multi-hot' if args.multihot else 'one-hot'} Wide&Deep train step, batch {B}, {ids} ids per sample, d = {tr.inp.d}, "
+          f"deep {DEEP}, wide kernel {tr.wk.dense.kernel.shape[0]} rows, launches per step: {tr.launches_per_step}")
     for name, fl in floors(B, ids, U).items():
         total = sum(fl.values())
         print(f"{name} bytes per step (computed): " + ", ".join(f"{k} {v / 1e6:.1f} MB" for k, v in fl.items())
