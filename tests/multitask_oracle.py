@@ -85,6 +85,29 @@ def dlrm_multitask_loss_and_grads(batch: Dict[str, np.ndarray], tables: Dict[str
     return float(total.item()), losses, logits, grads
 
 
+def heads_ref(x, W, b, losses, ys, sws, lws, mask_relu):
+    """The output heads alone (what mm_heads_fwd_bwd computes), float64 autograd on the device of x: (total loss,
+    per-head losses, logits (H, M), dx, dW, db)."""
+    x = x.double().clone().requires_grad_(True)
+    W = W.double().clone().requires_grad_(True)
+    b = b.double().clone().requires_grad_(True)
+    z = x @ W + b  # (M, H)
+    M = x.shape[0]
+    per = []
+    for h, l in enumerate(losses):
+        y = ys[h].double()
+        zh = z[:, h]
+        term = torch.clamp(zh, min=0) - zh * y + torch.log1p(torch.exp(-zh.abs())) if l == BCE else (zh - y) ** 2
+        sw = sws[h].double() if sws[h] is not None else torch.ones(M, dtype=torch.float64, device=x.device)
+        per.append((term * sw).sum() / M)
+    total = sum(lw * p for lw, p in zip(lws, per))
+    total.backward()
+    dx = x.grad
+    if mask_relu:
+        dx = dx * (x > 0)
+    return total.detach(), torch.stack([p.detach() for p in per]), z.detach().t(), dx, W.grad, b.grad
+
+
 def golden_inputs(z):
     """(batch, tables, feature_table, continuous, bottom, top, heads, targets) of the multitask fixture, heads in the
     package's output order (sorted output names)."""

@@ -13,6 +13,7 @@ from models_b200 import datasets, ops
 from models_b200.blocks import last_dense_path, set_dense_engine
 from models_b200.schema import ColumnSchema, Schema, Tags
 from tests import helpers as H
+from tests.multitask_oracle import heads_ref
 
 pytestmark = pytest.mark.gpu
 TOL = 3e-4
@@ -26,28 +27,6 @@ def close(got, ref, tol=TOL, what=""):
     scale = max(float(np.max(np.abs(ref))), 1e-30)
     err = float(np.max(np.abs(got - ref))) / scale
     assert err < tol, f"{what}: max |diff| / max |ref| = {err:.3e} (tol {tol})"
-
-
-def heads_ref(x, W, b, losses, ys, sws, lws, mask_relu):
-    """float64 autograd restatement: (total loss, per-head losses, logits (H, M), dx, dW, db)."""
-    x = x.double().clone().requires_grad_(True)
-    W = W.double().clone().requires_grad_(True)
-    b = b.double().clone().requires_grad_(True)
-    z = x @ W + b  # (M, H)
-    M = x.shape[0]
-    per = []
-    for h, l in enumerate(losses):
-        y = ys[h].double()
-        zh = z[:, h]
-        term = torch.clamp(zh, min=0) - zh * y + torch.log1p(torch.exp(-zh.abs())) if l == "binary_crossentropy" else (zh - y) ** 2
-        sw = sws[h].double() if sws[h] is not None else torch.ones(M, dtype=torch.float64, device=x.device)
-        per.append((term * sw).sum() / M)
-    total = sum(lw * p for lw, p in zip(lws, per))
-    total.backward()
-    dx = x.grad
-    if mask_relu:
-        dx = dx * (x > 0)
-    return total.detach(), torch.stack([p.detach() for p in per]), z.detach().t(), dx, W.grad, b.grad
 
 
 def _targets(g, M, losses, dtypes, device):
@@ -150,11 +129,14 @@ def test_mlp_tc_heads_matches_float64(device, H_, widths):
 # ---------------------------------------------------------------------------------------------------------------
 # models
 # ---------------------------------------------------------------------------------------------------------------
+REGRESSION_TARGETS = ("rating", "dwell", "watch_time")  # the other target names are binary
+
+
 def _mt_schema(cap=200, targets=("click", "conversion", "rating")):
     base = datasets.criteo_schema({k: min(v, cap) for k, v in datasets.CRITEO_MAX.items()})
     cols = [c for c in base if not c.has_tag(Tags.TARGET)]
     for t in targets:
-        if t == "rating":
+        if t in REGRESSION_TARGETS:
             cols.append(ColumnSchema(t, tags=(Tags.TARGET, Tags.REGRESSION), dtype="float32"))
         else:
             cols.append(ColumnSchema(t, tags=(Tags.TARGET, Tags.BINARY_CLASSIFICATION), dtype="int64"))
@@ -285,6 +267,52 @@ def test_train_step_multi_output_losses_and_head_gradients(device):
     np.testing.assert_allclose(m["rating/regression_output_loss"].item(), per[2].item(), rtol=1e-5)
     with pytest.raises(ValueError, match="conversion"):
         model.train_step((x, {k: v for k, v in y.items() if k != "conversion"}))
+
+
+# up to 8 outputs, binary and regression mixed (sorted by name they interleave)
+MANY_TARGETS = ("click", "rating", "conversion", "dwell", "like", "watch_time", "share", "follow")
+
+
+@pytest.mark.parametrize("top", [(64, 32), (64, 48)])  # last width 32: fused heads (mm_mlp_tc_heads); 48: mm_heads_fwd_bwd
+@pytest.mark.parametrize("n_out", [4, 5, 6, 7, 8])
+def test_four_to_eight_outputs_forward_step_and_served_predictions(device, n_out, top):
+    """A DLRM with 4..8 outputs: the forward per output against the oracle, through the kernel _LAST_HEADS names; one
+    training step's total and per-output losses and the stacked head's kernel and bias gradients (per column) against
+    float64 with unequal loss weights; and the model's forward on the step's batch against the activation of the
+    trainer's logits, per output."""
+    from models_b200.blocks import _LAST_HEADS
+
+    schema = _mt_schema(targets=MANY_TARGETS[:n_out])
+    model = _dlrm(schema, top, seed=40 + n_out)
+    model.build(device)
+    names = model.prediction.names
+    assert len(names) == n_out and {KINDS[c] for c in "br"} == set(model.prediction.losses)
+    B = 700
+    feats, ys = _batch(schema, B, 50 + n_out)
+    x = H.device_batch(feats, device)
+    out = model(x)
+    assert _LAST_HEADS[0] == ("mlp_tc" if top[-1] <= 32 else "heads")
+    for n, want in zip(names, oracle_dlrm_outputs(model, feats)):
+        assert tuple(out[n].shape) == (B, 1)
+        assert H.rel_err(out[n].cpu().numpy().reshape(-1), want) < 2e-4, n
+    lws = [0.25 + 0.25 * h for h in range(n_out)]
+    model.compile(optimizer=mm.SGD(0.0), loss_weights=lws)
+    yl = [torch.from_numpy(ys[o.target]).to(device) for o in model.output_blocks()]
+    tr = model.trainer(B)
+    tr.forward_backward(x, yl)
+    tot, per, _, _, rdW, rdb = _train_ref(model, tr, yl, lws)
+    np.testing.assert_allclose(tr.loss[0].item(), tot.item(), rtol=1e-5)
+    np.testing.assert_allclose(tr.loss[1:].cpu().numpy(), per.cpu().numpy(), rtol=1e-5)
+    g = tr.gradients()
+    hl = model.prediction.to_call
+    for h, n in enumerate(names):
+        close(g[f"{hl.name}/kernel"][:, h], rdW[:, h], what=f"dW of {n}")
+    close(g[f"{hl.name}/bias"], rdb, what="db")
+    served = model(x)
+    for h, (n, a) in enumerate(zip(names, model.prediction.activations)):
+        zl = tr.logits[h].double()
+        want = torch.sigmoid(zl) if a == "sigmoid" else zl
+        assert H.rel_err(served[n].cpu().numpy().reshape(-1), want.cpu().numpy()) < 2e-4, n
 
 
 def test_single_regression_output_forward_and_train(device):

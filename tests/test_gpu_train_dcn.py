@@ -155,7 +155,7 @@ def _schema(targets=("click",)):
             for n, mx in CATS]
     cols += [ColumnSchema(n, tags=(Tags.CONTINUOUS,), dtype="float32") for n in CONTS]
     for t in targets:
-        if t == "rating":
+        if t in ("rating", "dwell", "watch_time"):
             cols.append(ColumnSchema(t, tags=(Tags.TARGET, Tags.REGRESSION), dtype="float32"))
         else:
             cols.append(ColumnSchema(t, tags=(Tags.TARGET, Tags.BINARY_CLASSIFICATION), dtype="int64"))
@@ -433,6 +433,17 @@ def test_binary_and_regression_outputs(device):
         dense = torch.zeros(tr.tables[t].table.shape, dtype=torch.float64, device=device)
         dense.index_add_(0, tr._idx[t].long(), tr._slices[t].double())
         close(dense, grads[f"table/{f}"], what=f"table {f}")
+
+
+@pytest.mark.parametrize("n_out", [4, 8])
+def test_several_outputs_on_a_wide_head_input_are_refused(device, n_out):
+    """Several outputs read the head input from registers in the forward (at most 256 units), so a parallel body whose
+    [cross | deep] is 356 wide is refused when the model is built, naming the limit: the trainer's wide-head composition
+    (tensor-core logits, then mm_heads_fwd_bwd on the (B, H) logits with an identity kernel) runs with one output only."""
+    targets = ("click", "rating", "conversion", "dwell", "like", "watch_time", "share", "follow")[:n_out]
+    model = _dcn(stacked=False, targets=targets, **WIDE)
+    with pytest.raises(NotImplementedError, match="at most 256 units, got 356"):
+        model.build(device)
 
 
 @pytest.mark.parametrize("stacked,wide", [(True, False), (False, False), (False, True)])

@@ -176,3 +176,35 @@ def test_parallel_outputs_weights_before_build_and_width_limit():
     assert out.weights() == {}
     with pytest.raises(NotImplementedError, match="at most 256"):
         out.build(300)
+
+
+def test_nine_outputs_are_refused():
+    with pytest.raises(NotImplementedError, match=r"2\.\.8 outputs are supported, got 9"):
+        mm.OutputBlock(_schema(*[(f"t{i}", "bin" if i % 2 else "reg") for i in range(9)]))
+
+
+def test_heads_kernel_cases_reach_every_instantiation():
+    """tests/test_gpu_heads_kernels.py's CASES reach all 96 kernels mm_heads_fwd_bwd is compiled for: H = 1..8 heads x
+    {scalar, G2, G4, G8, G16, G32} x {training, forward only}, by heads_variant, the restatement of run_heads /
+    launch_heads (train_dense.cu).  Prints the H x variant table (T: training, F: forward only)."""
+    from tests.test_gpu_heads_kernels import CASES, VARIANTS, case_variants, heads_variant
+
+    # the restatement itself, on the deciding inputs: K, the row strides, 16-byte alignment of x / dx and of w for H = 1
+    assert [heads_variant(2, k, k, 0, 0) for k in (4, 8, 12, 16, 20, 32, 36, 64, 68, 128)] == \
+        ["G2", "G2", "G4", "G4", "G8", "G8", "G16", "G16", "G32", "G32"]
+    assert {heads_variant(2, k, k, 0, 0) for k in (1, 7, 130, 132, 256)} == {"scalar"}
+    assert heads_variant(1, 32, 32, 0, 4) == "scalar" and heads_variant(2, 32, 32, 0, 4) == "G8"
+    assert heads_variant(2, 32, 33, 0, 0) == "scalar" and heads_variant(2, 32, 40, 4, 0) == "scalar"
+    assert heads_variant(2, 32, 40, 16, 0, 36, 16) == "G8" and heads_variant(2, 32, 40, 16, 0, 34, 16) == "scalar"
+    assert heads_variant(2, 32, 40, 16, 0, 36, 20) == "scalar"
+    seen = {}
+    for c in CASES:
+        train, fwd = case_variants(c)
+        seen.setdefault((c[0], train), set()).add("T")
+        seen.setdefault((c[0], fwd), set()).add("F")
+    rows = ["H  " + "".join(f"{v:>8}" for v in VARIANTS)]
+    rows += [f"{h:<3}" + "".join(f"{''.join(sorted(seen.get((h, v), ()), reverse=True)):>8}" for v in VARIANTS) for h in range(1, 9)]
+    print("\n".join(rows))
+    triples = {(h, v, t) for (h, v), ts in seen.items() for t in ts}
+    assert triples == {(h, v, t) for h in range(1, 9) for v in VARIANTS for t in "TF"}, "missing: " + str(
+        sorted({(h, v, t) for h in range(1, 9) for v in VARIANTS for t in "TF"} - triples))
