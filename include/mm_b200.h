@@ -539,6 +539,20 @@ int mm_cross_backward(const float* x0, int64_t x0_stride, const float* z, int64_
 int mm_concat_backward(const float* const* addends_host, const int64_t* addend_strides_host, int n_addends, int64_t B, int d,
                        const mm_column_slice* slices_host, int n_slices, void* stream);
 
+/* Added with matrix factorization training; no existing entry point changed.
+ *   mm_concat_backward_l2  mm_concat_backward plus the gradient of the embeddings' L2 penalty
+ *                          reg = sum_t l2_t sum_b ||x0[b, col_t : col_t + width_t]||^2 (the reference's embeddings_l2_reg on
+ *                          the batch's looked-up, pooled rows): dst_t[b, :] = sum_a addend_a[b, col_t : +width_t]
+ *                          + 2 l2_t x0[b, col_t : +width_t], and loss[0] += reg, loss[1] += reg (loss: 2 device floats,
+ *                          [total, regularization]).  The arguments and rules of mm_concat_backward, plus x0 (B, d) fp32
+ *                          rows x0_stride >= d apart (no alignment beyond fp32), l2_host: n_slices HOST floats, each finite
+ *                          and >= 0, and a device workspace `partials` of n_partials >= n_slices * MM_CONCAT_L2_CTAS floats.
+ *                          reg is reduced in a fixed order (per-CTA partials, then one fold): equal inputs give equal bits. */
+#define MM_CONCAT_L2_CTAS 512
+int mm_concat_backward_l2(const float* const* addends_host, const int64_t* addend_strides_host, int n_addends, int64_t B, int d,
+                          const mm_column_slice* slices_host, int n_slices, const float* x0, int64_t x0_stride,
+                          const float* l2_host, float* partials, int64_t n_partials, float* loss, void* stream);
+
 /* ---------------------------------------------------------------------------------------
  * K15  Factorization-machine heads (blocks/interaction.py:205-332; DeepFMModel models/ranking.py:171-279).
  *   mm_fm_pairwise   FMPairwiseInteraction.call: x (B, A, K) -> out (B, K) = 0.5 ((sum_a x)^2 - sum_a x^2)

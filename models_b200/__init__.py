@@ -18,11 +18,11 @@ from .blocks import (CrossBlock, DLRMBlock, DotProductInteraction, MLPBlock, den
 from .blocks import BatchNormalization, CategoryEncoding, FMBlock, FMPairwiseInteraction, HashedCross, HashedCrossAll  # noqa: F401
 from .experts import CGCBlock, MMOEBlock, PLEBlock  # noqa: F401
 from .retrieval import (CategoricalOutput, ContrastiveOutput, Encoder, InBatchSampler, InBatchSamplerV2,  # noqa: F401
-                        ItemRetrievalScorer, ItemRetrievalTask, L2Norm, PopularityBasedSamplerV2, TwoTowerBlock,
-                        log_uniform_sampling_probs)
+                        ItemRetrievalScorer, ItemRetrievalTask, L2Norm, PopularityBasedSamplerV2,
+                        QueryItemIdsEmbeddingsBlock, TwoTowerBlock, log_uniform_sampling_probs)
 from .models import (BinaryClassificationTask, BinaryOutput, DCNModel, DeepFMModel, DLRMModel, Model, OutputBlock,  # noqa: F401
                      ParallelOutputs, RegressionOutput, WideAndDeepModel,
-                     RetrievalModel, RetrievalModelV2, TwoTowerModel, TwoTowerModelV2)
+                     MatrixFactorizationModel, RetrievalModel, RetrievalModelV2, TwoTowerModel, TwoTowerModelV2)
 from .topk import (AvgPrecisionAt, BruteForce, MRRAt, NDCGAt, PrecisionAt, RecallAt, TopKEncoder,  # noqa: F401
                    TopKIndexBlock, TopKPrediction, encode_candidates, unique_rows_by_features)
 from .loader import Loader, sample_batch  # noqa: F401

@@ -97,6 +97,7 @@ WIDE_MODES = {"multi_hot": 0, "count": 1}  # MM_WIDE_MULTI_HOT / MM_WIDE_COUNT
 OPTIMIZERS = {"sgd": 0, "adagrad": 1, "adam": 2}
 LOSS_KINDS = {"binary_crossentropy": 0, "mse": 1}  # MM_LOSS_BCE / MM_LOSS_MSE
 HYPER_LR, HYPER_BETA1, HYPER_BETA2, HYPER_EPS, HYPER_STEP, HYPER_LR_T, HYPER_COUNT = 0, 1, 2, 3, 4, 5, 8
+CONCAT_L2_CTAS = 512  # MM_CONCAT_L2_CTAS: mm_concat_backward_l2's partials per slice
 
 
 class ConcatPiece(C.Structure):
@@ -209,6 +210,8 @@ SIGNATURES = {
     "mm_fill_i32": (_i, [_vp, _i64, C.c_int32, _vp]),
     "mm_cross_backward": (_i, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _i, _i64, _i, _vp, _i64, _vp, _i, _vp]),
     "mm_concat_backward": (_i, [C.POINTER(C.c_void_p), C.POINTER(C.c_int64), _i, _i64, _i, C.POINTER(ColumnSlice), _i, _vp]),
+    "mm_concat_backward_l2": (_i, [C.POINTER(C.c_void_p), C.POINTER(C.c_int64), _i, _i64, _i, C.POINTER(ColumnSlice), _i, _vp, _i64,
+                                   C.POINTER(C.c_float), _vp, _i64, _vp, _vp]),
     "mm_inbatch_softmax_ce_backward": (_i, [_vp, _vp, _i64, _i64, _i, _vp, _vp, _i, _i, _f, _vp, _f, _vp, _vp, _vp, _vp, _i,
                                             _vp, _vp, _vp, _vp, _vp]),
     "mm_l2_normalize_backward": (_i, [_vp, _vp, _i64, _i, _i64, _i64, _vp, _i64, _vp]),

@@ -840,6 +840,12 @@ __global__ void __launch_bounds__(32 * CB_ROWS) cross_backward_kernel(const Cros
 // the IndexedSlices values.  Columns of no table (continuous features) are never read.  Offsets are arbitrary (width-1
 // continuous columns interleave by sorted name), so the addends are read as scalars; the slices are written as float4.
 // blockIdx.y = table.
+//
+// L2 = true (mm_concat_backward_l2) adds the gradient of the per-table penalty l2_t * sum_b ||x0[b, cols_t]||^2, which
+// the reference adds to the loss for every looked-up (pooled) embedding of the batch: slice_t += 2 l2_t x0[b, cols_t].
+// Each CTA also writes l2_t times its share of sum ||x0||^2 to partials[blockIdx.y * gridDim.x + blockIdx.x] (a fixed
+// order: per-thread sums in grid-stride order, then a fixed shuffle / shared-memory tree), and concat_l2_fold_kernel adds
+// the partials in index order into loss[0] (the total) and loss[1] (the regularization term): two runs give the same bits.
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int CB_MAX_ADD = 4;
 constexpr int CB_MAX_SLICES = 64;
@@ -849,12 +855,19 @@ struct ConcatBwdParams {
   mm_column_slice s[CB_MAX_SLICES];
   long long B;
   int n_add;
+  // L2 only
+  float l2[CB_MAX_SLICES];
+  const float* x0;
+  long long ldx;
+  float* partials;
 };
 
+template <bool L2>
 __global__ void __launch_bounds__(256) concat_backward_kernel(const __grid_constant__ ConcatBwdParams q) {
   const mm_column_slice& s = q.s[blockIdx.y];
   const int Q = s.width >> 2;
   const long long total = q.B * Q;
+  float sq = 0.f;
   for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
     const long long m = e / Q;
     const int c = (int)(e - m * Q) * 4;
@@ -864,7 +877,47 @@ __global__ void __launch_bounds__(256) concat_backward_kernel(const __grid_const
 #pragma unroll
       for (int j = 0; j < 4; ++j) v[j] += src[j];
     }
+    if constexpr (L2) {
+      const float two_l2 = 2.f * q.l2[blockIdx.y];
+      const float* x = q.x0 + m * q.ldx + s.col + c;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float xj = x[j];
+        v[j] += two_l2 * xj;
+        sq += xj * xj;
+      }
+    }
     *reinterpret_cast<float4*>(s.dst + m * s.dst_stride + c) = make_float4(v[0], v[1], v[2], v[3]);
+  }
+  if constexpr (L2) {
+    __shared__ float red[8];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = sq;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      float t = 0.f;
+#pragma unroll
+      for (int w = 0; w < 8; ++w) t += red[w];
+      q.partials[(long long)blockIdx.y * gridDim.x + blockIdx.x] = q.l2[blockIdx.y] * t;
+    }
+  }
+}
+
+__global__ void __launch_bounds__(256) concat_l2_fold_kernel(const float* __restrict__ partials, int n, float* __restrict__ loss) {
+  __shared__ double red[256];
+  double v = 0.0;
+  for (int i = threadIdx.x; i < n; i += 256) v += partials[i];
+  red[threadIdx.x] = v;
+  __syncthreads();
+  for (int w = 128; w > 0; w >>= 1) {
+    if (threadIdx.x < w) red[threadIdx.x] += red[threadIdx.x + w];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    const float reg = (float)red[0];
+    loss[0] += reg;
+    loss[1] += reg;
   }
 }
 
@@ -912,16 +965,17 @@ int mm_cross_backward(const float* x0, int64_t x0_stride, const float* z, int64_
   return mm::check_launch("mm_cross_backward");
 }
 
-int mm_concat_backward(const float* const* addends_host, const int64_t* addend_strides_host, int n_addends, int64_t B, int d,
-                       const mm_column_slice* slices_host, int n_slices, void* stream) {
+// The checks both concat backward entry points share, and their parameters; *blocks = the grid's x extent (0 when B == 0).
+static int concat_backward_params(const char* fn, const float* const* addends_host, const int64_t* addend_strides_host,
+                                  int n_addends, int64_t B, int d, const mm_column_slice* slices_host, int n_slices,
+                                  long long max_blocks, mm::trn::ConcatBwdParams& q, long long* blocks) {
   using namespace mm::trn;
-  MM_REQUIRE(addends_host && addend_strides_host && slices_host && B >= 0 && d >= 1, MM_ERR_ARG, "mm_concat_backward: null pointer or d < 1");
-  MM_REQUIRE(n_addends >= 1 && n_addends <= CB_MAX_ADD, MM_ERR_ARG, "mm_concat_backward: n_addends=%d outside [1, %d]", n_addends, CB_MAX_ADD);
-  MM_REQUIRE(n_slices >= 1 && n_slices <= CB_MAX_SLICES, MM_ERR_ARG, "mm_concat_backward: n_slices=%d outside [1, %d]", n_slices, CB_MAX_SLICES);
-  ConcatBwdParams q;
+  MM_REQUIRE(addends_host && addend_strides_host && slices_host && B >= 0 && d >= 1, MM_ERR_ARG, "%s: null pointer or d < 1", fn);
+  MM_REQUIRE(n_addends >= 1 && n_addends <= CB_MAX_ADD, MM_ERR_ARG, "%s: n_addends=%d outside [1, %d]", fn, n_addends, CB_MAX_ADD);
+  MM_REQUIRE(n_slices >= 1 && n_slices <= CB_MAX_SLICES, MM_ERR_ARG, "%s: n_slices=%d outside [1, %d]", fn, n_slices, CB_MAX_SLICES);
   memset(&q, 0, sizeof(q));
   for (int a = 0; a < n_addends; ++a) {
-    MM_REQUIRE(addends_host[a] && addend_strides_host[a] >= d, MM_ERR_ARG, "mm_concat_backward: addend %d: null or stride < d", a);
+    MM_REQUIRE(addends_host[a] && addend_strides_host[a] >= d, MM_ERR_ARG, "%s: addend %d: null or stride < d", fn, a);
     q.add[a] = addends_host[a];
     q.ld[a] = addend_strides_host[a];
   }
@@ -929,20 +983,58 @@ int mm_concat_backward(const float* const* addends_host, const int64_t* addend_s
   for (int t = 0; t < n_slices; ++t) {
     const mm_column_slice& s = slices_host[t];
     MM_REQUIRE(s.dst && s.width >= 4 && (s.width & 3) == 0 && s.col >= 0 && (int64_t)s.col + s.width <= d, MM_ERR_ARG,
-               "mm_concat_backward: slice %d: null destination, width not a positive multiple of 4, or columns outside [0, d)", t);
+               "%s: slice %d: null destination, width not a positive multiple of 4, or columns outside [0, d)", fn, t);
     MM_REQUIRE(s.dst_stride >= s.width && (s.dst_stride & 3) == 0 && ((uintptr_t)s.dst & 15) == 0, MM_ERR_ALIGN,
-               "mm_concat_backward: slice %d: destination must be 16-byte aligned with a row stride >= width and a multiple of 4", t);
+               "%s: slice %d: destination must be 16-byte aligned with a row stride >= width and a multiple of 4", fn, t);
     q.s[t] = s;
     if (s.width / 4 > qmax) qmax = s.width / 4;
   }
   q.B = B;
   q.n_add = n_addends;
+  *blocks = (B * qmax + 255) / 256;
+  if (*blocks > max_blocks) *blocks = max_blocks;
+  return MM_OK;
+}
+
+int mm_concat_backward(const float* const* addends_host, const int64_t* addend_strides_host, int n_addends, int64_t B, int d,
+                       const mm_column_slice* slices_host, int n_slices, void* stream) {
+  using namespace mm::trn;
+  ConcatBwdParams q;
+  long long blocks = 0;
+  const int rc = concat_backward_params("mm_concat_backward", addends_host, addend_strides_host, n_addends, B, d, slices_host,
+                                        n_slices, 4LL * mm::sm_count(), q, &blocks);
+  if (rc != MM_OK) return rc;
   if (B == 0) return MM_OK;
-  long long blocks = (B * qmax + 255) / 256;
-  const long long cap = 4LL * mm::sm_count();
-  if (blocks > cap) blocks = cap;
-  concat_backward_kernel<<<dim3((unsigned)blocks, (unsigned)n_slices), 256, 0, (cudaStream_t)stream>>>(q);
+  concat_backward_kernel<false><<<dim3((unsigned)blocks, (unsigned)n_slices), 256, 0, (cudaStream_t)stream>>>(q);
   return mm::check_launch("mm_concat_backward");
+}
+
+int mm_concat_backward_l2(const float* const* addends_host, const int64_t* addend_strides_host, int n_addends, int64_t B, int d,
+                          const mm_column_slice* slices_host, int n_slices, const float* x0, int64_t x0_stride,
+                          const float* l2_host, float* partials, int64_t n_partials, float* loss, void* stream) {
+  using namespace mm::trn;
+  ConcatBwdParams q;
+  long long blocks = 0;
+  const long long cap = std::min(4LL * mm::sm_count(), (long long)MM_CONCAT_L2_CTAS);
+  const int rc = concat_backward_params("mm_concat_backward_l2", addends_host, addend_strides_host, n_addends, B, d, slices_host,
+                                        n_slices, cap, q, &blocks);
+  if (rc != MM_OK) return rc;
+  MM_REQUIRE(x0 && x0_stride >= d && l2_host && partials && loss, MM_ERR_ARG,
+             "mm_concat_backward_l2: null x0 / l2 / partials / loss, or x0_stride < d");
+  MM_REQUIRE(n_partials >= (int64_t)n_slices * MM_CONCAT_L2_CTAS, MM_ERR_ARG,
+             "mm_concat_backward_l2: partials must hold n_slices * %d = %lld floats, got %lld", MM_CONCAT_L2_CTAS,
+             (long long)n_slices * MM_CONCAT_L2_CTAS, (long long)n_partials);
+  for (int t = 0; t < n_slices; ++t) {
+    MM_REQUIRE(l2_host[t] >= 0.f && l2_host[t] <= 3.0e38f, MM_ERR_ARG, "mm_concat_backward_l2: l2[%d] must be finite and >= 0", t);
+    q.l2[t] = l2_host[t];
+  }
+  q.x0 = x0;
+  q.ldx = x0_stride;
+  q.partials = partials;
+  if (B == 0) return MM_OK;
+  concat_backward_kernel<true><<<dim3((unsigned)blocks, (unsigned)n_slices), 256, 0, (cudaStream_t)stream>>>(q);
+  concat_l2_fold_kernel<<<1, 256, 0, (cudaStream_t)stream>>>(partials, (int)(blocks * n_slices), loss);
+  return mm::check_launch("mm_concat_backward_l2");
 }
 
 int mm_heads_fwd_bwd(const float* x, int64_t M, int K, int64_t x_stride, int H, const float* w, const float* bias,

@@ -449,7 +449,7 @@ class InputBlock(Block):
                  aggregation: Optional[str] = None, name: Optional[str] = None, **kwargs):
         super().__init__(name or unique_name("input_block"))
         self.schema = schema
-        opts = embedding_options
+        opts = self.embedding_options = embedding_options  # the training step reads embeddings_l2_reg from it
         cat = schema.select_by_tag(Tags.CATEGORICAL).excluding_by_tag(Tags.TARGET)
         con = schema.select_by_tag(Tags.CONTINUOUS).excluding_by_tag(Tags.TARGET)
         dims = dict(opts.embedding_dims or {})

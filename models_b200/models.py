@@ -17,7 +17,7 @@ from .blocks import (FM, MLP, CategoryEncoding, CrossBlock, CrossBlockSeq, DLRM,
                      dense_engine, run_dense_chain)
 from .core import Block, Prediction, TabularData, batch_size_of, default_device, to_device, unique_name
 from .inputs import EmbeddingOptions, EmbeddingsBlock, InputBlockV2
-from .retrieval import ItemRetrievalTask, TwoTowerBlock
+from .retrieval import ItemRetrievalTask, QueryItemIdsEmbeddingsBlock, TwoTowerBlock
 from .schema import Schema, Tags
 
 
@@ -527,6 +527,10 @@ class Model(Block, metaclass=_ModelMeta):
             out.update({f"{o.name}_loss": loss[1 + h] for h, o in enumerate(outs)})
         return out
 
+    # train_step entries that fit does not average into the History besides "loss" (a ranking model's regularization_loss
+    # is always 0)
+    _fit_skip = ("loss", "loss_batch", "regularization_loss")
+
     def fit(self, x=None, y=None, batch_size: Optional[int] = None, epochs: int = 1, steps_per_epoch: Optional[int] = None,
             verbose: int = 0, **kwargs):
         """Keras `fit` over a models_b200.Loader (or any iterable of (inputs, targets)): returns a History-like object
@@ -550,7 +554,7 @@ class Model(Block, metaclass=_ModelMeta):
                 if train_metrics is not None and n % every == 0:
                     self._update_train_metrics(train_metrics, targets)
                 # the loss-buffer views are valid until the next step: [loss_batch, per-output losses...] summed on the device
-                vec = torch.stack([m["loss_batch"]] + [v for k, v in m.items() if k not in ("loss", "loss_batch", "regularization_loss")])
+                vec = torch.stack([m["loss_batch"]] + [v for k, v in m.items() if k not in self._fit_skip])
                 total = vec.clone() if total is None else total + vec
                 n += 1
                 if steps_per_epoch and n >= steps_per_epoch:
@@ -559,7 +563,7 @@ class Model(Block, metaclass=_ModelMeta):
                 raise ValueError("fit: the loader produced no batches")
             means = (total / n).tolist()
             history["loss"].append(float(total[0].item()) / n)
-            for i, k in enumerate([k for k in m if k not in ("loss", "loss_batch", "regularization_loss")]):
+            for i, k in enumerate([k for k in m if k not in self._fit_skip]):
                 history.setdefault(k, []).append(means[1 + i])
             self._trainer.check_indices()
             self._fit_epoch_end(epoch, history, train_metrics, kwargs)
@@ -1283,10 +1287,12 @@ def _brute_force(k: int):
 
 
 class RetrievalModel(Model):
-    """models/base.py:2259-2489.  `compile(optimizer=...)` / `train_step` / `fit` train a v1 TwoTowerModel with its
-    ItemRetrievalTask's in-batch soft-max cross-entropy (models_b200/train.py: TwoTowerTrainer)."""
+    """models/base.py:2259-2489.  `compile(optimizer=...)` / `train_step` / `fit` train a v1 TwoTowerModel or a
+    MatrixFactorizationModel with its ItemRetrievalTask's in-batch soft-max cross-entropy plus the embeddings' L2 term
+    (models_b200/train.py: TwoTowerTrainer)."""
 
     _TRANSIENT = {"pre_eval_topk": None}
+    _fit_skip = ("loss", "loss_batch")  # History: "loss" and "regularization_loss"
 
     def train_step(self, data) -> Dict[str, torch.Tensor]:
         """One optimizer step on `data` = (inputs,) or (inputs, targets); the targets are ignored, because the retrieval task
@@ -1303,8 +1309,8 @@ class RetrievalModel(Model):
         x = data[0]
         self._check_inputs(x)
         tr = self.trainer(batch_size_of(x))
-        loss = tr.step(x, None)
-        return {"loss": loss[0], "loss_batch": loss[0], "regularization_loss": torch.zeros((), device=loss.device)}
+        loss = tr.step(x, None)  # [total, regularization]: the embeddings' L2 term is part of the total
+        return {"loss": loss[0], "loss_batch": loss[0], "regularization_loss": loss[1]}
 
     def fit(self, x=None, y=None, batch_size: Optional[int] = None, epochs: int = 1, steps_per_epoch: Optional[int] = None,
             verbose: int = 0, **kwargs):
@@ -1513,3 +1519,20 @@ def TwoTowerModel(schema: Schema, query_tower: MLP, item_tower: Optional[MLP] = 
                               query_tower_tag=query_tower_tag, item_tower_tag=item_tower_tag,
                               embedding_options=embedding_options, post=post)
     return RetrievalModel(two_tower, prediction_tasks, schema)
+
+
+def MatrixFactorizationModel(schema: Schema, dim: int, query_id_tag=Tags.USER_ID, item_id_tag=Tags.ITEM_ID,
+                             embeddings_initializers=None, embeddings_l2_reg: float = 0.0, post: Optional[Block] = None,
+                             prediction_tasks=None, logits_temperature: float = 1.0, samplers: Sequence = (),
+                             **kwargs) -> RetrievalModel:
+    """models/retrieval.py:27-103: a RetrievalModel over QueryItemIdsEmbeddingsBlock (user-id and item-id embeddings
+    of width `dim`, no MLP) with an ItemRetrievalTask (in-batch negatives by default).  embeddings_l2_reg adds
+    embeddings_l2_reg * sum ||e||^2 over the batch's looked-up embeddings to the training loss."""
+    if not prediction_tasks:
+        prediction_tasks = ItemRetrievalTask(schema, logits_temperature=logits_temperature, samplers=list(samplers), **kwargs)
+    if isinstance(prediction_tasks, (list, tuple)):
+        prediction_tasks = prediction_tasks[0]
+    mf = QueryItemIdsEmbeddingsBlock(schema=schema, dim=dim, query_id_tag=query_id_tag, item_id_tag=item_id_tag,
+                                     embeddings_initializers=embeddings_initializers, embeddings_l2_reg=embeddings_l2_reg,
+                                     post=post)
+    return RetrievalModel(mf, prediction_tasks, schema)

@@ -1300,6 +1300,35 @@ def concat_backward(addends: Sequence[torch.Tensor], slices: Sequence[tuple]) ->
     _cabi.check(_lib().mm_concat_backward(ap, st, len(addends), B, d, arr, len(slices), _stream()), "mm_concat_backward")
 
 
+def concat_l2_workspace(n_slices: int, device) -> torch.Tensor:
+    """The per-CTA partials concat_backward_l2 needs for up to n_slices slices."""
+    return torch.zeros(n_slices * _cabi.CONCAT_L2_CTAS, dtype=torch.float32, device=device)
+
+
+def concat_backward_l2(addends: Sequence[torch.Tensor], slices: Sequence[tuple], x0: torch.Tensor, l2: Sequence[float],
+                       loss: torch.Tensor, partials: torch.Tensor) -> None:
+    """concat_backward plus the embeddings' L2 penalty (mm_concat_backward_l2): for each (dst (B, w), col) in `slices` with
+    factor l2[t], dst = sum of the addends' columns [col, col + w) + 2 l2[t] x0[:, col:col + w]; reg = sum_t l2[t] ||x0's
+    columns of t||^2 is added to loss[0] (the total) and loss[1] in a fixed order.  partials: concat_l2_workspace."""
+    if not addends:
+        raise ValueError("concat_backward needs at least one addend")
+    B, d = addends[0].shape
+    _dev(x0, "x0", torch.float32), _dev(loss, "loss", torch.float32), _dev(partials, "partials", torch.float32)
+    if tuple(x0.shape) != (B, d):
+        raise ValueError(f"x0 must be ({B}, {d}), got {tuple(x0.shape)}")
+    if len(l2) != len(slices):
+        raise ValueError(f"one l2 factor per slice expected ({len(slices)}), got {len(l2)}")
+    if loss.numel() != 2 or not loss.is_contiguous():
+        raise ValueError("loss must hold 2 contiguous values [total, regularization]")
+    if not partials.is_contiguous():
+        raise ValueError("partials must be contiguous")
+    ap, st, arr = _addends_slices(addends, slices, B, d)
+    lam = (C.c_float * max(len(l2), 1))(*[float(v) for v in l2])
+    _cabi.check(_lib().mm_concat_backward_l2(ap, st, len(addends), B, d, arr, len(slices), x0.data_ptr(), _row_stride(x0, "x0"), lam,
+                                             partials.data_ptr(), partials.numel(), loss.data_ptr(), _stream()),
+                "mm_concat_backward_l2")
+
+
 def dense_apply(opt: str, w: torch.Tensor, grad: torch.Tensor, state1: Optional[torch.Tensor], state2: Optional[torch.Tensor],
                 hyper: torch.Tensor, grad_scale: float = 1.0) -> None:
     """Optimizer step over a flat fp32 arena; grad is scaled by grad_scale and cleared (mm_dense_apply)."""

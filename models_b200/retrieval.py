@@ -35,27 +35,31 @@ class L2Norm(Block):
 class TowerBlock(Block):
     """One tower: legacy InputBlock(schema subset) -> tower MLP (two_tower.py:98-118).  The
     sorted-name concat that the first _Dense applies to the InputBlock's dict is produced directly
-    by the fused gather (embeddings land at their concat offsets)."""
+    by the fused gather (embeddings land at their concat offsets).  mlp=None: the tower is the concat
+    of its embeddings (QueryItemIdsEmbeddingsBlock)."""
 
-    def __init__(self, inputs: InputBlock, mlp: MLP, name: str):
+    def __init__(self, inputs: InputBlock, mlp: Optional[MLP], name: str):
         super().__init__(name)
         self.inputs = inputs
         self.mlp = mlp
 
     def build(self, device=None):
         self.inputs.build(device)
-        _, _, width = self.inputs.layout()
-        self.mlp.build_from_width(width, device)
+        if self.mlp is not None:
+            _, _, width = self.inputs.layout()
+            self.mlp.build_from_width(width, device)
         self.built = True
         return self
 
     def weights(self):
         out = {f"inputs/{k}": v for k, v in self.inputs.weights().items()}
-        out.update({f"mlp/{k}": v for k, v in self.mlp.weights().items()})
+        if self.mlp is not None:
+            out.update({f"mlp/{k}": v for k, v in self.mlp.weights().items()})
         return out
 
     def call(self, inputs: TabularData, **kwargs) -> torch.Tensor:
-        return self.mlp(self.inputs.concat(inputs), **kwargs)
+        x = self.inputs.concat(inputs)
+        return x if self.mlp is None else self.mlp(x, **kwargs)
 
 
 class TwoTowerBlock(Block):
@@ -116,6 +120,30 @@ class TwoTowerBlock(Block):
         if self.post is not None:
             out = self.post(out)
         return out
+
+
+class QueryItemIdsEmbeddingsBlock(TwoTowerBlock):
+    """blocks/retrieval/matrix_factorization.py:31-112: a dual encoder whose towers are the id embeddings themselves
+    (no MLP): the query tower embeds the columns tagged `query_id_tag`, the item tower those tagged `item_id_tag`, each
+    table `dim` wide, with EmbeddingOptions(embedding_dim_default=dim, embeddings_l2_reg=...).  The training step adds
+    embeddings_l2_reg * sum ||e||^2 over the batch's looked-up embeddings to the loss, as the reference does."""
+
+    def __init__(self, schema: Schema, dim: int, query_id_tag=Tags.USER_ID, item_id_tag=Tags.ITEM_ID,
+                 embeddings_initializers=None, embeddings_l2_reg: float = 0.0, post: Optional[Block] = None, **kwargs):
+        if schema is None:
+            raise ValueError("The schema is required by QueryItemIdsEmbeddingsBlock")
+        if embeddings_l2_reg < 0:
+            raise ValueError(f"embeddings_l2_reg must be >= 0, got {embeddings_l2_reg}")
+        opts = EmbeddingOptions(embedding_dim_default=int(dim), embeddings_l2_reg=float(embeddings_l2_reg),
+                                embeddings_initializers=embeddings_initializers or None)
+        towers = []
+        for tag, name in ((query_id_tag, "query"), (item_id_tag, "item")):
+            sub = schema.select_by_tag(tag)
+            if not sub:
+                raise ValueError(f"The schema should contain features with the tag `{tag}`, required by the {name} embeddings")
+            towers.append(TowerBlock(InputBlock(sub, embedding_options=opts), None, name))
+        super().__init__(schema, towers[0], towers[1], post=post)
+        self.dim = int(dim)
 
 
 # ------------------------------------------------------------------------------------------------

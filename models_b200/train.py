@@ -31,7 +31,9 @@ one-hot features.
 DCNModel trains through DCNTrainer (below): the cross network's backward (mm_cross_backward per layer), the input block's
 backward straight into per-table slices (mm_concat_backward) and one sparse update per distinct embedding width.
 The v1 TwoTowerModel trains through TwoTowerTrainer: both towers as DCN's input block + deep tower, the in-batch soft-max
-cross-entropy forward and backward without the (B, 1+B) logits (mm_inbatch_softmax_ce[_backward]).
+cross-entropy forward and backward without the (B, 1+B) logits (mm_inbatch_softmax_ce[_backward]).  MatrixFactorizationModel
+trains there too, with towers that are the id embeddings themselves; the embeddings' L2 term (embeddings_l2_reg) is fused
+into the input block's backward (mm_concat_backward_l2).
 DeepFMModel trains through DeepFMTrainer: DCN's input block and deep tower, the FM / wide / output head forward and
 backward in one kernel (mm_deepfm_head_fwd_bwd), the FM term's input gradient (mm_fm_concat_backward) and the wide
 kernel's sparse update (mm_wide_rows_apply).
@@ -490,7 +492,8 @@ class _StepTrainer:
         a = self.arena
         ops.opt_tick(self.hyper)
         idx, slices, rows, scale = self._gradients_to_apply()
-        ops.dense_apply(self.opt.kind, a.w, a.grad, a.state1, a.state2, self.hyper, grad_scale=scale)
+        if a.size:  # a model without Dense layers (matrix factorization) has an empty arena
+            ops.dense_apply(self.opt.kind, a.w, a.grad, a.state1, a.state2, self.hyper, grad_scale=scale)
         for D, ts in self._by_width.items():
             onehot = [t for t in ts if t not in self._bags]
             for s in range(0, len(onehot), SPARSE_MAX_TABLES):
@@ -644,6 +647,9 @@ class _ConcatInput:
             cont = sorted(ib.continuous.features) if ib.continuous is not None else []
         self.feats, self.cont = list(feats), list(cont)
         self.tidx: List[int] = []
+        # embeddings_l2_reg per feature (set by a trainer that applies it) and mm_concat_backward_l2's partials
+        self.l2_reg: List[float] = [0.0] * len(self.feats)
+        self.l2_ws: Optional[torch.Tensor] = None
         self.oob = self.emb.counter(tr.device) if self.emb is not None else None
         f32 = dict(dtype=torch.float32, device=tr.device)
         self.x0 = torch.zeros((tr.B, _ld4(self.d)), **f32)
@@ -691,16 +697,27 @@ class _ConcatInput:
         ops.split_rows(x0, out=xs)
         return x0, xs, dx0
 
+    def set_l2_reg(self, l2: float) -> None:
+        """Apply embeddings_l2_reg = l2 to every table of the block: its gradient joins the backward, the term the loss."""
+        self.l2_reg = [float(l2)] * len(self.feats)
+        if l2 and self.l2_ws is None:
+            self.l2_ws = ops.concat_l2_workspace(min(len(self.feats), CONCAT_MAX_SLICES), self.tr.device)
+
     def backward(self, addends, b: int, fm: Optional[torch.Tensor] = None) -> None:
         """The tables' columns of the summed (b, d) addends into each table's slice of the trainer's _slices; fm: the FM
-        term's ds (b,), whose input gradient from x0 is added (mm_fm_concat_backward)."""
+        term's ds (b,), whose input gradient from x0 is added (mm_fm_concat_backward).  Tables with an L2 factor also get
+        2 l2 x0 (mm_concat_backward_l2), and the term goes into the trainer's loss vector [total, regularization]."""
         tr = self.tr
         slices = [(tr._slices[t], self.cols[f]) for t, f in zip(self.tidx, self.feats)]
         for s in range(0, len(slices), CONCAT_MAX_SLICES):
-            if fm is None:
-                ops.concat_backward(addends, slices[s:s + CONCAT_MAX_SLICES])
-            else:
+            l2 = self.l2_reg[s:s + CONCAT_MAX_SLICES]
+            if fm is not None:
                 ops.fm_concat_backward(addends, self.x0[:b, :self.d], fm, slices[s:s + CONCAT_MAX_SLICES])
+            elif any(l2):
+                ops.concat_backward_l2(addends, slices[s:s + CONCAT_MAX_SLICES], self.x0[:b, :self.d], l2, tr._loss_all[:2],
+                                       self.l2_ws)
+            else:
+                ops.concat_backward(addends, slices[s:s + CONCAT_MAX_SLICES])
 
 
 class _WideKernel:
@@ -1088,7 +1105,13 @@ class DCNTrainer(_StepTrainer):
 class TwoTowerTrainer(_StepTrainer):
     """Static-buffer training step of a v1 TwoTowerModel (RetrievalModel over a TwoTowerBlock, ItemRetrievalTask with
     in-batch negatives and false negatives down-scored by the item-id column) at one batch size; a smaller batch b runs in
-    the leading rows with its own b items as the negatives.
+    the leading rows with its own b items as the negatives.  A MatrixFactorizationModel trains here too: its towers have
+    no Dense layers, so a tower's output is its input block's x0 (and, without post, x0's split operand xs is what the
+    in-batch kernels read), the arena is empty and neither mm_dense_apply nor mm_split_weights runs.
+
+    The loss vector is [total, regularization]: with embeddings_l2_reg > 0 in a tower's EmbeddingOptions, the tower's
+    mm_concat_backward becomes mm_concat_backward_l2, which adds 2 l2 e to the tables' IndexedSlices and l2 sum ||e||^2
+    over the batch's looked-up (pooled) embeddings to both entries (the reference's EmbeddingFeatures.add_loss).
 
     forward   per tower: gather of its tables' rows (mm_gather_multi; ragged bags mm_gather_bag, (B, L) ids mm_gather_seq)
               and its continuous columns (mm_concat_columns) into x0 at their sorted-name offsets, its split operand, one
@@ -1133,11 +1156,14 @@ class TwoTowerTrainer(_StepTrainer):
         self.H = 1
         self.towers, self.inps = [], []  # per tower: its layers and buffers, its input block
         for tb in (body.query, body.item):
-            self._check_mlps([tb.mlp])
-            self._check_activations(tb.mlp.dense_layers)
-            self.towers.append(dict(name=tb.name, layers=tb.mlp.dense_layers))
-            self.inps.append(_ConcatInput(self, tb.inputs, dx0=True))  # a tower without tables has nothing below x0
-        out_w = {t["layers"][-1].units for t in self.towers}
+            layers = [] if tb.mlp is None else tb.mlp.dense_layers
+            if tb.mlp is not None:
+                self._check_mlps([tb.mlp])
+                self._check_activations(layers)
+            self.towers.append(dict(name=tb.name, layers=layers))
+            # a tower without tables has nothing below x0; a tower without layers hands its output gradient to the input block
+            self.inps.append(_ConcatInput(self, tb.inputs, dx0=bool(layers)))
+        out_w = {t["layers"][-1].units if t["layers"] else inp.d for t, inp in zip(self.towers, self.inps)}
         if len(out_w) != 1:
             raise ValueError(f"the query and item towers must end in the same width, got {sorted(out_w)}")
         self.D = out_w.pop()
@@ -1145,12 +1171,15 @@ class TwoTowerTrainer(_StepTrainer):
             raise NotImplementedError(f"tower output width {self.D}: the in-batch soft-max kernels take up to 128")
 
         self._init_inputs(self.inps)
+        for tb, inp in zip((body.query, body.item), self.inps):
+            inp.set_l2_reg(getattr(getattr(tb.inputs, "embedding_options", None), "embeddings_l2_reg", 0.0))
         self._init_dense([l for t in self.towers for l in t["layers"]], [])
         first_layer = {}
         li = 0
         for t, inp in zip(self.towers, self.inps):
             t["li0"] = li
-            first_layer[li] = bool(inp.feats)  # the first layer needs its input gradient only when the tower has tables
+            if t["layers"]:
+                first_layer[li] = bool(inp.feats)  # the first layer needs its input gradient only when the tower has tables
             li += len(t["layers"])
         self._init_wide(lambda i: first_layer.get(i, True))
 
@@ -1160,14 +1189,17 @@ class TwoTowerTrainer(_StepTrainer):
         bf = dict(dtype=torch.bfloat16, device=self.device)
         for t in self.towers:
             t["h"], t["h_split"], t["dh"] = self._chain_buffers(t["layers"])
+            t["dout"] = t["dh"][-1] if t["layers"] else torch.zeros((B, self.D), **f32)  # the gradient of the tower's output
             t["y"] = torch.zeros((B, self.D), **f32) if self.l2 else None  # the normalised output
-            t["split"] = torch.zeros((B, 2 * ops.tc_padded_k(self.D)), **bf)
+            # the in-batch kernels' operand of the output; a tower without layers or post hands them x0's split xs
+            t["split"] = torch.zeros((B, 2 * ops.tc_padded_k(self.D)), **bf) if (t["layers"] or self.l2) else None
         self.pos_logit = torch.zeros(B, **f32)
         self.stats = torch.zeros((B, 3), **f32)
         ws = max(ops.catalog_workspace_bytes(min(128 * m, B), min(128 * m, B)) for m in range(1, (B + 127) // 128 + 1))
         self.ws = torch.zeros(ws, dtype=torch.uint8, device=self.device)
         self._inv_b: Dict[int, torch.Tensor] = {}  # c = 1/b per batch size, one device float each
         self._init_loss(B)
+        self.loss = self._loss_all  # [total, regularization]
         self.logits = self.stats  # [max, log-sum-exp, positive logit] of every row of the last step
         # one counter for both towers (every gather receives it), so check_indices sees every table
         self.oob = next((p.oob for p in self.inps if p.oob is not None), None)
@@ -1213,19 +1245,31 @@ class TwoTowerTrainer(_StepTrainer):
             c = self._inv_b[b] = torch.full((1,), 1.0 / b, dtype=torch.float32, device=self.device)
         return c
 
-    def _tower_forward(self, tw: dict, inp: _ConcatInput, inputs, b: int) -> torch.Tensor:
-        _, xs, _ = inp.forward(inputs, b)
-        h = [x[:b] for x in tw["h"]]
-        self._chain_forward(xs, inp.d, tw["li0"], tw["layers"], h, [x[:b] for x in tw["h_split"]])
-        out = h[-1]
+    def _tower_forward(self, tw: dict, inp: _ConcatInput, inputs, b: int) -> tuple:
+        """(the tower's (normalised) output, its split operand)."""
+        x0, xs, _ = inp.forward(inputs, b)
+        if not tw["layers"] and not self.l2:
+            return x0, xs
+        out = x0
+        if tw["layers"]:
+            h = [x[:b] for x in tw["h"]]
+            self._chain_forward(xs, inp.d, tw["li0"], tw["layers"], h, [x[:b] for x in tw["h_split"]])
+            out = h[-1]
         if self.l2:
             out = ops.l2_normalize(out, out=tw["y"][:b])
         ops.split_rows(out, out=tw["split"][:b])
-        return out
+        return out, tw["split"][:b]
 
     def _tower_backward(self, tw: dict, inp: _ConcatInput, dout: torch.Tensor, b: int) -> None:
-        """dout: gradient of the tower's (normalised) output, overwritten by the pre-activation gradient of the last layer."""
+        """dout: gradient of the tower's (normalised) output, overwritten by the pre-activation gradient of the last layer
+        (without layers: by the gradient of x0)."""
         h, dh, layers = [x[:b] for x in tw["h"]], [x[:b] for x in tw["dh"]], tw["layers"]
+        if not layers:
+            x0, _, _ = inp.views(b)
+            if self.l2:
+                ops.l2_normalize_backward(x0, dout, dout)
+            inp.backward([dout], b)
+            return
         if self.l2:
             ops.l2_normalize_backward(h[-1], dout, dout)
         if layers[-1].activation == "relu":
@@ -1242,15 +1286,14 @@ class TwoTowerTrainer(_StepTrainer):
         if sample_weight is not None and not (isinstance(sample_weight, (list, tuple)) and all(s is None for s in sample_weight)):
             raise NotImplementedError("sample_weight is not implemented in the two-tower training step")
         b, _, _ = self._begin_step(inputs, targets, sample_weight)
-        q, it = (self._tower_forward(tw, inp, inputs, b) for tw, inp in zip(self.towers, self.inps))
-        qs, its = self.towers[0]["split"][:b], self.towers[1]["split"][:b]
+        (q, qs), (it, its) = (self._tower_forward(tw, inp, inputs, b) for tw, inp in zip(self.towers, self.inps))
         ids = ops.as_index(inputs[self.item_id]).reshape(-1) if self.downscore else None  # packed host-batch ids widened
         T = self.temperature
         ops.positive_scores(q, it, self.pos_logit[:b], temperature=T)
         ops.inbatch_softmax_ce_split(qs, its, self.D, self.pos_logit[:b], self.stats[:b], self.ws, pos_ids=ids, neg_ids=ids,
                                      downscore=self.downscore, false_neg_score=self.false_neg_score, temperature=T)
         # dq -> the query tower's last dh, d_item = dpos + dneg (the negatives are the positives) -> the item tower's
-        dq, di = self.towers[0]["dh"][-1][:b], self.towers[1]["dh"][-1][:b]
+        dq, di = self.towers[0]["dout"][:b], self.towers[1]["dout"][:b]
         ops.inbatch_softmax_ce_backward(qs, its, self.D, self.stats[:b], q, it, self._scale(b), dq, di, di, loss=self._loss_all[:1],
                                         pos_ids=ids, neg_ids=ids, downscore=self.downscore, false_neg_score=self.false_neg_score,
                                         temperature=T)
