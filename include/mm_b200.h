@@ -789,6 +789,29 @@ int mm_mmoe_task_heads_fwd_bwd(const float* const* x_host, const int64_t* x_stri
                                float* const* dx_host, const int64_t* dx_strides_host, int mask_relu, float* dw, float* db,
                                void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * K20  Neural collaborative filtering head (NCFModel, models/benchmark.py:32-100): the GMF branch
+ *      (MatrixFactorizationBlock with ElementWiseMultiply) next to the MLP branch's output h, concatenated as [mf | mlp]
+ *      and read by the output heads.
+ *   mm_ncf_head_fwd_bwd  in one pass over the batch: u = table_u[ids_u[b]], i = table_i[ids_i[b]] (D wide; ids of
+ *       idx_bytes 1, 2, 3, 4 or 8 as mm_lookup_table's, checked alike; an id outside [0, rows) reads a zero row and bumps
+ *       *oob_count, nullable), z_t = [u * i | h] . w[:, t] + bias[t] with w the (D + U, H) Keras kernel and h (B, U) rows
+ *       h_stride apart.  Losses, targets, sample weights, loss weights, the loss vector (1 + H) and the forward-only form
+ *       (targets null: out (H, B) = the activated predictions) as mm_heads_fwd_bwd; training writes out = the logits,
+ *         du (B, D) = r * i + 2 l2 u,  di (B, D) = r * u + 2 l2 i,  r = sum_t delta_t w[:D, t]  (contiguous rows in sample
+ *         order: the IndexedSlices values of both tables),
+ *         dh (B, U) = sum_t delta_t w[D:, t] (zeroed where h <= 0 when relu_h; rows dh_stride apart)
+ *       and ACCUMULATES dw (D + U, H), db (H,) (nullable) and the loss.  reg (1 device float, nullable) ACCUMULATES
+ *       l2 sum_b (|u_b|^2 + |i_b|^2 + |x_reg_b|^2), x_reg (B, x_reg_width) rows x_reg_stride apart (nullable: none); in
+ *       training the term is also added to loss[0].  1 <= D <= 128, 1 <= U <= 256, 1 <= H <= 8, l2 finite and >= 0. */
+int mm_ncf_head_fwd_bwd(const float* table_u, int64_t rows_u, const void* ids_u, int idx_bytes_u, const float* table_i,
+                        int64_t rows_i, const void* ids_i, int idx_bytes_i, int D, const float* h, int64_t h_stride, int U,
+                        int relu_h, int64_t B, int H, const float* w, const float* bias, const int* loss_kind,
+                        const float* loss_weight, const void* const* targets, const int* target_dtypes,
+                        const float* const* sample_weights, float l2, const float* x_reg, int64_t x_reg_stride, int x_reg_width,
+                        float* out, float* loss, float* reg, float* du, float* di, float* dh, int64_t dh_stride, float* dw,
+                        float* db, int32_t* oob_count, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

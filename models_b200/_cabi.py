@@ -237,6 +237,9 @@ SIGNATURES = {
     "mm_mmoe_task_heads_fwd_bwd": (_i, [C.POINTER(C.c_void_p), C.POINTER(C.c_int64), _i64, _i, _i, _vp, _vp, C.POINTER(C.c_int),
                                         C.POINTER(C.c_float), C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_void_p),
                                         _vp, _vp, C.POINTER(C.c_void_p), C.POINTER(C.c_int64), _i, _vp, _vp, _vp]),
+    "mm_ncf_head_fwd_bwd": (_i, [_vp, _i64, _vp, _i, _vp, _i64, _vp, _i, _i, _vp, _i64, _i, _i, _i64, _i, _vp, _vp, C.POINTER(C.c_int),
+                                 C.POINTER(C.c_float), C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_void_p), _f, _vp,
+                                 _i64, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp]),
 }
 
 

@@ -330,15 +330,14 @@ class EvalGraph:
         return tuple(key)
 
     def _step(self) -> None:
-        z, form = self.model.logits(self.inputs)
-        self.state.update(z, self.targets, form, self.sample_weight)
+        self.model._eval_step(self.state, self.inputs, self.targets, self.sample_weight)
 
     def _capture(self) -> None:
         from . import ops
         from .core import weights_version
 
         st = self.state
-        saved = (st.state.clone(), st.before_last.clone())
+        saved = (st.state.clone(), st.before_last.clone(), None if st.reg is None else st.reg.clone())
         old_ns = set_buffer_namespace(self.namespace)
         try:
             # warm-up on a side stream (split kernels, scratch buffers, the fused head's host bias, the metric workspace);
@@ -352,6 +351,8 @@ class EvalGraph:
             torch.cuda.synchronize()
             st.state.copy_(saved[0])
             st.before_last.copy_(saved[1])
+            if st.reg is not None:  # created by the warm-up when the model has an L2 term
+                st.reg.copy_(saved[2]) if saved[2] is not None else st.reg.zero_()
             self.workspace = st.workspace  # the graph holds its address: keep it alive
             self.graph = torch.cuda.CUDAGraph()
             n0 = ops.launch_count()

@@ -238,18 +238,33 @@ class MetricsState:
         self.before_last = torch.zeros((H, 2), dtype=torch.float64, device=device)  # loss sum / count before the last batch
         self.workspace = torch.empty(0, dtype=torch.uint8, device=device)
 
+    # the embeddings' L2 term of a model that has one, created by its first update: [sum_k b_k reg_k, sum_k b_k, last reg_k]
+    reg: Optional[torch.Tensor] = None
+
     def reset(self) -> None:
         self.state.zero_()
         self.before_last.zero_()
+        if self.reg is not None:
+            self.reg.zero_()
 
     def reserve(self, M: int) -> None:
         need = ops.metrics_workspace_bytes(M, len(self.spec.outputs))
         if self.workspace.numel() < need:
             self.workspace = torch.empty(need, dtype=torch.uint8, device=self.device)
 
-    def update(self, z: torch.Tensor, targets: Sequence[torch.Tensor], pred_form: int, sample_weight=None) -> None:
+    def update(self, z: torch.Tensor, targets: Sequence[torch.Tensor], pred_form: int, sample_weight=None,
+               regularization: Optional[torch.Tensor] = None) -> None:
         """z (H, b) logits; targets one (b,) tensor per output; sample_weight None, one (b,) tensor or one per output (the
-        loss and the weighted metrics use it, the plain metrics do not)."""
+        loss and the weighted metrics use it, the plain metrics do not); regularization: one device float, the batch's
+        embeddings L2 term, added to the loss batch-size weighted as the batch losses are."""
+        if regularization is not None:
+            if self.reg is None:
+                self.reg = torch.zeros(3, dtype=torch.float64, device=self.device)
+            b = z.shape[1]
+            r = regularization.reshape(-1)[:1].to(torch.float64)
+            self.reg[:1].add_(r, alpha=float(b))
+            self.reg[1:2].add_(float(b))
+            self.reg[2:].copy_(r)
         H = len(self.spec.outputs)
         sws = list(sample_weight) if isinstance(sample_weight, (list, tuple)) else [sample_weight] * H
         sws = [None if w is None else w.reshape(-1).to(torch.float32).contiguous() for w in sws]
@@ -263,10 +278,12 @@ class MetricsState:
         """One device-to-host copy of the state -> {name: value} in `spec.result_names()` order.  Raises ValueError naming
         the outputs that saw invalid samples (a binary target outside {0, 1}, a NaN target or logit)."""
         spec = self.spec
-        host = torch.cat([self.state.reshape(-1), self.before_last.reshape(-1)]).cpu().numpy()
+        reg = self.reg if self.reg is not None else torch.zeros(3, dtype=torch.float64, device=self.state.device)
+        host = torch.cat([self.state.reshape(-1), self.before_last.reshape(-1), reg]).cpu().numpy()
+        reg_sum, reg_n, reg_last = host[-3:]
         H, T = len(spec.outputs), spec.num_buckets
         st = host[:self.state.numel()].reshape(H, -1)
-        prev = host[self.state.numel():].reshape(H, 2)
+        prev = host[self.state.numel():-3].reshape(H, 2)
         bad = [f"{n} ({int(st[h, _cabi.METRICS_INVALID])} samples)" for h, n in enumerate(spec.names) if st[h, _cabi.METRICS_INVALID]]
         if bad:
             raise ValueError(f"invalid targets or predictions for {', '.join(bad)}: binary targets must be 0 or 1, and no "
@@ -274,7 +291,7 @@ class MetricsState:
         L, N = st[:, _cabi.METRICS_LOSS], st[:, _cabi.METRICS_COUNT]
         per = _div(L, N)
         last = _div(L - prev[:, 0], N - prev[:, 1])
-        out = {"loss": float(np.dot(spec.loss_weights, per))}
+        out = {"loss": float(np.dot(spec.loss_weights, per)) + (float(reg_sum / reg_n) if reg_n else 0.0)}
         if not spec.single:
             out.update({f"{n}_loss": float(per[h]) for h, n in enumerate(spec.names)})
         S = _cabi.METRICS_SCALARS
@@ -299,6 +316,6 @@ class MetricsState:
                         else:
                             v = float(_div(tp, tp + fp))
                     out[prefix + m.name if spec.single else f"{n}/{prefix}{m.name}"] = v
-        out["regularization_loss"] = 0.0
-        out["loss_batch"] = float(np.dot(spec.loss_weights, last))
+        out["regularization_loss"] = float(reg_last)
+        out["loss_batch"] = float(np.dot(spec.loss_weights, last)) + float(reg_last)
         return out

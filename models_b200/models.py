@@ -522,7 +522,9 @@ class Model(Block, metaclass=_ModelMeta):
         self._check_inputs(x)
         tr = self.trainer(batch_size_of(x))
         loss = tr.step(x, y, sw)
-        out = {"loss": loss[0], "loss_batch": loss[0], "regularization_loss": torch.zeros((), device=loss.device)}
+        reg = getattr(tr, "regularization", None)  # the embeddings' L2 term, part of the total (NCF)
+        out = {"loss": loss[0], "loss_batch": loss[0],
+               "regularization_loss": torch.zeros((), device=loss.device) if reg is None else reg}
         if len(outs) > 1:
             out.update({f"{o.name}_loss": loss[1 + h] for h, o in enumerate(outs)})
         return out
@@ -674,6 +676,22 @@ class RankingModel(Model):
 
     _TRANSIENT = {"_pinned": {}, "_trainer": None, "_eval_state": None, "_fit_state": None, "_eval_graph": None}
 
+    @property
+    def _fit_skip(self):
+        # an NCF model's History records its regularization_loss, as matrix factorization's does
+        return ("loss", "loss_batch") if isinstance(self.body, NCFBody) else Model._fit_skip
+
+    def _eval_regularization(self, device) -> Optional[torch.Tensor]:
+        """The device float the forward leaves the batch's embeddings L2 term in (None: the model has none)."""
+        if isinstance(self.body, NCFBody) and self.body.embeddings_l2_reg:
+            return self.body.regularization(device)
+        return None
+
+    def _eval_step(self, state, inputs: TabularData, targets, sample_weight) -> None:
+        """One batch of evaluate: the logits forward and the metric update (with the batch's L2 term, if any)."""
+        z, form = self.logits(inputs)
+        state.update(z, targets, form, sample_weight, regularization=self._eval_regularization(z.device))
+
     def _distributed(self) -> bool:
         """Row-sharded tables or a data-parallel training engine: each rank sees only its share of the data."""
         return getattr(self.body, "sharded", None) is not None or getattr(getattr(self, "_trainer", None), "group", None) is not None
@@ -759,8 +777,7 @@ class RankingModel(Model):
                     sw = [sw] * len(outs)
                 key = EvalGraph.layout(inputs, ys, sw, dev) if _EVAL_GRAPH[0] and batch_size_of(inputs) == full else None
                 if key is None:
-                    z, form = self.logits(inputs)
-                    state.update(z, ys, form, sw)
+                    self._eval_step(state, inputs, ys, sw)
                 else:
                     g = getattr(self, "_eval_graph", None)
                     if g is None or g.key != key or g.state is not state:
@@ -900,6 +917,9 @@ class RankingModel(Model):
             return self.body.forward(inputs, out_layer=self.prediction.to_call, logits=logits)
         if isinstance(self.body, WideAndDeepBody):
             return self.body.forward(inputs, out_layer=self.prediction.to_call, logits=logits)
+        if isinstance(self.body, NCFBody):
+            out = self.body.forward(inputs, self.output_blocks(), self.prediction.to_call, logits=logits)
+            return heads.split(out) if heads is not None else out.view(-1, 1)
         if isinstance(self.body, MMoEBody) and (self.body.mmoe is not None or output_towers(self.prediction)):
             out = self.body.forward(inputs, self.output_blocks(), self.prediction.to_call, output_towers(self.prediction),
                                     logits=logits)
@@ -1268,6 +1288,127 @@ def WideAndDeepModel(schema: Schema, deep_block: Optional[MLP] = None, wide_sche
         raise ValueError("At least the deep part (deep_schema/deep_input_block) or wide part (wide_schema/wide_input_block) must be provided.")
     body = WideAndDeepBody(deep_input_block, deep, deep_logit, wide, regularized=deep_regularizer is not None or wide_regularizer is not None)
     return RankingModel(body, prediction, schema)
+
+
+class NCFBody(Block):
+    """ParallelBlock({"mf": MatrixFactorizationBlock(aggregation=ElementWiseMultiply()), "mlp":
+    QueryItemIdsEmbeddingsBlock -> mlp_block}, aggregation="concat") (models/benchmark.py:32-100): (B, D + U) = [u_mf * i_mf |
+    h], h = mlp_block([i_mlp | u_mlp]) (the first Dense concatenates the dict {"query", "item"} in sorted-key order: item
+    first).  Four tables, each `dim` wide: the GMF product never reaches memory, because the GMF rows are gathered by the
+    output-head kernel itself (ops.ncf_head_fwd_bwd), which also runs the output heads."""
+
+    def __init__(self, mf: QueryItemIdsEmbeddingsBlock, mlp_ids: QueryItemIdsEmbeddingsBlock, mlp: MLP, embeddings_l2_reg: float):
+        super().__init__(unique_name("ncf_body"))
+        self.mf, self.mlp_ids, self.mlp = mf, mlp_ids, mlp
+        self.embeddings_l2_reg = float(embeddings_l2_reg)
+        self.dim = mf.dim
+        for branch, blk in (("mf", mf), ("mlp", mlp_ids)):
+            for side in ("query", "item"):
+                ib = getattr(blk, side).inputs
+                cols = ib.schema.excluding_by_tag(Tags.TARGET)
+                if len(cols) != 1 or ib.embeddings is None or cols.first.is_list:
+                    raise NotImplementedError(f"NCFModel: the {branch} branch's {side} side needs exactly one non-list id column, "
+                                              f"got {cols.column_names}")
+        if self.dim % 4 or not 4 <= self.dim <= ops.NCF_MAX_WIDTH:
+            raise NotImplementedError(f"NCFModel: embedding_dim {self.dim} is not supported (it needs a multiple of 4 no larger "
+                                      f"than {ops.NCF_MAX_WIDTH})")
+        if not mlp.dense_layers or mlp.dense_layers[-1].units > ops.NCF_MAX_UNITS:
+            raise NotImplementedError(f"NCFModel: the head kernel reads at most {ops.NCF_MAX_UNITS} units of mlp_block's last layer")
+        # [item | query]: the first Dense of mlp_block concatenates {"query", "item"} in sorted-key order
+        self.mlp_columns = {self.feature("mlp", "item"): 0, self.feature("mlp", "query"): self.dim}
+        self.mlp_embeddings = EmbeddingsBlock({t.table_name: t for t in (self.table("mlp", "item"), self.table("mlp", "query"))},
+                                              mlp_ids.schema, name="mlp_embeddings")
+        # the training step's input block over the same two tables (its columns at mlp_columns, not in sorted-name order)
+        self.mlp_input_block = InputBlockV2(mlp_ids.schema.select_by_name(list(self.mlp_columns)), categorical=self.mlp_embeddings)
+        self._reg: Optional[torch.Tensor] = None
+
+    _TRANSIENT = {"_reg": None}
+
+    def feature(self, branch: str, side: str) -> str:
+        """The id column of one side ("query" / "item") of one branch ("mf" / "mlp")."""
+        return getattr(self.mf if branch == "mf" else self.mlp_ids, side).inputs.embeddings.feature_names[0]
+
+    def table(self, branch: str, side: str):
+        blk = self.mf if branch == "mf" else self.mlp_ids
+        emb = getattr(blk, side).inputs.embeddings
+        return emb.feature_to_table[emb.feature_names[0]]
+
+    def build(self, device=None):
+        from .core import create_variable
+
+        for side in ("query", "item"):  # the mlp branch's own initial values, not a copy of the mf table of the same name
+            t = self.table("mlp", side)
+            if t.table is None:
+                t.table = create_variable((t.input_dim, t.dim), t.embeddings_initializer, device or default_device(),
+                                          f"mlp/{t.table_name}/embeddings")
+        self.mf.build(device)
+        self.mlp_ids.build(device)
+        self.mlp.build_from_width(2 * self.dim, device)
+        self.built = True
+        return self
+
+    def output_width(self) -> int:
+        return self.dim + self.mlp.dense_layers[-1].units
+
+    def weights(self):
+        out = {f"mf/{k}": v for k, v in self.mf.weights().items()}
+        out.update({f"mlp/{k}": v for k, v in self.mlp_ids.weights().items()})
+        out.update({f"mlp/mlp/{k}": v for k, v in self.mlp.weights().items()})
+        return out
+
+    def ids(self, inputs: TabularData, side: str) -> torch.Tensor:
+        """The GMF id column of one side, as the head kernel reads it (packed host-batch ids at their own width)."""
+        from .core import get_feature
+
+        f = self.feature("mf", side)
+        x = get_feature(inputs, f)
+        if isinstance(x, tuple) or self.table("mf", side).lookup_kind(x) != "onehot":
+            raise NotImplementedError(f"NCFModel: feature {f!r} must be one id per sample (ragged / multi-hot ids are not "
+                                      "implemented)")
+        return ops.fused_ids(x)
+
+    def mlp_input(self, inputs: TabularData) -> torch.Tensor:
+        """(B, 2 D) = [i_mlp | u_mlp], through the embeddings' concat path."""
+        B = batch_size_of(inputs)
+        x0 = torch.empty((B, 2 * self.dim), dtype=torch.float32, device=next(iter(inputs.values())).device)
+        self.mlp_embeddings.lookup_all_into(inputs, x0, self.mlp_columns)
+        return x0
+
+    def regularization(self, device) -> torch.Tensor:
+        """One device float: the embeddings' L2 term of the last forward (with embeddings_l2_reg > 0)."""
+        if self._reg is None or self._reg.device != device:
+            self._reg = torch.zeros(1, dtype=torch.float32, device=device)
+        return self._reg
+
+    def forward(self, inputs: TabularData, outputs: Sequence[Block], head: _Dense, logits: bool = False) -> torch.Tensor:
+        """(H, B): the activated predictions of the outputs, or their logits with logits=True.  With embeddings_l2_reg > 0
+        the batch's L2 term over the four tables' looked-up rows lands in regularization()."""
+        from .blocks import _LAST_HEADS
+
+        dev = next(iter(inputs.values())).device
+        if not self.built:
+            self.build(dev)
+        x0 = self.mlp_input(inputs)
+        h = run_dense_chain(x0, self.mlp.dense_layers)
+        B, H = x0.shape[0], len(outputs)
+        out = torch.empty((H, B), dtype=torch.float32, device=dev)
+        losses = ["mse"] * H if logits else [o.loss for o in outputs]
+        l2 = self.embeddings_l2_reg
+        reg = None
+        if l2:
+            reg = self.regularization(dev)
+            reg.zero_()
+        emb = self.mf.query.inputs.embeddings
+        oob = emb.counter(dev)
+        _LAST_HEADS[0] = "heads"
+        ops.ncf_head_fwd_bwd(self.table("mf", "query").embeddings, self.ids(inputs, "query"), self.table("mf", "item").embeddings,
+                             self.ids(inputs, "item"), h, head.kernel, head.bias, losses, None, out, reg=reg, l2=l2,
+                             relu_h=False, x_reg=x0 if l2 else None, oob=oob)
+        emb.finish_check(oob)
+        return out
+
+    def call(self, inputs: TabularData, **kwargs):
+        raise NotImplementedError("NCFBody runs inside its RankingModel (the output heads are fused with the GMF branch)")
 
 
 def DCNModel(schema: Schema, depth: int, deep_block: Optional[MLP] = None, stacked: bool = True,

@@ -1080,6 +1080,94 @@ def mmoe_task_heads_fwd_bwd(xs: Sequence[torch.Tensor], w: torch.Tensor, bias: O
     return out
 
 
+NCF_MAX_WIDTH, NCF_MAX_UNITS, NCF_MAX_HEADS = 128, 256, 8  # mm_ncf_head_fwd_bwd
+
+
+def ncf_head_fwd_bwd(table_u: torch.Tensor, ids_u: torch.Tensor, table_i: torch.Tensor, ids_i: torch.Tensor, h: torch.Tensor,
+                     w: torch.Tensor, bias: Optional[torch.Tensor], losses: Sequence[str], targets: Optional[Sequence[torch.Tensor]],
+                     out: torch.Tensor, loss: Optional[torch.Tensor] = None, reg: Optional[torch.Tensor] = None, l2: float = 0.0,
+                     du: Optional[torch.Tensor] = None, di: Optional[torch.Tensor] = None, dh: Optional[torch.Tensor] = None,
+                     dw: Optional[torch.Tensor] = None, db: Optional[torch.Tensor] = None,
+                     loss_weights: Optional[Sequence[float]] = None, relu_h: bool = True, sample_weight=None,
+                     x_reg: Optional[torch.Tensor] = None, oob: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """NCF's GMF branch and output heads in one pass (mm_ncf_head_fwd_bwd): u = table_u[ids_u], i = table_i[ids_i] (D wide,
+    ids of any width index_bytes_of accepts), z_t = [u * i | h] . w[:, t] + bias[t] with h (M, U) and w (D + U, H).
+    losses, targets, out, loss, dw, db, loss_weights and sample_weight as heads_fwd_bwd.  Training writes du, di (M, D)
+    contiguous (the two tables' IndexedSlices values, with 2 l2 u / 2 l2 i added) and dh (M, U) (relu-masked from h when
+    relu_h).  reg (1 value, nullable) accumulates l2 (sum |u|^2 + |i|^2 + |x_reg|^2); training adds it to loss[0] too."""
+    for n, t in (("table_u", table_u), ("table_i", table_i)):
+        if _dev(t, n, torch.float32).dim() != 2 or not t.is_contiguous():
+            raise ValueError(f"{n} must be a contiguous (rows, D) matrix")
+    D = table_u.shape[1]
+    if table_i.shape[1] != D:
+        raise ValueError(f"table_u and table_i must have the same width, got {D} and {table_i.shape[1]}")
+    _dev(h, "h", torch.float32), _dev(w, "w", torch.float32), _dev(out, "out", torch.float32)
+    if h.dim() != 2:
+        raise ValueError(f"h must be (M, U), got {tuple(h.shape)}")
+    M, U = h.shape
+    H = len(losses)
+    if not (1 <= D <= NCF_MAX_WIDTH and 1 <= U <= NCF_MAX_UNITS and 1 <= H <= NCF_MAX_HEADS):
+        raise ValueError(f"D = {D}, U = {U} and H = {H} must be in 1..{NCF_MAX_WIDTH}, 1..{NCF_MAX_UNITS} and 1..{NCF_MAX_HEADS}")
+    wu = _id_column(ids_u, M, "ids_u")
+    wi = _id_column(ids_i, M, "ids_i")
+    if tuple(w.shape) != (D + U, H) or not w.is_contiguous():
+        raise ValueError(f"w must be a contiguous ({D + U}, {H}) matrix")
+    _vec(bias, H, "bias")
+    if tuple(out.shape) != (H, M) or not out.is_contiguous():
+        raise ValueError(f"out must be a contiguous ({H}, {M}) matrix")
+    if any(l not in _cabi.LOSS_KINDS for l in losses):
+        raise ValueError(f"losses must be among {sorted(_cabi.LOSS_KINDS)}, got {list(losses)}")
+    if not (0.0 <= float(l2) < float("inf")):
+        raise ValueError(f"l2 must be finite and >= 0, got {l2}")
+    _vec(reg, 1, "reg")
+    if x_reg is not None:
+        if reg is None:
+            raise ValueError("x_reg needs reg")
+        if _dev(x_reg, "x_reg", torch.float32).dim() != 2 or x_reg.shape[0] != M or x_reg.shape[1] < 1:
+            raise ValueError(f"x_reg must be ({M}, n) with n >= 1, got {tuple(x_reg.shape)}")
+    if oob is not None and (_dev(oob, "oob", torch.int32).numel() < 1 or not oob.is_contiguous()):
+        raise ValueError("oob must be an int32 counter")
+    kinds = (C.c_int * H)(*[_cabi.LOSS_KINDS[l] for l in losses])
+    tp = dt = sp = lw = None
+    train = targets is not None
+    dhs = 0
+    if train:
+        if len(targets) != H:
+            raise ValueError(f"one target tensor per head: {H} expected, got {len(targets)}")
+        dt = (C.c_int * H)(*[_target(t, M, f"targets[{h_}]") for h_, t in enumerate(targets)])
+        if loss is None or du is None or di is None or dh is None or dw is None:
+            raise ValueError("training needs loss, du, di, dh and dw")
+        _vec(loss, 1 + H, "loss")
+        for n, g in (("du", du), ("di", di)):
+            if tuple(_dev(g, n, torch.float32).shape) != (M, D) or not g.is_contiguous():
+                raise ValueError(f"{n} must be a contiguous ({M}, {D}) matrix")
+        if tuple(_dev(dh, "dh", torch.float32).shape) != (M, U):
+            raise ValueError(f"dh must be ({M}, {U})")
+        dhs = _row_stride(dh, "dh")
+        if tuple(_dev(dw, "dw", torch.float32).shape) != (D + U, H) or not dw.is_contiguous():
+            raise ValueError(f"dw must be a contiguous ({D + U}, {H}) matrix")
+        _vec(db, H, "db")
+        sws = list(sample_weight) if isinstance(sample_weight, (list, tuple)) else [sample_weight] * H
+        if len(sws) != H:
+            raise ValueError(f"one sample-weight tensor per head: {H} expected, got {len(sws)}")
+        for h_, s_ in enumerate(sws):
+            _vec(s_, M, f"sample_weight[{h_}]", _SAMPLE_WEIGHT)
+        lws = [1.0] * H if loss_weights is None else [float(v) for v in loss_weights]
+        if len(lws) != H:
+            raise ValueError(f"one loss weight per head: {H} expected, got {len(lws)}")
+        tp = (C.c_void_p * H)(*[t.data_ptr() for t in targets])
+        sp = (C.c_void_p * H)(*[_ptr(s_) for s_ in sws])
+        lw = (C.c_float * H)(*lws)
+    _cabi.check(_lib().mm_ncf_head_fwd_bwd(
+        table_u.data_ptr(), table_u.shape[0], ids_u.data_ptr(), wu, table_i.data_ptr(), table_i.shape[0], ids_i.data_ptr(), wi, D,
+        h.data_ptr(), _row_stride(h, "h"), U, 1 if relu_h else 0, M, H, w.data_ptr(), _ptr(bias), kinds, lw, tp, dt, sp, float(l2),
+        _ptr(x_reg), 0 if x_reg is None else _row_stride(x_reg, "x_reg"), 0 if x_reg is None else x_reg.shape[1], out.data_ptr(),
+        _ptr(loss) if train else None, _ptr(reg), _ptr(du) if train else None, _ptr(di) if train else None,
+        _ptr(dh) if train else None, dhs, _ptr(dw) if train else None, _ptr(db) if train else None, _ptr(oob), _stream()),
+        "mm_ncf_head_fwd_bwd")
+    return out
+
+
 def _wgrad_n(M: int, K: int, dz: torch.Tensor, dw: torch.Tensor, db: Optional[torch.Tensor]) -> int:
     """N of the gradients of a Dense layer with M rows of K inputs: dz (M, N), dw a contiguous (K, N) matrix, db (N,) or None."""
     _dev(dz, "dz", torch.float32), _dev(dw, "dw", torch.float32)

@@ -2,7 +2,7 @@
 CUDA (include/mm_b200.h K14), behind the reference's `compile` / `fit` / `train_step`
 (merlin/models/tf/models/base.py:1121-1231; optimizers: tf.keras.optimizers.{SGD, Adagrad, Adam}, LazyAdam
 blocks/optimizer.py:342).  One trainer per model (DLRMTrainer, DCNTrainer, TwoTowerTrainer, DeepFMTrainer,
-WideAndDeepTrainer, MMoETrainer; trainer_for picks) holds what is particular to it; the parts they share are methods of
+WideAndDeepTrainer, MMoETrainer, NCFTrainer; trainer_for picks) holds what is particular to it; the parts they share are methods of
 _StepTrainer (the construction checks, the dense arena, the table checks and optimizer state, a chain of Dense layers forward
 and backward, multi-hot pooling, the output heads, the step's prologue, the update (apply_gradients), snapshot / restore,
 capture / replay) and two parts a trainer owns: the concatenating input block (_ConcatInput) and a wide kernel trained
@@ -37,6 +37,8 @@ into the input block's backward (mm_concat_backward_l2).
 DeepFMModel trains through DeepFMTrainer: DCN's input block and deep tower, the FM / wide / output head forward and
 backward in one kernel (mm_deepfm_head_fwd_bwd), the FM term's input gradient (mm_fm_concat_backward) and the wide
 kernel's sparse update (mm_wide_rows_apply).
+NCFModel trains through NCFTrainer: the mlp branch's rows and tower as DCN's input block and deep tower, and the GMF branch,
+the output heads and their loss forward and backward in one kernel that gathers the GMF rows itself (mm_ncf_head_fwd_bwd).
 
 All Dense variables of the model are re-homed into ONE flat fp32 arena (gradients and optimizer slots mirror its layout), so
 the dense update is one launch and data-parallel training needs one all-reduce.  Every buffer is static: a step can be
@@ -634,13 +636,17 @@ class _ConcatInput:
     """A trainer's concatenating input block (InputBlockV2): x0 (B, d) = [embedding rows | continuous columns] at their
     sorted-name offsets `cols`, its split operand xs and, for a caller that needs the input gradient, dx0 (None without
     tables).  feats: the features it gathers, by default every feature of the block's embeddings, at the trainer's table
-    positions tidx (set by _init_inputs); cont: its continuous columns, by default in sorted-name order."""
+    positions tidx (set by _init_inputs); cont: its continuous columns, by default in sorted-name order; cols: the
+    features' column offsets, by default the block's sorted-name layout."""
 
     def __init__(self, tr: _StepTrainer, ib, dx0: bool = False, feats: Optional[Sequence[str]] = None,
-                 cont: Optional[Sequence[str]] = None):
+                 cont: Optional[Sequence[str]] = None, cols: Optional[Dict[str, int]] = None):
         self.tr = tr
         self.emb = ib.embeddings
         self.cols, _, self.d = ib.layout()
+        if cols is not None:  # an explicit column offset per feature instead of the sorted-name concat (NCF's [item | query])
+            dims = self.emb.output_dims()
+            self.cols, self.d = dict(cols), max(c + dims[f] for f, c in cols.items())
         if feats is None:
             feats = self.emb.feature_names if self.emb is not None else []
         if cont is None:
@@ -1736,16 +1742,105 @@ class MMoETrainer(_StepTrainer):
         self._b = b
 
 
+class NCFTrainer(_StepTrainer):
+    """Static-buffer training step of an NCFModel (RankingModel over NCFBody; 1..8 BinaryOutput / RegressionOutput heads)
+    at one batch size.
+
+    forward   the mlp branch's rows [i_mlp | u_mlp] into x0 (mm_gather_multi) and its split operand; mm_dense_tc per
+              mlp_block layer (fp32 activation saved + the next layer's operand)
+    head      mm_ncf_head_fwd_bwd: the GMF rows gathered by id, u * i next to the tower's output h, the heads, their losses
+              and the backward in one pass: the GMF tables' IndexedSlices values (du, di, with 2 l2 e), dh (relu-masked),
+              the heads' dW / db in the arena, and the GMF part of the L2 term
+    backward  mm_dense_wgrad[_split] + mm_dense_dgrad per layer down to dx0; mm_concat_backward (mm_concat_backward_l2 with
+              embeddings_l2_reg > 0) into the mlp tables' IndexedSlices values
+    update    mm_opt_tick, mm_dense_apply over the arena, mm_sparse_rows_apply per embedding width (all four tables),
+              mm_split_weights refresh of the operand copies the model's forward reads.
+
+    The loss vector is [regularization, total, loss_0 ..]: `loss` is its tail, the vector of the other ranking steps, and
+    mm_concat_backward_l2 adds the mlp tables' term to its first two entries.  Fixed-shape ids capture into one CUDA graph."""
+
+    _model_name = "an NCFModel"
+    _onehot_only = True
+
+    def __init__(self, model, optimizer: Optimizer, batch_size: int, device=None, group=None):
+        from .models import NCFBody
+
+        body = model.body
+        if not isinstance(body, NCFBody):
+            raise NotImplementedError("NCFTrainer trains NCFModel bodies")
+        self._refuse_group(group)
+        self._require_tc_engine()
+        self._refuse_sharded(body)
+        for emb in model.embedding_blocks():
+            self._refuse_sharded(emb)
+        self._check_mlps([body.mlp])
+        self.layers = body.mlp.dense_layers
+        self._check_activations(self.layers)
+        self._init_common(model, optimizer, batch_size, device, None)
+        self._init_heads()
+        self.inp = _ConcatInput(self, body.mlp_input_block, dx0=True, cols=body.mlp_columns)
+        # table positions: the mlp branch's (the input block's order), then the GMF user and item tables
+        gmf = [(body.feature("mf", s), body.table("mf", s)) for s in ("query", "item")]
+        self.inp.tidx = list(range(len(self.inp.feats)))
+        self._init_tables(self.inp.feats + [f for f, _ in gmf], [self.inp.emb.feature_to_table[f] for f in self.inp.feats]
+                          + [t for _, t in gmf])
+        self.slices = [torch.zeros((self.B, t.table.shape[1]), dtype=torch.float32, device=self.device) for t in self.tables]
+        self.t_u, self.t_i = len(self.inp.feats), len(self.inp.feats) + 1
+        self.l2 = body.embeddings_l2_reg
+        self.inp.set_l2_reg(self.l2)
+        self._init_dense(self.layers, [self.head])
+        self._init_wide(lambda li: True)
+        self.h, self.h_split, self.dh = self._chain_buffers(self.layers)
+        self._init_loss(self.B)
+        self._loss_all = torch.zeros(2 + self.H, dtype=torch.float32, device=self.device)  # [regularization, total, loss_0 ..]
+        self.loss = self._loss_all[1:] if self.H > 1 else self._loss_all[1:2]
+        self.regularization = self._loss_all[0]
+        self.oob = self.inp.oob
+
+    def table_gradients(self) -> Dict[str, tuple]:
+        """{"mf/query" | "mf/item" | "mlp/query" | "mlp/item": (ids, rows)} of the last forward_backward: each table's
+        IndexedSlices before duplicates are summed."""
+        body = self.body
+        out = {f"mf/{s}": (self._idx[t], self._slices[t]) for s, t in (("query", self.t_u), ("item", self.t_i))}
+        for s in ("query", "item"):
+            t = self.inp.tidx[self.inp.feats.index(body.feature("mlp", s))]
+            out[f"mlp/{s}"] = (self._idx[t], self._slices[t])
+        return out
+
+    def forward_backward(self, inputs: Dict[str, torch.Tensor], targets, sample_weight=None) -> None:
+        """Forward (activations saved), loss and backward: fills the gradient arena and the four tables' IndexedSlices.
+        Batches smaller than the compiled size run in the leading rows of the same buffers."""
+        a, body = self.arena, self.body
+        b, targets, sample_weight = self._begin_step(inputs, targets, sample_weight)
+        hi = len(a.layers) - 1
+        _, xs, dx0 = self.inp.forward(inputs, b)
+        h, h_split, dh = ([x[:b] for x in bufs] for bufs in (self.h, self.h_split, self.dh))
+        self._chain_forward(xs, self.inp.d, 0, self.layers, h, h_split)
+        ids_u, ids_i = body.ids(inputs, "query"), body.ids(inputs, "item")
+        self._idx[self.t_u], self._idx[self.t_i] = ids_u, ids_i
+        ops.ncf_head_fwd_bwd(self.tables[self.t_u].table, ids_u, self.tables[self.t_i].table, ids_i, h[-1], self.head.kernel,
+                             self.head.bias, self.losses, [t.reshape(-1) for t in targets],
+                             self.logits.view(-1)[:self.H * b].view(self.H, b), loss=self._loss_all[1:],
+                             reg=self._loss_all[:1] if self.l2 else None, l2=self.l2, du=self._slices[self.t_u],
+                             di=self._slices[self.t_i], dh=dh[-1], dw=a.view(a.grad, hi, "kernel"), db=a.view(a.grad, hi, "bias"),
+                             loss_weights=self.loss_weights, relu_h=self.layers[-1].activation == "relu",
+                             sample_weight=sample_weight, oob=self.oob)
+        self._chain_backward(0, self.layers, h, dh, (xs, self.inp.d), dx0)
+        self.inp.backward([dx0], b)
+        self._b = b
+
+
 def trainer_for(model, optimizer: Optimizer, batch_size: int, group=None):
-    """The training engine of `model`: DLRMTrainer, DCNTrainer, DeepFMTrainer, WideAndDeepTrainer or MMoETrainer by the
-    ranking body, TwoTowerTrainer for a RetrievalModel."""
-    from .models import DCNBody, DeepFMBody, MMoEBody, RetrievalModel, RetrievalModelV2, WideAndDeepBody
+    """The training engine of `model`: DLRMTrainer, DCNTrainer, DeepFMTrainer, WideAndDeepTrainer, MMoETrainer or
+    NCFTrainer by the ranking body, TwoTowerTrainer for a RetrievalModel."""
+    from .models import DCNBody, DeepFMBody, MMoEBody, NCFBody, RetrievalModel, RetrievalModelV2, WideAndDeepBody
 
     if isinstance(model, RetrievalModelV2):
         raise NotImplementedError("training TwoTowerModelV2 / ContrastiveOutput is not implemented: train the v1 TwoTowerModel")
     if isinstance(model, RetrievalModel):
         return TwoTowerTrainer(model, optimizer, batch_size, group=group)
-    by_body = {DCNBody: DCNTrainer, DeepFMBody: DeepFMTrainer, WideAndDeepBody: WideAndDeepTrainer, MMoEBody: MMoETrainer}
+    by_body = {DCNBody: DCNTrainer, DeepFMBody: DeepFMTrainer, WideAndDeepBody: WideAndDeepTrainer, MMoEBody: MMoETrainer,
+               NCFBody: NCFTrainer}
     body = getattr(model, "body", None)
     cls = next((c for t, c in by_body.items() if isinstance(body, t)), DLRMTrainer)
     return cls(model, optimizer, batch_size, group=group)
