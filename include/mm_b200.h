@@ -234,8 +234,8 @@ int mm_dense_fp32(const float* x, int64_t B, int K, int64_t x_stride, const floa
  *   a_split : (M, 2*Kp) bf16, row = [hi(0..Kp) | lo(0..Kp)], Kp = K padded to 64
  *   w_split : (Np, 2*Kp) bf16, K-major transpose of the Keras kernel, same split, Np = N
  *             padded to 16 — produced once by mm_split_weights
- *   out_f32 : (M, N) fp32 (nullable);  out_split : (M, 2*Np_next) bf16 for the next layer
- *             (nullable; its padding columns are written as zeros)
+ *   out_f32 : (M, N) fp32 (nullable);  out_split : (M, 2*Kp(N)) bf16 for the next layer
+ *             (nullable; its padding columns N..Kp(N) of hi and lo are written as zeros)
  *   x0/xres : fp32 (M, N) operands of the cross epilogue (nullable, both or none)
  * ------------------------------------------------------------------------------------- */
 /* padded operand sizes used by the tensor-core path: Kp = ceil64(K); Np = ceil16(N) (N<=128) or ceil128(N) */

@@ -211,7 +211,7 @@ class _Dense(Block):
 
     def split_buffer(self, B: int, device) -> torch.Tensor:
         """Cached (B, 2*Kp(units)) bf16 buffer receiving this layer's output as the next layer's
-        operand; its padding columns are zeroed once and never written again."""
+        operand; mm_dense_tc writes every column of it, the padding ones as zeros."""
         key = (B, buffer_namespace())
         buf = self._split_bufs.get(key)
         if buf is None or buf.device != device:

@@ -470,6 +470,19 @@ dense_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
           }
         }
       }
+      if (p.out_split && p.Np < p.out_Kp) {
+        // N <= 128 and ceil16(N) < ceil64(N): the single n-tile ends at Np, but the next layer's k-block runs to
+        // out_Kp, so columns [Np, out_Kp) of hi and lo are written as zeros here (the two warps of the quarter share it)
+        const int gap = (p.out_Kp - p.Np) >> 3;  // 16-byte groups per half row
+        for (int e = half * 32 + lane; e < 32 * gap; e += 64) {
+          const long long grow = row0 + e / gap;
+          if (grow < p.M) {
+            __nv_bfloat16* oh = p.out_split + grow * (2ll * p.out_Kp) + p.Np + 8 * (e % gap);
+            *reinterpret_cast<uint4*>(oh) = make_uint4(0u, 0u, 0u, 0u);
+            *reinterpret_cast<uint4*>(oh + p.out_Kp) = make_uint4(0u, 0u, 0u, 0u);
+          }
+        }
+      }
     }
   }
 }

@@ -55,9 +55,30 @@ def _split_padding_zero(buf, rows, W, what):
         assert bool((pad.float() == 0).all()), f"{what}: a padding column of the split output is not zero"
 
 
-def _chain(h, layers, e=None):
+# activation: (float64 function, Lipschitz constant L, own rounding in units of E as (a, g): a |y| + g |z|); the
+# constants of tanh, selu, elu and gelu are derived in tests/test_gpu_dense_tc_kernels.py
+ACT_REF = {
+    None: (lambda z: z, 1.0, 0, 0), "linear": (lambda z: z, 1.0, 0, 0), "relu": (lambda z: z.clamp_min(0.0), 1.0, 0, 0),
+    "sigmoid": (torch.sigmoid, 0.25, 8, 0), "tanh": (torch.tanh, 1.0, 4, 0), "selu": (torch.nn.functional.selu, 1.76, 8, 0),
+    "elu": (torch.nn.functional.elu, 1.0, 2, 0), "gelu": (torch.nn.functional.gelu, 1.13, 1, 4),
+}
+
+
+def _act(z, ez, act):
+    """float64 act(z) and the bound of the device's act at a pre-activation within ez of z: L ez for the error carried
+    in, plus the activation's own rounding at that pre-activation, E (a (|y| + L ez) + g (|z| + ez))."""
+    f, L, a, g = ACT_REF[act]
+    y = f(z)
+    e = L * ez
+    if a or g:
+        e = e + E * (a * (y.abs() + e) + g * (z.abs() + ez))
+    return y, e
+
+
+def _chain(h, layers, e=None, unit=U):
     """float64 forward of Dense layers (W (K, N) fp32, b (N,) or None, activation) from h, which is within e of the
-    device's input, and the element-wise bound of the module docstring.  Returns (output, bound)."""
+    device's input, and the element-wise bound of the module docstring.  `unit`: the relative error of one product
+    (U for 3-pass split-bf16, 0 for fp32 CUDA-core dots).  Returns (output, bound)."""
     e = torch.zeros_like(h) if e is None else e
     for W, b, act in layers:
         Wd = W.double()
@@ -67,16 +88,8 @@ def _chain(h, layers, e=None):
         if b is not None:
             z = z + b.double()
             ba = b.double().abs()
-        ez = e @ Wa + (U + W.shape[0] * E) * ((h.abs() + e) @ Wa + ba)
-        if act == "relu":
-            h, e = z.clamp_min(0.0), ez
-        elif act == "sigmoid":
-            h = torch.sigmoid(z)
-            e = ez / 4 + 8 * E * h
-        elif act in (None, "linear"):
-            h, e = z, ez
-        else:
-            raise ValueError(act)
+        ez = e @ Wa + (unit + W.shape[0] * E) * ((h.abs() + e) @ Wa + ba)
+        h, e = _act(z, ez, act)
     return h, e
 
 
