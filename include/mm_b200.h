@@ -210,6 +210,11 @@ typedef struct {
  * copy of the tables in HBM (bottom: mm_mlp_tc_operand_out writes it directly). */
 #define MM_ROWS_F32 0
 #define MM_ROWS_OPERAND 1
+/* MM_ROWS_OPERAND_PAIRS: as MM_ROWS_OPERAND (a bottom vector is required), but the output row carries the pairs only:
+ * out_split (B, 2*out_Kp) = [hi(pairs) | lo(pairs)] with out_Kp a multiple of 8 >= F(F-1)/2 (Criteo: 352, 1 408-B rows);
+ * columns past the pairs are zeros.  The bottom vector is not copied out: mm_mlp_tc_pairs reads it from the bottom
+ * tower's own operand rows. */
+#define MM_ROWS_OPERAND_PAIRS 2
 int mm_dlrm_lookup_interact(const mm_lookup_table* tables_host, int n_tables, int64_t B, int D, int rank, int world,
                             const float* bottom, int64_t bottom_stride, int bottom_slot, float* out,
                             int64_t out_stride, void* out_split, int out_Kp, int32_t* oob_count, int row_format,
@@ -286,6 +291,17 @@ int mm_mlp_tc(const void* a_split, int64_t M, int K, int n_layers, const void* c
 int mm_mlp_tc_heads(const void* a_split, int64_t M, int K, int n_layers, const void* const* w_split, const int* widths,
                     const float* const* bias, const int* acts, int n_heads, const float* heads_w, const float* heads_b,
                     const int* heads_act, float* heads_out, void* stream);
+
+/* mm_mlp_tc (n_heads = 0) or mm_mlp_tc_heads (n_heads >= 1: head_w / head_out are heads_w / heads_out, out must be NULL)
+ * over a layer-1 input held in two buffers, the hand-off of mm_dlrm_lookup_interact(row_format = MM_ROWS_OPERAND_PAIRS):
+ *   bottom_split (M, 2*64) bf16 [hi | lo] = input columns 0..63 (the bottom tower's operand rows);
+ *   pairs_split  (M, 2*Kq) bf16 [hi(Kq) | lo(Kq)] = input columns 64..K-1, Kq = K - 64 rounded up to 8.
+ * Same k-blocks, MMAs and order as mm_mlp_tc over the concatenated row: results are bit-identical.  Columns of pairs_split
+ * past K - 64 are never read.  K > 64. */
+int mm_mlp_tc_pairs(const void* bottom_split, const void* pairs_split, int64_t M, int K, int n_layers, const void* const* w_split,
+                    const int* widths, const float* const* bias, const int* acts, float* out, int64_t out_stride,
+                    const float* head_w, float head_b, int head_act, float* head_out, int n_heads, const float* heads_b,
+                    const int* heads_act, void* stream);
 
 /* mm_mlp_tc whose last layer also (or only: out may be NULL) leaves its rows as split-bf16 rows
  * out_operand (M, 2 * widths[n-1]) bf16 = [hi | lo] per row (widths[n-1] % 4 == 0; the mm_split_rows layout when the

@@ -178,6 +178,8 @@ SIGNATURES = {
                        _vp, _i64, _vp, _f, _i, _vp, _vp]),
     "mm_mlp_tc_heads": (_i, [_vp, _i64, _i, _i, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_void_p), C.POINTER(C.c_int),
                              _i, _vp, _vp, C.POINTER(C.c_int), _vp, _vp]),
+    "mm_mlp_tc_pairs": (_i, [_vp, _vp, _i64, _i, _i, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_void_p),
+                             C.POINTER(C.c_int), _vp, _i64, _vp, _f, _i, _vp, _i, _vp, C.POINTER(C.c_int), _vp]),
     "mm_mlp_tc_operand_out": (_i, [_vp, _i64, _i, _i, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_void_p),
                                    C.POINTER(C.c_int), _vp, _i64, _vp, _vp]),
     "mm_tower2_small_supported": (_i, [_i, _i, _i]),

@@ -67,8 +67,28 @@ def table_mirror() -> bool:
     return os.environ.get("MM_TABLE_MIRROR", "1") != "0"
 
 
+def _fuses_head(layers) -> bool:
+    """A trailing Dense(N -> 1) (BinaryOutput) after a layer with N <= 32 units is evaluated inside that layer's GEMM
+    epilogue: one launch and one HBM round trip fewer."""
+    return (len(layers) >= 2 and layers[-1].units == 1 and layers[-2].units <= 32
+            and layers[-1].input_dim == layers[-2].units)
+
+
+def tower_kernel_applies(layers: "List[_Dense]", K: int, heads=None) -> bool:
+    """True when run_dense_chain runs `layers` (built, on K input columns) as ONE whole-tower launch (mm_mlp_tc /
+    mm_mlp_tc_heads): the condition for handing it its input as bottom rows + pairs rows (run_dense_chain(a_bottom=...))."""
+    if not _use_tc():
+        return False
+    widths = [l.units for l in layers]
+    if heads is not None:
+        return widths[-1] <= 32 and ops.mlp_tc_supported(K, widths, heads=True)
+    fuse = _fuses_head(layers)
+    return ops.mlp_tc_supported(K, widths[:-1] if fuse else widths, head=fuse)
+
+
 def run_dense_chain(x: Optional[torch.Tensor], layers: "List[_Dense]", a_split: Optional[torch.Tensor] = None,
-                    K: Optional[int] = None, operand_out: bool = False, heads=None, logits: bool = False) -> torch.Tensor:
+                    K: Optional[int] = None, operand_out: bool = False, heads=None, logits: bool = False,
+                    a_bottom: Optional[torch.Tensor] = None) -> torch.Tensor:
     """A chain of Dense layers on one input matrix.  operand_out=True: the result rows come back as bf16 split rows
     (B, 2*Kp) = [hi | lo] (the interaction kernel's operand format) — directly from the whole-tower kernel's last
     epilogue when it applies, by one mm_split_rows pass over the fp32 result otherwise.
@@ -84,7 +104,12 @@ def run_dense_chain(x: Optional[torch.Tensor], layers: "List[_Dense]", a_split: 
 
     logits=True: the output (the heads, or else the chain's last layer) skips its activation, through the same kernels with
     the activation argument linear: the result is the logits the activation would have read.  _LAST_HEADS records which
-    kernel computed the heads."""
+    kernel computed the heads.
+
+    a_bottom (B, 128): the input is split in two, columns 0..63 in these bottom rows and the rest in the pairs rows
+    a_split (ops.dlrm_lookup_interact(pairs_only=True)); only the whole-tower kernel reads it (tower_kernel_applies)."""
+    if a_bottom is not None and not tower_kernel_applies(layers, K, heads):
+        raise ValueError("a bottom + pairs input needs the whole-tower kernel (tower_kernel_applies)")
     if heads is not None:
         hl = heads.to_call
         dev = (x if x is not None else a_split).device
@@ -99,7 +124,8 @@ def run_dense_chain(x: Optional[torch.Tensor], layers: "List[_Dense]", a_split: 
             a = a_split if a_split is not None else ops.split_rows(x)
             return ops.mlp_tc_heads(a, K if a_split is not None else x.shape[1], [l.split_kernel() for l in layers],
                                     [l.units for l in layers], [l.bias for l in layers], [l.activation for l in layers],
-                                    hl.kernel, hl.bias, ["linear"] * len(heads.outputs) if logits else heads.activations, out)
+                                    hl.kernel, hl.bias, ["linear"] * len(heads.outputs) if logits else heads.activations, out,
+                                    a_bottom=a_bottom)
         if a_split is not None and not _use_tc():
             raise ValueError("the fp32 dense engine needs an fp32 input")
         h = run_dense_chain(x, layers, a_split=a_split, K=K)
@@ -125,10 +151,7 @@ def run_dense_chain(x: Optional[torch.Tensor], layers: "List[_Dense]", a_split: 
     if a_split is None:
         a = ops.split_rows(x)
     out = None
-    # a trailing Dense(N -> 1) (BinaryOutput) after a layer with N <= 32 units is evaluated inside that
-    # layer's GEMM epilogue: one launch and one HBM round trip fewer
-    fuse_head = (len(layers) >= 2 and layers[-1].units == 1 and layers[-2].units <= 32
-                 and layers[-1].input_dim == layers[-2].units)
+    fuse_head = _fuses_head(layers)
     if fuse_head:
         (head, layers), (head_act, acts) = (layers[-1], layers[:-1]), (acts[-1], acts[:-1])
     if K != layers[0].input_dim:
@@ -148,7 +171,7 @@ def run_dense_chain(x: Optional[torch.Tensor], layers: "List[_Dense]", a_split: 
         else:
             out = torch.empty((B, widths[-1]), dtype=torch.float32, device=device)
             kw = dict(out=out)
-        ops.mlp_tc(a, K, [l.split_kernel() for l in layers], widths, [l.bias for l in layers], acts, **kw)
+        ops.mlp_tc(a, K, [l.split_kernel() for l in layers], widths, [l.bias for l in layers], acts, a_bottom=a_bottom, **kw)
         return ops.split_rows(out) if operand_out else out
     _LAST_PATH[0] = "dense_tc"
     for i, (l, act) in enumerate(zip(layers, acts)):
@@ -938,10 +961,12 @@ class DLRM(Block):
         return ok
 
     def interaction_forward(self, inputs: TabularData, bottom: Optional[torch.Tensor], as_split: bool = False,
-                            operand_rows: bool = False) -> torch.Tensor:
+                            operand_rows: bool = False, pairs_only: bool = False) -> torch.Tensor:
         """[bottom |] interactions, (B, P + F(F-1)/2) fp32 — or, with as_split, the split-bf16 operand
         (B, 2*Kp) of the top MLP's first tensor-core layer, written directly by the kernel.  operand_rows: `bottom` is in
-        operand format and the tables' operand-format mirrors are used (see use_operand_rows)."""
+        operand format and the tables' operand-format mirrors are used (see use_operand_rows).  pairs_only (with
+        operand_rows, replicated one-hot tables only): the pairs alone, (B, 2*pairs_cols(F(F-1)/2)); the top tower reads the
+        bottom vector from `bottom` itself."""
         self.build(next(iter(inputs.values())).device)
         D = self.embedding_dim
         slots = self.slots()
@@ -951,7 +976,9 @@ class DLRM(Block):
         with_prefix = bottom is not None and self.top_block is not None
         P = D if with_prefix else 0
         width = P + F * (F - 1) // 2
-        if as_split:
+        if pairs_only:
+            out = torch.empty((B, 2 * ops.pairs_cols(width - P)), dtype=torch.bfloat16, device=dev)
+        elif as_split:
             out = torch.empty((B, 2 * ops.tc_padded_k(width)), dtype=torch.bfloat16, device=dev)
         else:
             out = torch.empty((B, width), dtype=torch.float32, device=dev)
@@ -961,6 +988,8 @@ class DLRM(Block):
 
         all_onehot = self.sharded is None and all(emb.feature_to_table[f].lookup_kind(get_feature(inputs, f)) == "onehot"
                                                   for f in feats)
+        if pairs_only and not (operand_rows and with_prefix and self.sharded is None and self.fused and all_onehot):
+            raise ValueError("pairs_only needs operand-format rows, a bottom vector and replicated one-hot tables")
         if self.can_emit_split() and with_prefix == (bottom is not None) and (self.sharded is not None or (self.fused and all_onehot)):
             oob = emb.counter(dev)
             if self.sharded is not None:
@@ -972,7 +1001,8 @@ class DLRM(Block):
                 idx = [ops.fused_ids(get_feature(inputs, f)) for f in feats]
                 tabs = [emb.feature_to_table[f].operand_mirror() if operand_rows else emb.feature_to_table[f].table for f in feats]
                 ops.dlrm_lookup_interact(tabs, idx, [slots[f] for f in feats], [t.shape[0] for t in tabs], D, bottom,
-                                         slots.get("bottom_block", -1), out, oob, operand_rows=operand_rows)
+                                         slots.get("bottom_block", -1), out, oob, operand_rows=operand_rows,
+                                         pairs_only=pairs_only)
             emb.finish_check(oob)
             return out
         # staged path: the (B,F,D) stack in HBM, then the interaction kernel

@@ -189,7 +189,10 @@ int mm_dlrm_lookup_interact(const mm_lookup_table* tables_host, int n_tables, in
                             int64_t out_stride, void* out_split, int out_Kp, int32_t* oob_count, int row_format,
                             void* stream) {
   const char* who = "mm_dlrm_lookup_interact";
-  MM_REQUIRE(row_format == MM_ROWS_F32 || row_format == MM_ROWS_OPERAND, MM_ERR_ARG, "%s: bad row_format", who);
+  MM_REQUIRE(row_format == MM_ROWS_F32 || row_format == MM_ROWS_OPERAND || row_format == MM_ROWS_OPERAND_PAIRS, MM_ERR_ARG,
+             "%s: bad row_format", who);
+  const bool pairs_only = row_format == MM_ROWS_OPERAND_PAIRS;
+  MM_REQUIRE(!pairs_only || bottom, MM_ERR_ARG, "%s: MM_ROWS_OPERAND_PAIRS needs the bottom vector", who);
   MM_REQUIRE(row_format == MM_ROWS_F32 || (out_split && !out), MM_ERR_ARG,
              "%s: operand-format rows need the split-bf16 output (the fp32 prefix cannot be rebuilt exactly)", who);
   MM_REQUIRE(tables_host && n_tables > 0 && (out || out_split) && B >= 0, MM_ERR_ARG, "%s: bad table list / null out / B<0", who);
@@ -209,14 +212,14 @@ int mm_dlrm_lookup_interact(const mm_lookup_table* tables_host, int n_tables, in
   for (int b = 0; b < 4; ++b)
     if ((1 << b) == world) lk.log2_world = b;
   if (const int rc = mm::fill_lookup_params(who, tables_host, n_tables, F, bottom ? bottom_slot : -1, rank, true, lk)) return rc;
-  const int P = bottom ? D : 0;
+  const int P = bottom && !pairs_only ? D : 0;  // pairs only: the bottom row is staged but not written out
   MM_REQUIRE(!out || out_stride >= P + F * (F - 1) / 2, MM_ERR_ARG, "%s: out_stride too small", who);
-  MM_REQUIRE(!out_split || (out_Kp % 64 == 0 && out_Kp >= P + F * (F - 1) / 2 && ((uintptr_t)out_split % 16) == 0), MM_ERR_ARG,
-             "%s: out_Kp must be a multiple of 64 >= the row width, out_split 16-B aligned", who);
+  MM_REQUIRE(!out_split || (out_Kp % (pairs_only ? 8 : 64) == 0 && out_Kp >= P + F * (F - 1) / 2 && ((uintptr_t)out_split % 16) == 0),
+             MM_ERR_ARG, "%s: out_Kp must be a multiple of %d >= the row width, out_split 16-B aligned", who, pairs_only ? 8 : 64);
   if (B == 0) return MM_OK;
   const int rc = mm::imma2::launch<1>(nullptr, 0, lk, bottom, bottom_stride, P, bottom ? bottom_slot : -1, B, F, D, out,
                                       out_stride, out_split, out_Kp, oob_count, (cudaStream_t)stream, who,
-                                      row_format == MM_ROWS_OPERAND);
+                                      row_format != MM_ROWS_F32);
   MM_REQUIRE(rc != MM_ERR_UNSUPPORTED, MM_ERR_UNSUPPORTED, "%s: shape outside the fused kernel (F=%d, D=%d)", who, F, D);
   return rc;
 }

@@ -54,6 +54,7 @@ struct ChainLayer {
 struct Params {
   long long M;
   int K1p, N1, N1p, act1, stages, n_chain;
+  int pairs;  // layer-1 A in two parts: k-block 0 from tmA (bottom rows), k-blocks 1.. from tmPhi / tmPlo (pairs rows)
   ChainLayer c[kMaxChain];
   const float* bias[kMaxChain + 1];  // layer 1, chain layers
   uint32_t w_bytes;                  // total resident weight bytes
@@ -123,7 +124,8 @@ template <int N1P, bool HEADS>
 __global__ void __launch_bounds__(kThreads, 1)
 mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmW1,
               const __grid_constant__ CUtensorMap tmC0, const __grid_constant__ CUtensorMap tmC1,
-              const __grid_constant__ CUtensorMap tmC2, const Params p) {
+              const __grid_constant__ CUtensorMap tmC2, const __grid_constant__ CUtensorMap tmPhi,
+              const __grid_constant__ CUtensorMap tmPlo, const Params p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);  // keeps the shared state space
   // layer-1 ring: each slot holds ONE half of a k-block of one tile, {A_hi, W1_hi} or {A_lo, W1_lo} (24 KB at
@@ -145,6 +147,10 @@ mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
   if (warp == kConsumerWarps && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmW1) : "memory");
+    if (p.pairs) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&tmPhi) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&tmPlo) : "memory");
+    }
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(smem_u32(full_bar + s), 1);
       mbar_init(smem_u32(empty_bar + s), kConsumerWarps / 2);
@@ -195,11 +201,20 @@ mlp_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ C
         const int m0 = (int)tile * BLOCK_M;
         for (int kb2 = 0; kb2 < 2 * KB; ++kb2) {  // slot order: hi(0), lo(0), hi(1), lo(1), ...
           const int kb = kb2 >> 1, col = (kb2 & 1) * p.K1p + kb * BLOCK_K;
+          // pairs hand-off: k-block 0 is the bottom row ([hi | lo], 64 columns each), k-blocks 1.. the pairs rows
+          const CUtensorMap* ma = &tmA;
+          int acol = col;
+          if (p.pairs && kb == 0) {
+            acol = (kb2 & 1) * BLOCK_K;
+          } else if (p.pairs) {
+            ma = (kb2 & 1) ? &tmPlo : &tmPhi;
+            acol = (kb - 1) * BLOCK_K;
+          }
           mbar_wait(smem_u32(empty_bar + stage), phase ^ 1);
           const uint32_t fb = smem_u32(full_bar + stage);
           uint8_t* st = smem + (size_t)stage * STAGE_BYTES;
           mbar_expect_tx(fb, STAGE_BYTES);
-          tma_load_2d(smem_u32(st), &tmA, fb, col, m0);
+          tma_load_2d(smem_u32(st), ma, fb, acol, m0);
           tma_load_2d(smem_u32(st + A_TILE_BYTES), &tmW1, fb, col, 0);
           if (++stage == p.stages) {
             stage = 0;
@@ -432,7 +447,7 @@ int mm_mlp_tc_supported(int K, int n_layers, const int* widths, int with_head) {
 }  // extern "C"
 
 typedef void (*MlpKernel)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap,
-                          const mm::mlp::Params);
+                          const CUtensorMap, const CUtensorMap, const mm::mlp::Params);
 
 // one instantiation per padded layer-1 width mm_tc_padded_n can return
 template <bool HEADS>
@@ -454,9 +469,14 @@ static MlpKernel kernel_for(int n1p) {
 static int mlp_tc_impl(const void* a_split, int64_t M, int K, int n_layers, const void* const* w_split, const int* widths,
                        const float* const* bias, const int* acts, float* out, int64_t out_stride, const float* head_w,
                        float head_b, int head_act, float* head_out, void* out_operand, void* stream,
-                       int n_heads = 0, const float* heads_b = nullptr, const int* heads_act = nullptr) {
+                       int n_heads = 0, const float* heads_b = nullptr, const int* heads_act = nullptr,
+                       const void* a_bottom = nullptr) {
   using namespace mm::mlp;
-  MM_REQUIRE(a_split && w_split && widths && bias && acts && M >= 0 && K > 0, MM_ERR_ARG, "mm_mlp_tc: null pointer or bad M/K");
+  MM_REQUIRE((a_split || M == 0) && w_split && widths && bias && acts && M >= 0 && K > 0, MM_ERR_ARG,
+             "mm_mlp_tc: null pointer or bad M/K");
+  if (M == 0) return MM_OK;  // an empty batch reads and writes nothing (its buffers may be null)
+  MM_REQUIRE(!a_bottom || (K > BLOCK_K && ((uintptr_t)a_bottom % 16) == 0), MM_ERR_ARG,
+             "mm_mlp_tc_pairs: needs K > %d and 16-B aligned bottom rows", BLOCK_K);
   MM_REQUIRE(n_layers >= 1 && n_layers <= kMaxChain + 1, MM_ERR_UNSUPPORTED, "mm_mlp_tc: 1..%d layers (got %d)", kMaxChain + 1,
              n_layers);
   MM_REQUIRE(out || head_out || out_operand, MM_ERR_ARG, "mm_mlp_tc: no output requested");
@@ -480,7 +500,6 @@ static int mlp_tc_impl(const void* a_split, int64_t M, int K, int n_layers, cons
     MM_REQUIRE(heads_act[hh] >= MM_ACT_LINEAR && heads_act[hh] <= MM_ACT_GELU, MM_ERR_ARG, "mm_mlp_tc_heads: unknown activation of head %d",
                hh);
   MM_REQUIRE(!out || out_stride >= n_last, MM_ERR_ARG, "mm_mlp_tc: out_stride < last width");
-  if (M == 0) return MM_OK;
 
   Params p;
   size_t smem = 0;
@@ -507,8 +526,20 @@ static int mlp_tc_impl(const void* a_split, int64_t M, int K, int n_layers, cons
     p.heads_out = head_out;
   }
 
-  CUtensorMap tmA, tmW1, tmC[kMaxChain];
-  int rc = mm::tc::make_map(&tmA, a_split, (uint64_t)M, (uint64_t)2 * p.K1p, BLOCK_M);
+  CUtensorMap tmA, tmW1, tmC[kMaxChain], tmPhi, tmPlo;
+  int rc;
+  if (a_bottom) {
+    // bottom rows (M, 2 * 64) = k-block 0; pairs rows [hi(Kq) | lo(Kq)], Kq = K - 64 rounded up to 8: the maps end at
+    // column K - 64, so the TMA zero-fills the rest of the last k-block
+    const uint64_t np = (uint64_t)(K - BLOCK_K), kq = (np + 7) & ~7ull;
+    p.pairs = 1;
+    rc = mm::tc::make_map(&tmA, a_bottom, (uint64_t)M, 2 * BLOCK_K, BLOCK_M);
+    if (!rc) rc = mm::tc::make_map(&tmPhi, a_split, (uint64_t)M, np, BLOCK_M, 4 * kq);
+    if (!rc) rc = mm::tc::make_map(&tmPlo, (const uint8_t*)a_split + 2 * kq, (uint64_t)M, np, BLOCK_M, 4 * kq);
+  } else {
+    rc = mm::tc::make_map(&tmA, a_split, (uint64_t)M, (uint64_t)2 * p.K1p, BLOCK_M);
+    tmPhi = tmPlo = tmA;
+  }
   if (rc) return rc;
   rc = mm::tc::make_map(&tmW1, w_split[0], (uint64_t)p.N1p, (uint64_t)2 * p.K1p, (uint32_t)p.N1p);
   if (rc) return rc;
@@ -535,7 +566,7 @@ static int mlp_tc_impl(const void* a_split, int64_t M, int K, int n_layers, cons
   const long long tiles = (M + BLOCK_M - 1) / BLOCK_M;
   const int sms = mm::sm_count();
   const unsigned grid = (unsigned)(tiles < sms ? tiles : sms);
-  kern<<<grid, kThreads, smem, (cudaStream_t)stream>>>(tmA, tmW1, tmC[0], tmC[1], tmC[2], p);
+  kern<<<grid, kThreads, smem, (cudaStream_t)stream>>>(tmA, tmW1, tmC[0], tmC[1], tmC[2], tmPhi, tmPlo, p);
   return mm::check_launch("mm_mlp_tc");
 }
 
@@ -556,6 +587,19 @@ int mm_mlp_tc_heads(const void* a_split, int64_t M, int K, int n_layers, const v
   MM_REQUIRE(heads_w && heads_out && heads_act, MM_ERR_ARG, "mm_mlp_tc_heads: null heads_w / heads_act / heads_out");
   return mlp_tc_impl(a_split, M, K, n_layers, w_split, widths, bias, acts, nullptr, 0, heads_w, 0.0f, 0, heads_out, nullptr, stream,
                      n_heads, heads_b, heads_act);
+}
+
+int mm_mlp_tc_pairs(const void* bottom_split, const void* pairs_split, int64_t M, int K, int n_layers, const void* const* w_split,
+                    const int* widths, const float* const* bias, const int* acts, float* out, int64_t out_stride,
+                    const float* head_w, float head_b, int head_act, float* head_out, int n_heads, const float* heads_b,
+                    const int* heads_act, void* stream) {
+  MM_REQUIRE(bottom_split != nullptr || M == 0, MM_ERR_ARG, "mm_mlp_tc_pairs: bottom_split is null");
+  MM_REQUIRE(n_heads >= 0 && n_heads <= mm::mlp::kMaxHeads, MM_ERR_UNSUPPORTED, "mm_mlp_tc_pairs: %d heads is not in 0..%d",
+             n_heads, mm::mlp::kMaxHeads);
+  MM_REQUIRE(!n_heads || (head_w && head_out && heads_act && !out), MM_ERR_ARG,
+             "mm_mlp_tc_pairs: heads need heads_w, heads_act and heads_out, and no fp32 rows");
+  return mlp_tc_impl(pairs_split, M, K, n_layers, w_split, widths, bias, acts, out, out_stride, head_w, head_b, head_act, head_out,
+                     nullptr, stream, n_heads, heads_b, heads_act, bottom_split);
 }
 
 int mm_mlp_tc_operand_out(const void* a_split, int64_t M, int K, int n_layers, const void* const* w_split, const int* widths,

@@ -230,12 +230,14 @@ static inline EncodeTiledFn encode_fn() {
   return fn;
 }
 
-// 2-D bf16 tensor map over a row-major (rows, cols) matrix, box = (64 cols, box_rows), SWIZZLE_128B
-static inline int make_map(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows) {
+// 2-D bf16 tensor map over a row-major (rows, cols) matrix, box = (64 cols, box_rows), SWIZZLE_128B.  pitch_bytes: row
+// pitch when the rows are wider than `cols` (0: cols * 2); elements past `cols` or `rows` load as zeros.
+static inline int make_map(CUtensorMap* map, const void* base, uint64_t rows, uint64_t cols, uint32_t box_rows,
+                           uint64_t pitch_bytes = 0) {
   EncodeTiledFn fn = encode_fn();
   MM_REQUIRE(fn != nullptr, MM_ERR_DRIVER, "cuTensorMapEncodeTiled is not available from the driver");
   cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {cols * 2};
+  cuuint64_t strides[1] = {pitch_bytes ? pitch_bytes : cols * 2};
   cuuint32_t box[2] = {64u, box_rows};
   cuuint32_t estr[2] = {1, 1};
   CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,

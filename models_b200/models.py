@@ -14,7 +14,7 @@ import torch
 
 from . import ops
 from .blocks import (FM, MLP, CategoryEncoding, CrossBlock, CrossBlockSeq, DLRM, DLRMBlock, FMBlock, MLPBlock, WideLinear, _Dense,
-                     dense_engine, run_dense_chain)
+                     dense_engine, run_dense_chain, tower_kernel_applies)
 from .core import Block, Prediction, TabularData, batch_size_of, default_device, to_device, unique_name
 from .inputs import EmbeddingOptions, EmbeddingsBlock, InputBlockV2
 from .retrieval import ItemRetrievalTask, QueryItemIdsEmbeddingsBlock, TwoTowerBlock
@@ -907,9 +907,13 @@ class RankingModel(Model):
                 # production path: bottom vector and table rows in the interaction kernel's operand format when the
                 # mirrors are on (no bf16 split inside the hot loop); split-bf16 row straight into the top tower
                 op = self.body.use_operand_rows() and self._all_onehot(inputs)
+                K = self.body.output_width_before_top()
                 bottom = self.body.bottom_forward(inputs, operand_out=op)
-                a = self.body.interaction_forward(inputs, bottom, as_split=True, operand_rows=op)
-                return chain(None, layers, a_split=a, K=self.body.output_width_before_top())
+                # the whole-tower kernel reads the bottom vector from the bottom tower's own rows: the interaction
+                # kernel then writes the pairs alone (the row sharded tables feed keeps [bottom | pairs])
+                pairs = op and self.body.sharded is None and tower_kernel_applies(layers, K, heads)
+                a = self.body.interaction_forward(inputs, bottom, as_split=True, operand_rows=op, pairs_only=pairs)
+                return chain(None, layers, a_split=a, K=K, a_bottom=bottom if pairs else None)
             bottom = self.body.bottom_forward(inputs)
             x = self.body.interaction_forward(inputs, bottom)
             return chain(x, layers)

@@ -262,16 +262,25 @@ def _lookup_tables(weights, indices, B: int, wdt: torch.dtype, wcols: int, slots
     return arr
 
 
+def pairs_cols(n_pairs: int) -> int:
+    """Columns per half of a pairs-only operand row (dlrm_lookup_interact(pairs_only=True), mlp_tc(a_bottom=...)): the pair
+    count rounded up to 8, so that each half is whole 16-byte groups."""
+    return (int(n_pairs) + 7) // 8 * 8
+
+
 def dlrm_lookup_interact(weights, indices, slots, rows, D: int, bottom: Optional[torch.Tensor], bottom_slot: int,
                          out: torch.Tensor, oob: Optional[torch.Tensor] = None, peers=None, rank: int = 0,
-                         world: int = 1, operand_rows: bool = False) -> torch.Tensor:
+                         world: int = 1, operand_rows: bool = False, pairs_only: bool = False) -> torch.Tensor:
     """Fused lookup + interaction with per-table id widths and optional row-sharded tables
     (mm_dlrm_lookup_interact).  weights[t]: the (rows, D) table or this rank's shard; indices[t]: (B,) ids
     (any width, see index_bytes_of); rows[t]: GLOBAL row count; peers[t]: None (replicated) or the `world`
     device pointers of the shards as mapped in this process.  operand_rows=True (D = 64): `weights`, the peers' shards
     and `bottom` are bf16 split rows (rows, 2*D) = [hi | lo] (split_rows / mlp_tc(out_operand=...)); needs a split-bf16
-    `out`."""
+    `out`.  pairs_only=True (with operand_rows and a bottom vector): `out` is (B, 2*pairs_cols(F(F-1)/2)) bf16 and gets the
+    pairs only, [hi | lo] (MM_ROWS_OPERAND_PAIRS); the top tower reads the bottom rows from `bottom` (mlp_tc(a_bottom=...))."""
     _dev(out, "out")
+    if pairs_only and (not operand_rows or bottom is None):
+        raise ValueError("pairs_only needs operand_rows and a bottom vector")
     B = out.shape[0]
     n = len(weights)
     if not (len(indices) == n and len(slots) == n and len(rows) == n):
@@ -289,11 +298,18 @@ def dlrm_lookup_interact(weights, indices, slots, rows, D: int, bottom: Optional
             pa = (C.c_void_p * world)(*[int(x) for x in pt])
             keep.append(pa)
             arr[t].peer_weights_host = C.cast(pa, C.POINTER(C.c_void_p))
-    o32, ostride, osplit, okp = _split_out_args(out)
+    if pairs_only:
+        F = n + 1
+        if out.dtype != torch.bfloat16 or tuple(out.shape) != (B, 2 * pairs_cols(F * (F - 1) // 2)) or not out.is_contiguous():
+            raise ValueError(f"pairs_only: out must be a contiguous bf16 ({B}, {2 * pairs_cols(F * (F - 1) // 2)}) matrix")
+        o32, ostride, osplit, okp = None, 0, out.data_ptr(), out.shape[1] // 2
+    else:
+        o32, ostride, osplit, okp = _split_out_args(out)
     _cabi.check(
         _lib().mm_dlrm_lookup_interact(arr, n, B, D, rank, world, _ptr(bottom),
                                        0 if bottom is None else (_row_stride(_dev(bottom, "bottom", wdt), "bottom") // (2 if operand_rows else 1)),
-                                       bottom_slot, o32, ostride, osplit, okp, _ptr(oob), 1 if operand_rows else 0, _stream()),
+                                       bottom_slot, o32, ostride, osplit, okp, _ptr(oob), 2 if pairs_only else 1 if operand_rows else 0,
+                                       _stream()),
         "mm_dlrm_lookup_interact")
     return out
 
@@ -722,16 +738,25 @@ def mlp_tc_supported(K: int, widths: Sequence[int], head: bool = False, heads: b
 
 
 def _tower(who: str, a_split: torch.Tensor, K: int, w_splits: Sequence[torch.Tensor], widths: Sequence[int],
-           biases: Sequence[Optional[torch.Tensor]], acts: Sequence[Optional[str]]):
+           biases: Sequence[Optional[torch.Tensor]], acts: Sequence[Optional[str]], a_bottom: Optional[torch.Tensor] = None):
     """(M, n, weight pointers, widths, bias pointers, activation codes) of a tower over the split-bf16 rows a_split
     (M, 2*Kp): layer l is w_splits[l], the mm_split_weights layout of a (k, widths[l]) kernel, biases[l] None or
-    widths[l] fp32 values, acts[l] its activation."""
+    widths[l] fp32 values, acts[l] its activation.  With a_bottom (M, 128), input columns 0..63 come from a_bottom and
+    a_split holds columns 64..K-1 as (M, 2*pairs_cols(K - 64)) rows (mm_mlp_tc_pairs)."""
     n = len(widths)
     if not (len(w_splits) == len(biases) == len(acts) == n):
         raise ValueError(f"{who}: w_splits / widths / biases / acts must have one entry per layer")
     _dev(a_split, "a_split", torch.bfloat16)
-    if a_split.dim() != 2 or a_split.shape[1] != 2 * tc_padded_k(K) or not a_split.is_contiguous():
-        raise ValueError(f"a_split must be a contiguous (M, {2 * tc_padded_k(K)}) bf16 matrix")
+    cols = 2 * tc_padded_k(K)
+    if a_bottom is not None:
+        if K <= 64:
+            raise ValueError(f"{who}: a_bottom needs K > 64")
+        cols = 2 * pairs_cols(K - 64)
+        _dev(a_bottom, "a_bottom", torch.bfloat16)
+        if tuple(a_bottom.shape) != (a_split.shape[0], 128) or not a_bottom.is_contiguous():
+            raise ValueError(f"a_bottom must be a contiguous ({a_split.shape[0]}, 128) bf16 matrix")
+    if a_split.dim() != 2 or a_split.shape[1] != cols or not a_split.is_contiguous():
+        raise ValueError(f"a_split must be a contiguous (M, {cols}) bf16 matrix")
     k = K
     for l in range(n):
         _dev(w_splits[l], f"w_split[{l}]", torch.bfloat16)
@@ -750,11 +775,14 @@ def _tower(who: str, a_split: torch.Tensor, K: int, w_splits: Sequence[torch.Ten
 def mlp_tc(a_split: torch.Tensor, K: int, w_splits: Sequence[torch.Tensor], widths: Sequence[int],
            biases: Sequence[Optional[torch.Tensor]], acts: Sequence[Optional[str]], out: Optional[torch.Tensor] = None,
            head_w: Optional[torch.Tensor] = None, head_b: float = 0.0, head_act: Optional[str] = None,
-           head_out: Optional[torch.Tensor] = None, out_operand: Optional[torch.Tensor] = None):
+           head_out: Optional[torch.Tensor] = None, out_operand: Optional[torch.Tensor] = None,
+           a_bottom: Optional[torch.Tensor] = None):
     """Whole MLP tower in one launch (mm_mlp_tc): layer 1 from the split-bf16 rows `a_split`, layers 2..n on
     chip (activations stay in registers).  out: (M, widths[-1]) fp32 and/or head_out: (M, 1); out_operand:
-    (M, 2*widths[-1]) bf16 split rows [hi | lo] for the interaction kernel (mm_mlp_tc_operand_out)."""
-    M, n, wp, wd, bp, ac = _tower("mlp_tc", a_split, K, w_splits, widths, biases, acts)
+    (M, 2*widths[-1]) bf16 split rows [hi | lo] for the interaction kernel (mm_mlp_tc_operand_out).  a_bottom: layer 1
+    reads input columns 0..63 from these (M, 128) bottom rows and the rest from the pairs rows `a_split`
+    (mm_mlp_tc_pairs)."""
+    M, n, wp, wd, bp, ac = _tower("mlp_tc", a_split, K, w_splits, widths, biases, acts, a_bottom)
     if out is not None:
         _dev(out, "out", torch.float32)
         if out.dim() != 2 or tuple(out.shape) != (M, int(widths[-1])) or out.stride(1) != 1:
@@ -765,6 +793,15 @@ def mlp_tc(a_split: torch.Tensor, K: int, w_splits: Sequence[torch.Tensor], widt
         _dev(head_w, "head_w", torch.float32), _dev(head_out, "head_out", torch.float32)
         if head_w.numel() != int(widths[-1]) or not head_w.is_contiguous() or head_out.numel() != M or not head_out.is_contiguous():
             raise ValueError("head_w must hold widths[-1] weights and head_out M contiguous values")
+    if a_bottom is not None:
+        if out_operand is not None:
+            raise ValueError("a_bottom and out_operand exclude each other")
+        _cabi.check(
+            _lib().mm_mlp_tc_pairs(a_bottom.data_ptr(), a_split.data_ptr(), M, K, n, wp, wd, bp, ac, _ptr(out),
+                                   out.stride(0) if out is not None else 0, _ptr(head_w), float(head_b), ACTIVATIONS[head_act],
+                                   _ptr(head_out), 0, None, None, _stream()),
+            "mm_mlp_tc_pairs")
+        return out if out is not None else head_out
     if out_operand is not None:
         if head_w is not None:
             raise ValueError("out_operand and the fused head exclude each other")
@@ -785,11 +822,12 @@ def mlp_tc(a_split: torch.Tensor, K: int, w_splits: Sequence[torch.Tensor], widt
 
 def mlp_tc_heads(a_split: torch.Tensor, K: int, w_splits: Sequence[torch.Tensor], widths: Sequence[int],
                  biases: Sequence[Optional[torch.Tensor]], acts: Sequence[Optional[str]], heads_w: torch.Tensor,
-                 heads_b: Optional[torch.Tensor], heads_act: Sequence[Optional[str]], out: torch.Tensor) -> torch.Tensor:
+                 heads_b: Optional[torch.Tensor], heads_act: Sequence[Optional[str]], out: torch.Tensor,
+                 a_bottom: Optional[torch.Tensor] = None) -> torch.Tensor:
     """mm_mlp_tc_heads: the whole tower with H <= 8 fused output heads; out (H, M) with
     out[h] = heads_act[h](tower(x) @ heads_w[:, h] + heads_b[h]).  heads_w (widths[-1], H) Keras layout, heads_b (H,) on the
-    device (read by the kernel, not copied to the host)."""
-    M, n, wp, wd, bp, ac = _tower("mlp_tc_heads", a_split, K, w_splits, widths, biases, acts)
+    device (read by the kernel, not copied to the host).  a_bottom: as mlp_tc (mm_mlp_tc_pairs)."""
+    M, n, wp, wd, bp, ac = _tower("mlp_tc_heads", a_split, K, w_splits, widths, biases, acts, a_bottom)
     _dev(heads_w, "heads_w", torch.float32), _dev(out, "out", torch.float32)
     H = len(heads_act)
     if tuple(heads_w.shape) != (int(widths[-1]), H) or not heads_w.is_contiguous():
@@ -798,6 +836,11 @@ def mlp_tc_heads(a_split: torch.Tensor, K: int, w_splits: Sequence[torch.Tensor]
     if tuple(out.shape) != (H, M) or not out.is_contiguous():
         raise ValueError(f"out must be a contiguous ({H}, {M}) matrix")
     ha = (C.c_int * H)(*[ACTIVATIONS[a] for a in heads_act])
+    if a_bottom is not None:
+        _cabi.check(_lib().mm_mlp_tc_pairs(a_bottom.data_ptr(), a_split.data_ptr(), M, K, n, wp, wd, bp, ac, None, 0,
+                                           heads_w.data_ptr(), 0.0, 0, out.data_ptr(), H, _ptr(heads_b), ha, _stream()),
+                    "mm_mlp_tc_pairs")
+        return out
     _cabi.check(_lib().mm_mlp_tc_heads(a_split.data_ptr(), M, K, n, wp, wd, bp, ac, H, heads_w.data_ptr(), _ptr(heads_b), ha,
                                        out.data_ptr(), _stream()), "mm_mlp_tc_heads")
     return out
