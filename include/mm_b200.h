@@ -828,6 +828,51 @@ int mm_ncf_head_fwd_bwd(const float* table_u, int64_t rows_u, const void* ids_u,
                         float* out, float* loss, float* reg, float* du, float* di, float* dh, int64_t dh_stride, float* dw,
                         float* db, int32_t* oob_count, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * K21  In-batch pairwise ranking losses of the retrieval step (losses/pairwise.py: BPR, BPR-max, TOP1, TOP1-v2,
+ * TOP1-max, logistic, hinge), forward and backward without the (B, N) scores.  Added with the pairwise retrieval
+ * losses; no existing entry point changed.
+ *   Scores: sp[b] = pos_logit[b] (mm_positive_scores, already / T); s[b,n] = masked ? false_neg_score / T : q_b.neg_n / T
+ *   with masked = downscore && pos_ids[b] == neg_ids[n] (a constant: no gradient).  d = sp - s, w = softmax_n(s[b,:]),
+ *   eps0(x) = (x == 0 ? x + 1e-24 : x) decided on float32 values computed without flush-to-zero.  Per element:
+ *     MM_PAIRWISE_BPR       -log(eps0(sigmoid(d)))
+ *     MM_PAIRWISE_BPR_MAX   -log(eps0(sigmoid(d) w)) + reg_lambda s^2 w
+ *     MM_PAIRWISE_TOP1      sigmoid(-d) + sigmoid(s^2)
+ *     MM_PAIRWISE_TOP1_V2   as TOP1, plus - sigmoid(sp^2) once per row
+ *     MM_PAIRWISE_TOP1_MAX  (sigmoid(-d) + sigmoid(s^2)) w
+ *     MM_PAIRWISE_LOGISTIC  relu(-d) + log1p(eps0(exp(-|d|)))
+ *     MM_PAIRWISE_HINGE     relu(1 - d)
+ *   loss = c sum over the B N elements (+ the TOP1_V2 row terms), c = 1 / (B N): Keras' mean over the (B, N) losses
+ *   (TOP1_V2: its mean over N, then over B).  Masked elements take part with their constant score.
+ *   mm_inbatch_pairwise_fwd  stats (B, 4) = [row loss, dloss/dsp (without c / T), lse over the row's negatives, A] (lse
+ *       and A: the -max kinds' soft-max terms the backward reads); loss (nullable) += c sum_b stats[b, 0] in a fixed
+ *       order (zero it first).  One CTA per 128 queries streams the negatives once, the -max kinds twice (the first
+ *       pass finds the log-sum-exp the eps0 decision needs).
+ *   mm_inbatch_pairwise_bwd  from the forward's stats: g = c / T dloss/ds,
+ *         dq[b] = c / T stats[b, 1] pos[b] + sum_n g[b,n] neg[n];  dpos[b] = c / T stats[b, 1] q[b];  dneg[n] = sum_b g[b,n] q[b]
+ *       dpos may alias dneg when the negatives are the positives (N == B): the sum is written; dq aliases neither.  Two
+ *       wgmma kernels recompute the scores tile by tile (one CTA per 128 queries / per 128 negatives); each output row
+ *       is written by one CTA: deterministic.
+ *   Both: q_split / neg_split the split-bf16 operands (mm_split_rows, Kp = mm_tc_padded_k(D) <= 128, 16-B aligned),
+ *   pos_logit (B,), stats 16-B aligned, q, pos (B, D), dq, dpos (B, D), dneg (N, D) contiguous fp32.  Errors before any
+ *   launch: MM_ERR_ARG (null pointer, T <= 0, N <= 0, unknown kind, reg_lambda not finite, ids missing for
+ *   down-scoring, dpos == dneg with N != B), MM_ERR_UNSUPPORTED (D > 128, sizes >= 2^31), MM_ERR_ALIGN.
+ * ------------------------------------------------------------------------------------- */
+#define MM_PAIRWISE_BPR 0
+#define MM_PAIRWISE_BPR_MAX 1
+#define MM_PAIRWISE_TOP1 2
+#define MM_PAIRWISE_TOP1_V2 3
+#define MM_PAIRWISE_TOP1_MAX 4
+#define MM_PAIRWISE_LOGISTIC 5
+#define MM_PAIRWISE_HINGE 6
+int mm_inbatch_pairwise_fwd(const void* q_split, const void* neg_split, int64_t B, int64_t N, int D, const void* pos_ids,
+                            const void* neg_ids, int id_dtype, int downscore, float false_neg_score, float temperature, int kind,
+                            float reg_lambda, const float* pos_logit, float* stats, float* loss, void* stream);
+int mm_inbatch_pairwise_bwd(const void* q_split, const void* neg_split, int64_t B, int64_t N, int D, const void* pos_ids,
+                            const void* neg_ids, int id_dtype, int downscore, float false_neg_score, float temperature, int kind,
+                            float reg_lambda, const float* pos_logit, const float* stats, const float* q, const float* pos,
+                            float* dq, float* dpos, float* dneg, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

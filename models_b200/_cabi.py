@@ -96,6 +96,8 @@ class WideBag(C.Structure):
 WIDE_MODES = {"multi_hot": 0, "count": 1}  # MM_WIDE_MULTI_HOT / MM_WIDE_COUNT
 OPTIMIZERS = {"sgd": 0, "adagrad": 1, "adam": 2}
 LOSS_KINDS = {"binary_crossentropy": 0, "mse": 1}  # MM_LOSS_BCE / MM_LOSS_MSE
+# mm_inbatch_pairwise_fwd / _bwd loss kinds (MM_PAIRWISE_*), by the reference's registry names
+PAIRWISE_KINDS = {"bpr": 0, "bpr-max": 1, "top1": 2, "top1_v2": 3, "top1-max": 4, "logistic": 5, "hinge": 6}
 HYPER_LR, HYPER_BETA1, HYPER_BETA2, HYPER_EPS, HYPER_STEP, HYPER_LR_T, HYPER_COUNT = 0, 1, 2, 3, 4, 5, 8
 CONCAT_L2_CTAS = 512  # MM_CONCAT_L2_CTAS: mm_concat_backward_l2's partials per slice
 
@@ -239,6 +241,9 @@ SIGNATURES = {
     "mm_mmoe_task_heads_fwd_bwd": (_i, [C.POINTER(C.c_void_p), C.POINTER(C.c_int64), _i64, _i, _i, _vp, _vp, C.POINTER(C.c_int),
                                         C.POINTER(C.c_float), C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_void_p),
                                         _vp, _vp, C.POINTER(C.c_void_p), C.POINTER(C.c_int64), _i, _vp, _vp, _vp]),
+    "mm_inbatch_pairwise_fwd": (_i, [_vp, _vp, _i64, _i64, _i, _vp, _vp, _i, _i, _f, _f, _i, _f, _vp, _vp, _vp, _vp]),
+    "mm_inbatch_pairwise_bwd": (_i, [_vp, _vp, _i64, _i64, _i, _vp, _vp, _i, _i, _f, _f, _i, _f, _vp, _vp, _vp, _vp, _vp, _vp,
+                                     _vp, _vp]),
     "mm_ncf_head_fwd_bwd": (_i, [_vp, _i64, _vp, _i, _vp, _i64, _vp, _i, _i, _vp, _i64, _i, _i, _i64, _i, _vp, _vp, C.POINTER(C.c_int),
                                  C.POINTER(C.c_float), C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_void_p), _f, _vp,
                                  _i64, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp]),

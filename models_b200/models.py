@@ -1439,6 +1439,16 @@ class RetrievalModel(Model):
     _TRANSIENT = {"pre_eval_topk": None}
     _fit_skip = ("loss", "loss_batch")  # History: "loss" and "regularization_loss"
 
+    def _compile_training(self, optimizer, loss=None, loss_weights=None, metrics=None, weighted_metrics=None) -> None:
+        """As Model's, and `loss` may also name one of the reference's pairwise losses (models_b200/losses.py): "bpr",
+        "bpr-max", "top1", "top1_v2", "top1-max", "logistic", "hinge" or a loss object.  `pairwise_loss` keeps it (None:
+        the in-batch soft-max cross-entropy)."""
+        from .losses import get
+
+        pairwise = None if isinstance(loss, dict) else get(loss)
+        super()._compile_training(optimizer, None if pairwise is not None else loss, loss_weights, metrics, weighted_metrics)
+        self.pairwise_loss = pairwise
+
     def train_step(self, data) -> Dict[str, torch.Tensor]:
         """One optimizer step on `data` = (inputs,) or (inputs, targets); the targets are ignored, because the retrieval task
         builds its own one-hot targets (the positive item on column 0).  Returns {"loss", "loss_batch",

@@ -7,6 +7,7 @@ current CUDA stream.  There is no CPU path — a CPU tensor is an error.
 from __future__ import annotations
 
 import ctypes as C
+import math
 from typing import Optional, Sequence
 
 import torch
@@ -488,6 +489,68 @@ def inbatch_softmax_ce_backward(q_split, neg_split, D: int, stats, q, pos, row_s
                                               stats.data_ptr(), q.data_ptr(), pos.data_ptr(), row_scale.data_ptr(), int(scalar),
                                               dq.data_ptr(), dpos.data_ptr(), dneg.data_ptr(), _ptr(loss), _stream()),
         "mm_inbatch_softmax_ce_backward")
+
+
+def _pairwise_args(kind: str, reg_lambda: float, q_split, neg_split, D: int, pos_logit, stats) -> tuple:
+    """The checks mm_inbatch_pairwise_fwd / _bwd share; returns (B, N, kind code)."""
+    if kind not in _cabi.PAIRWISE_KINDS:
+        raise ValueError(f"pairwise loss kind must be among {sorted(_cabi.PAIRWISE_KINDS)}, got {kind!r}")
+    if not math.isfinite(float(reg_lambda)):
+        raise ValueError(f"reg_lambda must be finite, got {reg_lambda}")
+    _dev(q_split, "q_split", torch.bfloat16), _dev(neg_split, "neg_split", torch.bfloat16)
+    _dev(pos_logit, "pos_logit", torch.float32), _dev(stats, "stats", torch.float32)
+    B, N = q_split.shape[0], neg_split.shape[0]
+    if N == 0:
+        raise ValueError("in-batch pairwise losses need at least one negative")
+    Kp = tc_padded_k(D)
+    for n_, t_, shape in (("q_split", q_split, (B, 2 * Kp)), ("neg_split", neg_split, (N, 2 * Kp)), ("stats", stats, (B, 4))):
+        if tuple(t_.shape) != shape or not t_.is_contiguous():
+            raise ValueError(f"{n_} must be contiguous {shape}, got {tuple(t_.shape)}")
+    _vec(pos_logit, B, "pos_logit")
+    return B, N, _cabi.PAIRWISE_KINDS[kind]
+
+
+def inbatch_pairwise(q_split, neg_split, D: int, pos_logit, stats, kind: str, loss=None, pos_ids=None, neg_ids=None,
+                     downscore=True, false_neg_score: float = -655.04, temperature: float = 1.0,
+                     reg_lambda: float = 1.0) -> torch.Tensor:
+    """Forward of an in-batch pairwise ranking loss (mm_inbatch_pairwise_fwd): kind one of _cabi.PAIRWISE_KINDS (the
+    reference's names "bpr", "bpr-max", "top1", "top1_v2", "top1-max", "logistic", "hinge"); the positive scores
+    pos_logit (B,) (positive_scores, already / T) against the masked scores q_split @ neg_split^T / T.  Writes stats
+    (B, 4) = [row loss, dloss/dsp, log-sum-exp, A] for inbatch_pairwise_backward and adds the mean loss over the B N
+    elements to `loss` (nullable, one float).  Nothing is allocated, so a training step can be captured into a CUDA graph."""
+    B, N, code = _pairwise_args(kind, reg_lambda, q_split, neg_split, D, pos_logit, stats)
+    if loss is not None and (_dev(loss, "loss", torch.float32).numel() < 1):
+        raise ValueError("loss must hold at least one value")
+    pos_ids, neg_ids, id_dt = _item_ids(pos_ids, neg_ids, downscore)
+    _cabi.check(
+        _lib().mm_inbatch_pairwise_fwd(q_split.data_ptr(), neg_split.data_ptr(), B, N, int(D), _ptr(pos_ids), _ptr(neg_ids), id_dt,
+                                       int(bool(downscore)), float(false_neg_score), float(temperature), code, float(reg_lambda),
+                                       pos_logit.data_ptr(), stats.data_ptr(), _ptr(loss), _stream()),
+        "mm_inbatch_pairwise_fwd")
+    return stats
+
+
+def inbatch_pairwise_backward(q_split, neg_split, D: int, pos_logit, stats, q, pos, dq, dpos, dneg, kind: str, pos_ids=None,
+                              neg_ids=None, downscore=True, false_neg_score: float = -655.04, temperature: float = 1.0,
+                              reg_lambda: float = 1.0) -> None:
+    """Backward of inbatch_pairwise (mm_inbatch_pairwise_bwd) from the operands and stats of the forward: writes dq, dpos
+    (B, D) and dneg (N, D) of the mean loss.  dpos may be dneg (in-batch negatives, N == B): the sum is written."""
+    B, N, code = _pairwise_args(kind, reg_lambda, q_split, neg_split, D, pos_logit, stats)
+    for n_, t_, shape in (("q", q, (B, D)), ("pos", pos, (B, D)), ("dq", dq, (B, D)), ("dpos", dpos, (B, D)), ("dneg", dneg, (N, D))):
+        _dev(t_, n_, torch.float32)
+        if tuple(t_.shape) != shape or not t_.is_contiguous():
+            raise ValueError(f"{n_} must be contiguous {shape}, got {tuple(t_.shape)}")
+    if dpos.data_ptr() == dneg.data_ptr() and N != B:
+        raise ValueError("dpos may be dneg only when the negatives are the positives (N == B)")
+    if dq.data_ptr() in (dpos.data_ptr(), dneg.data_ptr()):
+        raise ValueError("dq must not alias dpos / dneg")
+    pos_ids, neg_ids, id_dt = _item_ids(pos_ids, neg_ids, downscore)
+    _cabi.check(
+        _lib().mm_inbatch_pairwise_bwd(q_split.data_ptr(), neg_split.data_ptr(), B, N, int(D), _ptr(pos_ids), _ptr(neg_ids), id_dt,
+                                       int(bool(downscore)), float(false_neg_score), float(temperature), code, float(reg_lambda),
+                                       pos_logit.data_ptr(), stats.data_ptr(), q.data_ptr(), pos.data_ptr(), dq.data_ptr(),
+                                       dpos.data_ptr(), dneg.data_ptr(), _stream()),
+        "mm_inbatch_pairwise_bwd")
 
 
 _CONCAT_DTYPES = {torch.int32: _cabi.MM_I32, torch.int64: _cabi.MM_I64, torch.float32: _cabi.MM_F32,

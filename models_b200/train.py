@@ -1124,7 +1124,8 @@ class TwoTowerTrainer(_StepTrainer):
               mm_dense_tc per layer (fp32 activation saved + the next layer's operand); mm_l2_normalize (post="l2-norm");
               mm_split_rows of both outputs; mm_positive_scores + mm_inbatch_softmax_ce (no (b, 1+b) logits)
     backward  mm_inbatch_softmax_ce_backward (c = 1/b: Keras' mean; dpos and dneg summed into one item gradient, the loss
-              accumulated on the device); mm_l2_normalize_backward; per tower mm_dense_wgrad[_split] + mm_dense_dgrad down to
+              accumulated on the device) — or, compiled with a pairwise loss (models_b200/losses.py), mm_inbatch_pairwise_fwd
+              + mm_inbatch_pairwise_bwd in place of mm_inbatch_softmax_ce and its backward; mm_l2_normalize_backward; per tower mm_dense_wgrad[_split] + mm_dense_dgrad down to
               x0; mm_concat_backward into each table's (b, D) IndexedSlices buffer; mm_bag_grad_rows for multi-hot features
     update    mm_opt_tick, mm_dense_apply over ONE arena holding both towers, one mm_sparse_rows_apply per embedding width
               (and per multi-hot table), mm_split_weights refresh of the operand copies the model's forward reads."""
@@ -1200,13 +1201,18 @@ class TwoTowerTrainer(_StepTrainer):
             # the in-batch kernels' operand of the output; a tower without layers or post hands them x0's split xs
             t["split"] = torch.zeros((B, 2 * ops.tc_padded_k(self.D)), **bf) if (t["layers"] or self.l2) else None
         self.pos_logit = torch.zeros(B, **f32)
-        self.stats = torch.zeros((B, 3), **f32)
-        ws = max(ops.catalog_workspace_bytes(min(128 * m, B), min(128 * m, B)) for m in range(1, (B + 127) // 128 + 1))
-        self.ws = torch.zeros(ws, dtype=torch.uint8, device=self.device)
+        # the compiled loss: None = the soft-max cross-entropy, else a models_b200.losses.PairwiseLoss
+        self.pairwise = getattr(model, "pairwise_loss", None)
+        if self.pairwise is None:
+            self.stats = torch.zeros((B, 3), **f32)
+            ws = max(ops.catalog_workspace_bytes(min(128 * m, B), min(128 * m, B)) for m in range(1, (B + 127) // 128 + 1))
+            self.ws = torch.zeros(ws, dtype=torch.uint8, device=self.device)
+        else:
+            self.stats = torch.zeros((B, 4), **f32)  # [row loss, dloss/dsp, lse, A] of mm_inbatch_pairwise_fwd
         self._inv_b: Dict[int, torch.Tensor] = {}  # c = 1/b per batch size, one device float each
         self._init_loss(B)
         self.loss = self._loss_all  # [total, regularization]
-        self.logits = self.stats  # [max, log-sum-exp, positive logit] of every row of the last step
+        self.logits = self.stats  # per row of the last step: CE [max, log-sum-exp, positive logit]; pairwise as above
         # one counter for both towers (every gather receives it), so check_indices sees every table
         self.oob = next((p.oob for p in self.inps if p.oob is not None), None)
 
@@ -1296,13 +1302,20 @@ class TwoTowerTrainer(_StepTrainer):
         ids = ops.as_index(inputs[self.item_id]).reshape(-1) if self.downscore else None  # packed host-batch ids widened
         T = self.temperature
         ops.positive_scores(q, it, self.pos_logit[:b], temperature=T)
-        ops.inbatch_softmax_ce_split(qs, its, self.D, self.pos_logit[:b], self.stats[:b], self.ws, pos_ids=ids, neg_ids=ids,
-                                     downscore=self.downscore, false_neg_score=self.false_neg_score, temperature=T)
         # dq -> the query tower's last dh, d_item = dpos + dneg (the negatives are the positives) -> the item tower's
         dq, di = self.towers[0]["dout"][:b], self.towers[1]["dout"][:b]
-        ops.inbatch_softmax_ce_backward(qs, its, self.D, self.stats[:b], q, it, self._scale(b), dq, di, di, loss=self._loss_all[:1],
-                                        pos_ids=ids, neg_ids=ids, downscore=self.downscore, false_neg_score=self.false_neg_score,
-                                        temperature=T)
+        pw = self.pairwise
+        if pw is None:
+            ops.inbatch_softmax_ce_split(qs, its, self.D, self.pos_logit[:b], self.stats[:b], self.ws, pos_ids=ids, neg_ids=ids,
+                                         downscore=self.downscore, false_neg_score=self.false_neg_score, temperature=T)
+            ops.inbatch_softmax_ce_backward(qs, its, self.D, self.stats[:b], q, it, self._scale(b), dq, di, di, loss=self._loss_all[:1],
+                                            pos_ids=ids, neg_ids=ids, downscore=self.downscore,
+                                            false_neg_score=self.false_neg_score, temperature=T)
+        else:
+            kw = dict(pos_ids=ids, neg_ids=ids, downscore=self.downscore, false_neg_score=self.false_neg_score, temperature=T,
+                      reg_lambda=getattr(pw, "reg_lambda", 1.0))
+            ops.inbatch_pairwise(qs, its, self.D, self.pos_logit[:b], self.stats[:b], pw.kind, loss=self._loss_all[:1], **kw)
+            ops.inbatch_pairwise_backward(qs, its, self.D, self.pos_logit[:b], self.stats[:b], q, it, dq, di, di, pw.kind, **kw)
         for tw, inp, dout in zip(self.towers, self.inps, (dq, di)):
             self._tower_backward(tw, inp, dout, b)
         self._bag_grads()
