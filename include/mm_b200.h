@@ -646,10 +646,11 @@ int mm_wide_rows_apply(float* wide, float* state1, float* state2, int64_t wide_r
  *       q_split / neg_split: the operands the forward read (mm_split_rows, Kp = mm_tc_padded_k(D) <= 128, 16-B aligned);
  *       stats (B,3): mm_inbatch_softmax_ce's output; q, pos (B, D), dq, dpos (B, D), dneg (N, D): contiguous fp32.
  *       dpos may alias dneg when the negatives are the positives (in-batch, N == B): the sum is written.  dq aliases
- *       neither.  Two wgmma kernels recompute the logits tile by tile (inbatch_ce_dq_kernel: one CTA per 128 queries;
- *       inbatch_ce_dn_kernel: one CTA per 128 negatives), each output row is written by one CTA: deterministic.
+ *       neither.  Two wgmma kernels recompute the logits tile by tile (inbatch_flash_kernel<SoftmaxCE, DQ>: one CTA per
+ *       128 queries; <SoftmaxCE, DN>: one CTA per 128 negatives), each output row is written by one CTA: deterministic.
  *       Errors before any launch: MM_ERR_ARG (null pointer, T <= 0, N <= 0, ids missing for down-scoring, dpos == dneg with
- *       N != B), MM_ERR_UNSUPPORTED (D > 128, sizes >= 2^31), MM_ERR_ALIGN (split operands not 16-B aligned).
+ *       N != B), MM_ERR_UNSUPPORTED (D > 128, sizes >= 2^31), MM_ERR_ALIGN (split operands not 16-B aligned, an fp32
+ *       buffer not 4-B aligned).  Arguments that break several rules get the code of one of them, not a fixed one.
  *   mm_l2_normalize_backward  backward of mm_l2_normalize from its INPUT x: s = sum(x^2), n = sqrt(s), y = x / n;
  *       s >= 1e-12: dx = (dy - y (y.dy)) / n, else dx = dy / 1e-6 (TF's gradient of maximum(s, 1e-12) flows to s only
  *       where s >= 1e-12).  dx may alias x or dy.
@@ -856,7 +857,8 @@ int mm_ncf_head_fwd_bwd(const float* table_u, int64_t rows_u, const void* ids_u,
  *   Both: q_split / neg_split the split-bf16 operands (mm_split_rows, Kp = mm_tc_padded_k(D) <= 128, 16-B aligned),
  *   pos_logit (B,), stats 16-B aligned, q, pos (B, D), dq, dpos (B, D), dneg (N, D) contiguous fp32.  Errors before any
  *   launch: MM_ERR_ARG (null pointer, T <= 0, N <= 0, unknown kind, reg_lambda not finite, ids missing for
- *   down-scoring, dpos == dneg with N != B), MM_ERR_UNSUPPORTED (D > 128, sizes >= 2^31), MM_ERR_ALIGN.
+ *   down-scoring, dpos == dneg with N != B), MM_ERR_UNSUPPORTED (D > 128, sizes >= 2^31), MM_ERR_ALIGN.  Arguments that
+ *   break several rules get the code of one of them, not a fixed one.
  * ------------------------------------------------------------------------------------- */
 #define MM_PAIRWISE_BPR 0
 #define MM_PAIRWISE_BPR_MAX 1

@@ -49,12 +49,6 @@ struct Params {
   float false_neg_score, inv_temp;
 };
 
-__device__ __forceinline__ float ex2_approx(float x) {  // x <= 0 here: flush-to-zero underflow is exact enough
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-
 // insert (x, id) into the descending list (tv, ti) of length k (x > tv[k-1] is known); returns the new k-th value
 static __device__ __noinline__ float topk_insert(float* tv, long long* ti, int k, float x, long long id) {
   int pos = k - 1;

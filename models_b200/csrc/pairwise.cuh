@@ -1,5 +1,6 @@
 // Per-element functions of the in-batch pairwise ranking losses (the reference's losses/pairwise.py), shared by the
-// forward statistics kernel and the two backward kernels of inbatch_pairwise.cu so that they evaluate one formula.  The
+// forward statistics kernel and the two backward kernels (inbatch_flash.cu, Pairwise<KIND>) so that they evaluate one
+// formula.  The
 // dq kernel recomputes the forward's scores bit for bit; the dn kernel's S^T = N Q^T may differ in the last bit, so an
 // element within rounding of an eps0 / relu boundary can fall on the other side there (one element of c / T).
 //

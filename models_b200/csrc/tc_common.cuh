@@ -1,4 +1,5 @@
-// wgmma / TMA / mbarrier PTX wrappers shared by the tensor-core kernels (dense_tc.cu, mlp_tc.cu, catalog_tc.cu).
+// wgmma / TMA / mbarrier PTX wrappers shared by the tensor-core kernels (dense_tc.cu, mlp_tc.cu, catalog_tc.cu,
+// inbatch_flash.cu).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -51,6 +52,13 @@ __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_grou
 __device__ __forceinline__ void wgmma_fence_acc(float (&d)[64]) {
 #pragma unroll
   for (int i = 0; i < 64; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// 2^x with flush-to-zero: the soft-max exp of the catalog forward, which the in-batch soft-max backward must repeat
+// exactly.  Only where x <= 0 (underflow to 0 is exact enough) and no `== 0` test reads the result.
+__device__ __forceinline__ float ex2_approx(float x) {
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
 }
 __device__ __forceinline__ void named_bar(int id, int threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");

@@ -461,21 +461,10 @@ def inbatch_softmax_ce_backward(q_split, neg_split, D: int, stats, q, pos, row_s
     (q_split (B, 2*Kp), neg_split (N, 2*Kp)) and its stats (B, 3), writes dq, dpos (B, D) and dneg (N, D) of
     sum_b c[b] (lse[b] - s[b,0]) and adds that loss to `loss` (nullable).  row_scale: (B,) or (1,) fp32 c.  dpos may be
     dneg (in-batch negatives, N == B): the sum is written."""
-    _dev(q_split, "q_split", torch.bfloat16), _dev(neg_split, "neg_split", torch.bfloat16)
-    for n_, t_ in (("stats", stats), ("q", q), ("pos", pos), ("row_scale", row_scale), ("dq", dq), ("dpos", dpos), ("dneg", dneg)):
-        _dev(t_, n_, torch.float32)
-        if not t_.is_contiguous():
-            raise ValueError(f"{n_} must be contiguous")
+    B, N = _inbatch_buffers(D, q_split, neg_split, stats, 3, (q, pos, dq, dpos, dneg), extra=(("row_scale", row_scale),),
+                            joint=False)
     if loss is not None:
         _dev(loss, "loss", torch.float32)
-    B, N = q_split.shape[0], neg_split.shape[0]
-    Kp = tc_padded_k(D)
-    for n_, t_, shape in (("q_split", q_split, (B, 2 * Kp)), ("neg_split", neg_split, (N, 2 * Kp)), ("stats", stats, (B, 3)),
-                          ("q", q, (B, D)), ("pos", pos, (B, D)), ("dq", dq, (B, D)), ("dpos", dpos, (B, D)), ("dneg", dneg, (N, D))):
-        if tuple(t_.shape) != shape:
-            raise ValueError(f"{n_} must be {shape}, got {tuple(t_.shape)}")
-    if not (q_split.is_contiguous() and neg_split.is_contiguous()):
-        raise ValueError("q_split and neg_split must be contiguous")
     _vec(neg_prob, N, "neg_prob")
     if loss is not None and loss.numel() < 1:
         raise ValueError("loss must hold at least one value")
@@ -491,21 +480,41 @@ def inbatch_softmax_ce_backward(q_split, neg_split, D: int, stats, q, pos, row_s
         "mm_inbatch_softmax_ce_backward")
 
 
-def _pairwise_args(kind: str, reg_lambda: float, q_split, neg_split, D: int, pos_logit, stats) -> tuple:
-    """The checks mm_inbatch_pairwise_fwd / _bwd share; returns (B, N, kind code)."""
+def _inbatch_buffers(D: int, q_split, neg_split, stats, stats_cols: int, grads=None, extra=(), joint=True) -> tuple:
+    """The buffers every in-batch kernel reads: the split operands q_split (B, 2*Kp) and neg_split (N, 2*Kp), bf16, and
+    the fp32 stats (B, stats_cols); with grads = (q, pos, dq, dpos, dneg), a backward's fp32 q, pos, dq, dpos (B, D) and
+    dneg (N, D); extra: more (name, fp32 tensor) pairs of any shape.  All contiguous on the device; returns (B, N).
+    joint: one "X must be contiguous (shape), got ..." error per tensor (the pairwise wrappers); otherwise the soft-max
+    backward's separate "X must be contiguous", "X must be (shape), got ..." and "q_split and neg_split must be
+    contiguous"."""
+    _dev(q_split, "q_split", torch.bfloat16), _dev(neg_split, "neg_split", torch.bfloat16)
+    B, N = q_split.shape[0], neg_split.shape[0]
+    Kp = tc_padded_k(D)
+    fp32 = [("stats", stats, (B, stats_cols))]
+    if grads is not None:
+        fp32 += list(zip(("q", "pos", "dq", "dpos", "dneg"), grads, [(B, D)] * 4 + [(N, D)]))
+    for n_, t_ in [(n_, t_) for n_, t_, _ in fp32] + list(extra):
+        _dev(t_, n_, torch.float32)
+        if not joint and not t_.is_contiguous():
+            raise ValueError(f"{n_} must be contiguous")
+    for n_, t_, shape in [("q_split", q_split, (B, 2 * Kp)), ("neg_split", neg_split, (N, 2 * Kp))] + fp32:
+        if tuple(t_.shape) != shape or (joint and not t_.is_contiguous()):
+            raise ValueError(f"{n_} must be {'contiguous ' if joint else ''}{shape}, got {tuple(t_.shape)}")
+    if not (q_split.is_contiguous() and neg_split.is_contiguous()):
+        raise ValueError("q_split and neg_split must be contiguous")
+    return B, N
+
+
+def _pairwise_args(kind: str, reg_lambda: float, q_split, neg_split, D: int, pos_logit, stats, grads=None) -> tuple:
+    """The checks mm_inbatch_pairwise_fwd / _bwd share (grads: as _inbatch_buffers); returns (B, N, kind code)."""
     if kind not in _cabi.PAIRWISE_KINDS:
         raise ValueError(f"pairwise loss kind must be among {sorted(_cabi.PAIRWISE_KINDS)}, got {kind!r}")
     if not math.isfinite(float(reg_lambda)):
         raise ValueError(f"reg_lambda must be finite, got {reg_lambda}")
-    _dev(q_split, "q_split", torch.bfloat16), _dev(neg_split, "neg_split", torch.bfloat16)
-    _dev(pos_logit, "pos_logit", torch.float32), _dev(stats, "stats", torch.float32)
-    B, N = q_split.shape[0], neg_split.shape[0]
+    _dev(pos_logit, "pos_logit", torch.float32)
+    B, N = _inbatch_buffers(D, q_split, neg_split, stats, 4, grads)
     if N == 0:
         raise ValueError("in-batch pairwise losses need at least one negative")
-    Kp = tc_padded_k(D)
-    for n_, t_, shape in (("q_split", q_split, (B, 2 * Kp)), ("neg_split", neg_split, (N, 2 * Kp)), ("stats", stats, (B, 4))):
-        if tuple(t_.shape) != shape or not t_.is_contiguous():
-            raise ValueError(f"{n_} must be contiguous {shape}, got {tuple(t_.shape)}")
     _vec(pos_logit, B, "pos_logit")
     return B, N, _cabi.PAIRWISE_KINDS[kind]
 
@@ -535,11 +544,7 @@ def inbatch_pairwise_backward(q_split, neg_split, D: int, pos_logit, stats, q, p
                               reg_lambda: float = 1.0) -> None:
     """Backward of inbatch_pairwise (mm_inbatch_pairwise_bwd) from the operands and stats of the forward: writes dq, dpos
     (B, D) and dneg (N, D) of the mean loss.  dpos may be dneg (in-batch negatives, N == B): the sum is written."""
-    B, N, code = _pairwise_args(kind, reg_lambda, q_split, neg_split, D, pos_logit, stats)
-    for n_, t_, shape in (("q", q, (B, D)), ("pos", pos, (B, D)), ("dq", dq, (B, D)), ("dpos", dpos, (B, D)), ("dneg", dneg, (N, D))):
-        _dev(t_, n_, torch.float32)
-        if tuple(t_.shape) != shape or not t_.is_contiguous():
-            raise ValueError(f"{n_} must be contiguous {shape}, got {tuple(t_.shape)}")
+    B, N, code = _pairwise_args(kind, reg_lambda, q_split, neg_split, D, pos_logit, stats, (q, pos, dq, dpos, dneg))
     if dpos.data_ptr() == dneg.data_ptr() and N != B:
         raise ValueError("dpos may be dneg only when the negatives are the positives (N == B)")
     if dq.data_ptr() in (dpos.data_ptr(), dneg.data_ptr()):
