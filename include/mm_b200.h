@@ -875,6 +875,39 @@ int mm_inbatch_pairwise_bwd(const void* q_split, const void* neg_split, int64_t 
                             float reg_lambda, const float* pos_logit, const float* stats, const float* q, const float* pos,
                             float* dq, float* dpos, float* dneg, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * K22  Backward of the full-catalog soft-max cross-entropy (CategoricalOutput over a weight-tied EmbeddingTable,
+ * outputs/classification.py:127-216 and :311-382; CategoricalCrossentropy(from_logits=True)) without the (B, N) logits.
+ * Added with catalog training; no existing entry point changed.
+ *   mm_catalog_softmax_ce_backward  x_split = mm_split_rows(x / T) (the tempered queries), e_split = mm_split_rows(E)
+ *       (N, D), bias (N,) = b / T or null, T = temperature: the operands mm_catalog_score read for stats (B, 3).  With
+ *       s[b,j] = (x_b / T).e_j + b_j / T recomputed from them exactly as that call did, p = exp(s - stats[b,1]) and
+ *       y = labels (B,) (label_dtype MM_I32 / MM_I64):
+ *         G[b,j] = c[b] (p[b,j] - [j == y_b])
+ *         dx[b] = 1/T sum_j G[b,j] e_j  (the gradient of x itself);  de[j] = sum_b G[b,j] x_b / T;  db[j] = 1/T sum_b G[b,j]
+ *         *loss += sum_b c[b] (stats[b,1] - stats[b,2])   (loss nullable; accumulated: zero it first)
+ *       c = row_scale: (B,) device floats, or ONE device float when row_scale_is_scalar.  db nullable (no bias gradient).
+ *       A label outside [0, N) is never used as an address: it matches no column, so its row's gradient keeps the
+ *       soft-max term only (and mm_catalog_score leaves its target logit NaN), and it adds one to *oob_count (nullable,
+ *       int32: the out-of-range counter of the gathers, which the trainers read after the step).  dx (B, D), de (N, D), db (N,): fp32,
+ *       contiguous, dx and de distinct.  Two wgmma kernels (inbatch_flash_kernel<CatalogCE, DQ / DN>): one CTA per 128 queries
+ *       streaming the catalog and one per 128 catalog rows streaming the queries; each output row is written by one CTA.
+ *       When ceil(B / 128) is below the SM count the dq kernel splits the catalog over several CTAs per query tile, which
+ *       write partial dx into `workspace` that one more kernel sums in split order: deterministic, no atomics.  Both
+ *       kernels add their wgmma accumulator into their own output rows every 256 streamed tiles (long fp32 accumulations
+ *       on wgmma lose magnitude), so the workspace stays below 128 * SMs * D floats for any catalog.
+ *       workspace: at least mm_catalog_softmax_ce_workspace_bytes(B, N, D) bytes, 16-B aligned (null when that is 0).
+ *       Errors before any launch: MM_ERR_ARG (null pointer, T <= 0, N <= 0, bad label dtype, workspace too small),
+ *       MM_ERR_UNSUPPORTED (D > 128, sizes >= 2^31), MM_ERR_ALIGN.  Arguments that break several rules get the code of
+ *       one of them, not a fixed one.
+ *   mm_catalog_softmax_ce_workspace_bytes  the workspace those shapes need (0: no split); depends on the device's SM count.
+ * ------------------------------------------------------------------------------------- */
+int64_t mm_catalog_softmax_ce_workspace_bytes(int64_t B, int64_t N, int D);
+int mm_catalog_softmax_ce_backward(const void* x_split, const void* e_split, int64_t B, int64_t N, int D, const float* bias,
+                                   const void* labels, int label_dtype, float temperature, const float* stats,
+                                   const float* row_scale, int row_scale_is_scalar, float* dx, float* de, float* db, float* loss,
+                                   int* oob_count, void* workspace, int64_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

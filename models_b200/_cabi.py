@@ -218,6 +218,9 @@ SIGNATURES = {
                                    C.POINTER(C.c_float), _vp, _i64, _vp, _vp]),
     "mm_inbatch_softmax_ce_backward": (_i, [_vp, _vp, _i64, _i64, _i, _vp, _vp, _i, _i, _f, _vp, _f, _vp, _vp, _vp, _vp, _i,
                                             _vp, _vp, _vp, _vp, _vp]),
+    "mm_catalog_softmax_ce_workspace_bytes": (_i64, [_i64, _i64, _i]),
+    "mm_catalog_softmax_ce_backward": (_i, [_vp, _vp, _i64, _i64, _i, _vp, _vp, _i, _f, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp,
+                                            _i64, _vp]),
     "mm_l2_normalize_backward": (_i, [_vp, _vp, _i64, _i, _i64, _i64, _vp, _i64, _vp]),
     "mm_deepfm_head_fwd_bwd": (_i, [_vp, _i64, C.POINTER(C.c_int64), _i, C.POINTER(WideBlock), _i, C.POINTER(ConcatPiece),
                                     C.POINTER(C.c_int64), _i, _vp, _vp, _vp, _i64, _i, _i, _vp, _vp, _i, _vp, _vp, _i, _vp, _i, _vp,

@@ -16,7 +16,12 @@
 //   Pairwise<KIND>  BPR, BPR-max, TOP1, TOP1-v2, TOP1-max, logistic, hinge (the reference's losses/pairwise.py; element
 //                   functions in pairwise.cuh): G = c / T dloss/ds with c = 1 / (B N) (Keras' SUM_OVER_BATCH_SIZE over
 //                   the (B, N) per-element losses; top1_v2's per-row mean over N and batch mean over B give the same c)
-// and inbatch_loss_kernel adds either loss from the per-row statistics in a fixed order (one CTA).
+//   CatalogCE       backward of the full-catalog soft-max cross-entropy (CategoricalOutput over a weight-tied table): the
+//                   queries are x / T, the streamed "negatives" are the catalog rows, the tempered bias b / T is a column
+//                   value and the one-hot compares the column index with the row's label in registers.  DQ: G = c / T
+//                   (softmax - onehot), dX = G E; DN: G = c (softmax - onehot), dE = G^T (x / T), db = 1 / T sum_b G.
+//                   DQ may split the catalog over gridDim.y CTAs per query tile (partial dX, summed in a fixed order)
+// and inbatch_loss_kernel adds any of the losses from the per-row statistics in a fixed order (one CTA).
 //
 // Two warpgroups (64 resident rows each) over a TMA ring of streamed tiles: the forward catalog kernel's structure
 // (catalog_tc.cu) without its producer warp.  The scores use the forward's 3-pass split-bf16 products.  The second product
@@ -60,7 +65,18 @@ struct Params {
   const float* pos;        // (B, D) fp32
   float* out;              // dq (B, D) or dneg (N, D)
   float* dpos;             // dq kernel: dpos when it is its own buffer; dn kernel: non-null = dpos aliases dneg (add g0 q)
+  // catalog soft-max only (null / unused for the other losses)
+  const void* labels;   // (B,) class ids, id_is64 wide
+  const float* bias;    // (N,) the tempered bias b / T, or null
+  float* db;            // dn kernel: (N,) bias gradient, or null
+  int tiles_per_split;  // dq kernel: streamed tiles per CTA of a query tile (gridDim.y CTAs share one)
+  int* oob;             // dq kernel: labels outside [0, N) are counted here (null: not counted)
 };
+
+// The catalog kernels stream up to N / 128 tiles into one wgmma fp32 accumulator, which loses magnitude over millions of
+// additions (dx of a 10 M catalog in 4 splits came out 0.2 % small).  Every kFlushTiles tiles a CTA adds its accumulator
+// into its own output rows (read, add, write: each row has one owner) and restarts it from zero.
+constexpr int kFlushTiles = 256;
 
 __device__ __forceinline__ long long id_at(const void* p, long long i, int is64) {
   return is64 ? reinterpret_cast<const long long*>(p)[i] : (long long)reinterpret_cast<const int*>(p)[i];
@@ -73,6 +89,7 @@ __device__ __forceinline__ long long id_at(const void* p, long long i, int is64)
 
 struct SoftmaxCE {
   static constexpr bool kTwoPass = false;
+  static constexpr bool kCatalog = false;
   __device__ __forceinline__ static float logq_bias(const float* prob, long long n) {  // the forward's -log(p + 1e-16)
     return prob ? -logf(prob[n] + 1e-16f) : 0.0f;
   }
@@ -125,6 +142,7 @@ template <int KIND>
 struct Pairwise {
   static constexpr int kKind = KIND;
   static constexpr bool kTwoPass = pw::is_max<KIND>::value;  // the forward's lse pass
+  static constexpr bool kCatalog = false;
   template <int MODE>
   static constexpr int cols() {
     return MODE == DN ? 3 : 0;
@@ -159,6 +177,61 @@ struct Pairwise {
     return p.c * p.inv_temp * g;
   }
   __device__ __forceinline__ static float g0(const Params& p, long long b) { return p.c * p.inv_temp * p.stats[b * 4 + 1]; }
+};
+
+// Integer values (a label, a row or column index) travel through the float row / column slots bit for bit.  A label
+// outside [0, N) becomes -1, which matches no column: its row keeps the soft-max term and loses the one-hot.
+struct CatalogCE {
+  static constexpr bool kTwoPass = false;
+  static constexpr bool kCatalog = true;
+  __device__ __forceinline__ static float label_of(const Params& p, long long b, long long n_classes) {
+    const long long y = id_at(p.labels, b, p.id_is64);
+    return __int_as_float(y >= 0 && y < n_classes ? (int)y : -1);
+  }
+  __device__ __forceinline__ static float bias_of(const Params& p, long long n) { return p.bias ? p.bias[n] : 0.0f; }
+  template <int MODE>
+  static constexpr int cols() {
+    return MODE == DN ? 3 : 2;
+  }
+  // DQ: the query's [lse, c/T, label]; DN: the catalog row's [b/T, its index]
+  template <int MODE>
+  __device__ __forceinline__ static void row_vals(const Params& p, long long r, float (&v)[3]) {
+    if (MODE == DN) {
+      v[0] = bias_of(p, r);
+      v[1] = __int_as_float((int)r);
+    } else {
+      v[0] = p.stats[r * 3 + 1];
+      v[1] = (p.scale_is_scalar ? p.row_scale[0] : p.row_scale[r]) * p.inv_temp;
+      v[2] = label_of(p, r, p.I);
+    }
+  }
+  // DQ: the catalog row's [b/T, its index]; DN: the query's [lse, c, label]
+  template <int MODE>
+  __device__ __forceinline__ static void col_vals(const Params& p, long long c, float (&v)[3]) {
+    if (MODE == DN) {
+      v[0] = p.stats[c * 3 + 1];
+      v[1] = p.scale_is_scalar ? p.row_scale[0] : p.row_scale[c];
+      v[2] = label_of(p, c, p.M);
+    } else {
+      v[0] = bias_of(p, c);
+      v[1] = __int_as_float((int)c);
+    }
+  }
+  // the forward's logit: (x / T) . e + b / T, the same fp32 add mm_catalog_score does
+  template <int MODE>
+  __device__ __forceinline__ static float score(const Params&, float a, const float (&r)[3], const float* c) {
+    return a + (MODE == DN ? r[0] : c[0]);
+  }
+  // DQ: c/T (softmax - onehot); DN: c (softmax - onehot)
+  template <int MODE>
+  __device__ __forceinline__ static float grad(const Params&, float s, const float (&r)[3], const float* c) {
+    const float lse = MODE == DN ? c[0] : r[0];
+    const float sc = MODE == DN ? c[kColStride] : r[1];
+    const bool hit = MODE == DN ? __float_as_int(c[2 * kColStride]) == __float_as_int(r[1])
+                                : __float_as_int(r[2]) == __float_as_int(c[kColStride]);
+    return sc * (ex2_approx((s - lse) * LOG2E) - (hit ? 1.0f : 0.0f));
+  }
+  __device__ __forceinline__ static float g0(const Params&, long long) { return 0.0f; }
 };
 
 // wgmma with the A operand from registers and an MN-major (transposed) B operand: D[64 x n] += A[64 x 16] . B[16 x n]
@@ -235,13 +308,15 @@ inbatch_flash_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long long m0 = (long long)blockIdx.x * BM;
-  const int total = PASSES * p.n_tiles;
+  // the catalog loss's dq kernel streams only its split's tiles t_base .. t_base + total - 1
+  const int t_base = Loss::kCatalog ? (int)blockIdx.y * p.tiles_per_split : 0;
+  const int total = Loss::kCatalog ? min(p.n_tiles - t_base, p.tiles_per_split) : PASSES * p.n_tiles;
   // Thread 0 issues every TMA load.  The two warpgroups meet at a named barrier at the start of each tile; by then both
   // have waited for their MMAs of the previous tile, so its stage is free and is refilled right there.  No producer warp:
   // a ninth warp would share a register sub-partition with two consumer warps and cap every thread at 168 registers.
   auto load_tile = [&](int t) {
     const int stage = t % p.stages;
-    const int tile = PASSES == 1 ? t : t % p.n_tiles;
+    const int tile = t_base + (PASSES == 1 ? t : t % p.n_tiles);
     const uint32_t fb = smem_u32(full_bar + stage);
     uint8_t* st = smem_b + (size_t)stage * STAGE_BYTES;
     mbar_expect_tx(fb, STAGE_BYTES);
@@ -284,23 +359,30 @@ inbatch_flash_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
     if (rvalid[h]) {
       Loss::template row_vals<MODE>(p, row[h], rv[h]);
       if (do_mask) my_id[h] = id_at(p.row_ids, row[h], p.id_is64);
+      if constexpr (Loss::kCatalog && MODE == DQ) {  // one count per row: the quad's lane 0 of the first split
+        if (p.oob && part == 0 && blockIdx.y == 0 && __float_as_int(rv[h][2]) < 0) atomicAdd(p.oob, 1);
+      }
     }
   }
   // forward: per row, this thread's partials over the columns it sees (the four lanes of a quad share a row)
   pw::RowAcc racc[2];
   float run_m[2] = {-INFINITY, -INFINITY}, run_s[2] = {0.0f, 0.0f};
   float dacc[64];
+  float dbacc[2] = {0.0f, 0.0f};  // catalog dn kernel: this thread's part of the row's bias gradient sum_b G
   if (MODE != FWD) {
 #pragma unroll
     for (int i = 0; i < 64; ++i) dacc[i] = 0.0f;
   }
+  // the catalog dq kernel writes its split's partial dX (gridDim.y > 1) or dX itself
+  float* out = p.out;
+  if constexpr (Loss::kCatalog) out += (long long)blockIdx.y * p.M * p.D;
   int stage = 0, buf = 0;
   uint32_t phase = 0;
   mbar_wait(smem_u32(a_full), 0);
   const uint32_t a_base = smem_u32(smem_a) + (uint32_t)wg * (TILE_BYTES / 2);
   for (int t = 0; t < total; ++t) {
     const int pass = PASSES == 1 ? 0 : t / p.n_tiles;
-    const long long n0 = (long long)(t - pass * p.n_tiles) * BN;
+    const long long n0 = (long long)(t_base + t - pass * p.n_tiles) * BN;
     float* cv = col_v + buf * BN;
     int* cl = ids_lo + buf * BN;
     int* chh = ids_hi + buf * BN;
@@ -417,6 +499,7 @@ inbatch_flash_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
               const float s = Loss::template score<MODE>(p, acc[i], rv[h], cv + c);
               const float g = Loss::template grad<MODE>(p, s, rv[h], cv + c);
               acc[i] = ok ? g : 0.0f;
+              if constexpr (Loss::kCatalog && MODE == DN) dbacc[h] += acc[i];
             }
           }
         }
@@ -472,6 +555,25 @@ inbatch_flash_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
       wgmma_commit();
       wgmma_wait_all();
       wgmma_fence_acc(dacc);
+      if constexpr (Loss::kCatalog) {
+        if ((t + 1) % kFlushTiles == 0 && t + 1 < total) {
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+#pragma unroll
+            for (int j = 0; j < KP / 8; ++j) {
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const int c = 8 * j + 2 * part + e;
+                if (rvalid[h] && c < p.D) {
+                  const long long o = row[h] * p.D + c;
+                  out[o] = t + 1 > kFlushTiles ? out[o] + dacc[4 * j + 2 * h + e] : dacc[4 * j + 2 * h + e];
+                }
+                dacc[4 * j + 2 * h + e] = 0.0f;
+              }
+            }
+          }
+        }
+      }
     }
     if (++stage == p.stages) {
       stage = 0;
@@ -501,13 +603,25 @@ inbatch_flash_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
       }
     }
   } else {
+    if constexpr (Loss::kCatalog && MODE == DN) {
+      // ---- the row's bias gradient: the quad's four partials summed in the same order in every lane ----
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int o = 1; o < 4; o <<= 1) {
+          const float ov = __shfl_xor_sync(0xffffffffu, dbacc[h], o);
+          dbacc[h] = (o & lane) ? ov + dbacc[h] : dbacc[h] + ov;
+        }
+        if (p.db && rvalid[h] && part == 0) p.db[row[h]] = dbacc[h] * p.inv_temp;
+      }
+    }
     // ---- epilogue: dacc[4 j + 2 h + e] is output row h, feature column 8 j + 2 part + e ----
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       if (!rvalid[h]) continue;
       const long long r = row[h];
       // dQ: + g0[b] pos[b] (and dpos = g0[b] q[b] in its own buffer); dN with dpos aliasing dneg: + g0[n] q[n]
-      const bool add = TRANS ? p.dpos != nullptr : true;
+      const bool add = Loss::kCatalog ? false : TRANS ? p.dpos != nullptr : true;
       const float g0 = add ? Loss::g0(p, r) : 0.0f;
       const float* addend = TRANS ? p.q : p.pos;
 #pragma unroll
@@ -519,7 +633,8 @@ inbatch_flash_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
             const long long o = r * p.D + c;
             float v = dacc[4 * j + 2 * h + e];
             if (add) v = fmaf(g0, addend[o], v);
-            p.out[o] = v;
+            if (Loss::kCatalog && total > kFlushTiles) v = out[o] + v;  // after the flushed chunks
+            out[o] = v;
             if (!TRANS && p.dpos) p.dpos[o] = g0 * p.q[o];
           }
         }
@@ -549,11 +664,34 @@ __global__ void inbatch_loss_kernel(long long B, const float* __restrict__ stats
   if (threadIdx.x == 0) loss[0] += (float)(factor * part[0]);
 }
 
+// out[i] = sum_s part[s n + i] over the S partial dX of the catalog dq kernel's splits, in split order
+__global__ void split_sum_kernel(long long n, int S, const float* __restrict__ part, float* __restrict__ out) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    float s = part[i];
+    for (int k = 1; k < S; ++k) s += part[(long long)k * n + i];
+    out[i] = s;
+  }
+}
+
+// The catalog dq kernel's splits per query tile: one query tile per CTA leaves SMs idle while ceil(B / 128) is below the
+// SM count (B = 4096 is 32 CTAs), so each query tile's catalog is split over floor(SMs / query tiles) CTAs (one CTA
+// fits per SM: one wave), at most one per catalog tile and with no empty split.  The workspace is S B D floats with
+// S B <= 128 SMs whatever the catalog size.
+static int catalog_splits(long long B, long long N) {
+  const long long m_blocks = (B + BM - 1) / BM, n_tiles = (N + BN - 1) / BN;
+  long long S = sm_count() / m_blocks;
+  if (S > n_tiles) S = n_tiles;
+  if (S < 1) S = 1;
+  const long long per = (n_tiles + S - 1) / S;
+  return (int)((n_tiles + per - 1) / per);
+}
+
 typedef void (*Kernel)(const CUtensorMap, const CUtensorMap, const Params);
 
-// one CTA per 128 of the p.M resident rows, streaming the p.I others through as many stages as fit (at most 4)
+// one CTA per 128 of the p.M resident rows (times `splits` for the catalog dq kernel), streaming the p.I others through
+// as many stages as fit (at most 4)
 static int launch(const char* who, Kernel kern, int Kp, const CUtensorMap& tmA, const CUtensorMap& tmB, Params p,
-                  cudaStream_t st) {
+                  cudaStream_t st, int splits = 1) {
   const size_t tile_bytes = 2ull * (Kp / BLOCK_K) * TILE_BYTES;  // the resident tile and one stage are the same size
   const size_t extra = (kColVals + 2) * 2 * BN * sizeof(float);  // per-tile column data: the values and two id words
   const size_t fixed = 1024 + tile_bytes + 8 * sizeof(uint64_t) + extra;
@@ -562,13 +700,14 @@ static int launch(const char* who, Kernel kern, int Kp, const CUtensorMap& tmA, 
   MM_REQUIRE(stages >= 2, MM_ERR_UNSUPPORTED, "%s: tiles do not fit two pipeline stages", who);
   p.stages = stages;
   p.n_tiles = (int)((p.I + BN - 1) / BN);
+  p.tiles_per_split = (p.n_tiles + splits - 1) / splits;
   const size_t smem = 1024 + tile_bytes + stages * tile_bytes + (stages + 2) * sizeof(uint64_t) + extra;
   cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (e != cudaSuccess) {
     mm::set_error("%s: cudaFuncSetAttribute failed: %s", who, cudaGetErrorString(e));
     return (int)e;
   }
-  kern<<<(unsigned)((p.M + BM - 1) / BM), kThreads, smem, st>>>(tmA, tmB, p);
+  kern<<<dim3((unsigned)((p.M + BM - 1) / BM), (unsigned)splits), kThreads, smem, st>>>(tmA, tmB, p);
   return mm::check_launch(who);
 }
 
@@ -666,6 +805,10 @@ template <int MODE>
 static Kernel pick_ce(int Kp) {
   return Kp == 64 ? inbatch_flash_kernel<SoftmaxCE, MODE, 64> : inbatch_flash_kernel<SoftmaxCE, MODE, 128>;
 }
+template <int MODE>
+static Kernel pick_catalog(int Kp) {
+  return Kp == 64 ? inbatch_flash_kernel<CatalogCE, MODE, 64> : inbatch_flash_kernel<CatalogCE, MODE, 128>;
+}
 
 }  // namespace flash
 }  // namespace mm
@@ -749,6 +892,70 @@ int mm_inbatch_pairwise_bwd(const void* q_split, const void* neg_split, int64_t 
   p.pos = pos;
   return launch_bwd(who, pick_pairwise<DQ>(Kp, kind), pick_pairwise<DN>(Kp, kind), Kp, tmQ, tmN, p, dq, dpos, dneg,
                     (cudaStream_t)stream);
+}
+
+int64_t mm_catalog_softmax_ce_workspace_bytes(int64_t B, int64_t N, int D) {
+  if (B <= 0 || N <= 0 || D <= 0) return 0;
+  const int S = mm::flash::catalog_splits(B, N);
+  return S > 1 ? (int64_t)S * B * D * (int64_t)sizeof(float) : 0;
+}
+
+int mm_catalog_softmax_ce_backward(const void* x_split, const void* e_split, int64_t B, int64_t N, int D, const float* bias,
+                                   const void* labels, int label_dtype, float temperature, const float* stats,
+                                   const float* row_scale, int row_scale_is_scalar, float* dx, float* de, float* db, float* loss,
+                                   int* oob_count, void* workspace, int64_t workspace_bytes, void* stream) {
+  const char* who = "mm_catalog_softmax_ce_backward";
+  using namespace mm::flash;
+  MM_REQUIRE(labels && stats && row_scale && dx && de, MM_ERR_ARG,
+             "%s: null pointer (labels, stats, row_scale, dx and de are required)", who);
+  MM_REQUIRE(((uintptr_t)stats | (uintptr_t)row_scale | (uintptr_t)dx | (uintptr_t)de | (uintptr_t)(bias ? bias : stats) |
+              (uintptr_t)(db ? db : stats) | (uintptr_t)(loss ? loss : stats)) % 4 == 0,
+             MM_ERR_ALIGN, "%s: fp32 buffers must be 4-B aligned", who);
+  MM_REQUIRE(((uintptr_t)workspace % 16) == 0 && ((uintptr_t)oob_count % 4) == 0, MM_ERR_ALIGN,
+             "%s: workspace must be 16-B and oob_count 4-B aligned", who);
+  int Kp = 0;
+  CUtensorMap tmX, tmE;
+  Params p{};
+  int rc = prepare(who, x_split, e_split, B, N, D, nullptr, nullptr, label_dtype, 0, temperature, dx, nullptr, de, &Kp, &tmX, &tmE,
+                   &p);
+  if (rc) return rc;
+  const int64_t need = mm_catalog_softmax_ce_workspace_bytes(B, N, D);
+  MM_REQUIRE(workspace_bytes >= need && (need == 0 || workspace), MM_ERR_ARG, "%s: workspace too small (%lld < %lld)", who,
+             (long long)workspace_bytes, (long long)need);
+  if (B == 0) return MM_OK;
+  p.labels = labels;
+  p.bias = bias;
+  p.stats = const_cast<float*>(stats);
+  p.row_scale = row_scale;
+  p.scale_is_scalar = row_scale_is_scalar != 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  Params pq = p;
+  pq.oob = oob_count;
+  // dX: one CTA per (query tile, catalog split); the splits' partials are summed in split order
+  const int S = catalog_splits(B, N);
+  pq.out = S > 1 ? (float*)workspace : dx;
+  rc = launch(who, pick_catalog<DQ>(Kp), Kp, tmX, tmE, pq, st, S);
+  if (rc) return rc;
+  if (S > 1) {
+    const long long n = B * (long long)D;
+    long long blocks = (n + 255) / 256;
+    const long long cap = (long long)mm::sm_count() * 8;
+    split_sum_kernel<<<(unsigned)(blocks < cap ? blocks : cap), 256, 0, st>>>(n, S, (const float*)workspace, dx);
+    rc = mm::check_launch(who);
+    if (rc) return rc;
+  }
+  // dE and db: one CTA per 128 catalog rows streaming the queries
+  Params pn = p;
+  pn.M = N;
+  pn.I = B;
+  pn.out = de;
+  pn.db = db;
+  rc = launch(who, pick_catalog<DN>(Kp), Kp, tmE, tmX, pn, st);
+  if (rc == MM_OK && loss) {
+    inbatch_loss_kernel<<<1, 1024, 0, st>>>(B, stats, 3, 1, 2, row_scale, row_scale_is_scalar != 0, 1.0, loss);
+    rc = mm::check_launch(who);
+  }
+  return rc;
 }
 
 }  // extern "C"

@@ -480,6 +480,55 @@ def inbatch_softmax_ce_backward(q_split, neg_split, D: int, stats, q, pos, row_s
         "mm_inbatch_softmax_ce_backward")
 
 
+def catalog_softmax_ce_workspace_bytes(B: int, N: int, D: int) -> int:
+    """Bytes of the partial-dX workspace catalog_softmax_ce_backward needs for these shapes (0: the catalog is not split)."""
+    return int(_lib().mm_catalog_softmax_ce_workspace_bytes(int(B), int(N), int(D)))
+
+
+def catalog_softmax_ce_backward(x_split, e_split, D: int, stats, labels, row_scale, dx, de, db=None, bias=None, loss=None,
+                                temperature: float = 1.0, workspace=None, oob=None) -> None:
+    """Backward of the full-catalog soft-max cross-entropy (mm_catalog_softmax_ce_backward) from the operands
+    catalog_score read for `stats` (B, 3): x_split = split_rows(x / T) (B, 2*Kp), e_split = split_rows(E) (N, 2*Kp) and
+    bias (N,) = b / T (None: no bias).  With G = c (softmax - onehot(labels)) of the logits (x E^T + b) / T, writes dx
+    (B, D) = G E / T, the gradient of x itself; de (N, D) = G^T x / T; db (N,) = sum_b G / T (None: not written); and
+    adds sum_b c[b] (lse[b] - logit[b, label]) to `loss` (nullable).  labels (B,) int32 / int64 class ids; a label
+    outside [0, N) is never used as an address: it takes no one-hot term (its loss term is NaN) and adds one to `oob`
+    (nullable int32 counter, the gathers' out-of-range counter).  row_scale: (B,) or (1,) fp32 c.  workspace: uint8 of at
+    least catalog_softmax_ce_workspace_bytes(B, N, D) bytes; None allocates one (not during graph capture)."""
+    B, N = _inbatch_buffers(D, x_split, e_split, stats, 3, extra=(("row_scale", row_scale),), joint=True)
+    for n_, t_, shape in (("dx", dx, (B, D)), ("de", de, (N, D))):
+        if tuple(_dev(t_, n_, torch.float32).shape) != shape or not t_.is_contiguous():
+            raise ValueError(f"{n_} must be contiguous {shape}, got {tuple(t_.shape)}")
+    if dx.data_ptr() == de.data_ptr():
+        raise ValueError("dx and de must be distinct buffers")
+    _vec(db, N, "db")
+    _vec(bias, N, "bias")
+    if loss is not None and _dev(loss, "loss", torch.float32).numel() < 1:
+        raise ValueError("loss must hold at least one value")
+    if row_scale.numel() not in (1, B):
+        raise ValueError(f"row_scale must hold 1 or {B} values, got {row_scale.numel()}")
+    if not float(temperature) > 0.0:
+        raise ValueError(f"temperature must be positive, got {temperature}")
+    labels = _dev(labels, "labels").reshape(-1)
+    if labels.numel() != B or not labels.is_contiguous():
+        raise ValueError(f"labels must hold {B} contiguous class ids, got {tuple(labels.shape)}")
+    label_dt = _idx_dtype(labels, "labels")
+    if oob is not None and (_dev(oob, "oob", torch.int32).numel() < 1):
+        raise ValueError("oob must hold at least one int32 counter")
+    need = catalog_softmax_ce_workspace_bytes(B, N, D)
+    if workspace is None:
+        workspace = torch.empty(max(need, 16), dtype=torch.uint8, device=x_split.device)
+    elif _dev(workspace, "workspace", torch.uint8).numel() < need:
+        raise ValueError(f"workspace must hold at least {need} bytes, got {workspace.numel()}")
+    scalar = row_scale.numel() == 1 and B != 1
+    _cabi.check(
+        _lib().mm_catalog_softmax_ce_backward(x_split.data_ptr(), e_split.data_ptr(), B, N, int(D), _ptr(bias), labels.data_ptr(),
+                                              label_dt, float(temperature), stats.data_ptr(), row_scale.data_ptr(), int(scalar),
+                                              dx.data_ptr(), de.data_ptr(), _ptr(db), _ptr(loss), _ptr(oob), workspace.data_ptr(),
+                                              workspace.numel(), _stream()),
+        "mm_catalog_softmax_ce_backward")
+
+
 def _inbatch_buffers(D: int, q_split, neg_split, stats, stats_cols: int, grads=None, extra=(), joint=True) -> tuple:
     """The buffers every in-batch kernel reads: the split operands q_split (B, 2*Kp) and neg_split (N, 2*Kp), bf16, and
     the fp32 stats (B, stats_cols); with grads = (q, pos, dq, dpos, dneg), a backward's fp32 q, pos, dq, dpos (B, D) and
