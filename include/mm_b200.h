@@ -908,6 +908,23 @@ int mm_catalog_softmax_ce_backward(const void* x_split, const void* e_split, int
                                    const float* row_scale, int row_scale_is_scalar, float* dx, float* de, float* db, float* loss,
                                    int* oob_count, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * K23  IndexedSlices into a dense gradient (the weight-tied catalog step: the tied table's input-side rows added to the
+ * output side's dE).  Added with the catalog training step; no existing entry point changed.
+ *   mm_slices_add_dense  dense[ids[i]] += rows[i] for i in [0, n): ids (n,) MM_I32 / MM_I64, rows (n, D) fp32 contiguous,
+ *       dense (N, D) fp32 contiguous.  An id outside [0, N) (a multi-hot expansion's -1, an out-of-range id the gathers
+ *       counted) adds nothing.  Duplicate ids are summed in index order and each dense row has one writer: a stable radix
+ *       sort of the ids (8-bit digits, ceil(log2(N + 1) / 8) passes), then each run of equal ids summed in 256-position
+ *       pieces whose partials are added in piece order (a run of length r costs one group at most 256 + r / 256 row
+ *       additions); no float atomics, so repeats are bit-identical.  4 <= D <= 128, D % 4 == 0; n, N < 2^31.  workspace: at least
+ *       mm_slices_add_dense_workspace_bytes(n) bytes, 16-B aligned.  Errors before any launch: MM_ERR_ARG, MM_ERR_UNSUPPORTED,
+ *       MM_ERR_ALIGN.
+ *   mm_slices_add_dense_workspace_bytes  the workspace of n slices (0 for n <= 0).
+ * ------------------------------------------------------------------------------------- */
+int64_t mm_slices_add_dense_workspace_bytes(int64_t n);
+int mm_slices_add_dense(const void* ids, int idx_dtype, const float* rows, int64_t n, int D, float* dense, int64_t N,
+                        void* workspace, int64_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -20,7 +20,7 @@ from .experts import CGCBlock, MMOEBlock, PLEBlock  # noqa: F401
 from .retrieval import (CategoricalOutput, ContrastiveOutput, Encoder, InBatchSampler, InBatchSamplerV2,  # noqa: F401
                         ItemRetrievalScorer, ItemRetrievalTask, L2Norm, PopularityBasedSamplerV2,
                         QueryItemIdsEmbeddingsBlock, TwoTowerBlock, log_uniform_sampling_probs)
-from .models import (BinaryClassificationTask, BinaryOutput, DCNModel, DeepFMModel, DLRMModel, Model, OutputBlock,  # noqa: F401
+from .models import (BinaryClassificationTask, BinaryOutput, CatalogModel, DCNModel, DeepFMModel, DLRMModel, Model, OutputBlock,  # noqa: F401
                      ParallelOutputs, RegressionOutput, WideAndDeepModel,
                      MatrixFactorizationModel, RetrievalModel, RetrievalModelV2, TwoTowerModel, TwoTowerModelV2)
 from .topk import (AvgPrecisionAt, BruteForce, MRRAt, NDCGAt, PrecisionAt, RecallAt, TopKEncoder,  # noqa: F401

@@ -221,6 +221,8 @@ SIGNATURES = {
     "mm_catalog_softmax_ce_workspace_bytes": (_i64, [_i64, _i64, _i]),
     "mm_catalog_softmax_ce_backward": (_i, [_vp, _vp, _i64, _i64, _i, _vp, _vp, _i, _f, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp,
                                             _i64, _vp]),
+    "mm_slices_add_dense_workspace_bytes": (_i64, [_i64]),
+    "mm_slices_add_dense": (_i, [_vp, _i, _vp, _i64, _i, _vp, _i64, _vp, _i64, _vp]),
     "mm_l2_normalize_backward": (_i, [_vp, _vp, _i64, _i, _i64, _i64, _vp, _i64, _vp]),
     "mm_deepfm_head_fwd_bwd": (_i, [_vp, _i64, C.POINTER(C.c_int64), _i, C.POINTER(WideBlock), _i, C.POINTER(ConcatPiece),
                                     C.POINTER(C.c_int64), _i, _vp, _vp, _vp, _i64, _i, _i, _vp, _vp, _i, _vp, _vp, _i, _vp, _i, _vp,

@@ -327,10 +327,14 @@ def _sequential_model(*blocks) -> "RankingModel":
     from .blocks import MLP
     from .experts import MMOEBlock
 
+    from .retrieval import CategoricalOutput
+
     ib, mid, out = blocks[0], list(blocks[1:-1]), blocks[-1]
     order = "Model(*blocks) takes InputBlockV2, then optionally one MLPBlock, then optionally one MMOEBlock, then the output"
     if ib.aggregation != "concat":
         raise NotImplementedError("Model(*blocks): the input block must concatenate its features (aggregation='concat')")
+    if isinstance(out, CategoricalOutput):
+        return _catalog_model(ib, mid, out)
     if not isinstance(out, (BinaryOutput, ParallelOutputs)):
         raise NotImplementedError(f"{order} (BinaryOutput, RegressionOutput or OutputBlock(schema)); got {type(out).__name__} last")
     bottom = mmoe = None
@@ -346,6 +350,24 @@ def _sequential_model(*blocks) -> "RankingModel":
     if mmoe is not None:
         mmoe.bind(out.names if isinstance(out, ParallelOutputs) else [out.name])
     return RankingModel(MMoEBody(ib, bottom, mmoe), out, ib.schema)
+
+
+def _catalog_model(ib: InputBlockV2, mid: list, out) -> "CatalogModel":
+    """Model(InputBlockV2, MLPBlock, CategoricalOutput(to_call=EmbeddingTable)): the weight-tied next-item classifier
+    (outputs/classification.py:127-216, :311-382).  The MLP's last width must be the table's width."""
+    from .experts import MMOEBlock
+
+    if any(isinstance(b, MMOEBlock) for b in mid) or getattr(out, "task_blocks", None):
+        raise NotImplementedError("Model(*blocks): an MMOEBlock or task towers before a CategoricalOutput are not implemented")
+    if len(mid) != 1 or not isinstance(mid[0], MLP):
+        raise NotImplementedError("Model(*blocks) with a CategoricalOutput takes InputBlockV2, exactly one MLPBlock and the output; "
+                                  f"got {[type(b).__name__ for b in [ib] + mid + [out]]}")
+    mlp = mid[0]
+    last, D = mlp.dense_layers[-1].units, out.table.dim
+    if last != D:
+        raise ValueError(f"the MLPBlock ends in {last} units but the CategoricalOutput's table {out.table.table_name!r} is "
+                         f"{D} wide: the query must have the table's width")
+    return CatalogModel(MMoEBody(ib, mlp, None), out, ib.schema)
 
 
 class _ModelMeta(type):
@@ -940,6 +962,141 @@ class RankingModel(Model):
             return chain(x, layers)
         x = self.body(inputs, training=training)
         return self.prediction(x, logits=True) if logits else self.prediction(x)
+
+
+class CatalogModel(Model):
+    """Model(InputBlockV2, MLPBlock, CategoricalOutput(to_call=EmbeddingTable)): the reference's weight-tied next-item
+    classifier.  The input block and the MLP make the query x (B, D); the output scores it against the item table E
+    (N_I, D) that an input feature may also read.  Calling the model returns CategoricalOutput's (B, N_I) logits without
+    the temperature; `top_k` streams the table without them.  `compile` / `fit` / `train_step` train it with
+    CategoricalCrossentropy(from_logits=True) on the tempered logits (train.CatalogTrainer); `evaluate` reports that loss
+    and top-k metrics of the label among the whole table (default_categorical_prediction_metrics(k=10))."""
+
+    _TRANSIENT = {"_pinned": {}, "_trainer": None}
+
+    @property
+    def mlp(self) -> MLP:
+        return self.body.bottom
+
+    def build(self, device=None):
+        self.body.build(device)
+        self.prediction.build(device)
+        self.built = True
+        return self
+
+    def query(self, inputs: TabularData) -> torch.Tensor:
+        """(B, D): the MLP's output, what the output layer scores against the table."""
+        self._check_inputs(inputs)
+        if not self.built:
+            self.build(next(iter(inputs.values())).device)
+        return run_dense_chain(self.body.input_block(inputs), self.mlp.dense_layers)
+
+    def call(self, inputs: TabularData, targets=None, training: bool = False, testing: bool = False, **kwargs):
+        return self.prediction(self.query(inputs))
+
+    def top_k(self, inputs: TabularData, k: int):
+        """(scores, ids) (B, k) of the whole table, in tf.math.top_k order."""
+        return self.prediction.top_k(self.query(inputs), k)
+
+    def _compile_training(self, optimizer, loss=None, loss_weights=None, metrics=None, weighted_metrics=None) -> None:
+        from .topk import TopKMetric, _FUSED_MAX_K
+
+        if loss not in (None, "categorical_crossentropy", "CategoricalCrossentropy"):
+            raise NotImplementedError(f"loss {loss!r}: a CategoricalOutput trains with its default, categorical_crossentropy")
+        if loss_weights is not None or weighted_metrics:
+            raise NotImplementedError("loss_weights / weighted_metrics: a CategoricalOutput model has one output and unweighted "
+                                      "top-k metrics")
+        metrics = list(metrics) if metrics else default_categorical_metrics()
+        for m in metrics:
+            if not isinstance(m, TopKMetric):
+                raise NotImplementedError(f"metric {m!r}: a CategoricalOutput model evaluates top-k metrics (RecallAt, MRRAt, "
+                                          "NDCGAt, AvgPrecisionAt, PrecisionAt)")
+            if not 1 <= m.k <= _FUSED_MAX_K:
+                raise ValueError(f"{m.label}: k must be in [1, {_FUSED_MAX_K}] (the fused top-k's limit)")
+        super()._compile_training(optimizer, None, None)
+        self.topk_metrics = metrics
+
+    @property
+    def metrics_names(self) -> List[str]:
+        return ["loss"] + [m.label for m in self._compiled_topk()]
+
+    def _compiled_topk(self):
+        metrics = getattr(self, "topk_metrics", None)
+        if metrics is None:
+            raise RuntimeError("You must compile your model before training/testing. Use `model.compile(optimizer, loss)`.")
+        return metrics
+
+    def evaluate(self, x, y=None, batch_size: Optional[int] = None, steps: Optional[int] = None, return_dict: bool = False,
+                 verbose: int = 0, callbacks=None, **kwargs):
+        """Keras `evaluate` over an iterable of (inputs, targets[, sample_weight]) batches (targets: the class ids, or a
+        dict holding them under `target_name`): `loss` is the catalog soft-max cross-entropy of the tempered logits (as in
+        testing mode), weighted by sample_weight and averaged over the rows; each top-k metric has the label as the one
+        relevant item among the top k of the whole table.  One mm_catalog_score pass per batch gives both (no (B, N_I)
+        logits).  Returns the values in `metrics_names` order, or a dict with return_dict=True.  A label outside [0, N_I)
+        is counted on the device and raises IndexError at the end."""
+        from .topk import evaluate_topk
+
+        metrics = self._compiled_topk()
+        if y is not None:
+            raise NotImplementedError("evaluate(x, y): pass an iterable of (inputs, targets[, sample_weight]) batches")
+        if callbacks:
+            raise NotImplementedError("evaluate(callbacks=...) is not implemented")
+        out, N = self.prediction, self.prediction.num_classes
+        kmax = max(m.k for m in metrics)
+        acc = {"loss": None, "rows": 0, "bad": None}
+
+        def batches():
+            for n, batch in enumerate(x):
+                if steps is not None and n >= int(steps):
+                    return
+                if not isinstance(batch, (tuple, list)) or len(batch) < 2:
+                    raise ValueError("evaluate expects batches of (inputs, targets) or (inputs, targets, sample_weight)")
+                yield batch
+
+        def predict(batch):
+            inputs, targets = batch[0], batch[1]
+            dev = next(iter(inputs.values())).device
+            yv = torch.as_tensor(self._targets_by_output(targets)[0], device=dev).reshape(-1)
+            if yv.dtype not in (torch.int32, torch.int64):
+                raise ValueError(f"targets must be int32 / int64 class ids, got {yv.dtype}")
+            bad = ((yv < 0) | (yv >= N)).sum()
+            acc["bad"] = bad if acc["bad"] is None else acc["bad"] + bad
+            # one pass over the table: the statistics of the tempered logits and their top-k (T > 0 keeps the order)
+            xt, bt = out._tempered(self.query(inputs))
+            stats, _, ids = ops.catalog_score(xt, out._catalog_split(), N, bias=bt, targets=yv, k=kmax)
+            per = stats[:, 1] - stats[:, 2]  # an out-of-range label's target logit is NaN: counted above, raised below
+            if len(batch) > 2 and batch[2] is not None:
+                sw = batch[2][out.name] if isinstance(batch[2], dict) else batch[2]
+                per = per * torch.as_tensor(sw, device=dev, dtype=torch.float32).reshape(-1)
+            acc["loss"] = per.sum() if acc["loss"] is None else acc["loss"] + per.sum()
+            acc["rows"] += yv.numel()
+            return Prediction(None, (ids == yv.view(-1, 1).to(ids.dtype)).to(torch.float32),
+                              label_relevant_counts=torch.ones(yv.numel(), device=dev))
+
+        res = evaluate_topk(predict, batches(), metrics)
+        bad = int(acc["bad"].item())
+        if bad:
+            raise IndexError(f"evaluate: {bad} labels out of range for the {N} classes of {out.table.table_name!r}")
+        res = {"loss": float(acc["loss"].item()) / acc["rows"], **res}
+        return res if return_dict else [res[k] for k in self.metrics_names]
+
+    def _fit_epoch_end(self, epoch: int, history, train_metrics, fit_kwargs) -> None:
+        data = fit_kwargs.get("validation_data")
+        if data is None:
+            return
+        freq = fit_kwargs.get("validation_freq", 1)
+        due = (epoch + 1) in freq if isinstance(freq, (list, tuple, set, range)) else (epoch + 1) % int(freq) == 0
+        if due:
+            res = self.evaluate(data, steps=fit_kwargs.get("validation_steps"), return_dict=True)
+            for k, v in res.items():
+                history.setdefault(f"val_{k}", []).append(v)
+
+
+def default_categorical_metrics(k: int = 10) -> list:
+    """metrics/topk.py default_categorical_prediction_metrics(k=10): RecallAt, MRRAt, NDCGAt, AvgPrecisionAt, PrecisionAt."""
+    from .topk import AvgPrecisionAt, MRRAt, NDCGAt, PrecisionAt, RecallAt
+
+    return [RecallAt(k), MRRAt(k), NDCGAt(k), AvgPrecisionAt(k), PrecisionAt(k)]
 
 
 class MMoEBody(Block):

@@ -529,6 +529,55 @@ def catalog_softmax_ce_backward(x_split, e_split, D: int, stats, labels, row_sca
         "mm_catalog_softmax_ce_backward")
 
 
+def catalog_stats_split(x_split, D: int, e_split, stats, labels, workspace, bias=None) -> torch.Tensor:
+    """catalog_score's soft-max statistics on operands the caller owns (mm_catalog_score with k = 0): stats (B, 3) =
+    [max, log-sum-exp, logit[label]] of x_split (B, 2*Kp) against e_split (N, 2*Kp) with bias (N,) (nullable); workspace:
+    uint8 of at least catalog_workspace_bytes(B, N) bytes.  Nothing is allocated, so a training step can be captured."""
+    _dev(x_split, "x_split", torch.bfloat16), _dev(e_split, "e_split", torch.bfloat16)
+    _dev(stats, "stats", torch.float32), _dev(workspace, "workspace", torch.uint8)
+    B, N = x_split.shape[0], e_split.shape[0]
+    if stats.numel() != 3 * B or not stats.is_contiguous():
+        raise ValueError(f"stats must be contiguous ({B}, 3)")
+    _vec(bias, N, "bias")
+    labels = _dev(labels, "labels").reshape(-1)
+    if labels.numel() != B or not labels.is_contiguous():
+        raise ValueError(f"labels must hold {B} contiguous class ids, got {tuple(labels.shape)}")
+    _cabi.check(
+        _lib().mm_catalog_score(x_split.data_ptr(), B, int(D), e_split.data_ptr(), N, _ptr(bias), labels.data_ptr(),
+                                _idx_dtype(labels, "labels"), stats.data_ptr(), 0, None, None, workspace.data_ptr(),
+                                workspace.numel(), _stream()),
+        "mm_catalog_score")
+    return stats
+
+
+def slices_add_dense_workspace_bytes(n: int) -> int:
+    """Bytes of the workspace slices_add_dense needs for n slices."""
+    return int(_lib().mm_slices_add_dense_workspace_bytes(int(n)))
+
+
+def slices_add_dense(ids, rows, dense, workspace=None) -> None:
+    """dense (N, D) += the IndexedSlices (ids (n,) int32 / int64, rows (n, D)) (mm_slices_add_dense): duplicates summed in
+    index order, one writer per row, no float atomics (bit-identical repeats); ids outside [0, N) add nothing.
+    workspace: uint8 of at least slices_add_dense_workspace_bytes(n) bytes; None allocates one (not during graph capture)."""
+    ids = _dev(ids, "ids").reshape(-1)
+    _dev(rows, "rows", torch.float32), _dev(dense, "dense", torch.float32)
+    n = ids.numel()
+    if dense.dim() != 2 or not dense.is_contiguous():
+        raise ValueError(f"dense must be a contiguous (N, D) matrix, got {tuple(dense.shape)}")
+    N, D = dense.shape
+    if tuple(rows.shape) != (n, D) or not rows.is_contiguous() or not ids.is_contiguous():
+        raise ValueError(f"rows must be contiguous ({n}, {D}) and ids hold {n} contiguous values, got {tuple(rows.shape)}")
+    need = slices_add_dense_workspace_bytes(n)
+    if workspace is None:
+        workspace = torch.empty(max(need, 16), dtype=torch.uint8, device=dense.device)
+    elif _dev(workspace, "workspace", torch.uint8).numel() < need:
+        raise ValueError(f"workspace must hold at least {need} bytes, got {workspace.numel()}")
+    _cabi.check(
+        _lib().mm_slices_add_dense(ids.data_ptr(), _idx_dtype(ids, "ids"), rows.data_ptr(), n, D, dense.data_ptr(), N,
+                                   workspace.data_ptr(), workspace.numel(), _stream()),
+        "mm_slices_add_dense")
+
+
 def _inbatch_buffers(D: int, q_split, neg_split, stats, stats_cols: int, grads=None, extra=(), joint=True) -> tuple:
     """The buffers every in-batch kernel reads: the split operands q_split (B, 2*Kp) and neg_split (N, 2*Kp), bf16, and
     the fp32 stats (B, stats_cols); with grads = (q, pos, dq, dpos, dneg), a backward's fp32 q, pos, dq, dpos (B, D) and

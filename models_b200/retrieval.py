@@ -530,15 +530,27 @@ class CategoricalOutput(Block):
                                     CategoricalCrossEntropy(from_logits=True) needs
                                     (losses/listwise.py:38-50): loss = lse - logit[target]
     top_k(x, k)                  -> (scores, ids) in tf.math.top_k order (outputs/topk.py:221-223)
-    The last two stream the catalog through one wgmma GEMM without ever writing (B, N_I)."""
+    The last two stream the catalog through one wgmma GEMM without ever writing (B, N_I).
+    `Model(InputBlockV2, MLPBlock, CategoricalOutput)` trains it (models.CatalogModel, train.CatalogTrainer) on the
+    `target_name` column."""
 
-    def __init__(self, to_call, logits_temperature: float = 1.0, use_bias: bool = True, name: Optional[str] = None, **kwargs):
+    loss = "categorical_crossentropy"
+
+    def __init__(self, to_call, logits_temperature: float = 1.0, use_bias: bool = True, name: Optional[str] = None,
+                 target_name: Optional[str] = None, **kwargs):
         from .inputs import EmbeddingTable
 
         super().__init__(name or unique_name("categorical_output"))
         if not isinstance(to_call, EmbeddingTable):
             raise NotImplementedError("CategoricalOutput(to_call=...) supports a weight-tied EmbeddingTable")
         self.table = to_call
+        # the target column: class ids in [0, N_I) (classification.py:190-196 takes the table's column by default and a
+        # `target=` keyword over it)
+        target = kwargs.pop("target", None)
+        if target is not None and target_name is not None and target != target_name:
+            raise ValueError(f"CategoricalOutput: target={target!r} and target_name={target_name!r} name different columns")
+        self.target_name = target_name or target or to_call.col_schema.name
+        self.target = self.target_name
         self.num_classes = to_call.input_dim
         self.logits_temperature = float(logits_temperature)
         self.use_bias = use_bias

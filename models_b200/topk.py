@@ -452,7 +452,8 @@ def _max_k(metrics, default: int) -> int:
 
 def evaluate_topk(predict, batches, metrics: Optional[Sequence[TopKMetric]] = None) -> Dict[str, float]:
     """Mean of every metric over all rows of all batches; `predict(device batch) -> Prediction(scores, targets)`
-    with rows already sorted by score (top-k kernels return them sorted)."""
+    with rows already sorted by score (top-k kernels return them sorted).  Dict batches are moved to the device first;
+    other batches (a model's (inputs, targets) tuples) reach `predict` as they are."""
     metrics = list(metrics) if metrics else [RecallAt(10), NDCGAt(10)]
     if isinstance(batches, dict):
         batches = [batches]
@@ -460,7 +461,7 @@ def evaluate_topk(predict, batches, metrics: Optional[Sequence[TopKMetric]] = No
     sums = {m.label: 0.0 for m in metrics}
     rows = 0
     for b in batches:
-        pred = predict(to_device(b, dev))
+        pred = predict(to_device(b, dev) if isinstance(b, dict) else b)
         rel = pred.extra.get("label_relevant_counts") if isinstance(pred, Prediction) else None
         for m in metrics:
             sums[m.label] += float(m(pred.targets, rel).sum().item())

@@ -224,7 +224,8 @@ class _StepTrainer:
     head: Optional[_Dense] = None  # the output layer; a trainer whose task builds its own targets has none
     _model_name = "this model"  # how the construction checks' messages name the model
     _onehot_only = False  # the model's input block trains one-hot features only
-    wk: Optional["_WideKernel"] = None  # a wide kernel trained outside the arena (DeepFM, Wide&Deep)
+    # a variable trained outside the arena: a wide kernel (DeepFM, Wide&Deep) or the weight-tied item table (_TiedTable)
+    wk: Optional["_WideKernel"] = None
 
     # ---- construction checks ------------------------------------------------------------------------------------------
     def _refuse_group(self, group) -> None:
@@ -1843,11 +1844,234 @@ class NCFTrainer(_StepTrainer):
         self._b = b
 
 
+class _TiedTable:
+    """The weight-tied item table E (N_I, D) of a CategoricalOutput and its bias (N_I,), trained outside the arena on
+    DENSE gradients: grad = [dE | db], where dE is the output side's G^T x / T (every row) plus the input side's
+    IndexedSlices (mm_slices_add_dense), as TensorFlow sums a gather's and a matmul's gradient of one variable.  So every
+    optimizer (LazyAdam too) updates every row of E every step.  E's optimizer slots are the trainer's table slots when an
+    input feature reads E, its own otherwise; e_split and bt are the operands the catalog kernels read (E's split rows and
+    b / T), refreshed after each update."""
+
+    def __init__(self, tr: "_StepTrainer", out, t: Optional[int]):
+        opt, dev = tr.opt, tr.device
+        self.tr, self.out, self.t = tr, out, t
+        self.E, self.bias = out.table.table, out.bias
+        N, D = self.E.shape
+        self.T = float(out.logits_temperature)
+        nb = N if self.bias is not None else 0
+        self.grad = torch.zeros(_align(N * D) + nb, dtype=torch.float32, device=dev)
+        self.dE = self.grad[:N * D].view(N, D)
+        self.db = self.grad[_align(N * D):] if nb else None
+        if t is None:  # no input feature reads E: its own slots
+            self.s1 = torch.full_like(self.E, opt.initial_accumulator_value) if opt.slots >= 1 else None
+            self.s2 = torch.zeros_like(self.E) if opt.slots >= 2 else None
+        else:
+            self.s1, self.s2 = tr.tstate1[t], tr.tstate2[t]
+        self.b_s1 = torch.full((nb,), opt.initial_accumulator_value, dtype=torch.float32, device=dev) if nb and opt.slots >= 1 else None
+        self.b_s2 = torch.zeros(nb, dtype=torch.float32, device=dev) if nb and opt.slots >= 2 else None
+        self.e_split = ops.split_rows(self.E)
+        self.bt = None
+        if self.bias is not None:
+            self.bt = self.bias if self.T == 1.0 else torch.zeros_like(self.bias)
+            self._inv_t = torch.full((1,), 1.0 / self.T, dtype=torch.float32, device=dev)
+            self._zero = torch.zeros(1, dtype=torch.float32, device=dev)
+        self.refresh()
+
+    def state(self) -> Dict[str, Optional[torch.Tensor]]:
+        """The variables a step changes that the trainer's table state does not already hold."""
+        st = {"tied/bias": self.bias, "tied/bias/s1": self.b_s1, "tied/bias/s2": self.b_s2}
+        if self.t is None:
+            st.update({"tied/embeddings": self.E, "tied/embeddings/s1": self.s1, "tied/embeddings/s2": self.s2})
+        return st
+
+    def apply(self) -> None:
+        kind, hyper = self.tr.opt.kind, self.tr.hyper
+        ops.dense_apply(kind, self.E.view(-1), self.dE.view(-1), None if self.s1 is None else self.s1.view(-1),
+                        None if self.s2 is None else self.s2.view(-1), hyper)
+        if self.bias is not None:
+            ops.dense_apply(kind, self.bias, self.db, self.b_s1, self.b_s2, hyper)
+
+    def refresh(self) -> None:
+        """The catalog kernels' operands (E's split rows, b / T) and E's lookup mirror, if it has one, from the variables."""
+        ops.split_rows(self.E, out=self.e_split)
+        if self.bt is not None and self.bt is not self.bias:
+            N = self.bias.numel()
+            ops.scale_shift(self.bias.view(N, 1), self._inv_t, self._zero, out=self.bt.view(N, 1))
+        m = self.out.table._mirror
+        if m is not None and m.shape[0] == self.E.shape[0]:
+            ops.split_rows(self.E, out=m)
+
+
+class CatalogTrainer(_StepTrainer):
+    """Static-buffer training step of Model(InputBlockV2, MLPBlock, CategoricalOutput(to_call=EmbeddingTable)) — the
+    weight-tied next-item classifier — at one batch size, with Keras CategoricalCrossentropy(from_logits=True) on
+    z = (x E^T + b) / T: loss = sum_b c_b (lse_b - z_b[y_b]), c = sample_weight / B (1 / B without weights).
+
+    forward   the input block as MMoETrainer's (one-hot features gathered, multi-hot features pooled) into x0 and its split
+              operand; mm_dense_tc per MLP layer (the last one emits x's split operand when T = 1); x / T by mm_scale_shift
+              and its split (T != 1); mm_catalog_score's soft-max statistics against the trainer's split copy of E with
+              b / T, without the (B, N_I) logits
+    backward  mm_catalog_softmax_ce_backward: dx, dE (N_I, D) over every row, db and the loss; the MLP's backward down to
+              dx0; mm_concat_backward into the tables' IndexedSlices, mm_bag_grad_rows for multi-hot features; the tied
+              table's input-side slices added into dE by mm_slices_add_dense (duplicates in index order, one writer per row)
+    update    mm_opt_tick, mm_dense_apply over the arena, over E (flat N_I D) and over the bias, mm_sparse_rows_apply for
+              the untied tables; then E's split copy, b / T and the MLP's split weights are refreshed, and after the step
+              CategoricalOutput.refresh() drops its cached operands, so a later forward, top_k or evaluate sees the update.
+    A label outside [0, N_I) is never used as an address: it adds one to the gathers' out-of-range counter, which
+    check_indices (once per `fit` epoch) turns into an IndexError.  Fixed-length list features can be captured into one
+    CUDA graph; ragged ones train eagerly."""
+
+    _model_name = "a Model(InputBlockV2, MLPBlock, CategoricalOutput)"
+
+    def __init__(self, model, optimizer: Optimizer, batch_size: int, device=None, group=None):
+        from .models import CatalogModel
+
+        if not isinstance(model, CatalogModel):
+            raise NotImplementedError("CatalogTrainer trains Model(InputBlockV2, MLPBlock, CategoricalOutput)")
+        self._refuse_group(group)
+        self._require_tc_engine()
+        ib, out = model.body.input_block, model.prediction
+        self._refuse_sharded(ib.embeddings)
+        self._check_mlps([model.body.bottom])
+        D = out.table.dim
+        if D > 128 or D % 4:
+            raise NotImplementedError(f"table {out.table.table_name!r}: training a CategoricalOutput needs an item table width "
+                                      f"that is a multiple of 4 no larger than 128 (the catalog kernels'), got {D}")
+        if not out.table.trainable:
+            raise NotImplementedError(f"table {out.table.table_name!r}: a frozen CategoricalOutput table is not implemented")
+        self._init_common(model, optimizer, batch_size, device, None)
+        self.layers = model.body.bottom.dense_layers
+        self._check_activations(self.layers)
+        self.outputs, self.H, self.losses, self.loss_weights = [out], 1, [out.loss], [1.0]
+        self.inp = _ConcatInput(self, ib, dx0=True)
+        self.inp.check_multihot_widths(model.schema)
+        self._init_inputs([self.inp])
+        tt = next((t for t, tb in enumerate(self.tables) if tb is out.table), None)
+        if tt is not None:  # the tied table's gradient is dense: it leaves the sparse updates
+            self._by_width = {w: [t for t in ts if t != tt] for w, ts in self._by_width.items()}
+        self._init_dense(self.layers, [])
+        self._init_wide(lambda li: li > 0 or bool(self.tables))
+        self.T = float(out.logits_temperature)
+        self.D, self.N = D, out.num_classes
+        B = self.B
+        f32 = dict(dtype=torch.float32, device=self.device)
+        self.h, self.h_split, self.dh = self._chain_buffers(self.layers, split_last=self.T == 1.0)
+        if self.T != 1.0:
+            self.xt = torch.zeros((B, D), **f32)
+            self.xt_split = torch.zeros((B, 2 * ops.tc_padded_k(D)), dtype=torch.bfloat16, device=self.device)
+            self._t_vec = (torch.full((D,), 1.0 / self.T, **f32), torch.zeros(D, **f32))
+        self.stats = torch.zeros((B, 3), **f32)
+        # workspaces for every batch size up to B (their sizes need not grow with it)
+        self.ws_stats = torch.zeros(max(16, max(ops.catalog_workspace_bytes(m, self.N) for m in range(1, B + 1))),
+                                    dtype=torch.uint8, device=self.device)
+        self.ws_bwd = torch.zeros(max(16, max(ops.catalog_softmax_ce_workspace_bytes(m, self.N, D) for m in range(1, B + 1))),
+                                  dtype=torch.uint8, device=self.device)
+        self.c = torch.zeros(B, **f32)  # per-row loss weights c = sample_weight / b
+        self._inv_b: Dict[int, torch.Tensor] = {}
+        self._zero = torch.zeros(1, **f32)
+        self.ws_merge: Optional[torch.Tensor] = None  # mm_slices_add_dense's workspace, sized by the first batch
+        self.tt = tt
+        self.wk = _TiedTable(self, out, tt)
+        self._init_loss(B)
+        self.logits = self.stats  # per row of the last step: [max, log-sum-exp, target logit] of the tempered logits
+        self.oob = self.inp.oob if self.inp.oob is not None else torch.zeros(1, dtype=torch.int32, device=self.device)
+
+    def _scale(self, b: int) -> torch.Tensor:
+        c = self._inv_b.get(b)
+        if c is None:
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError("the loss scale of a new batch size cannot be created during graph capture")
+            c = self._inv_b[b] = torch.full((1,), 1.0 / b, dtype=torch.float32, device=self.device)
+        return c
+
+    def _labels(self, targets, b: int) -> torch.Tensor:
+        ys = list(targets) if isinstance(targets, (list, tuple)) else [targets]
+        if len(ys) != 1:
+            raise ValueError(f"one target tensor expected (the class ids), got {len(ys)}")
+        y = ys[0].reshape(-1)
+        if y.numel() != b or y.dtype not in (torch.int32, torch.int64):
+            raise ValueError(f"targets must hold {b} int32 / int64 class ids, got {tuple(ys[0].shape)} {ys[0].dtype}")
+        return y
+
+    def table_gradients(self) -> Dict[str, tuple]:
+        """{feature: (ids, rows)} of the last forward_backward: every input table's IndexedSlices before duplicates are
+        summed (multi-hot features: one row per id); the tied table's are already in `gradients()['tied/embeddings']`."""
+        out = {}
+        for t, f in enumerate(self.feats):
+            bag = self._bags.get(t)
+            out[f] = (self._idx[t], self._slices[t]) if bag is None else (bag["apply_ids"], bag["rows"])
+        return out
+
+    def gradients(self) -> Dict[str, torch.Tensor]:
+        """The MLP's gradients by variable name, the tied table's dense dE (both sides) and the bias' db (after
+        forward_backward, before apply_gradients)."""
+        out = super().gradients()
+        out["tied/embeddings"] = self.wk.dE
+        if self.wk.db is not None:
+            out["tied/bias"] = self.wk.db
+        return out
+
+    def forward_backward(self, inputs: Dict[str, torch.Tensor], targets, sample_weight=None) -> None:
+        """Forward (activations saved), the catalog soft-max cross-entropy and the backward: fills the arena's gradients,
+        the tables' IndexedSlices and the tied table's [dE | db].  Batches smaller than the compiled size run in the
+        leading rows of the same buffers."""
+        b, targets, sample_weight = self._begin_step(inputs, targets, sample_weight)
+        y = self._labels(targets, b)
+        wk, D = self.wk, self.D
+        _, xs, dx0 = self.inp.forward(inputs, b)
+        h, h_split, dh = ([t[:b] for t in bufs] for bufs in (self.h, self.h_split, self.dh))
+        self._chain_forward(xs, self.inp.d, 0, self.layers, h, h_split)
+        x = h[-1]
+        if self.T == 1.0:
+            x_split = h_split[-1]
+        else:
+            ops.scale_shift(x, *self._t_vec, out=self.xt[:b])
+            x_split = ops.split_rows(self.xt[:b], out=self.xt_split[:b])
+        stats = self.stats[:b]
+        ops.catalog_stats_split(x_split, D, wk.e_split, stats, y, self.ws_stats, bias=wk.bt)
+        if sample_weight is None:
+            c = self._scale(b)
+        else:
+            sw = sample_weight.reshape(-1)
+            if sw.numel() != b or sw.dtype != torch.float32:
+                raise ValueError(f"sample_weight must hold {b} float32 values, got {tuple(sample_weight.shape)} {sample_weight.dtype}")
+            c = self.c[:b]
+            ops.scale_shift(sw.contiguous().view(b, 1), self._scale(b), self._zero, out=c.view(b, 1))
+        ops.catalog_softmax_ce_backward(x_split, wk.e_split, D, stats, y, c, dh[-1], wk.dE, db=wk.db, bias=wk.bt,
+                                        loss=self._loss_all[:1], temperature=self.T, workspace=self.ws_bwd, oob=self.oob)
+        if self.layers[-1].activation == "relu":
+            ops.relu_mask(dh[-1], x)
+        self._chain_backward(0, self.layers, h, dh, (xs, self.inp.d), dx0)
+        if self.tables:
+            self.inp.backward([dx0], b)
+            self._bag_grads()
+        if self.tt is not None:  # the tied table's input side: its IndexedSlices added into dE
+            bag = self._bags.get(self.tt)
+            ids, rows = (self._idx[self.tt], self._slices[self.tt]) if bag is None else (bag["apply_ids"], bag["rows"])
+            need = max(16, ops.slices_add_dense_workspace_bytes(ids.numel()))
+            if self.ws_merge is None or self.ws_merge.numel() < need:
+                if torch.cuda.is_current_stream_capturing():
+                    raise RuntimeError("the row-merge workspace cannot grow during graph capture")
+                self.ws_merge = torch.empty(need, dtype=torch.uint8, device=self.device)
+            ops.slices_add_dense(ids, rows, wk.dE, workspace=self.ws_merge)
+        self._b = b
+
+    def _refresh_operands(self) -> None:
+        super()._refresh_operands()
+        self.wk.refresh()
+
+    def _after_step(self) -> None:
+        super()._after_step()
+        self.model.prediction.refresh()  # CategoricalOutput's cached split copies and b / T
+
+
 def trainer_for(model, optimizer: Optimizer, batch_size: int, group=None):
     """The training engine of `model`: DLRMTrainer, DCNTrainer, DeepFMTrainer, WideAndDeepTrainer, MMoETrainer or
-    NCFTrainer by the ranking body, TwoTowerTrainer for a RetrievalModel."""
-    from .models import DCNBody, DeepFMBody, MMoEBody, NCFBody, RetrievalModel, RetrievalModelV2, WideAndDeepBody
+    NCFTrainer by the ranking body, TwoTowerTrainer for a RetrievalModel, CatalogTrainer for a CatalogModel."""
+    from .models import CatalogModel, DCNBody, DeepFMBody, MMoEBody, NCFBody, RetrievalModel, RetrievalModelV2, WideAndDeepBody
 
+    if isinstance(model, CatalogModel):
+        return CatalogTrainer(model, optimizer, batch_size, group=group)
     if isinstance(model, RetrievalModelV2):
         raise NotImplementedError("training TwoTowerModelV2 / ContrastiveOutput is not implemented: train the v1 TwoTowerModel")
     if isinstance(model, RetrievalModel):
