@@ -254,6 +254,15 @@ int mm_dense_tc(const void* a_split, int64_t M, int K, int Kp, const void* w_spl
                 int64_t x_stride, float* out_f32, int64_t out_stride, void* out_split,
                 int out_Kp, void* stream);
 
+/* mm_dense_tc followed by Keras Dropout(rate) in training (the weight-tied next-item step's MLP): after the activation,
+ * v = keep(row, col) ? v / (1 - rate) : 0 into out_f32 and out_split alike, keep = Philox4x32-10 of (col, row, layer,
+ * step) under key `seed`, word 0 >= round(rate 2^32) (csrc/dropout.cuh).  step: ONE device float, the optimizer's
+ * MM_HYPER_STEP counter (mm_opt_tick advances it every step), read by the kernel so graph replays draw fresh masks.
+ * A compile-time epilogue variant (dense_tc_kernel<true>): mm_dense_tc's kernel is unchanged.  No cross / scorer / head
+ * epilogue.  Errors: mm_dense_tc's, and MM_ERR_ARG for rate outside [0, 1), a null or unaligned step, layer < 0. */
+int mm_dense_tc_dropout(const void* a_split, int64_t M, int K, int Kp, const void* w_split, int N, int Np, const float* bias,
+                        int act, int passes, float* out_f32, int64_t out_stride, void* out_split, int out_Kp, float rate,
+                        uint64_t seed, const float* step, int layer, void* stream);
 /* mm_dense_tc with a fused output head: out_head[m] = head_act( act(x W + b)[m,:] . head_w + head_b ),
  * i.e. the layer followed by Dense(N -> 1) (BinaryOutput's Dense(1, sigmoid),
  * outputs/classification.py:114) evaluated in the GEMM epilogue; N <= 32.  head_w: (N,) device. */
@@ -907,6 +916,38 @@ int mm_catalog_softmax_ce_backward(const void* x_split, const void* e_split, int
                                    const void* labels, int label_dtype, float temperature, const float* stats,
                                    const float* row_scale, int row_scale_is_scalar, float* dx, float* de, float* db, float* loss,
                                    int* oob_count, void* workspace, int64_t workspace_bytes, void* stream);
+
+/* K22 with label smoothing (Keras CategoricalCrossentropy(from_logits=True, label_smoothing=eps): the target is
+ * (1 - eps) onehot(y) + eps / N).  Added with label-smoothed catalog training; no existing entry point changed.
+ *   mm_catalog_smoothed_ce_backward  the arguments of mm_catalog_softmax_ce_backward and label_smoothing = eps in [0, 1).
+ *       eps == 0 runs exactly mm_catalog_softmax_ce_backward (same kernels, same workspace, bit-identical outputs).  For
+ *       eps > 0, with s_E = sum_j e_j (D,), beta = sum_j bias_j (bias already b / T; 0 when null) and u[b] =
+ *       (eps / N) ((x_b / T).s_E + beta), the mean logit times eps:
+ *         G[b,j] = c[b] (p[b,j] - (1 - eps) [j == y_b] - eps / N)
+ *         dx[b] = 1/T sum_j G[b,j] e_j;  de[j] = sum_b G[b,j] x_b / T;  db[j] = 1/T sum_b G[b,j]
+ *         *loss += sum_b c[b] (stats[b,1] - (1 - eps) stats[b,2] - u[b])
+ *       The wgmma kernels (inbatch_flash_kernel<SmoothedCatalogCE, DQ / DN>) weigh the one-hot by 1 - eps; the uniform
+ *       part is rank one and is added where each output row is written, from two fixed-order column reductions per call
+ *       (of e_split with the bias, and of x_split weighted by c), so the (N, D) de is not passed over twice.  An
+ *       out-of-range label keeps K22's rule (no one-hot term, counted in *oob_count, loss NaN); its uniform term applies.
+ *       workspace: at least mm_catalog_smoothed_ce_workspace_bytes(B, N, D) bytes (eps == 0: K22's), 16-B aligned.
+ *       Errors before any launch: K22's, and MM_ERR_ARG for eps outside [0, 1).
+ *   mm_catalog_mean_logit  out[b] = mean_j ((x_b / T).e_j + bias_j) over the N catalog rows (the uniform target's logit,
+ *       for the smoothed loss of an evaluation pass): x_split (B, 2*Kp), e_split (N, 2*Kp), bias (N,) or null, out (B,)
+ *       fp32; the same column reduction, then one warp per row.  workspace: mm_catalog_mean_logit_workspace_bytes(N)
+ *       bytes (the column reduction's partials and sums), 16-B aligned.  Errors before any launch: MM_ERR_ARG,
+ *       MM_ERR_UNSUPPORTED (D > 128), MM_ERR_ALIGN.
+ *   mm_catalog_smoothed_ce_workspace_bytes  the backward's workspace for those shapes; depends on the device's SM count.
+ * ------------------------------------------------------------------------------------- */
+int64_t mm_catalog_smoothed_ce_workspace_bytes(int64_t B, int64_t N, int D);
+int mm_catalog_smoothed_ce_backward(const void* x_split, const void* e_split, int64_t B, int64_t N, int D, const float* bias,
+                                    const void* labels, int label_dtype, float temperature, float label_smoothing,
+                                    const float* stats, const float* row_scale, int row_scale_is_scalar, float* dx, float* de,
+                                    float* db, float* loss, int* oob_count, void* workspace, int64_t workspace_bytes,
+                                    void* stream);
+int64_t mm_catalog_mean_logit_workspace_bytes(int64_t N);
+int mm_catalog_mean_logit(const void* x_split, const void* e_split, int64_t B, int64_t N, int D, const float* bias, float* out,
+                          void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * K23  IndexedSlices into a dense gradient (the weight-tied catalog step: the tied table's input-side rows added to the

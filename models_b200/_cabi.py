@@ -174,6 +174,7 @@ SIGNATURES = {
     "mm_split_weights": (_i, [_vp, _i, _i, _vp, _i, _i, _vp]),
     "mm_dense_tc": (_i, [_vp, _i64, _i, _i, _vp, _i, _i, _vp, _i, _i, _vp, _vp, _i64, _vp, _i64,
                          _vp, _i, _vp]),
+    "mm_dense_tc_dropout": (_i, [_vp, _i64, _i, _i, _vp, _i, _i, _vp, _i, _i, _vp, _i64, _vp, _i, _f, _u64, _vp, _i, _vp]),
     "mm_dense_tc_head": (_i, [_vp, _i64, _i, _i, _vp, _i, _i, _vp, _i, _i, _vp, _f, _i, _vp, _vp]),
     "mm_mlp_tc_supported": (_i, [_i, _i, C.POINTER(C.c_int), _i]),
     "mm_mlp_tc": (_i, [_vp, _i64, _i, _i, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_void_p), C.POINTER(C.c_int),
@@ -221,6 +222,11 @@ SIGNATURES = {
     "mm_catalog_softmax_ce_workspace_bytes": (_i64, [_i64, _i64, _i]),
     "mm_catalog_softmax_ce_backward": (_i, [_vp, _vp, _i64, _i64, _i, _vp, _vp, _i, _f, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp, _vp,
                                             _i64, _vp]),
+    "mm_catalog_smoothed_ce_workspace_bytes": (_i64, [_i64, _i64, _i]),
+    "mm_catalog_smoothed_ce_backward": (_i, [_vp, _vp, _i64, _i64, _i, _vp, _vp, _i, _f, _f, _vp, _vp, _i, _vp, _vp, _vp, _vp, _vp,
+                                             _vp, _i64, _vp]),
+    "mm_catalog_mean_logit_workspace_bytes": (_i64, [_i64]),
+    "mm_catalog_mean_logit": (_i, [_vp, _vp, _i64, _i64, _i, _vp, _vp, _vp, _i64, _vp]),
     "mm_slices_add_dense_workspace_bytes": (_i64, [_i64]),
     "mm_slices_add_dense": (_i, [_vp, _i, _vp, _i64, _i, _vp, _i64, _vp, _i64, _vp]),
     "mm_l2_normalize_backward": (_i, [_vp, _vp, _i64, _i, _i64, _i64, _vp, _i64, _vp]),

@@ -365,10 +365,19 @@ class MLP(SequentialBlock):
     BatchNormalization, blocks/mlp.py:108-135; dropout is identity at inference and is not a layer here)."""
 
     def __init__(self, layers: Sequence[_Dense], filter_names: Optional[List[str]] = None, block_name: str = "MLPBlock",
-                 dropout: Optional[float] = None):
+                 dropout: Optional[float] = None, no_activation_last_layer: bool = False):
         super().__init__(layers, block_name=block_name)
         self.filter_names = filter_names
         self.dropout = dropout
+        self.no_activation_last_layer = no_activation_last_layer
+
+    def dropout_rates(self) -> List[float]:
+        """Per Dense layer, the training-mode dropout rate after it (blocks/mlp.py:97-131: after every layer, except the
+        last one when no_activation_last_layer); 0.0 where there is none."""
+        n = len(self.dense_layers)
+        rate = float(self.dropout or 0.0)
+        last = getattr(self, "no_activation_last_layer", False)
+        return [0.0 if (last and i == n - 1) else rate for i in range(n)]
 
     @property
     def dense_layers(self) -> List[_Dense]:
@@ -511,7 +520,8 @@ def MLPBlock(dimensions: List[int], activation: Union[str, List[str]] = "relu", 
             names = list(filter)
         else:
             raise ValueError("MLPBlock(filter=Tags) needs a schema; pass a Schema or a list of names")
-    return MLP(layers, filter_names=names, block_name=block_name, dropout=dropout)
+    return MLP(layers, filter_names=names, block_name=block_name, dropout=dropout,
+               no_activation_last_layer=no_activation_last_layer)
 
 
 class FMPairwiseInteraction(Block):

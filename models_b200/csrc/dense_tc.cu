@@ -24,6 +24,7 @@
 #include <cuda_bf16.h>
 
 #include "mm_common.cuh"
+#include "dropout.cuh"
 #include "tc_common.cuh"
 
 namespace mm {
@@ -68,11 +69,18 @@ struct Params {
   float head_b;
   int head_act;
   float* head_out;
+  // dropout (dense_tc_kernel<true> only): after the activation, v = keep(row, col) ? v * drop_scale : 0 (dropout.cuh),
+  // the step counter read from device memory so each graph replay draws a fresh mask
+  int drop;
+  float drop_scale;
+  const float* drop_step;
+  uint32_t drop_k0, drop_k1, drop_layer, drop_threshold;
 };
 
 // ---------------------------------------------------------------------------------------------
 // the GEMM kernel
 // ---------------------------------------------------------------------------------------------
+template <bool DROP>
 __global__ void __launch_bounds__(kThreads, 1)
 dense_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const Params p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -390,6 +398,15 @@ dense_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
           for (int j = 0; j < 32; ++j)
             if (n0 + c0 + j < p.N) v[j] = apply_act_slow(v[j], p.act);  // warp-uniform: skip padding columns
         }
+        if constexpr (DROP) {  // Keras Dropout(rate) in training, after the activation: the fp32 and split outputs both
+          const mm::drop::Mask mk{p.drop_k0, p.drop_k1, (uint32_t)__ldg(p.drop_step), p.drop_layer, p.drop_threshold};
+          const uint32_t grow = (uint32_t)(row0 + lane);
+#pragma unroll
+          for (int j = 0; j < 32; ++j) {
+            const uint32_t col = (uint32_t)(n0 + c0 + j);
+            v[j] = mk.keep(grow, col) ? v[j] * p.drop_scale : 0.0f;
+          }
+        }
         // padding columns (n >= N) must be exact zeros for the next layer's operand
         if (n0 + c0 + 32 > p.N) {
 #pragma unroll
@@ -560,7 +577,8 @@ static int dense_tc_launch(const void* a_split, int64_t M, int K, int Kp, const 
                            int64_t x_stride, float* out_f32, int64_t out_stride, void* out_split, int out_Kp,
                            int score_mode, const void* pos_ids, const void* neg_ids, int id_is64, float fns,
                            float temperature, int64_t b_rows, const float* head_w, float head_b, int head_act,
-                           float* head_out, void* stream) {
+                           float* head_out, void* stream, const mm::drop::Mask* drop = nullptr, float drop_scale = 1.0f,
+                           const float* drop_step = nullptr) {
   using namespace mm::tc;
   MM_REQUIRE(a_split && w_split && M >= 0 && K > 0 && N > 0, MM_ERR_ARG, "mm_dense_tc: null operand or non-positive K/N");
   MM_REQUIRE(Kp == mm_tc_padded_k(K) && Np == mm_tc_padded_n(N), MM_ERR_ARG,
@@ -610,6 +628,13 @@ static int dense_tc_launch(const void* a_split, int64_t M, int K, int Kp, const 
   p.head_b = head_b;
   p.head_act = head_act;
   p.head_out = head_out;
+  p.drop = drop != nullptr;
+  p.drop_scale = drop_scale;
+  p.drop_step = drop_step;
+  p.drop_k0 = drop ? drop->k0 : 0;
+  p.drop_k1 = drop ? drop->k1 : 0;
+  p.drop_layer = drop ? drop->layer : 0;
+  p.drop_threshold = drop ? drop->threshold : 0;
   // resident-A schedule: many n-tiles per m-tile and a short K (the in-batch scorer): operand traffic halves
   p.resident_a = (score_mode && passes == 3 && Kp <= 2 * BLOCK_K && p.n_tiles_n >= 8) ? 1 : 0;
   const size_t a_res_bytes = p.resident_a ? (size_t)(Kp / BLOCK_K) * 2 * A_TILE_BYTES : 0;
@@ -630,21 +655,22 @@ static int dense_tc_launch(const void* a_split, int64_t M, int K, int Kp, const 
   rc = make_map(&tmB, w_split, (uint64_t)b_rows, (uint64_t)2 * Kp, (uint32_t)p.BN);  // rows past b_rows read as zeros
   if (rc) return rc;
 
-  static size_t smem_set = 0;  // raise the dynamic-smem limit once (monotone), not per launch
-  if (smem > smem_set) {
-    cudaError_t e = cudaFuncSetAttribute(dense_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+  static size_t smem_set[2] = {0, 0};  // raise each kernel's dynamic-smem limit once (monotone), not per launch
+  auto kern = p.drop ? dense_tc_kernel<true> : dense_tc_kernel<false>;
+  if (smem > smem_set[p.drop]) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) {
       mm::set_error("mm_dense_tc: cudaFuncSetAttribute(227 KB smem) failed: %s", cudaGetErrorString(e));
       return (int)e;
     }
-    smem_set = 227 * 1024;
+    smem_set[p.drop] = 227 * 1024;
   }
   const long long tiles = ((M + BLOCK_M - 1) / BLOCK_M) * p.n_tiles_n;
   const int sms = mm::sm_count();
   unsigned grid = (unsigned)(tiles < sms ? tiles : sms);
   p.tiles_per_cta = (tiles + grid - 1) / grid;
   if (p.resident_a) grid = (unsigned)((tiles + p.tiles_per_cta - 1) / p.tiles_per_cta);  // no empty CTAs
-  dense_tc_kernel<<<grid, kThreads, smem, (cudaStream_t)stream>>>(tmA, tmB, p);
+  kern<<<grid, kThreads, smem, (cudaStream_t)stream>>>(tmA, tmB, p);
   return mm::check_launch("mm_dense_tc");
 }
 
@@ -654,6 +680,18 @@ int mm_dense_tc(const void* a_split, int64_t M, int K, int Kp, const void* w_spl
                 void* stream) {
   return dense_tc_launch(a_split, M, K, Kp, w_split, N, Np, bias, act, passes, x0, xres, x_stride, out_f32, out_stride,
                          out_split, out_Kp, 0, nullptr, nullptr, 0, 0.0f, 1.0f, Np, nullptr, 0.0f, 0, nullptr, stream);
+}
+
+int mm_dense_tc_dropout(const void* a_split, int64_t M, int K, int Kp, const void* w_split, int N, int Np, const float* bias,
+                        int act, int passes, float* out_f32, int64_t out_stride, void* out_split, int out_Kp, float rate,
+                        uint64_t seed, const float* step, int layer, void* stream) {
+  MM_REQUIRE(rate >= 0.0f && rate < 1.0f, MM_ERR_ARG, "mm_dense_tc_dropout: rate must be in [0, 1)");
+  MM_REQUIRE(step && ((uintptr_t)step % 4) == 0 && layer >= 0, MM_ERR_ARG,
+             "mm_dense_tc_dropout: a 4-B aligned step counter and a layer >= 0 are required");
+  const mm::drop::Mask mk{(uint32_t)seed, (uint32_t)(seed >> 32), 0u, (uint32_t)layer, mm::drop::threshold_of(rate)};
+  return dense_tc_launch(a_split, M, K, Kp, w_split, N, Np, bias, act, passes, nullptr, nullptr, 0, out_f32, out_stride,
+                         out_split, out_Kp, 0, nullptr, nullptr, 0, 0.0f, 1.0f, Np, nullptr, 0.0f, 0, nullptr, stream, &mk,
+                         1.0f / (1.0f - rate), step);
 }
 
 int mm_dense_tc_head(const void* a_split, int64_t M, int K, int Kp, const void* w_split, int N, int Np,

@@ -21,6 +21,8 @@
 //                   value and the one-hot compares the column index with the row's label in registers.  DQ: G = c / T
 //                   (softmax - onehot), dX = G E; DN: G = c (softmax - onehot), dE = G^T (x / T), db = 1 / T sum_b G.
 //                   DQ may split the catalog over gridDim.y CTAs per query tile (partial dX, summed in a fixed order)
+//   SmoothedCatalogCE  CatalogCE against the label-smoothed target (1 - eps) onehot + eps / N: the one-hot weighs 1 - eps
+//                   and the uniform part's rank-one terms are added in the epilogue from fixed-order column sums
 // and inbatch_loss_kernel adds any of the losses from the per-row statistics in a fixed order (one CTA).
 //
 // Two warpgroups (64 resident rows each) over a TMA ring of streamed tiles: the forward catalog kernel's structure
@@ -71,7 +73,14 @@ struct Params {
   float* db;            // dn kernel: (N,) bias gradient, or null
   int tiles_per_split;  // dq kernel: streamed tiles per CTA of a query tile (gridDim.y CTAs share one)
   int* oob;             // dq kernel: labels outside [0, N) are counted here (null: not counted)
+  // label-smoothed catalog soft-max only (SmoothedCatalogCE)
+  float keep;           // 1 - eps: the one-hot's weight in the smoothed target
+  const float* ls_e;    // [kAux]: (eps / N) sum_j e_j per column, (eps / N) sum_j b_j / T at kAuxExtra
+  const float* ls_x;    // [kAux]: (eps / N) sum_b c_b x_b / T per column, (eps / N) sum_b c_b at kAuxExtra
 };
+
+// the label-smoothing vectors: 128 columns and one extra sum at kAuxExtra, padded to kAux floats
+constexpr int kAux = 160, kAuxExtra = 128;
 
 // The catalog kernels stream up to N / 128 tiles into one wgmma fp32 accumulator, which loses magnitude over millions of
 // additions (dx of a 10 M catalog in 4 splits came out 0.2 % small).  Every kFlushTiles tiles a CTA adds its accumulator
@@ -90,6 +99,7 @@ __device__ __forceinline__ long long id_at(const void* p, long long i, int is64)
 struct SoftmaxCE {
   static constexpr bool kTwoPass = false;
   static constexpr bool kCatalog = false;
+  static constexpr bool kSmooth = false;
   __device__ __forceinline__ static float logq_bias(const float* prob, long long n) {  // the forward's -log(p + 1e-16)
     return prob ? -logf(prob[n] + 1e-16f) : 0.0f;
   }
@@ -143,6 +153,7 @@ struct Pairwise {
   static constexpr int kKind = KIND;
   static constexpr bool kTwoPass = pw::is_max<KIND>::value;  // the forward's lse pass
   static constexpr bool kCatalog = false;
+  static constexpr bool kSmooth = false;
   template <int MODE>
   static constexpr int cols() {
     return MODE == DN ? 3 : 0;
@@ -184,6 +195,7 @@ struct Pairwise {
 struct CatalogCE {
   static constexpr bool kTwoPass = false;
   static constexpr bool kCatalog = true;
+  static constexpr bool kSmooth = false;
   __device__ __forceinline__ static float label_of(const Params& p, long long b, long long n_classes) {
     const long long y = id_at(p.labels, b, p.id_is64);
     return __int_as_float(y >= 0 && y < n_classes ? (int)y : -1);
@@ -232,6 +244,21 @@ struct CatalogCE {
     return sc * (ex2_approx((s - lse) * LOG2E) - (hit ? 1.0f : 0.0f));
   }
   __device__ __forceinline__ static float g0(const Params&, long long) { return 0.0f; }
+};
+
+// CatalogCE against the label-smoothed target (1 - eps) onehot + eps / N.  The tile keeps G = c (softmax - (1 - eps)
+// onehot); the uniform part -c eps / N is the same for every column, so its products are rank-one and come from the
+// column sums in ls_e / ls_x, added where each output row is written: dx -= c / T ls_e, dE -= ls_x, db -= ls_x[extra] / T.
+struct SmoothedCatalogCE : CatalogCE {
+  static constexpr bool kSmooth = true;
+  template <int MODE>
+  __device__ __forceinline__ static float grad(const Params& p, float s, const float (&r)[3], const float* c) {
+    const float lse = MODE == DN ? c[0] : r[0];
+    const float sc = MODE == DN ? c[kColStride] : r[1];
+    const bool hit = MODE == DN ? __float_as_int(c[2 * kColStride]) == __float_as_int(r[1])
+                                : __float_as_int(r[2]) == __float_as_int(c[kColStride]);
+    return sc * (ex2_approx((s - lse) * LOG2E) - (hit ? p.keep : 0.0f));
+  }
 };
 
 // wgmma with the A operand from registers and an MN-major (transposed) B operand: D[64 x n] += A[64 x 16] . B[16 x n]
@@ -612,6 +639,7 @@ inbatch_flash_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
           const float ov = __shfl_xor_sync(0xffffffffu, dbacc[h], o);
           dbacc[h] = (o & lane) ? ov + dbacc[h] : dbacc[h] + ov;
         }
+        if constexpr (Loss::kSmooth) dbacc[h] -= p.ls_x[kAuxExtra];
         if (p.db && rvalid[h] && part == 0) p.db[row[h]] = dbacc[h] * p.inv_temp;
       }
     }
@@ -634,6 +662,12 @@ inbatch_flash_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
             float v = dacc[4 * j + 2 * h + e];
             if (add) v = fmaf(g0, addend[o], v);
             if (Loss::kCatalog && total > kFlushTiles) v = out[o] + v;  // after the flushed chunks
+            if constexpr (Loss::kSmooth) {  // the uniform target's term, in the first split's partial only
+              if (TRANS)
+                v -= p.ls_x[c];
+              else if (blockIdx.y == 0)
+                v = fmaf(-rv[h][1], p.ls_e[c], v);
+            }
             out[o] = v;
             if (!TRANS && p.dpos) p.dpos[o] = g0 * p.q[o];
           }
@@ -673,6 +707,148 @@ __global__ void split_sum_kernel(long long n, int S, const float* __restrict__ p
   }
 }
 
+// ---- label smoothing: column sums of a split operand, in a fixed order ----
+// The rows are cut into chunks (at most kSumChunks, a function of the row count only); warp w of a chunk's CTA adds rows
+// w, w + 8, ... of the chunk in row order, in double, and the CTA adds its warps in warp order into the chunk's partial
+// (kPartStride doubles: the columns, then the extra sum at kAuxExtra).  colsum_finish_kernel adds the partials in chunk
+// order.  The extra sum is sum_r extra[r] (the bias), or sum_r w[r] (the row weights c) when extra is null.
+constexpr int kSumWarps = 8, kSumChunks = 1024, kPartStride = 130;
+
+static long long sum_chunks(long long R) {
+  const long long c = (R + 255) / 256;
+  return c < kSumChunks ? c : kSumChunks;
+}
+
+template <int KB>
+__global__ void __launch_bounds__(kSumWarps * 32)
+colsum_partial_kernel(const __nv_bfloat16* __restrict__ split, long long R, int D, long long per_chunk, const float* __restrict__ w,
+                      int w_scalar, const float* __restrict__ extra, double* __restrict__ part) {
+  constexpr int KP = 64 * KB;
+  __shared__ double sm[kSumWarps][kPartStride];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long long r0 = (long long)blockIdx.x * per_chunk, r1 = min(R, r0 + per_chunk);
+  double acc[2 * KB] = {}, ex = 0.0;
+  for (long long r = r0 + warp; r < r1; r += kSumWarps) {
+    const __nv_bfloat16* row = split + r * 2 * KP;
+    const float wr = w ? w[w_scalar ? 0 : r] : 1.0f;
+#pragma unroll
+    for (int k = 0; k < KB; ++k) {
+      const int c = 64 * k + 2 * lane;
+      const float2 hi = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(row + c));
+      const float2 lo = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(row + KP + c));
+      acc[2 * k] += (double)(wr * (hi.x + lo.x));
+      acc[2 * k + 1] += (double)(wr * (hi.y + lo.y));
+    }
+    if (lane == 0) ex += extra ? (double)extra[r] : w ? (double)wr : 0.0;
+  }
+#pragma unroll
+  for (int k = 0; k < KB; ++k) {
+#pragma unroll
+    for (int e = 0; e < 2; ++e) {
+      const int c = 64 * k + 2 * lane + e;
+      sm[warp][c] = c < D ? acc[2 * k + e] : 0.0;
+    }
+  }
+  if (lane == 0) sm[warp][kAuxExtra] = ex;
+  __syncthreads();
+  for (int c = threadIdx.x; c <= kAuxExtra; c += blockDim.x) {
+    double s = 0.0;
+    if (c < KP || c == kAuxExtra) {
+      for (int i = 0; i < kSumWarps; ++i) s += sm[i][c];
+    }
+    part[blockIdx.x * (long long)kPartStride + c] = s;
+  }
+}
+
+// out[c] = scale sum_chunk part[chunk][c] in chunk order, c in [0, kAux) (zero past the sums)
+__global__ void colsum_finish_kernel(const double* __restrict__ part, int chunks, double scale, float* __restrict__ out) {
+  for (int c = threadIdx.x; c < kAux; c += blockDim.x) {
+    double s = 0.0;
+    if (c <= kAuxExtra) {
+      for (int i = 0; i < chunks; ++i) s += part[(long long)i * kPartStride + c];
+    }
+    out[c] = (float)(scale * s);
+  }
+}
+
+// out[b] = x_split[b] . aux[0:Kp] + aux[kAuxExtra]: one warp per row, the lanes' products added in a fixed butterfly
+template <int KB>
+__global__ void __launch_bounds__(256) row_dot_kernel(const __nv_bfloat16* __restrict__ split, long long B, int D,
+                                                      const float* __restrict__ aux, float* __restrict__ out) {
+  constexpr int KP = 64 * KB;
+  const int lane = threadIdx.x & 31;
+  const long long b = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (b >= B) return;
+  const __nv_bfloat16* row = split + b * 2 * KP;
+  float s = 0.0f;
+#pragma unroll
+  for (int k = 0; k < KB; ++k) {
+    const int c = 64 * k + 2 * lane;
+    const float2 hi = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(row + c));
+    const float2 lo = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(row + KP + c));
+    if (c < D) s = fmaf(hi.x + lo.x, aux[c], s);
+    if (c + 1 < D) s = fmaf(hi.y + lo.y, aux[c + 1], s);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float v = __shfl_xor_sync(0xffffffffu, s, o);
+    s = (o & lane) ? v + s : s + v;
+  }
+  if (lane == 0) out[b] = s + aux[kAuxExtra];
+}
+
+// loss[0] += sum_b c[b] (stats[b,1] - keep stats[b,2] - u[b]): the smoothed loss with u[b] = eps mean_j z[b,j]; one CTA,
+// the fixed order of inbatch_loss_kernel
+__global__ void smoothed_loss_kernel(long long B, const float* __restrict__ stats, float keep, const float* __restrict__ u,
+                                     const float* __restrict__ row_scale, int scale_is_scalar, float* __restrict__ loss) {
+  __shared__ double part[1024];
+  double s = 0.0;
+  for (long long b = threadIdx.x; b < B; b += blockDim.x) {
+    const double d = (double)stats[b * 3 + 1] - (double)keep * (double)stats[b * 3 + 2] - (double)u[b];
+    s = fma((double)(scale_is_scalar ? row_scale[0] : row_scale[b]), d, s);
+  }
+  part[threadIdx.x] = s;
+  __syncthreads();
+  for (int o = blockDim.x / 2; o > 0; o >>= 1) {
+    if ((int)threadIdx.x < o) part[threadIdx.x] += part[threadIdx.x + o];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) loss[0] += (float)part[0];
+}
+
+// scale * (column sums of split (R, 2*Kp), extra sum) -> out[kAux]: two launches, part holds sum_chunks(R) partials
+static int colsum(const char* who, const void* split, long long R, int D, int Kp, const float* w, int w_scalar, const float* extra,
+                  double scale, double* part, float* out, cudaStream_t st) {
+  const long long chunks = sum_chunks(R), per = (R + chunks - 1) / chunks;
+  const __nv_bfloat16* s = (const __nv_bfloat16*)split;
+  if (Kp == 64)
+    colsum_partial_kernel<1><<<(unsigned)chunks, kSumWarps * 32, 0, st>>>(s, R, D, per, w, w_scalar, extra, part);
+  else
+    colsum_partial_kernel<2><<<(unsigned)chunks, kSumWarps * 32, 0, st>>>(s, R, D, per, w, w_scalar, extra, part);
+  int rc = mm::check_launch(who);
+  if (rc) return rc;
+  colsum_finish_kernel<<<1, kAux, 0, st>>>(part, (int)chunks, scale, out);
+  return mm::check_launch(who);
+}
+
+static int row_dot(const char* who, const void* split, long long B, int D, int Kp, const float* aux, float* out, cudaStream_t st) {
+  const unsigned blocks = (unsigned)((B + 7) / 8);
+  const __nv_bfloat16* s = (const __nv_bfloat16*)split;
+  if (Kp == 64)
+    row_dot_kernel<1><<<blocks, 256, 0, st>>>(s, B, D, aux, out);
+  else
+    row_dot_kernel<2><<<blocks, 256, 0, st>>>(s, B, D, aux, out);
+  return mm::check_launch(who);
+}
+
+// The smoothing workspace after the dq splits' partials (256-B aligned): the E and X column partials, ls_e, ls_x, u (B,)
+struct SmoothLayout {
+  double *part_e, *part_x;
+  float *ls_e, *ls_x, *u;
+  int64_t end;
+};
+static int64_t align256(int64_t n) { return (n + 255) & ~(int64_t)255; }
+
 // The catalog dq kernel's splits per query tile: one query tile per CTA leaves SMs idle while ceil(B / 128) is below the
 // SM count (B = 4096 is 32 CTAs), so each query tile's catalog is split over floor(SMs / query tiles) CTAs (one CTA
 // fits per SM: one wave), at most one per catalog tile and with no empty split.  The workspace is S B D floats with
@@ -684,6 +860,27 @@ static int catalog_splits(long long B, long long N) {
   if (S < 1) S = 1;
   const long long per = (n_tiles + S - 1) / S;
   return (int)((n_tiles + per - 1) / per);
+}
+
+static int64_t split_bytes(int64_t B, int64_t N, int D) {
+  const int S = catalog_splits(B, N);
+  return S > 1 ? (int64_t)S * B * D * (int64_t)sizeof(float) : 0;
+}
+
+static SmoothLayout smooth_layout(int64_t B, int64_t N, int D, void* ws) {
+  uint8_t* base = (uint8_t*)ws;
+  SmoothLayout l{};
+  int64_t o = align256(split_bytes(B, N, D));
+  l.part_e = (double*)(base + o);
+  o += align256(sum_chunks(N) * kPartStride * (int64_t)sizeof(double));
+  l.part_x = (double*)(base + o);
+  o += align256(sum_chunks(B) * kPartStride * (int64_t)sizeof(double));
+  l.ls_e = (float*)(base + o);
+  l.ls_x = l.ls_e + kAux;
+  o += align256(2 * kAux * (int64_t)sizeof(float));
+  l.u = (float*)(base + o);
+  l.end = o + align256(B * (int64_t)sizeof(float));
+  return l;
 }
 
 typedef void (*Kernel)(const CUtensorMap, const CUtensorMap, const Params);
@@ -805,9 +1002,84 @@ template <int MODE>
 static Kernel pick_ce(int Kp) {
   return Kp == 64 ? inbatch_flash_kernel<SoftmaxCE, MODE, 64> : inbatch_flash_kernel<SoftmaxCE, MODE, 128>;
 }
-template <int MODE>
+template <class Loss, int MODE>
 static Kernel pick_catalog(int Kp) {
-  return Kp == 64 ? inbatch_flash_kernel<CatalogCE, MODE, 64> : inbatch_flash_kernel<CatalogCE, MODE, 128>;
+  return Kp == 64 ? inbatch_flash_kernel<Loss, MODE, 64> : inbatch_flash_kernel<Loss, MODE, 128>;
+}
+
+// mm_catalog_softmax_ce_backward (eps == 0: the CatalogCE kernels) and its label-smoothed form (eps > 0: the column sums,
+// then the SmoothedCatalogCE kernels and the smoothed loss)
+static int catalog_backward(const char* who, const void* x_split, const void* e_split, int64_t B, int64_t N, int D,
+                            const float* bias, const void* labels, int label_dtype, float temperature, float eps,
+                            const float* stats, const float* row_scale, int row_scale_is_scalar, float* dx, float* de, float* db,
+                            float* loss, int* oob_count, void* workspace, int64_t workspace_bytes, void* stream) {
+  MM_REQUIRE(labels && stats && row_scale && dx && de, MM_ERR_ARG,
+             "%s: null pointer (labels, stats, row_scale, dx and de are required)", who);
+  MM_REQUIRE(((uintptr_t)stats | (uintptr_t)row_scale | (uintptr_t)dx | (uintptr_t)de | (uintptr_t)(bias ? bias : stats) |
+              (uintptr_t)(db ? db : stats) | (uintptr_t)(loss ? loss : stats)) % 4 == 0,
+             MM_ERR_ALIGN, "%s: fp32 buffers must be 4-B aligned", who);
+  MM_REQUIRE(((uintptr_t)workspace % 16) == 0 && ((uintptr_t)oob_count % 4) == 0, MM_ERR_ALIGN,
+             "%s: workspace must be 16-B and oob_count 4-B aligned", who);
+  int Kp = 0;
+  CUtensorMap tmX, tmE;
+  Params p{};
+  int rc = prepare(who, x_split, e_split, B, N, D, nullptr, nullptr, label_dtype, 0, temperature, dx, nullptr, de, &Kp, &tmX, &tmE,
+                   &p);
+  if (rc) return rc;
+  const int64_t need = B <= 0 ? 0 : eps > 0.0f ? smooth_layout(B, N, D, nullptr).end : split_bytes(B, N, D);
+  MM_REQUIRE(workspace_bytes >= need && (need == 0 || workspace), MM_ERR_ARG, "%s: workspace too small (%lld < %lld)", who,
+             (long long)workspace_bytes, (long long)need);
+  if (B == 0) return MM_OK;
+  p.labels = labels;
+  p.bias = bias;
+  p.stats = const_cast<float*>(stats);
+  p.row_scale = row_scale;
+  p.scale_is_scalar = row_scale_is_scalar != 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool smooth = eps > 0.0f;
+  SmoothLayout sl{};
+  if (smooth) {
+    // (eps / N) sum_j e_j and sum_j b_j / T; (eps / N) sum_b c_b x_b / T and sum_b c_b; u[b] = eps mean_j z[b, j]
+    sl = smooth_layout(B, N, D, workspace);
+    const double en = (double)eps / (double)N;
+    rc = colsum(who, e_split, N, D, Kp, nullptr, 0, bias, en, sl.part_e, sl.ls_e, st);
+    if (rc == MM_OK) rc = colsum(who, x_split, B, D, Kp, row_scale, p.scale_is_scalar, nullptr, en, sl.part_x, sl.ls_x, st);
+    if (rc == MM_OK && loss) rc = row_dot(who, x_split, B, D, Kp, sl.ls_e, sl.u, st);
+    if (rc) return rc;
+    p.keep = 1.0f - eps;
+    p.ls_e = sl.ls_e;
+    p.ls_x = sl.ls_x;
+  }
+  Params pq = p;
+  pq.oob = oob_count;
+  // dX: one CTA per (query tile, catalog split); the splits' partials are summed in split order
+  const int S = catalog_splits(B, N);
+  pq.out = S > 1 ? (float*)workspace : dx;
+  rc = launch(who, smooth ? pick_catalog<SmoothedCatalogCE, DQ>(Kp) : pick_catalog<CatalogCE, DQ>(Kp), Kp, tmX, tmE, pq, st, S);
+  if (rc) return rc;
+  if (S > 1) {
+    const long long n = B * (long long)D;
+    long long blocks = (n + 255) / 256;
+    const long long cap = (long long)mm::sm_count() * 8;
+    split_sum_kernel<<<(unsigned)(blocks < cap ? blocks : cap), 256, 0, st>>>(n, S, (const float*)workspace, dx);
+    rc = mm::check_launch(who);
+    if (rc) return rc;
+  }
+  // dE and db: one CTA per 128 catalog rows streaming the queries
+  Params pn = p;
+  pn.M = N;
+  pn.I = B;
+  pn.out = de;
+  pn.db = db;
+  rc = launch(who, smooth ? pick_catalog<SmoothedCatalogCE, DN>(Kp) : pick_catalog<CatalogCE, DN>(Kp), Kp, tmE, tmX, pn, st);
+  if (rc == MM_OK && loss) {
+    if (smooth)
+      smoothed_loss_kernel<<<1, 1024, 0, st>>>(B, stats, p.keep, sl.u, row_scale, row_scale_is_scalar != 0, loss);
+    else
+      inbatch_loss_kernel<<<1, 1024, 0, st>>>(B, stats, 3, 1, 2, row_scale, row_scale_is_scalar != 0, 1.0, loss);
+    rc = mm::check_launch(who);
+  }
+  return rc;
 }
 
 }  // namespace flash
@@ -896,66 +1168,62 @@ int mm_inbatch_pairwise_bwd(const void* q_split, const void* neg_split, int64_t 
 
 int64_t mm_catalog_softmax_ce_workspace_bytes(int64_t B, int64_t N, int D) {
   if (B <= 0 || N <= 0 || D <= 0) return 0;
-  const int S = mm::flash::catalog_splits(B, N);
-  return S > 1 ? (int64_t)S * B * D * (int64_t)sizeof(float) : 0;
+  return mm::flash::split_bytes(B, N, D);
 }
 
 int mm_catalog_softmax_ce_backward(const void* x_split, const void* e_split, int64_t B, int64_t N, int D, const float* bias,
                                    const void* labels, int label_dtype, float temperature, const float* stats,
                                    const float* row_scale, int row_scale_is_scalar, float* dx, float* de, float* db, float* loss,
                                    int* oob_count, void* workspace, int64_t workspace_bytes, void* stream) {
-  const char* who = "mm_catalog_softmax_ce_backward";
+  return mm::flash::catalog_backward("mm_catalog_softmax_ce_backward", x_split, e_split, B, N, D, bias, labels, label_dtype,
+                                     temperature, 0.0f, stats, row_scale, row_scale_is_scalar, dx, de, db, loss, oob_count,
+                                     workspace, workspace_bytes, stream);
+}
+
+int64_t mm_catalog_smoothed_ce_workspace_bytes(int64_t B, int64_t N, int D) {
+  if (B <= 0 || N <= 0 || D <= 0) return 0;
+  return mm::flash::smooth_layout(B, N, D, nullptr).end;
+}
+
+int mm_catalog_smoothed_ce_backward(const void* x_split, const void* e_split, int64_t B, int64_t N, int D, const float* bias,
+                                    const void* labels, int label_dtype, float temperature, float label_smoothing,
+                                    const float* stats, const float* row_scale, int row_scale_is_scalar, float* dx, float* de,
+                                    float* db, float* loss, int* oob_count, void* workspace, int64_t workspace_bytes,
+                                    void* stream) {
+  const char* who = "mm_catalog_smoothed_ce_backward";
+  MM_REQUIRE(label_smoothing >= 0.0f && label_smoothing < 1.0f, MM_ERR_ARG, "%s: label_smoothing must be in [0, 1)", who);
+  return mm::flash::catalog_backward(who, x_split, e_split, B, N, D, bias, labels, label_dtype, temperature, label_smoothing,
+                                     stats, row_scale, row_scale_is_scalar, dx, de, db, loss, oob_count, workspace,
+                                     workspace_bytes, stream);
+}
+
+int64_t mm_catalog_mean_logit_workspace_bytes(int64_t N) {
   using namespace mm::flash;
-  MM_REQUIRE(labels && stats && row_scale && dx && de, MM_ERR_ARG,
-             "%s: null pointer (labels, stats, row_scale, dx and de are required)", who);
-  MM_REQUIRE(((uintptr_t)stats | (uintptr_t)row_scale | (uintptr_t)dx | (uintptr_t)de | (uintptr_t)(bias ? bias : stats) |
-              (uintptr_t)(db ? db : stats) | (uintptr_t)(loss ? loss : stats)) % 4 == 0,
-             MM_ERR_ALIGN, "%s: fp32 buffers must be 4-B aligned", who);
-  MM_REQUIRE(((uintptr_t)workspace % 16) == 0 && ((uintptr_t)oob_count % 4) == 0, MM_ERR_ALIGN,
-             "%s: workspace must be 16-B and oob_count 4-B aligned", who);
-  int Kp = 0;
-  CUtensorMap tmX, tmE;
-  Params p{};
-  int rc = prepare(who, x_split, e_split, B, N, D, nullptr, nullptr, label_dtype, 0, temperature, dx, nullptr, de, &Kp, &tmX, &tmE,
-                   &p);
-  if (rc) return rc;
-  const int64_t need = mm_catalog_softmax_ce_workspace_bytes(B, N, D);
-  MM_REQUIRE(workspace_bytes >= need && (need == 0 || workspace), MM_ERR_ARG, "%s: workspace too small (%lld < %lld)", who,
+  if (N <= 0) return 0;
+  return align256(sum_chunks(N) * kPartStride * (int64_t)sizeof(double)) + kAux * (int64_t)sizeof(float);
+}
+
+int mm_catalog_mean_logit(const void* x_split, const void* e_split, int64_t B, int64_t N, int D, const float* bias, float* out,
+                          void* workspace, int64_t workspace_bytes, void* stream) {
+  const char* who = "mm_catalog_mean_logit";
+  using namespace mm::flash;
+  MM_REQUIRE(x_split && e_split && out, MM_ERR_ARG, "%s: null pointer (x_split, e_split and out are required)", who);
+  MM_REQUIRE(B >= 0 && N > 0 && D > 0, MM_ERR_ARG, "%s: bad size (B >= 0, N > 0, D > 0)", who);
+  const int Kp = mm_tc_padded_k(D);
+  MM_REQUIRE(Kp <= 128, MM_ERR_UNSUPPORTED, "%s: D up to 128", who);
+  MM_REQUIRE(((uintptr_t)x_split % 16) == 0 && ((uintptr_t)e_split % 16) == 0 && ((uintptr_t)workspace % 16) == 0 &&
+                 ((uintptr_t)out | (uintptr_t)(bias ? bias : out)) % 4 == 0,
+             MM_ERR_ALIGN, "%s: split operands and workspace must be 16-B, fp32 buffers 4-B aligned", who);
+  const int64_t need = mm_catalog_mean_logit_workspace_bytes(N);
+  MM_REQUIRE(workspace_bytes >= need && workspace, MM_ERR_ARG, "%s: workspace too small (%lld < %lld)", who,
              (long long)workspace_bytes, (long long)need);
   if (B == 0) return MM_OK;
-  p.labels = labels;
-  p.bias = bias;
-  p.stats = const_cast<float*>(stats);
-  p.row_scale = row_scale;
-  p.scale_is_scalar = row_scale_is_scalar != 0;
   cudaStream_t st = (cudaStream_t)stream;
-  Params pq = p;
-  pq.oob = oob_count;
-  // dX: one CTA per (query tile, catalog split); the splits' partials are summed in split order
-  const int S = catalog_splits(B, N);
-  pq.out = S > 1 ? (float*)workspace : dx;
-  rc = launch(who, pick_catalog<DQ>(Kp), Kp, tmX, tmE, pq, st, S);
-  if (rc) return rc;
-  if (S > 1) {
-    const long long n = B * (long long)D;
-    long long blocks = (n + 255) / 256;
-    const long long cap = (long long)mm::sm_count() * 8;
-    split_sum_kernel<<<(unsigned)(blocks < cap ? blocks : cap), 256, 0, st>>>(n, S, (const float*)workspace, dx);
-    rc = mm::check_launch(who);
-    if (rc) return rc;
-  }
-  // dE and db: one CTA per 128 catalog rows streaming the queries
-  Params pn = p;
-  pn.M = N;
-  pn.I = B;
-  pn.out = de;
-  pn.db = db;
-  rc = launch(who, pick_catalog<DN>(Kp), Kp, tmE, tmX, pn, st);
-  if (rc == MM_OK && loss) {
-    inbatch_loss_kernel<<<1, 1024, 0, st>>>(B, stats, 3, 1, 2, row_scale, row_scale_is_scalar != 0, 1.0, loss);
-    rc = mm::check_launch(who);
-  }
-  return rc;
+  // [E's chunk partials][the (1 / N) column sums and bias sum]
+  double* part = (double*)workspace;
+  float* aux = (float*)((uint8_t*)workspace + align256(sum_chunks(N) * kPartStride * (int64_t)sizeof(double)));
+  int rc = colsum(who, e_split, N, D, Kp, nullptr, 0, bias, 1.0 / (double)N, part, aux, st);
+  return rc ? rc : row_dot(who, x_split, B, D, Kp, aux, out, st);
 }
 
 }  // extern "C"

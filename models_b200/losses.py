@@ -7,6 +7,11 @@ Each class only names a loss (its kind and, for BPR-max, reg_lambda): the retrie
 (models_b200/train.py: TwoTowerTrainer) computes it over the in-batch scores with mm_inbatch_pairwise_fwd / _bwd.  The
 positive is column 0 of the scores, the negatives the batch's items (false negatives down-scored to a constant), and the
 loss is the mean over the (B, N) per-element losses (Keras' SUM_OVER_BATCH_SIZE; top1_v2: the mean of its (B, 1) rows).
+
+CategoricalCrossEntropy / CategoricalCrossentropy name the full-catalog soft-max cross-entropy of a CategoricalOutput
+model with its label smoothing (models_b200/train.py: CatalogTrainer):
+
+    model.compile(optimizer="adam", loss=mm.losses.CategoricalCrossEntropy(from_logits=True, label_smoothing=0.1))
 """
 from __future__ import annotations
 
@@ -78,6 +83,38 @@ class HingeLoss(PairwiseLoss):
     """relu(1 + s_n - s_p)."""
 
     kind = "hinge"
+
+
+class CategoricalCrossentropy:
+    """Keras CategoricalCrossentropy(from_logits, label_smoothing) as a loss of a CategoricalOutput model
+    (CatalogModel.compile): the soft-max cross-entropy of the tempered logits against (1 - label_smoothing) onehot(y) +
+    label_smoothing / N_I.  Only from_logits=True with label_smoothing in [0, 1) trains (CatalogModel refuses the rest);
+    Keras' default is from_logits=False."""
+
+    def __init__(self, from_logits: bool = False, label_smoothing: float = 0.0):
+        self.from_logits = bool(from_logits)
+        self.label_smoothing = float(label_smoothing)
+
+    def get_config(self) -> dict:
+        return {"from_logits": self.from_logits, "label_smoothing": self.label_smoothing}
+
+    def __repr__(self) -> str:
+        args = ", ".join(f"{k}={v!r}" for k, v in self.get_config().items())
+        return f"{type(self).__name__}({args})"
+
+    def __eq__(self, other) -> bool:
+        return isinstance(other, CategoricalCrossentropy) and other.get_config() == self.get_config()
+
+    def __hash__(self) -> int:
+        return hash(tuple(sorted(self.get_config().items())))
+
+
+class CategoricalCrossEntropy(CategoricalCrossentropy):
+    """The reference's CategoricalCrossEntropy (losses/listwise.py): Keras' CategoricalCrossentropy with
+    from_logits=True by default."""
+
+    def __init__(self, from_logits: bool = True, label_smoothing: float = 0.0):
+        super().__init__(from_logits=from_logits, label_smoothing=label_smoothing)
 
 
 REGISTRY: Dict[str, Type[PairwiseLoss]] = {c.kind: c for c in (BPRLoss, BPRmaxLoss, TOP1Loss, TOP1v2Loss, TOP1maxLoss,

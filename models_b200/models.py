@@ -969,7 +969,8 @@ class CatalogModel(Model):
     classifier.  The input block and the MLP make the query x (B, D); the output scores it against the item table E
     (N_I, D) that an input feature may also read.  Calling the model returns CategoricalOutput's (B, N_I) logits without
     the temperature; `top_k` streams the table without them.  `compile` / `fit` / `train_step` train it with
-    CategoricalCrossentropy(from_logits=True) on the tempered logits (train.CatalogTrainer); `evaluate` reports that loss
+    CategoricalCrossentropy(from_logits=True), optionally label-smoothed (losses.CategoricalCrossEntropy(label_smoothing=
+    eps)), on the tempered logits (train.CatalogTrainer); `evaluate` reports that loss
     and top-k metrics of the label among the whole table (default_categorical_prediction_metrics(k=10))."""
 
     _TRANSIENT = {"_pinned": {}, "_trainer": None}
@@ -999,10 +1000,20 @@ class CatalogModel(Model):
         return self.prediction.top_k(self.query(inputs), k)
 
     def _compile_training(self, optimizer, loss=None, loss_weights=None, metrics=None, weighted_metrics=None) -> None:
+        from .losses import CategoricalCrossentropy
         from .topk import TopKMetric, _FUSED_MAX_K
 
-        if loss not in (None, "categorical_crossentropy", "CategoricalCrossentropy"):
-            raise NotImplementedError(f"loss {loss!r}: a CategoricalOutput trains with its default, categorical_crossentropy")
+        if isinstance(loss, CategoricalCrossentropy):
+            if not loss.from_logits:
+                raise NotImplementedError(f"loss {loss!r}: a CategoricalOutput trains on its logits (from_logits=True)")
+            if not 0.0 <= loss.label_smoothing < 1.0:
+                raise NotImplementedError(f"loss {loss!r}: label_smoothing in [0, 1) is implemented")
+            label_smoothing = loss.label_smoothing
+        elif isinstance(loss, str) and loss in ("categorical_crossentropy", "CategoricalCrossentropy") or loss is None:
+            label_smoothing = 0.0
+        else:
+            raise NotImplementedError(f"loss {loss!r}: a CategoricalOutput trains with its default, categorical_crossentropy, "
+                                      "or CategoricalCrossEntropy(from_logits=True, label_smoothing=...)")
         if loss_weights is not None or weighted_metrics:
             raise NotImplementedError("loss_weights / weighted_metrics: a CategoricalOutput model has one output and unweighted "
                                       "top-k metrics")
@@ -1015,6 +1026,7 @@ class CatalogModel(Model):
                 raise ValueError(f"{m.label}: k must be in [1, {_FUSED_MAX_K}] (the fused top-k's limit)")
         super()._compile_training(optimizer, None, None)
         self.topk_metrics = metrics
+        self.label_smoothing = label_smoothing
 
     @property
     def metrics_names(self) -> List[str]:
@@ -1032,7 +1044,8 @@ class CatalogModel(Model):
         dict holding them under `target_name`): `loss` is the catalog soft-max cross-entropy of the tempered logits (as in
         testing mode), weighted by sample_weight and averaged over the rows; each top-k metric has the label as the one
         relevant item among the top k of the whole table.  One mm_catalog_score pass per batch gives both (no (B, N_I)
-        logits).  Returns the values in `metrics_names` order, or a dict with return_dict=True.  A label outside [0, N_I)
+        logits); with the compiled loss' label_smoothing eps the loss is against the smoothed target, whose uniform part
+        takes the rows' mean logit from mm_catalog_mean_logit.  Returns the values in `metrics_names` order, or a dict with return_dict=True.  A label outside [0, N_I)
         is counted on the device and raises IndexError at the end."""
         from .topk import evaluate_topk
 
@@ -1042,6 +1055,7 @@ class CatalogModel(Model):
         if callbacks:
             raise NotImplementedError("evaluate(callbacks=...) is not implemented")
         out, N = self.prediction, self.prediction.num_classes
+        eps = float(getattr(self, "label_smoothing", 0.0))
         kmax = max(m.k for m in metrics)
         acc = {"loss": None, "rows": 0, "bad": None}
 
@@ -1064,7 +1078,12 @@ class CatalogModel(Model):
             # one pass over the table: the statistics of the tempered logits and their top-k (T > 0 keeps the order)
             xt, bt = out._tempered(self.query(inputs))
             stats, _, ids = ops.catalog_score(xt, out._catalog_split(), N, bias=bt, targets=yv, k=kmax)
-            per = stats[:, 1] - stats[:, 2]  # an out-of-range label's target logit is NaN: counted above, raised below
+            # an out-of-range label's target logit is NaN: counted above, raised below
+            if eps:  # the smoothed target: lse - (1 - eps) z[y] - eps mean_j z[j]
+                mean = ops.catalog_mean_logit(ops.split_rows(xt), out._catalog_split(), xt.shape[1], bias=bt)
+                per = stats[:, 1] - (1.0 - eps) * stats[:, 2] - eps * mean
+            else:
+                per = stats[:, 1] - stats[:, 2]
             if len(batch) > 2 and batch[2] is not None:
                 sw = batch[2][out.name] if isinstance(batch[2], dict) else batch[2]
                 per = per * torch.as_tensor(sw, device=dev, dtype=torch.float32).reshape(-1)

@@ -485,8 +485,20 @@ def catalog_softmax_ce_workspace_bytes(B: int, N: int, D: int) -> int:
     return int(_lib().mm_catalog_softmax_ce_workspace_bytes(int(B), int(N), int(D)))
 
 
+def catalog_smoothed_ce_workspace_bytes(B: int, N: int, D: int) -> int:
+    """Bytes of the workspace catalog_softmax_ce_backward needs with label_smoothing > 0, and catalog_mean_logit needs."""
+    return int(_lib().mm_catalog_smoothed_ce_workspace_bytes(int(B), int(N), int(D)))
+
+
+def _check_label_smoothing(label_smoothing) -> float:
+    eps = float(label_smoothing)
+    if not 0.0 <= eps < 1.0:
+        raise ValueError(f"label_smoothing must be in [0, 1), got {label_smoothing}")
+    return eps
+
+
 def catalog_softmax_ce_backward(x_split, e_split, D: int, stats, labels, row_scale, dx, de, db=None, bias=None, loss=None,
-                                temperature: float = 1.0, workspace=None, oob=None) -> None:
+                                temperature: float = 1.0, workspace=None, oob=None, label_smoothing: float = 0.0) -> None:
     """Backward of the full-catalog soft-max cross-entropy (mm_catalog_softmax_ce_backward) from the operands
     catalog_score read for `stats` (B, 3): x_split = split_rows(x / T) (B, 2*Kp), e_split = split_rows(E) (N, 2*Kp) and
     bias (N,) = b / T (None: no bias).  With G = c (softmax - onehot(labels)) of the logits (x E^T + b) / T, writes dx
@@ -494,7 +506,13 @@ def catalog_softmax_ce_backward(x_split, e_split, D: int, stats, labels, row_sca
     adds sum_b c[b] (lse[b] - logit[b, label]) to `loss` (nullable).  labels (B,) int32 / int64 class ids; a label
     outside [0, N) is never used as an address: it takes no one-hot term (its loss term is NaN) and adds one to `oob`
     (nullable int32 counter, the gathers' out-of-range counter).  row_scale: (B,) or (1,) fp32 c.  workspace: uint8 of at
-    least catalog_softmax_ce_workspace_bytes(B, N, D) bytes; None allocates one (not during graph capture)."""
+    least catalog_softmax_ce_workspace_bytes(B, N, D) bytes; None allocates one (not during graph capture).
+
+    label_smoothing = eps in [0, 1): the target is (1 - eps) onehot(labels) + eps / N (Keras CategoricalCrossentropy's
+    label_smoothing), so G = c (softmax - (1 - eps) onehot - eps / N) and the loss is sum_b c[b] (lse[b] - (1 - eps)
+    logit[b, label] - eps mean_j logit[b, j]) (mm_catalog_smoothed_ce_backward; the workspace must then hold
+    catalog_smoothed_ce_workspace_bytes(B, N, D) bytes).  eps = 0 is the call above, bit for bit."""
+    eps = _check_label_smoothing(label_smoothing)
     B, N = _inbatch_buffers(D, x_split, e_split, stats, 3, extra=(("row_scale", row_scale),), joint=True)
     for n_, t_, shape in (("dx", dx, (B, D)), ("de", de, (N, D))):
         if tuple(_dev(t_, n_, torch.float32).shape) != shape or not t_.is_contiguous():
@@ -515,18 +533,50 @@ def catalog_softmax_ce_backward(x_split, e_split, D: int, stats, labels, row_sca
     label_dt = _idx_dtype(labels, "labels")
     if oob is not None and (_dev(oob, "oob", torch.int32).numel() < 1):
         raise ValueError("oob must hold at least one int32 counter")
-    need = catalog_softmax_ce_workspace_bytes(B, N, D)
+    need = catalog_softmax_ce_workspace_bytes(B, N, D) if eps == 0.0 else catalog_smoothed_ce_workspace_bytes(B, N, D)
     if workspace is None:
         workspace = torch.empty(max(need, 16), dtype=torch.uint8, device=x_split.device)
     elif _dev(workspace, "workspace", torch.uint8).numel() < need:
         raise ValueError(f"workspace must hold at least {need} bytes, got {workspace.numel()}")
     scalar = row_scale.numel() == 1 and B != 1
+    if eps > 0.0:
+        _cabi.check(
+            _lib().mm_catalog_smoothed_ce_backward(x_split.data_ptr(), e_split.data_ptr(), B, N, int(D), _ptr(bias),
+                                                   labels.data_ptr(), label_dt, float(temperature), eps, stats.data_ptr(),
+                                                   row_scale.data_ptr(), int(scalar), dx.data_ptr(), de.data_ptr(), _ptr(db),
+                                                   _ptr(loss), _ptr(oob), workspace.data_ptr(), workspace.numel(), _stream()),
+            "mm_catalog_smoothed_ce_backward")
+        return
     _cabi.check(
         _lib().mm_catalog_softmax_ce_backward(x_split.data_ptr(), e_split.data_ptr(), B, N, int(D), _ptr(bias), labels.data_ptr(),
                                               label_dt, float(temperature), stats.data_ptr(), row_scale.data_ptr(), int(scalar),
                                               dx.data_ptr(), de.data_ptr(), _ptr(db), _ptr(loss), _ptr(oob), workspace.data_ptr(),
                                               workspace.numel(), _stream()),
         "mm_catalog_softmax_ce_backward")
+
+
+def catalog_mean_logit(x_split, e_split, D: int, bias=None, out=None, workspace=None) -> torch.Tensor:
+    """(B,) mean_j of the logits x_split[b] . e_j + bias_j over the N catalog rows (mm_catalog_mean_logit), from the split
+    operands catalog_score reads (x_split (B, 2*Kp) of the tempered queries, e_split (N, 2*Kp), bias (N,) = b / T or
+    None): the logit of the label-smoothed target's uniform part.  workspace: uint8 of at least
+    mm_catalog_mean_logit_workspace_bytes(N) bytes; None allocates one."""
+    _dev(x_split, "x_split", torch.bfloat16), _dev(e_split, "e_split", torch.bfloat16)
+    B, N = x_split.shape[0], e_split.shape[0]
+    _vec(bias, N, "bias")
+    if out is None:
+        out = torch.empty(B, dtype=torch.float32, device=x_split.device)
+    elif _dev(out, "out", torch.float32).numel() != B or not out.is_contiguous():
+        raise ValueError(f"out must be contiguous ({B},)")
+    need = int(_lib().mm_catalog_mean_logit_workspace_bytes(int(N)))
+    if workspace is None:
+        workspace = torch.empty(max(need, 16), dtype=torch.uint8, device=x_split.device)
+    elif _dev(workspace, "workspace", torch.uint8).numel() < need:
+        raise ValueError(f"workspace must hold at least {need} bytes, got {workspace.numel()}")
+    _cabi.check(
+        _lib().mm_catalog_mean_logit(x_split.data_ptr(), e_split.data_ptr(), B, N, int(D), _ptr(bias), out.data_ptr(),
+                                     workspace.data_ptr(), workspace.numel(), _stream()),
+        "mm_catalog_mean_logit")
+    return out
 
 
 def catalog_stats_split(x_split, D: int, e_split, stats, labels, workspace, bias=None) -> torch.Tensor:
@@ -839,8 +889,9 @@ def split_weights(W: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.
 def dense_tc(a_split: torch.Tensor, K: int, w_split: torch.Tensor, N: int, bias: Optional[torch.Tensor],
              act: Optional[str], passes: int = 3, out_f32: Optional[torch.Tensor] = None,
              out_split: Optional[torch.Tensor] = None, x0: Optional[torch.Tensor] = None,
-             xres: Optional[torch.Tensor] = None) -> None:
-    """One tensor-core dense layer (mm_dense_tc); see include/mm_b200.h."""
+             xres: Optional[torch.Tensor] = None, dropout=None) -> None:
+    """One tensor-core dense layer (mm_dense_tc); see include/mm_b200.h.  dropout = (rate, seed, step, layer): Keras
+    Dropout(rate) in training after the activation (mm_dense_tc_dropout), step a one-float device counter."""
     _dev(a_split, "a_split", torch.bfloat16), _dev(w_split, "w_split", torch.bfloat16)
     if act not in ACTIVATIONS:
         raise ValueError(f"unsupported activation {act!r}")
@@ -860,6 +911,18 @@ def dense_tc(a_split: torch.Tensor, K: int, w_split: torch.Tensor, N: int, bias:
         if xres is None or x0.stride(0) != xres.stride(0):
             raise ValueError("x0 and xres must both be given with equal row strides")
         xs = _row_stride(x0, "x0")
+    if dropout is not None:
+        rate, seed, step, layer = dropout
+        if x0 is not None or not 0.0 <= float(rate) < 1.0:
+            raise ValueError(f"dropout: rate in [0, 1) on a plain dense layer, got rate {rate}")
+        _dev(step, "step", torch.float32)
+        _cabi.check(
+            _lib().mm_dense_tc_dropout(a_split.data_ptr(), M, K, Kp, w_split.data_ptr(), N, Np, _ptr(bias), ACTIVATIONS[act],
+                                       passes, _ptr(out_f32), 0 if out_f32 is None else _row_stride(out_f32, "out_f32"),
+                                       _ptr(out_split), out_Kp, float(rate), int(seed) & (2**64 - 1), step.data_ptr(),
+                                       int(layer), _stream()),
+            "mm_dense_tc_dropout")
+        return
     _cabi.check(
         _lib().mm_dense_tc(a_split.data_ptr(), M, K, Kp, w_split.data_ptr(), N, Np, _ptr(bias), ACTIVATIONS[act],
                            passes, _ptr(x0), _ptr(xres), xs, _ptr(out_f32),

@@ -243,9 +243,9 @@ class _StepTrainer:
         if getattr(owner, "sharded", None) is not None:
             raise NotImplementedError(f"training {self._model_name} with row-sharded tables is not implemented")
 
-    def _check_mlps(self, blocks) -> None:
+    def _check_mlps(self, blocks, allow_dropout: bool = False) -> None:
         for blk in blocks:
-            if not isinstance(blk, MLP) or blk.has_normalization or blk.dropout:
+            if not isinstance(blk, MLP) or blk.has_normalization or (blk.dropout and not allow_dropout):
                 raise NotImplementedError(f"{blk.name}: training {self._model_name} supports MLPBlocks without normalization / "
                                           "dropout")
 
@@ -424,22 +424,27 @@ class _StepTrainer:
                     state2=self.tstate2[t], mirror=mirror, dense_grad=self.tdense[t])
 
     # ---- a chain of Dense layers (layers li0 .. of _tc_layers) on b-row views of _chain_buffers -----------------------
-    def _chain_forward(self, op: torch.Tensor, K: int, li0: int, layers, h, h_split) -> None:
+    def _chain_forward(self, op: torch.Tensor, K: int, li0: int, layers, h, h_split, drop=None) -> None:
         """The chain on the split operand `op` of its (b, K) input: fp32 activations into h, each layer's split output
-        (where h_split has one) into the operand of the next."""
+        (where h_split has one) into the operand of the next.  drop: per layer None or ops.dense_tc's dropout tuple."""
         for i, l in enumerate(layers):
             nxt = h_split[i] if i < len(h_split) else None
-            ops.dense_tc(op, K, self._wsplit[li0 + i], l.units, l.bias, l.activation, out_f32=h[i], out_split=nxt)
+            ops.dense_tc(op, K, self._wsplit[li0 + i], l.units, l.bias, l.activation, out_f32=h[i], out_split=nxt,
+                         dropout=None if drop is None else drop[i])
             op, K = nxt, l.units
 
-    def _chain_backward(self, li0: int, layers, h, dh, first_in, dx: Optional[torch.Tensor]) -> None:
+    def _chain_backward(self, li0: int, layers, h, dh, first_in, dx: Optional[torch.Tensor], drop_scale=None) -> None:
         """From dh[-1] (the pre-activation gradient of the last layer) down: per layer dW, db into the arena and the input
         gradient with the relu mask of the layer below.  first_in: the chain's input, as (split operand, K) or as an fp32
-        matrix; dx: where the first layer's input gradient goes (None: nothing below needs it)."""
+        matrix; dx: where the first layer's input gradient goes (None: nothing below needs it).  drop_scale: per layer
+        None or the (units,) vector 1 / (1 - rate) of a relu layer with dropout: its saved output is zero where the mask
+        dropped, so the relu mask applies the dropout mask too and only the scale is left (dh[-1] comes scaled)."""
         a = self.arena
         for i in range(len(layers) - 1, 0, -1):
             ops.dense_wgrad(h[i - 1], dh[i], a.view(a.grad, li0 + i, "kernel"), a.view(a.grad, li0 + i, "bias"))
             self._dgrad(li0 + i, layers[i], dh[i], dh[i - 1], h[i - 1] if layers[i - 1].activation == "relu" else None)
+            if drop_scale is not None and drop_scale[i - 1] is not None:
+                ops.scale_shift(dh[i - 1], drop_scale[i - 1], self._drop_zero[: dh[i - 1].shape[1]], out=dh[i - 1])
         if isinstance(first_in, tuple):
             ops.dense_wgrad_split(first_in[0], first_in[1], dh[0], a.view(a.grad, li0, "kernel"), a.view(a.grad, li0, "bias"))
         else:
@@ -1905,7 +1910,10 @@ class _TiedTable:
 class CatalogTrainer(_StepTrainer):
     """Static-buffer training step of Model(InputBlockV2, MLPBlock, CategoricalOutput(to_call=EmbeddingTable)) — the
     weight-tied next-item classifier — at one batch size, with Keras CategoricalCrossentropy(from_logits=True) on
-    z = (x E^T + b) / T: loss = sum_b c_b (lse_b - z_b[y_b]), c = sample_weight / B (1 / B without weights).
+    z = (x E^T + b) / T: loss = sum_b c_b (lse_b - z_b[y_b]), c = sample_weight / B (1 / B without weights).  With the
+    compiled loss' label_smoothing eps the target is (1 - eps) onehot(y) + eps / N_I: loss = sum_b c_b (lse_b - (1 - eps)
+    z_b[y_b] - eps mean_j z_b[j]) (mm_catalog_smoothed_ce_backward).  The MLPBlock's dropout trains here (and only here):
+    mm_dense_tc_dropout draws each layer's mask in its epilogue, and the backward scales the relu-masked gradient.
 
     forward   the input block as MMoETrainer's (one-hot features gathered, multi-hot features pooled) into x0 and its split
               operand; mm_dense_tc per MLP layer (the last one emits x's split operand when T = 1); x / T by mm_scale_shift
@@ -1932,7 +1940,7 @@ class CatalogTrainer(_StepTrainer):
         self._require_tc_engine()
         ib, out = model.body.input_block, model.prediction
         self._refuse_sharded(ib.embeddings)
-        self._check_mlps([model.body.bottom])
+        self._check_mlps([model.body.bottom], allow_dropout=True)
         D = out.table.dim
         if D > 128 or D % 4:
             raise NotImplementedError(f"table {out.table.table_name!r}: training a CategoricalOutput needs an item table width "
@@ -1942,6 +1950,15 @@ class CatalogTrainer(_StepTrainer):
         self._init_common(model, optimizer, batch_size, device, None)
         self.layers = model.body.bottom.dense_layers
         self._check_activations(self.layers)
+        # Keras Dropout(rate) in training after the MLP's layers (blocks/mlp.py:97-131), drawn in mm_dense_tc's epilogue:
+        # the mask hashes (seed of mm.set_seed, the optimizer's device step counter, layer, row, column), so eager steps
+        # and graph replays from one state draw the same masks and every step draws new ones
+        rates = model.body.bottom.dropout_rates()
+        for l, r in zip(self.layers, rates):
+            if r and l.activation != "relu":
+                raise NotImplementedError(f"{l.name}: dropout in training after a {l.activation!r} layer is not implemented "
+                                          "(relu layers only)")
+        self.dropout_rates = rates
         self.outputs, self.H, self.losses, self.loss_weights = [out], 1, [out.loss], [1.0]
         self.inp = _ConcatInput(self, ib, dx0=True)
         self.inp.check_multihot_widths(model.schema)
@@ -1964,8 +1981,10 @@ class CatalogTrainer(_StepTrainer):
         # workspaces for every batch size up to B (their sizes need not grow with it)
         self.ws_stats = torch.zeros(max(16, max(ops.catalog_workspace_bytes(m, self.N) for m in range(1, B + 1))),
                                     dtype=torch.uint8, device=self.device)
-        self.ws_bwd = torch.zeros(max(16, max(ops.catalog_softmax_ce_workspace_bytes(m, self.N, D) for m in range(1, B + 1))),
-                                  dtype=torch.uint8, device=self.device)
+        self.eps = float(getattr(model, "label_smoothing", 0.0))
+        ws_bytes = ops.catalog_smoothed_ce_workspace_bytes if self.eps else ops.catalog_softmax_ce_workspace_bytes
+        self.ws_bwd = torch.zeros(max(16, max(ws_bytes(m, self.N, D) for m in range(1, B + 1))), dtype=torch.uint8,
+                                  device=self.device)
         self.c = torch.zeros(B, **f32)  # per-row loss weights c = sample_weight / b
         self._inv_b: Dict[int, torch.Tensor] = {}
         self._zero = torch.zeros(1, **f32)
@@ -1973,6 +1992,12 @@ class CatalogTrainer(_StepTrainer):
         self.tt = tt
         self.wk = _TiedTable(self, out, tt)
         self._init_loss(B)
+        from .core import _SEED
+
+        step = self.hyper[_cabi.HYPER_STEP:_cabi.HYPER_STEP + 1]
+        self._drop = [None if not r else (r, _SEED[0], step, i) for i, r in enumerate(rates)]
+        self._drop_scale = [None if not r else torch.full((l.units,), 1.0 / (1.0 - r), **f32) for l, r in zip(self.layers, rates)]
+        self._drop_zero = torch.zeros(max(l.units for l in self.layers), **f32)
         self.logits = self.stats  # per row of the last step: [max, log-sum-exp, target logit] of the tempered logits
         self.oob = self.inp.oob if self.inp.oob is not None else torch.zeros(1, dtype=torch.int32, device=self.device)
 
@@ -2020,7 +2045,7 @@ class CatalogTrainer(_StepTrainer):
         wk, D = self.wk, self.D
         _, xs, dx0 = self.inp.forward(inputs, b)
         h, h_split, dh = ([t[:b] for t in bufs] for bufs in (self.h, self.h_split, self.dh))
-        self._chain_forward(xs, self.inp.d, 0, self.layers, h, h_split)
+        self._chain_forward(xs, self.inp.d, 0, self.layers, h, h_split, drop=self._drop)
         x = h[-1]
         if self.T == 1.0:
             x_split = h_split[-1]
@@ -2038,10 +2063,13 @@ class CatalogTrainer(_StepTrainer):
             c = self.c[:b]
             ops.scale_shift(sw.contiguous().view(b, 1), self._scale(b), self._zero, out=c.view(b, 1))
         ops.catalog_softmax_ce_backward(x_split, wk.e_split, D, stats, y, c, dh[-1], wk.dE, db=wk.db, bias=wk.bt,
-                                        loss=self._loss_all[:1], temperature=self.T, workspace=self.ws_bwd, oob=self.oob)
+                                        loss=self._loss_all[:1], temperature=self.T, workspace=self.ws_bwd, oob=self.oob,
+                                        label_smoothing=self.eps)
         if self.layers[-1].activation == "relu":
             ops.relu_mask(dh[-1], x)
-        self._chain_backward(0, self.layers, h, dh, (xs, self.inp.d), dx0)
+        if self._drop_scale[-1] is not None:
+            ops.scale_shift(dh[-1], self._drop_scale[-1], self._drop_zero[:D], out=dh[-1])
+        self._chain_backward(0, self.layers, h, dh, (xs, self.inp.d), dx0, drop_scale=self._drop_scale)
         if self.tables:
             self.inp.backward([dx0], b)
             self._bag_grads()

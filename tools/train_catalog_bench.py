@@ -1,7 +1,7 @@
 """Training step of the weight-tied next-item classifier Model(InputBlockV2, MLPBlock, CategoricalOutput), captured as one
 CUDA graph, in two legs, and its output layer's launches timed alone against the computed floors.
 
-    python tools/train_catalog_bench.py [--blocks 5] [--steps 5] [--legs a,b]
+    python tools/train_catalog_bench.py [--blocks 5] [--steps 5] [--legs a,b] [--dropout 0.2] [--label-smoothing 0.1]
 
 Schema: user_id (1 M rows x 64), two small user columns (100 and 1 000 rows), a fixed-length 20-id item history tied to
 the output (mean-pooled), and the next_item target; MLPBlock([128, 64]), D = 64, T = 1, a bias, Adagrad(0.01).  Leg (a):
@@ -13,6 +13,11 @@ statistics (mm_catalog_score), the backward's dq + dn kernels (mm_catalog_softma
 tied table's update (mm_dense_apply over N_I D), next to the output layer's FLOP floor
 (5 products x 3 split-bf16 passes x 2 B N_I D at 989 TFLOP/s) and the table update's byte floor (Adagrad reads E, dE and
 the accumulator and writes E, the accumulator and the cleared dE: 6 x 4 N_I D bytes at 3.35 TB/s).
+
+--dropout rate and / or --label-smoothing eps build a second, identical model with MLPBlock(dropout=rate) (a mask drawn in
+each layer's epilogue) compiled with CategoricalCrossEntropy(label_smoothing=eps), and time its captured step in blocks
+alternating with the plain step's, so both rows share the card's state (read by nvidia-smi in the same run); the smoothed
+backward (column sums of E and x, the smoothed dq + dn kernels) is timed beside the plain one.
 """
 import argparse
 import statistics
@@ -72,14 +77,16 @@ def events(fn, n: int) -> float:
     return statistics.median(out)
 
 
-def leg(name: str, n_items: int, B: int, args, dev) -> None:
-    s = schema(n_items)
+def step(s: Schema, n_items: int, B: int, eps: float, rate: float, dev):
+    """(model, trainer) of the benchmark's model with its step captured; eps > 0: the label-smoothed loss; rate > 0:
+    dropout after the MLP's layers."""
     mm.set_seed(1)
     emb = mm.Embeddings(s.select_by_tag(Tags.CATEGORICAL), dim={"user_id": 64, "user_age": 8, "user_city": 16, "item_history": D},
                         embeddings_initializer={"hash_seed": 5}, sequence_combiner="mean")
     out = mm.CategoricalOutput(emb.tables["item_id"], target_name="next_item")
-    model = mm.Model(mm.InputBlockV2(s, categorical=emb), mm.MLPBlock([128, D]), out)
-    model.compile(optimizer=mm.Adagrad(0.01))
+    model = mm.Model(mm.InputBlockV2(s, categorical=emb), mm.MLPBlock([128, D], dropout=rate or None), out)
+    model.compile(optimizer=mm.Adagrad(0.01),
+                  loss=mm.losses.CategoricalCrossEntropy(from_logits=True, label_smoothing=eps) if eps else None)
     model.build(dev)
     tr = model.trainer(B)
     x, y = batch(s, n_items, B, 0, dev)
@@ -87,19 +94,46 @@ def leg(name: str, n_items: int, B: int, args, dev) -> None:
     for i in range(3):  # warm-up replays
         tr.replay()
     torch.cuda.synchronize()
-    per_block = []
-    for _ in range(args.blocks):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        for _ in range(args.steps):
-            tr.replay()
-        b.record()
-        b.synchronize()
-        per_block.append(a.elapsed_time(b) / args.steps)
-    ms = statistics.median(per_block)
-    print(f"leg ({name}): N_I = {n_items:,}, B = {B:,}, D = {D}: {tr.launches_per_step} launches per step, "
-          f"{ms:.2f} ms per step (median of {args.blocks} blocks x {args.steps} replays, spread "
-          f"{min(per_block):.2f}-{max(per_block):.2f}), {B / ms * 1e3:,.0f} samples/s")
+    return model, tr
+
+
+def leg(name: str, n_items: int, B: int, args, dev) -> None:
+    s = schema(n_items)
+    eps, rate = float(args.label_smoothing), float(args.dropout)
+    runs = [("plain", *step(s, n_items, B, 0.0, 0.0, dev))]
+    if eps or rate:
+        runs.append((f"dropout={rate}, label_smoothing={eps}", *step(s, n_items, B, eps, rate, dev)))
+    per_block = {k: [] for k, _, _ in runs}
+    for _ in range(args.blocks):  # the steps alternate block by block
+        for k, _, tr in runs:
+            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            a.record()
+            for _ in range(args.steps):
+                tr.replay()
+            b.record()
+            b.synchronize()
+            per_block[k].append(a.elapsed_time(b) / args.steps)
+    for k, _, tr in runs:
+        pb = per_block[k]
+        ms = statistics.median(pb)
+        print(f"leg ({name}) {k}: N_I = {n_items:,}, B = {B:,}, D = {D}: {tr.launches_per_step} launches per step, "
+              f"{ms:.2f} ms per step (median of {args.blocks} blocks x {args.steps} replays, spread "
+              f"{min(pb):.2f}-{max(pb):.2f}), {B / ms * 1e3:,.0f} samples/s")
+    if len(runs) > 1:
+        print(f"  {runs[1][0]} / plain: {statistics.median(per_block[runs[1][0]]) / statistics.median(per_block['plain']):.4f}")
+    if eps:
+        _, tr_s = runs[1][1:]
+        wk = tr_s.wk
+        tr_s.forward_backward(tr_s._static, tr_s._static_y)
+        xs = tr_s.h_split[-1][:B]
+        yy = tr_s._static_y[0]
+        t_sm = events(lambda: ops.catalog_softmax_ce_backward(xs, wk.e_split, D, tr_s.stats, yy, tr_s._scale(B), tr_s.dh[-1][:B],
+                                                              wk.dE, db=wk.db, bias=wk.bt, workspace=tr_s.ws_bwd,
+                                                              label_smoothing=eps), 3)
+        print(f"  smoothed backward (column sums + dq + dn) {t_sm:.2f} ms")
+        del tr_s
+    del runs[1:]
+    _, model, tr = runs[0]
     # the output layer's launches alone, on the step's own buffers (after a forward_backward of the captured batch)
     wk = tr.wk
     tr.forward_backward(tr._static, tr._static_y)
@@ -130,6 +164,8 @@ def main():
     ap.add_argument("--blocks", type=int, default=5)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--legs", default="a,b")
+    ap.add_argument("--label-smoothing", type=float, default=0.0)
+    ap.add_argument("--dropout", type=float, default=0.0)
     args = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("train_catalog_bench.py needs a CUDA device")
