@@ -234,9 +234,10 @@ def test_lookup_interact_at_scale(device, D, rows_fmt, out_fmt, B):
 # 2. mm_mlp_tc / mm_mlp_tc_heads: the DLRM top tower
 # ---------------------------------------------------------------------------------------------------------------
 def _tower_laps(M, sms):
-    """Laps of mlp_tc_kernel (mlp_tc_impl: one CTA per SM, 128-row tiles)."""
-    tiles = -(-M // 128)
-    return -(-tiles // min(tiles, sms))
+    """Fewest tiles any consumer warpgroup of mlp_tc_kernel runs (mlp_tc_impl: one CTA per SM over 64-row tiles, which
+    the CTA's two consumer warpgroups take in turn)."""
+    tiles = -(-M // 64)
+    return tiles // min(tiles, sms) // 2
 
 
 @pytest.mark.parametrize("M", [BIG, RAGGED])
