@@ -966,6 +966,39 @@ int64_t mm_slices_add_dense_workspace_bytes(int64_t n);
 int mm_slices_add_dense(const void* ids, int idx_dtype, const float* rows, int64_t n, int D, float* dense, int64_t N,
                         void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---------------------------------------------------------------------------------------
+ * K24  Pretrained embeddings (PretrainedEmbeddings, inputs/embedding.py:717-800; the dataloader's EmbeddingOperator):
+ * rows of a device-resident fp32 matrix P (rows, Dp) at row stride p_stride, looked up by ids (B,) MM_I32 / MM_I64, go
+ * straight into their slot of the input block's concat.  ids == NULL reads row b of a dense (B, Dp) input instead
+ * (rows >= B).  An id outside [0, rows) reads a zero row and adds 1 to *oob_count (when non-null), once per sample.
+ * Added with the pretrained input slots; no existing entry point changed.
+ *   mm_pretrained_gather  out[b, 0:Dp] = P[ids[b]]; `out` points at the slot's first column, columns outside [0, Dp) of
+ *       each row are not written.  1 <= Dp <= MM_PRETRAINED_MAX_DIM.
+ *   mm_pretrained_project  out[b, 0:N] = P[ids[b]] W + bias (W (Dp, N) fp32 contiguous, bias (N,) or NULL), fp32
+ *       products in ascending k; the gathered rows are staged in shared memory only.  1 <= N <= MM_PRETRAINED_MAX_OUT.
+ *       Grid: min(ceil(B/64) * ceil(N/64), MM_PRETRAINED_CTAS_PER_SM * SMs) CTAs of 256 threads over the 64x64 tiles.
+ *   mm_pretrained_project_backward  g = sum of the n_addends (1..4) (B, N) matrices (each at its own row stride; pass
+ *       pointers to the slot's first column), through the l2-norm backward at the pre-norm projection ypre when non-null
+ *       (mm_l2_normalize_backward's rule), then dW (Dp, N) = P[ids]^T g and db (N,) = sum_b g (db may be NULL), both
+ *       overwritten.  Fixed row chunks (a function of B, Dp, N) and a chunk-ordered sum: repeats are bit-identical.
+ *       workspace: mm_pretrained_backward_workspace_bytes(B, Dp, N) bytes, 16-B aligned; that size is non-decreasing in B,
+ *       so a workspace sized for B serves every batch of at most B samples.
+ * Errors before any launch: MM_ERR_ARG, MM_ERR_UNSUPPORTED.
+ * ------------------------------------------------------------------------------------- */
+#define MM_PRETRAINED_MAX_DIM 1024
+#define MM_PRETRAINED_MAX_OUT 256
+#define MM_PRETRAINED_CTAS_PER_SM 8
+int mm_pretrained_gather(const float* P, int64_t rows, int Dp, int64_t p_stride, const void* ids, int idx_dtype, int64_t B,
+                         float* out, int64_t out_stride, int32_t* oob_count, void* stream);
+int mm_pretrained_project(const float* P, int64_t rows, int Dp, int64_t p_stride, const void* ids, int idx_dtype, int64_t B,
+                          const float* W, const float* bias, int N, float* out, int64_t out_stride, int32_t* oob_count,
+                          void* stream);
+int64_t mm_pretrained_backward_workspace_bytes(int64_t B, int Dp, int N);
+int mm_pretrained_project_backward(const float* P, int64_t rows, int Dp, int64_t p_stride, const void* ids, int idx_dtype,
+                                   int64_t B, const float* const* addends, const int64_t* addend_strides, int n_addends,
+                                   const float* ypre, int64_t y_stride, int N, float* dW, float* db, void* workspace,
+                                   int64_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -26,6 +26,7 @@ from .models import (BinaryClassificationTask, BinaryOutput, CatalogModel, DCNMo
 from .topk import (AvgPrecisionAt, BruteForce, MRRAt, NDCGAt, PrecisionAt, RecallAt, TopKEncoder,  # noqa: F401
                    TopKIndexBlock, TopKPrediction, encode_candidates, unique_rows_by_features)
 from .loader import Loader, sample_batch  # noqa: F401
+from .pretrained import EmbeddingOperator, PretrainedEmbeddings, TensorInitializer  # noqa: F401
 from .graph import CompiledForward, HostBatch, PipelinedForward  # noqa: F401
 from .sharded import ShardedEmbeddings, shard_model  # noqa: F401
 from .train import SGD, Adagrad, Adam, DLRMTrainer, LazyAdam  # noqa: F401

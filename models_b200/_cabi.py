@@ -100,6 +100,8 @@ LOSS_KINDS = {"binary_crossentropy": 0, "mse": 1}  # MM_LOSS_BCE / MM_LOSS_MSE
 PAIRWISE_KINDS = {"bpr": 0, "bpr-max": 1, "top1": 2, "top1_v2": 3, "top1-max": 4, "logistic": 5, "hinge": 6}
 HYPER_LR, HYPER_BETA1, HYPER_BETA2, HYPER_EPS, HYPER_STEP, HYPER_LR_T, HYPER_COUNT = 0, 1, 2, 3, 4, 5, 8
 CONCAT_L2_CTAS = 512  # MM_CONCAT_L2_CTAS: mm_concat_backward_l2's partials per slice
+# K24 limits and launch shape (MM_PRETRAINED_*)
+PRETRAINED_MAX_DIM, PRETRAINED_MAX_OUT, PRETRAINED_CTAS_PER_SM = 1024, 256, 8
 
 
 class ConcatPiece(C.Structure):
@@ -258,6 +260,11 @@ SIGNATURES = {
     "mm_ncf_head_fwd_bwd": (_i, [_vp, _i64, _vp, _i, _vp, _i64, _vp, _i, _i, _vp, _i64, _i, _i, _i64, _i, _vp, _vp, C.POINTER(C.c_int),
                                  C.POINTER(C.c_float), C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_void_p), _f, _vp,
                                  _i64, _i, _vp, _vp, _vp, _vp, _vp, _vp, _i64, _vp, _vp, _vp, _vp]),
+    "mm_pretrained_gather": (_i, [_vp, _i64, _i, _i64, _vp, _i, _i64, _vp, _i64, _vp, _vp]),
+    "mm_pretrained_project": (_i, [_vp, _i64, _i, _i64, _vp, _i, _i64, _vp, _vp, _i, _vp, _i64, _vp, _vp]),
+    "mm_pretrained_backward_workspace_bytes": (_i64, [_i64, _i, _i]),
+    "mm_pretrained_project_backward": (_i, [_vp, _i64, _i, _i64, _vp, _i, _i64, C.POINTER(C.c_void_p), C.POINTER(C.c_int64), _i,
+                                            _vp, _i64, _i, _vp, _vp, _vp, _i64, _vp]),
 }
 
 

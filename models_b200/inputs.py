@@ -238,7 +238,7 @@ class EmbeddingsBlock(Block):
 
     def finish_check(self, oob: Optional[torch.Tensor]) -> None:
         if oob is not None and not self.defer_check:
-            _raise_on_oob(oob, ",".join(self.tables))
+            _raise_on_oob(oob, ",".join(self.tables) or self.name)
 
     @property
     def feature_names(self) -> List[str]:
@@ -376,8 +376,8 @@ class InputBlockV2(Block):
     The embeddings are gathered directly at their concat offsets (no intermediate tensors)."""
 
     def __init__(self, schema: Schema, categorical: Union[Tags, EmbeddingsBlock] = Tags.CATEGORICAL,
-                 continuous: Union[Tags, ContinuousFeatures] = Tags.CONTINUOUS, aggregation: Optional[str] = "concat",
-                 name: Optional[str] = None, **embedding_kwargs):
+                 continuous: Union[Tags, ContinuousFeatures] = Tags.CONTINUOUS, pretrained_embeddings=Tags.EMBEDDING,
+                 aggregation: Optional[str] = "concat", name: Optional[str] = None, **embedding_kwargs):
         super().__init__(name or unique_name("input_block"))
         if aggregation not in ("concat", None):
             raise ValueError(f"InputBlockV2: unsupported aggregation {aggregation!r} (concat or None)")
@@ -393,23 +393,47 @@ class InputBlockV2(Block):
         else:
             con = schema.select_by_tag(continuous).excluding_by_tag(Tags.TARGET)
             self.continuous = ContinuousFeatures.from_schema(con) if len(con) else None
-        if self.embeddings is None and self.continuous is None:
-            raise ValueError("InputBlockV2: the schema has neither categorical nor continuous features")
+        from .pretrained import PretrainedEmbeddings, PretrainedEmbeddingsBlock
+
+        if isinstance(pretrained_embeddings, PretrainedEmbeddingsBlock):
+            self.pretrained: Optional[PretrainedEmbeddingsBlock] = pretrained_embeddings
+        else:
+            pre = schema.select_by_tag(pretrained_embeddings).excluding_by_tag(Tags.TARGET)
+            self.pretrained = PretrainedEmbeddings(pre) if len(pre) else None
+        if self.embeddings is None and self.continuous is None and self.pretrained is None:
+            raise ValueError("InputBlockV2: the schema has neither categorical, continuous nor pretrained features")
+        # the pretrained lookups count out-of-range ids in the tables' counter; without tables an EmbeddingsBlock without
+        # tables owns it, so the model's checks (fit, CompiledForward) find it as they find the tables'
+        self.pretrained_ids: Optional[EmbeddingsBlock] = (
+            EmbeddingsBlock({}, Schema([]), name="pretrained_ids") if self.pretrained is not None and self.embeddings is None
+            else None)
+
+    def __setstate__(self, state):
+        self.__dict__.update(state)
+        for k in ("pretrained", "pretrained_ids"):  # a model saved before input blocks had pretrained features
+            self.__dict__.setdefault(k, None)
 
     def build(self, device=None):
         if self.embeddings is not None:
             self.embeddings.build(device)
+        if self.pretrained is not None:
+            self.pretrained.build(device)
         self.built = True
         return self
 
     def weights(self):
-        return {} if self.embeddings is None else {f"embeddings/{k}": v for k, v in self.embeddings.weights().items()}
+        out = {} if self.embeddings is None else {f"embeddings/{k}": v for k, v in self.embeddings.weights().items()}
+        if self.pretrained is not None:
+            out.update({f"{self.pretrained.name}/{k}": v for k, v in self.pretrained.weights().items()})
+        return out
 
     def layout(self) -> Tuple[Dict[str, int], Dict[str, int], int]:
         """(column offset, width) of every feature in the sorted-name concat, and the total width."""
         widths: Dict[str, int] = {}
         if self.embeddings is not None:
             widths.update(self.embeddings.output_dims())
+        if self.pretrained is not None:
+            widths.update(self.pretrained.output_dims())
         if self.continuous is not None:
             widths.update({n: 1 for n in self.continuous.features})
         cols, c = {}, 0
@@ -426,10 +450,19 @@ class InputBlockV2(Block):
                 out.update(self.embeddings(inputs))
             if self.continuous is not None:
                 out.update(self.continuous(inputs))
+            if self.pretrained is not None:
+                out.update(self.pretrained(inputs))
             return out
         B = batch_size_of(inputs)
         dev = next(iter(inputs.values())).device
         buf = torch.empty((B, total), dtype=torch.float32, device=dev)
+        if self.pretrained is not None:
+            # the tables' counter, checked after their own gathers below; without tables pretrained_ids', checked here
+            owner = self.embeddings if self.embeddings is not None else self.pretrained_ids
+            oob = owner.counter(dev)
+            self.pretrained.write_into(inputs, buf, cols, oob)
+            if owner is self.pretrained_ids:
+                owner.finish_check(oob)
         if self.embeddings is not None:
             self.embeddings.lookup_all_into(inputs, buf, cols)
         if self.continuous is not None:

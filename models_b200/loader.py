@@ -136,7 +136,7 @@ class Loader:
                  global_size: Optional[int] = None, global_rank: Optional[int] = None, drop_last: bool = False,
                  sparse_names=None, sparse_max=None, sparse_as_dense: bool = False, schema: Optional[Schema] = None,
                  index_dtype: str = "int32", prefetch: int = 2, id_bytes: Optional[Dict[str, int]] = None,
-                 **loader_kwargs):
+                 transforms: Optional[Sequence] = None, **loader_kwargs):
         if batch_size is None or int(batch_size) <= 0:
             raise ValueError("`batch_size` must be a positive integer")
         self.batch_size = int(batch_size)
@@ -161,6 +161,18 @@ class Loader:
         missing = [n for n in feats + self.label_names if n not in have]
         if missing:
             raise ValueError(f"columns {missing} are not in the dataset (has {sorted(have)})")
+        # EmbeddingOperator transforms: their vectors stay on the device and are looked up by the model, so a batch
+        # only has to carry each operator's lookup ids
+        self.transforms = list(transforms or [])
+        for op in self.transforms:
+            from .pretrained import EmbeddingOperator
+
+            if not isinstance(op, EmbeddingOperator):
+                raise NotImplementedError(f"Loader transform {type(op).__name__} is not implemented (EmbeddingOperator only)")
+            if op.lookup_key not in have:
+                raise ValueError(f"EmbeddingOperator {op.embedding_name!r}: lookup key {op.lookup_key!r} is not in the dataset")
+            if op.lookup_key not in feats:
+                feats.append(op.lookup_key)
         self.feature_names = feats
         self.cat_names = [n for n in feats if n in (cat_names or tagged_cat)]
         self._cols = cols
@@ -207,7 +219,10 @@ class Loader:
     def output_schema(self) -> Optional[Schema]:
         if self.schema is None:
             return None
-        return self.schema.select_by_name(self.feature_names + self.label_names)
+        out = self.schema.select_by_name(self.feature_names + self.label_names)
+        for op in self.transforms:
+            out = op.compute_output_schema(out)
+        return out
 
     @property
     def input_schema(self) -> Optional[Schema]:

@@ -304,9 +304,12 @@ def resolve_loss_weights(outputs: Sequence[Block], loss=None, loss_weights=None)
 
 
 def expected_input_columns(schema: Schema) -> List[str]:
-    """models/base.py:1730-1749: non-target columns; list columns as `__values` + `__offsets`."""
+    """models/base.py:1730-1749: non-target columns; list columns as `__values` + `__offsets`.  Pretrained (EMBEDDING)
+    columns are optional: an EmbeddingOperator serves them from the batch's lookup ids when the batch does not carry them."""
     cols = []
     for c in schema.excluding_by_tag(Tags.TARGET):
+        if c.has_tag(Tags.EMBEDDING):
+            continue
         if c.is_list and c.is_ragged:
             cols += [c.name + "__values", c.name + "__offsets"]
         else:

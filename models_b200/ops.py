@@ -849,6 +849,98 @@ def l2_normalize_backward(x: torch.Tensor, dy: torch.Tensor, dx: Optional[torch.
 
 
 # ---------------------------------------------------------------------------------------------
+# pretrained embeddings (K24): rows of a device-resident matrix by id, straight into their slot of x0
+# ---------------------------------------------------------------------------------------------
+def _pretrained_source(P: torch.Tensor, ids: Optional[torch.Tensor], B: int) -> tuple:
+    """(rows, Dp, row stride, ids pointer, ids dtype) of a lookup of P (rows, Dp) at ids (B,); ids None: P is a dense
+    (B, Dp) input read row by row."""
+    _dev(P, "P", torch.float32)
+    stride = _row_stride(P, "P")
+    if not 1 <= P.shape[1] <= _cabi.PRETRAINED_MAX_DIM:
+        raise NotImplementedError(f"pretrained vectors of width {P.shape[1]}: the kernels take 1..{_cabi.PRETRAINED_MAX_DIM}")
+    if ids is None:
+        if P.shape[0] != B:
+            raise ValueError(f"a dense pretrained input must have {B} rows, got {tuple(P.shape)}")
+        return P.shape[0], P.shape[1], stride, None, MM_I32
+    _dev(ids, "ids")
+    if ids.numel() != B or not ids.is_contiguous():
+        raise ValueError(f"ids must be {B} contiguous ids, got {tuple(ids.shape)}")
+    return P.shape[0], P.shape[1], stride, ids.data_ptr(), _idx_dtype(ids, "ids")
+
+
+def pretrained_gather(P: torch.Tensor, ids: Optional[torch.Tensor], out: torch.Tensor,
+                      oob: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out (B, Dp), a column slice of x0 = P[ids] (ids None: row b of the dense (B, Dp) P)  (mm_pretrained_gather)."""
+    _dev(out, "out", torch.float32)
+    B = out.shape[0]
+    rows, Dp, ps, ip, dt = _pretrained_source(P, ids, B)
+    if out.shape[1] != Dp:
+        raise ValueError(f"out must be ({B}, {Dp}), got {tuple(out.shape)}")
+    _cabi.check(_lib().mm_pretrained_gather(P.data_ptr(), rows, Dp, ps, ip, dt, B, out.data_ptr(), _row_stride(out, "out"),
+                                            _ptr(oob), _stream()), "mm_pretrained_gather")
+    return out
+
+
+def pretrained_project(P: torch.Tensor, ids: Optional[torch.Tensor], W: torch.Tensor, bias: Optional[torch.Tensor],
+                       out: torch.Tensor, oob: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out (B, N), a column slice of x0 or a (B, N) buffer = P[ids] W + bias, the gathered rows never written
+    (mm_pretrained_project)."""
+    _dev(out, "out", torch.float32), _dev(W, "W", torch.float32)
+    B = out.shape[0]
+    rows, Dp, ps, ip, dt = _pretrained_source(P, ids, B)
+    if W.dim() != 2 or W.shape[0] != Dp or not W.is_contiguous():
+        raise ValueError(f"W must be a contiguous ({Dp}, N) matrix, got {tuple(W.shape)}")
+    N = W.shape[1]
+    if not 1 <= N <= _cabi.PRETRAINED_MAX_OUT:
+        raise NotImplementedError(f"a projection to {N} columns: the kernels take 1..{_cabi.PRETRAINED_MAX_OUT}")
+    _vec(bias, N, "bias")
+    if out.shape[1] != N:
+        raise ValueError(f"out must be ({B}, {N}), got {tuple(out.shape)}")
+    _cabi.check(_lib().mm_pretrained_project(P.data_ptr(), rows, Dp, ps, ip, dt, B, W.data_ptr(), _ptr(bias), N, out.data_ptr(),
+                                             _row_stride(out, "out"), _ptr(oob), _stream()), "mm_pretrained_project")
+    return out
+
+
+def pretrained_backward_workspace(B: int, Dp: int, N: int, device) -> torch.Tensor:
+    """The workspace of pretrained_project_backward at (B, Dp, N)."""
+    nbytes = int(_lib().mm_pretrained_backward_workspace_bytes(B, Dp, N))
+    return torch.empty(max(1, (nbytes + 15) // 16 * 4), dtype=torch.float32, device=device)
+
+
+def pretrained_project_backward(P: torch.Tensor, ids: Optional[torch.Tensor], addends: Sequence[torch.Tensor],
+                                dW: torch.Tensor, db: Optional[torch.Tensor], ypre: Optional[torch.Tensor] = None,
+                                workspace: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """dW (Dp, N) = P[ids]^T g, db (N,) = sum_b g, with g the sum of the (B, N) addends (the slot's columns of the input
+    gradient), taken through the l2-norm backward at the pre-norm projection ypre (B, N) when given; deterministic
+    (mm_pretrained_project_backward)."""
+    _dev(dW, "dW", torch.float32)
+    if not addends or len(addends) > 4:
+        raise ValueError("between 1 and 4 addends")
+    B = addends[0].shape[0]
+    rows, Dp, ps, ip, dt = _pretrained_source(P, ids, B)
+    N = addends[0].shape[1]
+    if tuple(dW.shape) != (Dp, N) or not dW.is_contiguous():
+        raise ValueError(f"dW must be a contiguous ({Dp}, {N}) matrix")
+    _vec(db, N, "db")
+    for i, a in enumerate(addends):
+        _dev(a, f"addends[{i}]", torch.float32)
+        if tuple(a.shape) != (B, N):
+            raise ValueError(f"addends[{i}] must be ({B}, {N}), got {tuple(a.shape)}")
+    if ypre is not None and (tuple(_dev(ypre, "ypre", torch.float32).shape) != (B, N)):
+        raise ValueError(f"ypre must be ({B}, {N})")
+    if workspace is None:
+        workspace = pretrained_backward_workspace(B, Dp, N, dW.device)
+    ptrs = (C.c_void_p * len(addends))(*[a.data_ptr() for a in addends])
+    strides = (C.c_int64 * len(addends))(*[_row_stride(a, f"addends[{i}]") for i, a in enumerate(addends)])
+    _cabi.check(_lib().mm_pretrained_project_backward(P.data_ptr(), rows, Dp, ps, ip, dt, B, ptrs, strides, len(addends),
+                                                      _ptr(ypre), 0 if ypre is None else _row_stride(ypre, "ypre"), N,
+                                                      dW.data_ptr(), _ptr(db), workspace.data_ptr(),
+                                                      workspace.numel() * 4, _stream()),
+                "mm_pretrained_project_backward")
+    return dW
+
+
+# ---------------------------------------------------------------------------------------------
 # tensor-core dense path (wgmma split-bf16)
 # ---------------------------------------------------------------------------------------------
 def tc_padded_k(K: int) -> int:

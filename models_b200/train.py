@@ -646,10 +646,17 @@ class _ConcatInput:
     features' column offsets, by default the block's sorted-name layout."""
 
     def __init__(self, tr: _StepTrainer, ib, dx0: bool = False, feats: Optional[Sequence[str]] = None,
-                 cont: Optional[Sequence[str]] = None, cols: Optional[Dict[str, int]] = None):
+                 cont: Optional[Sequence[str]] = None, cols: Optional[Dict[str, int]] = None, pretrained_ok: bool = False):
         self.tr = tr
         self.emb = ib.embeddings
         self.cols, _, self.d = ib.layout()
+        # pretrained features (PretrainedEmbeddings): gathered, or gathered and projected, into their slots of x0
+        self.pre = getattr(ib, "pretrained", None)
+        self.pslots = list(self.pre.branches.values()) if self.pre is not None else []
+        if self.pslots and not pretrained_ok:
+            raise NotImplementedError(f"training {tr._model_name} with pretrained embeddings (PretrainedEmbeddings) is not "
+                                      "implemented")
+        self.proj_layers = [br.projection for br in self.pslots if br.projection is not None]
         if cols is not None:  # an explicit column offset per feature instead of the sorted-name concat (NCF's [item | query])
             dims = self.emb.output_dims()
             self.cols, self.d = dict(cols), max(c + dims[f] for f, c in cols.items())
@@ -662,11 +669,17 @@ class _ConcatInput:
         # embeddings_l2_reg per feature (set by a trainer that applies it) and mm_concat_backward_l2's partials
         self.l2_reg: List[float] = [0.0] * len(self.feats)
         self.l2_ws: Optional[torch.Tensor] = None
-        self.oob = self.emb.counter(tr.device) if self.emb is not None else None
+        ids_owner = self.emb if self.emb is not None else getattr(ib, "pretrained_ids", None)
+        self.oob = ids_owner.counter(tr.device) if ids_owner is not None else None
         f32 = dict(dtype=torch.float32, device=tr.device)
         self.x0 = torch.zeros((tr.B, _ld4(self.d)), **f32)
         self.xs = torch.zeros((tr.B, 2 * ops.tc_padded_k(self.d)), dtype=torch.bfloat16, device=tr.device)
-        self.dx0 = torch.zeros((tr.B, _ld4(self.d)), **f32) if dx0 and self.feats else None
+        self.dx0 = torch.zeros((tr.B, _ld4(self.d)), **f32) if dx0 and (self.feats or self.proj_layers) else None
+        # per projected slot: the pre-norm projection (l2-normalised slots) and the backward's workspace
+        self.ypre = [torch.zeros((tr.B, br.width), **f32) if br.projection is not None and br.l2 else None for br in self.pslots]
+        self.pws = [ops.pretrained_backward_workspace(tr.B, br.dim, br.width, tr.device) if br.projection is not None else None
+                    for br in self.pslots]
+        self._psrc: List[tuple] = [None] * len(self.pslots)
 
     def check_multihot_widths(self, schema) -> None:
         """Refuse a list feature whose table the multi-hot gradient expansion (mm_bag_grad_rows) cannot serve."""
@@ -706,6 +719,19 @@ class _ConcatInput:
                 tr._idx[t] = i
         if self.cont:
             ops.concat_columns([inputs[n] for n in self.cont], x0, [self.cols[n] for n in self.cont])
+        for i, br in enumerate(self.pslots):
+            P, ids = self._psrc[i] = self.pre.source(inputs, br.name)
+            slot = x0[:, self.cols[br.name]:self.cols[br.name] + br.width]
+            if br.projection is None:
+                ops.pretrained_gather(P, ids, slot, self.oob)
+            else:
+                y = slot if self.ypre[i] is None else self.ypre[i][:b]
+                ops.pretrained_project(P, ids, br.projection.kernel, br.projection.bias, y, self.oob)
+                if y is not slot:
+                    ops.l2_normalize(y, out=slot)
+                continue
+            if br.l2:
+                ops.l2_normalize(slot, out=slot)
         ops.split_rows(x0, out=xs)
         return x0, xs, dx0
 
@@ -730,6 +756,15 @@ class _ConcatInput:
                                        self.l2_ws)
             else:
                 ops.concat_backward(addends, slices[s:s + CONCAT_MAX_SLICES])
+        a = tr.arena
+        for i, br in enumerate(self.pslots):  # a projection's dW, db from its slot's columns; nothing flows into P
+            if br.projection is None:
+                continue
+            c, li = self.cols[br.name], a.layers.index(br.projection)
+            P, ids = self._psrc[i]
+            ops.pretrained_project_backward(P, ids, [x[:, c:c + br.width] for x in addends], a.view(a.grad, li, "kernel"),
+                                            a.view(a.grad, li, "bias"), ypre=None if self.ypre[i] is None else self.ypre[i][:b],
+                                            workspace=self.pws[i])
 
 
 class _WideKernel:
@@ -991,11 +1026,11 @@ class DCNTrainer(_StepTrainer):
         self.deep = body.deep.dense_layers
         self._init_heads()
         self._check_activations(self.deep)
-        self.inp = _ConcatInput(self, ib)
+        self.inp = _ConcatInput(self, ib, pretrained_ok=True)
         self._init_inputs([self.inp])
         d = self.inp.d
 
-        self._init_dense(self.cross + self.deep, [self.head])
+        self._init_dense(self.cross + self.deep, self.inp.proj_layers + [self.head])
         # every layer needs its input gradient (x0 is the tables' rows); mm_cross_backward writes the split of a cross
         # layer's dz itself
         L = len(self.cross)
@@ -1603,7 +1638,7 @@ class MMoETrainer(_StepTrainer):
         self._check_activations(self.bottom + chain_layers + ([mo.experts] if mo is not None else []))
         if self.head.input_dim > 256:
             raise NotImplementedError("the output layer's input must be <= 256 wide")
-        self.inp = _ConcatInput(self, ib, dx0=True)
+        self.inp = _ConcatInput(self, ib, dx0=True, pretrained_ok=True)
         self.inp.check_multihot_widths(model.schema)
         self._init_inputs([self.inp])
         # arena order: bottom, [experts, stacked gates], gate chains, towers, heads; li0 of each chain
@@ -1622,12 +1657,12 @@ class MMoETrainer(_StepTrainer):
         for c in self.towers:
             self.tower_li0.append(len(tc))
             tc += c
-        self._init_dense(tc, [self.head])
+        self._init_dense(tc, self.inp.proj_layers + [self.head])
         nb = len(self.bottom)
         firsts = set(self.gate_li0) | (set() if mo is not None else set(self.tower_li0))
         # layers whose input gradient _dgrad computes (> 128 units: through the transposed kernel); the layers reading the
         # shared vector take theirs together, and a tower's first layer reading the mixture takes it alone
-        self._init_wide(lambda li: (li < nb and (li > 0 or bool(self.tables))) or (li >= nb + (2 if mo is not None and mo.gates is not None else 1 if mo is not None else 0) and li not in firsts))
+        self._init_wide(lambda li: (li < nb and (li > 0 or self.inp.dx0 is not None)) or (li >= nb + (2 if mo is not None and mo.gates is not None else 1 if mo is not None else 0) and li not in firsts))
 
         B = self.B
         f32 = dict(dtype=torch.float32, device=self.device)
@@ -1755,7 +1790,7 @@ class MMoETrainer(_StepTrainer):
                 ops.relu_mask(dx_in, h[-1])
         if nb:
             self._chain_backward(0, self.bottom, h, dh, (xs, d), dx0)
-        if self.tables:
+        if dx0 is not None:
             self.inp.backward([dx0], b)
             self._bag_grads()
         self._b = b
