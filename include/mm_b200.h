@@ -459,7 +459,8 @@ int mm_init_uniform_hash_rows(float* w, int64_t local_rows, int D, uint64_t seed
  *                             really holds are updated (with Adam, a zero-gradient row would still move).  The max
  *                             combiner (and sqrtn on fixed-length bags) returns MM_ERR_UNSUPPORTED.
  *   mm_dense_apply            the same update rules over a flat fp32 arena; g is scaled by grad_scale and CLEARED.
- *   mm_opt_tick               step counter += 1 and the Adam bias-corrected rate (once per step, before the applies)
+ *   mm_opt_tick               step counter += 1 and the Adam bias-corrected rate (once per step, before the applies);
+ *                             the counter is fp32, exact up to 2^24 steps (K25's mm_opt_tick_schedule also sets lr)
  * Update rules (hyper: device float[MM_HYPER_COUNT], so a captured CUDA graph follows a learning-rate schedule):
  *   MM_OPT_SGD      w -= lr g
  *   MM_OPT_ADAGRAD  a += g^2;  w -= lr g / (sqrt(a) + eps)                       (a starts at 0.1 in Keras)
@@ -998,6 +999,45 @@ int mm_pretrained_project_backward(const float* P, int64_t rows, int Dp, int64_t
                                    int64_t B, const float* const* addends, const int64_t* addend_strides, int n_addends,
                                    const float* ypre, int64_t y_stride, int N, float* dW, float* db, void* workspace,
                                    int64_t workspace_bytes, void* stream);
+
+/* ---------------------------------------------------------------------------------------
+ * K25  Learning-rate schedules evaluated on the device (tf.keras.optimizers.schedules of TF 2.9-2.12), so a captured CUDA
+ * graph follows the schedule without host work.  Added with schedules and per-block optimizers; no existing entry point
+ * changed.
+ *   mm_opt_tick_schedule  s = hyper[MM_HYPER_STEP] (the optimizer's `iterations` before this step's update);
+ *       hyper[MM_HYPER_LR] = lr(s) in fp32; then what mm_opt_tick does: step = s + 1 and
+ *       hyper[MM_HYPER_LR_T] = lr(s) sqrt(1 - b2^(s+1)) / (1 - b1^(s+1)).  One thread.
+ *   sched: device float[MM_SCHED_COUNT]: [MM_SCHED_KIND] one of MM_SCHED_*, then the schedule's parameters
+ *       (init = initial_learning_rate, decay_steps > 0, rate = decay_rate / end_learning_rate / alpha, power,
+ *       flag = staircase / cycle as 0 or 1) and, for MM_SCHED_PIECEWISE, nb (1..MM_SCHED_MAX_BOUNDARIES) increasing
+ *       boundaries and nb + 1 values.  lr(s), p = s / decay_steps (floored when staircase):
+ *         EXPONENTIAL   init * rate^p
+ *         PIECEWISE     values[0] if s <= b[0]; values[i] if b[i-1] < s <= b[i]; values[nb] if s > b[nb-1]
+ *         POLYNOMIAL    (init - rate) * (1 - s'/D)^power + rate; no cycle: s' = min(s, decay_steps), D = decay_steps;
+ *                       cycle: s' = s, D = decay_steps * max(1, ceil(s / decay_steps))
+ *         INVERSE_TIME  init / (1 + rate * p)
+ *         COSINE        init * ((1 - rate) * 0.5 * (1 + cos(pi * min(s, decay_steps) / decay_steps)) + rate)
+ *   The step counter is fp32: it counts exactly up to 2^24 steps (the step after 16 777 216 stays at 16 777 216).
+ *   An unknown kind or an out-of-range nb is refused by the host wrapper; the kernel leaves MM_HYPER_LR as it is then.
+ * Errors before any launch: MM_ERR_ARG (null pointer).
+ * ------------------------------------------------------------------------------------- */
+#define MM_SCHED_EXPONENTIAL 1
+#define MM_SCHED_PIECEWISE 2
+#define MM_SCHED_POLYNOMIAL 3
+#define MM_SCHED_INVERSE_TIME 4
+#define MM_SCHED_COSINE 5
+#define MM_SCHED_KIND 0
+#define MM_SCHED_INIT 1
+#define MM_SCHED_DECAY_STEPS 2
+#define MM_SCHED_RATE 3
+#define MM_SCHED_POWER 4
+#define MM_SCHED_FLAG 5
+#define MM_SCHED_NB 6
+#define MM_SCHED_MAX_BOUNDARIES 32
+#define MM_SCHED_BOUNDARIES 8
+#define MM_SCHED_VALUES (MM_SCHED_BOUNDARIES + MM_SCHED_MAX_BOUNDARIES)
+#define MM_SCHED_COUNT (MM_SCHED_VALUES + MM_SCHED_MAX_BOUNDARIES + 1)
+int mm_opt_tick_schedule(float* hyper, const float* sched, void* stream);
 
 #ifdef __cplusplus
 }

@@ -30,7 +30,8 @@ from .pretrained import EmbeddingOperator, PretrainedEmbeddings, TensorInitializ
 from .graph import CompiledForward, HostBatch, PipelinedForward  # noqa: F401
 from .sharded import ShardedEmbeddings, shard_model  # noqa: F401
 from .train import SGD, Adagrad, Adam, DLRMTrainer, LazyAdam  # noqa: F401
-from . import benchmark, datasets, io, losses, metrics, ops, train  # noqa: F401
+from .optimizer import MultiOptimizer, OptimizerBlocks, split_embeddings_on_size  # noqa: F401
+from . import benchmark, datasets, io, losses, metrics, ops, schedules, train  # noqa: F401
 from .io import load_merlin_metadata, save_merlin_metadata  # noqa: F401
 
 __version__ = "0.1.0"

@@ -99,6 +99,13 @@ LOSS_KINDS = {"binary_crossentropy": 0, "mse": 1}  # MM_LOSS_BCE / MM_LOSS_MSE
 # mm_inbatch_pairwise_fwd / _bwd loss kinds (MM_PAIRWISE_*), by the reference's registry names
 PAIRWISE_KINDS = {"bpr": 0, "bpr-max": 1, "top1": 2, "top1_v2": 3, "top1-max": 4, "logistic": 5, "hinge": 6}
 HYPER_LR, HYPER_BETA1, HYPER_BETA2, HYPER_EPS, HYPER_STEP, HYPER_LR_T, HYPER_COUNT = 0, 1, 2, 3, 4, 5, 8
+# K25 learning-rate schedules (MM_SCHED_*): kinds, the parameter layout of the device array, its size and boundary limit
+SCHED_KINDS = {"ExponentialDecay": 1, "PiecewiseConstantDecay": 2, "PolynomialDecay": 3, "InverseTimeDecay": 4,
+               "CosineDecay": 5}
+SCHED_KIND, SCHED_INIT, SCHED_DECAY_STEPS, SCHED_RATE, SCHED_POWER, SCHED_FLAG, SCHED_NB = 0, 1, 2, 3, 4, 5, 6
+SCHED_MAX_BOUNDARIES, SCHED_BOUNDARIES = 32, 8
+SCHED_VALUES = SCHED_BOUNDARIES + SCHED_MAX_BOUNDARIES
+SCHED_COUNT = SCHED_VALUES + SCHED_MAX_BOUNDARIES + 1
 CONCAT_L2_CTAS = 512  # MM_CONCAT_L2_CTAS: mm_concat_backward_l2's partials per slice
 # K24 limits and launch shape (MM_PRETRAINED_*)
 PRETRAINED_MAX_DIM, PRETRAINED_MAX_OUT, PRETRAINED_CTAS_PER_SM = 1024, 256, 8
@@ -214,6 +221,7 @@ SIGNATURES = {
     "mm_bag_grad_rows": (_i, [_vp, _i64, _i, _i64, _vp, _i, _vp, _i, _i, _i64, _i64, _i, _vp, _vp, _vp]),
     "mm_dense_apply": (_i, [_i, _vp, _vp, _vp, _vp, _i64, _vp, _f, _vp]),
     "mm_opt_tick": (_i, [_vp, _vp]),
+    "mm_opt_tick_schedule": (_i, [_vp, _vp, _vp]),
     "mm_fill_i32": (_i, [_vp, _i64, C.c_int32, _vp]),
     "mm_cross_backward": (_i, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _i, _i64, _i, _vp, _i64, _vp, _i, _vp]),
     "mm_concat_backward": (_i, [C.POINTER(C.c_void_p), C.POINTER(C.c_int64), _i, _i64, _i, C.POINTER(ColumnSlice), _i, _vp]),

@@ -17,6 +17,8 @@
 //   mm_bag_grad_rows            backward of a pooled multi-hot feature: the pooled-row gradient expanded to one scaled
 //       row per id, the IndexedSlices that mm_sparse_rows_apply consumes.
 //   mm_dense_apply              SGD / Adagrad / Adam over a flat parameter arena (+ clears the gradients).
+//   mm_opt_tick[_schedule]      the per-step tick of one optimizer's device hyper-parameters (step counter, Adam's lr_t),
+//       with a learning-rate schedule evaluated at the step counter first (K25).
 #include <cuda_bf16.h>
 
 #include <climits>
@@ -1031,6 +1033,58 @@ __global__ void opt_tick_kernel(float* hyper) {
   hyper[MM_HYPER_LR_T] = hyper[MM_HYPER_LR] * sqrtf(1.0f - powf(b2, t)) / (1.0f - powf(b1, t));
 }
 
+// lr(s) of a K25 schedule, in fp32 and in the order of operations of tf.keras.optimizers.schedules (TF 2.9-2.12).
+__device__ float schedule_lr(const float* sc, float s, float lr) {
+  const int kind = (int)sc[MM_SCHED_KIND];
+  const float init = sc[MM_SCHED_INIT], ds = sc[MM_SCHED_DECAY_STEPS], rate = sc[MM_SCHED_RATE];
+  const bool flag = sc[MM_SCHED_FLAG] != 0.0f;
+  switch (kind) {
+    case MM_SCHED_EXPONENTIAL: {
+      float p = s / ds;
+      if (flag) p = floorf(p);
+      return init * powf(rate, p);
+    }
+    case MM_SCHED_INVERSE_TIME: {
+      float p = s / ds;
+      if (flag) p = floorf(p);
+      return init / (1.0f + rate * p);
+    }
+    case MM_SCHED_POLYNOMIAL: {
+      float d = ds, sp = s;
+      if (flag) {
+        d = ds * (s == 0.0f ? 1.0f : ceilf(s / ds));
+      } else {
+        sp = fminf(s, ds);
+      }
+      return (init - rate) * powf(1.0f - sp / d, sc[MM_SCHED_POWER]) + rate;
+    }
+    case MM_SCHED_COSINE: {
+      const float frac = fminf(s, ds) / ds;
+      const float cd = 0.5f * (1.0f + cosf(3.14159265358979323846f * frac));
+      return init * ((1.0f - rate) * cd + rate);
+    }
+    case MM_SCHED_PIECEWISE: {
+      const int nb = (int)sc[MM_SCHED_NB];
+      if (nb < 1 || nb > MM_SCHED_MAX_BOUNDARIES) return lr;
+      int i = 0;
+      while (i < nb && s > sc[MM_SCHED_BOUNDARIES + i]) ++i;
+      return sc[MM_SCHED_VALUES + i];
+    }
+    default:
+      return lr;
+  }
+}
+
+__global__ void opt_tick_schedule_kernel(float* hyper, const float* sched) {
+  const float s = hyper[MM_HYPER_STEP];
+  const float lr = schedule_lr(sched, s, hyper[MM_HYPER_LR]);
+  hyper[MM_HYPER_LR] = lr;
+  const float t = s + 1.0f;
+  hyper[MM_HYPER_STEP] = t;
+  const float b1 = hyper[MM_HYPER_BETA1], b2 = hyper[MM_HYPER_BETA2];
+  hyper[MM_HYPER_LR_T] = lr * sqrtf(1.0f - powf(b2, t)) / (1.0f - powf(b1, t));
+}
+
 __global__ void fill_i32_kernel(int* p, long long n, int v) {
   long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long stride = (long long)gridDim.x * blockDim.x;
@@ -1202,6 +1256,12 @@ int mm_opt_tick(float* hyper, void* stream) {
   MM_REQUIRE(hyper, MM_ERR_ARG, "mm_opt_tick: null pointer");
   mm::trs::opt_tick_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(hyper);
   return mm::check_launch("mm_opt_tick");
+}
+
+int mm_opt_tick_schedule(float* hyper, const float* sched, void* stream) {
+  MM_REQUIRE(hyper && sched, MM_ERR_ARG, "mm_opt_tick_schedule: null pointer");
+  mm::trs::opt_tick_schedule_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(hyper, sched);
+  return mm::check_launch("mm_opt_tick_schedule");
 }
 
 int mm_bag_grad_rows(const float* g, int64_t B, int D, int64_t g_stride, const void* ids, int idx_dtype, const void* offsets,

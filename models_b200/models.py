@@ -647,16 +647,17 @@ class Model(Block, metaclass=_ModelMeta):
 
         * `compile(optimizer="adam")` / `compile("adagrad")` / `compile(optimizer=mm.Adagrad(0.01))` — Keras `compile`
           (models/base.py: the reference's models are compiled before `fit`): picks the optimizer of the training step
-          (models_b200/train.py).  The loss is the prediction task's default (binary cross-entropy for BinaryOutput).
+          (models_b200/train.py), or a MultiOptimizer of one optimizer per block (models_b200/optimizer.py).  The loss is the prediction task's default (binary cross-entropy for BinaryOutput).
           Ranking models take `metrics` / `weighted_metrics` (models_b200/metrics.py: None = each output's reference
           defaults) for `evaluate` and `fit`; `run_eagerly` is accepted for signature parity.
         * `compile(example_batch, **call_kwargs)` — capture this model's forward for `example`'s batch layout into a CUDA
           graph; the result maps a packed pinned HostBatch to pinned host predictions with one H2D, one graph launch and
           one D2H (models_b200/graph.py)."""
         from .graph import CompiledForward, HostBatch
+        from .optimizer import MultiOptimizer
         from .train import Optimizer
 
-        if optimizer is not None or isinstance(example, (str, Optimizer)) or example is None:
+        if optimizer is not None or isinstance(example, (str, Optimizer, MultiOptimizer)) or example is None:
             if example is not None and optimizer is not None:
                 raise ValueError("compile(): pass either an example batch (graph capture) or an optimizer (training)")
             return self._compile_training(optimizer if optimizer is not None else (example or "adam"), loss,

@@ -10,6 +10,7 @@ import ctypes as C
 import math
 from typing import Optional, Sequence
 
+import numpy as np
 import torch
 
 from . import _cabi
@@ -1794,6 +1795,48 @@ def dense_apply(opt: str, w: torch.Tensor, grad: torch.Tensor, state1: Optional[
 
 def opt_tick(hyper: torch.Tensor) -> None:
     _cabi.check(_lib().mm_opt_tick(_dev(hyper, "hyper", torch.float32).data_ptr(), _stream()), "mm_opt_tick")
+
+
+def schedule_params(kind: str, initial_learning_rate: float = 0.0, decay_steps: float = 1.0, rate: float = 0.0,
+                    power: float = 1.0, flag: bool = False, boundaries: Sequence[float] = (),
+                    values: Sequence[float] = ()) -> np.ndarray:
+    """The K25 device array float[SCHED_COUNT] of a learning-rate schedule `kind` (a key of _cabi.SCHED_KINDS); rate is
+    decay_rate, end_learning_rate or alpha, flag staircase or cycle.  PiecewiseConstantDecay takes 1..SCHED_MAX_BOUNDARIES
+    increasing boundaries and one value more."""
+    if kind not in _cabi.SCHED_KINDS:
+        raise ValueError(f"unknown learning-rate schedule {kind!r}; supported: {sorted(_cabi.SCHED_KINDS)}")
+    s = np.zeros(_cabi.SCHED_COUNT, dtype=np.float32)
+    s[_cabi.SCHED_KIND] = _cabi.SCHED_KINDS[kind]
+    if kind == "PiecewiseConstantDecay":
+        nb = len(boundaries)
+        if not 1 <= nb <= _cabi.SCHED_MAX_BOUNDARIES:
+            raise NotImplementedError(f"PiecewiseConstantDecay with {nb} boundaries: the device schedule takes "
+                                      f"1..{_cabi.SCHED_MAX_BOUNDARIES}")
+        if len(values) != nb + 1:
+            raise ValueError(f"{nb} boundaries need {nb + 1} values, got {len(values)}")
+        b = np.asarray(boundaries, dtype=np.float32)
+        if np.any(np.diff(b) <= 0):
+            raise ValueError(f"boundaries must be increasing, got {list(boundaries)}")
+        s[_cabi.SCHED_NB] = nb
+        s[_cabi.SCHED_BOUNDARIES:_cabi.SCHED_BOUNDARIES + nb] = b
+        s[_cabi.SCHED_VALUES:_cabi.SCHED_VALUES + nb + 1] = np.asarray(values, dtype=np.float32)
+        return s
+    if not decay_steps > 0:
+        raise ValueError(f"decay_steps must be > 0, got {decay_steps}")
+    s[_cabi.SCHED_INIT], s[_cabi.SCHED_DECAY_STEPS], s[_cabi.SCHED_RATE] = initial_learning_rate, decay_steps, rate
+    s[_cabi.SCHED_POWER], s[_cabi.SCHED_FLAG] = power, 1.0 if flag else 0.0
+    return s
+
+
+def opt_tick_schedule(hyper: torch.Tensor, sched: torch.Tensor) -> None:
+    """mm_opt_tick with hyper[HYPER_LR] = lr(step) of the schedule `sched` (schedule_params' array on the device) first."""
+    _dev(hyper, "hyper", torch.float32), _dev(sched, "sched", torch.float32)
+    if hyper.numel() < _cabi.HYPER_COUNT or not hyper.is_contiguous():
+        raise ValueError(f"hyper must hold {_cabi.HYPER_COUNT} contiguous values, got {tuple(hyper.shape)}")
+    _vec(sched, _cabi.SCHED_COUNT, "sched")
+    if sched.device != hyper.device:
+        raise ValueError(f"sched is on {sched.device}, hyper on {hyper.device}")
+    _cabi.check(_lib().mm_opt_tick_schedule(hyper.data_ptr(), sched.data_ptr(), _stream()), "mm_opt_tick_schedule")
 
 
 def fill_i32(t: torch.Tensor, value: int) -> torch.Tensor:

@@ -51,7 +51,7 @@ from typing import Dict, List, Optional, Sequence
 import numpy as np
 import torch
 
-from . import _cabi, ops
+from . import _cabi, ops, schedules
 from .blocks import DLRM, MLP, _Dense
 from .core import batch_size_of, default_device, get_feature
 from .graph import graph_capture
@@ -71,21 +71,33 @@ class History:
 
 
 class Optimizer:
-    """Hyper-parameters of one of the update rules in include/mm_b200.h (Keras argument names and defaults)."""
+    """Hyper-parameters of one of the update rules in include/mm_b200.h (Keras argument names and defaults).
+    learning_rate: a float, or one of the built-in schedules of models_b200.schedules (evaluated on the device each step
+    from the optimizer's step counter, K25)."""
 
     kind = "sgd"
 
-    def __init__(self, learning_rate: float, beta_1: float = 0.0, beta_2: float = 0.0, epsilon: float = 1e-7,
+    def __init__(self, learning_rate, beta_1: float = 0.0, beta_2: float = 0.0, epsilon: float = 1e-7,
                  initial_accumulator_value: float = 0.0):
-        if learning_rate < 0:
-            raise ValueError("learning_rate must be >= 0")
-        self.learning_rate = float(learning_rate)
+        if callable(learning_rate) or isinstance(learning_rate, schedules.LearningRateSchedule):
+            schedules.check_trainable(learning_rate)
+            self.learning_rate = learning_rate
+        else:
+            if learning_rate < 0:
+                raise ValueError("learning_rate must be >= 0")
+            self.learning_rate = float(learning_rate)
         self.beta_1, self.beta_2, self.epsilon = float(beta_1), float(beta_2), float(epsilon)
         self.initial_accumulator_value = float(initial_accumulator_value)
 
+    @property
+    def schedule(self) -> Optional[schedules.LearningRateSchedule]:
+        return self.learning_rate if isinstance(self.learning_rate, schedules.LearningRateSchedule) else None
+
     def hyper(self) -> np.ndarray:
+        """The device hyper-parameters before the first step; a schedule's lr(0) as the learning rate."""
         h = np.zeros(_cabi.HYPER_COUNT, dtype=np.float32)
-        h[_cabi.HYPER_LR], h[_cabi.HYPER_BETA1], h[_cabi.HYPER_BETA2] = self.learning_rate, self.beta_1, self.beta_2
+        lr = self.learning_rate if self.schedule is None else self.schedule(0)
+        h[_cabi.HYPER_LR], h[_cabi.HYPER_BETA1], h[_cabi.HYPER_BETA2] = lr, self.beta_1, self.beta_2
         h[_cabi.HYPER_EPS] = self.epsilon
         return h
 
@@ -94,7 +106,8 @@ class Optimizer:
         return {"sgd": 0, "adagrad": 1, "adam": 2}[self.kind]
 
     def get_config(self) -> dict:
-        return {"name": type(self).__name__, "learning_rate": self.learning_rate, "beta_1": self.beta_1, "beta_2": self.beta_2,
+        lr = self.learning_rate if self.schedule is None else schedules.serialize(self.schedule)
+        return {"name": type(self).__name__, "learning_rate": lr, "beta_1": self.beta_1, "beta_2": self.beta_2,
                 "epsilon": self.epsilon, "initial_accumulator_value": self.initial_accumulator_value}
 
 
@@ -103,7 +116,7 @@ class SGD(Optimizer):
 
     kind = "sgd"
 
-    def __init__(self, learning_rate: float = 0.01, momentum: float = 0.0, **kwargs):
+    def __init__(self, learning_rate=0.01, momentum: float = 0.0, **kwargs):
         if momentum:
             raise NotImplementedError("SGD momentum is not implemented")
         super().__init__(learning_rate)
@@ -114,7 +127,7 @@ class Adagrad(Optimizer):
 
     kind = "adagrad"
 
-    def __init__(self, learning_rate: float = 0.001, initial_accumulator_value: float = 0.1, epsilon: float = 1e-7, **kwargs):
+    def __init__(self, learning_rate=0.001, initial_accumulator_value: float = 0.1, epsilon: float = 1e-7, **kwargs):
         if initial_accumulator_value < 0:
             raise ValueError("initial_accumulator_value must be non-negative")
         super().__init__(learning_rate, epsilon=epsilon, initial_accumulator_value=initial_accumulator_value)
@@ -126,7 +139,7 @@ class Adam(Optimizer):
 
     kind = "adam"
 
-    def __init__(self, learning_rate: float = 0.001, beta_1: float = 0.9, beta_2: float = 0.999, epsilon: float = 1e-7, **kwargs):
+    def __init__(self, learning_rate=0.001, beta_1: float = 0.9, beta_2: float = 0.999, epsilon: float = 1e-7, **kwargs):
         super().__init__(learning_rate, beta_1, beta_2, epsilon)
 
 
@@ -135,8 +148,11 @@ LazyAdam = Adam
 _BY_NAME = {"sgd": SGD, "adagrad": Adagrad, "adam": Adam, "lazyadam": Adam, "lazy_adam": Adam}
 
 
-def get_optimizer(spec) -> Optimizer:
-    if isinstance(spec, Optimizer):
+def get_optimizer(spec):
+    """An Optimizer (or a MultiOptimizer) from a name or an instance."""
+    from .optimizer import MultiOptimizer
+
+    if isinstance(spec, (Optimizer, MultiOptimizer)):
         return spec
     if isinstance(spec, str):
         if spec.lower() not in _BY_NAME:
@@ -156,10 +172,13 @@ def _ld4(d: int) -> int:
 
 class DenseArena:
     """All Dense variables of a chain of layers in one flat fp32 buffer (kernel then bias per layer, 256-byte aligned);
-    `grad`, `state1`, `state2` share the layout.  The layers' `kernel` / `bias` become views of it."""
+    `grad`, `state1`, `state2` share the layout.  The layers' `kernel` / `bias` become views of it.  optimizer: one
+    optimizer for every layer, or one per layer (anything with `slots` and `initial_accumulator_value`); `runs` holds
+    (start, end, optimizer) per contiguous run of layers with the same optimizer, in arena order."""
 
-    def __init__(self, layers: Sequence[_Dense], optimizer: Optimizer, device):
+    def __init__(self, layers: Sequence[_Dense], optimizer, device):
         self.layers = list(layers)
+        opts = list(optimizer) if isinstance(optimizer, (list, tuple)) else [optimizer] * len(self.layers)
         off = 0
         self.kernel_off, self.bias_off = [], []
         for l in self.layers:
@@ -171,10 +190,21 @@ class DenseArena:
             if l.bias is not None:
                 off = _align(off + l.bias.numel())
         self.size = off
+        self.runs: List[tuple] = []
+        for i, o in enumerate(opts):
+            if self.runs and self.runs[-1][2] is o:
+                continue
+            if self.runs:
+                self.runs[-1] = (self.runs[-1][0], self.kernel_off[i], self.runs[-1][2])
+            self.runs.append((self.kernel_off[i], off, o))
         self.w = torch.zeros(off, dtype=torch.float32, device=device)
         self.grad = torch.zeros_like(self.w)
-        self.state1 = torch.full_like(self.w, optimizer.initial_accumulator_value) if optimizer.slots >= 1 else None
-        self.state2 = torch.zeros_like(self.w) if optimizer.slots >= 2 else None
+        slots = max((o.slots for o in (opts or ([] if isinstance(optimizer, (list, tuple)) else [optimizer]))), default=0)
+        self.state1 = torch.zeros_like(self.w) if slots >= 1 else None
+        self.state2 = torch.zeros_like(self.w) if slots >= 2 else None
+        for s, e, o in self.runs:
+            if o.slots >= 1:
+                self.state1[s:e] = o.initial_accumulator_value
         for i, l in enumerate(self.layers):
             k = self.view(self.w, i, "kernel")
             k.copy_(l.kernel)
@@ -193,6 +223,68 @@ class DenseArena:
         if self.bias_off[i] is None:
             return None
         return buf[self.bias_off[i]: self.bias_off[i] + l.units]
+
+
+class _OptGroup:
+    """One optimizer of a training step: its update rule, its device hyper-parameters (own step counter, lr, Adam's
+    lr_t) and, with a learning-rate schedule, the K25 schedule array its tick evaluates."""
+
+    def __init__(self, opt: Optimizer, device):
+        self.opt, self.kind, self.slots = opt, opt.kind, opt.slots
+        self.initial_accumulator_value = opt.initial_accumulator_value
+        self.hyper = torch.from_numpy(opt.hyper()).to(device)
+        sch = opt.schedule
+        self.sched = None if sch is None else torch.from_numpy(sch.device_params()).to(device)
+
+    def tick(self) -> None:
+        if self.sched is None:
+            ops.opt_tick(self.hyper)
+        else:
+            ops.opt_tick_schedule(self.hyper, self.sched)
+
+
+class _OptGroups:
+    """The optimizer groups of a trainer, created in order of first use: one for a plain optimizer; for a MultiOptimizer
+    one per optimizer that some variable of the model resolves to."""
+
+    def __init__(self, optimizer, model, device):
+        from .optimizer import MultiOptimizer
+
+        self.device = device
+        self.multi = optimizer if isinstance(optimizer, MultiOptimizer) else None
+        self.single = None if self.multi is not None else optimizer
+        self._assign = self.multi.assignments(model) if self.multi is not None else {}
+        self.groups: List[_OptGroup] = []
+        self._by_opt: Dict[int, _OptGroup] = {}
+
+    def of(self, var) -> _OptGroup:
+        """The group of a variable (a _Dense, an EmbeddingTable or a CategoricalOutput's bias)."""
+        opt = self.single if self.multi is None else self._assign.get(id(var), self.multi.default_optimizer)
+        if isinstance(opt, str):
+            from .optimizer import variable_name
+
+            raise NotImplementedError(f"{variable_name(var)}: no OptimizerBlocks entry covers it and the MultiOptimizer's "
+                                      f"default_optimizer {opt!r} (RMSprop) is not implemented: cover every variable or pass "
+                                      "another default_optimizer")
+        g = self._by_opt.get(id(opt))
+        if g is None:
+            g = self._by_opt[id(opt)] = _OptGroup(opt, self.device)
+            self.groups.append(g)
+        return g
+
+
+def _by_group(items: Sequence, group_of) -> List[tuple]:
+    """[(group, [items...])] in order of first appearance: one entry when every item shares a group."""
+    out: List[tuple] = []
+    for it in items:
+        g = group_of(it)
+        for og, lst in out:
+            if og is g:
+                lst.append(it)
+                break
+        else:
+            out.append((g, [it]))
+    return out
 
 
 def gather_slices(ids: torch.Tensor, slices: torch.Tensor, group) -> tuple:
@@ -258,6 +350,9 @@ class _StepTrainer:
     def _init_common(self, model, optimizer: Optimizer, batch_size: int, device, group) -> None:
         self.model, self.body, self.opt = model, model.body, optimizer
         self.device = torch.device(device) if device is not None else default_device()
+        if not model.built:
+            model.build(self.device)
+        self._groups = _OptGroups(optimizer, model, self.device)
         self.B = int(batch_size)
         self.group = group
         self.world = 1
@@ -265,8 +360,11 @@ class _StepTrainer:
             import torch.distributed as dist
 
             self.world = dist.get_world_size(group)
-        if not model.built:
-            model.build(self.device)
+
+    @property
+    def hyper(self) -> torch.Tensor:
+        """The first optimizer group's device hyper-parameters (every group's step counter moves together)."""
+        return self._groups.groups[0].hyper
 
     def _init_heads(self) -> None:
         self.head = self.model.prediction.to_call
@@ -291,12 +389,12 @@ class _StepTrainer:
     def _init_dense(self, tc_layers: Sequence[_Dense], fused_layers: Sequence[_Dense]) -> None:
         """One arena over tc_layers (run by mm_dense_tc: each gets a split operand copy that follows the updates) and
         fused_layers (read as fp32 by a fused kernel), and the optimizer's hyper-parameters in device memory."""
-        self.arena = DenseArena(list(tc_layers) + list(fused_layers), self.opt, self.device)
+        layers = list(tc_layers) + list(fused_layers)
+        self.arena = DenseArena(layers, [self._groups.of(l) for l in layers], self.device)
         self._tc_layers = list(tc_layers)
         self._wsplit = [ops.split_weights(l.kernel) for l in self._tc_layers]
         for l, ws in zip(self._tc_layers, self._wsplit):
             l._w_split = ws  # the model's forward keeps reading the refreshed operand copies
-        self.hyper = torch.from_numpy(self.opt.hyper()).to(self.device)
 
     def _init_tables(self, feats: Sequence[str], tables: Sequence, check_width: bool = True) -> None:
         """feats / tables (one table per feature, by position) after the checks every sparse update needs, their
@@ -313,10 +411,11 @@ class _StepTrainer:
                 raise NotImplementedError(f"table {t.table_name!r}: embedding width {D} is not supported by the sparse update "
                                           "(it needs a multiple of 4 no larger than 128)")
         self.feats, self.tables = list(feats), list(tables)
-        opt = self.opt
+        self.tgroup = [self._groups.of(t) for t in self.tables]
         self.rep = [ops.fill_i32(torch.empty(t.table.shape[0], dtype=torch.int32, device=self.device), INT32_MAX) for t in self.tables]
-        self.tstate1 = [torch.full_like(t.table, opt.initial_accumulator_value) if opt.slots >= 1 else None for t in self.tables]
-        self.tstate2 = [torch.zeros_like(t.table) if opt.slots >= 2 else None for t in self.tables]
+        self.tstate1 = [torch.full_like(t.table, g.initial_accumulator_value) if g.slots >= 1 else None
+                        for t, g in zip(self.tables, self.tgroup)]
+        self.tstate2 = [torch.zeros_like(t.table) if g.slots >= 2 else None for t, g in zip(self.tables, self.tgroup)]
         # tables with few rows (every id repeats many times per batch) sum their slices into a dense accumulator
         self.tdense = [torch.zeros_like(t.table) if t.table.shape[0] <= DENSE_PATH_MAX_ROWS else None for t in self.tables]
         self._by_width: Dict[int, List[int]] = {}
@@ -497,21 +596,26 @@ class _StepTrainer:
         return self._idx, self._slices, self._b, 1.0
 
     def apply_gradients(self) -> None:
+        """Each optimizer group's tick, then mm_dense_apply per run of the arena that one group owns (the whole arena for
+        one optimizer), mm_sparse_rows_apply per (embedding width, group), the wide kernel or tied table."""
         a = self.arena
-        ops.opt_tick(self.hyper)
+        for g in self._groups.groups:
+            g.tick()
         idx, slices, rows, scale = self._gradients_to_apply()
-        if a.size:  # a model without Dense layers (matrix factorization) has an empty arena
-            ops.dense_apply(self.opt.kind, a.w, a.grad, a.state1, a.state2, self.hyper, grad_scale=scale)
+        for s, e, g in a.runs:  # a model without Dense layers (matrix factorization) has an empty arena
+            ops.dense_apply(g.kind, a.w[s:e], a.grad[s:e], a.state1[s:e] if g.slots >= 1 else None,
+                            a.state2[s:e] if g.slots >= 2 else None, g.hyper, grad_scale=scale)
         for D, ts in self._by_width.items():
-            onehot = [t for t in ts if t not in self._bags]
-            for s in range(0, len(onehot), SPARSE_MAX_TABLES):
-                chunk = onehot[s:s + SPARSE_MAX_TABLES]
-                ops.sparse_rows_apply(self.opt.kind, [self._table_args(t, idx[t], slices[t]) for t in chunk], rows, D, self.hyper)
+            for g, onehot in _by_group([t for t in ts if t not in self._bags], lambda t: self.tgroup[t]):
+                for s in range(0, len(onehot), SPARSE_MAX_TABLES):
+                    chunk = onehot[s:s + SPARSE_MAX_TABLES]
+                    ops.sparse_rows_apply(g.kind, [self._table_args(t, idx[t], slices[t]) for t in chunk], rows, D, g.hyper)
             for t in ts:
                 bag = self._bags.get(t)
                 if bag is not None and bag["rows"].shape[0] > 0:  # a multi-hot table: its own call over the nnz expanded rows
+                    g = self.tgroup[t]
                     tab = self._table_args(t, bag["apply_ids"], bag["rows"])
-                    ops.sparse_rows_apply(self.opt.kind, [tab], bag["rows"].shape[0], D, self.hyper)
+                    ops.sparse_rows_apply(g.kind, [tab], bag["rows"].shape[0], D, g.hyper)
         if self.wk is not None:
             self.wk.apply()
         self._refresh_operands()
@@ -577,6 +681,7 @@ class _StepTrainer:
         table and its optimizer slots, and the wide kernel's; None where an optimizer has no such slot."""
         a = self.arena
         state = dict(w=a.w, s1=a.state1, s2=a.state2, hyper=self.hyper)
+        state.update({f"hyper{i}": g.hyper for i, g in enumerate(self._groups.groups) if i})
         for t, (tb, s1, s2) in enumerate(zip(self.tables, self.tstate1, self.tstate2)):
             state.update({f"table{t}": tb.table, f"table{t}/s1": s1, f"table{t}/s2": s2})
         if self.wk is not None:
@@ -624,6 +729,9 @@ class _StepTrainer:
                              "(TF raises InvalidArgumentError: indices[...] is not in [0, rows))")
 
     def set_learning_rate(self, lr: float) -> None:
+        if len(self._groups.groups) > 1 or self._groups.groups[0].sched is not None:
+            raise NotImplementedError("set_learning_rate: the learning rates of a MultiOptimizer or a schedule are set by "
+                                      "their optimizers (schedules move on the device)")
         self.opt.learning_rate = float(lr)
         self.hyper[_cabi.HYPER_LR] = float(lr)
 
@@ -777,7 +885,7 @@ class _WideKernel:
     def __init__(self, tr: _StepTrainer, dense: _Dense, cont_offsets: Sequence[int] = ()):
         self.tr, self.dense = tr, dense
         self.cont_offsets = list(cont_offsets)
-        opt = tr.opt
+        self.group = opt = tr._groups.of(dense)
         f32 = dict(dtype=torch.float32, device=tr.device)
         W = dense.kernel.numel()
         nb = 1 if dense.bias is not None else 0
@@ -799,10 +907,10 @@ class _WideKernel:
         wk, bias = self.dense.kernel.reshape(-1), self.dense.bias
         for i, (ids, rows, offs, g) in enumerate(self.calls):
             first = i == 0
-            ops.wide_rows_apply(self.tr.opt.kind, wk, self.wk_s1, self.wk_s2, ids, rows, offs, g, self.acc, self.rep,
+            ops.wide_rows_apply(self.group.kind, wk, self.wk_s1, self.wk_s2, ids, rows, offs, g, self.acc, self.rep,
                                 self.cont_offsets if first else [], self.grad if first and self.grad.numel() else None,
                                 bias.reshape(-1) if first and bias is not None else None, self.wb_s1 if first else None,
-                                self.wb_s2 if first else None, self.tr.hyper)
+                                self.wb_s2 if first else None, self.group.hyper)
 
     def gradients(self) -> Dict[str, torch.Tensor]:
         """The kernel's gradient (W, 1) and the bias' (after forward_backward, before apply_gradients), assembled in float64
@@ -1893,9 +2001,12 @@ class _TiedTable:
     b / T), refreshed after each update."""
 
     def __init__(self, tr: "_StepTrainer", out, t: Optional[int]):
-        opt, dev = tr.opt, tr.device
+        dev = tr.device
         self.tr, self.out, self.t = tr, out, t
         self.E, self.bias = out.table.table, out.bias
+        # E trains with its table's optimizer group, the bias with the CategoricalOutput's
+        self.gE = opt = tr._groups.of(out.table)
+        self.gb = tr._groups.of(out) if self.bias is not None else None
         N, D = self.E.shape
         self.T = float(out.logits_temperature)
         nb = N if self.bias is not None else 0
@@ -1907,8 +2018,9 @@ class _TiedTable:
             self.s2 = torch.zeros_like(self.E) if opt.slots >= 2 else None
         else:
             self.s1, self.s2 = tr.tstate1[t], tr.tstate2[t]
-        self.b_s1 = torch.full((nb,), opt.initial_accumulator_value, dtype=torch.float32, device=dev) if nb and opt.slots >= 1 else None
-        self.b_s2 = torch.zeros(nb, dtype=torch.float32, device=dev) if nb and opt.slots >= 2 else None
+        gb = self.gb
+        self.b_s1 = torch.full((nb,), gb.initial_accumulator_value, dtype=torch.float32, device=dev) if nb and gb.slots >= 1 else None
+        self.b_s2 = torch.zeros(nb, dtype=torch.float32, device=dev) if nb and gb.slots >= 2 else None
         self.e_split = ops.split_rows(self.E)
         self.bt = None
         if self.bias is not None:
@@ -1925,11 +2037,10 @@ class _TiedTable:
         return st
 
     def apply(self) -> None:
-        kind, hyper = self.tr.opt.kind, self.tr.hyper
-        ops.dense_apply(kind, self.E.view(-1), self.dE.view(-1), None if self.s1 is None else self.s1.view(-1),
-                        None if self.s2 is None else self.s2.view(-1), hyper)
+        ops.dense_apply(self.gE.kind, self.E.view(-1), self.dE.view(-1), None if self.s1 is None else self.s1.view(-1),
+                        None if self.s2 is None else self.s2.view(-1), self.gE.hyper)
         if self.bias is not None:
-            ops.dense_apply(kind, self.bias, self.db, self.b_s1, self.b_s2, hyper)
+            ops.dense_apply(self.gb.kind, self.bias, self.db, self.b_s1, self.b_s2, self.gb.hyper)
 
     def refresh(self) -> None:
         """The catalog kernels' operands (E's split rows, b / T) and E's lookup mirror, if it has one, from the variables."""
