@@ -37,39 +37,6 @@ def close(got, ref, tol=TOL, what=""):
 # ---------------------------------------------------------------------------------------------------------------
 # kernels
 # ---------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("M", [1, 37, 1000, 4099])
-@pytest.mark.parametrize("K,N", [(13, 128), (128, 64), (415, 128), (64, 32), (31, 24), (24, 8), (200, 100), (16, 16)])
-def test_dense_wgrad_and_dgrad(device, M, K, N):
-    g = torch.Generator(device="cpu").manual_seed(M * 1000 + K + N)
-    ldx = (K + 3) // 4 * 4 if K % 2 else K  # a padded row stride as the trainer uses for the interaction output
-    xb = torch.zeros((M, ldx), dtype=torch.float32)
-    xb[:, :K] = torch.randn((M, K), generator=g).clamp_min(0.0)  # relu output: doubles as the mask
-    x = xb.to(device)[:, :K]
-    dz = torch.randn((M, N), generator=g).to(device)
-    W = (torch.randn((K, N), generator=g) * 0.1).to(device)
-    dw = torch.zeros((K, N), dtype=torch.float32, device=device)
-    db = torch.zeros(N, dtype=torch.float32, device=device)
-    ops.dense_wgrad(x, dz, dw, db)
-    close(dw, x.double().t() @ dz.double(), what="dW")
-    close(db, dz.double().sum(0), what="db")
-    ops.dense_wgrad(x, dz, dw, db)  # accumulates
-    close(dw, 2 * (x.double().t() @ dz.double()), what="dW accumulated")
-    dw.zero_()
-    db.zero_()
-    ops.dense_wgrad_split(ops.split_rows(x), K, dz, dw, db)  # X as the split-bf16 operand of the forward layer
-    close(dw, x.double().t() @ dz.double(), what="dW from the split operand")
-    close(db, dz.double().sum(0), what="db (split operand)")
-    if N <= 128:
-        dxb = torch.full((M, ldx), 7.0, dtype=torch.float32, device=device)
-        dx = dxb[:, :K]
-        ops.dense_dgrad(dz, W, dx)
-        close(dx, dz.double() @ W.double().t(), what="dX")
-        ops.dense_dgrad(dz, W, dx, mask=x)
-        close(dx, (dz.double() @ W.double().t()) * (x > 0), what="dX masked")
-        if ldx > K:
-            assert float(dxb[:, K:].min()) == 7.0 and float(dxb[:, K:].max()) == 7.0  # padding columns untouched
-
-
 def test_dense_dgrad_rejects_wide_layers(device):
     with pytest.raises(ValueError, match="N=256"):
         ops.dense_dgrad(torch.zeros((4, 256), device=device), torch.zeros((8, 256), device=device), torch.zeros((4, 8), device=device))
